@@ -1,18 +1,19 @@
 #!/usr/bin/env python
 """Benchmark of the hot path: bf16 forward of ViT-B/16 224^2 (BASELINE.json configs[1]), images/sec.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 512]            # this repo's fused sm_100a path
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 512]            # this repo's fused sm_90a path
     python bench.py --impl reference [...]                                       # UNMODIFIED reference on host cores
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...             # one rank per GPU (weak scaling)
     python bench.py --model vit_l16|vit_h14|navit [--dim-head 80]                # the other BASELINE.json configs
 
 One "step" = one forward of a synthetic batch per GPU (+ the all-gather of the logits when N > 1).  Prints ONE JSON
-line on rank 0 (see DESIGN.md "Measurement" for every field).
+line on rank 0.  --dump-outputs DIR additionally writes the logits of
+the last timed step as DIR/logits.npy (float32); weights and inputs are seeded, so two builds can be compared.
 
 Baselines carried by the GPU arm's line (rank 0, N = 1):
   * `cpu_baseline`        the unmodified reference (baseline/_ref, kind "reference") on the host cores, bounded sample;
   * `gpu_eager_baseline`  the unmodified reference's eager bf16 forward on the SAME GPU, same weights, same batch,
-                          same CUDA-event protocol (the on-box bar of BASELINE.md section 5), plus the max |logit|
+                          same CUDA-event protocol (the on-GPU bar), plus the max |logit|
                           difference between it and the fused path.
 """
 from __future__ import annotations
@@ -24,6 +25,7 @@ import random
 import statistics
 import subprocess
 import sys
+import tempfile
 import time
 
 import torch
@@ -79,8 +81,8 @@ def read_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    # fallback stated in /opt/skills/guides/B200_PROFILING.md
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- an upper bound, not a measurement
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "data sheet"
 
 
 def cpu_model_string() -> str:
@@ -104,11 +106,10 @@ class ClockSampler:
     def __init__(self, index: int) -> None:
         self.index = index
         self.proc = None
-        self.path = os.path.join(ROOT, "gpurun_out", f"clocks_{index}.csv")
+        self.path = os.path.join(tempfile.gettempdir(), f"vit_bench_clocks_{os.getpid()}_{index}.csv")
 
     def start(self) -> None:
         try:
-            os.makedirs(os.path.dirname(self.path), exist_ok=True)
             self.f = open(self.path, "w")
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), f"--query-gpu={self.FIELDS}",
                                           "--format=csv,noheader,nounits", "-lms", "100"], stdout=self.f,
@@ -138,6 +139,7 @@ class ClockSampler:
             for n, v in zip(names, parts[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(n)
+        os.remove(self.path)
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["no samples"]}
         return {"sm_mhz": statistics.median(sm), "sm_max_mhz": max(mx), "power_w_max": max(pw),
@@ -155,7 +157,7 @@ def model_cfg(args) -> dict:
 
 
 def navit_sizes(batch: int, seed: int):
-    """SURVEY.md 8d config 5: H, W = 16 * randrange(4, 33) per image."""
+    """Config 5: H, W = 16 * randrange(4, 33) per image."""
     rng = random.Random(seed)
     return [(16 * rng.randrange(4, 33), 16 * rng.randrange(4, 33)) for _ in range(batch)]
 
@@ -173,7 +175,7 @@ def navit_flops(cfg: dict, sizes) -> tuple:
 
 
 def import_reference():
-    """The UNMODIFIED reference package installed into baseline/_ref (pip --target, see DESIGN.md); None if absent."""
+    """The UNMODIFIED reference package installed into baseline/_ref (pip --target); None if absent."""
     if not os.path.isdir(os.path.join(REF_DIR, "vit_pytorch")):
         return None
     sys.dont_write_bytecode = True
@@ -240,7 +242,7 @@ def time_cpu(fn, steps: int, warmup: int) -> float:
 
 
 def cpu_matrix(model: str, cfg: dict, budget_s: float) -> list:
-    """BASELINE.md section 4 protocol: fp32 and bf16, B = 16 and 64, all host threads, 1 warm-up + best of 3."""
+    """fp32 and bf16, B = 16 and 64, all host threads, 1 warm-up + best of 3."""
     out = []
     t_end = time.perf_counter() + budget_s
     for dt_name, dt in (("bf16", torch.bfloat16), ("fp32", torch.float32)):
@@ -392,6 +394,10 @@ def run_gpu_arm(args, rank: int, local_rank: int, world: int) -> None:
     e1.record()
     torch.cuda.synchronize()
     launches = _lib.launch_count()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), out.float().cpu().numpy())
     per_rank_ms = all_ranks(e0.elapsed_time(e1))
     ms_total = max(per_rank_ms)
     sync_all()
@@ -488,7 +494,7 @@ def run_gpu_arm(args, rank: int, local_rank: int, world: int) -> None:
             dist.destroy_process_group()
         return
 
-    # ---- roofline of the dominant kernel (the tcgen05 GEMM): CUDA events around every launch of a few more steps ----
+    # ---- roofline of the dominant kernel (the wgmma GEMM): CUDA events around every launch of a few more steps ----
     peaks, peak_src = read_peaks()
     nprof = min(args.steps, 5)
     _lib.profile_start()
@@ -508,16 +514,8 @@ def run_gpu_arm(args, rank: int, local_rank: int, world: int) -> None:
     g = by["gemm"]
     achieved = g["flops"] / g["ms"] / 1e9                     # TFLOP/s over the GEMM launches of the step
     peak = float(peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"]))   # kernel timed inside a long step
-    # dram traffic of the dominant kernel: only from an ncu capture of THIS round's library (profiles/gemm_traffic.json
-    # carries the library version it was taken with); otherwise null
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        if tj.get("lib_version") == int(_lib.lib().b200vit_version()) and tj.get("model", "vit_b16") == args.model:
-            traffic = tj.get("dram_bytes_per_launch")
-    roofline = {"bound": "tensor", "kernel": "gemm2_kernel (tcgen05 cta_group::2)", "achieved": achieved, "peak": peak,
-                "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic, "peak_source": f"{peak_src} sustained",
+    roofline = {"bound": "tensor", "kernel": "gemm_bf16_kernel (wgmma)", "achieved": achieved, "peak": peak,
+                "unit": "TFLOP/s", "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                 "avg_launch_ms": g["ms"] / g["launches"], "launches_per_step": g["launches"] // nprof}
     attn_key = "attention_varlen" if "attention_varlen" in by else ("attention" if "attention" in by else None)
     roofline_attention = None
@@ -554,7 +552,8 @@ def run_gpu_arm(args, rank: int, local_rank: int, world: int) -> None:
                 fn(); n += 1
             dt_s = time.perf_counter() - t0
         cpu_baseline = {"value": args.cpu_batch * n / dt_s, "unit": "images/sec", "cores": cores, "kind": kind,
-                        "sample": f"baseline/_ref reference, bf16, {n} forwards of {args.cpu_batch} images, "
+                        "sample": f"{'baseline/_ref reference' if kind == 'reference' else 'oracle port'}, bf16, "
+                                  f"{n} forwards of {args.cpu_batch} images, "
                                   f"{cores} threads, {cpu_model_string()}"}
 
     energy = None
@@ -567,7 +566,7 @@ def run_gpu_arm(args, rank: int, local_rank: int, world: int) -> None:
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": workload_name(args.model, CFG, B), "batch_per_gpu": B,
                    "global_batch": B * world, "parallelism": f"dp{world}",
-                   "l2_policy": "inputs and activations (GBs/step) exceed the 126 MB L2",
+                   "l2_policy": "inputs and activations (GBs/step) exceed the 50 MB L2",
                    "ln_mode": os.environ.get("B200VIT_LN_MODE", "fold"),
                    "weights": "random init, torch.manual_seed(0)", **extra_cfg},
         "tflops_per_gpu": tf,
@@ -636,7 +635,11 @@ def main() -> None:
                     help="reference arm: seconds the timed steps may take; the per-step sample is halved until they fit")
     ap.add_argument("--model", default="vit_b16", choices=sorted(MODELS), help="vit_b16 is the headline config")
     ap.add_argument("--dim-head", type=int, default=64, help="ViT-H/14 canonical is 80")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="write the logits of the last timed step to DIR/logits.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

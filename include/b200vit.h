@@ -1,8 +1,8 @@
 /*
- * b200vit.h -- C ABI of libb200vit.so: hand-written sm_100a kernels for the ViT encoder forward path.
+ * b200vit.h -- C ABI of libb200vit.so: hand-written sm_90a (H100) kernels for the ViT encoder forward path.
  *
- * The reference (lucidrains/vit-pytorch, /root/reference) is pure Python and has NO plugin / FFI interface;
- * its operator boundary for this path is the nn.Module surface (SURVEY.md 8b).  Each entry point below therefore
+ * The reference (lucidrains/vit-pytorch) is pure Python and has NO plugin / FFI interface;
+ * its operator boundary for this path is the nn.Module surface.  Each entry point below therefore
  * names the reference *operator sequence* it replaces (file:line), and INTEGRATION.md shows the ctypes binding a
  * maintainer of the reference would add.
  *
@@ -27,7 +27,7 @@ extern "C" {
 #define B200VIT_OK 0
 #define B200VIT_ERR_INVALID -1  /* bad argument (shape, alignment, null pointer) */
 #define B200VIT_ERR_CUDA -2     /* a CUDA runtime / driver call failed */
-#define B200VIT_ERR_DEVICE -3   /* not an sm_100 device */
+#define B200VIT_ERR_DEVICE -3   /* not an sm_90 device */
 
 /* GEMM epilogue flags (b200vit_gemm_bf16) */
 #define B200VIT_EPI_BIAS 1      /* + bias[n] (fp32) */
@@ -35,7 +35,6 @@ extern "C" {
 #define B200VIT_EPI_RESIDUAL 4  /* + resid[m, n] (fp32); resid may alias out_f32 (in-place residual stream) */
 #define B200VIT_EPI_LNFOLD 8    /* A is the un-normalised bf16 row, W carries gamma: y = rstd_m*(acc - mu_m*s_n) + bias_n */
 #define B200VIT_EPI_STATS 16    /* write per-row partial (sum, sum^2) of the bf16-rounded result into stats_out */
-#define B200VIT_EPI_HEADNORM 32 /* internal to b200vit_gemm_headnorm_bf16: normalise leading 64-wide heads */
 #define B200VIT_EPI_HEADLN 64   /* b200vit_gemm_headnorm_bf16: per-head LayerNorm (no bias) instead of the RMS norm */
 
 const char* b200vit_last_error(void);
@@ -43,12 +42,12 @@ int b200vit_version(void);
 /* number of kernels this library has launched in the calling process (all threads) since load / last reset */
 int64_t b200vit_launch_count(void);
 void b200vit_reset_launch_count(void);
-/* 0 when device `dev` is sm_100 and the driver entry points the library needs resolve; negative otherwise */
+/* 0 when device `dev` is sm_90 and the driver entry points the library needs resolve; negative otherwise */
 int b200vit_device_ok(int dev);
 
 /*
- * out[M, N] = epilogue( A[M, K] (bf16, row stride lda) x W[N, K]^T (bf16, row stride ldw) ), fp32 accumulate in TMEM.
- * TMA-fed tcgen05 GEMM, persistent, warp specialised.  Replaces every nn.Linear on the path:
+ * out[M, N] = epilogue( A[M, K] (bf16, row stride lda) x W[N, K]^T (bf16, row stride ldw) ), fp32 accumulate.
+ * TMA-fed wgmma GEMM, persistent, warp specialised (one producer and two consumer warpgroups).  Replaces every nn.Linear on the path:
  *   vit.py:20,23 (FeedForward), vit.py:44,47 (to_qkv / to_out), vit.py:102 (patch projection), vit.py:116 (mlp_head);
  *   simple_vit.py:30,32,47,48,93,108.
  * out_bf16 and/or out_f32 (either may be NULL, not both), row stride ldo (elements).
@@ -98,7 +97,7 @@ int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, 
 
 /*
  * im2col-free patch embedding for 16 x 16 patches (vit.py:100-102 without materialising the Rearrange or the
- * LayerNorm): y[B*n, D] fp32 = LN(patch pixels; gamma, beta) W^T + b, with the A operand of the tcgen05 GEMM loaded
+ * LayerNorm): y[B*n, D] fp32 = LN(patch pixels; gamma, beta) W^T + b, with the A operand of the wgmma GEMM loaded
  * straight out of the NCHW bf16 image by a 5-D TMA tensor map (pixel | pixel row | patch column | patch row |
  * image x channel), the LayerNorm folded into the epilogue.
  *   b200vit_patch_stats: stats[B*n][2] = (sum, sum of squares) of each patch's C*256 pixels.
@@ -119,11 +118,9 @@ int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats, int M, in
  * Multi-head softmax attention straight out of the packed QKV buffer:
  *   qkv[B*N, 3*H*dh] bf16 (columns: [q | k | v], each head-major h*dh + d; vit.py:54-55)
  *   out[B*N, H*dh]   bf16 (merged heads, vit.py:63) = softmax(q k^T * scale) v          (vit.py:57-62)
- * One pass over the keys (N <= 512): S = QK^T and O = PV on tcgen05 with TMEM accumulators, fp32 softmax.
- * dh = 64, or 80 (canonical ViT-H/14): an 80-wide head is staged as a 64-wide + a 16-wide shared-memory slab.
- * N = 257 (ViT-H/14 with its cls token) .. 260: the score tile keeps 256 keys, so that two CTAs still share an SM's
- * 512 TMEM columns, and the softmax threads add the last 1..4 keys themselves from shared memory.
- * (A software-pipelined variant for N <= 224, attention_pipe.cu, is built but only reachable through the test hook.)
+ * N <= 512 (longer sequences: b200vit_attention_varlen).  128-row query tiles, keys streamed in blocks with an
+ * online softmax in fp32; S = QK^T and O = PV on the tensor cores (bf16 operands, fp32 accumulation).
+ * dh = 64, or 80 (canonical ViT-H/14).
  */
 int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* stream);
 
@@ -131,7 +128,7 @@ int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, f
  * Variable-length attention over PACKED sequences (any length): tokens [cu_seqlens[s], cu_seqlens[s+1]) of
  * qkv[total_tokens, 3*H*dh] attend only among themselves; out[total_tokens, H*dh].  This is the block-diagonal
  * "same image" attention of NaViT (na_vit.py:335-337 mask + 161-166 SDPA) without padding or an O(L^2) mask, and the
- * long-sequence (N > 512) path of ViT.  cu_seqlens_dev[num_seqs+1] and tile_prefix_dev[num_seqs+1] (number of 128-row
+ * long-sequence (N > 512) path of ViT.  dh = 64 or 80.  cu_seqlens_dev[num_seqs+1] and tile_prefix_dev[num_seqs+1] (number of 128-row
  * query tiles before sequence s; tile_prefix[num_seqs] == total_tiles) are DEVICE int32 arrays built by the caller.
  */
 int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev,
@@ -159,8 +156,7 @@ int b200vit_qk_rmsnorm(void* qkv, const float* gamma_qk, int T, int H, int dh, v
  *   out[M, N] bf16 = epilogue(A W^T)   with flags in {EPI_BIAS, EPI_LNFOLD} exactly as b200vit_gemm_bf16, then the first
  *   norm_heads heads (dh = 64 columns each, from column 0) of every row are replaced by
  *   v / max(||v||, 1e-12) * sqrt(dh) * head_gamma[h, d]   (norm computed on the bf16-rounded projection, like the
- *   reference's bf16 module).  Large problems run the norm inside the CTA-pair GEMM epilogue (one warp owns one
- *   head of 32 rows); small ones run b200vit_gemm_bf16 + b200vit_rmsnorm_heads / b200vit_layernorm_heads.
+ *   reference's bf16 module): b200vit_gemm_bf16 followed by b200vit_rmsnorm_heads / b200vit_layernorm_heads.
  *   flags | EPI_HEADLN: the heads get nn.LayerNorm(dh, bias=False) instead -- (v - mean) * rsqrt(var + head_eps) *
  *   head_gamma[h, d] -- the q / k norm of the nested-tensor NaViT (na_vit_nested_tensor.py:61-62,101-102).
  */
@@ -244,19 +240,13 @@ int b200vit_encoder_blocks(const b200vit_layer* layers, int depth, float* x, con
 /*
  * TEST HOOKS -- process-global switches for A/B tests and bring-up; NOT part of the re-entrant API above (a value set
  * here changes every later call of every thread).  Production code never calls them.
- *   key 1: b200vit_attention kernel choice: 0 = auto, 1 = round-1 kernels only, 2 = pipelined kernel wherever N <= 224
- *   key 2 / 3: V (MN-major) descriptor LBO / SBO bytes (bring-up probe)
- *   key 4: GEMM kernel choice: 0 = auto, 1 = single-CTA kernel, 2 = CTA-pair kernel wherever its epilogue applies
- *   key 11: varlen attention kernel: 0 = pipelined 64-key blocks, one pass (default), 1 = serial 128-key blocks,
- *           2 = pipelined 64-key blocks, two passes (exact max first)
- *   key 12: fp32-epilogue warps of the CTA-pair GEMM: 0 = auto (4 when K >= 2048, else 8), 4 / 8 = forced
- *   key 14 / 15: dim_head 80: LBO / SBO bytes of the 16-wide V slab descriptor (bring-up probe)
- *   key 16: b200vit_attention key tail on the CUDA cores (N = 256 + 1..4 keys): 1 = on (default), 0 = off
- *   key 13: pipelined attention: 0 = all softmax exponentials on MUFU (default), 1 = half of them on the FMA pipe
+ *   key 1: b200vit_attention key block: 0 / 1 = 64 keys (default), 2 = 128 keys
+ *   key 11: b200vit_attention_varlen: 0 = 64-key blocks (default), 1 = 128-key blocks, 2 = 64-key blocks with half of
+ *           the softmax exponentials on the FMA pipe
+ *   key 12: BLOCK_N of b200vit_gemm_bf16: 0 = auto (256 when N > 128, else 128), 1 = 128, 2 = 256
+ *   key 13: b200vit_attention: 0 = all softmax exponentials on MUFU (default), 1 = half of them on the FMA pipe
  */
 int b200vit_debug_set(int key, int value);
-/* timing experiment: device buffer of int64[64][16] receiving %globaltimer stamps of CTA 0 of b200vit_attention_varlen */
-void b200vit_debug_set_trace(void* dev_buf);
 
 #ifdef __cplusplus
 }

@@ -1,8 +1,7 @@
-"""Generate golden fixtures from the UNMODIFIED reference (lucidrains/vit-pytorch at /root/reference).
+"""Generate golden fixtures from the UNMODIFIED reference (lucidrains/vit-pytorch 1.23.6, a checkout of which
+VIT_REFERENCE points at):
 
-Run in the build container only (the GPU box has no /root/reference):
-
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    VIT_REFERENCE=<checkout> PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py [reference_live]
 
 For each case: build the reference model under torch.manual_seed(seed), round its parameters to bf16-representable
 values (so the same numbers can be fed to the bf16 CUDA path), run the reference forward in fp32 on CPU on a
@@ -17,7 +16,7 @@ import sys
 
 import torch
 
-REF = os.environ.get("VIT_REFERENCE", "/root/reference")
+REF = os.environ["VIT_REFERENCE"]
 sys.path.insert(0, REF)
 sys.dont_write_bytecode = True
 
@@ -27,7 +26,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
 CASES = {
-    # BASELINE.json configs[0]: SimpleViT tiny (num_classes / mlp_dim chosen in SURVEY.md 8d)
+    # BASELINE.json configs[0]: SimpleViT tiny
     "simplevit_tiny": dict(kind="simple", seed=0, batch=4, img=(32, 32),
                            kwargs=dict(image_size=32, patch_size=4, num_classes=10, dim=192, depth=2, heads=3,
                                        mlp_dim=768)),
@@ -45,7 +44,7 @@ CASES = {
                                         mlp_dim=256)),
 }
 
-# Round 2: attention without output projection (vit.py:34,46-49) and the SURVEY.md 8(f3) SimpleViT-family variants.
+# Round 2: attention without output projection (vit.py:34,46-49) and the SimpleViT-family variants.
 # `kind` = module name inside the reference package for the variants.
 CASES2 = {
     "vit_tiny_noproj": dict(kind="vit", seed=4, batch=3, img=(32, 32),
@@ -66,7 +65,7 @@ CASES2 = {
 }
 
 
-# Round 2, later: the 1-D / 3-D front-ends of SURVEY.md 8(f3) (series and video inputs; `img` = the non-channel dims)
+# Round 2, later: the 1-D / 3-D front-ends (series and video inputs; `img` = the non-channel dims)
 CASES3 = {
     "simplevit_1d": dict(kind="simple_vit_1d", seed=12, batch=3, img=(256,),
                          kwargs=dict(seq_len=256, patch_size=16, num_classes=10, dim=128, depth=2, heads=2,
@@ -126,7 +125,7 @@ def make(name: str, spec: dict) -> None:
         "logits_fp32": logits.clone(),
         "logits_ref_bf16": logits_bf16.float().clone(),
         "tokens_fp32": None if tokens is None else tokens.clone(),
-        "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6 @ /root/reference"},
+        "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6"},
     }
     path = os.path.join(HERE, name + ".pt")
     torch.save(blob, path)
@@ -158,7 +157,7 @@ def make_navit() -> None:
             "state_dict": {k: v.bfloat16() for k, v in model.state_dict().items()},
             "images": imgs, "rows": rows, "group_max_seq_len": 80,
             "logits_fp32": packed.clone(), "logits_grouped_fp32": grouped.clone(),
-            "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6 @ /root/reference"}}
+            "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6"}}
     path = os.path.join(HERE, "navit_tiny.pt")
     torch.save(blob, path)
     print(f"navit_tiny: logits {tuple(packed.shape)} |max| {packed.abs().max():.4f}; packed vs grouped "
@@ -180,7 +179,7 @@ def make_navit_config5() -> None:
              "frac_within_tol": (d <= 1e-3 + 1e-2 * fp32.abs()).float().mean().item()}
     blob = {"name": "navit_config5", "kind": "navit", "spec": NAVIT_C5, "logits_fp32": fp32.clone(),
             "logits_ref_bf16": bf16.clone(), "ref_bf16_floor": floor,
-            "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6 @ /root/reference"}}
+            "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6"}}
     path = os.path.join(HERE, "navit_config5.pt")
     torch.save(blob, path)
     print(f"navit_config5: logits {tuple(fp32.shape)} |max| {fp32.abs().max():.4f}; reference-bf16 floor {floor}; "
@@ -213,14 +212,98 @@ def make_navit_nested() -> None:
         blob = {"name": name, "kind": "navit_nested", "kwargs": kwargs,
                 "state_dict": {k: v.bfloat16() for k, v in model.state_dict().items()}, "images": imgs,
                 "logits_fp32": fp32.clone(), "logits_ref_bf16": bf16.float().clone(),
-                "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6 @ /root/reference"}}
+                "versions": {"torch": str(torch.__version__), "reference": "vit-pytorch 1.23.6"}}
         path = os.path.join(HERE, name + ".pt")
         torch.save(blob, path)
         print(f"{name}: logits {tuple(fp32.shape)} |max| {fp32.abs().max():.4f}; ref-bf16 max err "
               f"{(bf16.float() - fp32).abs().max():.5f}; {os.path.getsize(path) / 1e6:.2f} MB")
 
 
+def state_digest(sd) -> dict:
+    """sha256 of every tensor's bytes: bit-identical initialisation is checked without storing the weights."""
+    import hashlib
+    return {k: (tuple(v.shape), str(v.dtype), hashlib.sha256(v.detach().contiguous().cpu().numpy().tobytes()).hexdigest())
+            for k, v in sd.items()}
+
+
+def signature(cls) -> list:
+    import inspect
+    return [(k, repr(v.default)) for k, v in inspect.signature(cls.__init__).parameters.items() if k != "self"]
+
+
+def make_reference_live():
+    """tests/golden/reference_live.pt: what the tests used to read off a live reference checkout -- same-seed
+    initialisations (as digests), constructor signatures, reference logits of seeded models and inputs, and the
+    reference Recorder's attention maps."""
+    import importlib
+    ref = importlib.import_module("vit_pytorch")
+    out = {"init": {}, "signature": {}, "logits": {}, "versions": {"torch": str(torch.__version__),
+                                                                    "reference": "vit-pytorch 1.23.6"}}
+    kw = dict(image_size=32, patch_size=8, num_classes=5, dim=64, depth=2, heads=2, mlp_dim=96, dim_head=32)
+    for kind, cls in (("vit", ref.ViT), ("simple", ref.SimpleViT)):
+        torch.manual_seed(123)
+        m = cls(**kw)
+        out["init"][f"dropin_{kind}"] = state_digest(m.state_dict())
+        if kind == "simple":
+            out["init"]["dropin_simple_pos"] = state_digest({"pos_embedding": m.pos_embedding})
+    # SimpleViT-family variants and the nested-tensor NaViT (tests/test_variants.py)
+    for name, spec in {**CASES2, **CASES3}.items():
+        if spec["kind"] == "vit":
+            continue
+        cls = importlib.import_module("vit_pytorch." + spec["kind"]).SimpleViT
+        out["signature"][name] = signature(cls)
+        torch.manual_seed(123)
+        out["init"][name] = state_digest(cls(**spec["kwargs"]).state_dict())
+    nested = importlib.import_module("vit_pytorch.na_vit_nested_tensor").NaViT
+    out["signature"]["navit_nested"] = signature(nested)
+    torch.manual_seed(5)
+    out["init"]["navit_nested"] = state_digest(nested(image_size=32, patch_size=8, num_classes=5, dim=64, depth=1,
+                                                      heads=1, mlp_dim=64).state_dict())
+    # NaViT: init and forward on three images in two groups (tests/test_navit.py)
+    navit = importlib.import_module("vit_pytorch.na_vit").NaViT
+    nkw = dict(image_size=32, patch_size=8, num_classes=5, dim=64, depth=1, heads=2, mlp_dim=96, dim_head=32)
+    torch.manual_seed(9)
+    a = navit(**nkw).eval()
+    out["init"]["navit"] = state_digest(a.state_dict())
+    imgs = [torch.randn(3, 32, 16), torch.randn(3, 8, 8), torch.randn(3, 24, 32)]
+    with torch.inference_mode():
+        out["logits"]["navit"] = {"logits": a([imgs[:2], imgs[2:]])}
+    # seeded reference forwards (tests/test_oracle.py): model under seed, then the input from the global generator
+    for kind, seed in (("vit", 11), ("simple", 12), ("vit", 13)):
+        torch.manual_seed(seed)
+        okw = dict(image_size=64, patch_size=16, num_classes=17, dim=128, depth=2, heads=2, mlp_dim=192)
+        if kind == "vit" and seed == 13:
+            okw["pool"] = "mean"
+        model = (ref.ViT if kind == "vit" else ref.SimpleViT)(**okw).eval()
+        out["init"][f"oracle_{kind}_{seed}"] = state_digest(model.state_dict())
+        img = torch.randn(3, 3, 64, 64)
+        with torch.inference_mode():
+            out["logits"][f"oracle_{kind}_{seed}"] = {"logits": model(img)}
+    torch.manual_seed(0)
+    bkw = dict(image_size=224, patch_size=16, num_classes=1000, dim=768, depth=12, heads=12, mlp_dim=3072)
+    model = ref.ViT(**bkw).eval()
+    out["init"]["oracle_vit_b16"] = state_digest(model.state_dict())
+    torch.manual_seed(1)
+    img = torch.randn(1, 3, 224, 224)
+    with torch.inference_mode():
+        out["logits"]["oracle_vit_b16"] = {"logits": model(img)}
+    # the reference Recorder's attention maps (tests/test_dropin.py::test_recorder_and_extractor_twins)
+    Recorder = importlib.import_module("vit_pytorch.recorder").Recorder
+    torch.manual_seed(0)
+    r = ref.ViT(image_size=32, patch_size=8, num_classes=3, dim=32, depth=2, heads=2, mlp_dim=48, dim_head=16).eval()
+    out["init"]["recorder_vit"] = state_digest(r.state_dict())
+    img = torch.randn(2, 3, 32, 32)
+    with torch.no_grad():
+        out["logits"]["recorder"] = {"attns": Recorder(r)(img)[1]}
+    path = os.path.join(HERE, "reference_live.pt")
+    torch.save(out, path)
+    print(f"reference_live: {os.path.getsize(path) / 1e3:.1f} kB")
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "reference_live":
+        make_reference_live()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "navit_nested":
         make_navit_nested()
         sys.exit(0)

@@ -1,5 +1,5 @@
 """bench.py output contract (CPU side): the reference arm prints ONE JSON line with the keys the driver reads, and the
-flop / metric bookkeeping of the GPU arm matches SURVEY.md 8d."""
+flop / metric bookkeeping of the GPU arm matches the analytic FLOP counts."""
 import json
 import os
 import subprocess
@@ -33,11 +33,11 @@ def test_algorithmic_flops_match_the_survey():
     sys.path.insert(0, ROOT)
     import bench
     from oracle import vit_oracle as O
-    assert abs(O.flops_per_image(**bench.VIT_B16) / 1e9 - 35.128) < 0.01      # SURVEY.md 8d: ViT-B/16 (cls)
+    assert abs(O.flops_per_image(**bench.VIT_B16) / 1e9 - 35.128) < 0.01      # ViT-B/16 (cls)
     assert abs(O.flops_per_image(**bench.MODELS["vit_l16"]) / 1e9 - 123.109) < 0.05
     assert abs(O.flops_per_image(**bench.MODELS["vit_h14"]) / 1e9 - 310.867) < 0.1
     assert abs(O.flops_per_image(**bench.MODELS["vit_h14"], dim_head=80) / 1e9 - 334.590) < 0.1
-    # NaViT config 5 (SURVEY.md 8d): 256 images / 83 901 tokens, block-diagonal attention 1.017 TFLOP
+    # NaViT config 5: 256 images / 83 901 tokens, block-diagonal attention 1.017 TFLOP
     sizes = bench.navit_sizes(256, 0)
     gemm, attn = bench.navit_flops(bench.MODELS["navit"], sizes)
     assert sum((h // 16) * (w // 16) for h, w in sizes) == 83901

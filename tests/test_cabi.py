@@ -68,14 +68,16 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
         _lib.lib()
 
 
-def test_library_contains_blackwell_instructions():
-    """SASS evidence that the hot kernels are tcgen05 / TMA code (B200_PROFILING.md 'What proves ...')."""
+def test_library_contains_hopper_instructions():
+    """SASS evidence that the GEMM and the attention are wgmma code fed by TMA through mbarriers."""
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump) or not _lib.LIB_PATH.exists():
         pytest.skip("cuobjdump or library not available")
     sass = subprocess.run([cuobjdump, "-sass", str(_lib.LIB_PATH)], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "STTM"):
+    assert "arch = sm_90a" in sass
+    for mnemonic in ("HGMMA.64x256x16.F32.BF16", "HGMMA.64x128x16.F32.BF16", "HGMMA.64x64x16.F32.BF16", "UTMALDG",
+                     "SYNCS"):
         assert mnemonic in sass, mnemonic
-    assert "HMMA.16816" not in sass          # no legacy mma.sync tensor path
+    assert "HMMA.16816" not in sass          # no warp-level mma.sync tensor path

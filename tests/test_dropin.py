@@ -1,4 +1,4 @@
-"""Host-side drop-in contract of vit_pytorch_b200.ViT / SimpleViT (SURVEY.md 8b): constructor signature, state_dict
+"""Host-side drop-in contract of vit_pytorch_b200.ViT / SimpleViT: constructor signature, state_dict
 layout, attribute surface, eager-graph values against the reference goldens, dispatch rules.  CPU only."""
 import inspect
 
@@ -6,7 +6,7 @@ import pytest
 import torch
 from torch import nn
 
-from conftest import import_reference, load_golden, reference_available
+from conftest import import_reference, load_golden, reference_available, reference_live, state_digest
 from vit_pytorch_b200 import SimpleViT, ViT
 from vit_pytorch_b200 import simple_vit as sv_mod
 from vit_pytorch_b200 import vit as vit_mod
@@ -121,26 +121,24 @@ def test_hooks_force_the_observable_graph():
     h.remove()
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference checkout not present (GPU box)")
 @pytest.mark.parametrize("kind", ["vit", "simple"])
 def test_same_seed_gives_bit_identical_init(kind):
-    ref = import_reference()
+    """The reference's initialisation under the same seed, stored as per-tensor digests of its state_dict."""
+    want = reference_live()["init"][f"dropin_{kind}"]
     kwargs = dict(image_size=32, patch_size=8, num_classes=5, dim=64, depth=2, heads=2, mlp_dim=96, dim_head=32)
     torch.manual_seed(123)
-    a = (ref.ViT if kind == "vit" else ref.SimpleViT)(**kwargs)
-    torch.manual_seed(123)
     b = (ViT if kind == "vit" else SimpleViT)(**kwargs)
-    sa, sb = a.state_dict(), b.state_dict()
-    assert list(sa) == list(sb)
-    for k in sa:
-        assert torch.equal(sa[k], sb[k]), k
+    got = state_digest(b.state_dict())
+    assert list(got) == list(want)
+    for k in want:
+        assert got[k] == want[k], k
     if kind == "simple":
-        assert torch.equal(a.pos_embedding, b.pos_embedding)
+        assert state_digest({"pos_embedding": b.pos_embedding}) == reference_live()["init"]["dropin_simple_pos"]
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference checkout not present (GPU box)")
+@pytest.mark.skipif(not reference_available(), reason="runs the reference's own code: no reference package (oracle/_ref or VIT_REFERENCE)")
 def test_reference_wrappers_accept_the_dropin():
-    """Recorder / Extractor from the reference operate on our module tree (SURVEY.md 3.4)."""
+    """Recorder / Extractor from the reference operate on our module tree."""
     import importlib
     import_reference()
     Extractor = importlib.import_module("vit_pytorch.extractor").Extractor
@@ -161,7 +159,7 @@ def _pair_with_reference(**kwargs):
     return ours, ref
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference checkout not present")
+@pytest.mark.skipif(not reference_available(), reason="runs the reference's own code: no reference package (oracle/_ref or VIT_REFERENCE)")
 def test_reference_mae_wrapper_runs_on_the_dropin():
     """MAE (reference mae.py:28-31,50-55,74) reads `to_patch_embedding[0]`, `[1:]`, `[2].weight`, `pos_embedding`,
     `pool` and calls `encoder.transformer(tokens)` on the unmasked quarter of the tokens: same loss as on the
@@ -188,7 +186,7 @@ def test_reference_mae_wrapper_runs_on_the_dropin():
     assert ours.transformer.layers[0][0].to_qkv.weight.grad is not None
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference checkout not present")
+@pytest.mark.skipif(not reference_available(), reason="runs the reference's own code: no reference package (oracle/_ref or VIT_REFERENCE)")
 def test_reference_distill_wrapper_accepts_the_dropin_as_teacher():
     """DistillWrapper (reference distill.py:104-152) calls `teacher(img)` under no_grad."""
     import importlib
@@ -224,19 +222,13 @@ def test_recorder_and_extractor_twins():
         first = Extractor(v, layer=v.transformer.layers[0][1], layer_save_input=True)
         _, inp = first(img)
         assert isinstance(inp, tuple) and inp[0].shape == (2, 17, 32)
-    if reference_available():
-        import importlib
-        import_reference()
-        RefRecorder = importlib.import_module("vit_pytorch.recorder").Recorder
-        RefViT = importlib.import_module("vit_pytorch.vit").ViT
-        r = RefViT(image_size=32, patch_size=8, num_classes=3, dim=32, depth=2, heads=2, mlp_dim=48, dim_head=16).eval()
-        r.load_state_dict(v.state_dict())
-        with torch.no_grad():
-            _, ref_attns = RefRecorder(r)(img)
-        assert torch.allclose(ref_attns, attns, atol=1e-6)
+    # the reference's Recorder on the reference ViT with the same seed and input
+    live = reference_live()
+    assert state_digest(v.state_dict()) == live["init"]["recorder_vit"]
+    assert torch.allclose(live["logits"]["recorder"]["attns"], attns, atol=1e-6)
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference checkout not present")
+@pytest.mark.skipif(not reference_available(), reason="runs the reference's own code: no reference package (oracle/_ref or VIT_REFERENCE)")
 def test_reference_accept_video_wrapper_runs_on_the_dropin():
     """AcceptVideoWrapper (reference accept_video_wrapper.py:26-150) reads `image_net.patch_size` and feeds the frames
     of a clip through `image_net.forward` as one batch: same output as on the reference's own ViT."""

@@ -139,7 +139,7 @@ def test_patchify_ln(C, H, W, p):
 @pytest.mark.parametrize("B,C,H,W,D", [(3, 3, 224, 224, 256), (2, 3, 32, 48, 64), (2, 1, 64, 64, 128), (5, 3, 16, 16, 64),
                                         (2, 3, 16, 512, 72), (1, 4, 48, 16, 64)])
 def test_patch_embed_tma_matches_patchify_layernorm_linear(B, C, H, W, D):
-    """im2col-free patch embedding: the tcgen05 GEMM reads the NCHW image through a 5-D TMA map, LayerNorm(patch) is
+    """im2col-free patch embedding: the wgmma GEMM reads the NCHW image through a 5-D TMA map, LayerNorm(patch) is
     folded into its epilogue -- against Rearrange -> LayerNorm -> Linear (vit.py:100-102) in fp32 on the CPU."""
     torch.manual_seed(H * W + C)
     pd = C * 256
@@ -203,7 +203,7 @@ def test_rowstats_cast():
 @pytest.mark.parametrize("M,N,K", [(2048, 768, 768), (1300, 1024, 512),
                                    (1536, 384, 384), (1100, 320, 2304)])   # last N tile only partly valid (ViT-S dims)
 def test_gemm_pair_kernel_dual_epilogue(M, N, K):
-    """CTA-pair kernel, LN-fold producer epilogue: fp32 stream in place + bf16 copy + row statistics."""
+    """Producer epilogue of the residual GEMMs: fp32 stream in place + bf16 copy + row statistics."""
     torch.manual_seed(M)
     a = torch.randn(M, K, device=DEV).bfloat16()
     w = (torch.randn(N, K, device=DEV) / math.sqrt(K)).bfloat16()
@@ -242,11 +242,9 @@ def test_gelu_epilogue_accuracy():
 
 @pytest.mark.parametrize("B,N,H", [(4, 197, 12), (3, 64, 3), (2, 257, 16), (5, 50, 4), (2, 16, 2), (2, 129, 2),
                                    (1, 512, 1), (2, 1, 2),
-                                   # pipelined kernel (N <= 224): more units than SMs (several units per CTA, ring
-                                   # wrap-around of the 3 K/V stages), one-tile units, the 224-key TMEM limit, and 225
-                                   # keys = first shape of the round-1 kernel again
+                                   # more CTAs than SMs, key counts on and just past a key-block boundary
                                    (40, 197, 12), (70, 196, 16), (200, 128, 3), (37, 224, 5), (3, 225, 2), (9, 33, 7)])
-@pytest.mark.parametrize("kernel", [0, 2])      # test hook 1: 0 = default kernels, 2 = pipelined kernel (N <= 224)
+@pytest.mark.parametrize("kernel", [0, 2])      # test hook 1: 0 = 64-key blocks (default), 2 = 128-key blocks
 def test_attention(B, N, H, kernel):
     torch.manual_seed(N)
     dh = 64
@@ -268,8 +266,8 @@ def test_attention(B, N, H, kernel):
 
 @pytest.mark.parametrize("knob,value,B,N", [(1, 2, 3, 197), (1, 2, 40, 128), (1, 2, 2, 50), (13, 1, 3, 197)])
 def test_attention_kernel_variants_agree(knob, value, B, N):
-    """b200vit_debug_set(1, 2) routes N <= 224 to the software-pipelined kernel, (13, 1) puts half of its
-    exponentials on the FMA pipe: every implementation must produce the same attention."""
+    """b200vit_debug_set(1, 2) streams the keys in 128-key blocks, (13, 1) puts half of the softmax exponentials on
+    the FMA pipe: every implementation must produce the same attention."""
     L = _lib.lib()
     torch.manual_seed(7)
     H, dh = 4, 64
@@ -291,7 +289,7 @@ def test_attention_kernel_variants_agree(knob, value, B, N):
 
 @pytest.mark.parametrize("B,N,H", [(2, 257, 16), (3, 197, 4), (5, 64, 2), (2, 400, 3), (1, 512, 2), (40, 129, 5)])
 def test_attention_dim_head_80(B, N, H):
-    """Canonical ViT-H/14 head width (reference vit.py:86 `dim_head`): 64-wide + 16-wide shared-memory slabs."""
+    """Canonical ViT-H/14 head width (reference vit.py:86 `dim_head`)."""
     torch.manual_seed(N)
     dh = 80
     I = H * dh
@@ -309,9 +307,8 @@ def test_attention_dim_head_80(B, N, H):
 @pytest.mark.parametrize("dh", [64, 80])
 @pytest.mark.parametrize("B,N,H", [(3, 257, 4), (2, 258, 2), (2, 260, 3), (40, 257, 16), (1, 261, 2), (300, 257, 2)])
 def test_attention_key_tail(B, N, H, dh):
-    """N = 256 + (1..4): the S tile keeps 256 keys (two CTAs per SM) and the softmax threads add the last keys' scores
-    and P V terms from shared memory.  Checked against the fp32 oracle with the tail keys made the dominant ones, and
-    against the 272-column-tile path (test hook 16 = 0)."""
+    """N = 256 + (1..5): the last keys sit alone in the final key block.  Checked against the fp32 oracle with the tail
+    keys made the dominant ones, with 64-key and 128-key blocks (test hook 1 = 1 / 2), and the two against each other."""
     torch.manual_seed(N + dh)
     I = H * dh
     qkv = torch.randn(B * N, 3 * I, device=DEV)
@@ -319,29 +316,28 @@ def test_attention_key_tail(B, N, H, dh):
     qkv = qkv.bfloat16()
     L = _lib.lib()
     outs = {}
-    for tails in (1, 0):
+    for tails in (1, 2):
         out = torch.zeros(B * N, I, device=DEV, dtype=torch.bfloat16)
-        L.b200vit_debug_set(16, tails)
+        L.b200vit_debug_set(1, tails)
         try:
             _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5)
             torch.cuda.synchronize()
         finally:
-            L.b200vit_debug_set(16, 1)
+            L.b200vit_debug_set(1, 0)
         outs[tails] = out.float().cpu()
     q, k, v = qkv.float().cpu().view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
     ref = (O.softmax_last((q @ k.transpose(-1, -2)) * dh ** -0.5) @ v).permute(0, 2, 1, 3).reshape(B * N, I)
-    for tails in (1, 0):
+    for tails in (1, 2):
         assert within(outs[tails], ref) > 0.995, tails
         assert (outs[tails] - ref).abs().max() < 2e-2, tails
-    assert (outs[1] - outs[0]).abs().max() < 2e-2
+    assert (outs[1] - outs[2]).abs().max() < 2e-2
 
 
 def test_attention_is_deterministic_and_batch_invariant():
-    """The persistent kernel strides units over CTAs: the same (image, head) must give the same bits wherever it
-    lands in the batch and on repeated launches."""
+    """The same (image, head) must give the same bits wherever it lands in the batch and on repeated launches."""
     torch.manual_seed(11)
     B, N, H, dh = 64, 197, 12, 64
-    _lib.lib().b200vit_debug_set(1, 2)          # the persistent pipelined kernel (test hook), restored below
+    _lib.lib().b200vit_debug_set(1, 2)          # 128-key blocks (test hook), restored below
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV).bfloat16()
     out = torch.zeros(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
     out2 = torch.zeros_like(out)
@@ -356,8 +352,8 @@ def test_attention_is_deterministic_and_batch_invariant():
     assert torch.equal(out3, out[5 * N: 9 * N])
 
 
-def test_gemm_long_k_epilogue_warp_variants_agree():
-    """K >= 2048 fp32 epilogues run with 4 epilogue warps and one more operand stage (test hook 12 forces either)."""
+def test_gemm_long_k_block_n_variants_agree():
+    """Long-K fp32 epilogues with 128- and 256-column tiles (test hook 12 forces either): the same bits."""
     torch.manual_seed(12)
     M, N, K = 2048 + 64, 768, 3072
     a = torch.randn(M, K, device=DEV).bfloat16()
@@ -366,7 +362,7 @@ def test_gemm_long_k_epilogue_warp_variants_agree():
     x0 = torch.randn(M, N, device=DEV)
     res = {}
     L = _lib.lib()
-    for ew in (4, 8):
+    for ew in (1, 2):
         L.b200vit_debug_set(12, ew)
         try:
             x = x0.clone()
@@ -380,14 +376,14 @@ def test_gemm_long_k_epilogue_warp_variants_agree():
             L.b200vit_debug_set(12, 0)
         res[ew] = (x, xb, st.sum(dim=1), y)
     ref = x0.cpu() + a.float().cpu() @ w.float().cpu().t() + bias.cpu()
-    for ew in (4, 8):
+    for ew in (1, 2):
         x, xb, st, y = res[ew]
         assert torch.isfinite(st).all()
         assert within(x, ref, rtol=1e-3, atol=2e-3) > 0.999
         assert torch.equal(xb, x.bfloat16())
         assert torch.allclose(st[:, 0].cpu(), xb.float().sum(1).cpu(), rtol=1e-3, atol=1e-2)
         assert torch.allclose(st[:, 1].cpu(), (xb.float() ** 2).sum(1).cpu(), rtol=1e-3, atol=1e-2)
-    assert torch.equal(res[4][0], res[8][0]) and torch.equal(res[4][3], res[8][3])
+    assert torch.equal(res[1][0], res[2][0]) and torch.equal(res[1][3], res[2][3])
 
 
 def test_attention_large_logits_are_stable():

@@ -109,7 +109,7 @@ def test_fused_equals_own_eager_graph_closely():
 @pytest.mark.parametrize("kind", ["vit", "simple"])
 def test_vit_b16_against_oracle(kind):
     """BASELINE.json configs[1] geometry at B=2 (the oracle finishes in seconds): error vs the fp32 oracle must be
-    below the reference's own bf16 noise floor measured in BASELINE.md section 6 (max 0.0211 / 64.6 % within tol for
+    below the reference's own bf16 noise floor (max 0.0211 / 64.6 % within tol for
     ViT-B/16; 0.0046 / 92.8 % for SimpleViT-B/16)."""
     kwargs = dict(image_size=224, patch_size=16, num_classes=1000, dim=768, depth=12, heads=12, mlp_dim=3072)
     torch.manual_seed(0)
@@ -128,12 +128,12 @@ def test_vit_b16_against_oracle(kind):
 
 @pytest.mark.parametrize("name,kwargs,floor_max,floor_frac", [
     # BASELINE.json configs[2] / configs[3] geometry (dim_head = reference default 64); the floors are the reference's
-    # own bf16 forward against its fp32 forward, BASELINE.md section 6
+    # own bf16 forward against its fp32 forward
     ("ViT-L/16", dict(image_size=224, patch_size=16, num_classes=1000, dim=1024, depth=24, heads=16, mlp_dim=4096),
      0.0249, 0.525),
     ("ViT-H/14", dict(image_size=224, patch_size=14, num_classes=1000, dim=1280, depth=32, heads=16, mlp_dim=5120),
      0.0257, 0.478),
-    # the canonical ViT-H/14 head width: dim_head = 80 (SURVEY.md 8d config 4 "run with dim_head=64 and 80")
+    # the canonical ViT-H/14 head width: dim_head = 80
     ("ViT-H/14 dim_head 80", dict(image_size=224, patch_size=14, num_classes=1000, dim=1280, depth=32, heads=16,
                                   mlp_dim=5120, dim_head=80), 0.0298, 0.478),
 ])
@@ -227,7 +227,7 @@ def test_cuda_graph_replay_is_bit_identical():
 @pytest.mark.parametrize("kind", ["vit_cls", "vit_mean", "simple"])
 def test_extractor_hook_keeps_the_fused_path(kind):
     """Extractor (reference extractor.py:50-59) hooks `vit.transformer`: the fused forward routes the tokens through
-    that module call, so the hook sees the encoder output while every block still runs in the sm_100a kernels."""
+    that module call, so the hook sees the encoder output while every block still runs in the sm_90a kernels."""
     from vit_pytorch_b200.extractor import Extractor
     torch.manual_seed(0)
     kw = dict(image_size=64, patch_size=8, num_classes=10, dim=128, depth=2, heads=2, mlp_dim=256)
@@ -357,10 +357,10 @@ def test_trained_like_statistics_stay_below_the_bf16_floor(mode, monkeypatch):
 
 def test_reference_distill_wrapper_runs_its_teacher_on_the_fused_path():
     """DistillWrapper (reference distill.py:104-152) calls `teacher(img)` under no_grad: with the drop-in as the
-    teacher (cuda, bf16) that call is the fused sm_100a forward; the student is the reference's own DistillableViT."""
+    teacher (cuda, bf16) that call is the fused sm_90a forward; the student is the reference's own DistillableViT."""
     from conftest import import_reference, reference_available
     if not reference_available():
-        pytest.skip("no reference package (neither /root/reference nor baseline/_ref)")
+        pytest.skip("runs the reference's own code: no reference package (oracle/_ref or VIT_REFERENCE)")
     import importlib
     import_reference()
     distill = importlib.import_module("vit_pytorch.distill")

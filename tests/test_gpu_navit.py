@@ -1,4 +1,4 @@
-"""-m gpu: NaViT through the fused padding-free sm_100a path against the reference golden and the per-image oracle."""
+"""-m gpu: NaViT through the fused padding-free sm_90a path against the reference golden and the per-image oracle."""
 import random
 
 import pytest
@@ -86,7 +86,7 @@ def test_navit_config5_geometry_against_reference_golden():
     assert torch.equal(out, out_rows)
 
 
-# 0: pipelined 64-key blocks, one pass (default); 1: serial 128-key blocks; 2: pipelined, two passes (max first)
+# test hook 11: 0 = 64-key blocks (default), 1 = 128-key blocks, 2 = 64-key blocks, half the exponentials on the FMA pipe
 @pytest.mark.parametrize("mode", [0, 1, 2])
 def test_varlen_attention_kernel_against_oracle(mode):
     lengths = [197, 1, 130, 577, 64, 1024, 129, 65, 63, 128, 300]
@@ -114,10 +114,10 @@ def test_varlen_attention_kernel_against_oracle(mode):
 
 @pytest.mark.parametrize("pattern", ["rising", "falling", "spike_late", "mixed_rows"])
 def test_varlen_attention_one_pass_moves_its_reference_max(pattern):
-    """The default one-pass kernel takes exponentials against a reference max that it only moves when a later key
-    block exceeds it by more than 2^24, rescaling O in TMEM.  Scores built to rise by ~2^40 per 64-key block (every
-    block triggers the rescale), to fall, to spike in the last block only, and to do so for some rows of a warp only;
-    same expectation (fp32 softmax on the CPU) as the ordinary test, and equal to the two-pass kernel's output."""
+    """The online softmax rescales O whenever a later key block raises the running max.  Scores built to rise by ~2^40
+    per 64-key block (every block triggers the rescale), to fall, to spike in the last block only, and to do so for
+    some rows of a warp only; same expectation (fp32 softmax on the CPU) as the ordinary test, and equal to the
+    output of the variant with half of the exponentials on the FMA pipe."""
     lengths = [700, 130, 64, 321]
     H, dh = 2, 64
     T = sum(lengths)
@@ -272,7 +272,7 @@ def test_navit_ln_modes_agree_with_golden(mode, monkeypatch):
     assert mx < 1.5e-2 and frac > 0.85
 
 
-@pytest.mark.parametrize("M", [300, 5000])           # small: GEMM + rmsnorm_heads; large: fused CTA-pair epilogue
+@pytest.mark.parametrize("M", [300, 5000])
 @pytest.mark.parametrize("fold", [False, True])
 def test_gemm_headnorm_matches_gemm_then_rmsnorm(M, fold):
     torch.manual_seed(8)

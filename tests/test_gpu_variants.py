@@ -1,4 +1,4 @@
-"""-m gpu: the SURVEY.md 8(f3) variants and attention without output projection through the fused sm_100a path, against
+"""-m gpu: the variants and attention without output projection through the fused sm_90a path, against
 the UNMODIFIED reference's fp32 logits (goldens) with the reference's own bf16 error as the pass criterion."""
 import importlib
 

@@ -1,13 +1,12 @@
-"""Host-side drop-in contract of the SURVEY.md 8(f3) SimpleViT-family variants and of attention without output
+"""Host-side drop-in contract of the SimpleViT-family variants and of attention without output
 projection: same state_dict layout, same fp32 values as the UNMODIFIED reference (goldens made by
 tests/golden/make_golden.py round2), same constructor keywords, bit-identical init under one seed.  CPU only."""
 import importlib
-import inspect
 
 import pytest
 import torch
 
-from conftest import import_reference, load_golden, reference_available
+from conftest import load_golden, reference_live, signature, state_digest
 
 VARIANTS = ["simplevit_registers", "simplevit_qknorm", "simplevit_patchdrop", "simplevit_flash",
             "simplevit_1d", "simplevit_3d", "simplevit_3d_pf1"]
@@ -47,26 +46,17 @@ def test_eager_forward_equals_reference_golden(g):
 
 @pytest.mark.parametrize("name", VARIANTS)
 def test_constructor_keywords_and_same_seed_init_equal_the_reference(name):
-    if not reference_available():
-        pytest.skip("reference checkout not present")
+    """Against the reference's constructor signature and same-seed state_dict digests (tests/golden/reference_live.pt)."""
     g = load_golden(name)
-    import_reference()
-    ref_cls = importlib.import_module("vit_pytorch." + g["kind"]).SimpleViT
+    live = reference_live()
     our_cls = dropin_class(g["kind"])
-    ps_ref = [p for p in inspect.signature(ref_cls.__init__).parameters if p != "self"]
-    ps_our = [p for p in inspect.signature(our_cls.__init__).parameters if p != "self"]
-    assert ps_ref == ps_our
-    for p in ps_ref:
-        assert inspect.signature(ref_cls.__init__).parameters[p].default == \
-            inspect.signature(our_cls.__init__).parameters[p].default, p
-    torch.manual_seed(123)
-    a = ref_cls(**g["kwargs"])
+    assert signature(our_cls) == live["signature"][name]
     torch.manual_seed(123)
     b = our_cls(**g["kwargs"])
-    sa, sb = a.state_dict(), b.state_dict()
-    assert list(sa.keys()) == list(sb.keys())
-    for k in sa:
-        assert torch.equal(sa[k], sb[k]), k
+    got, want = state_digest(b.state_dict()), live["init"][name]
+    assert list(got.keys()) == list(want.keys())
+    for k in want:
+        assert got[k] == want[k], k
 
 
 def test_patch_dropout_is_training_only():
@@ -105,7 +95,7 @@ def test_refresh_fused_weights_invalidates_prepared_copies():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# nested-tensor NaViT front-end (SURVEY.md 8(f2), reference na_vit_nested_tensor.py)
+# nested-tensor NaViT front-end, reference na_vit_nested_tensor.py)
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["navit_nested_tiny", "navit_nested_noqknorm"])
 def test_navit_nested_dropin_equals_reference_golden(name):
@@ -124,23 +114,13 @@ def test_navit_nested_dropin_equals_reference_golden(name):
 
 
 def test_navit_nested_same_seed_init_and_signature_equal_the_reference():
-    if not reference_available():
-        pytest.skip("reference checkout not present")
-    import_reference()
-    ref_cls = importlib.import_module("vit_pytorch.na_vit_nested_tensor").NaViT
     from vit_pytorch_b200.na_vit_nested_tensor import NaViT
-    pr = inspect.signature(ref_cls.__init__).parameters
-    po = inspect.signature(NaViT.__init__).parameters
-    assert list(pr) == list(po)
-    for k in pr:
-        if k != "self":
-            assert pr[k].default == po[k].default, k
+    live = reference_live()
+    assert signature(NaViT) == live["signature"]["navit_nested"]
     kw = dict(image_size=32, patch_size=8, num_classes=5, dim=64, depth=1, heads=1, mlp_dim=64)
     torch.manual_seed(5)
-    a = ref_cls(**kw)
-    torch.manual_seed(5)
     b = NaViT(**kw)
-    sa, sb = a.state_dict(), b.state_dict()
-    assert list(sa.keys()) == list(sb.keys())
-    for k in sa:
-        assert torch.equal(sa[k], sb[k]), k
+    got, want = state_digest(b.state_dict()), live["init"]["navit_nested"]
+    assert list(got.keys()) == list(want.keys())
+    for k in want:
+        assert got[k] == want[k], k

@@ -1,4 +1,4 @@
-"""vit_pytorch_b200: a Blackwell (sm_100a) native ViT encoder forward, drop-in for vit_pytorch.ViT / SimpleViT / NaViT.
+"""vit_pytorch_b200: a Hopper (sm_90a) native ViT encoder forward, drop-in for vit_pytorch.ViT / SimpleViT / NaViT.
 
     from vit_pytorch_b200 import ViT, SimpleViT      # same constructor keywords and state_dict as the reference
 

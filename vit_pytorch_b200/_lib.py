@@ -284,7 +284,7 @@ def gemm_headnorm(a: torch.Tensor, w: torch.Tensor, *, out_bf16: torch.Tensor, h
     if head_layernorm_eps is not None:
         flags |= EPI_HEADLN
         head_eps = float(head_layernorm_eps)
-    with _Timed("gemm", M=M, N=N, K=K, flags=flags | 32, flops=2.0 * M * N * K):
+    with _Timed("gemm", M=M, N=N, K=K, flags=flags, flops=2.0 * M * N * K):
         rc = lib().b200vit_gemm_headnorm_bf16(_ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out_bf16),
                                               out_bf16.stride(0), _ptr(bias), _ptr(ln_sums), ln_parts, float(ln_eps),
                                               _ptr(col_s), _ptr(head_gamma), norm_heads, dh, head_eps, M, N, K, flags,

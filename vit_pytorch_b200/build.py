@@ -1,9 +1,9 @@
-"""In-tree build of libb200vit.so (sm_100a only) with plain nvcc.
+"""In-tree build of libb200vit.so (sm_90a only) with plain nvcc.
 
     python -m vit_pytorch_b200.build            # build if sources are newer than the library
     python -m vit_pytorch_b200.build --force
 
-The library lands in vit_pytorch_b200/lib/libb200vit.so (git-ignored, travels to the GPU box with gpurun).
+The library lands in vit_pytorch_b200/lib/libb200vit.so (git-ignored build product).
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ OBJDIR = PKG / "lib" / "obj"
 LIB = LIBDIR / "libb200vit.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-std=c++17", "-O3", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -69,7 +69,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     srcs = sources()
     with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(lambda s: _compile(s, verbose), srcs))
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs)]
+    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs)]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,559 +1,298 @@
-// Multi-head softmax attention for short sequences (N <= 512 keys: one pass over the keys, no online rescale),
-// reading q/k/v tiles straight out of the packed [B*N, 3*H*dh] QKV buffer with TMA (no head-split copies) and
-// writing the merged-heads [B*N, H*dh] layout directly.  Replaces vit.py:55-63 / simple_vit.py:54-61:
-//     q,k,v = split heads;  dots = q k^T * scale;  attn = softmax(dots);  out = attn v;  merge heads
-//
-// Per work unit (image b, head h, round of NWG query tiles of 128 rows):
-//   TMA warp   : K[KP,64], V[KP,64], Q[128,64] x NWG  -> 128B-swizzled smem (3-D tensor map => rows >= N are zero)
-//   MMA thread : S_t = Q_t K^T           tcgen05.mma 128 x KP x 64      -> TMEM region t (fp32, KP columns)
-//   softmax WG : thread == query row (tcgen05.ld 32x32b): row max, p = exp2((s-max)*scale*log2e), row sum,
-//                P as packed bf16 back into TMEM (aliasing S, FA4 style)
-//   MMA thread : O_t = P_t V             tcgen05.mma 128 x 64 x KP, A from TMEM, B = V as MN-major smem operand
-//   softmax WG : O / rowsum -> bf16 -> out[b, row, h*64 : h*64+64]
-//
-// TMEM map of one region (512/NWG columns): S at [0,KP); P (packed bf16 pairs) at [0,KP/2); O at [REGION-64, REGION).
+// Multi-head softmax attention straight out of the packed QKV buffer, for sm_90a:
+//   b200vit_attention          B sequences of N tokens (N <= 512)
+//   b200vit_attention_varlen   packed sequences of any length (cu_seqlens), the block-diagonal attention of NaViT and
+//                              the long-sequence path of ViT
+// One CTA = one 128-row query tile of one (sequence, head): two warpgroups of 64 query rows each.  Thread 0 loads the
+// Q tile and the K / V blocks of KB keys with TMA into a two-stage ring of 128B-swizzled shared memory (mbarrier
+// complete_tx; a stage is reloaded once both warpgroups have released it).  Per key block each warpgroup computes
+// S = Q K^T with wgmma (both operands in shared memory), runs an online softmax in fp32 on the accumulator registers
+// and accumulates O += P V with wgmma, P (bf16) taken from registers as the A operand and V read as the transposed
+// (MN-major) B operand.  dh = 64, or 80: an 80-wide head is a 64-wide (128B swizzle) plus a 16-wide (32B swizzle)
+// slab.  Keys of a block beyond the sequence get probability 0; TMA zero-fills rows beyond the buffer.
 #include "common.cuh"
 #include "host_util.h"
 
 namespace b200 {
 
-constexpr int ATT_DH = 64;
+constexpr int ATT_QROWS = 128;
+constexpr int ATT_THREADS = 256;
 
 struct AttnParams {
-  int B, N, H;
-  int KP;         // keys padded to a multiple of 16
-  int kv_boxes;   // number of TMA boxes per K (and per V)
-  int kv_box_rows;
-  int rounds;     // query-tile rounds per (b, h)
-  int units;      // B * H * rounds
-  int I;          // H * dh
-  float scale_log2e;
   __nv_bfloat16* out;
-  unsigned v_lbo, v_sbo;  // V (MN-major) descriptor strides, bytes
-  unsigned v16_lbo, v16_sbo;  // dim_head 80: descriptor strides of the 16-wide V slab (32-byte swizzle)
-  int ktail;      // keys [N - ktail, N) are NOT in the S tile: their scores and P V terms run on the CUDA cores (<= 4)
+  int N;                      // fixed-length mode: tokens per sequence (grid.z = sequence)
+  const int32_t* cu_seqlens;  // varlen mode: [num_seqs + 1] token offsets, tile_prefix: 128-row tiles before s
+  const int32_t* tile_prefix;
+  int num_seqs;
+  int H, I;                   // heads, H * dh
+  float scale_log2e;
 };
 
-__host__ __device__ inline int att_kv_bytes(int kv_boxes, int kv_box_rows) { return kv_boxes * kv_box_rows * 128; }
+template <int DH, int KB>
+struct AttnSmem {
+  static constexpr bool WIDE = DH == 80;
+  static constexpr int Q64 = ATT_QROWS * 128;        // 64 columns, 128B swizzle
+  static constexpr int Q16 = WIDE ? ATT_QROWS * 32 : 0;  // columns 64..79, 32B swizzle
+  static constexpr int KV64 = KB * 128;
+  static constexpr int KV16 = WIDE ? KB * 32 : 0;
+  static constexpr int STAGE = 2 * (KV64 + KV16);   // K64 | V64 | K16 | V16
+  static constexpr int STAGE_OFF = Q64 + Q16;
+  static constexpr int BAR_OFF = STAGE_OFF + 2 * STAGE;
+  static constexpr int BYTES = BAR_OFF + 5 * 8 + 1024;  // full[2], empty[2], q; slack for 1024B alignment
+};
 
-// TMEM_COLS = 512: one CTA per SM (NWG regions of 512/NWG columns).  TMEM_COLS = 256 (NWG = 1, one K/V/Q stage):
-// TWO independent CTAs per SM, each with one softmax warpgroup -- while one CTA waits for its MMAs or loads, the
-// other one's softmax keeps the MUFU / issue slots busy.
-// (The round-1 experiments -- FMA-pipe exp2, split PV accumulation, skipped row max, 8 warps per tile, globaltimer
-// traces -- are recorded in profiles/r01*; their code is gone.  attention_pipe.cu, a software-pipelined variant for
-// N <= 224, is reachable through the test hook only: it measured 6 % slower, profiles/r02_attention.md.)
-//
-// DH = 64 or 80 (canonical ViT-H/14, reference vit.py:86 `dim_head`).  128-byte swizzled TMA boxes are 64 bf16 wide, so
-// an 80-wide head is staged as a 64-wide slab plus a 16-wide slab (32-byte rows, 32-byte swizzle): Q K^T gets a
-// fifth k-step from the 16-wide slabs, P V a second MMA per key step with N = 16 into O columns [64, 80).
-// KTAIL: the last p.ktail (1..4) keys are not in the S tile -- N = 257 keeps a 256-column tile (two CTAs per SM, 256
-// TMEM columns each) and the softmax threads add the 257th key's score and P V term themselves from shared memory.
-template <int NWG, int STAGES, int TMEM_COLS, int DH, bool KTAIL = false>
-__global__ void __launch_bounds__((4 * NWG + 2) * 32, TMEM_COLS == 256 ? 2 : 1)
+template <int DH, int KB, bool VARLEN, bool EMUL>
+__global__ void __launch_bounds__(ATT_THREADS, (DH == 64 && KB == 64) ? 2 : 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                  const __grid_constant__ CUtensorMap tmQ16, const __grid_constant__ CUtensorMap tmKV16,
                  const AttnParams p) {
-  static_assert(DH == 64 || DH == 80, "dim_head 64 or 80");
-  constexpr bool X16 = DH == 80;  // the extra 16-wide slabs exist
-  constexpr int REGION = TMEM_COLS / NWG;
-  constexpr int O_COL = REGION - DH;
-  constexpr int NUM_SOFTMAX_WARPS = 4 * NWG;
-  constexpr int Q_TILE_BYTES = 128 * 128 + (X16 ? 128 * 32 : 0);  // [128 x 64] slab, then [128 x 16] slab
-
+  using L = AttnSmem<DH, KB>;
+  constexpr bool WIDE = L::WIDE;
+  constexpr int NS = KB / 2;  // score accumulators per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int kv64_bytes = att_kv_bytes(p.kv_boxes, p.kv_box_rows);  // multiple of 1024
-  const int kv16_bytes = X16 ? p.kv_boxes * p.kv_box_rows * 32 : 0;   // multiple of 256 (8-row atoms of 32 bytes)
-  const int kv_bytes = kv64_bytes + (X16 ? (kv16_bytes + 1023) / 1024 * 1024 : 0);  // K (or V): 64-slab, 16-slab
-  const int stage_bytes = 2 * kv_bytes + NWG * Q_TILE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* s_full = empty_bar + STAGES;
-  uint64_t* p_ready = s_full + NWG;
-  uint64_t* o_full = p_ready + NWG;
-  uint64_t* o_free = o_full + NWG;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(o_free + NWG);
-  uint8_t* vtail_base = reinterpret_cast<uint8_t*>(bars) + 256;   // KTAIL: 2 x [4][DH] bf16, V rows of the tail keys (host adds 2 KB)
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
+  uint64_t* empty = full + 2;
+  uint64_t* qbar = full + 4;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  constexpr int TMA_WARP = NUM_SOFTMAX_WARPS;
-  constexpr int MMA_WARP = NUM_SOFTMAX_WARPS + 1;
+  const int h = blockIdx.y;
+  int seq_start, len, q0;
+  if (VARLEN) {
+    const int tile = blockIdx.x;
+    int lo = 0, hi = p.num_seqs - 1;  // last s with tile_prefix[s] <= tile
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (p.tile_prefix[mid] <= tile) lo = mid;
+      else hi = mid - 1;
+    }
+    seq_start = p.cu_seqlens[lo];
+    len = p.cu_seqlens[lo + 1] - seq_start;
+    q0 = (tile - p.tile_prefix[lo]) * ATT_QROWS;
+  } else {
+    seq_start = blockIdx.z * p.N;
+    len = p.N;
+    q0 = blockIdx.x * ATT_QROWS;
+  }
+  const int nblocks = (len + KB - 1) / KB;
+  const int colq = h * DH, colk = p.I + h * DH, colv = 2 * p.I + h * DH;
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, t = tid & 127, warp = t >> 5, lane = t & 31;
 
-  if (warp == TMA_WARP && lane == 0) {
+  auto issue_kv = [&](int blk) {
+    const int st = blk & 1;
+    uint8_t* sb = smem + L::STAGE_OFF + st * L::STAGE;
+    const int row = seq_start + blk * KB;
+    mbar_arrive_expect_tx(&full[st], L::STAGE);
+    tma_load_2d(sb, &tmKV, &full[st], colk, row);
+    tma_load_2d(sb + L::KV64, &tmKV, &full[st], colv, row);
+    if (WIDE) {
+      tma_load_2d(sb + 2 * L::KV64, &tmKV16, &full[st], colk + 64, row);
+      tma_load_2d(sb + 2 * L::KV64 + L::KV16, &tmKV16, &full[st], colv + 64, row);
+    }
+  };
+
+  if (tid == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmKV);
-    if (X16) {
-      tma_prefetch_desc(&tmQ16);
-      tma_prefetch_desc(&tmKV16);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 2);  // one arrive per warpgroup
     }
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int t = 0; t < NWG; ++t) {
-      mbar_init(&s_full[t], 1);
-      mbar_init(&p_ready[t], 4);
-      mbar_init(&o_full[t], 1);
-      mbar_init(&o_free[t], 4);
-    }
+    mbar_init(qbar, 1);
     fence_mbar_init();
   }
-  if (warp == MMA_WARP) {
-    tmem_alloc(tmem_base_smem, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
+  if (tid == 0) {
+    mbar_arrive_expect_tx(qbar, L::Q64 + L::Q16);
+    tma_load_2d(smem, &tmQ, qbar, colq, seq_start + q0);
+    if (WIDE) tma_load_2d(smem + L::Q64, &tmQ16, qbar, colq + 64, seq_start + q0);
+    issue_kv(0);
+    if (nblocks > 1) issue_kv(1);
+  }
 
-  if (warp == TMA_WARP) {
-    // ---------------------------------------------------------------- producer
-    if (lane == 0) {
-      int it = 0;
-      for (int u = blockIdx.x; u < p.units; u += gridDim.x, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        const int round = u % p.rounds;
-        const int bh = u / p.rounds;
-        const int h = bh % p.H, b = bh / p.H;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        uint8_t* sk = smem + s * stage_bytes;
-        uint8_t* sv = sk + kv_bytes;
-        uint8_t* sq = sv + kv_bytes;
-        // bytes that will land: the TMA boxes, not the (1024-aligned) slab sizes
-        mbar_arrive_expect_tx(&full_bar[s], 2 * (kv64_bytes + kv16_bytes) + NWG * Q_TILE_BYTES);
-        for (int i = 0; i < p.kv_boxes; ++i) {
-          tma_load_3d(sk + i * p.kv_box_rows * 128, &tmKV, &full_bar[s], p.I + h * DH, i * p.kv_box_rows, b);
-          tma_load_3d(sv + i * p.kv_box_rows * 128, &tmKV, &full_bar[s], 2 * p.I + h * DH, i * p.kv_box_rows, b);
-          if (X16) {
-            tma_load_3d(sk + kv64_bytes + i * p.kv_box_rows * 32, &tmKV16, &full_bar[s], p.I + h * DH + 64,
-                        i * p.kv_box_rows, b);
-            tma_load_3d(sv + kv64_bytes + i * p.kv_box_rows * 32, &tmKV16, &full_bar[s], 2 * p.I + h * DH + 64,
-                        i * p.kv_box_rows, b);
-          }
+  float o[32], o16[8];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) o16[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const uint32_t qa = smem_u32(smem) + wg * 64 * 128;
+  const uint32_t qa16 = smem_u32(smem + L::Q64) + wg * 64 * 32;
+  mbar_wait(qbar, 0);
+
+  for (int kb = 0; kb < nblocks; ++kb) {
+    const int st = kb & 1;
+    const uint32_t ph = (kb >> 1) & 1;
+    mbar_wait(&full[st], ph);
+    const uint32_t sb = smem_u32(smem + L::STAGE_OFF + st * L::STAGE);
+
+    // S = Q K^T (64 rows x KB keys per warpgroup)
+    float s[NS];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t ad = make_wgmma_desc(qa, 1024, WGMMA_SW128) + 2 * k;
+      const uint64_t bd = make_wgmma_desc(sb, 1024, WGMMA_SW128) + 2 * k;
+      if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, k != 0);
+      else wgmma_m64n64k16(s, ad, bd, k != 0);
+    }
+    if constexpr (WIDE) {
+      const uint64_t ad = make_wgmma_desc(qa16, 256, WGMMA_SW32);
+      const uint64_t bd = make_wgmma_desc(sb + 2 * L::KV64, 256, WGMMA_SW32);
+      if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, 1);
+      else wgmma_m64n64k16(s, ad, bd, 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+
+    // online softmax (log2 units); s[4j + e]: row 16 warp + lane/4 + 8 (e >> 1), key 8 j + 2 (lane % 4) + (e & 1)
+    const int key0 = kb * KB + 2 * (lane & 3);
+    float mx[2] = {m[0], m[1]};
+#pragma unroll
+    for (int j = 0; j < KB / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const bool valid = key0 + j * 8 + (e & 1) < len;
+        s[4 * j + e] = valid ? s[4 * j + e] * p.scale_log2e : -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * j + e]);
+      }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float corr = fast_ex2(m[r] - mx[r]);  // m = -inf on the first block: exp2(-inf) = 0
+      l[r] *= corr;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        o[4 * i + 2 * r] *= corr;
+        o[4 * i + 2 * r + 1] *= corr;
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        o16[4 * i + 2 * r] *= corr;
+        o16[4 * i + 2 * r + 1] *= corr;
+      }
+      m[r] = mx[r];
+    }
+#pragma unroll
+    for (int j = 0; j < KB / 8; ++j) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float e0, e1;
+        const float x0 = s[4 * j + 2 * r] - m[r], x1 = s[4 * j + 2 * r + 1] - m[r];
+        if (EMUL && (j & 1)) {
+          // half of the exponentials on the FMA pipe (masked keys are -inf: forced to 0)
+          exp2_emul2(f2_make(x0, x1), e0, e1);
+          e0 = s[4 * j + 2 * r] == -INFINITY ? 0.f : e0;
+          e1 = s[4 * j + 2 * r + 1] == -INFINITY ? 0.f : e1;
+        } else {
+          e0 = fast_ex2(x0);
+          e1 = fast_ex2(x1);
         }
-        for (int t = 0; t < NWG; ++t) {
-          const int qt = round * NWG + t;  // may be >= q_tiles: box fully out of bounds -> zeros
-          tma_load_3d(sq + t * Q_TILE_BYTES, &tmQ, &full_bar[s], h * DH, qt * 128, b);
-          if (X16) tma_load_3d(sq + t * Q_TILE_BYTES + 128 * 128, &tmQ16, &full_bar[s], h * DH + 64, qt * 128, b);
-        }
+        s[4 * j + 2 * r] = e0;
+        s[4 * j + 2 * r + 1] = e1;
+        l[r] += e0 + e1;
       }
     }
-  } else if (warp == MMA_WARP) {
-    // ---------------------------------------------------------------- MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc_pv = make_idesc_bf16(128, 64, 0, 1);    // B = V is MN-major
-      const uint32_t idesc_pv16 = make_idesc_bf16(128, 16, 0, 1);  // dim_head 80: the 16-wide V slab
-      // S_t(it) = Q_t K^T into region t  (waits until the epilogue of unit it-1 has drained the region)
-      auto issue_s = [&](int it, int t) {
-        const int s = it % STAGES;
-        const uint32_t sk = smem_u32(smem + s * stage_bytes);
-        const uint32_t sq = sk + 2 * kv_bytes;
-        mbar_wait(&o_free[t], (it & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_s = tmem_base + t * REGION;
-        for (int n0 = 0; n0 < p.KP; n0 += 256) {
-          const int nn = (p.KP - n0) < 256 ? (p.KP - n0) : 256;
-          const uint32_t idesc_s = make_idesc_bf16(128, nn, 0, 0);
-          const uint64_t adesc = make_smem_desc_sw128(sq + t * Q_TILE_BYTES, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(sk + n0 * 128, 16, 1024);
+
+    // O += P V: the score accumulators of 16 keys are the A fragment of one k-step (bf16)
+    wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_ss(d_s + n0, adesc + 2 * k, bdesc + 2 * k, idesc_s, k != 0);
-          if (X16) {
-            // fifth k-step (dims 64..79): K-major slabs with 32-byte rows, 32-byte swizzle, 8-row atoms of 256 bytes
-            const uint64_t a16 = make_smem_desc(sq + t * Q_TILE_BYTES + 128 * 128, 16, 256, 6);
-            const uint64_t b16 = make_smem_desc(sk + kv64_bytes + n0 * 32, 16, 256, 6);
-            umma_ss(d_s + n0, a16, b16, idesc_s, 1);
-          }
-        }
-        umma_commit(&s_full[t]);
-      };
-      // O_t(it) = P_t V  (A = P from TMEM, B = V as MN-major smem operand: 16 keys = two 8-row groups = 2048 B)
-      auto issue_pv = [&](int it, int t) {
-        const int s = it % STAGES;
-        const uint32_t sv = smem_u32(smem + s * stage_bytes) + kv_bytes;
-        mbar_wait(&p_ready[t], it & 1);
-        tc_fence_after();
-        const uint32_t d_o = tmem_base + t * REGION + O_COL;
-        const int ksteps = p.KP / 16;
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t vdesc = make_smem_desc_sw128(sv + k * 2048, p.v_lbo, p.v_sbo);
-          umma_ts(d_o, tmem_base + t * REGION + k * 8, vdesc, idesc_pv, k != 0);
-          if (X16) {  // O[:, 64:80] += P_k V_k[:, 64:80]: 16 keys = two 8-row atoms of 256 bytes
-            const uint64_t v16 = make_smem_desc(sv + kv64_bytes + k * 512, p.v16_lbo, p.v16_sbo, 6);
-            umma_ts(d_o + 64, tmem_base + t * REGION + k * 8, v16, idesc_pv16, k != 0);
-          }
-        }
-        umma_commit(&o_full[t]);
-      };
-      auto wait_full = [&](int it) {
-        mbar_wait(&full_bar[it % STAGES], (it / STAGES) & 1);
-        tc_fence_after();
-      };
-      const int n_units = blockIdx.x < p.units ? (p.units - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-      if (NWG == 2 && STAGES == 2) {
-        // Skewed schedule: the two warpgroups run half a unit out of phase, so that one of them is in its softmax
-        // while the other waits for its PV / next S MMAs:
-        //     S0(0) | S1(i)  PV0(i)  S0(i+1)  PV1(i) | ...
-        if (n_units > 0) {
-          wait_full(0);
-          issue_s(0, 0);
-        }
-        for (int it = 0; it < n_units; ++it) {
-          issue_s(it, 1);
-          issue_pv(it, 0);
-          if (it + 1 < n_units) {
-            wait_full(it + 1);
-            issue_s(it + 1, 0);
-          }
-          issue_pv(it, 1);
-          umma_commit(&empty_bar[it % STAGES]);  // every MMA reading this K/V/Q stage has been issued before
-        }
-      } else {
-        for (int it = 0; it < n_units; ++it) {
-          wait_full(it);
-          for (int t = 0; t < NWG; ++t) issue_s(it, t);
-          for (int t = 0; t < NWG; ++t) issue_pv(it, t);
-          umma_commit(&empty_bar[it % STAGES]);
-        }
-      }
+    for (int kk = 0; kk < KB / 16; ++kk) {
+      const uint32_t a[4] = {pack_bf16x2(s[8 * kk], s[8 * kk + 1]), pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]),
+                             pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7])};
+      wgmma_m64n64k16_rs_tb(o, a, make_wgmma_desc_lbo(sb + L::KV64 + kk * 2048, 1024, 1024, WGMMA_SW128));
+      if constexpr (WIDE)
+        wgmma_m64n16k16_rs_tb(o16, a, make_wgmma_desc_lbo(sb + 2 * L::KV64 + L::KV16 + kk * 512, 256, 256, WGMMA_SW32));
     }
-  } else {
-    // ---------------------------------------------------------------- softmax / epilogue warpgroups
-    const int t = warp >> 2;
-    const int quad = warp & 3;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + t * REGION;
-    const int r_in_tile = quad * 32 + lane;
-    const float c = p.scale_log2e;
-    int it = 0;
-    for (int u = blockIdx.x; u < p.units; u += gridDim.x, ++it) {
-      const uint32_t up = it & 1;
-      const int round = u % p.rounds;
-      const int bh = u / p.rounds;
-      const int h = bh % p.H, b = bh / p.H;
-      const int qrow = (round * NWG + t) * 128 + r_in_tile;
-
-      // warps whose 32 query rows all lie beyond N skip the arithmetic but keep the barrier protocol in lockstep
-      const bool warp_active = (round * NWG + t) * 128 + quad * 32 < p.N;
-
-      mbar_wait(&s_full[t], up);
-      tc_fence_after();
-      const uint8_t* stage = smem + (it % STAGES) * stage_bytes;
-      uint8_t* vtail = vtail_base + (it & 1) * (4 * DH * 2);
-      if constexpr (KTAIL) {
-        // the tail keys' V rows leave the stage before P V is released (after it the producer refills the stage):
-        // un-swizzled copy into a scratch area every softmax thread reads in the epilogue.  All four warps pass here
-        // (also the ones without valid rows).  Two scratch areas alternate, so the readers of unit it - 2 and this
-        // write are separated by the bar.sync of unit it - 1 (they are ordered through o_free -> S MMA -> s_full as
-        // well, but that chain is invisible to racecheck).
-        mbar_wait(&full_bar[it % STAGES], (it / STAGES) & 1);     // TMA bytes visible to THIS thread
-        if (quad == 0) {
-          const int nk0 = p.N - p.ktail;
-          for (int idx = lane; idx < p.ktail * (DH / 8); idx += 32) {
-            const int tt = idx / (DH / 8), ch = idx % (DH / 8);
-            const int kr = nk0 + tt;
-            const uint8_t* src = ch < 8 ? stage + kv_bytes + kr * 128 + ((ch ^ (kr & 7)) << 4)
-                                        : stage + kv_bytes + kv64_bytes + kr * 32 + (((ch - 8) ^ ((kr >> 2) & 1)) << 4);
-            *reinterpret_cast<uint4*>(vtail + tt * (DH * 2) + ch * 16) = *reinterpret_cast<const uint4*>(src);
-          }
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-      float sum = 1.f;
-      float pt[4] = {0.f, 0.f, 0.f, 0.f};   // KTAIL: softmax numerators of the tail keys (P V term added in the epilogue)
-      if (warp_active) {
-        // Columns [0, 32*nfull) need no key mask; the rest (< 48 columns) is handled 16 at a time with the mask.
-        const int nk = KTAIL ? p.N - p.ktail : p.N;   // keys in the S tile
-        const int nfull = nk >> 5;
-        uint32_t ra[32], rb[32];
-        // ---------------- key tail (N = 257: the S tile keeps 256 columns, so that two CTAs share an SM): scores of
-        // the last ktail keys from the Q / K rows in shared memory (swizzled as TMA wrote them), fp32
-        float st[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-        if constexpr (KTAIL) {
-          const uint8_t* qrow64 = stage + 2 * kv_bytes + t * Q_TILE_BYTES + r_in_tile * 128;
-          uint4 qv[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) qv[j] = *reinterpret_cast<const uint4*>(qrow64 + ((j ^ (r_in_tile & 7)) << 4));
-          uint4 qx[2];
-          if constexpr (X16) {
-            const uint8_t* qrow16 = stage + 2 * kv_bytes + t * Q_TILE_BYTES + 128 * 128 + r_in_tile * 32;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) qx[j] = *reinterpret_cast<const uint4*>(qrow16 + ((j ^ ((r_in_tile >> 2) & 1)) << 4));
-          }
-          auto dot8 = [](const uint4& a, const uint4& b, float acc) {
-            const __nv_bfloat162* x = reinterpret_cast<const __nv_bfloat162*>(&a);
-            const __nv_bfloat162* y = reinterpret_cast<const __nv_bfloat162*>(&b);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 fx = __bfloat1622float2(x[i]), fy = __bfloat1622float2(y[i]);
-              acc = fmaf(fx.x, fy.x, acc);
-              acc = fmaf(fx.y, fy.y, acc);
-            }
-            return acc;
-          };
-#pragma unroll
-          for (int tt = 0; tt < 4; ++tt) {
-            if (tt < p.ktail) {
-              const int kr = nk + tt;
-              const uint8_t* krow = stage + kr * 128;
-              float acc = 0.f;
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                acc = dot8(qv[j], *reinterpret_cast<const uint4*>(krow + ((j ^ (kr & 7)) << 4)), acc);
-              if constexpr (X16) {
-                const uint8_t* krow16 = stage + kv64_bytes + kr * 32;
-#pragma unroll
-                for (int j = 0; j < 2; ++j)
-                  acc = dot8(qx[j], *reinterpret_cast<const uint4*>(krow16 + ((j ^ ((kr >> 2) & 1)) << 4)), acc);
-              }
-              st[tt] = acc;
-            }
-          }
-        }
-        // ---------------- pass 1: row max (4 independent chains; next chunk's tcgen05.ld in flight)
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#define ATT_MAX32(R)                                                    \
-  _Pragma("unroll") for (int j = 0; j < 32; j += 4) {                   \
-    m0 = fmaxf(m0, __uint_as_float(R[j]));                              \
-    m1 = fmaxf(m1, __uint_as_float(R[j + 1]));                          \
-    m2 = fmaxf(m2, __uint_as_float(R[j + 2]));                          \
-    m3 = fmaxf(m3, __uint_as_float(R[j + 3]));                          \
-  }
-        int ci = 0;
-        if (nfull > 0) tmem_ld_32x32b_x32(t_lane, ra);
-        for (; ci + 1 < nfull; ci += 2) {
-          tmem_ld_wait();
-          tmem_ld_32x32b_x32(t_lane + (ci + 1) * 32, rb);
-          ATT_MAX32(ra)
-          tmem_ld_wait();
-          if (ci + 2 < nfull) tmem_ld_32x32b_x32(t_lane + (ci + 2) * 32, ra);
-          ATT_MAX32(rb)
-        }
-        if (ci < nfull) {
-          tmem_ld_wait();
-          ATT_MAX32(ra)
-        }
-        for (int c0 = nfull * 32; c0 < p.KP; c0 += 16) {
-          uint32_t r16[16];
-          tmem_ld_32x32b_x16(t_lane + c0, r16);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (c0 + j < nk) m0 = fmaxf(m0, __uint_as_float(r16[j]));
-        }
-        if constexpr (KTAIL) {
-          m0 = fmaxf(fmaxf(m0, st[0]), st[1]);
-          m1 = fmaxf(fmaxf(m1, st[2]), st[3]);
-        }
-        const float mc = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)) * c;
-        // ---------------- pass 2: p = exp2(s*c - max*c), row sum, P (bf16 pairs) -> TMEM over S
-        float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#define ATT_EXP32_PLAIN(R, C0)                                                                \
-  {                                                                                           \
-    uint32_t pk[16];                                                                          \
-    _Pragma("unroll") for (int j = 0; j < 32; j += 4) {                                       \
-      const float e0 = fast_ex2(fmaf(__uint_as_float(R[j]), c, -mc));                         \
-      const float e1 = fast_ex2(fmaf(__uint_as_float(R[j + 1]), c, -mc));                     \
-      const float e2 = fast_ex2(fmaf(__uint_as_float(R[j + 2]), c, -mc));                     \
-      const float e3 = fast_ex2(fmaf(__uint_as_float(R[j + 3]), c, -mc));                     \
-      s0 += e0; s1 += e1; s2 += e2; s3 += e3;                                                 \
-      pk[j >> 1] = pack_bf16x2(e0, e1);                                                       \
-      pk[(j >> 1) + 1] = pack_bf16x2(e2, e3);                                                 \
-    }                                                                                         \
-    tmem_st_32x32b_x16(t_lane + ((C0) >> 1), pk);                                             \
-  }
-#define ATT_EXP32(R, C0) ATT_EXP32_PLAIN(R, C0)
-        ci = 0;
-        if (nfull > 0) tmem_ld_32x32b_x32(t_lane, ra);
-        for (; ci + 1 < nfull; ci += 2) {
-          tmem_ld_wait();
-          tmem_ld_32x32b_x32(t_lane + (ci + 1) * 32, rb);
-          ATT_EXP32(ra, ci * 32)
-          tmem_ld_wait();
-          if (ci + 2 < nfull) tmem_ld_32x32b_x32(t_lane + (ci + 2) * 32, ra);
-          ATT_EXP32(rb, (ci + 1) * 32)
-        }
-        if (ci < nfull) {
-          tmem_ld_wait();
-          ATT_EXP32(ra, ci * 32)
-        }
-        for (int c0 = nfull * 32; c0 < p.KP; c0 += 16) {
-          uint32_t r16[16];
-          tmem_ld_32x32b_x16(t_lane + c0, r16);
-          tmem_ld_wait();
-          uint32_t pk8[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const float e0 = (c0 + j < nk) ? fast_ex2(fmaf(__uint_as_float(r16[j]), c, -mc)) : 0.f;
-            const float e1 = (c0 + j + 1 < nk) ? fast_ex2(fmaf(__uint_as_float(r16[j + 1]), c, -mc)) : 0.f;
-            s0 += e0;
-            s1 += e1;
-            pk8[j >> 1] = pack_bf16x2(e0, e1);
-          }
-          tmem_st_32x32b_x8(t_lane + (c0 >> 1), pk8);
-        }
-#undef ATT_MAX32
-#undef ATT_EXP32
-#undef ATT_EXP32_PLAIN
-        sum = (s0 + s1) + (s2 + s3);
-        if constexpr (KTAIL) {
-#pragma unroll
-          for (int tt = 0; tt < 4; ++tt) {
-            if (tt < p.ktail) {
-              pt[tt] = fast_ex2(fmaf(st[tt], c, -mc));
-              sum += pt[tt];
-            }
-          }
-        }
-        tmem_st_wait();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_ready[t]);
-
-      // epilogue: O / sum -> bf16 -> global
-      const float inv = 1.0f / sum;
-      mbar_wait(&o_full[t], up);
-      tc_fence_after();
-      uint32_t ob[DH / 2];  // DH output columns as packed bf16 pairs
-      if (warp_active) {
-        if constexpr (!X16) {
-          uint32_t r0[32];
-#pragma unroll
-          for (int hcol = 0; hcol < 2; ++hcol) {
-            tmem_ld_32x32b_x32(t_lane + O_COL + 32 * hcol, r0);
-            tmem_ld_wait();
-            if constexpr (KTAIL) {
-#pragma unroll
-              for (int tt = 0; tt < 4; ++tt) {
-                if (tt >= p.ktail) break;
-#pragma unroll
-                for (int q4 = 0; q4 < 4; ++q4) {   // 8 columns per 16-byte broadcast read
-                  const uint4 raw = *reinterpret_cast<const uint4*>(vtail + tt * (DH * 2) + hcol * 64 + q4 * 16);
-                  const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&raw);
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    const float2 f = __bfloat1622float2(h2[i]);
-                    r0[8 * q4 + 2 * i] = __float_as_uint(fmaf(pt[tt], f.x, __uint_as_float(r0[8 * q4 + 2 * i])));
-                    r0[8 * q4 + 2 * i + 1] = __float_as_uint(fmaf(pt[tt], f.y, __uint_as_float(r0[8 * q4 + 2 * i + 1])));
-                  }
-                }
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              ob[16 * hcol + j] = pack_bf16x2(__uint_as_float(r0[2 * j]) * inv, __uint_as_float(r0[2 * j + 1]) * inv);
-          }
-        } else {  // 80 columns: five 16-column groups (O_COL is a multiple of 16, not of 32)
-          uint32_t r0[16];
-#pragma unroll
-          for (int g = 0; g < DH / 16; ++g) {
-            tmem_ld_32x32b_x16(t_lane + O_COL + 16 * g, r0);
-            tmem_ld_wait();
-            if constexpr (KTAIL) {
-#pragma unroll
-              for (int tt = 0; tt < 4; ++tt) {
-                if (tt >= p.ktail) break;
-#pragma unroll
-                for (int q4 = 0; q4 < 2; ++q4) {
-                  const uint4 raw = *reinterpret_cast<const uint4*>(vtail + tt * (DH * 2) + g * 32 + q4 * 16);
-                  const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&raw);
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    const float2 f = __bfloat1622float2(h2[i]);
-                    r0[8 * q4 + 2 * i] = __float_as_uint(fmaf(pt[tt], f.x, __uint_as_float(r0[8 * q4 + 2 * i])));
-                    r0[8 * q4 + 2 * i + 1] = __float_as_uint(fmaf(pt[tt], f.y, __uint_as_float(r0[8 * q4 + 2 * i + 1])));
-                  }
-                }
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              ob[8 * g + j] = pack_bf16x2(__uint_as_float(r0[2 * j]) * inv, __uint_as_float(r0[2 * j + 1]) * inv);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&o_free[t]);
-      if (warp_active && qrow < p.N) {
-        uint4* op = reinterpret_cast<uint4*>(p.out + ((size_t)b * p.N + qrow) * p.I + h * DH);
-#pragma unroll
-        for (int j = 0; j < DH / 8; ++j) op[j] = make_uint4(ob[4 * j], ob[4 * j + 1], ob[4 * j + 2], ob[4 * j + 3]);
-      }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    fence_regs(o16);
+    if (t == 0) mbar_arrive(&empty[st]);
+    if (tid == 0 && kb + 2 < nblocks) {
+      mbar_wait(&empty[st], ph);  // both warpgroups are done with this stage
+      issue_kv(kb + 2);
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    l[r] = 1.0f / l[r];
+  }
+  const int qr = q0 + wg * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = qr + 8 * r;
+    if (row >= len) continue;
+    __nv_bfloat16* op = p.out + (long long)(seq_start + row) * p.I + h * DH + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<uint32_t*>(op + j * 8) = pack_bf16x2(o[4 * j + 2 * r] * l[r], o[4 * j + 2 * r + 1] * l[r]);
+    if constexpr (WIDE) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        *reinterpret_cast<uint32_t*>(op + 64 + j * 8) =
+            pack_bf16x2(o16[4 * j + 2 * r] * l[r], o16[4 * j + 2 * r + 1] * l[r]);
+    }
   }
 }
 
-
-// test hooks (b200vit_debug_set): process-global, NOT part of the re-entrant API
-// 0 auto, 1 force the kernels below, 2 force the pipelined kernel (attention_pipe.cu) wherever N <= 224.  Auto is
-// currently the kernels below: at ViT-B/16 batch 512 they need 221 us per layer, the pipelined one 235 us
-// (profiles/r02_attention.md has the timelines and the reasons).
-static std::atomic<int> g_attn_mode{0};
-static std::atomic<int> g_attn_v_lbo{1024};  // V descriptor leading-dim byte offset (bring-up probe)
-static std::atomic<int> g_attn_v_sbo{1024};  // V descriptor stride-dim byte offset
-static std::atomic<int> g_attn_v16_lbo{256};  // dim_head 80: the same two for the 16-wide V slab (bring-up probe)
-static std::atomic<int> g_attn_v16_sbo{256};
-static std::atomic<int> g_attn_tail{1};       // 1: key tail (N = 257..260) on the CUDA cores; 0: 272-column tiles
-
-bool attention_pipe_eligible(int N, int dh);
-int launch_attention_pipe(const void* qkv, void* out, int B, int N, int H, float scale, unsigned v_lbo, unsigned v_sbo,
-                          cudaStream_t stream);
-
-template <int NWG, int STAGES, int TMEM_COLS, int DH, bool KTAIL = false>
-static int launch_attention_t(const CUtensorMap* tm, const AttnParams& p, size_t smem_bytes, cudaStream_t stream) {
-  auto kern = attention_kernel<NWG, STAGES, TMEM_COLS, DH, KTAIL>;
-  B200_ENSURE_SMEM(kern, smem_bytes);
-  const int slots = num_sms() * (TMEM_COLS == 256 ? 2 : 1);
-  const int grid = p.units < slots ? p.units : slots;
-  kern<<<grid, (4 * NWG + 2) * 32, smem_bytes, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
+// Tensor maps over qkv[T, 3 I]: 64-column boxes (128B swizzle) of 128 query rows / KB key rows, and -- dh 80 -- the
+// same with 16 columns (32B swizzle).
+template <int DH, int KB, bool VARLEN, bool EMUL>
+static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 grid, cudaStream_t stream) {
+  using L = AttnSmem<DH, KB>;
+  CUtensorMap tm[4];
+  const uint64_t dims[2] = {(uint64_t)3 * p.I, (uint64_t)T};
+  const uint64_t strides[1] = {(uint64_t)3 * p.I * 2};
+  const uint32_t qbox[2] = {64, ATT_QROWS}, kvbox[2] = {64, KB}, qbox16[2] = {16, ATT_QROWS}, kvbox16[2] = {16, KB};
+  int rc = encode_tmap_bf16(&tm[0], qkv, 2, dims, strides, qbox);
+  if (!rc) rc = encode_tmap_bf16(&tm[1], qkv, 2, dims, strides, kvbox);
+  if (!rc && DH == 80) rc = encode_tmap_bf16_sw(&tm[2], qkv, 2, dims, strides, qbox16, 32);
+  if (!rc && DH == 80) rc = encode_tmap_bf16_sw(&tm[3], qkv, 2, dims, strides, kvbox16, 32);
+  if (rc) return rc;
+  if (DH != 80) tm[2] = tm[0], tm[3] = tm[1];
+  auto kern = attention_kernel<DH, KB, VARLEN, EMUL>;
+  B200_ENSURE_SMEM(kern, L::BYTES);
+  kern<<<grid, ATT_THREADS, L::BYTES, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
 }
-template <int NWG, int STAGES, int TMEM_COLS = 512>
-static int launch_attention(const CUtensorMap* tm, int dh, const AttnParams& p, size_t smem_bytes,
-                            cudaStream_t stream) {
-  if (dh == 80) return launch_attention_t<NWG, STAGES, TMEM_COLS, 80>(tm, p, smem_bytes, stream);
-  return launch_attention_t<NWG, STAGES, TMEM_COLS, 64>(tm, p, smem_bytes, stream);
+
+template <bool VARLEN>
+static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, int kb, bool emul, dim3 grid,
+                            cudaStream_t st) {
+  if (dh == 80) {
+    if (kb == 128) return emul ? launch_attention_t<80, 128, VARLEN, true>(qkv, T, p, grid, st)
+                               : launch_attention_t<80, 128, VARLEN, false>(qkv, T, p, grid, st);
+    return emul ? launch_attention_t<80, 64, VARLEN, true>(qkv, T, p, grid, st)
+                : launch_attention_t<80, 64, VARLEN, false>(qkv, T, p, grid, st);
+  }
+  if (kb == 128) return emul ? launch_attention_t<64, 128, VARLEN, true>(qkv, T, p, grid, st)
+                             : launch_attention_t<64, 128, VARLEN, false>(qkv, T, p, grid, st);
+  return emul ? launch_attention_t<64, 64, VARLEN, true>(qkv, T, p, grid, st)
+              : launch_attention_t<64, 64, VARLEN, false>(qkv, T, p, grid, st);
 }
+
+// test hooks (include/b200vit.h)
+static std::atomic<int> g_attn_mode{0};    // key 1
+static std::atomic<int> g_attn_emul{0};    // key 13
+static std::atomic<int> g_varlen_mode{0};  // key 11
 
 }  // namespace b200
 
 using namespace b200;
 
-namespace b200 {
-void attention_pipe_set_trace(long long* buf);
-void attention_pipe_set_emul(int v);
-}
-extern "C" void b200vit_debug_set_trace(void* dev_buf) {
-  attention_varlen_set_trace(reinterpret_cast<long long*>(dev_buf));
-  attention_pipe_set_trace(reinterpret_cast<long long*>(dev_buf));
-}
-
 extern "C" int b200vit_debug_set(int key, int value) {
   switch (key) {
     case 1: g_attn_mode = value; return 0;
-    case 2: g_attn_v_lbo = value; return 0;
-    case 3: g_attn_v_sbo = value; return 0;
-    case 4: gemm_force_version(value); return 0;
-    case 12: gemm2_force_epilogue_warps(value); return 0;
-    case 13: attention_pipe_set_emul(value); return 0;
-    case 14: g_attn_v16_lbo = value; return 0;
-    case 15: g_attn_v16_sbo = value; return 0;
-    case 16: g_attn_tail = value; return 0;
-    case 11: attention_varlen_set_mode(value); return 0;
+    case 11: g_varlen_mode = value; return 0;
+    case 12: gemm_set_block_n(value); return 0;
+    case 13: g_attn_emul = value; return 0;
     default: return B200VIT_ERR_INVALID;
   }
 }
@@ -562,83 +301,40 @@ extern "C" int b200vit_attention(const void* qkv, void* out, int B, int N, int H
   B200_CHECK_ARG(qkv && out, "attention: null pointer");
   B200_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention: bad shape B=%d N=%d H=%d", B, N, H);
   B200_CHECK_ARG(dh == 64 || dh == 80, "attention: dim_head=%d not supported by this build (64 or 80)", dh);
-  B200_CHECK_ARG(N <= 512, "attention: N=%d > 512 needs the (unbuilt) online-softmax path", N);
+  B200_CHECK_ARG(N <= 512, "attention: N=%d > 512 goes through b200vit_attention_varlen", N);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention: pointers must be 16-byte aligned");
-  const int mode = g_attn_mode.load();
-  if (mode == 2 && attention_pipe_eligible(N, dh))
-    return launch_attention_pipe(qkv, out, B, N, H, scale, (unsigned)g_attn_v_lbo.load(), (unsigned)g_attn_v_sbo.load(),
-                                 reinterpret_cast<cudaStream_t>(stream));
+  B200_CHECK_ARG(B <= 65535, "attention: B=%d exceeds the grid", B);
   AttnParams p{};
-  p.B = B; p.N = N; p.H = H;
-  p.I = H * dh;
-  // N = 256 + (1..4) (ViT-H/14 with its cls token: 257): a 272-column S tile would not fit twice into TMEM, so the tile
-  // keeps 256 keys (two CTAs per SM) and the softmax threads take the last keys themselves (g_attn_tail = 0: off).
-  // (A CUDA-core kernel for the 257th QUERY row instead of a third 128-row tile was measured too: 58 us per launch at
-  // batch 128 x 16 heads against 50 us for the tile -- not kept.)
-  p.ktail = (g_attn_tail.load() != 0 && N > 256 && N <= 260) ? N - 256 : 0;
-  p.KP = (N - p.ktail + 15) / 16 * 16;
-  // occupancy 2 (two single-warpgroup CTAs per SM, 256 TMEM columns each) whenever one region can hold S | P | O
-  const bool occ2 = p.KP <= 256;
-  const int nwg = occ2 ? 1 : ((N > 128 && p.KP <= 256) ? 2 : 1);
-  const int kv_rows = p.ktail ? (N + 7) / 8 * 8 : p.KP;   // rows of K / V staged in shared memory
-  p.kv_boxes = (kv_rows + 255) / 256;
-  p.kv_box_rows = ((kv_rows + p.kv_boxes - 1) / p.kv_boxes + 7) / 8 * 8;
-  const int q_tiles = (N + 127) / 128;
-  p.rounds = (q_tiles + nwg - 1) / nwg;
-  p.units = B * H * p.rounds;
-  p.scale_log2e = scale * 1.4426950408889634f;
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
-  p.v_lbo = (unsigned)g_attn_v_lbo.load();
-  p.v_sbo = (unsigned)g_attn_v_sbo.load();
-  p.v16_lbo = (unsigned)g_attn_v16_lbo.load();
-  p.v16_sbo = (unsigned)g_attn_v16_sbo.load();
+  p.N = N;
+  p.H = H;
+  p.I = H * dh;
+  p.scale_log2e = scale * 1.4426950408889634f;
+  const dim3 grid((N + ATT_QROWS - 1) / ATT_QROWS, H, B);
+  return launch_attention<false>(qkv, B * N, p, dh, g_attn_mode.load() == 2 ? 128 : 64, g_attn_emul.load() != 0,
+                                 grid, reinterpret_cast<cudaStream_t>(stream));
+}
 
-  CUtensorMap tm[4];  // Q and K/V boxes of 64 columns (128-byte swizzle), and -- dim_head 80 -- of 16 columns (32-byte)
-  CUtensorMap &tmQ = tm[0], &tmKV = tm[1];
-  const uint64_t dims[3] = {(uint64_t)3 * p.I, (uint64_t)N, (uint64_t)B};
-  const uint64_t strides[2] = {(uint64_t)3 * p.I * 2, (uint64_t)N * 3 * p.I * 2};
-  {
-    const uint32_t box[3] = {64, 128, 1};
-    int rc = encode_tmap_bf16(&tmQ, qkv, 3, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    const uint32_t box[3] = {64, (uint32_t)p.kv_box_rows, 1};
-    int rc = encode_tmap_bf16(&tmKV, qkv, 3, dims, strides, box);
-    if (rc) return rc;
-  }
-  tm[2] = tm[0];
-  tm[3] = tm[1];
-  if (dh == 80) {  // the 16-wide slabs: 32-byte rows, 32-byte swizzle
-    const uint32_t qbox[3] = {16, 128, 1};
-    int rc = encode_tmap_bf16_sw(&tm[2], qkv, 3, dims, strides, qbox, 32);
-    if (rc) return rc;
-    const uint32_t kvbox[3] = {16, (uint32_t)p.kv_box_rows, 1};
-    rc = encode_tmap_bf16_sw(&tm[3], qkv, 3, dims, strides, kvbox, 32);
-    if (rc) return rc;
-  }
-  const size_t kv64 = (size_t)att_kv_bytes(p.kv_boxes, p.kv_box_rows);
-  const size_t kv16 = dh == 80 ? ((size_t)p.kv_boxes * p.kv_box_rows * 32 + 1023) / 1024 * 1024 : 0;
-  const size_t kv_bytes = kv64 + kv16;
-  const size_t stage_bytes = 2 * kv_bytes + (size_t)nwg * (128 * 128 + (dh == 80 ? 128 * 32 : 0));
-  auto smem_for = [&](int st) { return st * stage_bytes + (2 * st + 4 * nwg) * 8 + 16 + 1024 + (p.ktail ? 2048 : 0); };
-  // two K/V/Q stages when they fit (prefetch of the next unit), else one; the occupancy-2 variant uses one
-  const int stages = (!occ2 && smem_for(2) <= 227 * 1024) ? 2 : 1;
-  const size_t smem_bytes = smem_for(stages);
-  B200_CHECK_ARG(smem_bytes <= 227 * 1024, "attention: N=%d needs %zu bytes of shared memory", N, smem_bytes);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc;
-  if (p.ktail) {
-    B200_CHECK_ARG(occ2 && smem_bytes <= 113 * 1024, "attention: key-tail layout does not fit (N=%d)", N);
-    rc = dh == 80 ? launch_attention_t<1, 1, 256, 80, true>(tm, p, smem_bytes, st)
-                  : launch_attention_t<1, 1, 256, 64, true>(tm, p, smem_bytes, st);
-  } else if (occ2 && smem_bytes <= 113 * 1024) {
-    rc = launch_attention<1, 1, 256>(tm, dh, p, smem_bytes, st);
-  } else if (nwg == 2) {
-    rc = stages == 1 ? launch_attention<2, 1>(tm, dh, p, smem_bytes, st) : launch_attention<2, 2>(tm, dh, p, smem_bytes, st);
-  } else {
-    rc = stages == 1 ? launch_attention<1, 1>(tm, dh, p, smem_bytes, st) : launch_attention<1, 2>(tm, dh, p, smem_bytes, st);
-  }
-  return rc;
+extern "C" int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev,
+                                        const int32_t* tile_prefix_dev, int num_seqs, int total_tokens, int total_tiles,
+                                        int H, int dh, float scale, void* stream) {
+  B200_CHECK_ARG(qkv && out && cu_seqlens_dev && tile_prefix_dev, "attention_varlen: null pointer");
+  B200_CHECK_ARG(num_seqs > 0 && total_tokens > 0 && total_tiles > 0 && H > 0, "attention_varlen: bad shape");
+  B200_CHECK_ARG(dh == 64 || dh == 80, "attention_varlen: dim_head=%d not supported by this build (64 or 80)", dh);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+                 "attention_varlen: pointers must be 16-byte aligned");
+  B200_CHECK_ARG(H <= 65535, "attention_varlen: H=%d exceeds the grid", H);
+  AttnParams p{};
+  p.out = reinterpret_cast<__nv_bfloat16*>(out);
+  p.cu_seqlens = cu_seqlens_dev;
+  p.tile_prefix = tile_prefix_dev;
+  p.num_seqs = num_seqs;
+  p.H = H;
+  p.I = H * dh;
+  p.scale_log2e = scale * 1.4426950408889634f;
+  const int mode = g_varlen_mode.load();
+  const dim3 grid(total_tiles, H, 1);
+  return launch_attention<true>(qkv, total_tokens, p, dh, mode == 1 ? 128 : 64, mode == 2, grid,
+                                reinterpret_cast<cudaStream_t>(stream));
 }

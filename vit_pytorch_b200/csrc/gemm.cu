@@ -1,11 +1,10 @@
-// Persistent, warp-specialised bf16 GEMM for sm_100a:  out = epilogue(A[M,K] * W[N,K]^T)
+// Persistent, warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] * W[N,K]^T)
 //
-//   warp 0        : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warp 1        : MMA issuer    (one thread; tcgen05.mma cta_group::1 kind::f16, 128 x BLOCK_N x 16, D in TMEM)
-//   warp 2        : TMEM allocator
-//   warps 4..11   : epilogue      (tcgen05.ld 32x32b -> registers -> bias / LN-fold / GELU / residual -> global)
+//   warpgroup 0     : TMA producer  (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
+//   warpgroups 1, 2 : consumers     (wgmma m64 x BLOCK_N x k16, fp32 accumulators in registers, 64 rows each), then
+//                     the epilogue straight from the accumulator registers: bias / LN-fold / GELU / residual -> global
 //
-// Two TMEM accumulator stages (2 x BLOCK_N columns) so the epilogue of tile i overlaps the MMAs of tile i+1.
+// The producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
 // Replaces the nn.Linear call sites listed in include/b200vit.h.
 #include "common.cuh"
 #include "host_util.h"
@@ -14,10 +13,8 @@ namespace b200 {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int NUM_NON_EPI_THREADS = 128;
-constexpr int NUM_EPI_WARPS = 8;
-constexpr int NUM_THREADS = NUM_NON_EPI_THREADS + NUM_EPI_WARPS * 32;
+constexpr int WGMMA_K = 16;
+constexpr int NUM_THREADS = 384;
 
 struct GemmParams {
   int M, N, K;
@@ -31,35 +28,34 @@ struct GemmParams {
   const float* ln_sums;  // [M][ln_parts][2]
   int ln_parts;
   int stats_parts;
+  int stats_width;       // output columns per statistics part (64 or 128)
   float ln_inv_dim;
   float ln_eps;
   const float* col_s;  // [N]
-  float* stats_out;    // [M][2]
+  float* stats_out;    // [M][stats_parts][2]
   // Rows of A (and of the output) per tile: BLOCK_M, or -- patch mode -- the patches of `patch_ght` patch rows of one
   // image (<= 128; the rest of the 128-row MMA tile is ignored).
   int rows_per_tile;
   // Patch mode (b200vit_patch_embed_tma): A is not a matrix in memory but the NCHW image itself, read through a 5-D
   // tensor map (pixel 16 | patch column | patch row | pixel row 16 | image x channel).  k block kb = channel * 4 + g
-  // covers pixel rows 4g .. 4g+3 of every patch.  With a swizzled tensor map every box row (16 pixels = 32 bytes)
-  // lands on its own 128-byte shared-memory row (measured: tools/patch_tma_probe.py), so the four pixel rows of a
-  // k block cannot share one operand row; they are loaded as four boxes into four 16 KB slabs, each a K-major
-  // operand of which the tensor core reads the first 16 k (one tcgen05.mma k-step per slab).
+  // covers pixel rows 4g .. 4g+3 of every patch, loaded as four boxes of 16 pixels (32 bytes) per patch into four
+  // 32B-swizzled slabs of 128 rows x 16 k: each slab is the K-major operand of one wgmma k-step.
   int patch;
   int patch_ght;            // patch rows per tile
   int patch_tiles_per_img;  // gh / patch_ght
   int patch_C;              // channels
 };
 
-// PATCH: the A stage holds FOUR 16 KB slabs, one per 16-wide k-step (see GemmParams::patch).
+// PATCH: the A stage holds FOUR 4 KB slabs, one per 16-wide k-step (see GemmParams::patch).
 template <int BLOCK_N, int STAGES, bool PATCH = false>
 struct GemmSmem {
-  static constexpr int A_SLAB = BLOCK_M * BLOCK_K * 2;
+  static constexpr int A_SLAB = PATCH ? BLOCK_M * 32 : BLOCK_M * BLOCK_K * 2;
   static constexpr int A_BYTES = PATCH ? 4 * A_SLAB : A_SLAB;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-  // full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], tmem base
-  static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 4) * 8 + 16;
+  // full[STAGES], empty[STAGES]
+  static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024B alignment
 };
 
@@ -68,49 +64,32 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
   using L = GemmSmem<BLOCK_N, STAGES, PATCH>;
-  constexpr int TMEM_COLS = 2 * BLOCK_N;  // 512 or 256 (power of two)
-  static_assert(TMEM_COLS == 512 || TMEM_COLS == 256 || TMEM_COLS == 128, "TMEM columns must be a power of two");
+  constexpr int NACC = BLOCK_N / 2;          // fp32 accumulators per consumer thread (64 rows x BLOCK_N / 128)
+  constexpr int CHUNKS = BLOCK_N / 64;       // 64-column statistics chunks per tile
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], NUM_EPI_WARPS);
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_base_smem, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -140,197 +119,182 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (single thread)
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BLOCK_N, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-          const uint64_t adesc = make_smem_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(sb, 16, 1024);
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: MMA + epilogue
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;                       // rows [64c, 64c + 64) of the tile
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
+  const int flags = p.flags;
+  const bool vec_ok = (p.ldo & 1) == 0;
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[NACC];
+
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m_blk = tile / p.num_n_tiles;
+    const int n_blk = tile % p.num_n_tiles;
+
+    int prev_stage = -1;
+    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
+      const uint32_t sb = sa + L::A_BYTES;
+      const uint64_t bdesc = make_wgmma_desc(sb, 1024, WGMMA_SW128);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            // advance 16 elements (32 B) along K inside the 128B swizzle row: +2 in the (addr >> 4) field
-            // (patch mode: the k-th 16 k of A are the first 32 bytes of the rows of slab k)
-            const uint64_t ad = PATCH ? make_smem_desc_sw128(sa + k * L::A_SLAB, 16, 1024) : adesc + 2 * k;
-            umma_ss(d_tmem, ad, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
+      for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
+        // patch mode: the k-th 16 k of A are the 32-byte rows of slab k; otherwise +32 B inside the 128B swizzle row
+        const uint64_t ad = PATCH ? make_wgmma_desc(sa + k * L::A_SLAB + c * 64 * 32, 256, WGMMA_SW32)
+                                  : make_wgmma_desc(sa + c * 64 * 128, 1024, WGMMA_SW128) + 2 * k;
+        if constexpr (BLOCK_N == 256) wgmma_m64n256k16(acc, ad, bdesc + 2 * k, (kb | k) != 0);
+        else wgmma_m64n128k16(acc, ad, bdesc + 2 * k, (kb | k) != 0);
+      }
+      wgmma_commit();
+      // the MMAs of the previous k block have finished reading their stage once at most one group is in flight
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && t == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
       }
     }
-  } else if (warp >= NUM_NON_EPI_THREADS / 32) {
-    // ------------------------------------------------------------------ epilogue
-    const int e = warp - NUM_NON_EPI_THREADS / 32;  // 0..7
-    const int quad = warp & 3;                      // TMEM lane quadrant this warp may access
-    constexpr int COLS_PER_WARP = BLOCK_N / (NUM_EPI_WARPS / 4);
-    const int col_off = (e >> 2) * COLS_PER_WARP;
-    const int flags = p.flags;
-    const bool vec_ok = (p.ldo & 7) == 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile / p.num_n_tiles;
-      const int n_blk = tile % p.num_n_tiles;
-      const int row = m_blk * p.rows_per_tile + quad * 32 + lane;
-      const bool row_ok = row < p.M && quad * 32 + lane < p.rows_per_tile;
-      float mu = 0.f, rstd = 1.f;
-      if ((flags & B200VIT_EPI_LNFOLD) && row_ok) {
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (t == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    // ---------------------------------------------------------------- epilogue
+    // accumulator layout (wgmma m64nN, fp32): acc[4j + h] holds row (16 warp + lane/4 + 8 (h >> 1)),
+    // column (8 j + 2 (lane % 4) + (h & 1)) of this warpgroup's 64 x BLOCK_N block
+    const int tr0 = c * 64 + warp * 16 + (lane >> 2);
+    float mu[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+    int row[2];
+    bool row_ok[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int tr = tr0 + 8 * h;
+      row[h] = m_blk * p.rows_per_tile + tr;
+      row_ok[h] = row[h] < p.M && tr < p.rows_per_tile;
+      if ((flags & B200VIT_EPI_LNFOLD) && row_ok[h]) {
         float s1 = 0.f, s2 = 0.f;
         for (int i = 0; i < p.ln_parts; ++i) {
-          const float2 ss = *reinterpret_cast<const float2*>(p.ln_sums + 2 * ((size_t)row * p.ln_parts + i));
+          const float2 ss = *reinterpret_cast<const float2*>(p.ln_sums + 2 * ((size_t)row[h] * p.ln_parts + i));
           s1 += ss.x;
           s2 += ss.y;
         }
-        mu = s1 * p.ln_inv_dim;
-        const float var = fmaxf(s2 * p.ln_inv_dim - mu * mu, 0.f);
-        rstd = rsqrtf(var + p.ln_eps);
+        mu[h] = s1 * p.ln_inv_dim;
+        const float var = fmaxf(s2 * p.ln_inv_dim - mu[h] * mu[h], 0.f);
+        rstd[h] = rsqrtf(var + p.ln_eps);
       }
-      float st_sum = 0.f, st_sq = 0.f;
+    }
+    float st_sum[2][CHUNKS], st_sq[2][CHUNKS];
+#pragma unroll
+    for (int q = 0; q < CHUNKS; ++q) st_sum[0][q] = st_sum[1][q] = st_sq[0][q] = st_sq[1][q] = 0.f;
 
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * BLOCK_N + col_off;
-#pragma unroll 1
-      for (int c = 0; c < COLS_PER_WARP; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(t_row + c, r);
-        tmem_ld_wait();
-        const int col0 = n_blk * BLOCK_N + col_off + c;
-        if (row_ok && col0 < p.N) {
+    const int n0 = n_blk * BLOCK_N;
 #pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            const int col = col0 + j;
-            if (col >= p.N) continue;
-            float v[8];
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      if (col >= p.N) continue;
+      const bool pair = vec_ok && col + 1 < p.N;
+      float b0 = 0.f, b1 = 0.f, s0 = 0.f, s1 = 0.f;
+      if (flags & B200VIT_EPI_BIAS) {
+        b0 = p.bias[col];
+        b1 = col + 1 < p.N ? p.bias[col + 1] : 0.f;
+      }
+      if (flags & B200VIT_EPI_LNFOLD) {
+        s0 = p.col_s[col];
+        s1 = col + 1 < p.N ? p.col_s[col + 1] : 0.f;
+      }
 #pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[j + i]);
-            const bool full8 = (col + 8 <= p.N);
-            if (full8 && vec_ok) {
-              if (flags & (B200VIT_EPI_LNFOLD | B200VIT_EPI_BIAS)) {
-                // y = acc * rstd + (bias - rstd*mu * s): the same two FMAs as the CTA-pair kernel, so both kernels
-                // give bit-identical results (batch-size invariance across the kernel switch at M = 1024)
-                const bool fold = (flags & B200VIT_EPI_LNFOLD) != 0;
-                float cv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                if (flags & B200VIT_EPI_BIAS) {
-                  const float4 b0 = *reinterpret_cast<const float4*>(p.bias + col);
-                  const float4 b1 = *reinterpret_cast<const float4*>(p.bias + col + 4);
-                  cv[0] = b0.x; cv[1] = b0.y; cv[2] = b0.z; cv[3] = b0.w;
-                  cv[4] = b1.x; cv[5] = b1.y; cv[6] = b1.z; cv[7] = b1.w;
-                }
-                if (fold) {
-                  const float4 s0 = *reinterpret_cast<const float4*>(p.col_s + col);
-                  const float4 s1 = *reinterpret_cast<const float4*>(p.col_s + col + 4);
-                  const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                  const float k = -rstd * mu;
+      for (int h = 0; h < 2; ++h) {
+        if (!row_ok[h]) continue;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (flags & (B200VIT_EPI_LNFOLD | B200VIT_EPI_BIAS)) {
+          // y = acc * rstd + (bias - rstd*mu * s)
+          const bool fold = (flags & B200VIT_EPI_LNFOLD) != 0;
+          const float k = -rstd[h] * mu[h];
+          const float c0 = fold ? fmaf(k, s0, b0) : b0, c1 = fold ? fmaf(k, s1, b1) : b1;
+          const float rs = fold ? rstd[h] : 1.0f;
+          v0 = fmaf(v0, rs, c0);
+          v1 = fmaf(v1, rs, c1);
+        }
+        if (flags & B200VIT_EPI_GELU) gelu_erf2(v0, v1);
+        const size_t o = (size_t)row[h] * p.ldo + col;
+        float r0 = 0.f, r1 = 0.f;
+        if (pair) {
+          if (flags & B200VIT_EPI_RESIDUAL) {
+            const float2 rr = *reinterpret_cast<const float2*>(p.resid + o);
+            v0 += rr.x;
+            v1 += rr.y;
+          }
+          if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(v0, v1);
+          const uint32_t pk = pack_bf16x2(v0, v1);
+          if (p.out_bf16) *reinterpret_cast<uint32_t*>(p.out_bf16 + o) = pk;
+          r0 = __uint_as_float(pk << 16);
+          r1 = __uint_as_float(pk & 0xFFFF0000u);
+        } else {
+          // scalar tail (N or ldo odd)
+          const float vv[2] = {v0, v1};
+          float rr[2] = {0.f, 0.f};
+          for (int i = 0; i < 2 && col + i < p.N; ++i) {
+            float x = vv[i];
+            if (flags & B200VIT_EPI_RESIDUAL) x += p.resid[o + i];
+            if (p.out_f32) p.out_f32[o + i] = x;
+            const __nv_bfloat16 xb = __float2bfloat16_rn(x);
+            if (p.out_bf16) p.out_bf16[o + i] = xb;
+            rr[i] = __bfloat162float(xb);
+          }
+          r0 = rr[0];
+          r1 = rr[1];
+        }
+        if (flags & B200VIT_EPI_STATS) {
+          st_sum[h][j / 8] += r0 + r1;
+          st_sq[h][j / 8] = fmaf(r0, r0, fmaf(r1, r1, st_sq[h][j / 8]));
+        }
+      }
+    }
+    if (flags & B200VIT_EPI_STATS) {
+      // the four lanes of a quad hold the same two rows: reduce, then lane 0 of the quad writes every part of the tile
 #pragma unroll
-                  for (int i = 0; i < 8; ++i) cv[i] = fmaf(k, sv[i], cv[i]);
-                }
-                const float rs = fold ? rstd : 1.0f;
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = fmaf(v[i], rs, cv[i]);
-              }
-              if (flags & B200VIT_EPI_GELU) {
+        for (int q = 0; q < CHUNKS; ++q) {
+          st_sum[h][q] += __shfl_xor_sync(0xffffffffu, st_sum[h][q], 1);
+          st_sum[h][q] += __shfl_xor_sync(0xffffffffu, st_sum[h][q], 2);
+          st_sq[h][q] += __shfl_xor_sync(0xffffffffu, st_sq[h][q], 1);
+          st_sq[h][q] += __shfl_xor_sync(0xffffffffu, st_sq[h][q], 2);
+        }
+      if ((lane & 3) == 0) {
+        const int per = p.stats_width / 64;   // 64-column chunks per part
+        const int first = n0 / p.stats_width;
+        const int last = (n_blk == p.num_n_tiles - 1) ? p.stats_parts : first + CHUNKS / per;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = gelu_erf(v[i]);
-              }
-              if (flags & B200VIT_EPI_RESIDUAL) {
-                const float* rp = p.resid + (size_t)row * p.ldo + col;
-                const float4 r0 = *reinterpret_cast<const float4*>(rp);
-                const float4 r1 = *reinterpret_cast<const float4*>(rp + 4);
-                v[0] += r0.x; v[1] += r0.y; v[2] += r0.z; v[3] += r0.w;
-                v[4] += r1.x; v[5] += r1.y; v[6] += r1.z; v[7] += r1.w;
-              }
-              if (p.out_f32) {
-                float* op = p.out_f32 + (size_t)row * p.ldo + col;
-                *reinterpret_cast<float4*>(op) = make_float4(v[0], v[1], v[2], v[3]);
-                *reinterpret_cast<float4*>(op + 4) = make_float4(v[4], v[5], v[6], v[7]);
-              }
-              uint4 pk;
-              pk.x = pack_bf16x2(v[0], v[1]);
-              pk.y = pack_bf16x2(v[2], v[3]);
-              pk.z = pack_bf16x2(v[4], v[5]);
-              pk.w = pack_bf16x2(v[6], v[7]);
-              if (p.out_bf16) *reinterpret_cast<uint4*>(p.out_bf16 + (size_t)row * p.ldo + col) = pk;
-              if (flags & B200VIT_EPI_STATS) {
-                const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
+        for (int h = 0; h < 2; ++h) {
+          if (!row_ok[h]) continue;
+          float* so = p.stats_out + 2 * (size_t)row[h] * p.stats_parts;
+          for (int part = first; part < last; ++part) {
+            float a = 0.f, b = 0.f;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const float lo = __uint_as_float(w[i] << 16);
-                  const float hi = __uint_as_float(w[i] & 0xFFFF0000u);
-                  st_sum += lo + hi;
-                  st_sq = fmaf(lo, lo, fmaf(hi, hi, st_sq));
-                }
+            for (int q = 0; q < CHUNKS; ++q)
+              if (first + q / per == part) {
+                a += st_sum[h][q];
+                b += st_sq[h][q];
               }
-            } else {
-              // scalar tail (N or ldo not a multiple of 8)
-              for (int i = 0; i < 8 && col + i < p.N; ++i) {
-                float x = v[i];
-                const int cc = col + i;
-                if (flags & (B200VIT_EPI_LNFOLD | B200VIT_EPI_BIAS)) {
-                  float cvs = (flags & B200VIT_EPI_BIAS) ? p.bias[cc] : 0.f;
-                  if (flags & B200VIT_EPI_LNFOLD) cvs = fmaf(-rstd * mu, p.col_s[cc], cvs);
-                  x = fmaf(x, (flags & B200VIT_EPI_LNFOLD) ? rstd : 1.0f, cvs);
-                }
-                if (flags & B200VIT_EPI_GELU) x = gelu_erf(x);
-                if (flags & B200VIT_EPI_RESIDUAL) x += p.resid[(size_t)row * p.ldo + cc];
-                if (p.out_f32) p.out_f32[(size_t)row * p.ldo + cc] = x;
-                const __nv_bfloat16 xb = __float2bfloat16_rn(x);
-                if (p.out_bf16) p.out_bf16[(size_t)row * p.ldo + cc] = xb;
-                if (flags & B200VIT_EPI_STATS) {
-                  const float xr = __bfloat162float(xb);
-                  st_sum += xr;
-                  st_sq = fmaf(xr, xr, st_sq);
-                }
-              }
-            }
+            *reinterpret_cast<float2*>(so + 2 * part) = make_float2(a, b);
           }
         }
       }
-      // release the accumulator stage back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if ((flags & B200VIT_EPI_STATS) && row_ok) {
-        const int part = n_blk * (NUM_EPI_WARPS / 4) + (e >> 2);
-        *reinterpret_cast<float2*>(p.stats_out + 2 * ((size_t)row * p.stats_parts + part)) =
-            make_float2(st_sum, st_sq);
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
     }
   }
-
-  // ------------------------------------------------------------------ teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
+
+// test hook 12: BLOCK_N of b200vit_gemm_bf16 -- 0 = auto (256 when N > 128), 1 = 128, 2 = 256
+static std::atomic<int> g_gemm_block_n{0};
+void gemm_set_block_n(int v) { g_gemm_block_n = v; }
 
 template <int BLOCK_N, int STAGES, bool PATCH = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, cudaStream_t stream) {
@@ -342,6 +306,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
   p.num_m_tiles = (p.M + p.rows_per_tile - 1) / p.rows_per_tile;
   p.num_n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
   p.num_k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+  p.stats_width = p.N > 128 ? 128 : 64;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(tmA, tmB, p);
@@ -353,7 +318,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
 }  // namespace b200
 
 extern "C" int b200vit_stats_parts(int N) {
-  const int block_n = N > 128 ? 256 : 128;      // both GEMM kernels: two column halves per N tile
+  const int block_n = N > 128 ? 256 : 128;      // two statistics parts per 256 (or, N <= 128, 128) columns
   return 2 * ((N + block_n - 1) / block_n);
 }
 
@@ -380,9 +345,6 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
                  "gemm: epilogue pointers must be 16-byte aligned");
 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (gemm2_eligible(M, N, K, ldo, flags, out_bf16, out_f32, resid))
-    return launch_gemm2(A, lda, W, ldw, out_bf16, out_f32, ldo, bias, resid, ln_sums, ln_parts, ln_eps, col_s,
-                        stats_out, M, N, K, flags, st);
 
   // K-tail: TMA zero-fills out-of-bounds columns of both operands, so any K works as long as rows are 16B multiples.
   GemmParams p{};
@@ -401,7 +363,8 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   p.col_s = col_s;
   p.stats_out = stats_out;
 
-  const bool wide = N > 128;
+  const int force = g_gemm_block_n.load();
+  const bool wide = force == 0 ? N > 128 : force == 2;
   const uint32_t block_n = wide ? 256 : 128;
   CUtensorMap tmA, tmB;
   {
@@ -438,17 +401,6 @@ extern "C" int b200vit_gemm_headnorm_bf16(const void* A, int64_t lda, const void
                  "gemm_headnorm: unsupported flags %d", flags);
   const bool hln = (flags & B200VIT_EPI_HEADLN) != 0;
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(head_gamma) & 15) == 0, "gemm_headnorm: head_gamma must be 16-byte aligned");
-  // fused: the CTA-pair kernel's bf16 epilogue, where one warp holds one whole head of its 32 rows
-  if (M > 0 && N > 0 && K > 0 && A && W && gemm2_eligible(M, N, K, ldo, flags, out_bf16, nullptr, nullptr) &&
-      (ldo % 8) == 0) {
-    B200_CHECK_ARG(!(flags & B200VIT_EPI_BIAS) || bias, "gemm_headnorm: EPI_BIAS without bias");
-    B200_CHECK_ARG(!(flags & B200VIT_EPI_LNFOLD) || (ln_sums && col_s && ln_parts >= 1 && ln_parts <= 64),
-                   "gemm_headnorm: EPI_LNFOLD needs ln_sums, col_s and 1 <= ln_parts <= 64");
-    B200_CHECK_ARG((lda & 7) == 0 && (ldw & 7) == 0 && lda >= K && ldw >= K && ldo >= N, "gemm_headnorm: bad strides");
-    return launch_gemm2(A, lda, W, ldw, out_bf16, nullptr, ldo, bias, nullptr, ln_sums, ln_parts, ln_eps, col_s,
-                        nullptr, M, N, K, flags | B200VIT_EPI_HEADNORM, reinterpret_cast<cudaStream_t>(stream),
-                        head_gamma, norm_heads * 64, head_eps);
-  }
   int rc = b200vit_gemm_bf16(A, lda, W, ldw, out_bf16, nullptr, ldo, bias, nullptr, ln_sums, ln_parts, ln_eps, col_s,
                              nullptr, M, N, K, flags & ~B200VIT_EPI_HEADLN, stream);
   if (rc) return rc;
@@ -458,8 +410,8 @@ extern "C" int b200vit_gemm_headnorm_bf16(const void* A, int64_t lda, const void
 
 
 // ------------------------------------------------------------------------------------------------------------------
-// im2col-free patch embedding (north star: "stages p x p x 3 pixels through TMA into shared memory and feeds a tcgen05
-// GEMM"): the patch projection reads the NCHW image directly; Rearrange('b c (h p1) (w p2) -> b (h w) (p1 p2 c)') and
+// im2col-free patch embedding (p x p x C pixels staged through TMA into shared memory feed the wgmma GEMM directly):
+// the patch projection reads the NCHW image directly; Rearrange('b c (h p1) (w p2) -> b (h w) (p1 p2 c)') and
 // the LayerNorm over the patch (vit.py:100-101) never materialise.  LayerNorm is folded exactly like everywhere else:
 //   LN(x) W^T + b  =  rstd (x (gamma W)^T - mu colsum) + (W beta + b),
 // x = raw bf16 pixels (the A operand), (mu, rstd) from b200vit_patch_stats.  The K order of the operand is
@@ -506,7 +458,7 @@ extern "C" int b200vit_patch_embed_tma(const void* img, const void* w_perm, cons
     const uint64_t dims[5] = {16, (uint64_t)gw, (uint64_t)gh, 16, (uint64_t)B * C};
     const uint64_t strides[4] = {32, (uint64_t)16 * W * 2, (uint64_t)W * 2, (uint64_t)H * W * 2};
     const uint32_t box[5] = {16, (uint32_t)gw, (uint32_t)ght, 1, 1};
-    int rc = encode_tmap_bf16(&tmA, img, 5, dims, strides, box);
+    int rc = encode_tmap_bf16_sw(&tmA, img, 5, dims, strides, box, 32);
     if (rc) return rc;
   }
   {
@@ -516,5 +468,5 @@ extern "C" int b200vit_patch_embed_tma(const void* img, const void* w_perm, cons
     int rc = encode_tmap_bf16(&tmB, w_perm, 2, dims, strides, box);
     if (rc) return rc;
   }
-  return launch_gemm<256, 2, true>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_gemm<256, 4, true>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
 }

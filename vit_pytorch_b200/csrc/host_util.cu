@@ -35,7 +35,7 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// Descriptor cache (SURVEY.md 8b): a forward re-encodes the same (pointer, shape, box) maps every call -- weights
+// Descriptor cache: a forward re-encodes the same (pointer, shape, box) maps every call -- weights
 // never move and the caching allocator hands the same activation buffers back -- so the 128-byte descriptors are
 // kept per key.  The descriptor depends on nothing but the key, so a stale entry cannot exist; the table is simply
 // emptied when it grows past kTmapCacheMax entries.
@@ -191,7 +191,7 @@ int ensure_dyn_smem(const void* kernel, size_t bytes) {
 extern "C" {
 
 const char* b200vit_last_error(void) { return b200::g_err; }
-int b200vit_version(void) { return 210; }  /* round 2, final kernels */
+int b200vit_version(void) { return 300; }  /* sm_90a kernels */
 int64_t b200vit_launch_count(void) { return b200::g_launches.load(); }
 void b200vit_reset_launch_count(void) { b200::g_launches.store(0); }
 
@@ -202,8 +202,8 @@ int b200vit_device_ok(int dev) {
     b200::set_error("cudaGetDeviceProperties(%d): %s", dev, cudaGetErrorString(e));
     return B200VIT_ERR_CUDA;
   }
-  if (prop.major != 10) {
-    b200::set_error("device %d is sm_%d%d; libb200vit contains sm_100a code only", dev, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    b200::set_error("device %d is sm_%d%d; libb200vit contains sm_90a code only", dev, prop.major, prop.minor);
     return B200VIT_ERR_DEVICE;
   }
   if (!b200::get_encode()) {

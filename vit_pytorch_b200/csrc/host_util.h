@@ -45,17 +45,8 @@ int encode_tmap_f32(CUtensorMap* tm, const void* base, int rank, const uint64_t*
 
 void tmap_cache_stats(int64_t* hits, int64_t* misses);
 
-// gemm2.cu (CTA-pair kernel)
-int gemm2_eligible(int M, int N, int K, int64_t ldo, int flags, const void* out_bf16, const float* out_f32,
-                   const float* resid);
-int launch_gemm2(const void* A, int64_t lda, const void* W, int64_t ldw, void* out_bf16, float* out_f32, int64_t ldo,
-                 const float* bias, const float* resid, const float* ln_sums, int ln_parts, float ln_eps,
-                 const float* col_s, float* stats_out, int M, int N, int K, int flags, cudaStream_t stream,
-                 const float* head_gamma = nullptr, int norm_cols = 0, float head_eps = 0.f);
-void gemm_force_version(int v);
-void gemm2_force_epilogue_warps(int v);
-void attention_varlen_set_mode(int v);
-void attention_varlen_set_trace(long long* buf);
+// test hook 12 (gemm.cu)
+void gemm_set_block_n(int v);
 
 // SM count of the CURRENT device (cached per device).
 int num_sms();

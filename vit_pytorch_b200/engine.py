@@ -1,4 +1,4 @@
-"""Host-side engine of the fused sm_100a forward: weight preparation, workspaces and the kernel schedule.
+"""Host-side engine of the fused sm_90a forward: weight preparation, workspaces and the kernel schedule.
 
 The nn.Modules in vit.py / simple_vit.py own the parameters (reference-compatible names); this file turns them into
 the flat bf16 / fp32 device buffers the C ABI (include/b200vit.h) consumes and issues the launches on torch's current
@@ -6,8 +6,8 @@ stream.  Nothing here computes on the host and nothing falls back: a missing lib
 
 Schedule per encoder layer (reference vit.py:78-81), M = B*N token rows, residual stream x kept in fp32:
     xn  = LayerNorm(x)                         b200vit_layernorm      fp32 -> bf16              (vit.py:52)
-    qkv = xn Wqkv^T                            b200vit_gemm_bf16      tcgen05, bf16 out         (vit.py:54)
-    o   = softmax(q k^T * scale) v             b200vit_attention      tcgen05 + TMEM            (vit.py:55-63)
+    qkv = xn Wqkv^T                            b200vit_gemm_bf16      wgmma, bf16 out           (vit.py:54)
+    o   = softmax(q k^T * scale) v             b200vit_attention      wgmma, online softmax     (vit.py:55-63)
     x  += o Wout^T + b                         b200vit_gemm_bf16      residual epilogue, fp32   (vit.py:64,80)
     xn  = LayerNorm(x)                         b200vit_layernorm                               (vit.py:19)
     h   = GELU(xn W1^T + b1)                   b200vit_gemm_bf16      bias+GELU epilogue        (vit.py:20-21)
@@ -33,7 +33,7 @@ def ln_mode() -> str:
     """'exact' : LayerNorm kernel -> bf16 -> GEMM, the literal operator sequence of the reference.
        'fold'  : (default) no standalone LayerNorm kernels inside the layer loop.  The residual GEMMs (out-proj, fc2) also emit
                  a bf16 copy of x plus per-row (sum, sum^2); the following GEMM multiplies that copy by gamma*W and
-                 applies  rstd*(acc - mu*colsum) + (W beta + b)  in its epilogue (SURVEY.md A.2).  The statistics are
+                 applies  rstd*(acc - mu*colsum) + (W beta + b)  in its epilogue.  The statistics are
                  written as per-tile partials (no atomics) and summed in a fixed order, so results are deterministic."""
     m = os.environ.get(_LN_MODE_ENV, "fold")
     if m not in ("fold", "exact"):
@@ -105,8 +105,8 @@ def why_not_fused(params: List[torch.Tensor], x: torch.Tensor, *, training: bool
         return "autograd is recording (fused path is forward only)"
     if training and dropout_p > 0.0:
         return "dropout is active"
-    if torch.cuda.get_device_capability(x.device)[0] != 10:
-        return "device is not sm_100"
+    if torch.cuda.get_device_capability(x.device) != (9, 0):
+        return "device is not sm_90"
     return None
 
 
@@ -467,7 +467,7 @@ class PatchEmbedEngine:
         y = torch.empty(B * n, D, device=dev, dtype=torch.float32)
         if ("tma.w" in t and (ph, pw) == (16, 16) and os.environ.get(_PATCH_MODE_ENV, "tma") == "tma"
                 and W // pw <= 128 and D % 8 == 0):
-            # the tcgen05 GEMM reads the image itself: no patch matrix, no LayerNorm pass
+            # the wgmma GEMM reads the image itself: no patch matrix, no LayerNorm pass
             stats_p = torch.empty(B * n, 2, device=dev, dtype=torch.float32)
             _lib.patch_embed_tma(img.contiguous(), t["tma.w"], t["tma.b"], t["tma.s"], stats_p, y,
                                  eps=o.to_patch_embedding[1].eps)

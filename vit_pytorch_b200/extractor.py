@@ -1,7 +1,7 @@
 """`Extractor` with the interface of `vit_pytorch.extractor.Extractor` (reference extractor.py:18-92): returns the
 logits together with the output (or input) of one layer, `vit.transformer` by default.
 
-With the default layer the wrapped model stays on the fused sm_100a path: its forward notices the hook on the
+With the default layer the wrapped model stays on the fused sm_90a path: its forward notices the hook on the
 Transformer module and passes the tokens through that module call (engine.hooked_transformer_tokens).  A layer strictly
 inside the transformer needs the materialised PyTorch graph, which the model's dispatch then runs for that call.
 """

@@ -5,10 +5,10 @@ Same constructor keywords, parameter / buffer names, shapes and registration ord
 attention pooling with one learned query, bias-free head), same `forward(List[Tensor] | List[List[Tensor]],
 group_images=False, group_max_seq_len=2048) -> (num_images, num_classes)` and the same greedy packing helper.
 
-Two executions of the same arithmetic (SURVEY.md 8a rows a13-a16):
+Two executions of the same arithmetic:
   * PyTorch graph (CPU, fp32, training, autograd, hooks): packed rows + a boolean mask built from per-token image ids,
     like the reference.
-  * fused sm_100a path (CUDA bf16, eval, no autograd): images never interact, so the packing and the O(B L^2) mask are
+  * fused sm_90a path (CUDA bf16, eval, no autograd): images never interact, so the packing and the O(B L^2) mask are
     dropped altogether -- all tokens of all images form ONE padding-free [T, D] matrix described by cu_seqlens, the
     encoder GEMMs run on it unchanged, attention is the varlen block-diagonal kernel (`b200vit_attention_varlen`,
     pipelined 64-key blocks, any image size), the q/k RMSNorm is an epilogue of the QKV GEMM and the attention pooling
@@ -167,7 +167,7 @@ class NaViT(FusedWeightsMixin, nn.Module):
         return next(self.parameters()).device
 
     # ------------------------------------------------------------------------------------------------------------
-    # fused sm_100a path
+    # fused sm_90a path
     # ------------------------------------------------------------------------------------------------------------
     def fused_reason(self, batched_images=None) -> Optional[str]:
         """None if forward(batched_images) runs the hand-written kernels, else the reason for the PyTorch graph."""

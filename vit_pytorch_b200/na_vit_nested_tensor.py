@@ -9,7 +9,7 @@ scale `dim_head ** -0.5`, and attention pooling WITHOUT the residual query (`for
 Two executions of the same arithmetic:
   * PyTorch graph (CPU / fp32 / training / autograd / hooks): images never interact, so the reference's jagged batch is
     evaluated image by image with plain dense tensors -- no dependence on the prototype nested-tensor operators.
-  * fused sm_100a path (CUDA bf16, eval): exactly `na_vit.NaViT`'s padding-free schedule -- all tokens in one [T, D]
+  * fused sm_90a path (CUDA bf16, eval): exactly `na_vit.NaViT`'s padding-free schedule -- all tokens in one [T, D]
     matrix described by `cu_seqlens`, `b200vit_patchify_varlen_ln`, `b200vit_embed_varlen`, LN-folded QKV GEMM with the
     per-head LayerNorm as its epilogue (`EPI_HEADLN`), `b200vit_attention_varlen`, dual-epilogue residual GEMMs,
     `b200vit_attn_pool`.  The LayerNorm biases of the patch embedding are folded on the host (beta_1 into the patch
@@ -150,7 +150,7 @@ class NaViT(FusedWeightsMixin, nn.Module):
         return self.mlp_head(self.to_latent(logits))
 
     # ------------------------------------------------------------------------------------------------------------
-    # fused sm_100a path
+    # fused sm_90a path
     # ------------------------------------------------------------------------------------------------------------
     def fused_reason(self, images=None) -> Optional[str]:
         if not images:

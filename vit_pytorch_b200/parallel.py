@@ -1,5 +1,5 @@
 """Data-parallel execution over the GPUs of one box: one process per GPU, weights replicated, the batch sharded
-contiguously, and exactly one collective -- an all-gather of the [B_local, num_classes] logits (SURVEY.md 8e).
+contiguously, and exactly one collective -- an all-gather of the [B_local, num_classes] logits.
 
 The encoder has no cross-sample operation (no BatchNorm; reference vit.py / simple_vit.py), so nothing else is
 exchanged.  Backend: NCCL over NVLink/NVSwitch on GPUs, gloo in the CPU tests.
@@ -27,7 +27,7 @@ def shard_sizes(total: int, world: int) -> List[int]:
 
 def balanced_bounds(costs: Sequence[float], world: int) -> List[Tuple[int, int]]:
     """Contiguous [lo, hi) slices of a list of items with per-item `costs`, one per rank, minimising the largest
-    slice cost (binary search on the bottleneck + greedy fill).  For NaViT (SURVEY.md 8e: "shard packed rows") the
+    slice cost (binary search on the bottleneck + greedy fill).  For NaViT the
     items are images and the cost of an image with n tokens is `navit_image_cost(n, ...)`: an even split by image
     COUNT can leave one rank with several times the tokens of another.  Every rank computes the same bounds."""
     n = len(costs)

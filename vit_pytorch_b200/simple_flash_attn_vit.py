@@ -3,7 +3,7 @@ twin whose attention calls `F.scaled_dot_product_attention` (`use_flash=True`, t
 softmax(q k^T) v (`use_flash=False`), whose Transformer has NO final LayerNorm, and whose head is
 `Sequential(LayerNorm, Linear)`; the sin-cos table is built from the input's own patch grid on every call.
 
-Both `use_flash` settings compute the same function; on the fused sm_100a path both are this repo's own attention
+Both `use_flash` settings compute the same function; on the fused sm_90a path both are this repo's own attention
 kernel (the flag only selects the PyTorch operator of the eager graph, exactly as in the reference).
 """
 from __future__ import annotations

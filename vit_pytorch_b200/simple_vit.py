@@ -1,4 +1,4 @@
-"""Drop-in `SimpleViT` for `vit_pytorch.SimpleViT` (reference simple_vit.py:80-120) with a fused sm_100a forward.
+"""Drop-in `SimpleViT` for `vit_pytorch.SimpleViT` (reference simple_vit.py:80-120) with a fused sm_90a forward.
 
 Differences from vit.ViT that the reference defines and this mirrors: no cls token and no dropout modules, a fixed
 2-D sin-cos positional table kept as a plain tensor attribute (not a parameter / buffer, so it is absent from

@@ -3,7 +3,7 @@
 matrix on every call, mean pool, linear head.
 
 Same constructor keywords, parameter names / registration order (=> identical `state_dict`, identical init under one
-seed).  The encoder blocks are simple_vit's; on the fused sm_100a path the series is handed to the patch kernels as a
+seed).  The encoder blocks are simple_vit's; on the fused sm_90a path the series is handed to the patch kernels as a
 `(B, C, 1, L)` image with a `1 x patch_size` patch box -- `'b c (n p) -> b n (p c)'` (reference :84) is the 2-D
 `(p1 p2 c)` order with `p1 = 1` -- so no new kernel is involved.
 """

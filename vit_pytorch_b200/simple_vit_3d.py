@@ -3,7 +3,7 @@
 call, mean pool, linear head.
 
 Same constructor keywords, parameter names / registration order (=> identical `state_dict`, identical init under one
-seed).  The encoder blocks are simple_vit's.  On the fused sm_100a path the video is handed to the 2-D patch kernels
+seed).  The encoder blocks are simple_vit's.  On the fused sm_90a path the video is handed to the 2-D patch kernels
 as a `(B, C, F' * H, W)` image: with `frame_patch_size == 1` that is the video's own memory (a view; 16 x 16 boxes then
 go through the TMA patch embedding), otherwise one device-side permute first puts the `pf` frames of a box under each
 other so that `(pf p1)` becomes the box height -- `'(pf p1 p2 c)'` (reference :97) is the 2-D `(p1' p2 c)` order with

@@ -3,7 +3,7 @@ simple_vit_with_patch_dropout.py:27-141): SimpleViT that, IN TRAINING, keeps a r
 (`PatchDropout`), and builds its sin-cos positional table from the input's own patch grid on every call (so any
 resolution divisible by the patch size is accepted).
 
-In eval mode `PatchDropout` is the identity (reference :34-35) and the fused sm_100a path is simple_vit's schedule;
+In eval mode `PatchDropout` is the identity (reference :34-35) and the fused sm_90a path is simple_vit's schedule;
 in training with prob > 0 the PyTorch graph runs (random token subsets are a training-time feature, the fused path
 is forward only).
 """

@@ -5,7 +5,7 @@ softmax scale 1.
 Mirrored as the reference defines it, including its quirk that `linear_head` is `nn.LayerNorm(dim)` -- the model
 returns (B, dim) normalised features and `num_classes` is unused (simple_vit_with_qk_norm.py:128,141).
 
-Fused sm_100a path: the q / k normalisation is the head-norm epilogue of the CTA-pair QKV GEMM
+Fused sm_90a path: the q / k normalisation runs right after the QKV GEMM
 (`b200vit_gemm_headnorm_bf16`, built for NaViT), attention runs with scale 1, everything else is simple_vit's schedule.
 """
 from __future__ import annotations

@@ -3,7 +3,7 @@ simple_vit_with_register_tokens.py:85-134): SimpleViT plus `num_register_tokens`
 image's sequence (no positional embedding on them), dropped again before the mean pool.
 
 Same constructor keywords, parameter names / registration order (=> identical `state_dict` and identical init under one
-seed) as the reference.  The encoder blocks are exactly simple_vit's, so the fused sm_100a path is the same kernel
+seed) as the reference.  The encoder blocks are exactly simple_vit's, so the fused sm_90a path is the same kernel
 schedule on N = patches + registers tokens; the registers are written by the token-assembly kernel
 (`b200vit_embed_tokens`, tail rows) and the pooling kernel averages only the patch tokens.
 """

@@ -1,12 +1,12 @@
-"""Drop-in `ViT` for lucidrains/vit-pytorch's `vit_pytorch.ViT` with a fused sm_100a forward.
+"""Drop-in `ViT` for lucidrains/vit-pytorch's `vit_pytorch.ViT` with a fused sm_90a forward.
 
 Same constructor keywords, parameter names / shapes / registration order (=> identical `state_dict` and identical
 random init under the same seed) and the same attribute surface the reference's wrappers reach into
 (`to_patch_embedding[0..3]`, `cls_token`, `pos_embedding`, `dropout`, `transformer`, `pool`, `to_latent`, `mlp_head`,
 `patch_size`; reference vit.py:85-138, users: mae.py:25-31, simmim.py:19-25, recorder.py:26-28, extractor.py:46-59).
 
-forward() dispatch (SURVEY.md 8b):
-  * CUDA sm_100 + bf16 parameters and input + no autograd recording + dropout inactive + no forward hooks inside the
+forward() dispatch:
+  * CUDA sm_90 + bf16 parameters and input + no autograd recording + dropout inactive + no forward hooks inside the
     model  ->  hand-written kernels of libb200vit.so through the C ABI (engine.py).  If the library is missing or a
     kernel call fails this RAISES; there is no silent fallback for an eligible call.
   * anything else (CPU, fp32, training with dropout, Recorder/Extractor hooks) -> the plain PyTorch graph below, which
@@ -180,7 +180,7 @@ class ViT(FusedWeightsMixin, nn.Module):
 
     # ---------------------------------------------------------------------------------------------- dispatch
     def fused_reason(self, img: torch.Tensor) -> Optional[str]:
-        """None if forward(img) will run the fused sm_100a kernels, else the reason for the PyTorch graph."""
+        """None if forward(img) will run the fused sm_90a kernels, else the reason for the PyTorch graph."""
         if img.dim() != 4:
             return "input is not (B, C, H, W)"
         if img.shape[1] * self.patch_size[0] * self.patch_size[1] != self.to_patch_embedding[1].normalized_shape[0]:
