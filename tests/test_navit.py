@@ -95,31 +95,55 @@ def test_varlen_index_arrays_host_logic():
     assert ix.cu.data_ptr() % 4 == 0 and ix.img_ptrs.data_ptr() % 8 == 0
 
 
-def test_navit_lnfold_prepared_tensors_reproduce_layernorm_linear():
-    """Host side of the LN-fold (na_vit.py:_prepared): with W_g = W * gamma (bf16), s = rowsum(W_g) and the row
-    statistics of the bf16 token copy,  rstd * (xb W_g^T - mu * s) + t  equals  Linear(LayerNorm(x))  of the reference
-    modules (Attention.norm -> to_q / to_kv and FeedForward[0] -> [1], na_vit.py:142-146,105-113)."""
+# per transformer family: module path, model class, LN -> [q | k | v] of one layer, LN -> fc1 of one layer, whether its
+# attention normalises q and k per head, whether its LayerNorms have a shift
+_VIT_QKV = lambda a, x: a.to_qkv(a.norm(x))                            # noqa: E731
+_VIT_FC1 = lambda ff, x: ff.net[1](ff.net[0](x))                       # noqa: E731
+LNFOLD_FAMILIES = {
+    "vit": ("vit_pytorch_b200.vit", "ViT", _VIT_QKV, _VIT_FC1, False, True),
+    "simple_vit": ("vit_pytorch_b200.simple_vit", "SimpleViT", _VIT_QKV, _VIT_FC1, False, True),
+    "simple_vit_with_qk_norm": ("vit_pytorch_b200.simple_vit_with_qk_norm", "SimpleViT", _VIT_QKV, _VIT_FC1, True, True),
+    "simple_flash_attn_vit": ("vit_pytorch_b200.simple_flash_attn_vit", "SimpleViT", _VIT_QKV, _VIT_FC1, False, True),
+    "na_vit": ("vit_pytorch_b200.na_vit", "NaViT",
+               lambda a, x: torch.cat([a.to_q(a.norm(x)), a.to_kv(a.norm(x))], dim=-1),
+               lambda ff, x: ff[1](ff[0](x)), True, False),
+    "na_vit_nested_tensor": ("vit_pytorch_b200.na_vit_nested_tensor", "NaViT",
+                             lambda a, x: torch.cat([a.to_queries(a.norm(x)), a.to_keys(a.norm(x)),
+                                                     a.to_values(a.norm(x))], dim=-1),
+                             lambda ff, x: ff[1](ff[0](x)), True, False),
+}
+
+
+@pytest.mark.parametrize("family", list(LNFOLD_FAMILIES))
+def test_navit_lnfold_prepared_tensors_reproduce_layernorm_linear(family):
+    """Host side of the LN-fold (engine.TransformerEngine.prepared, from each family's encoder_layers()): with
+    W_g = W * gamma (bf16), s = rowsum(W_g) and the row statistics of the bf16 token copy,  rstd * (xb W_g^T - mu * s) + t
+    equals  Linear(LayerNorm(x))  of the reference modules (Attention.norm -> QKV projection and FeedForward's
+    LayerNorm -> first Linear; e.g. na_vit.py:142-146,105-113)."""
+    import importlib
+    path, cls, qkv, fc1, qk_norm, has_beta = LNFOLD_FAMILIES[family]
     torch.manual_seed(0)
-    m = NaViT(image_size=64, patch_size=8, num_classes=5, dim=64, depth=2, heads=2, mlp_dim=128).eval()
+    m = getattr(importlib.import_module(path), cls)(image_size=64, patch_size=8, num_classes=5, dim=64, depth=2,
+                                                    heads=2, mlp_dim=128).eval()
     with torch.no_grad():
-        for p in m.parameters():                      # non-trivial gammas
+        for p in m.parameters():                      # non-trivial gammas (and betas, where the family has them)
             if p.ndim == 1:
                 p.add_(0.3 * torch.randn_like(p))
-    t = m._prepared()
+    t = m.transformer.engine().prepared()
     x = torch.randn(37, 64) * 2 + 0.5
     xb = x.bfloat16().float()
     mu = xb.mean(1, keepdim=True)
     rstd = torch.rsqrt((xb * xb).mean(1, keepdim=True) - mu * mu + 1e-5)
     for i, (attn, ff) in enumerate(m.transformer.layers):
         with torch.no_grad():
-            xn = attn.norm(xb)
-            want_qkv = torch.cat([attn.to_q(xn), attn.to_kv(xn)], dim=-1)
-            want_h = ff[1](ff[0](xb))
-        got_qkv = rstd * (xb @ t[f"{i}.a.qkvg"].float().t() - mu * t[f"{i}.a.qkvs"]) + t[f"{i}.a.qkvt"]
-        got_h = rstd * (xb @ t[f"{i}.f.w1g"].float().t() - mu * t[f"{i}.f.w1s"]) + t[f"{i}.f.b1"]
+            want_qkv = qkv(attn, xb)
+            want_h = fc1(ff, xb)
+        got_qkv = rstd * (xb @ t[f"{i}.qkv.wg"].float().t() - mu * t[f"{i}.qkv.s"]) + t[f"{i}.qkv.t"]
+        got_h = rstd * (xb @ t[f"{i}.fc1.wg"].float().t() - mu * t[f"{i}.fc1.s"]) + t[f"{i}.fc1.t"]
         assert torch.allclose(got_qkv, want_qkv, rtol=2e-2, atol=2e-2), (got_qkv - want_qkv).abs().max()
         assert torch.allclose(got_h, want_h, rtol=2e-2, atol=2e-2), (got_h - want_h).abs().max()
-        assert t[f"{i}.a.gqk"].numel() == 2 * 2 * 64 and t[f"{i}.a.qkvt"].abs().max() == 0
+        assert (f"{i}.gqk" in t) == qk_norm and (not qk_norm or t[f"{i}.gqk"].numel() == 2 * 2 * 64)
+        assert has_beta or t[f"{i}.qkv.t"].abs().max() == 0
 
 
 def test_oracle_and_dropin_at_config5_geometry_equal_the_reference_golden():

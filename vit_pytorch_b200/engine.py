@@ -1,8 +1,10 @@
 """Host-side engine of the fused sm_90a forward: weight preparation, workspaces and the kernel schedule.
 
-The nn.Modules in vit.py / simple_vit.py own the parameters (reference-compatible names); this file turns them into
-the flat bf16 / fp32 device buffers the C ABI (include/b200vit.h) consumes and issues the launches on torch's current
-stream.  Nothing here computes on the host and nothing falls back: a missing library or a failing call raises.
+The nn.Modules in vit.py, simple_vit.py, na_vit.py, ... own the parameters (reference-compatible names); each
+Transformer describes its layers to this file as EncoderLayer records, the only thing the engine knows about a model
+family.  This file turns them into the flat bf16 / fp32 device buffers the C ABI (include/b200vit.h) consumes and
+issues the launches on torch's current stream.  Nothing here computes on the host and nothing falls back: a missing
+library or a failing call raises.
 
 Schedule per encoder layer (reference vit.py:78-81), M = B*N token rows, residual stream x kept in fp32:
     xn  = LayerNorm(x)                         b200vit_layernorm      fp32 -> bf16              (vit.py:52)
@@ -16,7 +18,8 @@ Schedule per encoder layer (reference vit.py:78-81), M = B*N token rows, residua
 from __future__ import annotations
 
 import os
-from typing import Dict, List, Optional, Tuple
+from dataclasses import dataclass
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 from torch import nn
@@ -110,9 +113,37 @@ def why_not_fused(params: List[torch.Tensor], x: torch.Tensor, *, training: bool
     return None
 
 
-def _softmax_scale(attn) -> float:
-    """dim_head ** -0.5 (vit.py:37,57) unless the module says otherwise (q/k-normalised attention uses 1)."""
-    return float(getattr(attn, "softmax_scale", attn.scale))
+class Norm(NamedTuple):
+    """A LayerNorm over the feature dim.  beta None: the norm has no shift."""
+    gamma: torch.Tensor
+    beta: Optional[torch.Tensor]
+    eps: float
+
+    @staticmethod
+    def of(ln: nn.LayerNorm) -> "Norm":
+        return Norm(ln.weight, ln.bias, ln.eps)
+
+
+@dataclass
+class EncoderLayer:
+    """One pre-LN encoder layer as a model family describes it to the engine (reference vit.py:78-81):
+        x += out(attention(qkv(LN1(x))))        x += fc2(GELU(fc1(LN2(x))))
+    The tensors are the module's own parameters; TransformerEngine.prepared() derives the device copies from them."""
+    ln1: Norm
+    qkv_w: torch.Tensor                            # [3 * heads * dim_head, D], rows q | k | v
+    out_w: Optional[torch.Tensor]                  # None: to_out is the identity (heads == 1 and dim_head == D)
+    out_b: Optional[torch.Tensor]
+    ln2: Norm
+    fc1_w: torch.Tensor
+    fc1_b: torch.Tensor
+    fc2_w: torch.Tensor
+    fc2_b: torch.Tensor
+    heads: int
+    dim_head: int
+    scale: float                                   # softmax scale
+    qk_norm: Optional[str] = None                  # per-head norm of q and k after the projection: None, "rms" or "ln"
+    qk_gamma: Tuple[torch.Tensor, ...] = ()        # (q gamma, k gamma), each heads * dim_head values
+    qk_eps: float = 0.0                            # eps of the "ln" head norm
 
 
 class _Prepared:
@@ -156,8 +187,8 @@ class FusedWeightsMixin:
         return out
 
 
-def _f32(p: torch.Tensor) -> torch.Tensor:
-    return p.detach().float().contiguous()
+def _f32(p: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    return None if p is None else p.detach().float().contiguous()
 
 
 def _bf16_rows(p: torch.Tensor, k_pad: Optional[int] = None) -> torch.Tensor:
@@ -170,35 +201,60 @@ def _bf16_rows(p: torch.Tensor, k_pad: Optional[int] = None) -> torch.Tensor:
     return w.to(torch.bfloat16).contiguous()
 
 
+def _fold(t: Dict[str, torch.Tensor], prefix: str, w: torch.Tensor, b: Optional[torch.Tensor], ln: Norm) -> None:
+    """LayerNorm folded into the Linear that follows it:
+        LN(x) W^T + b  ==  rstd * (x (gamma*W)^T - mu * colsum) + (W beta + b)
+    t[prefix + '.wg'] = gamma*W (bf16), '.s' = its row sums, '.t' = W beta + b (just b, or zeros, when beta is None)."""
+    w32 = w.detach().float()
+    wg = (w32 * ln.gamma.detach().float()[None, :]).to(torch.bfloat16).contiguous()
+    t[prefix + ".wg"] = wg
+    t[prefix + ".s"] = wg.float().sum(dim=1).contiguous()          # from the ROUNDED weights the MMA sees
+    if ln.beta is None:
+        # still a bias vector: the GEMM keeps its bias epilogue whether or not the LayerNorm has a shift
+        t[prefix + ".t"] = _f32(b) if b is not None else torch.zeros(w.shape[0], device=w.device, dtype=torch.float32)
+    else:
+        tb = w32 @ ln.beta.detach().float()
+        t[prefix + ".t"] = (tb + b.detach().float() if b is not None else tb).contiguous()
+
+
+class FusedEncoder:
+    """nn.Module mixin of the Transformers the engine runs.  A class using it provides
+        encoder_layers() -> (List[EncoderLayer], final Norm or None)
+    and gets engine(), its TransformerEngine (made on first use, kept with the module)."""
+
+    def engine(self) -> "TransformerEngine":
+        eng = getattr(self, "_engine", None)
+        if eng is None:
+            eng = self._engine = TransformerEngine(self)
+        return eng
+
+
 class TransformerEngine:
-    """Fused execution of a vit.Transformer / simple_vit.Transformer module (reference vit.py:66-83)."""
+    """Fused execution of the encoder layers a FusedEncoder module describes (reference vit.py:66-83)."""
 
     def __init__(self, transformer: nn.Module) -> None:
         self.mod = transformer
         self.prep = _Prepared()
+        # what prepared() was built from: the layers and the final LayerNorm (simple_flash_attn_vit.py has none)
+        self.layers: List[EncoderLayer] = []
+        self.norm: Optional[Norm] = None
         self.ws_key: Optional[tuple] = None
         self.ws: Dict[str, torch.Tensor] = {}
         self.c_ws = None                       # _lib.EncoderWs over self.ws
-
-    # -------------------------------------------------------------------------------------------- structure
-    def _layers(self):
-        for attn, ff in self.mod.layers:
-            yield attn, ff
+        self._vl_key: Optional[tuple] = None
+        self._vl = None                        # varlen index of the fixed grid, for N > 512
 
     def params(self) -> List[torch.Tensor]:
         return list(self.mod.parameters())
 
-    def has_final_norm(self) -> bool:
-        """simple_flash_attn_vit.py's Transformer has no final LayerNorm (its head carries one instead)."""
-        return getattr(self.mod, "norm", None) is not None
-
     def unsupported_reason(self, N: int) -> Optional[str]:
-        for attn, ff in self._layers():
-            if attn.dim_head not in (64, 80):
-                return f"dim_head={attn.dim_head} (the attention kernels are built for 64 and 80)"
-            if attn.dim_head == 80 and (N > 512 or getattr(attn, "q_norm", None) is not None):
+        # only shapes are read, and a module's shapes are fixed at construction: any description of it serves
+        for L in self.layers or self.mod.encoder_layers()[0]:
+            if L.dim_head not in (64, 80):
+                return f"dim_head={L.dim_head} (the attention kernels are built for 64 and 80)"
+            if L.dim_head == 80 and (N > 512 or L.qk_norm is not None):
                 return "dim_head=80 is built for the single-pass attention kernel (N <= 512, no q/k norm) only"
-            if attn.dim % 8 or ff.hidden_dim % 8:
+            if L.qkv_w.shape[1] % 8 or L.fc1_w.shape[0] % 8:
                 return "dim / mlp_dim not multiples of 8"
         if N > 16384:
             return f"sequence length {N} > 16384"
@@ -210,71 +266,61 @@ class TransformerEngine:
         key = _version_key(params)
         if self.prep.key == key:
             return self.prep.t
+        layers, norm = self.mod.encoder_layers()
         t: Dict[str, torch.Tensor] = {}
-
-        def fold(prefix: str, lin_w: torch.Tensor, lin_b: Optional[torch.Tensor], g: torch.Tensor, b: torch.Tensor):
-            # LN(x) W^T + bias  ==  rstd * (x (gamma*W)^T - mu * colsum) + (W beta + bias)
-            w32 = lin_w.detach().float()
-            wg = (w32 * g.detach().float()[None, :]).to(torch.bfloat16).contiguous()
-            t[prefix + ".wg"] = wg
-            t[prefix + ".s"] = wg.float().sum(dim=1).contiguous()          # from the ROUNDED weights the MMA sees
-            tb = w32 @ b.detach().float()
-            t[prefix + ".t"] = (tb + lin_b.detach().float() if lin_b is not None else tb).contiguous()
-
-        for i, (attn, ff) in enumerate(self._layers()):
-            t[f"{i}.ln1.w"], t[f"{i}.ln1.b"] = _f32(attn.norm.weight), _f32(attn.norm.bias)
-            t[f"{i}.qkv.w"] = _bf16_rows(attn.to_qkv.weight)
-            fold(f"{i}.qkv", attn.to_qkv.weight, None, attn.norm.weight, attn.norm.bias)
-            fold(f"{i}.fc1", ff.parts()[1].weight, ff.parts()[1].bias, ff.parts()[0].weight, ff.parts()[0].bias)
-            out_lin = attn.out_linear() if getattr(attn, "project_out", True) else None
-            if out_lin is None:
+        for i, L in enumerate(layers):
+            t[f"{i}.ln1.w"], t[f"{i}.ln1.b"] = _f32(L.ln1.gamma), _f32(L.ln1.beta)
+            t[f"{i}.qkv.w"] = _bf16_rows(L.qkv_w)
+            _fold(t, f"{i}.qkv", L.qkv_w, None, L.ln1)
+            if L.qk_norm is not None:
+                # per-head q / k norm: epilogue of the QKV GEMM
+                t[f"{i}.gqk"] = torch.cat([_f32(g).reshape(-1) for g in L.qk_gamma])
+            if L.out_w is None:
                 # reference vit.py:34,46-49: heads == 1 and dim_head == dim -> to_out is nn.Identity.  The residual
                 # GEMM then runs with an identity weight: bf16 x 1.0 products accumulate exactly, so x += o bit for bit
-                t[f"{i}.out.w"] = torch.eye(attn.dim, device=attn.to_qkv.weight.device, dtype=torch.bfloat16)
-                t[f"{i}.out.b"] = None
+                t[f"{i}.out.w"] = torch.eye(L.qkv_w.shape[1], device=L.qkv_w.device, dtype=torch.bfloat16)
             else:
-                t[f"{i}.out.w"] = _bf16_rows(out_lin.weight)
-                t[f"{i}.out.b"] = _f32(out_lin.bias) if out_lin.bias is not None else None
-            if getattr(attn, "q_norm", None) is not None:
-                # per-head q / k RMSNorm (simple_vit_with_qk_norm.py:29-37,60-67): epilogue of the QKV GEMM
-                t[f"{i}.gqk"] = torch.cat([_f32(attn.q_norm.gamma).reshape(-1), _f32(attn.k_norm.gamma).reshape(-1)])
-            ln, fc1, fc2 = ff.parts()
-            t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(ln.weight), _f32(ln.bias)
-            t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(fc1.weight), _f32(fc1.bias)
-            t[f"{i}.fc2.w"], t[f"{i}.fc2.b"] = _bf16_rows(fc2.weight), _f32(fc2.bias)
-        if self.has_final_norm():
-            t["norm.w"], t["norm.b"] = _f32(self.mod.norm.weight), _f32(self.mod.norm.bias)
+                t[f"{i}.out.w"] = _bf16_rows(L.out_w)
+            t[f"{i}.out.b"] = _f32(L.out_b)
+            t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(L.ln2.gamma), _f32(L.ln2.beta)
+            _fold(t, f"{i}.fc1", L.fc1_w, L.fc1_b, L.ln2)
+            t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(L.fc1_w), _f32(L.fc1_b)
+            t[f"{i}.fc2.w"], t[f"{i}.fc2.b"] = _bf16_rows(L.fc2_w), _f32(L.fc2_b)
+        if norm is not None:
+            t["norm.w"], t["norm.b"] = _f32(norm.gamma), _f32(norm.beta)
+        self.layers, self.norm = layers, norm
         t["c_layers"] = self._c_layers(t)            # type: ignore[assignment]
         self.prep.key, self.prep.t = key, t
         return t
 
     def _c_layers(self, t: Dict[str, torch.Tensor]):
         """(ctypes array of b200vit_layer, heads, dh, hidden, scale) for the one-call encoder (b200vit_encoder_blocks),
-        or None when the layers are not uniform.  The pointers stay valid as long as `t` (which holds the tensors)."""
-        layers = list(self._layers())
-        a0, f0 = layers[0]
-        sig = (a0.heads, a0.dim_head, f0.hidden_dim, _softmax_scale(a0))
-        if any((a.heads, a.dim_head, f.hidden_dim, _softmax_scale(a)) != sig for a, f in layers):
+        or None when it cannot run these layers: they are not uniform, or one has a per-head LayerNorm (the one-call
+        encoder has no EPI_HEADLN).  The pointers stay valid as long as `t` (which holds the tensors)."""
+        sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.scale)      # noqa: E731
+        if any(L.qk_norm == "ln" or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
-        arr = (_lib.Layer * len(layers))()
+        arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
-        for i, (attn, ff) in enumerate(layers):
-            L = arr[i]
-            L.qkv_wg, L.qkv_t, L.qkv_s = p(t[f"{i}.qkv.wg"]), p(t[f"{i}.qkv.t"]), p(t[f"{i}.qkv.s"])
-            L.qk_gamma = p(t.get(f"{i}.gqk"))
-            L.out_w, L.out_b = p(t[f"{i}.out.w"]), p(t[f"{i}.out.b"])
-            L.fc1_wg, L.fc1_t, L.fc1_s = p(t[f"{i}.fc1.wg"]), p(t[f"{i}.fc1.t"]), p(t[f"{i}.fc1.s"])
-            L.fc2_w, L.fc2_b = p(t[f"{i}.fc2.w"]), p(t[f"{i}.fc2.b"])
-            L.ln1_eps, L.ln2_eps = float(attn.norm.eps), float(ff.parts()[0].eps)
-        return arr, sig
+        for i, L in enumerate(self.layers):
+            c = arr[i]
+            c.qkv_wg, c.qkv_t, c.qkv_s = p(t[f"{i}.qkv.wg"]), p(t[f"{i}.qkv.t"]), p(t[f"{i}.qkv.s"])
+            c.qk_gamma = p(t.get(f"{i}.gqk"))
+            c.out_w, c.out_b = p(t[f"{i}.out.w"]), p(t[f"{i}.out.b"])
+            c.fc1_wg, c.fc1_t, c.fc1_s = p(t[f"{i}.fc1.wg"]), p(t[f"{i}.fc1.t"]), p(t[f"{i}.fc1.s"])
+            c.fc2_w, c.fc2_b = p(t[f"{i}.fc2.w"]), p(t[f"{i}.fc2.b"])
+            c.ln1_eps, c.ln2_eps = float(L.ln1.eps), float(L.ln2.eps)
+        return arr, sig(self.layers[0])
 
     # -------------------------------------------------------------------------------------------- workspaces
     def workspace(self, M: int, device: torch.device) -> Dict[str, torch.Tensor]:
-        attn0, ff0 = next(iter(self._layers()))
-        D, I, Hd = attn0.dim, attn0.heads * attn0.dim_head, ff0.hidden_dim
-        # one workspace per (shape, stream): two streams running the same model must not share scratch buffers
-        key = (M, D, I, Hd, device, torch.cuda.current_stream(device).cuda_stream)
+        # one workspace per (rows, stream): two streams running the same model must not share scratch buffers.  The
+        # other dimensions are the module's own and do not change.
+        key = (M, device, torch.cuda.current_stream(device).cuda_stream)
         if self.ws_key != key:
+            self.prepared()
+            L = self.layers[0]
+            D, I, Hd = L.qkv_w.shape[1], L.heads * L.dim_head, L.fc1_w.shape[0]
             bf = dict(device=device, dtype=torch.bfloat16)
             self.ws = {
                 "xn": torch.empty(M, D, **bf),          # exact: LayerNorm output; fold: bf16 copy of x
@@ -293,78 +339,75 @@ class TransformerEngine:
         return self.ws
 
     # -------------------------------------------------------------------------------------------- execution
-    def _attention(self, ws: Dict[str, torch.Tensor], B: int, N: int, attn) -> None:
-        """Single-pass kernel for N <= 512 keys, the key-block (varlen) kernel beyond."""
+    def _varlen_args(self, B: int, N: int, varlen: Optional[_lib.VarlenIndex], device: torch.device):
+        """(cu_seqlens, tile_prefix, total_tiles) of the key-block (varlen) attention kernel, or None for the
+        single-pass kernel: a packed batch always takes the varlen kernel, a fixed (B, N) grid does beyond 512 keys."""
+        if varlen is not None:
+            return varlen.cu, varlen.tile_prefix, varlen.total_tiles
         if N <= 512:
-            _lib.attention(ws["qkv"], ws["o"], B, N, attn.heads, attn.dim_head, _softmax_scale(attn))
-            return
-        key = (B, N, ws["qkv"].device)
-        if getattr(self, "_vl_key", None) != key:
-            self._vl = _lib.varlen_index([N] * B, ws["qkv"].device)
-            self._vl_key = key
-        cu, tp, tiles = self._vl
-        _lib.attention_varlen(ws["qkv"], ws["o"], cu, tp, tiles, attn.heads, attn.dim_head, _softmax_scale(attn))
+            return None
+        key = (B, N, device)
+        if self._vl_key != key:
+            self._vl, self._vl_key = _lib.varlen_index([N] * B, device), key
+        return self._vl
 
-    def run_blocks(self, x: torch.Tensor, B: int, N: int, primed: bool = False) -> None:
-        """All encoder layers, in place on the fp32 residual stream x[B*N, D] (no final LayerNorm).
+    def run_blocks(self, x: torch.Tensor, B: int = 0, N: int = 0, primed: bool = False,
+                   varlen: Optional[_lib.VarlenIndex] = None) -> None:
+        """All encoder layers, in place on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
+        B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
-        the caller (embed_tokens) already wrote them, otherwise one rowstats_cast pass produces them."""
+        the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
         t = self.prepared()
-        M = B * N
-        ws = self.workspace(M, x.device)
-        if ln_mode() == "fold":
-            xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
-            if t["c_layers"] is not None and not _lib.profiling() and os.environ.get(_HOST_LOOP_ENV, "c") == "c":
-                # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
-                arr, (heads, dh, hidden, scale) = t["c_layers"]
-                varlen = None
-                if N > 512:
-                    key = (B, N, x.device)
-                    if getattr(self, "_vl_key", None) != key:
-                        self._vl = _lib.varlen_index([N] * B, x.device)
-                        self._vl_key = key
-                    varlen = self._vl
-                _lib.encoder_blocks(arr, len(arr), x, self.c_ws, B, N, x.shape[1], heads, dh, hidden, scale, primed,
-                                    varlen)
-                return
-            if not primed:
-                _lib.rowstats_cast(x, xb, ws["stats_in"])
-            for i, (attn, ff) in enumerate(self._layers()):
-                if f"{i}.gqk" in t:
-                    _lib.gemm_headnorm(xb, t[f"{i}.qkv.wg"], out_bf16=ws["qkv"], bias=t[f"{i}.qkv.t"],
-                                       ln_sums=ws["stats_in"] if i == 0 else sa, col_s=t[f"{i}.qkv.s"],
-                                       ln_eps=attn.norm.eps, head_gamma=t[f"{i}.gqk"], norm_heads=2 * attn.heads)
-                else:
-                    _lib.gemm(xb, t[f"{i}.qkv.wg"], out_bf16=ws["qkv"], bias=t[f"{i}.qkv.t"],
-                              ln_sums=ws["stats_in"] if i == 0 else sa, col_s=t[f"{i}.qkv.s"], ln_eps=attn.norm.eps)
-                self._attention(ws, B, N, attn)
+        ws = self.workspace(x.shape[0], x.device)
+        vl = self._varlen_args(B, N, varlen, x.device)
+        fold = ln_mode() == "fold"
+        if (fold and varlen is None and t["c_layers"] is not None and not _lib.profiling()
+                and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
+            # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
+            arr, (heads, dh, hidden, scale) = t["c_layers"]
+            _lib.encoder_blocks(arr, len(arr), x, self.c_ws, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl)
+            return
+        xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
+        if fold and not primed:
+            _lib.rowstats_cast(x, xb, ws["stats_in"])
+        for i, L in enumerate(self.layers):
+            # xb = LN1(x) -> qkv   (fold: xb already holds the bf16 copy of x; LN1 is applied in the GEMM epilogue)
+            if fold:
+                w, ln = t[f"{i}.qkv.wg"], dict(bias=t[f"{i}.qkv.t"], ln_sums=ws["stats_in"] if i == 0 else sa,
+                                               col_s=t[f"{i}.qkv.s"], ln_eps=L.ln1.eps)
+            else:
+                _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
+                w, ln = t[f"{i}.qkv.w"], {}
+            if L.qk_norm is None:
+                _lib.gemm(xb, w, out_bf16=ws["qkv"], **ln)
+            else:
+                _lib.gemm_headnorm(xb, w, out_bf16=ws["qkv"], head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads,
+                                   dh=L.dim_head, head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None, **ln)
+            if vl is None:
+                _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale)
+            else:
+                _lib.attention_varlen(ws["qkv"], ws["o"], *vl, L.heads, L.dim_head, L.scale)
+            if fold:
+                # the residual GEMMs also write the bf16 copy of x and its row statistics for the next folded GEMM
                 _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.out.b"], resid=x,
                           stats_out=sb)
                 _lib.gemm(xb, t[f"{i}.fc1.wg"], out_bf16=ws["h"], bias=t[f"{i}.fc1.t"], gelu=True, ln_sums=sb,
-                          col_s=t[f"{i}.fc1.s"], ln_eps=ff.parts()[0].eps)
+                          col_s=t[f"{i}.fc1.s"], ln_eps=L.ln2.eps)
                 _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.fc2.b"], resid=x,
                           stats_out=sa)
-            return
-        for i, (attn, ff) in enumerate(self._layers()):
-            _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=ws["xn"], eps=attn.norm.eps)
-            if f"{i}.gqk" in t:
-                _lib.gemm_headnorm(ws["xn"], t[f"{i}.qkv.w"], out_bf16=ws["qkv"], head_gamma=t[f"{i}.gqk"],
-                                   norm_heads=2 * attn.heads)
             else:
-                _lib.gemm(ws["xn"], t[f"{i}.qkv.w"], out_bf16=ws["qkv"])
-            self._attention(ws, B, N, attn)
-            _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
-            _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=ws["xn"], eps=ff.parts()[0].eps)
-            _lib.gemm(ws["xn"], t[f"{i}.fc1.w"], out_bf16=ws["h"], bias=t[f"{i}.fc1.b"], gelu=True)
-            _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, bias=t[f"{i}.fc2.b"], resid=x)
+                _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
+                _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=xb, eps=L.ln2.eps)
+                _lib.gemm(xb, t[f"{i}.fc1.w"], out_bf16=ws["h"], bias=t[f"{i}.fc1.b"], gelu=True)
+                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, bias=t[f"{i}.fc2.b"], resid=x)
 
     def final_norm(self, x: torch.Tensor, *, out_bf16: Optional[torch.Tensor] = None,
                    out_f32: Optional[torch.Tensor] = None, row_index: Optional[torch.Tensor] = None) -> None:
         t = self.prepared()
-        assert self.has_final_norm()
+        assert self.norm is not None
         _lib.layernorm(x, t["norm.w"], t["norm.b"], out_bf16=out_bf16, out_f32=out_f32, row_index=row_index,
-                       eps=self.mod.norm.eps)
+                       eps=self.norm.eps)
 
     def forward_tokens(self, tokens: torch.Tensor) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
@@ -374,7 +417,7 @@ class TransformerEngine:
             x = tokens.reshape(B * N, D).float().contiguous()
             self.run_blocks(x, B, N)
             out = torch.empty(B * N, D, device=tokens.device, dtype=torch.bfloat16)
-            if self.has_final_norm():
+            if self.norm is not None:
                 self.final_norm(x, out_bf16=out)
             else:
                 _lib.cast_f32_bf16(x.view(-1), out.view(-1))
@@ -503,13 +546,34 @@ class HeadEngine:
         params = self.params()
         key = _version_key(params)
         if self.prep.key != key:
-            self.prep.t = {"w": _bf16_rows(self.lin.weight),
-                           "b": _f32(self.lin.bias) if self.lin.bias is not None else None}
+            self.prep.t = {"w": _bf16_rows(self.lin.weight), "b": _f32(self.lin.bias)}
             self.prep.key = key
         t = self.prep.t
         out = torch.empty(pooled_bf16.shape[0], t["w"].shape[0], device=pooled_bf16.device, dtype=torch.bfloat16)
         _lib.gemm(pooled_bf16.contiguous(), t["w"], out_bf16=out, bias=t["b"])
         return out
+
+
+def patch_engine(owner: nn.Module) -> PatchEmbedEngine:
+    """The owner's PatchEmbedEngine, made on first use."""
+    if getattr(owner, "_patch_engine", None) is None:
+        owner._patch_engine = PatchEmbedEngine(owner)
+    return owner._patch_engine
+
+
+def fused_encode(owner: nn.Module, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None,
+                 pos: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, int, int]:
+    """Patch embedding -> encoder blocks of the single-image models: (x, B, N) with x the fp32 residual stream
+    [B*N, D] after the last layer, before the final LayerNorm.  In fold mode the patch embedding also writes the
+    engine's bf16 copy of x and its row statistics, which the first layer reads.  Must run inside on_device(img)."""
+    pe, eng = patch_engine(owner), owner.transformer.engine()
+    B, N = pe.geometry(img, patch)
+    primed = ln_mode() == "fold"
+    ws = eng.workspace(B * N, img.device) if primed else None
+    x, B, N = pe.run(img, xb=ws["xn"] if primed else None, stats=ws["stats_in"] if primed else None,
+                     patch=patch, pos=pos)
+    eng.run_blocks(x, B, N, primed=primed)
+    return x, B, N
 
 
 def fused_mean_pooled_features(owner: nn.Module, img: torch.Tensor, pool_tokens: Optional[int] = None,
@@ -519,23 +583,16 @@ def fused_mean_pooled_features(owner: nn.Module, img: torch.Tensor, pool_tokens:
     patch embedding (+ register tokens) -> encoder blocks -> final LayerNorm if the Transformer has one -> mean over
     the first `pool_tokens` tokens of every image (all tokens by default).  Returns fp32 [B, D]; must run inside
     on_device(img)."""
-    if getattr(owner, "_patch_engine", None) is None:
-        owner._patch_engine = PatchEmbedEngine(owner)
-    eng = owner.transformer.engine()
-    B, N = owner._patch_engine.geometry(img, patch)
     if transformer_is_hooked(owner):
-        x, B, N = owner._patch_engine.run(img, patch=patch, pos=pos)
+        x, B, N = patch_engine(owner).run(img, patch=patch, pos=pos)
         xf = hooked_transformer_tokens(owner, x, B, N).reshape(B * N, -1).float()
         pm = torch.empty(B, xf.shape[1], device=img.device, dtype=torch.float32)
         _lib.mean_pool(xf, pm, B, N, xf.shape[1], n_pool=pool_tokens)
         return pm
-    primed = ln_mode() == "fold"
-    ws = eng.workspace(B * N, img.device) if primed else None
-    x, B, N = owner._patch_engine.run(img, xb=ws["xn"] if primed else None, stats=ws["stats_in"] if primed else None,
-                                      patch=patch, pos=pos)
+    x, B, N = fused_encode(owner, img, patch=patch, pos=pos)
     D = x.shape[1]
-    eng.run_blocks(x, B, N, primed=primed)
-    if eng.has_final_norm():
+    eng = owner.transformer.engine()
+    if eng.norm is not None:
         xf = torch.empty_like(x)
         eng.final_norm(x, out_f32=xf)
     else:

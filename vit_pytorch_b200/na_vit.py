@@ -18,14 +18,15 @@ Two executions of the same arithmetic:
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, List, Optional, Sequence, Union
+from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 import torch.nn.functional as F
 from torch import Tensor, nn
 
 from . import _lib
-from .engine import FusedWeightsMixin, _version_key, hooks_inside, ln_mode, on_device, why_not_fused
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, hooks_inside, ln_mode,
+                     on_device, why_not_fused)
 
 
 def group_images_by_max_seq_len(images: Sequence[Tensor], patch_size: int,
@@ -117,7 +118,13 @@ class Attention(nn.Module):
         return self.to_out(out.transpose(1, 2).reshape(b, n, -1))
 
 
-class Transformer(nn.Module):
+def _norm(ln: LayerNorm) -> Norm:
+    """beta = None: the fused path assumes the zero `beta` buffer the reference registers (NaViT._nonzero_beta checks
+    it); eps is that of F.layer_norm, which LayerNorm.forward uses."""
+    return Norm(ln.gamma, None, 1e-5)
+
+
+class Transformer(FusedEncoder, nn.Module):
     def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int, dropout: float = 0.) -> None:
         super().__init__()
         self.layers = nn.ModuleList([])
@@ -127,6 +134,17 @@ class Transformer(nn.Module):
                 FeedForward(dim, mlp_dim, dropout=dropout),
             ]))
         self.norm = LayerNorm(dim)
+
+    def encoder_layers(self) -> Tuple[List[EncoderLayer], Norm]:
+        layers = []
+        for attn, ff in self.layers:
+            layers.append(EncoderLayer(
+                ln1=_norm(attn.norm), qkv_w=torch.cat([attn.to_q.weight, attn.to_kv.weight], dim=0),
+                out_w=attn.to_out[0].weight, out_b=attn.to_out[0].bias,
+                ln2=_norm(ff[0]), fc1_w=ff[1].weight, fc1_b=ff[1].bias, fc2_w=ff[4].weight, fc2_b=ff[4].bias,
+                heads=attn.heads, dim_head=attn.to_q.weight.shape[0] // attn.heads, scale=1.0,
+                qk_norm="rms", qk_gamma=(attn.q_norm.gamma, attn.k_norm.gamma)))
+        return layers, _norm(self.norm)
 
     def forward(self, x: Tensor, mask: Optional[Tensor] = None, attn_mask: Optional[Tensor] = None) -> Tensor:
         for attn, ff in self.layers:
@@ -210,7 +228,9 @@ class NaViT(FusedWeightsMixin, nn.Module):
         return self._beta_nonzero
 
     def _prepared(self) -> Dict[str, Tensor]:
-        params = list(self.parameters())
+        """Device copies of the patch-embedding, positional, pooling and head weights (the encoder layers are the
+        transformer engine's)."""
+        params = [p for n, p in self.named_parameters() if not n.startswith("transformer.")]
         key = _version_key(params)
         if getattr(self, "_prep_key", None) == key:
             return self._prep
@@ -220,33 +240,11 @@ class NaViT(FusedWeightsMixin, nn.Module):
         pe = self.to_patch_embedding
         t["pe.ln1"], t["pe.w"], t["pe.b"], t["pe.ln2"] = f32(pe[0].gamma), bf(pe[1].weight), f32(pe[1].bias), f32(pe[2].gamma)
         t["pos_h"], t["pos_w"] = f32(self.pos_embed_height), f32(self.pos_embed_width)
-
-        def attn_w(prefix: str, a: Attention) -> None:
-            t[prefix + "ln"] = f32(a.norm.gamma)
-            t[prefix + "qkv"] = bf(torch.cat([a.to_q.weight, a.to_kv.weight], dim=0))       # rows: q | k | v
-            t[prefix + "kv"] = bf(a.to_kv.weight)
-            t[prefix + "gqk"] = torch.cat([f32(a.q_norm.gamma).reshape(-1), f32(a.k_norm.gamma).reshape(-1)]).contiguous()
-            t[prefix + "gk"] = f32(a.k_norm.gamma).reshape(-1).contiguous()
-            t[prefix + "out"] = bf(a.to_out[0].weight)
-
-        def fold(name: str, w: Tensor, gamma: Tensor) -> None:
-            # LN(x; gamma, beta = 0) W^T == rstd * (x (gamma * W)^T - mu * colsum): see engine.TransformerEngine
-            wg = (w.detach().float() * gamma.detach().float()[None, :]).to(torch.bfloat16).contiguous()
-            t[name + "g"] = wg
-            t[name + "s"] = wg.float().sum(dim=1).contiguous()       # from the ROUNDED weights the MMA sees
-
-        for i, (attn, ff) in enumerate(self.transformer.layers):
-            attn_w(f"{i}.a.", attn)
-            fold(f"{i}.a.qkv", torch.cat([attn.to_q.weight, attn.to_kv.weight], dim=0), attn.norm.gamma)
-            t[f"{i}.a.qkvt"] = torch.zeros(t[f"{i}.a.qkvs"].shape[0], device=t[f"{i}.a.qkvs"].device)
-            fold(f"{i}.f.w1", ff[1].weight, ff[0].gamma)
-            t[f"{i}.f.ln"] = f32(ff[0].gamma)
-            t[f"{i}.f.w1"], t[f"{i}.f.b1"] = bf(ff[1].weight), f32(ff[1].bias)
-            t[f"{i}.f.w2"], t[f"{i}.f.b2"] = bf(ff[4].weight), f32(ff[4].bias)
-        t["norm"] = f32(self.transformer.norm.gamma)
-        attn_w("pool.", self.attn_pool)
         # the pooling query is the same for every image: LayerNorm -> to_q -> per-head RMSNorm, once per weight version
         pool = self.attn_pool
+        t["pool.kv"] = bf(pool.to_kv.weight)
+        t["pool.gk"] = f32(pool.k_norm.gamma).reshape(-1).contiguous()
+        t["pool.out"] = bf(pool.to_out[0].weight)
         qv = self.attn_pool_queries.detach().float()
         qn = F.layer_norm(qv, qv.shape, pool.norm.gamma.detach().float(), None)
         qh = (pool.to_q.weight.detach().float() @ qn).reshape(pool.heads, -1)
@@ -263,11 +261,12 @@ class NaViT(FusedWeightsMixin, nn.Module):
             batched_images = [batched_images]
         images = [im for row in batched_images for im in row]        # output order of the reference: row major
         t = self._prepared()
+        eng = self.transformer.engine()
         dev = images[0].device
         p, c = self.patch_size, self.channels
         heads = self.attn_pool.heads
         D = t["pos_h"].shape[1]
-        I = t["0.a.out"].shape[1]
+        I = t["pool.out"].shape[1]
         max_gh, max_gw = self.pos_embed_height.shape[0], self.pos_embed_width.shape[0]
         for img in images:
             assert img.ndim == 3 and img.shape[0] == c
@@ -292,38 +291,13 @@ class NaViT(FusedWeightsMixin, nn.Module):
         y = torch.empty(T, D, **f32)
         _lib.gemm(a0, t["pe.w"], out_f32=y, bias=t["pe.b"])
         x = torch.empty_like(y)
-        xn = torch.empty(T, D, **bf16)              # exact: LayerNorm output; fold: bf16 copy of the residual stream
-        st_in = torch.empty(T, 1, 2, **f32) if fold else None
-        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=xn if fold else None, stats=st_in)
+        ws = eng.workspace(T, dev)     # fold: the embedding writes the bf16 copy of x and its row sums for layer 0
+        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=ws["xn"] if fold else None,
+                          stats=ws["stats_in"] if fold else None)
         # ---- encoder layers on the packed [T, D] matrix                                     (na_vit.py:183-193)
-        qkv = torch.empty(T, 3 * I, **bf16)
-        o = torch.empty(T, I, **bf16)
-        hbuf = torch.empty(T, t["0.f.w1"].shape[0], **bf16)
-        depth = len(self.transformer.layers)
-        if fold:
-            # LayerNorm folded into the QKV / FC1 GEMMs (engine.py): the residual GEMMs emit the bf16 copy of x and
-            # the partial row statistics the next folded GEMM needs
-            parts = _lib.stats_parts(D)
-            sa, sb = torch.empty(T, parts, 2, **f32), torch.empty(T, parts, 2, **f32)
-            for i in range(depth):
-                _lib.gemm_headnorm(xn, t[f"{i}.a.qkvg"], out_bf16=qkv, bias=t[f"{i}.a.qkvt"],
-                                   ln_sums=st_in if i == 0 else sa, col_s=t[f"{i}.a.qkvs"],
-                                   head_gamma=t[f"{i}.a.gqk"], norm_heads=2 * heads)   # q / k RMSNorm in the epilogue
-                _lib.attention_varlen(qkv, o, ix.cu, ix.tile_prefix, ix.total_tiles, heads, 64, 1.0)
-                _lib.gemm(o, t[f"{i}.a.out"], out_f32=x, out_bf16=xn, resid=x, stats_out=sb)
-                _lib.gemm(xn, t[f"{i}.f.w1g"], out_bf16=hbuf, bias=t[f"{i}.f.b1"], gelu=True, ln_sums=sb,
-                          col_s=t[f"{i}.f.w1s"])
-                _lib.gemm(hbuf, t[f"{i}.f.w2"], out_f32=x, out_bf16=xn, bias=t[f"{i}.f.b2"], resid=x, stats_out=sa)
-        else:
-            for i in range(depth):
-                _lib.layernorm(x, t[f"{i}.a.ln"], None, out_bf16=xn)
-                _lib.gemm_headnorm(xn, t[f"{i}.a.qkv"], out_bf16=qkv, head_gamma=t[f"{i}.a.gqk"], norm_heads=2 * heads)
-                _lib.attention_varlen(qkv, o, ix.cu, ix.tile_prefix, ix.total_tiles, heads, 64, 1.0)
-                _lib.gemm(o, t[f"{i}.a.out"], out_f32=x, resid=x)
-                _lib.layernorm(x, t[f"{i}.f.ln"], None, out_bf16=xn)
-                _lib.gemm(xn, t[f"{i}.f.w1"], out_bf16=hbuf, bias=t[f"{i}.f.b1"], gelu=True)
-                _lib.gemm(hbuf, t[f"{i}.f.w2"], out_f32=x, bias=t[f"{i}.f.b2"], resid=x)
-        _lib.layernorm(x, t["norm"], None, out_bf16=xn)
+        eng.run_blocks(x, primed=fold, varlen=ix)
+        xn = ws["xn"]
+        eng.final_norm(x, out_bf16=xn)
         # ---- attention pooling: one query per image over that image's (un-normalised-again) tokens (na_vit.py:371-387)
         kv = torch.empty(T, 2 * I, **bf16)
         _lib.gemm_headnorm(xn, t["pool.kv"], out_bf16=kv, head_gamma=t["pool.gk"], norm_heads=heads)   # k half only

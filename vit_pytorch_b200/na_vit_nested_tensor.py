@@ -17,14 +17,15 @@ Two executions of the same arithmetic:
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
 from torch import Tensor, nn
 
 from . import _lib
-from .engine import FusedWeightsMixin, _version_key, hooks_inside, ln_mode, on_device, why_not_fused
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, hooks_inside, ln_mode,
+                     on_device, why_not_fused)
 
 
 def FeedForward(dim: int, hidden_dim: int, dropout: float = 0.) -> nn.Sequential:
@@ -59,7 +60,7 @@ class Attention(nn.Module):
         return self.to_out(out.transpose(-3, -2).flatten(-2))
 
 
-class Transformer(nn.Module):
+class Transformer(FusedEncoder, nn.Module):
     def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int, dropout: float = 0.,
                  qk_norm: bool = True) -> None:
         super().__init__()
@@ -70,6 +71,22 @@ class Transformer(nn.Module):
                 FeedForward(dim, mlp_dim, dropout=dropout),
             ]))
         self.norm = nn.LayerNorm(dim, bias=False)
+
+    def encoder_layers(self) -> Tuple[List[EncoderLayer], Norm]:
+        layers = []
+        for attn, ff in self.layers:
+            h, dh = attn.heads, attn.dim_head
+            qk_ln = not isinstance(attn.query_norm, nn.Identity)   # one LayerNorm(dim_head) shared by all heads
+            layers.append(EncoderLayer(
+                ln1=Norm.of(attn.norm),
+                qkv_w=torch.cat([attn.to_queries.weight, attn.to_keys.weight, attn.to_values.weight], dim=0),
+                out_w=attn.to_out.weight, out_b=attn.to_out.bias,
+                ln2=Norm.of(ff[0]), fc1_w=ff[1].weight, fc1_b=ff[1].bias, fc2_w=ff[4].weight, fc2_b=ff[4].bias,
+                heads=h, dim_head=dh, scale=dh ** -0.5,
+                qk_norm="ln" if qk_ln else None,
+                qk_gamma=(attn.query_norm.weight.expand(h, dh), attn.key_norm.weight.expand(h, dh)) if qk_ln else (),
+                qk_eps=attn.query_norm.eps if qk_ln else 0.0))
+        return layers, Norm.of(self.norm)
 
     def forward(self, x: Tensor) -> Tensor:
         for attn, ff in self.layers:
@@ -179,7 +196,9 @@ class NaViT(FusedWeightsMixin, nn.Module):
         return r
 
     def _prepared(self) -> Dict[str, Tensor]:
-        params = list(self.parameters())
+        """Device copies of the patch-embedding, positional, pooling and head weights (the encoder layers are the
+        transformer engine's)."""
+        params = [p for n, p in self.named_parameters() if not n.startswith("transformer.")]
         key = _version_key(params)
         if getattr(self, "_prep_key", None) == key:
             return self._prep
@@ -194,34 +213,10 @@ class NaViT(FusedWeightsMixin, nn.Module):
         t["pe.ln2"] = f32(ln2.weight)
         t["pos_h"] = (self.pos_embed_height.detach().float() + ln2.bias.detach().float()[None, :]).contiguous()
         t["pos_w"] = f32(self.pos_embed_width)
-
-        def fold(name: str, w: Tensor, gamma: Tensor) -> None:
-            wg = (w.detach().float() * gamma.detach().float()[None, :]).to(torch.bfloat16).contiguous()
-            t[name + "g"] = wg
-            t[name + "s"] = wg.float().sum(dim=1).contiguous()
-
-        def head_gamma(a: Attention, which) -> Optional[Tensor]:
-            mods = [getattr(a, n) for n in which]
-            if isinstance(mods[0], nn.Identity):
-                return None
-            return torch.cat([f32(m.weight).repeat(a.heads) for m in mods]).contiguous()   # same gamma for every head
-
-        for i, (attn, ff) in enumerate(self.transformer.layers):
-            w = torch.cat([attn.to_queries.weight, attn.to_keys.weight, attn.to_values.weight], dim=0)
-            t[f"{i}.qkv"] = bf(w)
-            fold(f"{i}.qkv", w, attn.norm.weight)
-            t[f"{i}.qkvt"] = torch.zeros(w.shape[0], device=w.device)
-            t[f"{i}.ln1"] = f32(attn.norm.weight)
-            t[f"{i}.gqk"] = head_gamma(attn, ("query_norm", "key_norm"))
-            t[f"{i}.out"] = bf(attn.to_out.weight)
-            fold(f"{i}.w1", ff[1].weight, ff[0].weight)
-            t[f"{i}.ln2"] = f32(ff[0].weight)
-            t[f"{i}.w1"], t[f"{i}.b1"] = bf(ff[1].weight), f32(ff[1].bias)
-            t[f"{i}.w2"], t[f"{i}.b2"] = bf(ff[4].weight), f32(ff[4].bias)
-        t["norm"] = f32(self.transformer.norm.weight)
         pool = self.attn_pool
         t["pool.kv"] = bf(torch.cat([pool.to_keys.weight, pool.to_values.weight], dim=0))
-        t["pool.gk"] = head_gamma(pool, ("key_norm",))
+        t["pool.gk"] = (None if isinstance(pool.key_norm, nn.Identity)
+                        else f32(pool.key_norm.weight).repeat(pool.heads).contiguous())    # same gamma for every head
         t["pool.out"] = bf(pool.to_out.weight)
         # the pooling query is the same for every image: LayerNorm -> to_queries -> per-head LayerNorm, times the
         # softmax scale dim_head ** -0.5 (the pooling kernel uses scale 1)
@@ -239,6 +234,7 @@ class NaViT(FusedWeightsMixin, nn.Module):
     def forward_fused(self, images: List[Tensor]) -> Tensor:
         self._check(images)
         t = self._prepared()
+        eng = self.transformer.engine()
         dev = images[0].device
         p, c = self.patch_size, self.channels
         pool = self.attn_pool
@@ -259,54 +255,19 @@ class NaViT(FusedWeightsMixin, nn.Module):
         bf16 = dict(device=dev, dtype=torch.bfloat16)
         f32 = dict(device=dev, dtype=torch.float32)
         fold = ln_mode() == "fold"
-        scale = dh ** -0.5
-        lyr = self.transformer.layers
         # ---- patch embedding (reference :186-192,226-262)
         a0 = torch.empty(T, c * p * p, **bf16)
         _lib.patchify_varlen_ln(images, t["pe.ln1"], a0, ix.cu, p, eps=self.to_patch_embedding[0].eps, index=ix)
         y = torch.empty(T, D, **f32)
         _lib.gemm(a0, t["pe.w"], out_f32=y, bias=t["pe.b"])
         x = torch.empty_like(y)
-        xn = torch.empty(T, D, **bf16)
-        st_in = torch.empty(T, 1, 2, **f32) if fold else None
-        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=xn if fold else None, stats=st_in,
-                          eps=self.to_patch_embedding[2].eps)
+        ws = eng.workspace(T, dev)     # fold: the embedding writes the bf16 copy of x and its row sums for layer 0
+        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=ws["xn"] if fold else None,
+                          stats=ws["stats_in"] if fold else None, eps=self.to_patch_embedding[2].eps)
         # ---- encoder layers on the packed [T, D] matrix (reference :121-132)
-        qkv = torch.empty(T, 3 * I, **bf16)
-        o = torch.empty(T, I, **bf16)
-        hbuf = torch.empty(T, t["0.w1"].shape[0], **bf16)
-        parts = _lib.stats_parts(D)
-        sa, sb = (torch.empty(T, parts, 2, **f32), torch.empty(T, parts, 2, **f32)) if fold else (None, None)
-        for i, (attn, ff) in enumerate(lyr):
-            gqk = t[f"{i}.gqk"]
-            hln = None if gqk is None else attn.query_norm.eps
-            if fold:
-                kw = dict(out_bf16=qkv, bias=t[f"{i}.qkvt"], ln_sums=st_in if i == 0 else sa, col_s=t[f"{i}.qkvs"],
-                          ln_eps=attn.norm.eps)
-                if gqk is None:
-                    _lib.gemm(xn, t[f"{i}.qkvg"], **kw)
-                else:
-                    _lib.gemm_headnorm(xn, t[f"{i}.qkvg"], head_gamma=gqk, norm_heads=2 * heads,
-                                       head_layernorm_eps=hln, **kw)
-            else:
-                _lib.layernorm(x, t[f"{i}.ln1"], None, out_bf16=xn, eps=attn.norm.eps)
-                if gqk is None:
-                    _lib.gemm(xn, t[f"{i}.qkv"], out_bf16=qkv)
-                else:
-                    _lib.gemm_headnorm(xn, t[f"{i}.qkv"], out_bf16=qkv, head_gamma=gqk, norm_heads=2 * heads,
-                                       head_layernorm_eps=hln)
-            _lib.attention_varlen(qkv, o, ix.cu, ix.tile_prefix, ix.total_tiles, heads, dh, scale)
-            if fold:
-                _lib.gemm(o, t[f"{i}.out"], out_f32=x, out_bf16=xn, resid=x, stats_out=sb)
-                _lib.gemm(xn, t[f"{i}.w1g"], out_bf16=hbuf, bias=t[f"{i}.b1"], gelu=True, ln_sums=sb,
-                          col_s=t[f"{i}.w1s"], ln_eps=ff[0].eps)
-                _lib.gemm(hbuf, t[f"{i}.w2"], out_f32=x, out_bf16=xn, bias=t[f"{i}.b2"], resid=x, stats_out=sa)
-            else:
-                _lib.gemm(o, t[f"{i}.out"], out_f32=x, resid=x)
-                _lib.layernorm(x, t[f"{i}.ln2"], None, out_bf16=xn, eps=ff[0].eps)
-                _lib.gemm(xn, t[f"{i}.w1"], out_bf16=hbuf, bias=t[f"{i}.b1"], gelu=True)
-                _lib.gemm(hbuf, t[f"{i}.w2"], out_f32=x, bias=t[f"{i}.b2"], resid=x)
-        _lib.layernorm(x, t["norm"], None, out_bf16=xn, eps=self.transformer.norm.eps)
+        eng.run_blocks(x, primed=fold, varlen=ix)
+        xn = ws["xn"]
+        eng.final_norm(x, out_bf16=xn)
         # ---- attention pooling, one query per image, no residual (reference :284-296)
         kv = torch.empty(T, 2 * I, **bf16)
         if t["pool.gk"] is None:

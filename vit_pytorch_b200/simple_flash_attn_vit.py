@@ -15,11 +15,10 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib
-from .engine import (FusedWeightsMixin, HeadEngine, TransformerEngine, fused_mean_pooled_features, hooks_inside,
-                     on_device, why_not_fused)
+from .engine import FusedWeightsMixin, HeadEngine, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
 from .simple_vit import FeedForward, posemb_sincos_2d
 from .simple_vit_with_patch_dropout import GridPatchify
-from .vit import pair
+from .vit import FusedTransformer, pair
 
 
 class Attend(nn.Module):
@@ -38,17 +37,13 @@ class Attention(nn.Module):
     def __init__(self, dim: int, heads: int = 8, dim_head: int = 64, use_flash: bool = True) -> None:
         super().__init__()
         inner_dim = dim_head * heads
-        self.dim, self.dim_head = dim, dim_head
-        self.project_out = True
+        self.dim_head = dim_head
         self.heads = heads
         self.scale = dim_head ** -0.5
         self.norm = nn.LayerNorm(dim)
         self.attend = Attend(use_flash=use_flash)
         self.to_qkv = nn.Linear(dim, inner_dim * 3, bias=False)
         self.to_out = nn.Linear(inner_dim, dim, bias=False)
-
-    def out_linear(self) -> nn.Linear:
-        return self.to_out
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         b, n, _ = x.shape
@@ -57,47 +52,17 @@ class Attention(nn.Module):
         return self.to_out(out.permute(0, 2, 1, 3).reshape(b, n, -1))
 
 
-class Transformer(FusedWeightsMixin, nn.Module):
+class Transformer(FusedTransformer):
     """No final LayerNorm (reference :117-131)."""
 
     def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int, use_flash: bool) -> None:
         super().__init__()
-        self.dropout_p = 0.0
         self.layers = nn.ModuleList([])
         for _ in range(depth):
             self.layers.append(nn.ModuleList([
                 Attention(dim, heads=heads, dim_head=dim_head, use_flash=use_flash),
                 FeedForward(dim, mlp_dim),
             ]))
-        self._engine: Optional[TransformerEngine] = None
-
-    def engine(self) -> TransformerEngine:
-        if self._engine is None:
-            self._engine = TransformerEngine(self)
-        return self._engine
-
-    def fused_reason(self, x: torch.Tensor) -> Optional[str]:
-        if len(self.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), x, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self):
-            r = "forward hooks registered inside the transformer"
-        if r is None and x.dim() != 3:
-            r = "input is not (B, N, D)"
-        if r is None:
-            r = self.engine().unsupported_reason(x.shape[1])
-        return r
-
-    def forward_eager(self, x: torch.Tensor) -> torch.Tensor:
-        for attn, ff in self.layers:
-            x = attn(x) + x
-            x = ff(x) + x
-        return x
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.fused_reason(x) is None:
-            return self.engine().forward_tokens(x)
-        return self.forward_eager(x)
 
 
 class SimpleViT(FusedWeightsMixin, nn.Module):

@@ -14,9 +14,9 @@ import torch
 from torch import nn
 
 from . import _lib
-from .engine import (FusedWeightsMixin, HeadEngine, PatchEmbedEngine, TransformerEngine, fused_mean_pooled_features,
-                     hooks_inside, ln_mode, on_device, transformer_is_hooked, why_not_fused)
-from .vit import Patchify, pair
+from .engine import (FusedWeightsMixin, HeadEngine, PatchEmbedEngine, fused_mean_pooled_features, hooks_inside,
+                     on_device, why_not_fused)
+from .vit import FusedTransformer, Patchify, pair
 
 
 def posemb_sincos_2d(h: int, w: int, dim: int, temperature: int = 10000, dtype=torch.float32) -> torch.Tensor:
@@ -34,16 +34,12 @@ def posemb_sincos_2d(h: int, w: int, dim: int, temperature: int = 10000, dtype=t
 class FeedForward(nn.Module):
     def __init__(self, dim: int, hidden_dim: int) -> None:
         super().__init__()
-        self.dim, self.hidden_dim = dim, hidden_dim
         self.net = nn.Sequential(
             nn.LayerNorm(dim),
             nn.Linear(dim, hidden_dim),
             nn.GELU(),
             nn.Linear(hidden_dim, dim),
         )
-
-    def parts(self):
-        return self.net[0], self.net[1], self.net[3]
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return self.net(x)
@@ -53,17 +49,13 @@ class Attention(nn.Module):
     def __init__(self, dim: int, heads: int = 8, dim_head: int = 64) -> None:
         super().__init__()
         inner_dim = dim_head * heads
-        self.dim, self.dim_head = dim, dim_head
-        self.project_out = True
+        self.dim_head = dim_head
         self.heads = heads
         self.scale = dim_head ** -0.5
         self.norm = nn.LayerNorm(dim)
         self.attend = nn.Softmax(dim=-1)
         self.to_qkv = nn.Linear(dim, inner_dim * 3, bias=False)
         self.to_out = nn.Linear(inner_dim, dim, bias=False)
-
-    def out_linear(self) -> nn.Linear:
-        return self.to_out
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         b, n, _ = x.shape
@@ -74,10 +66,9 @@ class Attention(nn.Module):
         return self.to_out(out)
 
 
-class Transformer(FusedWeightsMixin, nn.Module):
+class Transformer(FusedTransformer):
     def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int) -> None:
         super().__init__()
-        self.dropout_p = 0.0
         self.norm = nn.LayerNorm(dim)
         self.layers = nn.ModuleList([])
         for _ in range(depth):
@@ -85,35 +76,6 @@ class Transformer(FusedWeightsMixin, nn.Module):
                 Attention(dim, heads=heads, dim_head=dim_head),
                 FeedForward(dim, mlp_dim),
             ]))
-        self._engine: Optional[TransformerEngine] = None
-
-    def engine(self) -> TransformerEngine:
-        if self._engine is None:
-            self._engine = TransformerEngine(self)
-        return self._engine
-
-    def fused_reason(self, x: torch.Tensor) -> Optional[str]:
-        if len(self.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), x, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self):
-            r = "forward hooks registered inside the transformer"
-        if r is None and x.dim() != 3:
-            r = "input is not (B, N, D)"
-        if r is None:
-            r = self.engine().unsupported_reason(x.shape[1])
-        return r
-
-    def forward_eager(self, x: torch.Tensor) -> torch.Tensor:
-        for attn, ff in self.layers:
-            x = attn(x) + x
-            x = ff(x) + x
-        return self.norm(x)
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.fused_reason(x) is None:
-            return self.engine().forward_tokens(x)
-        return self.forward_eager(x)
 
 
 class SimpleViT(FusedWeightsMixin, nn.Module):
@@ -179,26 +141,8 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         return self.linear_head(self.to_latent(x))
 
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
-        if self._patch_engine is None:
-            self._patch_engine = PatchEmbedEngine(self)
-        eng = self.transformer.engine()
-        dev = img.device
-        if transformer_is_hooked(self):                # Extractor-style hook on .transformer: tokens through the module
-            pm = fused_mean_pooled_features(self, img)
-            B, D = pm.shape
-        else:
-            B, N = self._patch_engine.geometry(img)
-            primed = ln_mode() == "fold"
-            ws = eng.workspace(B * N, img.device) if primed else None
-            x, B, N = self._patch_engine.run(img, xb=ws["xn"] if primed else None,
-                                             stats=ws["stats_in"] if primed else None)
-            D = x.shape[1]
-            eng.run_blocks(x, B, N, primed=primed)
-            xf = torch.empty_like(x)
-            eng.final_norm(x, out_f32=xf)
-            pm = torch.empty(B, D, device=dev, dtype=torch.float32)
-            _lib.mean_pool(xf, pm, B, N, D)
-        pooled = torch.empty(B, D, device=dev, dtype=torch.bfloat16)
+        pm = fused_mean_pooled_features(self, img)
+        pooled = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
         _lib.cast_f32_bf16(pm, pooled)
         pooled = self.to_latent(pooled)
         if self._head_engine is None:

@@ -17,10 +17,9 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib
-from .engine import (FusedWeightsMixin, TransformerEngine, fused_mean_pooled_features, hooks_inside, on_device,
-                     why_not_fused)
+from .engine import FusedWeightsMixin, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
 from .simple_vit import FeedForward, posemb_sincos_2d
-from .vit import Patchify, pair
+from .vit import FusedTransformer, Patchify, pair
 
 
 class RMSNorm(nn.Module):
@@ -37,20 +36,15 @@ class Attention(nn.Module):
     def __init__(self, dim: int, heads: int = 8, dim_head: int = 64) -> None:
         super().__init__()
         inner_dim = dim_head * heads
-        self.dim, self.dim_head = dim, dim_head
-        self.project_out = True
+        self.dim_head = dim_head
         self.heads = heads
-        self.softmax_scale = 1.0            # no dim_head ** -0.5: q and k are normalised (reference :75)
-        self.scale = 1.0
+        self.scale = 1.0                    # no dim_head ** -0.5: q and k are normalised (reference :75)
         self.norm = nn.LayerNorm(dim)
         self.attend = nn.Softmax(dim=-1)
         self.q_norm = RMSNorm(heads, dim_head)
         self.k_norm = RMSNorm(heads, dim_head)
         self.to_qkv = nn.Linear(dim, inner_dim * 3, bias=False)
         self.to_out = nn.Linear(inner_dim, dim, bias=False)
-
-    def out_linear(self) -> nn.Linear:
-        return self.to_out
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         b, n, _ = x.shape
@@ -61,43 +55,13 @@ class Attention(nn.Module):
         return self.to_out(out)
 
 
-class Transformer(FusedWeightsMixin, nn.Module):
+class Transformer(FusedTransformer):
     def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int) -> None:
         super().__init__()
-        self.dropout_p = 0.0
         self.norm = nn.LayerNorm(dim)
         self.layers = nn.ModuleList([])
         for _ in range(depth):
             self.layers.append(nn.ModuleList([Attention(dim, heads=heads, dim_head=dim_head), FeedForward(dim, mlp_dim)]))
-        self._engine: Optional[TransformerEngine] = None
-
-    def engine(self) -> TransformerEngine:
-        if self._engine is None:
-            self._engine = TransformerEngine(self)
-        return self._engine
-
-    def fused_reason(self, x: torch.Tensor) -> Optional[str]:
-        if len(self.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), x, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self):
-            r = "forward hooks registered inside the transformer"
-        if r is None and x.dim() != 3:
-            r = "input is not (B, N, D)"
-        if r is None:
-            r = self.engine().unsupported_reason(x.shape[1])
-        return r
-
-    def forward_eager(self, x: torch.Tensor) -> torch.Tensor:
-        for attn, ff in self.layers:
-            x = attn(x) + x
-            x = ff(x) + x
-        return self.norm(x)
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.fused_reason(x) is None:
-            return self.engine().forward_tokens(x)
-        return self.forward_eager(x)
 
 
 class SimpleViT(FusedWeightsMixin, nn.Module):

@@ -14,14 +14,15 @@ forward() dispatch:
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 from torch import nn
 
 from . import _lib
-from .engine import (FusedWeightsMixin, HeadEngine, PatchEmbedEngine, TransformerEngine, hooked_transformer_tokens,
-                     hooks_inside, ln_mode, on_device, transformer_is_hooked, why_not_fused)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, HeadEngine, Norm, PatchEmbedEngine, fused_encode,
+                     hooked_transformer_tokens, hooks_inside, on_device, patch_engine, transformer_is_hooked,
+                     why_not_fused)
 
 
 def pair(t):
@@ -51,7 +52,6 @@ class FeedForward(nn.Module):
 
     def __init__(self, dim: int, hidden_dim: int, dropout: float = 0.) -> None:
         super().__init__()
-        self.dim, self.hidden_dim = dim, hidden_dim
         self.net = nn.Sequential(
             nn.LayerNorm(dim),
             nn.Linear(dim, hidden_dim),
@@ -60,9 +60,6 @@ class FeedForward(nn.Module):
             nn.Linear(hidden_dim, dim),
             nn.Dropout(dropout),
         )
-
-    def parts(self):
-        return self.net[0], self.net[1], self.net[4]
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return self.net(x)
@@ -74,7 +71,7 @@ class Attention(nn.Module):
     def __init__(self, dim: int, heads: int = 8, dim_head: int = 64, dropout: float = 0.) -> None:
         super().__init__()
         inner_dim = dim_head * heads
-        self.dim, self.dim_head = dim, dim_head
+        self.dim_head = dim_head
         self.project_out = not (heads == 1 and dim_head == dim)
         self.heads = heads
         self.scale = dim_head ** -0.5
@@ -84,9 +81,6 @@ class Attention(nn.Module):
         self.to_qkv = nn.Linear(dim, inner_dim * 3, bias=False)
         self.to_out = nn.Sequential(nn.Linear(inner_dim, dim), nn.Dropout(dropout)) if self.project_out \
             else nn.Identity()
-
-    def out_linear(self) -> nn.Linear:
-        return self.to_out[0]
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         b, n, _ = x.shape
@@ -99,28 +93,34 @@ class Attention(nn.Module):
         return self.to_out(out)
 
 
-class Transformer(FusedWeightsMixin, nn.Module):
-    """depth x (attention, feed-forward) residual blocks + final LayerNorm (reference vit.py:66-83).
+class FusedTransformer(FusedEncoder, FusedWeightsMixin, nn.Module):
+    """depth x (attention, feed-forward) residual blocks + final LayerNorm (reference vit.py:66-83), the Transformer of
+    vit, simple_vit, simple_vit_with_qk_norm and simple_flash_attn_vit.  Subclasses only build `layers` -- pairs of
+    (Attention with norm / to_qkv / to_out, FeedForward with `net` = LayerNorm, Linear, ..., Linear, ...) -- and `norm`
+    (simple_flash_attn_vit has none), and set `dropout_p` when they have dropout.
 
     Callable on arbitrary (B, N, D) tokens, as the reference's MAE / SimMIM / distillation wrappers do.
     """
 
-    def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int, dropout: float = 0.) -> None:
-        super().__init__()
-        self.dropout_p = float(dropout)
-        self.norm = nn.LayerNorm(dim)
-        self.layers = nn.ModuleList([])
-        for _ in range(depth):
-            self.layers.append(nn.ModuleList([
-                Attention(dim, heads=heads, dim_head=dim_head, dropout=dropout),
-                FeedForward(dim, mlp_dim, dropout=dropout),
-            ]))
-        self._engine: Optional[TransformerEngine] = None
+    dropout_p = 0.0
 
-    def engine(self) -> TransformerEngine:
-        if self._engine is None:
-            self._engine = TransformerEngine(self)
-        return self._engine
+    def encoder_layers(self) -> Tuple[List[EncoderLayer], Optional[Norm]]:
+        layers = []
+        for attn, ff in self.layers:
+            # to_out: Linear, Sequential(Linear, Dropout), or Identity (vit.py: heads == 1 and dim_head == dim)
+            out = attn.to_out[0] if isinstance(attn.to_out, nn.Sequential) else attn.to_out
+            identity = isinstance(out, nn.Identity)
+            fc1, fc2 = [m for m in ff.net if isinstance(m, nn.Linear)]
+            q_norm = getattr(attn, "q_norm", None)        # simple_vit_with_qk_norm: per-head RMSNorm of q and k
+            layers.append(EncoderLayer(
+                ln1=Norm.of(attn.norm), qkv_w=attn.to_qkv.weight,
+                out_w=None if identity else out.weight, out_b=None if identity else out.bias,
+                ln2=Norm.of(ff.net[0]), fc1_w=fc1.weight, fc1_b=fc1.bias, fc2_w=fc2.weight, fc2_b=fc2.bias,
+                heads=attn.heads, dim_head=attn.dim_head, scale=float(attn.scale),
+                qk_norm=None if q_norm is None else "rms",
+                qk_gamma=() if q_norm is None else (q_norm.gamma, attn.k_norm.gamma)))
+        norm = getattr(self, "norm", None)
+        return layers, None if norm is None else Norm.of(norm)
 
     def fused_reason(self, x: torch.Tensor) -> Optional[str]:
         """None if forward(x) will run the fused kernels, else why not."""
@@ -139,12 +139,26 @@ class Transformer(FusedWeightsMixin, nn.Module):
         for attn, ff in self.layers:
             x = attn(x) + x
             x = ff(x) + x
-        return self.norm(x)
+        norm = getattr(self, "norm", None)
+        return x if norm is None else norm(x)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.fused_reason(x) is None:
             return self.engine().forward_tokens(x)
         return self.forward_eager(x)
+
+
+class Transformer(FusedTransformer):
+    def __init__(self, dim: int, depth: int, heads: int, dim_head: int, mlp_dim: int, dropout: float = 0.) -> None:
+        super().__init__()
+        self.dropout_p = float(dropout)
+        self.norm = nn.LayerNorm(dim)
+        self.layers = nn.ModuleList([])
+        for _ in range(depth):
+            self.layers.append(nn.ModuleList([
+                Attention(dim, heads=heads, dim_head=dim_head, dropout=dropout),
+                FeedForward(dim, mlp_dim, dropout=dropout),
+            ]))
 
 
 class ViT(FusedWeightsMixin, nn.Module):
@@ -219,11 +233,8 @@ class ViT(FusedWeightsMixin, nn.Module):
 
     # ---------------------------------------------------------------------------------------------- fused kernels
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
-        if self._patch_engine is None:
-            self._patch_engine = PatchEmbedEngine(self)
-        eng = self.transformer.engine()
         if transformer_is_hooked(self):                # Extractor (reference extractor.py:50-59): hook on .transformer
-            x, B, N = self._patch_engine.run(img)
+            x, B, N = patch_engine(self).run(img)
             out = hooked_transformer_tokens(self, x, B, N)
             if self.mlp_head is None:
                 return out
@@ -232,13 +243,9 @@ class ViT(FusedWeightsMixin, nn.Module):
             if self._head_engine is None:
                 self._head_engine = HeadEngine(self.mlp_head)
             return self._head_engine.run(pooled)
-        B, N = self._patch_engine.geometry(img)
-        primed = ln_mode() == "fold"
-        ws = eng.workspace(B * N, img.device) if primed else None
-        x, B, N = self._patch_engine.run(img, xb=ws["xn"] if primed else None,
-                                         stats=ws["stats_in"] if primed else None)   # fp32 residual stream [B*N, D]
+        x, B, N = fused_encode(self, img)              # fp32 residual stream [B*N, D]
         D = x.shape[1]
-        eng.run_blocks(x, B, N, primed=primed)
+        eng = self.transformer.engine()
         dev = img.device
         if self.mlp_head is None:                      # reference vit.py:132-133: return the normalised tokens
             out = torch.empty(B * N, D, device=dev, dtype=torch.bfloat16)
