@@ -32,7 +32,8 @@ extern "C" {
 /* GEMM epilogue flags (b200vit_gemm_bf16) */
 #define B200VIT_EPI_BIAS 1      /* + bias[n] (fp32) */
 #define B200VIT_EPI_GELU 2      /* exact-erf GELU (nn.GELU default, vit.py:21) */
-#define B200VIT_EPI_RESIDUAL 4  /* + resid[m, n] (fp32); resid may alias out_f32 (in-place residual stream) */
+#define B200VIT_EPI_RESIDUAL 4  /* + resid[m, n] (fp32, row stride ldo, a multiple of 4); resid is either out_f32
+                                   itself (in-place residual stream) or does not overlap it */
 #define B200VIT_EPI_LNFOLD 8    /* A is the un-normalised bf16 row, W carries gamma: y = rstd_m*(acc - mu_m*s_n) + bias_n */
 #define B200VIT_EPI_STATS 16    /* write per-row partial (sum, sum^2) of the bf16-rounded result into stats_out */
 #define B200VIT_EPI_HEADLN 64   /* b200vit_gemm_headnorm_bf16: per-head LayerNorm (no bias) instead of the RMS norm */
@@ -47,7 +48,8 @@ int b200vit_device_ok(int dev);
 
 /*
  * out[M, N] = epilogue( A[M, K] (bf16, row stride lda) x W[N, K]^T (bf16, row stride ldw) ), fp32 accumulate.
- * TMA-fed wgmma GEMM, persistent, warp specialised (one producer and two consumer warpgroups).  Replaces every nn.Linear on the path:
+ * TMA-fed wgmma GEMM, persistent, warp specialised (one loader and two consumer warpgroups; the loaders also stage the
+ * residual tile, bias, col_s and LN-fold row sums in shared memory ahead of the epilogue).  Replaces every nn.Linear on the path:
  *   vit.py:20,23 (FeedForward), vit.py:44,47 (to_qkv / to_out), vit.py:102 (patch projection), vit.py:116 (mlp_head);
  *   simple_vit.py:30,32,47,48,93,108.
  * out_bf16 and/or out_f32 (either may be NULL, not both), row stride ldo (elements).

@@ -1,10 +1,16 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] * W[N,K]^T)
 //
-//   warpgroup 0     : TMA producer  (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
+//   warpgroup 0     : loaders
+//                     warp 0 (one thread): A / W tiles, cp.async.bulk.tensor -> 128B-swizzled smem ring
+//                     warp 1 (one thread, residual GEMMs only): the fp32 residual tile, TMA -> two 64-column slabs
+//                     warp 2: the tile's bias / col_s slices and LN-fold row sums -> smem (double buffered per tile)
 //   warpgroups 1, 2 : consumers     (wgmma m64 x BLOCK_N x k16, fp32 accumulators in registers, 64 rows each), then
 //                     the epilogue straight from the accumulator registers: bias / LN-fold / GELU / residual -> global
 //
-// The producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
+// The loaders run ahead into the next tile while the consumers finish the epilogue of the current one, so every
+// epilogue input is already in shared memory when the accumulators are ready: the epilogue's only global-memory
+// instructions are its stores.  (Read from global memory inside the epilogue, each residual load would wait behind the
+// previous column's stores -- resid may be out_f32 itself -- for a full memory latency.)
 // Replaces the nn.Linear call sites listed in include/b200vit.h.
 #include "common.cuh"
 #include "host_util.h"
@@ -15,6 +21,7 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
 constexpr int WGMMA_K = 16;
 constexpr int NUM_THREADS = 384;
+constexpr int NUM_CONSUMERS = 256;
 
 struct GemmParams {
   int M, N, K;
@@ -24,7 +31,6 @@ struct GemmParams {
   float* out_f32;
   long long ldo;
   const float* bias;
-  const float* resid;
   const float* ln_sums;  // [M][ln_parts][2]
   int ln_parts;
   int stats_parts;
@@ -47,30 +53,45 @@ struct GemmParams {
 };
 
 // PATCH: the A stage holds FOUR 4 KB slabs, one per 16-wide k-step (see GemmParams::patch).
-template <int BLOCK_N, int STAGES, bool PATCH = false>
+// RES (EPI_RESIDUAL launches): two residual slabs of 128 rows x 64 fp32 columns after the ring.  A slab is two TMA
+// boxes of 32 columns (128 B per row, 128B swizzle: 16-byte chunk c of row r sits at chunk c ^ (r % 8)), so that the
+// epilogue's float2 reads -- 8 rows x 4 column pairs per warp instruction -- touch every bank exactly twice.
+template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false>
 struct GemmSmem {
   static constexpr int A_SLAB = PATCH ? BLOCK_M * 32 : BLOCK_M * BLOCK_K * 2;
   static constexpr int A_BYTES = PATCH ? 4 * A_SLAB : A_SLAB;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-  // full[STAGES], empty[STAGES]
-  static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8;
+  static constexpr int RES_BOX = BLOCK_M * 32 * 4;
+  static constexpr int RES_SLAB = 2 * RES_BOX;
+  static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
+  // per tile, double buffered: bias[BLOCK_N], col_s[BLOCK_N], LN-fold row sums [BLOCK_M][2]
+  static constexpr int VEC_OFFSET = RES_OFFSET + (RES ? 2 * RES_SLAB : 0);
+  static constexpr int VEC_BYTES = (2 * BLOCK_N + 2 * BLOCK_M) * 4;
+  static constexpr int BAR_OFFSET = VEC_OFFSET + 2 * VEC_BYTES;
+  // full[STAGES], empty[STAGES], res_full[2], res_empty[2], vec_full[2], vec_empty[2]
+  static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 8) * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024B alignment
 };
 
-template <int BLOCK_N, int STAGES, bool PATCH>
+template <int BLOCK_N, int STAGES, bool PATCH, bool RES>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const GemmParams p) {
-  using L = GemmSmem<BLOCK_N, STAGES, PATCH>;
+                 const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
+  using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES>;
   constexpr int NACC = BLOCK_N / 2;          // fp32 accumulators per consumer thread (64 rows x BLOCK_N / 128)
-  constexpr int CHUNKS = BLOCK_N / 64;       // 64-column statistics chunks per tile
+  constexpr int CHUNKS = BLOCK_N / 64;       // 64-column statistics chunks (and residual slabs) per tile
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // offset from the __shared__ array itself (no round trip through an integer), so that the compiler knows every
+  // access below is to shared memory and may schedule the epilogue's smem reads ahead of its global stores
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* res_full = empty_bar + STAGES;
+  uint64_t* res_empty = res_full + 2;
+  uint64_t* vec_full = res_empty + 2;
+  uint64_t* vec_empty = vec_full + 2;
 
   const int wg = threadIdx.x >> 7;
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
@@ -78,16 +99,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (RES) tma_prefetch_desc(&tmR);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
+    }
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&res_full[s], 1);
+      mbar_init(&res_empty[s], NUM_CONSUMERS);
+      mbar_init(&vec_full[s], 64);  // every thread of loader warps 2 and 3
+      mbar_init(&vec_empty[s], NUM_CONSUMERS);
     }
     fence_mbar_init();
   }
   __syncthreads();
 
   if (wg == 0) {
-    // ------------------------------------------------------------------ TMA producer
+    // ------------------------------------------------------------------ loaders
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
@@ -118,6 +146,68 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
       }
+    } else if (RES && threadIdx.x == 32) {
+      // residual slabs: the consumers release slab q of a tile after its last column group, so the first two slabs
+      // of a tile load during the tile's main loop.  Boxes wholly right of N are not loaded (nor waited for).
+      int it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
+        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        const int nslab = min(CHUNKS, (p.N - n0 + 63) / 64);
+        for (int q = 0; q < nslab; ++q, ++it) {
+          const int buf = it & 1;
+          mbar_wait(&res_empty[buf], ((it >> 1) & 1) ^ 1);
+          const int c0 = n0 + 64 * q;
+          const int nbox = c0 + 32 < p.N ? 2 : 1;
+          mbar_arrive_expect_tx(&res_full[buf], nbox * L::RES_BOX);
+          uint8_t* slab = smem + L::RES_OFFSET + buf * L::RES_SLAB;
+          for (int b = 0; b < nbox; ++b) tma_load_2d(slab + b * L::RES_BOX, &tmR, &res_full[buf], c0 + 32 * b, m0);
+        }
+      }
+    } else if ((threadIdx.x >> 5) >= 2) {
+      // warp 2: the tile's bias / col_s slices (zero past N); warp 3: its rows' LN-fold sums (added up in part order)
+      const int lane = threadIdx.x & 31;
+      const bool vec_warp = (threadIdx.x >> 5) == 2;
+      int it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        const int m_blk = tile / p.num_n_tiles;
+        const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
+        const int vb = it & 1;
+        mbar_wait(&vec_empty[vb], ((it >> 1) & 1) ^ 1);
+        float* vbias = reinterpret_cast<float*>(smem + L::VEC_OFFSET + vb * L::VEC_BYTES);
+        float* vcs = vbias + BLOCK_N;
+        float2* vln = reinterpret_cast<float2*>(vcs + BLOCK_N);
+        if (vec_warp) {
+#pragma unroll
+          for (int i = lane; i < BLOCK_N; i += 32) {
+            const int col = n0 + i;
+            vbias[i] = (p.flags & B200VIT_EPI_BIAS) && col < p.N ? p.bias[col] : 0.f;
+            vcs[i] = (p.flags & B200VIT_EPI_LNFOLD) && col < p.N ? p.col_s[col] : 0.f;
+          }
+        } else if (p.flags & B200VIT_EPI_LNFOLD) {
+          float s1[BLOCK_M / 32], s2[BLOCK_M / 32];
+          bool ok[BLOCK_M / 32];
+#pragma unroll
+          for (int k = 0; k < BLOCK_M / 32; ++k) {
+            const int tr = lane + 32 * k;
+            ok[k] = m_blk * p.rows_per_tile + tr < p.M && tr < p.rows_per_tile;
+            s1[k] = s2[k] = 0.f;
+          }
+#pragma unroll 1  // four loads in flight per lane fit the loaders' 40 registers
+          for (int i = 0; i < p.ln_parts; ++i)
+#pragma unroll
+            for (int k = 0; k < BLOCK_M / 32; ++k)
+              if (ok[k]) {
+                const size_t row = (size_t)m_blk * p.rows_per_tile + lane + 32 * k;
+                const float2 ss = *reinterpret_cast<const float2*>(p.ln_sums + 2 * (row * p.ln_parts + i));
+                s1[k] += ss.x;
+                s2[k] += ss.y;
+              }
+#pragma unroll
+          for (int k = 0; k < BLOCK_M / 32; ++k) vln[lane + 32 * k] = make_float2(s1[k], s2[k]);
+        }
+        mbar_arrive(&vec_full[vb]);
+      }
     }
     return;
   }
@@ -131,9 +221,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const bool vec_ok = (p.ldo & 1) == 0;
   int stage = 0;
   uint32_t phase = 0;
+  int slab_it = 0;  // residual slabs consumed so far (the loader's count)
   float acc[NACC];
 
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  for (int tile = blockIdx.x, it = 0; tile < num_tiles; tile += gridDim.x, ++it) {
     const int m_blk = tile / p.num_n_tiles;
     const int n_blk = tile % p.num_n_tiles;
 
@@ -170,6 +261,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // accumulator layout (wgmma m64nN, fp32): acc[4j + h] holds row (16 warp + lane/4 + 8 (h >> 1)),
     // column (8 j + 2 (lane % 4) + (h & 1)) of this warpgroup's 64 x BLOCK_N block
     const int tr0 = c * 64 + warp * 16 + (lane >> 2);
+    const int vb = it & 1;
+    mbar_wait(&vec_full[vb], (it >> 1) & 1);
+    const float* vbias = reinterpret_cast<const float*>(smem + L::VEC_OFFSET + vb * L::VEC_BYTES);
+    const float* vcs = vbias + BLOCK_N;
+    const float2* vln = reinterpret_cast<const float2*>(vcs + BLOCK_N);
     float mu[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
     int row[2];
     bool row_ok[2];
@@ -179,12 +275,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       row[h] = m_blk * p.rows_per_tile + tr;
       row_ok[h] = row[h] < p.M && tr < p.rows_per_tile;
       if ((flags & B200VIT_EPI_LNFOLD) && row_ok[h]) {
-        float s1 = 0.f, s2 = 0.f;
-        for (int i = 0; i < p.ln_parts; ++i) {
-          const float2 ss = *reinterpret_cast<const float2*>(p.ln_sums + 2 * ((size_t)row[h] * p.ln_parts + i));
-          s1 += ss.x;
-          s2 += ss.y;
-        }
+        const float2 ss = vln[tr];
+        const float s1 = ss.x, s2 = ss.y;
         mu[h] = s1 * p.ln_inv_dim;
         const float var = fmaxf(s2 * p.ln_inv_dim - mu[h] * mu[h], 0.f);
         rstd[h] = rsqrtf(var + p.ln_eps);
@@ -195,23 +287,32 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int q = 0; q < CHUNKS; ++q) st_sum[0][q] = st_sum[1][q] = st_sq[0][q] = st_sq[1][q] = 0.f;
 
     const int n0 = n_blk * BLOCK_N;
+    const int nslab = RES ? min(CHUNKS, (p.N - n0 + 63) / 64) : 0;
+    // this thread's float2 in a residual slab: row tr0 (+ 8 h), 16-byte chunk (2 (j % 4) + (lane & 3) / 2) ^ (tr0 % 8)
+    // of box (j % 8) / 4, 8-byte half lane & 1
+    const int res_off = tr0 * 128 + (lane & 1) * 8;
+    const int res_xor = ((lane & 3) >> 1) ^ (lane >> 2);
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
-      const int col = n0 + 8 * j + 2 * (lane & 3);
-      if (col >= p.N) continue;
+      const int pc = 8 * j + 2 * (lane & 3);  // column of the pair in the tile
+      const int col = n0 + pc;
+      if (RES && j % 8 == 0 && j / 8 < nslab) mbar_wait(&res_full[slab_it & 1], (slab_it >> 1) & 1);
+      const uint8_t* slab = smem + L::RES_OFFSET + (slab_it & 1) * L::RES_SLAB + ((j % 8) / 4) * L::RES_BOX + res_off;
       const bool pair = vec_ok && col + 1 < p.N;
       float b0 = 0.f, b1 = 0.f, s0 = 0.f, s1 = 0.f;
       if (flags & B200VIT_EPI_BIAS) {
-        b0 = p.bias[col];
-        b1 = col + 1 < p.N ? p.bias[col + 1] : 0.f;
+        const float2 bb = *reinterpret_cast<const float2*>(vbias + pc);
+        b0 = bb.x;
+        b1 = bb.y;
       }
       if (flags & B200VIT_EPI_LNFOLD) {
-        s0 = p.col_s[col];
-        s1 = col + 1 < p.N ? p.col_s[col + 1] : 0.f;
+        const float2 ss = *reinterpret_cast<const float2*>(vcs + pc);
+        s0 = ss.x;
+        s1 = ss.y;
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (!row_ok[h]) continue;
+        if (!row_ok[h] || col >= p.N) continue;
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
         if (flags & (B200VIT_EPI_LNFOLD | B200VIT_EPI_BIAS)) {
           // y = acc * rstd + (bias - rstd*mu * s)
@@ -224,10 +325,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         if (flags & B200VIT_EPI_GELU) gelu_erf2(v0, v1);
         const size_t o = (size_t)row[h] * p.ldo + col;
+        float2 rr = make_float2(0.f, 0.f);
+        if (RES) rr = *reinterpret_cast<const float2*>(slab + h * 8 * 128 + ((((j % 4) * 2) ^ res_xor) << 4));
         float r0 = 0.f, r1 = 0.f;
         if (pair) {
-          if (flags & B200VIT_EPI_RESIDUAL) {
-            const float2 rr = *reinterpret_cast<const float2*>(p.resid + o);
+          if (RES) {
             v0 += rr.x;
             v1 += rr.y;
           }
@@ -238,25 +340,30 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           r1 = __uint_as_float(pk & 0xFFFF0000u);
         } else {
           // scalar tail (N or ldo odd)
-          const float vv[2] = {v0, v1};
-          float rr[2] = {0.f, 0.f};
+          const float vv[2] = {v0, v1}, res[2] = {rr.x, rr.y};
+          float rb[2] = {0.f, 0.f};
           for (int i = 0; i < 2 && col + i < p.N; ++i) {
             float x = vv[i];
-            if (flags & B200VIT_EPI_RESIDUAL) x += p.resid[o + i];
+            if (RES) x += res[i];
             if (p.out_f32) p.out_f32[o + i] = x;
             const __nv_bfloat16 xb = __float2bfloat16_rn(x);
             if (p.out_bf16) p.out_bf16[o + i] = xb;
-            rr[i] = __bfloat162float(xb);
+            rb[i] = __bfloat162float(xb);
           }
-          r0 = rr[0];
-          r1 = rr[1];
+          r0 = rb[0];
+          r1 = rb[1];
         }
         if (flags & B200VIT_EPI_STATS) {
           st_sum[h][j / 8] += r0 + r1;
           st_sq[h][j / 8] = fmaf(r0, r0, fmaf(r1, r1, st_sq[h][j / 8]));
         }
       }
+      if (RES && j % 8 == 7 && j / 8 < nslab) {
+        mbar_arrive(&res_empty[slab_it & 1]);
+        ++slab_it;
+      }
     }
+    mbar_arrive(&vec_empty[vb]);
     if (flags & B200VIT_EPI_STATS) {
       // the four lanes of a quad hold the same two rows: reduce, then lane 0 of the quad writes every part of the tile
 #pragma unroll
@@ -296,11 +403,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 static std::atomic<int> g_gemm_block_n{0};
 void gemm_set_block_n(int v) { g_gemm_block_n = v; }
 
-template <int BLOCK_N, int STAGES, bool PATCH = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, cudaStream_t stream) {
-  using L = GemmSmem<BLOCK_N, STAGES, PATCH>;
+template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, GemmParams& p,
+                       cudaStream_t stream) {
+  using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES>;
   static_assert(L::DYN_BYTES <= 227 * 1024, "gemm: shared memory budget");
-  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES>;
   B200_ENSURE_SMEM(kern, L::DYN_BYTES);
   if (!p.patch) p.rows_per_tile = BLOCK_M;
   p.num_m_tiles = (p.M + p.rows_per_tile - 1) / p.rows_per_tile;
@@ -309,7 +417,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
   p.stats_width = p.N > 128 ? 128 : 64;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(tmA, tmB, p);
+  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(tmA, tmB, tmR, p);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
@@ -337,6 +445,8 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   B200_CHECK_ARG(ldo >= N, "gemm: ldo=%lld < N=%d", (long long)ldo, N);
   B200_CHECK_ARG(!(flags & B200VIT_EPI_BIAS) || bias, "gemm: EPI_BIAS without bias");
   B200_CHECK_ARG(!(flags & B200VIT_EPI_RESIDUAL) || resid, "gemm: EPI_RESIDUAL without resid");
+  B200_CHECK_ARG(!(flags & B200VIT_EPI_RESIDUAL) || (ldo & 3) == 0,
+                 "gemm: EPI_RESIDUAL needs ldo=%lld to be a multiple of 4 (16-byte rows for TMA)", (long long)ldo);
   B200_CHECK_ARG(!(flags & B200VIT_EPI_LNFOLD) || (ln_sums && col_s && ln_parts >= 1 && ln_parts <= 64),
                  "gemm: EPI_LNFOLD needs ln_sums, col_s and 1 <= ln_parts <= 64");
   B200_CHECK_ARG(!(flags & B200VIT_EPI_STATS) || stats_out, "gemm: EPI_STATS without stats_out");
@@ -354,7 +464,6 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   p.out_f32 = out_f32;
   p.ldo = ldo;
   p.bias = bias;
-  p.resid = resid;
   p.ln_sums = ln_sums;
   p.ln_parts = ln_parts;
   p.stats_parts = b200vit_stats_parts(N);
@@ -366,7 +475,16 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   const int force = g_gemm_block_n.load();
   const bool wide = force == 0 ? N > 128 : force == 2;
   const uint32_t block_n = wide ? 256 : 128;
-  CUtensorMap tmA, tmB;
+  const bool res = (flags & B200VIT_EPI_RESIDUAL) != 0;
+  CUtensorMap tmA, tmB, tmR{};
+  if (res) {
+    // fp32 residual, 32-column boxes (128 B rows, 128B swizzle) of one tile's 128 rows
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
+    const uint64_t strides[1] = {(uint64_t)ldo * 4};
+    const uint32_t box[2] = {32, (uint32_t)BLOCK_M};
+    int rc = encode_tmap_f32(&tmR, resid, 2, dims, strides, box, true);
+    if (rc) return rc;
+  }
   {
     const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
     const uint64_t strides[1] = {(uint64_t)lda * 2};
@@ -381,8 +499,9 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
     int rc = encode_tmap_bf16(&tmB, W, 2, dims, strides, box);
     if (rc) return rc;
   }
-  if (wide) return launch_gemm<256, 4>(tmA, tmB, p, st);
-  return launch_gemm<128, 6>(tmA, tmB, p, st);
+  // residual launches trade ring stages for the two 32 KB residual slabs
+  if (wide) return res ? launch_gemm<256, 3, false, true>(tmA, tmB, tmR, p, st) : launch_gemm<256, 4>(tmA, tmB, tmR, p, st);
+  return res ? launch_gemm<128, 4, false, true>(tmA, tmB, tmR, p, st) : launch_gemm<128, 6>(tmA, tmB, tmR, p, st);
 }
 
 extern "C" int b200vit_rmsnorm_heads(void* buf, int64_t ld, const float* gamma, int T, int nheads, int dh, void* stream);
@@ -452,7 +571,7 @@ extern "C" int b200vit_patch_embed_tma(const void* img, const void* w_perm, cons
   p.patch_tiles_per_img = gh / ght;
   p.patch_C = C;
   p.rows_per_tile = ght * gw;
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmR{};
   {
     // innermost first: pixel in a patch row | patch column | patch row | pixel row in the patch | image x channel
     const uint64_t dims[5] = {16, (uint64_t)gw, (uint64_t)gh, 16, (uint64_t)B * C};
@@ -468,5 +587,5 @@ extern "C" int b200vit_patch_embed_tma(const void* img, const void* w_perm, cons
     int rc = encode_tmap_bf16(&tmB, w_perm, 2, dims, strides, box);
     if (rc) return rc;
   }
-  return launch_gemm<256, 4, true>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_gemm<256, 4, true>(tmA, tmB, tmR, p, reinterpret_cast<cudaStream_t>(stream));
 }
