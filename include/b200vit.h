@@ -122,7 +122,8 @@ int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats, int M, in
  *   out[B*N, H*dh]   bf16 (merged heads, vit.py:63) = softmax(q k^T * scale) v          (vit.py:57-62)
  * N <= 512 (longer sequences: b200vit_attention_varlen).  128-row query tiles, keys streamed in blocks with an
  * online softmax in fp32; S = QK^T and O = PV on the tensor cores (bf16 operands, fp32 accumulation).
- * dh = 64, or 80 (canonical ViT-H/14).
+ * dh = 32, 64, 80 (canonical ViT-H/14) or 128; a head is split into 64- and 16-column slabs (a 96-wide head would
+ * fall out of the same scheme as 64 + 2 x 16, but is not built).
  */
 int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* stream);
 
@@ -130,7 +131,7 @@ int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, f
  * Variable-length attention over PACKED sequences (any length): tokens [cu_seqlens[s], cu_seqlens[s+1]) of
  * qkv[total_tokens, 3*H*dh] attend only among themselves; out[total_tokens, H*dh].  This is the block-diagonal
  * "same image" attention of NaViT (na_vit.py:335-337 mask + 161-166 SDPA) without padding or an O(L^2) mask, and the
- * long-sequence (N > 512) path of ViT.  dh = 64 or 80.  cu_seqlens_dev[num_seqs+1] and tile_prefix_dev[num_seqs+1] (number of 128-row
+ * long-sequence (N > 512) path of ViT.  dh = 32, 64, 80 or 128.  cu_seqlens_dev[num_seqs+1] and tile_prefix_dev[num_seqs+1] (number of 128-row
  * query tiles before sequence s; tile_prefix[num_seqs] == total_tiles) are DEVICE int32 arrays built by the caller.
  */
 int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev,
@@ -150,13 +151,14 @@ int b200vit_patchify_varlen_ln(const int64_t* img_ptrs_dev, const int32_t* dims_
 /*
  * NaViT per-head q/k RMSNorm, in place on the packed qkv[T, 3*H*dh] buffer (q and k slices only):
  *   v <- v / max(||v||, 1e-12) * sqrt(dh) * gamma[h, d]    (na_vit.py:93-101,149-150).  gamma_qk fp32 [2][H][dh].
+ * dh = 32, 64, 80 or 128 (this and every head-norm / pooling entry point below).
  */
 int b200vit_qk_rmsnorm(void* qkv, const float* gamma_qk, int T, int H, int dh, void* stream);
 
 /*
  * Linear + per-head RMSNorm in one pass (NaViT to_q / to_kv followed by q_norm / k_norm, na_vit.py:145-150):
  *   out[M, N] bf16 = epilogue(A W^T)   with flags in {EPI_BIAS, EPI_LNFOLD} exactly as b200vit_gemm_bf16, then the first
- *   norm_heads heads (dh = 64 columns each, from column 0) of every row are replaced by
+ *   norm_heads heads (dh columns each, from column 0; norm_heads * dh <= N) of every row are replaced by
  *   v / max(||v||, 1e-12) * sqrt(dh) * head_gamma[h, d]   (norm computed on the bf16-rounded projection, like the
  *   reference's bf16 module): b200vit_gemm_bf16 followed by b200vit_rmsnorm_heads / b200vit_layernorm_heads.
  *   flags | EPI_HEADLN: the heads get nn.LayerNorm(dh, bias=False) instead -- (v - mean) * rsqrt(var + head_eps) *
@@ -247,6 +249,8 @@ int b200vit_encoder_blocks(const b200vit_layer* layers, int depth, float* x, con
  *           the softmax exponentials on the FMA pipe
  *   key 12: BLOCK_N of b200vit_gemm_bf16: 0 = auto (256 when N > 128, else 128), 1 = 128, 2 = 256
  *   key 13: b200vit_attention: 0 = all softmax exponentials on MUFU (default), 1 = half of them on the FMA pipe
+ * Keys 1, 11 and 13 select real attention instances for every head width (32, 64, 80, 128): all (key block, FMA
+ * exponential) combinations are built without register spills, so no setting falls back to a width's default.
  */
 int b200vit_debug_set(int key, int value);
 

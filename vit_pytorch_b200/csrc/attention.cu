@@ -7,8 +7,8 @@
 // complete_tx; a stage is reloaded once both warpgroups have released it).  Per key block each warpgroup computes
 // S = Q K^T with wgmma (both operands in shared memory), runs an online softmax in fp32 on the accumulator registers
 // and accumulates O += P V with wgmma, P (bf16) taken from registers as the A operand and V read as the transposed
-// (MN-major) B operand.  dh = 64, or 80: an 80-wide head is a 64-wide (128B swizzle) plus a 16-wide (32B swizzle)
-// slab.  Keys of a block beyond the sequence get probability 0; TMA zero-fills rows beyond the buffer.
+// (MN-major) B operand.  dh = 32, 64, 80 or 128: a head is split into 64-wide (128B swizzle) and 16-wide (32B swizzle)
+// slabs (AttnSmem).  Keys of a block beyond the sequence get probability 0; TMA zero-fills rows beyond the buffer.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -27,26 +27,36 @@ struct AttnParams {
   float scale_log2e;
 };
 
+// A head of DH columns is DH / 64 slabs 64 columns wide (128B swizzle) followed by (DH % 64) / 16 slabs 16 columns
+// wide (32B swizzle): dh 32 = 2 x 16, 64 = 64, 80 = 64 + 16, 128 = 2 x 64.  Shared memory: Q64[N64] | Q16[N16], then
+// per stage K64[N64] | V64[N64] | K16[N16] | V16[N16].
 template <int DH, int KB>
 struct AttnSmem {
-  static constexpr bool WIDE = DH == 80;
-  static constexpr int Q64 = ATT_QROWS * 128;        // 64 columns, 128B swizzle
-  static constexpr int Q16 = WIDE ? ATT_QROWS * 32 : 0;  // columns 64..79, 32B swizzle
+  static constexpr int N64 = DH / 64;
+  static constexpr int N16 = (DH % 64) / 16;
+  static_assert(N64 * 64 + N16 * 16 == DH, "dim_head must be a multiple of 16");
+  static constexpr int Q64 = ATT_QROWS * 128;        // one 64-column slab of Q
+  static constexpr int Q16 = ATT_QROWS * 32;         // one 16-column slab of Q
   static constexpr int KV64 = KB * 128;
-  static constexpr int KV16 = WIDE ? KB * 32 : 0;
-  static constexpr int STAGE = 2 * (KV64 + KV16);   // K64 | V64 | K16 | V16
-  static constexpr int STAGE_OFF = Q64 + Q16;
+  static constexpr int KV16 = KB * 32;
+  static constexpr int K16_OFF = 2 * N64 * KV64;     // within a stage
+  static constexpr int V16_OFF = K16_OFF + N16 * KV16;
+  static constexpr int STAGE = 2 * (N64 * KV64 + N16 * KV16);
+  static constexpr int STAGE_OFF = N64 * Q64 + N16 * Q16;
   static constexpr int BAR_OFF = STAGE_OFF + 2 * STAGE;
   static constexpr int BYTES = BAR_OFF + 5 * 8 + 1024;  // full[2], empty[2], q; slack for 1024B alignment
 };
 
+// CTAs per SM the register budget is planned for (ptxas -v: no spills at these bounds)
+constexpr int att_min_blocks(int dh, int kb) { return (dh == 64 && kb == 64) || dh == 32 ? 2 : 1; }
+
 template <int DH, int KB, bool VARLEN, bool EMUL>
-__global__ void __launch_bounds__(ATT_THREADS, (DH == 64 && KB == 64) ? 2 : 1)
+__global__ void __launch_bounds__(ATT_THREADS, att_min_blocks(DH, KB))
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                  const __grid_constant__ CUtensorMap tmQ16, const __grid_constant__ CUtensorMap tmKV16,
                  const AttnParams p) {
   using L = AttnSmem<DH, KB>;
-  constexpr bool WIDE = L::WIDE;
+  constexpr int N64 = L::N64, N16 = L::N16;
   constexpr int NS = KB / 2;  // score accumulators per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -82,11 +92,15 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     uint8_t* sb = smem + L::STAGE_OFF + st * L::STAGE;
     const int row = seq_start + blk * KB;
     mbar_arrive_expect_tx(&full[st], L::STAGE);
-    tma_load_2d(sb, &tmKV, &full[st], colk, row);
-    tma_load_2d(sb + L::KV64, &tmKV, &full[st], colv, row);
-    if (WIDE) {
-      tma_load_2d(sb + 2 * L::KV64, &tmKV16, &full[st], colk + 64, row);
-      tma_load_2d(sb + 2 * L::KV64 + L::KV16, &tmKV16, &full[st], colv + 64, row);
+#pragma unroll
+    for (int c = 0; c < N64; ++c) {
+      tma_load_2d(sb + c * L::KV64, &tmKV, &full[st], colk + 64 * c, row);
+      tma_load_2d(sb + (N64 + c) * L::KV64, &tmKV, &full[st], colv + 64 * c, row);
+    }
+#pragma unroll
+    for (int c = 0; c < N16; ++c) {
+      tma_load_2d(sb + L::K16_OFF + c * L::KV16, &tmKV16, &full[st], colk + 64 * N64 + 16 * c, row);
+      tma_load_2d(sb + L::V16_OFF + c * L::KV16, &tmKV16, &full[st], colv + 64 * N64 + 16 * c, row);
     }
   };
 
@@ -102,21 +116,29 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   }
   __syncthreads();
   if (tid == 0) {
-    mbar_arrive_expect_tx(qbar, L::Q64 + L::Q16);
-    tma_load_2d(smem, &tmQ, qbar, colq, seq_start + q0);
-    if (WIDE) tma_load_2d(smem + L::Q64, &tmQ16, qbar, colq + 64, seq_start + q0);
+    mbar_arrive_expect_tx(qbar, L::STAGE_OFF);
+#pragma unroll
+    for (int c = 0; c < N64; ++c) tma_load_2d(smem + c * L::Q64, &tmQ, qbar, colq + 64 * c, seq_start + q0);
+#pragma unroll
+    for (int c = 0; c < N16; ++c)
+      tma_load_2d(smem + N64 * L::Q64 + c * L::Q16, &tmQ16, qbar, colq + 64 * N64 + 16 * c, seq_start + q0);
     issue_kv(0);
     if (nblocks > 1) issue_kv(1);
   }
 
-  float o[32], o16[8];
+  // per-slab output accumulators (an array of extent 1 stands in for an absent kind; the compiler drops it)
+  float o[N64 > 0 ? N64 : 1][32], o16[N16 > 0 ? N16 : 1][8];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  for (int c = 0; c < N64; ++c)
 #pragma unroll
-  for (int i = 0; i < 8; ++i) o16[i] = 0.f;
+    for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
+#pragma unroll
+  for (int c = 0; c < N16; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o16[c][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const uint32_t qa = smem_u32(smem) + wg * 64 * 128;
-  const uint32_t qa16 = smem_u32(smem + L::Q64) + wg * 64 * 32;
+  const uint32_t qa16 = smem_u32(smem + N64 * L::Q64) + wg * 64 * 32;
   mbar_wait(qbar, 0);
 
   for (int kb = 0; kb < nblocks; ++kb) {
@@ -125,21 +147,24 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     mbar_wait(&full[st], ph);
     const uint32_t sb = smem_u32(smem + L::STAGE_OFF + st * L::STAGE);
 
-    // S = Q K^T (64 rows x KB keys per warpgroup)
+    // S = Q K^T (64 rows x KB keys per warpgroup): one k16 step per 16 columns, the 64-wide slabs first
     float s[NS];
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const uint64_t ad = make_wgmma_desc(qa, 1024, WGMMA_SW128) + 2 * k;
-      const uint64_t bd = make_wgmma_desc(sb, 1024, WGMMA_SW128) + 2 * k;
-      if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, k != 0);
-      else wgmma_m64n64k16(s, ad, bd, k != 0);
-    }
-    if constexpr (WIDE) {
-      const uint64_t ad = make_wgmma_desc(qa16, 256, WGMMA_SW32);
-      const uint64_t bd = make_wgmma_desc(sb + 2 * L::KV64, 256, WGMMA_SW32);
-      if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, 1);
-      else wgmma_m64n64k16(s, ad, bd, 1);
+    for (int c = 0; c < N64; ++c)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t ad = make_wgmma_desc(qa + c * L::Q64, 1024, WGMMA_SW128) + 2 * k;
+        const uint64_t bd = make_wgmma_desc(sb + c * L::KV64, 1024, WGMMA_SW128) + 2 * k;
+        if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, c != 0 || k != 0);
+        else wgmma_m64n64k16(s, ad, bd, c != 0 || k != 0);
+      }
+#pragma unroll
+    for (int c = 0; c < N16; ++c) {
+      const uint64_t ad = make_wgmma_desc(qa16 + c * L::Q16, 256, WGMMA_SW32);
+      const uint64_t bd = make_wgmma_desc(sb + L::K16_OFF + c * L::KV16, 256, WGMMA_SW32);
+      if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, N64 != 0 || c != 0);
+      else wgmma_m64n64k16(s, ad, bd, N64 != 0 || c != 0);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -163,15 +188,19 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const float corr = fast_ex2(m[r] - mx[r]);  // m = -inf on the first block: exp2(-inf) = 0
       l[r] *= corr;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        o[4 * i + 2 * r] *= corr;
-        o[4 * i + 2 * r + 1] *= corr;
-      }
+      for (int c = 0; c < N64; ++c)
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        o16[4 * i + 2 * r] *= corr;
-        o16[4 * i + 2 * r + 1] *= corr;
-      }
+        for (int i = 0; i < 8; ++i) {
+          o[c][4 * i + 2 * r] *= corr;
+          o[c][4 * i + 2 * r + 1] *= corr;
+        }
+#pragma unroll
+      for (int c = 0; c < N16; ++c)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          o16[c][4 * i + 2 * r] *= corr;
+          o16[c][4 * i + 2 * r + 1] *= corr;
+        }
       m[r] = mx[r];
     }
 #pragma unroll
@@ -195,20 +224,27 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
     }
 
-    // O += P V: the score accumulators of 16 keys are the A fragment of one k-step (bf16)
+    // O += P V: the score accumulators of 16 keys are the A fragment of one k-step (bf16); one MMA per slab
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < KB / 16; ++kk) {
       const uint32_t a[4] = {pack_bf16x2(s[8 * kk], s[8 * kk + 1]), pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]),
                              pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7])};
-      wgmma_m64n64k16_rs_tb(o, a, make_wgmma_desc_lbo(sb + L::KV64 + kk * 2048, 1024, 1024, WGMMA_SW128));
-      if constexpr (WIDE)
-        wgmma_m64n16k16_rs_tb(o16, a, make_wgmma_desc_lbo(sb + 2 * L::KV64 + L::KV16 + kk * 512, 256, 256, WGMMA_SW32));
+#pragma unroll
+      for (int c = 0; c < N64; ++c)
+        wgmma_m64n64k16_rs_tb(o[c], a,
+                              make_wgmma_desc_lbo(sb + (N64 + c) * L::KV64 + kk * 2048, 1024, 1024, WGMMA_SW128));
+#pragma unroll
+      for (int c = 0; c < N16; ++c)
+        wgmma_m64n16k16_rs_tb(o16[c], a,
+                              make_wgmma_desc_lbo(sb + L::V16_OFF + c * L::KV16 + kk * 512, 256, 256, WGMMA_SW32));
     }
     wgmma_commit();
     wgmma_wait<0>();
-    fence_regs(o);
-    fence_regs(o16);
+#pragma unroll
+    for (int c = 0; c < N64; ++c) fence_regs(o[c]);
+#pragma unroll
+    for (int c = 0; c < N16; ++c) fence_regs(o16[c]);
     if (t == 0) mbar_arrive(&empty[st]);
     if (tid == 0 && kb + 2 < nblocks) {
       mbar_wait(&empty[st], ph);  // both warpgroups are done with this stage
@@ -229,19 +265,23 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     if (row >= len) continue;
     __nv_bfloat16* op = p.out + (long long)(seq_start + row) * p.I + h * DH + 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<uint32_t*>(op + j * 8) = pack_bf16x2(o[4 * j + 2 * r] * l[r], o[4 * j + 2 * r + 1] * l[r]);
-    if constexpr (WIDE) {
+    for (int c = 0; c < N64; ++c)
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<uint32_t*>(op + 64 * c + j * 8) =
+            pack_bf16x2(o[c][4 * j + 2 * r] * l[r], o[c][4 * j + 2 * r + 1] * l[r]);
+#pragma unroll
+    for (int c = 0; c < N16; ++c)
 #pragma unroll
       for (int j = 0; j < 2; ++j)
-        *reinterpret_cast<uint32_t*>(op + 64 + j * 8) =
-            pack_bf16x2(o16[4 * j + 2 * r] * l[r], o16[4 * j + 2 * r + 1] * l[r]);
-    }
+        *reinterpret_cast<uint32_t*>(op + 64 * N64 + 16 * c + j * 8) =
+            pack_bf16x2(o16[c][4 * j + 2 * r] * l[r], o16[c][4 * j + 2 * r + 1] * l[r]);
   }
 }
 
-// Tensor maps over qkv[T, 3 I]: 64-column boxes (128B swizzle) of 128 query rows / KB key rows, and -- dh 80 -- the
-// same with 16 columns (32B swizzle).
+// Tensor maps over qkv[T, 3 I]: 64-column boxes (128B swizzle) of 128 query rows / KB key rows for the 64-wide slabs,
+// and the same with 16 columns (32B swizzle) for the 16-wide ones.  A kind the head does not use gets a copy of the
+// other (never read).
 template <int DH, int KB, bool VARLEN, bool EMUL>
 static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 grid, cudaStream_t stream) {
   using L = AttnSmem<DH, KB>;
@@ -249,12 +289,14 @@ static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 
   const uint64_t dims[2] = {(uint64_t)3 * p.I, (uint64_t)T};
   const uint64_t strides[1] = {(uint64_t)3 * p.I * 2};
   const uint32_t qbox[2] = {64, ATT_QROWS}, kvbox[2] = {64, KB}, qbox16[2] = {16, ATT_QROWS}, kvbox16[2] = {16, KB};
-  int rc = encode_tmap_bf16(&tm[0], qkv, 2, dims, strides, qbox);
-  if (!rc) rc = encode_tmap_bf16(&tm[1], qkv, 2, dims, strides, kvbox);
-  if (!rc && DH == 80) rc = encode_tmap_bf16_sw(&tm[2], qkv, 2, dims, strides, qbox16, 32);
-  if (!rc && DH == 80) rc = encode_tmap_bf16_sw(&tm[3], qkv, 2, dims, strides, kvbox16, 32);
+  int rc = 0;
+  if (L::N64) rc = encode_tmap_bf16(&tm[0], qkv, 2, dims, strides, qbox);
+  if (!rc && L::N64) rc = encode_tmap_bf16(&tm[1], qkv, 2, dims, strides, kvbox);
+  if (!rc && L::N16) rc = encode_tmap_bf16_sw(&tm[2], qkv, 2, dims, strides, qbox16, 32);
+  if (!rc && L::N16) rc = encode_tmap_bf16_sw(&tm[3], qkv, 2, dims, strides, kvbox16, 32);
   if (rc) return rc;
-  if (DH != 80) tm[2] = tm[0], tm[3] = tm[1];
+  if (!L::N16) tm[2] = tm[0], tm[3] = tm[1];
+  if (!L::N64) tm[0] = tm[2], tm[1] = tm[3];
   auto kern = attention_kernel<DH, KB, VARLEN, EMUL>;
   B200_ENSURE_SMEM(kern, L::BYTES);
   kern<<<grid, ATT_THREADS, L::BYTES, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
@@ -263,19 +305,25 @@ static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 
   return 0;
 }
 
+template <int DH, bool VARLEN>
+static int launch_attention_dh(const void* qkv, int T, const AttnParams& p, int kb, bool emul, dim3 grid,
+                               cudaStream_t st) {
+  if (kb == 128) return emul ? launch_attention_t<DH, 128, VARLEN, true>(qkv, T, p, grid, st)
+                             : launch_attention_t<DH, 128, VARLEN, false>(qkv, T, p, grid, st);
+  return emul ? launch_attention_t<DH, 64, VARLEN, true>(qkv, T, p, grid, st)
+              : launch_attention_t<DH, 64, VARLEN, false>(qkv, T, p, grid, st);
+}
+
+// one instance per width of head_width_ok() (dh 96 = 64 + 2 x 16 would fall out of the same slab scheme)
 template <bool VARLEN>
 static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, int kb, bool emul, dim3 grid,
                             cudaStream_t st) {
-  if (dh == 80) {
-    if (kb == 128) return emul ? launch_attention_t<80, 128, VARLEN, true>(qkv, T, p, grid, st)
-                               : launch_attention_t<80, 128, VARLEN, false>(qkv, T, p, grid, st);
-    return emul ? launch_attention_t<80, 64, VARLEN, true>(qkv, T, p, grid, st)
-                : launch_attention_t<80, 64, VARLEN, false>(qkv, T, p, grid, st);
+  switch (dh) {
+    case 32: return launch_attention_dh<32, VARLEN>(qkv, T, p, kb, emul, grid, st);
+    case 80: return launch_attention_dh<80, VARLEN>(qkv, T, p, kb, emul, grid, st);
+    case 128: return launch_attention_dh<128, VARLEN>(qkv, T, p, kb, emul, grid, st);
+    default: return launch_attention_dh<64, VARLEN>(qkv, T, p, kb, emul, grid, st);
   }
-  if (kb == 128) return emul ? launch_attention_t<64, 128, VARLEN, true>(qkv, T, p, grid, st)
-                             : launch_attention_t<64, 128, VARLEN, false>(qkv, T, p, grid, st);
-  return emul ? launch_attention_t<64, 64, VARLEN, true>(qkv, T, p, grid, st)
-              : launch_attention_t<64, 64, VARLEN, false>(qkv, T, p, grid, st);
 }
 
 // test hooks (include/b200vit.h)
@@ -300,7 +348,7 @@ extern "C" int b200vit_debug_set(int key, int value) {
 extern "C" int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* stream) {
   B200_CHECK_ARG(qkv && out, "attention: null pointer");
   B200_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention: bad shape B=%d N=%d H=%d", B, N, H);
-  B200_CHECK_ARG(dh == 64 || dh == 80, "attention: dim_head=%d not supported by this build (64 or 80)", dh);
+  B200_CHECK_ARG(head_width_ok(dh), "attention: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
   B200_CHECK_ARG(N <= 512, "attention: N=%d > 512 goes through b200vit_attention_varlen", N);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention: pointers must be 16-byte aligned");
@@ -321,7 +369,8 @@ extern "C" int b200vit_attention_varlen(const void* qkv, void* out, const int32_
                                         int H, int dh, float scale, void* stream) {
   B200_CHECK_ARG(qkv && out && cu_seqlens_dev && tile_prefix_dev, "attention_varlen: null pointer");
   B200_CHECK_ARG(num_seqs > 0 && total_tokens > 0 && total_tiles > 0 && H > 0, "attention_varlen: bad shape");
-  B200_CHECK_ARG(dh == 64 || dh == 80, "attention_varlen: dim_head=%d not supported by this build (64 or 80)", dh);
+  B200_CHECK_ARG(head_width_ok(dh), "attention_varlen: dim_head=%d not supported by this build (32, 64, 80 or 128)",
+                 dh);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention_varlen: pointers must be 16-byte aligned");
   B200_CHECK_ARG(H <= 65535, "attention_varlen: H=%d exceeds the grid", H);

@@ -514,8 +514,8 @@ extern "C" int b200vit_gemm_headnorm_bf16(const void* A, int64_t lda, const void
                                           int dh, float head_eps, int M, int N, int K, int flags, void* stream) {
   using namespace b200;
   B200_CHECK_ARG(out_bf16 && head_gamma, "gemm_headnorm: null pointer");
-  B200_CHECK_ARG(dh == 64, "gemm_headnorm: dim_head=%d not supported by this build (only 64)", dh);
-  B200_CHECK_ARG(norm_heads > 0 && norm_heads * 64 <= N, "gemm_headnorm: %d heads do not fit N=%d", norm_heads, N);
+  B200_CHECK_ARG(head_width_ok(dh), "gemm_headnorm: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
+  B200_CHECK_ARG(norm_heads > 0 && norm_heads * dh <= N, "gemm_headnorm: %d heads do not fit N=%d", norm_heads, N);
   B200_CHECK_ARG((flags & ~(B200VIT_EPI_BIAS | B200VIT_EPI_LNFOLD | B200VIT_EPI_HEADLN)) == 0,
                  "gemm_headnorm: unsupported flags %d", flags);
   const bool hln = (flags & B200VIT_EPI_HEADLN) != 0;

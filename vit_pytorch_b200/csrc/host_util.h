@@ -45,6 +45,9 @@ int encode_tmap_f32(CUtensorMap* tm, const void* base, int rank, const uint64_t*
 
 void tmap_cache_stats(int64_t* hits, int64_t* misses);
 
+// The head widths (dim_head) the attention, head-norm and pooling kernels are built for.
+inline bool head_width_ok(int dh) { return dh == 32 || dh == 64 || dh == 80 || dh == 128; }
+
 // test hook 12 (gemm.cu)
 void gemm_set_block_n(int v);
 

@@ -515,35 +515,50 @@ extern "C" int b200vit_cast_f32_bf16(const float* x, void* out_bf16, int64_t n, 
 // ---------------------------------------------------------------------------------------------------------------
 // NaViT: per-head q/k RMSNorm on the packed qkv buffer, in place (reference na_vit.py:93-101,149-150):
 //   v <- v / max(||v||_2, 1e-12) * sqrt(dh) * gamma[h, d]      for the q and k slices of every token and head.
-// gamma_qk: fp32 [2][H][dh] (q first), sqrt(dh) NOT folded in.  One warp per token, 2 elements per lane (dh = 64).
+// gamma_qk: fp32 [2][H][dh] (q first), sqrt(dh) NOT folded in.  One warp per token, 16 bytes per lane and step.
 // ---------------------------------------------------------------------------------------------------------------
 namespace b200 {
 
-// buf[T, ld] bf16: the `nheads` consecutive 64-wide heads starting at the row's column 0 are normalised in place.
-// One warp per token; 8 lanes per head (8 bf16 = 16 B each), so four heads are normalised per step with a 3-step
-// butterfly inside each 8-lane group; the loads of U steps are issued before the first reduction (a serial
-// load -> shuffle -> store chain per step left the kernel latency bound at a quarter of the HBM rate).
-// LN = true: LayerNorm over the head's 64 values without bias, (v - mean) * rsqrt(var + eps) * gamma -- the q / k norm
+template <int DH>
+struct HeadLanes {
+  static constexpr int CH = DH / 8;                                    // 16-byte chunks per head
+  static constexpr int LPH = CH <= 4 ? 4 : CH <= 8 ? 8 : 16;            // lanes per head: CH rounded up to a power of 2
+  static constexpr int HPS = 32 / LPH;                                 // heads per warp and step
+  static constexpr float SQRT_DH = DH == 32 ? 5.656854249492380f : DH == 64 ? 8.0f : DH == 80 ? 8.944271909999159f
+                                                                                            : 11.313708498984761f;
+  static_assert(CH * 8 == DH && CH <= 16, "head width");
+};
+
+// buf[T, ld] bf16: the `nheads` consecutive DH-wide heads starting at the row's column 0 are normalised in place.
+// One warp per token; LPH lanes per head (8 bf16 = 16 B each; dh 80 = 10 chunks leaves 6 of its 16 lanes idle, their
+// zeros join the sums), so HPS heads are normalised per step with a butterfly inside each LPH-lane group; the loads of
+// U steps are issued before the first reduction (a serial load -> shuffle -> store chain per step left the kernel
+// latency bound at a quarter of the HBM rate).
+// LN = true: LayerNorm over the head's DH values without bias, (v - mean) * rsqrt(var + eps) * gamma -- the q / k norm
 // of the nested-tensor NaViT (na_vit_nested_tensor.py:61-62,101-102) -- instead of the RMS norm.
-template <int U, bool LN>
+template <int DH, int U, bool LN>
 __global__ void __launch_bounds__(256)
 rmsnorm_heads_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float* __restrict__ gamma, int T,
                      int nheads, float eps) {
+  using HL = HeadLanes<DH>;
+  constexpr int LPH = HL::LPH, HPS = HL::HPS;
   const long long t = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (t >= T) return;
   __nv_bfloat16* row = buf + t * ld;
-  const int sub = lane & 7, grp = lane >> 3;
-  for (int base = 0; base < nheads; base += 4 * U) {
+  const int sub = lane % LPH, grp = lane / LPH;
+  const bool act = sub < HL::CH;  // (always true unless dh = 80)
+  for (int base = 0; base < nheads; base += HPS * U) {
     uint4 raw[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      const int hh = base + 4 * u + grp;  // (heads beyond nheads: the group only joins the shuffles)
-      raw[u] = *(reinterpret_cast<const uint4*>(row + (hh < nheads ? hh : 0) * 64) + sub);
+      const int hh = base + HPS * u + grp;  // (heads beyond nheads: the group only joins the shuffles)
+      raw[u] = act ? *(reinterpret_cast<const uint4*>(row + (hh < nheads ? hh : 0) * DH) + sub)
+                   : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      const int hh = base + 4 * u + grp;
+      const int hh = base + HPS * u + grp;
       __nv_bfloat162* h2 = reinterpret_cast<__nv_bfloat162*>(&raw[u]);
       float2 f[4];
       float ss = 0.f, s1 = 0.f;
@@ -553,65 +568,83 @@ rmsnorm_heads_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float*
         ss = fmaf(f[i].x, f[i].x, fmaf(f[i].y, f[i].y, ss));
         s1 += f[i].x + f[i].y;
       }
-      ss += __shfl_xor_sync(0xffffffffu, ss, 4);
-      ss += __shfl_xor_sync(0xffffffffu, ss, 2);
-      ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-      float inv = 8.0f / fmaxf(sqrtf(ss), 1e-12f);
+#pragma unroll
+      for (int o = LPH / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+      float inv = HL::SQRT_DH / fmaxf(sqrtf(ss), 1e-12f);
       if (LN) {
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 4);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-        const float mean = s1 * (1.0f / 64.0f);
-        inv = rsqrtf(fmaxf(ss * (1.0f / 64.0f) - mean * mean, 0.f) + eps);
+#pragma unroll
+        for (int o = LPH / 2; o > 0; o >>= 1) s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        const float mean = s1 * (1.0f / (float)DH);
+        inv = rsqrtf(fmaxf(ss * (1.0f / (float)DH) - mean * mean, 0.f) + eps);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           f[i].x -= mean;
           f[i].y -= mean;
         }
       }
-      if (hh < nheads) {
-        const float4 g0 = *reinterpret_cast<const float4*>(gamma + hh * 64 + 8 * sub);
-        const float4 g1 = *reinterpret_cast<const float4*>(gamma + hh * 64 + 8 * sub + 4);
+      if (hh < nheads && act) {
+        const float4 g0 = *reinterpret_cast<const float4*>(gamma + hh * DH + 8 * sub);
+        const float4 g1 = *reinterpret_cast<const float4*>(gamma + hh * DH + 8 * sub + 4);
         h2[0] = __floats2bfloat162_rn(f[0].x * inv * g0.x, f[0].y * inv * g0.y);
         h2[1] = __floats2bfloat162_rn(f[1].x * inv * g0.z, f[1].y * inv * g0.w);
         h2[2] = __floats2bfloat162_rn(f[2].x * inv * g1.x, f[2].y * inv * g1.y);
         h2[3] = __floats2bfloat162_rn(f[3].x * inv * g1.z, f[3].y * inv * g1.w);
-        *(reinterpret_cast<uint4*>(row + hh * 64) + sub) = raw[u];
+        *(reinterpret_cast<uint4*>(row + hh * DH) + sub) = raw[u];
       }
     }
   }
 }
 
 // NaViT attention pooling (reference na_vit.py:371-387): one learned query per image attends to that image's tokens.
-//   kv[T, 2*H*64] bf16 (k already RMS-normalised, then v), qn[H*64] fp32 (normalised query), sequences by cu_seqlens;
-//   out[S, H*64] bf16 = softmax_j(qn_h . k_jh) v_jh   (scale 1).  One CTA of 8 warps per (image, head): warp w walks the
+//   kv[T, 2*H*DH] bf16 (k already RMS-normalised, then v), qn[H*DH] fp32 (normalised query), sequences by cu_seqlens;
+//   out[S, H*DH] bf16 = softmax_j(qn_h . k_jh) v_jh   (scale 1).  One CTA of 8 warps per (image, head): warp w walks the
 //   token groups w, w + 8, ... (4 tokens each) with an online softmax, the 8 partial (max, sum, acc) are merged in
 //   shared memory -- a 1024-token image no longer takes 64x the time of a 16-token one on a single warp.
+//   Lane l owns the element pairs l, l + 32, ... of the head (NP = DH / 64 rounded up); pairs beyond DH / 2 (dh 32
+//   and 80) are masked: zero q, k and v, never stored.
+template <int DH>
 __global__ void __launch_bounds__(256)
 attn_pool_kernel(const __nv_bfloat16* __restrict__ kv, const float* __restrict__ qn, const int* __restrict__ cu,
                  __nv_bfloat16* __restrict__ out, int S, int H) {
   constexpr int NW = 8;
-  __shared__ float part[NW][4 + 64];   // m, l, -, -, acc[64]
+  constexpr int NP = (DH + 63) / 64;   // element pairs per lane
+  __shared__ float part[NW][4 + DH];   // m, l, -, -, acc[DH]
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int s = blockIdx.x / H, h = blockIdx.x % H;
-  const int I = H * 64;
-  const float2 q = *reinterpret_cast<const float2*>(qn + h * 64 + 2 * lane);
-  float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f;
+  const int I = H * DH;
+  bool act[NP];
+  float2 q[NP];
+#pragma unroll
+  for (int c = 0; c < NP; ++c) {
+    act[c] = 2 * (32 * c + lane) < DH;
+    q[c] = act[c] ? *reinterpret_cast<const float2*>(qn + h * DH + 2 * (32 * c + lane)) : make_float2(0.f, 0.f);
+  }
+  float m = -INFINITY, l = 0.f, a0[NP], a1[NP];
+#pragma unroll
+  for (int c = 0; c < NP; ++c) a0[c] = a1[c] = 0.f;
   const int j0 = cu[s], j1 = cu[s + 1];
   // four tokens per step: eight independent loads and four interleaved butterflies, one rescale of the running sums
   for (int j = j0 + 4 * warp; j < j1; j += 4 * NW) {
     const int cnt = j1 - j < 4 ? j1 - j : 4;
-    float2 k[4], v[4];
+    float2 k[4][NP], v[4][NP];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const __nv_bfloat16* r = kv + (long long)(j + (i < cnt ? i : 0)) * 2 * I + h * 64;
-      k[i] = __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(r) + lane));
-      v[i] = __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(r + I) + lane));
+      const __nv_bfloat16* r = kv + (long long)(j + (i < cnt ? i : 0)) * 2 * I + h * DH;
+#pragma unroll
+      for (int c = 0; c < NP; ++c) {
+        const float2 z = make_float2(0.f, 0.f);
+        k[i][c] = act[c] ? __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(r) + 32 * c + lane)) : z;
+        v[i][c] = act[c] ? __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(r + I) + 32 * c + lane)) : z;
+      }
     }
     float sc[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) sc[i] = q.x * k[i].x + q.y * k[i].y;
+    for (int i = 0; i < 4; ++i) {
+      sc[i] = q[0].x * k[i][0].x + q[0].y * k[i][0].y;
+#pragma unroll
+      for (int c = 1; c < NP; ++c) sc[i] += q[c].x * k[i][c].x + q[c].y * k[i][c].y;
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
@@ -622,13 +655,21 @@ attn_pool_kernel(const __nv_bfloat16* __restrict__ kv, const float* __restrict__
       if (i >= cnt) sc[i] = -INFINITY;         // tail group: the duplicated token 0 gets weight 0
     const float mn = fmaxf(fmaxf(m, fmaxf(sc[0], sc[1])), fmaxf(sc[2], sc[3]));
     const float corr = __expf(m - mn);
-    l *= corr; a0 *= corr; a1 *= corr;
+    l *= corr;
+#pragma unroll
+    for (int c = 0; c < NP; ++c) {
+      a0[c] *= corr;
+      a1[c] *= corr;
+    }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float pj = __expf(sc[i] - mn);
       l += pj;
-      a0 = fmaf(pj, v[i].x, a0);
-      a1 = fmaf(pj, v[i].y, a1);
+#pragma unroll
+      for (int c = 0; c < NP; ++c) {
+        a0[c] = fmaf(pj, v[i][c].x, a0[c]);
+        a1[c] = fmaf(pj, v[i][c].y, a1[c]);
+      }
     }
     m = mn;
   }
@@ -636,23 +677,32 @@ attn_pool_kernel(const __nv_bfloat16* __restrict__ kv, const float* __restrict__
     part[warp][0] = m;
     part[warp][1] = l;
   }
-  part[warp][4 + 2 * lane] = a0;
-  part[warp][5 + 2 * lane] = a1;
+#pragma unroll
+  for (int c = 0; c < NP; ++c)
+    if (act[c]) {
+      part[warp][4 + 2 * (32 * c + lane)] = a0[c];
+      part[warp][5 + 2 * (32 * c + lane)] = a1[c];
+    }
   __syncthreads();
   if (warp == 0) {
     float mm = -INFINITY;
 #pragma unroll
     for (int w = 0; w < NW; ++w) mm = fmaxf(mm, part[w][0]);
-    float L = 0.f, A0 = 0.f, A1 = 0.f;
 #pragma unroll
-    for (int w = 0; w < NW; ++w) {
-      const float f = part[w][0] == -INFINITY ? 0.f : __expf(part[w][0] - mm);   // warps without a token
-      L = fmaf(part[w][1], f, L);
-      A0 = fmaf(part[w][4 + 2 * lane], f, A0);
-      A1 = fmaf(part[w][5 + 2 * lane], f, A1);
+    for (int c = 0; c < NP; ++c) {
+      if (!act[c]) continue;
+      const int e = 2 * (32 * c + lane);
+      float L = 0.f, A0 = 0.f, A1 = 0.f;
+#pragma unroll
+      for (int w = 0; w < NW; ++w) {
+        const float f = part[w][0] == -INFINITY ? 0.f : __expf(part[w][0] - mm);   // warps without a token
+        L = fmaf(part[w][1], f, L);
+        A0 = fmaf(part[w][4 + e], f, A0);
+        A1 = fmaf(part[w][5 + e], f, A1);
+      }
+      const float inv = 1.0f / L;
+      *reinterpret_cast<__nv_bfloat162*>(out + (long long)s * I + h * DH + e) = __floats2bfloat162_rn(A0 * inv, A1 * inv);
     }
-    const float inv = 1.0f / L;
-    *(reinterpret_cast<__nv_bfloat162*>(out + (long long)s * I + h * 64) + lane) = __floats2bfloat162_rn(A0 * inv, A1 * inv);
   }
 }
 
@@ -717,16 +767,40 @@ embed_varlen_kernel(const float* __restrict__ y, const float* __restrict__ gamma
 
 }  // namespace b200
 
+// one launch of rmsnorm_heads_kernel<DH, U, LN> for a runtime dh (checked by the caller)
+template <bool LN>
+static void launch_heads_norm(__nv_bfloat16* b, int64_t ld, const float* gamma, int T, int nheads, int dh, float eps,
+                              cudaStream_t st) {
+  const dim3 grid((T + 7) / 8);
+  const bool big = nheads > 8;
+  switch (dh) {
+    case 32:
+      if (big) b200::rmsnorm_heads_kernel<32, 4, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      else b200::rmsnorm_heads_kernel<32, 2, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      break;
+    case 80:
+      if (big) b200::rmsnorm_heads_kernel<80, 4, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      else b200::rmsnorm_heads_kernel<80, 2, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      break;
+    case 128:
+      if (big) b200::rmsnorm_heads_kernel<128, 4, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      else b200::rmsnorm_heads_kernel<128, 2, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      break;
+    default:
+      if (big) b200::rmsnorm_heads_kernel<64, 4, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+      else b200::rmsnorm_heads_kernel<64, 2, LN><<<grid, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+  }
+}
+
 extern "C" int b200vit_layernorm_heads(void* buf, int64_t ld, const float* gamma, int T, int nheads, int dh, float eps,
                                        void* stream) {
   B200_CHECK_ARG(buf && gamma && T > 0 && nheads > 0, "layernorm_heads: bad argument");
-  B200_CHECK_ARG(dh == 64, "layernorm_heads: dim_head=%d not supported by this build (only 64)", dh);
-  B200_CHECK_ARG(ld >= (int64_t)nheads * 64 && (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0,
-                 "layernorm_heads: rows must be 16-byte aligned and hold nheads*64 columns (ld=%lld)", (long long)ld);
-  auto st = reinterpret_cast<cudaStream_t>(stream);
-  auto b = reinterpret_cast<__nv_bfloat16*>(buf);
-  if (nheads > 8) b200::rmsnorm_heads_kernel<4, true><<<(T + 7) / 8, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
-  else b200::rmsnorm_heads_kernel<2, true><<<(T + 7) / 8, 256, 0, st>>>(b, ld, gamma, T, nheads, eps);
+  B200_CHECK_ARG(head_width_ok(dh), "layernorm_heads: dim_head=%d not supported by this build (32, 64, 80 or 128)",
+                 dh);
+  B200_CHECK_ARG(ld >= (int64_t)nheads * dh && (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0,
+                 "layernorm_heads: rows must be 16-byte aligned and hold nheads*dh columns (ld=%lld)", (long long)ld);
+  launch_heads_norm<true>(reinterpret_cast<__nv_bfloat16*>(buf), ld, gamma, T, nheads, dh, eps,
+                          reinterpret_cast<cudaStream_t>(stream));
   B200_CHECK_CUDA(cudaGetLastError());
   b200::count_launch();
   return 0;
@@ -735,13 +809,12 @@ extern "C" int b200vit_layernorm_heads(void* buf, int64_t ld, const float* gamma
 extern "C" int b200vit_rmsnorm_heads(void* buf, int64_t ld, const float* gamma, int T, int nheads, int dh,
                                      void* stream) {
   B200_CHECK_ARG(buf && gamma && T > 0 && nheads > 0, "rmsnorm_heads: bad argument");
-  B200_CHECK_ARG(dh == 64, "rmsnorm_heads: dim_head=%d not supported by this build (only 64)", dh);
-  B200_CHECK_ARG(ld >= (int64_t)nheads * 64 && (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0,
-                 "rmsnorm_heads: rows must be 16-byte aligned and hold nheads*64 columns (ld=%lld)", (long long)ld);
-  auto st = reinterpret_cast<cudaStream_t>(stream);
-  auto b = reinterpret_cast<__nv_bfloat16*>(buf);
-  if (nheads > 8) b200::rmsnorm_heads_kernel<4, false><<<(T + 7) / 8, 256, 0, st>>>(b, ld, gamma, T, nheads, 0.f);
-  else b200::rmsnorm_heads_kernel<2, false><<<(T + 7) / 8, 256, 0, st>>>(b, ld, gamma, T, nheads, 0.f);
+  B200_CHECK_ARG(head_width_ok(dh), "rmsnorm_heads: dim_head=%d not supported by this build (32, 64, 80 or 128)",
+                 dh);
+  B200_CHECK_ARG(ld >= (int64_t)nheads * dh && (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0,
+                 "rmsnorm_heads: rows must be 16-byte aligned and hold nheads*dh columns (ld=%lld)", (long long)ld);
+  launch_heads_norm<false>(reinterpret_cast<__nv_bfloat16*>(buf), ld, gamma, T, nheads, dh, 0.f,
+                           reinterpret_cast<cudaStream_t>(stream));
   B200_CHECK_CUDA(cudaGetLastError());
   b200::count_launch();
   return 0;
@@ -749,8 +822,9 @@ extern "C" int b200vit_rmsnorm_heads(void* buf, int64_t ld, const float* gamma, 
 
 extern "C" int b200vit_qk_rmsnorm(void* qkv, const float* gamma_qk, int T, int H, int dh, void* stream) {
   B200_CHECK_ARG(qkv && gamma_qk && T > 0 && H > 0, "qk_rmsnorm: bad argument");
-  B200_CHECK_ARG(dh == 64, "qk_rmsnorm: dim_head=%d not supported by this build (only 64)", dh);
-  return b200vit_rmsnorm_heads(qkv, (int64_t)3 * H * 64, gamma_qk, T, 2 * H, dh, stream);  // q heads, then k heads
+  B200_CHECK_ARG(head_width_ok(dh), "qk_rmsnorm: dim_head=%d not supported by this build (32, 64, 80 or 128)",
+                 dh);
+  return b200vit_rmsnorm_heads(qkv, (int64_t)3 * H * dh, gamma_qk, T, 2 * H, dh, stream);  // q heads, then k heads
 }
 
 extern "C" int b200vit_embed_varlen(const float* y, const float* gamma, const float* pos_h, const float* pos_w,
@@ -771,9 +845,16 @@ extern "C" int b200vit_embed_varlen(const float* y, const float* gamma, const fl
 extern "C" int b200vit_attn_pool(const void* kv, const float* qn, const int32_t* cu_seqlens_dev, void* out, int S,
                                  int H, int dh, void* stream) {
   B200_CHECK_ARG(kv && qn && cu_seqlens_dev && out && S > 0 && H > 0, "attn_pool: bad argument");
-  B200_CHECK_ARG(dh == 64, "attn_pool: dim_head=%d not supported by this build (only 64)", dh);
-  attn_pool_kernel<<<S * H, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(kv), qn, cu_seqlens_dev, reinterpret_cast<__nv_bfloat16*>(out), S, H);
+  B200_CHECK_ARG(head_width_ok(dh), "attn_pool: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
+  const auto* k = reinterpret_cast<const __nv_bfloat16*>(kv);
+  auto* o = reinterpret_cast<__nv_bfloat16*>(out);
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  switch (dh) {
+    case 32: attn_pool_kernel<32><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H); break;
+    case 80: attn_pool_kernel<80><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H); break;
+    case 128: attn_pool_kernel<128><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H); break;
+    default: attn_pool_kernel<64><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H);
+  }
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;

@@ -113,6 +113,17 @@ def why_not_fused(params: List[torch.Tensor], x: torch.Tensor, *, training: bool
     return None
 
 
+HEAD_WIDTHS = (32, 64, 80, 128)
+
+
+def head_width_reason(dh: int) -> Optional[str]:
+    """None if the attention, head-norm and pooling kernels are built for heads `dh` wide, else the reason the eager
+    PyTorch graph is used.  One rule for every model family."""
+    if dh not in HEAD_WIDTHS:
+        return f"dim_head={dh} (the attention kernels are built for 32, 64, 80 and 128)"
+    return None
+
+
 class Norm(NamedTuple):
     """A LayerNorm over the feature dim.  beta None: the norm has no shift."""
     gamma: torch.Tensor
@@ -250,10 +261,9 @@ class TransformerEngine:
     def unsupported_reason(self, N: int) -> Optional[str]:
         # only shapes are read, and a module's shapes are fixed at construction: any description of it serves
         for L in self.layers or self.mod.encoder_layers()[0]:
-            if L.dim_head not in (64, 80):
-                return f"dim_head={L.dim_head} (the attention kernels are built for 64 and 80)"
-            if L.dim_head == 80 and (N > 512 or L.qk_norm is not None):
-                return "dim_head=80 is built for the single-pass attention kernel (N <= 512, no q/k norm) only"
+            r = head_width_reason(L.dim_head)
+            if r is not None:
+                return r
             if L.qkv_w.shape[1] % 8 or L.fc1_w.shape[0] % 8:
                 return "dim / mlp_dim not multiples of 8"
         if N > 16384:

@@ -25,8 +25,8 @@ import torch.nn.functional as F
 from torch import Tensor, nn
 
 from . import _lib
-from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, hooks_inside, ln_mode,
-                     on_device, why_not_fused)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, head_width_reason,
+                     hooks_inside, ln_mode, on_device, why_not_fused)
 
 
 def group_images_by_max_seq_len(images: Sequence[Tensor], patch_size: int,
@@ -212,8 +212,8 @@ class NaViT(FusedWeightsMixin, nn.Module):
             r = "token dropout is active"
         if r is None and hooks_inside(self, skip=(self.to_latent,)):
             r = "forward hooks registered inside the model"
-        if r is None and attn0.to_q.weight.shape[0] // attn0.heads != 64:
-            r = "dim_head != 64 (the attention kernels are built for 64)"
+        if r is None:
+            r = head_width_reason(attn0.to_q.weight.shape[0] // attn0.heads)
         if r is None and (self.pos_embed_height.shape[1] % 8 or (self.channels * self.patch_size ** 2) % 8):
             r = "dim / patch_dim not multiples of 8"
         return r
@@ -267,6 +267,7 @@ class NaViT(FusedWeightsMixin, nn.Module):
         heads = self.attn_pool.heads
         D = t["pos_h"].shape[1]
         I = t["pool.out"].shape[1]
+        dh = I // heads
         max_gh, max_gw = self.pos_embed_height.shape[0], self.pos_embed_width.shape[0]
         for img in images:
             assert img.ndim == 3 and img.shape[0] == c
@@ -300,9 +301,10 @@ class NaViT(FusedWeightsMixin, nn.Module):
         eng.final_norm(x, out_bf16=xn)
         # ---- attention pooling: one query per image over that image's (un-normalised-again) tokens (na_vit.py:371-387)
         kv = torch.empty(T, 2 * I, **bf16)
-        _lib.gemm_headnorm(xn, t["pool.kv"], out_bf16=kv, head_gamma=t["pool.gk"], norm_heads=heads)   # k half only
+        _lib.gemm_headnorm(xn, t["pool.kv"], out_bf16=kv, head_gamma=t["pool.gk"], norm_heads=heads,   # k half only
+                           dh=dh)
         pooled = torch.empty(S, I, **bf16)
-        _lib.attn_pool(kv, t["pool.qn"], ix.cu, pooled, heads, 64)
+        _lib.attn_pool(kv, t["pool.qn"], ix.cu, pooled, heads, dh)
         z = t["pool.queries"][None, :].expand(S, -1).contiguous()
         _lib.gemm(pooled, t["pool.out"], out_f32=z, resid=z)                      # + queries
         zl = torch.empty(S, D, **bf16)

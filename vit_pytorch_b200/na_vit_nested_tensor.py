@@ -24,8 +24,8 @@ import torch.nn.functional as F
 from torch import Tensor, nn
 
 from . import _lib
-from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, hooks_inside, ln_mode,
-                     on_device, why_not_fused)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, head_width_reason,
+                     hooks_inside, ln_mode, on_device, why_not_fused)
 
 
 def FeedForward(dim: int, hidden_dim: int, dropout: float = 0.) -> nn.Sequential:
@@ -189,8 +189,8 @@ class NaViT(FusedWeightsMixin, nn.Module):
             r = "token dropout is active"
         if r is None and hooks_inside(self, skip=(self.to_latent,)):
             r = "forward hooks registered inside the model"
-        if r is None and self.attn_pool.dim_head != 64:
-            r = "dim_head != 64 (the attention kernels are built for 64)"
+        if r is None:
+            r = head_width_reason(self.attn_pool.dim_head)
         if r is None and (self.pos_embed_height.shape[1] % 8 or (self.channels * self.patch_size ** 2) % 8):
             r = "dim / patch_dim not multiples of 8"
         return r
@@ -273,7 +273,7 @@ class NaViT(FusedWeightsMixin, nn.Module):
         if t["pool.gk"] is None:
             _lib.gemm(xn, t["pool.kv"], out_bf16=kv)
         else:
-            _lib.gemm_headnorm(xn, t["pool.kv"], out_bf16=kv, head_gamma=t["pool.gk"], norm_heads=heads,
+            _lib.gemm_headnorm(xn, t["pool.kv"], out_bf16=kv, head_gamma=t["pool.gk"], norm_heads=heads, dh=dh,
                                head_layernorm_eps=pool.key_norm.eps)
         pooled = torch.empty(S, I, **bf16)
         _lib.attn_pool(kv, t["pool.qn"], ix.cu, pooled, heads, dh)
