@@ -92,10 +92,22 @@ int b200vit_patchify_ln(const void* img, const float* gamma, const float* beta, 
  * written as the fp32 residual stream x[B*(ncls+n+ntail), D].  Optional (may be NULL): xb_bf16 = bf16 copy of x and
  * stats[M][2] = per-row (sum, sum of squares) of that copy -- the inputs of the first LN-folded GEMM.
  * Replaces nn.LayerNorm(dim) vit.py:103, cls concat vit.py:122-123, pos add vit.py:125-127 (simple_vit.py:94,114).
+ * pos == NULL: no positional term at all (the rotary ViTND, vit_nd_rotary.py:272-287, positions act on q / k instead).
  */
 int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, const float* cls, const float* pos,
                          const float* tail, float* x, void* xb_bf16, float* stats, int B, int n, int ncls, int ntail,
                          int D, float eps, void* stream);
+
+/*
+ * N-d patchify without a LayerNorm (vit_nd.py:130-145 / vit_nd_rotary.py:216-231, 'b c (f p0) (g p1) ... ->
+ * b (f g ...) (p0 p1 ... c)'): img[B, C, S_0 .. S_{r-1}] (bf16, contiguous), rank r = 1..7, patch[i] dividing shape[i]
+ * (shape / patch: HOST int arrays of r entries) -> A[B*n, ldo] bf16, n = prod(S_i / p_i), with
+ *   A[b*n + rowmajor(g_0 .. g_{r-1}), rowmajor(q_0 .. q_{r-1})*C + c] = img[b, c, g_0*p_0 + q_0, ..., g_{r-1}*p_{r-1} + q_{r-1}]
+ * as bit copies.  Columns [C * prod(p_i), ldo) are zero filled (K padding for the GEMM).  ldo multiple of 8, out_bf16
+ * 16-byte aligned.
+ */
+int b200vit_patchify_nd(const void* img, void* out_bf16, int64_t ldo, int B, int C, int rank, const int* shape,
+                        const int* patch, void* stream);
 
 /*
  * im2col-free patch embedding for 16 x 16 patches (vit.py:100-102 without materialising the Rearrange or the
@@ -170,6 +182,17 @@ int b200vit_gemm_headnorm_bf16(const void* A, int64_t lda, const void* W, int64_
                                int M, int N, int K, int flags, void* stream);
 
 /*
+ * Golden-gate N-d rotary embedding of q and k, in place on the packed qkv[T, 3*H*dh] buffer (v untouched;
+ * GoldenGateRoPENd.forward, vit_nd_rotary.py:74-96, applied at :143-147).  cs fp32 [R][H][dh/2][2] = (cos, sin) of
+ * theta; token t uses table row t % R (R = N: every image shares one patch grid; R = T: positions given per token).
+ * For every head and f < dh/2, with x = head[f], y = head[f + dh/2]:
+ *   x' = x cos - y sin,   y' = x sin + y cos
+ * in fp32 with every product and sum rounded on its own (no FMA), then rounded to bf16: bit-identical to the
+ * reference's expression for the same bf16 q / k and the same table.  qkv and cs 16-byte aligned.
+ */
+int b200vit_rope_qk(void* qkv, const float* cs, int R, int T, int H, int dh, void* stream);
+
+/*
  * The same normalisation on any row-major bf16 buffer: the `nheads` consecutive dh-wide heads that start at column 0
  * of every row buf[t*ld ...] (the k half of a [k | v] buffer for the attention pooling, na_vit.py:143-150);
  * gamma fp32 [nheads][dh].  ld in elements, multiple of 8; buf 16-byte aligned.
@@ -240,6 +263,12 @@ int b200vit_encoder_blocks(const b200vit_layer* layers, int depth, float* x, con
                            int D, int heads, int dh, int hidden, float scale, int primed,
                            const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev, int total_tiles,
                            void* stream);
+/* ... with rotary positions: b200vit_rope_qk(ws->qkv, rope_cs, rope_rows, ...) runs right after every layer's QKV GEMM
+ * (vit_nd_rotary.py:137-147).  b200vit_encoder_blocks is this call with rope_cs = NULL. */
+int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int depth, float* x, const b200vit_encoder_ws* ws, int B,
+                                int N, int D, int heads, int dh, int hidden, float scale, int primed,
+                                const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev, int total_tiles,
+                                const float* rope_cs, int rope_rows, void* stream);
 
 /*
  * TEST HOOKS -- process-global switches for A/B tests and bring-up; NOT part of the re-entrant API above (a value set

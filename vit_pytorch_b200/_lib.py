@@ -31,7 +31,7 @@ SYMBOLS = [
     "b200vit_stats_parts", "b200vit_attention_varlen", "b200vit_qk_rmsnorm", "b200vit_attn_pool",
     "b200vit_patchify_varlen_ln", "b200vit_rmsnorm_heads", "b200vit_embed_varlen",
     "b200vit_gemm_headnorm_bf16", "b200vit_layernorm_heads", "b200vit_patch_stats", "b200vit_patch_embed_tma",
-    "b200vit_encoder_blocks",
+    "b200vit_encoder_blocks", "b200vit_patchify_nd", "b200vit_rope_qk", "b200vit_encoder_blocks_rope",
 ]
 
 
@@ -118,6 +118,13 @@ def lib() -> C.CDLL:
     L.b200vit_encoder_blocks.restype = i32
     L.b200vit_encoder_blocks.argtypes = [C.POINTER(Layer), i32, vp, C.POINTER(EncoderWs), i32, i32, i32, i32, i32, i32,
                                          f32, i32, vp, vp, i32, vp]
+    L.b200vit_encoder_blocks_rope.restype = i32
+    L.b200vit_encoder_blocks_rope.argtypes = [C.POINTER(Layer), i32, vp, C.POINTER(EncoderWs), i32, i32, i32, i32, i32,
+                                              i32, f32, i32, vp, vp, i32, vp, i32, vp]
+    L.b200vit_patchify_nd.restype = i32
+    L.b200vit_patchify_nd.argtypes = [vp, vp, i64, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), vp]
+    L.b200vit_rope_qk.restype = i32
+    L.b200vit_rope_qk.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     _lib = L
     return L
 
@@ -183,14 +190,24 @@ def profiling() -> bool:
 
 
 def encoder_blocks(layers, depth: int, x: torch.Tensor, ws: "EncoderWs", B: int, N: int, D: int, heads: int, dh: int,
-                   hidden: int, scale: float, primed: bool, varlen=None) -> None:
+                   hidden: int, scale: float, primed: bool, varlen=None, rope=None) -> None:
     """All encoder layers in one library call (b200vit_encoder_blocks).  `layers`: ctypes array of Layer built from the
-    prepared weights; `ws`: EncoderWs over the engine's workspace; `varlen`: (cu, tile_prefix, total_tiles) if N > 512."""
+    prepared weights; `ws`: EncoderWs over the engine's workspace; `varlen`: (cu, tile_prefix, total_tiles) if N > 512;
+    `rope`: (cs table, rows) of rope_qk, applied after every QKV GEMM (b200vit_encoder_blocks_rope)."""
     _chk(x, torch.float32, "x")
     cu, tp, tiles = varlen if varlen is not None else (None, None, 0)
-    rc = lib().b200vit_encoder_blocks(layers, depth, _ptr(x), C.byref(ws), B, N, D, heads, dh, hidden, float(scale),
-                                      1 if primed else 0, _ptr(cu), _ptr(tp), int(tiles), _stream())
-    _check(rc, "b200vit_encoder_blocks")
+    if rope is None:
+        rc = lib().b200vit_encoder_blocks(layers, depth, _ptr(x), C.byref(ws), B, N, D, heads, dh, hidden,
+                                          float(scale), 1 if primed else 0, _ptr(cu), _ptr(tp), int(tiles), _stream())
+        _check(rc, "b200vit_encoder_blocks")
+        return
+    cs, rows = rope
+    _chk(cs, torch.float32, "rope table")
+    assert cs.is_contiguous()
+    rc = lib().b200vit_encoder_blocks_rope(layers, depth, _ptr(x), C.byref(ws), B, N, D, heads, dh, hidden,
+                                           float(scale), 1 if primed else 0, _ptr(cu), _ptr(tp), int(tiles), _ptr(cs),
+                                           int(rows), _stream())
+    _check(rc, "b200vit_encoder_blocks_rope")
 
 
 def launch_count() -> int:
@@ -329,6 +346,31 @@ def patchify_ln(img: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out_
     _check(rc, "b200vit_patchify_ln")
 
 
+def patchify_nd(img: torch.Tensor, out_bf16: torch.Tensor, patch) -> None:
+    """img [B, C, S_0 .. S_{r-1}] bf16 -> out [B*n, ldo] with the (p0 .. p_{r-1} c) patch rows, zero K padding."""
+    _chk(img, torch.bfloat16, "img"); _chk(out_bf16, torch.bfloat16, "out")
+    assert img.is_contiguous() and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    B, Cc, *shape = img.shape
+    r = len(shape)
+    shp, pat = (C.c_int * max(r, 1))(*shape), (C.c_int * max(r, 1))(*patch)
+    with _Timed("patchify_nd", bytes=img.numel() * 2 + out_bf16.shape[0] * out_bf16.stride(0) * 2):
+        rc = lib().b200vit_patchify_nd(_ptr(img), _ptr(out_bf16), out_bf16.stride(0), B, Cc, r, shp, pat, _stream())
+    _check(rc, "b200vit_patchify_nd")
+
+
+def rope_qk(qkv: torch.Tensor, cs: torch.Tensor, rows: int, H: int, dh: int) -> None:
+    """Rotate the q and k slices of qkv[T, 3*H*dh] in place with the (cos, sin) table cs[rows, H, dh/2, 2]; token t
+    uses table row t % rows."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(cs, torch.float32, "cs")
+    assert qkv.is_contiguous() and cs.is_contiguous() and cs.numel() == rows * H * dh
+    T = qkv.shape[0]
+    assert qkv.shape[1] == 3 * H * dh
+    # q and k read and written once (bf16) + the table (fp32)
+    with _Timed("rope_qk", bytes=T * 2 * H * dh * 4 + cs.numel() * 4):
+        rc = lib().b200vit_rope_qk(_ptr(qkv), _ptr(cs), int(rows), T, H, dh, _stream())
+    _check(rc, "b200vit_rope_qk")
+
+
 def patch_embed_tma(img: torch.Tensor, w_perm: torch.Tensor, bias: torch.Tensor, col_s: torch.Tensor,
                     stats: torch.Tensor, out_f32: torch.Tensor, eps: float = 1e-5) -> None:
     """out_f32[B*n, D] = LayerNorm(16x16 patches of img) @ W^T + b, the image read through a 5-D TMA map (no patch
@@ -351,17 +393,19 @@ def patch_embed_tma(img: torch.Tensor, w_perm: torch.Tensor, bias: torch.Tensor,
 
 
 def embed_tokens(y: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, cls: Optional[torch.Tensor],
-                 pos: torch.Tensor, x: torch.Tensor, B: int, n: int, ncls: int, eps: float = 1e-5,
+                 pos: Optional[torch.Tensor], x: torch.Tensor, B: int, n: int, ncls: int, eps: float = 1e-5,
                  xb: Optional[torch.Tensor] = None, stats: Optional[torch.Tensor] = None,
                  tail: Optional[torch.Tensor] = None) -> None:
-    """tail [ntail, D]: rows appended after the n patch tokens of every image (register tokens, no pos)."""
+    """tail [ntail, D]: rows appended after the n patch tokens of every image (register tokens, no pos).
+    pos None: no positional term."""
     _chk(xb, torch.bfloat16, "xb"); _chk(stats, torch.float32, "stats")
     for nm, t in (("y", y), ("gamma", gamma), ("beta", beta), ("cls", cls), ("pos", pos), ("x", x), ("tail", tail)):
         _chk(t, torch.float32, nm)
     D = y.shape[1]
     ntail = 0 if tail is None else tail.shape[0]
-    assert y.is_contiguous() and x.is_contiguous() and pos.is_contiguous() and (tail is None or tail.is_contiguous())
-    assert x.shape[0] == B * (n + ncls + ntail) and pos.shape[0] >= n + ncls
+    assert y.is_contiguous() and x.is_contiguous() and (tail is None or tail.is_contiguous())
+    assert x.shape[0] == B * (n + ncls + ntail)
+    assert pos is None or (pos.is_contiguous() and pos.shape[0] >= n + ncls)
     with _Timed("embed_tokens", bytes=(y.numel() + x.numel()) * 4):
         rc = lib().b200vit_embed_tokens(_ptr(y), _ptr(gamma), _ptr(beta), _ptr(cls), _ptr(pos), _ptr(tail), _ptr(x),
                                         _ptr(xb), _ptr(stats), B, n, ncls, ntail, D, float(eps), _stream())

@@ -4,6 +4,7 @@
 //   ->  FC1 GEMM (LN fold + bias + GELU)  ->  FC2 GEMM (+ bias + residual, bf16 copy, row stats).
 // Nothing here touches the device itself: it is the host-side loop, moved below the language boundary so that a Python
 // (ctypes) or C++ host pays one call instead of 5 x depth -- at small batches the forward is host bound.
+// With a rope table (b200vit_encoder_blocks_rope) a sixth launch rotates q and k right after the QKV GEMM.
 #include "../../include/b200vit.h"
 #include "host_util.h"
 
@@ -17,12 +18,22 @@ extern "C" int b200vit_encoder_blocks(const b200vit_layer* layers, int depth, fl
                                       int B, int N, int D, int heads, int dh, int hidden, float scale, int primed,
                                       const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev, int total_tiles,
                                       void* stream) {
+  return b200vit_encoder_blocks_rope(layers, depth, x, ws, B, N, D, heads, dh, hidden, scale, primed, cu_seqlens_dev,
+                                     tile_prefix_dev, total_tiles, nullptr, 0, stream);
+}
+
+extern "C" int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int depth, float* x,
+                                           const b200vit_encoder_ws* ws, int B, int N, int D, int heads, int dh,
+                                           int hidden, float scale, int primed, const int32_t* cu_seqlens_dev,
+                                           const int32_t* tile_prefix_dev, int total_tiles, const float* rope_cs,
+                                           int rope_rows, void* stream) {
   B200_CHECK_ARG(layers && x && ws && depth > 0, "encoder_blocks: null pointer / depth %d", depth);
   B200_CHECK_ARG(B > 0 && N > 0 && D > 0 && heads > 0 && hidden > 0, "encoder_blocks: bad shape");
   B200_CHECK_ARG(ws->xb && ws->qkv && ws->o && ws->h && ws->stats_in && ws->stats_a && ws->stats_b,
                  "encoder_blocks: incomplete workspace");
   B200_CHECK_ARG(N <= 512 || (cu_seqlens_dev && tile_prefix_dev && total_tiles > 0),
                  "encoder_blocks: N = %d > 512 needs the varlen index (cu_seqlens, tile_prefix)", N);
+  B200_CHECK_ARG(!rope_cs || rope_rows > 0, "encoder_blocks: rope table with %d rows", rope_rows);
   const int M = B * N, I = heads * dh;
   const int parts = b200vit_stats_parts(D);
   int rc = 0;
@@ -45,6 +56,11 @@ extern "C" int b200vit_encoder_blocks(const b200vit_layer* layers, int depth, fl
       rc = b200vit_gemm_bf16(ws->xb, D, L.qkv_wg, D, ws->qkv, nullptr, 3 * I, L.qkv_t, nullptr, sums, sum_parts,
                              L.ln1_eps, L.qkv_s, nullptr, M, 3 * I, D, B200VIT_EPI_BIAS | B200VIT_EPI_LNFOLD, stream);
     if (rc) return rc;
+    // rotary positions on q and k   (vit_nd_rotary.py:143-147)
+    if (rope_cs) {
+      rc = b200vit_rope_qk(ws->qkv, rope_cs, rope_rows, M, heads, dh, stream);
+      if (rc) return rc;
+    }
     // softmax(q k^T * scale) v, heads merged   (vit.py:55-63)
     if (N <= 512)
       rc = b200vit_attention(ws->qkv, ws->o, B, N, heads, dh, scale, stream);

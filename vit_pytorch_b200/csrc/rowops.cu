@@ -286,6 +286,8 @@ patchify_ln16c3_kernel(const __nv_bfloat16* __restrict__ img, const float* __res
 // ---------------------------------------------------------------------------------------------------------------
 // Token assembly: LN(dim) of the patch projection + positional embedding + cls row  -> fp32 residual stream
 // ---------------------------------------------------------------------------------------------------------------
+// POS = false: no positional term (vit_nd_rotary.py:272-287 has no table; rotary positions act on q / k instead)
+template <bool POS>
 __global__ void __launch_bounds__(256)
 embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma, const float* __restrict__ beta,
                     const float* __restrict__ cls, const float* __restrict__ pos, float* __restrict__ x,
@@ -298,7 +300,7 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
   const int b = (int)(row / N), t = (int)(row % N);
   float* xr = x + row * D;
   __nv_bfloat16* xbr = xb ? xb + row * D : nullptr;
-  const float* pr = pos + (long long)min(t, n + ncls - 1) * D;  // (tail rows carry no positional embedding)
+  const float* pr = POS ? pos + (long long)min(t, n + ncls - 1) * D : nullptr;  // (tail rows carry no positional embedding)
   float s1 = 0.f, s2 = 0.f;  // sum / sum of squares of the bf16-rounded row (LN-fold statistics for the first layer)
   auto emit = [&](int i, float v) {
     xr[i] = v;
@@ -309,7 +311,7 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
     s2 = fmaf(vr, vr, s2);
   };
   if (t < ncls) {
-    for (int i = lane; i < D; i += 32) emit(i, cls[(long long)t * D + i] + pr[i]);
+    for (int i = lane; i < D; i += 32) emit(i, POS ? cls[(long long)t * D + i] + pr[i] : cls[(long long)t * D + i]);
   } else if (t >= ncls + n) {  // register tokens appended after the patches (simple_vit_with_register_tokens.py:124-126)
     for (int i = lane; i < D; i += 32) emit(i, tail[(long long)(t - ncls - n) * D + i]);
   } else {
@@ -321,12 +323,19 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
         const float4 v = *reinterpret_cast<const float4*>(yr + i);
         const float4 g = *reinterpret_cast<const float4*>(gamma + i);
         const float4 be = *reinterpret_cast<const float4*>(beta + i);
-        const float4 p = *reinterpret_cast<const float4*>(pr + i);
         float4 o;
-        o.x = ((v.x - mean) * rstd * g.x + be.x) + p.x;
-        o.y = ((v.y - mean) * rstd * g.y + be.y) + p.y;
-        o.z = ((v.z - mean) * rstd * g.z + be.z) + p.z;
-        o.w = ((v.w - mean) * rstd * g.w + be.w) + p.w;
+        if (POS) {
+          const float4 p = *reinterpret_cast<const float4*>(pr + i);
+          o.x = ((v.x - mean) * rstd * g.x + be.x) + p.x;
+          o.y = ((v.y - mean) * rstd * g.y + be.y) + p.y;
+          o.z = ((v.z - mean) * rstd * g.z + be.z) + p.z;
+          o.w = ((v.w - mean) * rstd * g.w + be.w) + p.w;
+        } else {
+          o.x = (v.x - mean) * rstd * g.x + be.x;
+          o.y = (v.y - mean) * rstd * g.y + be.y;
+          o.z = (v.z - mean) * rstd * g.z + be.z;
+          o.w = (v.w - mean) * rstd * g.w + be.w;
+        }
         *reinterpret_cast<float4*>(xr + i) = o;
         uint2 pk;
         pk.x = pack_bf16x2(o.x, o.y);
@@ -338,7 +347,10 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
         s2 = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, fmaf(a3, a3, s2))));
       }
     } else {
-      for (int i = lane; i < D; i += 32) emit(i, ((yr[i] - mean) * rstd * gamma[i] + beta[i]) + pr[i]);
+      for (int i = lane; i < D; i += 32) {
+        const float v = (yr[i] - mean) * rstd * gamma[i] + beta[i];
+        emit(i, POS ? v + pr[i] : v);
+      }
     }
   }
   if (stats) {
@@ -480,12 +492,13 @@ extern "C" int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats
 extern "C" int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, const float* cls,
                                     const float* pos, const float* tail, float* x, void* xb_bf16, float* stats, int B,
                                     int n, int ncls, int ntail, int D, float eps, void* stream) {
-  B200_CHECK_ARG(y && gamma && beta && pos && x, "embed_tokens: null pointer");
+  B200_CHECK_ARG(y && gamma && beta && x, "embed_tokens: null pointer");
   B200_CHECK_ARG(ncls == 0 || cls, "embed_tokens: ncls=%d without cls", ncls);
   B200_CHECK_ARG(ntail == 0 || tail, "embed_tokens: ntail=%d without tail", ntail);
   B200_CHECK_ARG(B > 0 && n > 0 && D > 0 && ncls >= 0 && ntail >= 0, "embed_tokens: bad shape");
   const long long rows = (long long)B * (n + ncls + ntail);
-  embed_tokens_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  auto kern = pos ? embed_tokens_kernel<true> : embed_tokens_kernel<false>;
+  kern<<<(unsigned)((rows + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       y, gamma, beta, cls, pos, x, reinterpret_cast<__nv_bfloat16*>(xb_bf16), stats, B, n, ncls, D, eps, tail, ntail);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();

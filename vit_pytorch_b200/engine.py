@@ -362,9 +362,12 @@ class TransformerEngine:
         return self._vl
 
     def run_blocks(self, x: torch.Tensor, B: int = 0, N: int = 0, primed: bool = False,
-                   varlen: Optional[_lib.VarlenIndex] = None) -> None:
+                   varlen: Optional[_lib.VarlenIndex] = None,
+                   rope: Optional[Tuple[torch.Tensor, int]] = None) -> None:
         """All encoder layers, in place on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
         B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
+        `rope` = (table, rows): rotary positions on q and k after every QKV projection (and its head norm), token t
+        using table row t % rows (_lib.rope_qk; the rotary ViTND, vit_nd_rotary.py:143-147).
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
         the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
@@ -376,7 +379,8 @@ class TransformerEngine:
                 and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
             # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
             arr, (heads, dh, hidden, scale) = t["c_layers"]
-            _lib.encoder_blocks(arr, len(arr), x, self.c_ws, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl)
+            _lib.encoder_blocks(arr, len(arr), x, self.c_ws, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl,
+                                rope=rope)
             return
         xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
         if fold and not primed:
@@ -394,6 +398,8 @@ class TransformerEngine:
             else:
                 _lib.gemm_headnorm(xb, w, out_bf16=ws["qkv"], head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads,
                                    dh=L.dim_head, head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None, **ln)
+            if rope is not None:
+                _lib.rope_qk(ws["qkv"], rope[0], rope[1], L.heads, L.dim_head)
             if vl is None:
                 _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale)
             else:
@@ -419,13 +425,13 @@ class TransformerEngine:
         _lib.layernorm(x, t["norm.w"], t["norm.b"], out_bf16=out_bf16, out_f32=out_f32, row_index=row_index,
                        eps=self.norm.eps)
 
-    def forward_tokens(self, tokens: torch.Tensor) -> torch.Tensor:
+    def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
-        reference mae.py:74, simmim.py:70, distill.py:66)."""
+        reference mae.py:74, simmim.py:70, distill.py:66); `rope` as in run_blocks."""
         B, N, D = tokens.shape
         with on_device(tokens):
             x = tokens.reshape(B * N, D).float().contiguous()
-            self.run_blocks(x, B, N)
+            self.run_blocks(x, B, N, rope=rope)
             out = torch.empty(B * N, D, device=tokens.device, dtype=torch.bfloat16)
             if self.norm is not None:
                 self.final_norm(x, out_bf16=out)

@@ -104,6 +104,11 @@ class FusedTransformer(FusedEncoder, FusedWeightsMixin, nn.Module):
 
     dropout_p = 0.0
 
+    @staticmethod
+    def qkv_weight(attn: nn.Module) -> torch.Tensor:
+        """The layer's [3 * heads * dim_head, D] projection, rows q | k | v."""
+        return attn.to_qkv.weight
+
     def encoder_layers(self) -> Tuple[List[EncoderLayer], Optional[Norm]]:
         layers = []
         for attn, ff in self.layers:
@@ -113,7 +118,7 @@ class FusedTransformer(FusedEncoder, FusedWeightsMixin, nn.Module):
             fc1, fc2 = [m for m in ff.net if isinstance(m, nn.Linear)]
             q_norm = getattr(attn, "q_norm", None)        # simple_vit_with_qk_norm: per-head RMSNorm of q and k
             layers.append(EncoderLayer(
-                ln1=Norm.of(attn.norm), qkv_w=attn.to_qkv.weight,
+                ln1=Norm.of(attn.norm), qkv_w=self.qkv_weight(attn),
                 out_w=None if identity else out.weight, out_b=None if identity else out.bias,
                 ln2=Norm.of(ff.net[0]), fc1_w=fc1.weight, fc1_b=fc1.bias, fc2_w=fc2.weight, fc2_b=fc2.bias,
                 heads=attn.heads, dim_head=attn.dim_head, scale=float(attn.scale),
