@@ -97,6 +97,17 @@ int b200vit_patchify_ln(const void* img, const float* gamma, const float* beta, 
 int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, const float* cls, const float* pos,
                          const float* tail, float* x, void* xb_bf16, float* stats, int B, int n, int ncls, int ntail,
                          int D, float eps, void* stream);
+/*
+ * The same assembly over `groups` token groups (y holds groups*n patch rows) whose positional rows come from a block of
+ * a larger table: group g reads the block starting at row (g % pos_period) * pos_stride.  Within the block, patch t
+ * reads row ncls + t and cls row c row c when cls_pos != 0; with cls_pos == 0 patch t reads row t and the cls rows
+ * get no position.  ViViT's [F'max, n_max] table sliced to [:frames, :n] (vivit.py:227-231): groups = B*F',
+ * pos_period = F', pos_stride = n_max, cls_pos = 0.  b200vit_embed_tokens is this call with (1, 0, 1).
+ */
+int b200vit_embed_tokens_grouped(const float* y, const float* gamma, const float* beta, const float* cls,
+                                 const float* pos, const float* tail, float* x, void* xb_bf16, float* stats, int groups,
+                                 int n, int ncls, int ntail, int D, float eps, int pos_period, int pos_stride,
+                                 int cls_pos, void* stream);
 
 /*
  * N-d patchify without a LayerNorm (vit_nd.py:130-145 / vit_nd_rotary.py:216-231, 'b c (f p0) (g p1) ... ->
@@ -149,6 +160,19 @@ int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, f
 int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev,
                              int num_seqs, int total_tokens, int total_tiles, int H, int dh, float scale,
                              void* stream);
+
+/*
+ * Softmax attention over short strided sequences with an optional key mask (ViViT's temporal attention,
+ * vivit.py:144-150, and its masked temporal transformer, vivit.py:75-100,268):
+ *   qkv[B*L*G, 3*H*dh] bf16 packed as for b200vit_attention; out[B*L*G, H*dh] bf16.
+ *   Token j of sequence s = b*G + p is row b*L*G + j*G + p of both (G = 1: B contiguous sequences of L tokens).
+ *   key_mask: NULL, or a DEVICE uint8 [B][L] array (1 = keep) shared by the G sequences of batch element b.
+ * A query row whose keys are all masked gets 0 when zero_masked_rows != 0 (scaled_dot_product_attention with a boolean
+ * mask) and the mean of the L values of its sequence otherwise (masked_fill(-finfo.max) before the softmax).
+ * L <= 64, dh = 32, 64, 80 or 128; qkv and out 16-byte aligned.  Rows of out outside the addressed set are untouched.
+ */
+int b200vit_attention_axial(const void* qkv, void* out, const uint8_t* key_mask, int B, int L, int G, int H, int dh,
+                            float scale, int zero_masked_rows, void* stream);
 
 /*
  * NaViT patch extraction over a LIST of images of different resolutions + LayerNorm(patch_dim) without bias, one launch:

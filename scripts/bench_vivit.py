@@ -1,0 +1,144 @@
+"""Throughput of the fused ViViT (vit_pytorch_b200.vivit) on one GPU.
+
+    python scripts/bench_vivit.py [--steps 10] [--warmup 3] [--only NAME]
+
+Prints one JSON line per workload, ViViT-B dims (dim 768, heads 12, mlp 3072), 16 frames at 224 x 224, patch 16,
+frame_patch_size 2, batch 32:
+  factorized_encoder          spatial depth 12 over 32*8 sequences of 197 tokens, temporal depth 4 over 32 of 9
+  factorized_self_attention   depth 12, each layer spatial attention (32*8 x 197) then temporal attention over the
+                              32*197 strided sequences of 8 frames (b200vit_attention_axial)
+Each line: fused clips/s, the module's own eager bf16 graph on the same GPU, their largest logit difference, ms per
+step, launches and share of every library kernel (per-call CUDA events in a separate profiled step), with GB/s where
+the shapes give the bytes (attention_axial: 3*H*dh read and H*dh written, bf16, per token), the card's name and power
+limit read in the same run.  Writes
+nothing.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from vit_pytorch_b200 import _lib  # noqa: E402
+from vit_pytorch_b200.vivit import ViViT  # noqa: E402
+
+VIVIT_B = dict(image_size=224, image_patch_size=16, frames=16, frame_patch_size=2, num_classes=1000, dim=768,
+               heads=12, mlp_dim=3072)
+WORKLOADS = {
+    "factorized_encoder": dict(batch=32, kw=dict(variant="factorized_encoder", spatial_depth=12, temporal_depth=4,
+                                                 **VIVIT_B)),
+    "factorized_self_attention": dict(batch=32, kw=dict(variant="factorized_self_attention", spatial_depth=12,
+                                                        temporal_depth=12, **VIVIT_B)),
+}
+SHAPE = (3, 16, 224, 224)
+
+
+def card() -> dict:
+    out = {"name": torch.cuda.get_device_name(), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception as e:  # noqa: BLE001  (reported, not fatal)
+        out["power_limit_w"] = f"unavailable: {type(e).__name__}"
+    return out
+
+
+def timed(fn, steps: int, warmup: int) -> float:
+    """ms per call, CUDA events around `steps` calls after `warmup` calls."""
+    with torch.inference_mode():
+        for _ in range(warmup):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(steps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps
+
+
+def kernel_breakdown(fn) -> dict:
+    """One profiled step: per library kernel name, ms per step, launches, GB/s and TFLOP/s (from the shapes)."""
+    with torch.inference_mode():
+        _lib.profile_start()
+        fn()
+        rec = _lib.profile_stop()
+    agg: dict = {}
+    for name, meta, ms in rec:
+        a = agg.setdefault(name, {"ms_per_step": 0.0, "launches": 0, "bytes": 0.0, "flops": 0.0})
+        a["ms_per_step"] += ms
+        a["launches"] += 1
+        a["bytes"] += float(meta.get("bytes", 0.0))
+        a["flops"] += float(meta.get("flops", 0.0))
+    total = sum(a["ms_per_step"] for a in agg.values())
+    out = {}
+    for name, a in sorted(agg.items(), key=lambda kv: -kv[1]["ms_per_step"]):
+        e = {"ms_per_step": round(a["ms_per_step"], 4), "launches": a["launches"],
+             "share_of_profiled_step": round(a["ms_per_step"] / total, 4)}
+        if a["bytes"]:
+            e["GB_per_step"] = round(a["bytes"] / 1e9, 3)
+            e["GB_per_s"] = round(a["bytes"] / (a["ms_per_step"] / 1e3) / 1e9, 1)
+        if a["flops"]:
+            e["TFLOP_per_s"] = round(a["flops"] / (a["ms_per_step"] / 1e3) / 1e12, 1)
+        out[name] = e
+    return out
+
+
+def run(name: str, spec: dict, args, dev, info: dict) -> dict:
+    torch.manual_seed(0)
+    model = ViViT(**spec["kw"]).eval().to(dev, torch.bfloat16)
+    B = spec["batch"]
+    torch.manual_seed(1)
+    x = torch.randn(B, *SHAPE, device=dev).bfloat16()
+    with torch.inference_mode():
+        reason = model.fused_reason(x)
+    assert reason is None, reason
+    fused = lambda: model(x)                      # noqa: E731
+    ms = timed(fused, args.steps, args.warmup)
+    with torch.inference_mode():
+        out = model(x).float()
+    # the module's own PyTorch graph, every submodule included (the Transformers would otherwise dispatch fused)
+    os.environ["B200VIT_DISABLE_FUSED"] = "1"
+    try:
+        ms_eager = timed(fused, max(3, args.steps // 2), 2)
+        with torch.inference_mode():
+            diff = (model(x).float() - out).abs().max().item()
+    finally:
+        del os.environ["B200VIT_DISABLE_FUSED"]
+    line = {"workload": name, "model": "vit_pytorch_b200.vivit.ViViT", "batch": B, "input": list(SHAPE),
+            "fused_clips_per_s": round(B / ms * 1e3, 2), "fused_ms_per_step": round(ms, 3),
+            "eager_bf16_clips_per_s": round(B / ms_eager * 1e3, 2), "eager_bf16_ms_per_step": round(ms_eager, 3),
+            "speedup_vs_eager": round(ms_eager / ms, 3), "max_abs_logit_diff_fused_vs_eager": diff,
+            "kernels": kernel_breakdown(fused), "steps": args.steps, "gpu": info}
+    del model
+    torch.cuda.empty_cache()
+    return line
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--only", choices=sorted(WORKLOADS), default=None)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_vivit.py measures the GPU path and needs a CUDA device")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    if not _lib.device_ok(dev.index):
+        raise SystemExit("libb200vit.so cannot run on this device: " + _lib.lib().b200vit_last_error().decode())
+    info = card()
+    for name, spec in WORKLOADS.items():
+        if args.only in (None, name):
+            print(json.dumps(run(name, spec, args, dev, info)), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -32,6 +32,7 @@ SYMBOLS = [
     "b200vit_patchify_varlen_ln", "b200vit_rmsnorm_heads", "b200vit_embed_varlen",
     "b200vit_gemm_headnorm_bf16", "b200vit_layernorm_heads", "b200vit_patch_stats", "b200vit_patch_embed_tma",
     "b200vit_encoder_blocks", "b200vit_patchify_nd", "b200vit_rope_qk", "b200vit_encoder_blocks_rope",
+    "b200vit_attention_axial", "b200vit_embed_tokens_grouped",
 ]
 
 
@@ -125,6 +126,11 @@ def lib() -> C.CDLL:
     L.b200vit_patchify_nd.argtypes = [vp, vp, i64, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), vp]
     L.b200vit_rope_qk.restype = i32
     L.b200vit_rope_qk.argtypes = [vp, vp, i32, i32, i32, i32, vp]
+    L.b200vit_attention_axial.restype = i32
+    L.b200vit_attention_axial.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp]
+    L.b200vit_embed_tokens_grouped.restype = i32
+    L.b200vit_embed_tokens_grouped.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32,
+                                               i32, i32, vp]
     _lib = L
     return L
 
@@ -412,6 +418,28 @@ def embed_tokens(y: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, cls: 
     _check(rc, "b200vit_embed_tokens")
 
 
+def embed_tokens_grouped(y: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, cls: Optional[torch.Tensor],
+                         pos: Optional[torch.Tensor], x: torch.Tensor, groups: int, n: int, ncls: int, pos_period: int,
+                         pos_stride: int, cls_pos: bool, eps: float = 1e-5, xb: Optional[torch.Tensor] = None,
+                         stats: Optional[torch.Tensor] = None) -> None:
+    """embed_tokens over `groups` token groups whose positions come from blocks of a larger table: group g reads the
+    block at row (g % pos_period) * pos_stride; patch t reads row ncls + t of it (cls_pos) or row t, the cls rows then
+    getting no position (ViViT's per-frame table, reference vivit.py:227-231)."""
+    _chk(xb, torch.bfloat16, "xb"); _chk(stats, torch.float32, "stats")
+    for nm, t in (("y", y), ("gamma", gamma), ("beta", beta), ("cls", cls), ("pos", pos), ("x", x)):
+        _chk(t, torch.float32, nm)
+    D = y.shape[1]
+    assert y.is_contiguous() and x.is_contiguous() and y.shape[0] == groups * n and x.shape[0] == groups * (n + ncls)
+    if pos is not None:
+        last = (pos_period - 1) * pos_stride + n + (ncls if cls_pos else 0)
+        assert pos.is_contiguous() and pos.shape[0] >= last, f"positional table of {pos.shape[0]} rows, {last} needed"
+    with _Timed("embed_tokens", bytes=(y.numel() + x.numel()) * 4):
+        rc = lib().b200vit_embed_tokens_grouped(_ptr(y), _ptr(gamma), _ptr(beta), _ptr(cls), _ptr(pos), None, _ptr(x),
+                                                _ptr(xb), _ptr(stats), groups, n, ncls, 0, D, float(eps),
+                                                int(pos_period), int(pos_stride), 1 if cls_pos else 0, _stream())
+    _check(rc, "b200vit_embed_tokens_grouped")
+
+
 def rowstats_cast(x: torch.Tensor, xb: torch.Tensor, stats: torch.Tensor) -> None:
     _chk(x, torch.float32, "x"); _chk(xb, torch.bfloat16, "xb"); _chk(stats, torch.float32, "stats")
     assert x.is_contiguous() and xb.is_contiguous() and stats.is_contiguous()
@@ -428,6 +456,21 @@ def attention(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, H: int, dh: 
     with _Timed("attention", B=B, N=N, H=H, bytes=(qkv.numel() + out.numel()) * 2, flops=4.0 * B * H * N * N * dh):
         rc = lib().b200vit_attention(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), _stream())
     _check(rc, "b200vit_attention")
+
+
+def attention_axial(qkv: torch.Tensor, out: torch.Tensor, key_mask: Optional[torch.Tensor], B: int, L: int, G: int,
+                    H: int, dh: int, scale: float, zero_masked_rows: bool) -> None:
+    """Attention over the B*G sequences of L tokens of qkv[B*L*G, 3*H*dh], token j of sequence b*G + p at row
+    b*L*G + j*G + p; key_mask: None or uint8 [B, L] (1 = keep), shared by the G sequences of b."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out"); _chk(key_mask, torch.uint8, "key_mask")
+    assert qkv.is_contiguous() and out.is_contiguous()
+    assert qkv.shape == (B * L * G, 3 * H * dh) and out.shape == (B * L * G, H * dh)
+    assert key_mask is None or (key_mask.is_contiguous() and key_mask.numel() == B * L)
+    with _Timed("attention_axial", B=B, L=L, G=G, H=H, bytes=(qkv.numel() + out.numel()) * 2,
+                flops=4.0 * B * G * H * L * L * dh):
+        rc = lib().b200vit_attention_axial(_ptr(qkv), _ptr(out), _ptr(key_mask), B, L, G, H, dh, float(scale),
+                                           1 if zero_masked_rows else 0, _stream())
+    _check(rc, "b200vit_attention_axial")
 
 
 def varlen_index(lengths, device) -> tuple:

@@ -292,7 +292,8 @@ __global__ void __launch_bounds__(256)
 embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma, const float* __restrict__ beta,
                     const float* __restrict__ cls, const float* __restrict__ pos, float* __restrict__ x,
                     __nv_bfloat16* __restrict__ xb, float* __restrict__ stats, int B, int n, int ncls, int D,
-                    float eps, const float* __restrict__ tail, int ntail) {
+                    float eps, const float* __restrict__ tail, int ntail, int pos_period, int pos_stride,
+                    int cls_pos) {
   const int N = n + ncls + ntail;
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -300,7 +301,11 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
   const int b = (int)(row / N), t = (int)(row % N);
   float* xr = x + row * D;
   __nv_bfloat16* xbr = xb ? xb + row * D : nullptr;
-  const float* pr = POS ? pos + (long long)min(t, n + ncls - 1) * D : nullptr;  // (tail rows carry no positional embedding)
+  // positional row: group b reads the table block (b % pos_period) * pos_stride; the cls rows take the first rows of
+  // the block when cls_pos, else no position (vivit.py:227-231); tail rows carry no positional embedding
+  const int tc = min(t, n + ncls - 1);
+  const long long prow = (long long)(b % pos_period) * pos_stride + (cls_pos ? tc : max(tc - ncls, 0));
+  const float* pr = POS ? pos + prow * D : nullptr;
   float s1 = 0.f, s2 = 0.f;  // sum / sum of squares of the bf16-rounded row (LN-fold statistics for the first layer)
   auto emit = [&](int i, float v) {
     xr[i] = v;
@@ -311,7 +316,8 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
     s2 = fmaf(vr, vr, s2);
   };
   if (t < ncls) {
-    for (int i = lane; i < D; i += 32) emit(i, POS ? cls[(long long)t * D + i] + pr[i] : cls[(long long)t * D + i]);
+    for (int i = lane; i < D; i += 32)
+      emit(i, POS && cls_pos ? cls[(long long)t * D + i] + pr[i] : cls[(long long)t * D + i]);
   } else if (t >= ncls + n) {  // register tokens appended after the patches (simple_vit_with_register_tokens.py:124-126)
     for (int i = lane; i < D; i += 32) emit(i, tail[(long long)(t - ncls - n) * D + i]);
   } else {
@@ -489,20 +495,32 @@ extern "C" int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats
   return 0;
 }
 
-extern "C" int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, const float* cls,
-                                    const float* pos, const float* tail, float* x, void* xb_bf16, float* stats, int B,
-                                    int n, int ncls, int ntail, int D, float eps, void* stream) {
+extern "C" int b200vit_embed_tokens_grouped(const float* y, const float* gamma, const float* beta, const float* cls,
+                                            const float* pos, const float* tail, float* x, void* xb_bf16, float* stats,
+                                            int groups, int n, int ncls, int ntail, int D, float eps, int pos_period,
+                                            int pos_stride, int cls_pos, void* stream) {
   B200_CHECK_ARG(y && gamma && beta && x, "embed_tokens: null pointer");
   B200_CHECK_ARG(ncls == 0 || cls, "embed_tokens: ncls=%d without cls", ncls);
   B200_CHECK_ARG(ntail == 0 || tail, "embed_tokens: ntail=%d without tail", ntail);
-  B200_CHECK_ARG(B > 0 && n > 0 && D > 0 && ncls >= 0 && ntail >= 0, "embed_tokens: bad shape");
-  const long long rows = (long long)B * (n + ncls + ntail);
+  B200_CHECK_ARG(groups > 0 && n > 0 && D > 0 && ncls >= 0 && ntail >= 0, "embed_tokens: bad shape");
+  B200_CHECK_ARG(pos_period > 0 && pos_stride >= 0, "embed_tokens: bad positional period %d / stride %d", pos_period,
+                 pos_stride);
+  const long long rows = (long long)groups * (n + ncls + ntail);
   auto kern = pos ? embed_tokens_kernel<true> : embed_tokens_kernel<false>;
   kern<<<(unsigned)((rows + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      y, gamma, beta, cls, pos, x, reinterpret_cast<__nv_bfloat16*>(xb_bf16), stats, B, n, ncls, D, eps, tail, ntail);
+      y, gamma, beta, cls, pos, x, reinterpret_cast<__nv_bfloat16*>(xb_bf16), stats, groups, n, ncls, D, eps, tail,
+      ntail, pos_period, pos_stride, cls_pos != 0);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
+}
+
+extern "C" int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, const float* cls,
+                                    const float* pos, const float* tail, float* x, void* xb_bf16, float* stats, int B,
+                                    int n, int ncls, int ntail, int D, float eps, void* stream) {
+  // one table for every image, the cls rows positioned first
+  return b200vit_embed_tokens_grouped(y, gamma, beta, cls, pos, tail, x, xb_bf16, stats, B, n, ncls, ntail, D, eps, 1,
+                                      0, 1, stream);
 }
 
 extern "C" int b200vit_mean_pool(const float* x, float* out, int B, int N, int D, int n_pool, void* stream) {

@@ -135,6 +135,15 @@ class Norm(NamedTuple):
         return Norm(ln.weight, ln.bias, ln.eps)
 
 
+class AttnBlock(NamedTuple):
+    """A second pre-LN attention sub-block of a layer (same heads, dim_head and scale as the first):
+        x += out(attention(qkv(LN(x))))"""
+    ln: Norm
+    qkv_w: torch.Tensor                            # [3 * heads * dim_head, D], rows q | k | v
+    out_w: Optional[torch.Tensor]                  # None: to_out is the identity, as EncoderLayer.out_w
+    out_b: Optional[torch.Tensor]
+
+
 @dataclass
 class EncoderLayer:
     """One pre-LN encoder layer as a model family describes it to the engine (reference vit.py:78-81):
@@ -155,6 +164,9 @@ class EncoderLayer:
     qk_norm: Optional[str] = None                  # per-head norm of q and k after the projection: None, "rms" or "ln"
     qk_gamma: Tuple[torch.Tensor, ...] = ()        # (q gamma, k gamma), each heads * dim_head values
     qk_eps: float = 0.0                            # eps of the "ln" head norm
+    # attention along the time axis between the attention and the feed-forward block (ViViT's FactorizedTransformer,
+    # reference vivit.py:144-150); run_blocks needs `axial` to address its sequences
+    temporal: Optional[AttnBlock] = None
 
 
 class _Prepared:
@@ -292,6 +304,14 @@ class TransformerEngine:
             else:
                 t[f"{i}.out.w"] = _bf16_rows(L.out_w)
             t[f"{i}.out.b"] = _f32(L.out_b)
+            if L.temporal is not None:
+                T = L.temporal
+                t[f"{i}.tln.w"], t[f"{i}.tln.b"] = _f32(T.ln.gamma), _f32(T.ln.beta)
+                t[f"{i}.tqkv.w"] = _bf16_rows(T.qkv_w)
+                _fold(t, f"{i}.tqkv", T.qkv_w, None, T.ln)
+                t[f"{i}.tout.w"] = (torch.eye(T.qkv_w.shape[1], device=T.qkv_w.device, dtype=torch.bfloat16)
+                                    if T.out_w is None else _bf16_rows(T.out_w))
+                t[f"{i}.tout.b"] = _f32(T.out_b)
             t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(L.ln2.gamma), _f32(L.ln2.beta)
             _fold(t, f"{i}.fc1", L.fc1_w, L.fc1_b, L.ln2)
             t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(L.fc1_w), _f32(L.fc1_b)
@@ -305,10 +325,10 @@ class TransformerEngine:
 
     def _c_layers(self, t: Dict[str, torch.Tensor]):
         """(ctypes array of b200vit_layer, heads, dh, hidden, scale) for the one-call encoder (b200vit_encoder_blocks),
-        or None when it cannot run these layers: they are not uniform, or one has a per-head LayerNorm (the one-call
-        encoder has no EPI_HEADLN).  The pointers stay valid as long as `t` (which holds the tensors)."""
+        or None when it cannot run these layers: they are not uniform, one has a per-head LayerNorm (the one-call
+        encoder has no EPI_HEADLN) or a temporal sub-block.  The pointers stay valid as long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.scale)      # noqa: E731
-        if any(L.qk_norm == "ln" or sig(L) != sig(self.layers[0]) for L in self.layers):
+        if any(L.qk_norm == "ln" or L.temporal is not None or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -363,11 +383,17 @@ class TransformerEngine:
 
     def run_blocks(self, x: torch.Tensor, B: int = 0, N: int = 0, primed: bool = False,
                    varlen: Optional[_lib.VarlenIndex] = None,
-                   rope: Optional[Tuple[torch.Tensor, int]] = None) -> None:
+                   rope: Optional[Tuple[torch.Tensor, int]] = None,
+                   axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None) -> None:
         """All encoder layers, in place on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
         B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
         `rope` = (table, rows): rotary positions on q and k after every QKV projection (and its head norm), token t
         using table row t % rows (_lib.rope_qk; the rotary ViTND, vit_nd_rotary.py:143-147).
+        `axial` = (G, L, key_mask, zero_masked_rows): the sequences of _lib.attention_axial over the rows, token j of
+        sequence b*G + p at row b*L*G + j*G + p, key_mask None or uint8 [M / (L*G), L].  Layers with a temporal
+        sub-block run it there (the factorized layers of ViViT: spatial attention over the B sequences of N tokens,
+        G = N); layers without one run their attention there instead of over the B x N sequences (ViViT's masked
+        temporal transformer, G = 1).  These calls take the per-kernel loop below.
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
         the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
@@ -375,7 +401,7 @@ class TransformerEngine:
         ws = self.workspace(x.shape[0], x.device)
         vl = self._varlen_args(B, N, varlen, x.device)
         fold = ln_mode() == "fold"
-        if (fold and varlen is None and t["c_layers"] is not None and not _lib.profiling()
+        if (fold and varlen is None and axial is None and t["c_layers"] is not None and not _lib.profiling()
                 and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
             # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
             arr, (heads, dh, hidden, scale) = t["c_layers"]
@@ -385,7 +411,14 @@ class TransformerEngine:
         xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
         if fold and not primed:
             _lib.rowstats_cast(x, xb, ws["stats_in"])
+        def axial_attention(L: EncoderLayer) -> None:
+            G, Lt, key_mask, zero = axial
+            _lib.attention_axial(ws["qkv"], ws["o"], key_mask, x.shape[0] // (Lt * G), Lt, G, L.heads, L.dim_head,
+                                 L.scale, zero)
+
         for i, L in enumerate(self.layers):
+            if L.temporal is not None and axial is None:
+                raise ValueError("a layer with a temporal attention sub-block needs `axial` to address its sequences")
             # xb = LN1(x) -> qkv   (fold: xb already holds the bf16 copy of x; LN1 is applied in the GEMM epilogue)
             if fold:
                 w, ln = t[f"{i}.qkv.wg"], dict(bias=t[f"{i}.qkv.t"], ln_sums=ws["stats_in"] if i == 0 else sa,
@@ -400,7 +433,9 @@ class TransformerEngine:
                                    dh=L.dim_head, head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None, **ln)
             if rope is not None:
                 _lib.rope_qk(ws["qkv"], rope[0], rope[1], L.heads, L.dim_head)
-            if vl is None:
+            if axial is not None and L.temporal is None:
+                axial_attention(L)
+            elif vl is None:
                 _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale)
             else:
                 _lib.attention_varlen(ws["qkv"], ws["o"], *vl, L.heads, L.dim_head, L.scale)
@@ -408,12 +443,24 @@ class TransformerEngine:
                 # the residual GEMMs also write the bf16 copy of x and its row statistics for the next folded GEMM
                 _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.out.b"], resid=x,
                           stats_out=sb)
+                if L.temporal is not None:
+                    # temporal sub-block: LN folded into its QKV GEMM on the statistics the out-projection just wrote
+                    _lib.gemm(xb, t[f"{i}.tqkv.wg"], out_bf16=ws["qkv"], bias=t[f"{i}.tqkv.t"], ln_sums=sb,
+                              col_s=t[f"{i}.tqkv.s"], ln_eps=L.temporal.ln.eps)
+                    axial_attention(L)
+                    _lib.gemm(ws["o"], t[f"{i}.tout.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.tout.b"], resid=x,
+                              stats_out=sb)
                 _lib.gemm(xb, t[f"{i}.fc1.wg"], out_bf16=ws["h"], bias=t[f"{i}.fc1.t"], gelu=True, ln_sums=sb,
                           col_s=t[f"{i}.fc1.s"], ln_eps=L.ln2.eps)
                 _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.fc2.b"], resid=x,
                           stats_out=sa)
             else:
                 _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
+                if L.temporal is not None:
+                    _lib.layernorm(x, t[f"{i}.tln.w"], t[f"{i}.tln.b"], out_bf16=xb, eps=L.temporal.ln.eps)
+                    _lib.gemm(xb, t[f"{i}.tqkv.w"], out_bf16=ws["qkv"])
+                    axial_attention(L)
+                    _lib.gemm(ws["o"], t[f"{i}.tout.w"], out_f32=x, bias=t[f"{i}.tout.b"], resid=x)
                 _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=xb, eps=L.ln2.eps)
                 _lib.gemm(xb, t[f"{i}.fc1.w"], out_bf16=ws["h"], bias=t[f"{i}.fc1.b"], gelu=True)
                 _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, bias=t[f"{i}.fc2.b"], resid=x)
@@ -425,13 +472,14 @@ class TransformerEngine:
         _lib.layernorm(x, t["norm.w"], t["norm.b"], out_bf16=out_bf16, out_f32=out_f32, row_index=row_index,
                        eps=self.norm.eps)
 
-    def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None) -> torch.Tensor:
+    def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None,
+                       axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
-        reference mae.py:74, simmim.py:70, distill.py:66); `rope` as in run_blocks."""
+        reference mae.py:74, simmim.py:70, distill.py:66); `rope` and `axial` as in run_blocks."""
         B, N, D = tokens.shape
         with on_device(tokens):
             x = tokens.reshape(B * N, D).float().contiguous()
-            self.run_blocks(x, B, N, rope=rope)
+            self.run_blocks(x, B, N, rope=rope, axial=axial)
             out = torch.empty(B * N, D, device=tokens.device, dtype=torch.bfloat16)
             if self.norm is not None:
                 self.final_norm(x, out_bf16=out)
@@ -522,6 +570,23 @@ class PatchEmbedEngine:
             pos = self._pos_table(t, H // ph, W // pw, img.device)
         if pos.shape[0] < n + ncls:
             raise ValueError(f"sequence of {n + ncls} tokens exceeds the positional table ({pos.shape[0]})")
+        y = self.project(img, patch)
+        x = torch.empty(B * N, D, device=img.device, dtype=torch.float32)
+        _lib.embed_tokens(y, t["ln2.w"], t["ln2.b"], t["cls"], pos, x, B, n, ncls, xb=xb, stats=stats,
+                          eps=o.to_patch_embedding[3].eps, tail=t["tail"])
+        return x, B, N
+
+    def project(self, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None) -> torch.Tensor:
+        """The patch projection alone (vit.py:100-102): img [B, C, H, W] bf16 -> y fp32 [B*n, D] = LayerNorm(patch)
+        W^T + b, patches in row-major grid order, before the LayerNorm(dim) that token assembly applies."""
+        o = self.owner
+        ph, pw = patch if patch is not None else o.patch_size
+        B, C, H, W = img.shape
+        if H % ph or W % pw:
+            raise ValueError("Image dimensions must be divisible by the patch size.")
+        t = self.prepared(img.device)
+        n = (H // ph) * (W // pw)
+        D = t["w"].shape[0]
         dev = img.device
         y = torch.empty(B * n, D, device=dev, dtype=torch.float32)
         if ("tma.w" in t and (ph, pw) == (16, 16) and os.environ.get(_PATCH_MODE_ENV, "tma") == "tma"
@@ -534,10 +599,7 @@ class PatchEmbedEngine:
             a0 = torch.empty(B * n, t["kp"], device=dev, dtype=torch.bfloat16)
             _lib.patchify_ln(img.contiguous(), t["ln1.w"], t["ln1.b"], a0, ph, pw, eps=o.to_patch_embedding[1].eps)
             _lib.gemm(a0, t["w"], out_f32=y, bias=t["b"])
-        x = torch.empty(B * N, D, device=dev, dtype=torch.float32)
-        _lib.embed_tokens(y, t["ln2.w"], t["ln2.b"], t["cls"], pos, x, B, n, ncls, xb=xb, stats=stats,
-                          eps=o.to_patch_embedding[3].eps, tail=t["tail"])
-        return x, B, N
+        return y
 
     def geometry(self, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None) -> Tuple[int, int]:
         """(B, N) the image batch will produce, without running anything."""
