@@ -38,6 +38,9 @@ extern "C" {
 #define B200VIT_EPI_STATS 16    /* write per-row partial (sum, sum^2) of the bf16-rounded result into stats_out */
 #define B200VIT_EPI_HEADLN 64   /* b200vit_gemm_headnorm_bf16: per-head LayerNorm (no bias) instead of the RMS norm */
 
+/* attention flags (b200vit_attention_ex, b200vit_attention_varlen_ex, b200vit_encoder_blocks_ex) */
+#define B200VIT_ATTN_MASK_SELF 1  /* key i of query i gets probability 0 (LSA, vit_for_small_dataset.py:53-57) */
+
 const char* b200vit_last_error(void);
 int b200vit_version(void);
 /* number of kernels this library has launched in the calling process (all threads) since load / last reset */
@@ -84,6 +87,18 @@ int b200vit_patchify_ln(const void* img, const float* gamma, const float* beta, 
                         int C, int H, int W, int ph, int pw, float eps, void* stream);
 
 /*
+ * Shifted patch tokenization + LayerNorm(5*C*p*p) (SPT, vit_for_small_dataset.py:81-96): img[B, C, H, W] (bf16, NCHW
+ * contiguous) -> A[B*gh*gw, ldo] bf16 with, for k = 0..4,
+ *   A[b*(gh*gw) + h*gw + w, (p1*p + p2)*5C + k*C + c] = LN_over_patch(src_k[b, c, h*p + p1, w*p + p2]) * gamma + beta
+ *   src_0(y, x) = img(y, x), src_1 = img(y, x-1), src_2 = img(y, x+1), src_3 = img(y-1, x), src_4 = img(y+1, x),
+ * zero outside the image: the concat of the image and its four one-pixel shifts (F.pad by (1,-1,0,0), (-1,1,0,0),
+ * (0,0,1,-1), (0,0,-1,1)), cut into '(p1 p2 c)' patches over 5C channels, without materialising either.  Columns
+ * [5*C*p*p, ldo) are zero filled (K padding for the GEMM).  ldo multiple of 8, out_bf16 16-byte aligned.
+ */
+int b200vit_patchify_spt_ln(const void* img, const float* gamma, const float* beta, void* out_bf16, int64_t ldo, int B,
+                            int C, int H, int W, int p, float eps, void* stream);
+
+/*
  * Token assembly after the patch projection: y[B*n, D] (fp32, patch GEMM output incl. bias) ->
  *   x[b, t, :] = LN_D(y[b, t - ncls, :]) * gamma + beta + pos[t, :]   for t >= ncls
  *   x[b, 0, :] = cls[:] + pos[0, :]                                    if ncls == 1
@@ -93,6 +108,8 @@ int b200vit_patchify_ln(const void* img, const float* gamma, const float* beta, 
  * stats[M][2] = per-row (sum, sum of squares) of that copy -- the inputs of the first LN-folded GEMM.
  * Replaces nn.LayerNorm(dim) vit.py:103, cls concat vit.py:122-123, pos add vit.py:125-127 (simple_vit.py:94,114).
  * pos == NULL: no positional term at all (the rotary ViTND, vit_nd_rotary.py:272-287, positions act on q / k instead).
+ * gamma == NULL: no LayerNorm, the patch rows are y itself (beta is ignored; SPT has no LayerNorm(dim),
+ * vit_for_small_dataset.py:127-132).  Applies to b200vit_embed_tokens_grouped as well.
  */
 int b200vit_embed_tokens(const float* y, const float* gamma, const float* beta, const float* cls, const float* pos,
                          const float* tail, float* x, void* xb_bf16, float* stats, int B, int n, int ncls, int ntail,
@@ -149,6 +166,10 @@ int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats, int M, in
  * fall out of the same scheme as 64 + 2 x 16, but is not built).
  */
 int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* stream);
+/* ... with flags: B200VIT_ATTN_MASK_SELF excludes each query's own key (masked_fill(eye, -finfo.max),
+ * vit_for_small_dataset.py:53-57; a sequence of one token keeps it, as that fill does).  b200vit_attention is this call
+ * with flags = 0. */
+int b200vit_attention_ex(const void* qkv, void* out, int B, int N, int H, int dh, float scale, int flags, void* stream);
 
 /*
  * Variable-length attention over PACKED sequences (any length): tokens [cu_seqlens[s], cu_seqlens[s+1]) of
@@ -160,6 +181,10 @@ int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, f
 int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev,
                              int num_seqs, int total_tokens, int total_tiles, int H, int dh, float scale,
                              void* stream);
+/* ... with flags as b200vit_attention_ex (indices within each sequence); b200vit_attention_varlen is flags = 0. */
+int b200vit_attention_varlen_ex(const void* qkv, void* out, const int32_t* cu_seqlens_dev,
+                                const int32_t* tile_prefix_dev, int num_seqs, int total_tokens, int total_tiles, int H,
+                                int dh, float scale, int flags, void* stream);
 
 /*
  * Softmax attention over short strided sequences with an optional key mask (ViViT's temporal attention,
@@ -293,6 +318,14 @@ int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int depth, float* x
                                 int N, int D, int heads, int dh, int hidden, float scale, int primed,
                                 const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev, int total_tiles,
                                 const float* rope_cs, int rope_rows, void* stream);
+/* ... with a softmax scale per layer and attention flags: layer_scales is a HOST array of depth floats (NULL: `scale`
+ * for every layer; LSA's learned temperature.exp(), vit_for_small_dataset.py:35,53), attn_flags goes to every
+ * attention call (B200VIT_ATTN_MASK_SELF).  b200vit_encoder_blocks_rope is this call with (NULL, 0). */
+int b200vit_encoder_blocks_ex(const b200vit_layer* layers, int depth, float* x, const b200vit_encoder_ws* ws, int B,
+                              int N, int D, int heads, int dh, int hidden, float scale, int primed,
+                              const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev, int total_tiles,
+                              const float* rope_cs, int rope_rows, const float* layer_scales, int attn_flags,
+                              void* stream);
 
 /*
  * TEST HOOKS -- process-global switches for A/B tests and bring-up; NOT part of the re-entrant API above (a value set
@@ -304,6 +337,7 @@ int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int depth, float* x
  *   key 13: b200vit_attention: 0 = all softmax exponentials on MUFU (default), 1 = half of them on the FMA pipe
  * Keys 1, 11 and 13 select real attention instances for every head width (32, 64, 80, 128): all (key block, FMA
  * exponential) combinations are built without register spills, so no setting falls back to a width's default.
+ * They do not apply to calls with B200VIT_ATTN_MASK_SELF: those always run 64-key blocks with every exponential on MUFU.
  */
 int b200vit_debug_set(int key, int value);
 

@@ -22,6 +22,7 @@ EPI_RESIDUAL = 4
 EPI_LNFOLD = 8
 EPI_STATS = 16
 EPI_HEADLN = 64
+ATTN_MASK_SELF = 1
 
 # every symbol include/b200vit.h declares (tests check that the library exports each of them)
 SYMBOLS = [
@@ -32,7 +33,8 @@ SYMBOLS = [
     "b200vit_patchify_varlen_ln", "b200vit_rmsnorm_heads", "b200vit_embed_varlen",
     "b200vit_gemm_headnorm_bf16", "b200vit_layernorm_heads", "b200vit_patch_stats", "b200vit_patch_embed_tma",
     "b200vit_encoder_blocks", "b200vit_patchify_nd", "b200vit_rope_qk", "b200vit_encoder_blocks_rope",
-    "b200vit_attention_axial", "b200vit_embed_tokens_grouped",
+    "b200vit_attention_axial", "b200vit_embed_tokens_grouped", "b200vit_patchify_spt_ln", "b200vit_attention_ex",
+    "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex",
 ]
 
 
@@ -131,6 +133,15 @@ def lib() -> C.CDLL:
     L.b200vit_embed_tokens_grouped.restype = i32
     L.b200vit_embed_tokens_grouped.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32,
                                                i32, i32, vp]
+    L.b200vit_patchify_spt_ln.restype = i32
+    L.b200vit_patchify_spt_ln.argtypes = [vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_attention_ex.restype = i32
+    L.b200vit_attention_ex.argtypes = [vp, vp, i32, i32, i32, i32, f32, i32, vp]
+    L.b200vit_attention_varlen_ex.restype = i32
+    L.b200vit_attention_varlen_ex.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp]
+    L.b200vit_encoder_blocks_ex.restype = i32
+    L.b200vit_encoder_blocks_ex.argtypes = [C.POINTER(Layer), i32, vp, C.POINTER(EncoderWs), i32, i32, i32, i32, i32,
+                                            i32, f32, i32, vp, vp, i32, vp, i32, C.POINTER(C.c_float), i32, vp]
     _lib = L
     return L
 
@@ -196,12 +207,24 @@ def profiling() -> bool:
 
 
 def encoder_blocks(layers, depth: int, x: torch.Tensor, ws: "EncoderWs", B: int, N: int, D: int, heads: int, dh: int,
-                   hidden: int, scale: float, primed: bool, varlen=None, rope=None) -> None:
+                   hidden: int, scale: float, primed: bool, varlen=None, rope=None, layer_scales=None,
+                   attn_flags: int = 0) -> None:
     """All encoder layers in one library call (b200vit_encoder_blocks).  `layers`: ctypes array of Layer built from the
     prepared weights; `ws`: EncoderWs over the engine's workspace; `varlen`: (cu, tile_prefix, total_tiles) if N > 512;
-    `rope`: (cs table, rows) of rope_qk, applied after every QKV GEMM (b200vit_encoder_blocks_rope)."""
+    `rope`: (cs table, rows) of rope_qk, applied after every QKV GEMM (b200vit_encoder_blocks_rope);
+    `layer_scales`: ctypes float array of `depth` softmax scales (None: `scale` for every layer) and `attn_flags`
+    (ATTN_MASK_SELF) go to b200vit_encoder_blocks_ex."""
     _chk(x, torch.float32, "x")
     cu, tp, tiles = varlen if varlen is not None else (None, None, 0)
+    if layer_scales is not None or attn_flags:
+        cs, rows = rope if rope is not None else (None, 0)
+        _chk(cs, torch.float32, "rope table")
+        assert layer_scales is None or len(layer_scales) == depth
+        rc = lib().b200vit_encoder_blocks_ex(layers, depth, _ptr(x), C.byref(ws), B, N, D, heads, dh, hidden,
+                                             float(scale), 1 if primed else 0, _ptr(cu), _ptr(tp), int(tiles),
+                                             _ptr(cs), int(rows), layer_scales, int(attn_flags), _stream())
+        _check(rc, "b200vit_encoder_blocks_ex")
+        return
     if rope is None:
         rc = lib().b200vit_encoder_blocks(layers, depth, _ptr(x), C.byref(ws), B, N, D, heads, dh, hidden,
                                           float(scale), 1 if primed else 0, _ptr(cu), _ptr(tp), int(tiles), _stream())
@@ -352,6 +375,20 @@ def patchify_ln(img: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out_
     _check(rc, "b200vit_patchify_ln")
 
 
+def patchify_spt_ln(img: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out_bf16: torch.Tensor, p: int,
+                    eps: float = 1e-5) -> None:
+    """Shifted patch tokenization + LayerNorm(5*C*p*p): img [B, C, H, W] bf16 -> out [B*n, ldo] bf16 rows of the
+    '(p1 p2 c)' patches of cat(img, its four one-pixel shifts) over 5C channels, zero K padding."""
+    _chk(img, torch.bfloat16, "img"); _chk(out_bf16, torch.bfloat16, "out")
+    _chk(gamma, torch.float32, "gamma"); _chk(beta, torch.float32, "beta")
+    assert img.is_contiguous() and img.dim() == 4 and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    B, Cc, H, W = img.shape
+    with _Timed("patchify_spt_ln", bytes=img.numel() * 2 + out_bf16.numel() * 2):
+        rc = lib().b200vit_patchify_spt_ln(_ptr(img), _ptr(gamma), _ptr(beta), _ptr(out_bf16), out_bf16.stride(0), B,
+                                           Cc, H, W, int(p), float(eps), _stream())
+    _check(rc, "b200vit_patchify_spt_ln")
+
+
 def patchify_nd(img: torch.Tensor, out_bf16: torch.Tensor, patch) -> None:
     """img [B, C, S_0 .. S_{r-1}] bf16 -> out [B*n, ldo] with the (p0 .. p_{r-1} c) patch rows, zero K padding."""
     _chk(img, torch.bfloat16, "img"); _chk(out_bf16, torch.bfloat16, "out")
@@ -403,7 +440,7 @@ def embed_tokens(y: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, cls: 
                  xb: Optional[torch.Tensor] = None, stats: Optional[torch.Tensor] = None,
                  tail: Optional[torch.Tensor] = None) -> None:
     """tail [ntail, D]: rows appended after the n patch tokens of every image (register tokens, no pos).
-    pos None: no positional term."""
+    pos None: no positional term.  gamma None: no LayerNorm (beta ignored)."""
     _chk(xb, torch.bfloat16, "xb"); _chk(stats, torch.float32, "stats")
     for nm, t in (("y", y), ("gamma", gamma), ("beta", beta), ("cls", cls), ("pos", pos), ("x", x), ("tail", tail)):
         _chk(t, torch.float32, nm)
@@ -449,12 +486,18 @@ def rowstats_cast(x: torch.Tensor, xb: torch.Tensor, stats: torch.Tensor) -> Non
     _check(rc, "b200vit_rowstats_cast")
 
 
-def attention(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, H: int, dh: int, scale: float) -> None:
+def attention(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, H: int, dh: int, scale: float,
+              mask_self: bool = False) -> None:
+    """mask_self: each query's own key is excluded (b200vit_attention_ex with ATTN_MASK_SELF)."""
     _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out")
     assert qkv.is_contiguous() and out.is_contiguous()
     assert qkv.shape == (B * N, 3 * H * dh) and out.shape == (B * N, H * dh)
     with _Timed("attention", B=B, N=N, H=H, bytes=(qkv.numel() + out.numel()) * 2, flops=4.0 * B * H * N * N * dh):
-        rc = lib().b200vit_attention(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), _stream())
+        if mask_self:
+            rc = lib().b200vit_attention_ex(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), ATTN_MASK_SELF,
+                                            _stream())
+        else:
+            rc = lib().b200vit_attention(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), _stream())
     _check(rc, "b200vit_attention")
 
 
@@ -484,7 +527,7 @@ def varlen_index(lengths, device) -> tuple:
 
 
 def attention_varlen(qkv: torch.Tensor, out: torch.Tensor, cu_seqlens: torch.Tensor, tile_prefix: torch.Tensor,
-                     total_tiles: int, H: int, dh: int, scale: float) -> None:
+                     total_tiles: int, H: int, dh: int, scale: float, mask_self: bool = False) -> None:
     _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out")
     assert qkv.is_contiguous() and out.is_contiguous()
     assert cu_seqlens.dtype == torch.int32 and tile_prefix.dtype == torch.int32 and cu_seqlens.is_cuda
@@ -492,8 +535,12 @@ def attention_varlen(qkv: torch.Tensor, out: torch.Tensor, cu_seqlens: torch.Ten
     S = cu_seqlens.numel() - 1
     assert qkv.shape[1] == 3 * H * dh and out.shape == (T, H * dh) and tile_prefix.numel() == S + 1
     with _Timed("attention_varlen", bytes=(qkv.numel() + out.numel()) * 2):
-        rc = lib().b200vit_attention_varlen(_ptr(qkv), _ptr(out), _ptr(cu_seqlens), _ptr(tile_prefix), S, T,
-                                            int(total_tiles), H, dh, float(scale), _stream())
+        if mask_self:
+            rc = lib().b200vit_attention_varlen_ex(_ptr(qkv), _ptr(out), _ptr(cu_seqlens), _ptr(tile_prefix), S, T,
+                                                   int(total_tiles), H, dh, float(scale), ATTN_MASK_SELF, _stream())
+        else:
+            rc = lib().b200vit_attention_varlen(_ptr(qkv), _ptr(out), _ptr(cu_seqlens), _ptr(tile_prefix), S, T,
+                                                int(total_tiles), H, dh, float(scale), _stream())
     _check(rc, "b200vit_attention_varlen")
 
 

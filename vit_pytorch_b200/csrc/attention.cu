@@ -9,6 +9,9 @@
 // and accumulates O += P V with wgmma, P (bf16) taken from registers as the A operand and V read as the transposed
 // (MN-major) B operand.  dh = 32, 64, 80 or 128: a head is split into 64-wide (128B swizzle) and 16-wide (32B swizzle)
 // slabs (AttnSmem).  Keys of a block beyond the sequence get probability 0; TMA zero-fills rows beyond the buffer.
+// MASK_SELF instances (b200vit_attention_ex / _varlen_ex with B200VIT_ATTN_MASK_SELF) also give key i of query i
+// probability 0 -- LSA, vit_for_small_dataset.py:53-57 -- except in a sequence of one token, where the reference's
+// -finfo.max fill leaves that token's own key with weight 1.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -50,7 +53,7 @@ struct AttnSmem {
 // CTAs per SM the register budget is planned for (ptxas -v: no spills at these bounds)
 constexpr int att_min_blocks(int dh, int kb) { return (dh == 64 && kb == 64) || dh == 32 ? 2 : 1; }
 
-template <int DH, int KB, bool VARLEN, bool EMUL>
+template <int DH, int KB, bool VARLEN, bool EMUL, bool MASK_SELF>
 __global__ void __launch_bounds__(ATT_THREADS, att_min_blocks(DH, KB))
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                  const __grid_constant__ CUtensorMap tmQ16, const __grid_constant__ CUtensorMap tmKV16,
@@ -139,6 +142,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const uint32_t qa = smem_u32(smem) + wg * 64 * 128;
   const uint32_t qa16 = smem_u32(smem + N64 * L::Q64) + wg * 64 * 32;
+  // a length-1 sequence keeps its only key (see above), so for len >= 2 every row has a valid key in block 0 (keys 0 and
+  // 1) and m is finite from there on: no -inf - -inf
+  const bool mask_self = MASK_SELF && len > 1;
   mbar_wait(qbar, 0);
 
   for (int kb = 0; kb < nblocks; ++kb) {
@@ -177,7 +183,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     for (int j = 0; j < KB / 8; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const bool valid = key0 + j * 8 + (e & 1) < len;
+        const int key = key0 + j * 8 + (e & 1);
+        bool valid = key < len;
+        if constexpr (MASK_SELF)  // query index within the sequence of accumulator row e >> 1
+          valid = valid && !(mask_self && key == q0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * (e >> 1));
         s[4 * j + e] = valid ? s[4 * j + e] * p.scale_log2e : -INFINITY;
         mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * j + e]);
       }
@@ -282,7 +291,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 // Tensor maps over qkv[T, 3 I]: 64-column boxes (128B swizzle) of 128 query rows / KB key rows for the 64-wide slabs,
 // and the same with 16 columns (32B swizzle) for the 16-wide ones.  A kind the head does not use gets a copy of the
 // other (never read).
-template <int DH, int KB, bool VARLEN, bool EMUL>
+template <int DH, int KB, bool VARLEN, bool EMUL, bool MASK_SELF>
 static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 grid, cudaStream_t stream) {
   using L = AttnSmem<DH, KB>;
   CUtensorMap tm[4];
@@ -297,7 +306,7 @@ static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 
   if (rc) return rc;
   if (!L::N16) tm[2] = tm[0], tm[3] = tm[1];
   if (!L::N64) tm[0] = tm[2], tm[1] = tm[3];
-  auto kern = attention_kernel<DH, KB, VARLEN, EMUL>;
+  auto kern = attention_kernel<DH, KB, VARLEN, EMUL, MASK_SELF>;
   B200_ENSURE_SMEM(kern, L::BYTES);
   kern<<<grid, ATT_THREADS, L::BYTES, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -305,24 +314,27 @@ static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 
   return 0;
 }
 
+// the self-masked instances exist for the default key block and exponential mode only (test hooks 1, 11, 13 do not
+// apply to them)
 template <int DH, bool VARLEN>
-static int launch_attention_dh(const void* qkv, int T, const AttnParams& p, int kb, bool emul, dim3 grid,
-                               cudaStream_t st) {
-  if (kb == 128) return emul ? launch_attention_t<DH, 128, VARLEN, true>(qkv, T, p, grid, st)
-                             : launch_attention_t<DH, 128, VARLEN, false>(qkv, T, p, grid, st);
-  return emul ? launch_attention_t<DH, 64, VARLEN, true>(qkv, T, p, grid, st)
-              : launch_attention_t<DH, 64, VARLEN, false>(qkv, T, p, grid, st);
+static int launch_attention_dh(const void* qkv, int T, const AttnParams& p, int kb, bool emul, bool mask_self,
+                               dim3 grid, cudaStream_t st) {
+  if (mask_self) return launch_attention_t<DH, 64, VARLEN, false, true>(qkv, T, p, grid, st);
+  if (kb == 128) return emul ? launch_attention_t<DH, 128, VARLEN, true, false>(qkv, T, p, grid, st)
+                             : launch_attention_t<DH, 128, VARLEN, false, false>(qkv, T, p, grid, st);
+  return emul ? launch_attention_t<DH, 64, VARLEN, true, false>(qkv, T, p, grid, st)
+              : launch_attention_t<DH, 64, VARLEN, false, false>(qkv, T, p, grid, st);
 }
 
 // one instance per width of head_width_ok() (dh 96 = 64 + 2 x 16 would fall out of the same slab scheme)
 template <bool VARLEN>
-static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, int kb, bool emul, dim3 grid,
-                            cudaStream_t st) {
+static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, int kb, bool emul, bool mask_self,
+                            dim3 grid, cudaStream_t st) {
   switch (dh) {
-    case 32: return launch_attention_dh<32, VARLEN>(qkv, T, p, kb, emul, grid, st);
-    case 80: return launch_attention_dh<80, VARLEN>(qkv, T, p, kb, emul, grid, st);
-    case 128: return launch_attention_dh<128, VARLEN>(qkv, T, p, kb, emul, grid, st);
-    default: return launch_attention_dh<64, VARLEN>(qkv, T, p, kb, emul, grid, st);
+    case 32: return launch_attention_dh<32, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
+    case 80: return launch_attention_dh<80, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
+    case 128: return launch_attention_dh<128, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
+    default: return launch_attention_dh<64, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
   }
 }
 
@@ -346,6 +358,11 @@ extern "C" int b200vit_debug_set(int key, int value) {
 }
 
 extern "C" int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* stream) {
+  return b200vit_attention_ex(qkv, out, B, N, H, dh, scale, 0, stream);
+}
+
+extern "C" int b200vit_attention_ex(const void* qkv, void* out, int B, int N, int H, int dh, float scale, int flags,
+                                    void* stream) {
   B200_CHECK_ARG(qkv && out, "attention: null pointer");
   B200_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention: bad shape B=%d N=%d H=%d", B, N, H);
   B200_CHECK_ARG(head_width_ok(dh), "attention: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
@@ -353,6 +370,7 @@ extern "C" int b200vit_attention(const void* qkv, void* out, int B, int N, int H
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention: pointers must be 16-byte aligned");
   B200_CHECK_ARG(B <= 65535, "attention: B=%d exceeds the grid", B);
+  B200_CHECK_ARG((flags & ~B200VIT_ATTN_MASK_SELF) == 0, "attention: unknown flags 0x%x", flags);
   AttnParams p{};
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.N = N;
@@ -361,12 +379,19 @@ extern "C" int b200vit_attention(const void* qkv, void* out, int B, int N, int H
   p.scale_log2e = scale * 1.4426950408889634f;
   const dim3 grid((N + ATT_QROWS - 1) / ATT_QROWS, H, B);
   return launch_attention<false>(qkv, B * N, p, dh, g_attn_mode.load() == 2 ? 128 : 64, g_attn_emul.load() != 0,
-                                 grid, reinterpret_cast<cudaStream_t>(stream));
+                                 (flags & B200VIT_ATTN_MASK_SELF) != 0, grid, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev,
                                         const int32_t* tile_prefix_dev, int num_seqs, int total_tokens, int total_tiles,
                                         int H, int dh, float scale, void* stream) {
+  return b200vit_attention_varlen_ex(qkv, out, cu_seqlens_dev, tile_prefix_dev, num_seqs, total_tokens, total_tiles, H,
+                                     dh, scale, 0, stream);
+}
+
+extern "C" int b200vit_attention_varlen_ex(const void* qkv, void* out, const int32_t* cu_seqlens_dev,
+                                           const int32_t* tile_prefix_dev, int num_seqs, int total_tokens,
+                                           int total_tiles, int H, int dh, float scale, int flags, void* stream) {
   B200_CHECK_ARG(qkv && out && cu_seqlens_dev && tile_prefix_dev, "attention_varlen: null pointer");
   B200_CHECK_ARG(num_seqs > 0 && total_tokens > 0 && total_tiles > 0 && H > 0, "attention_varlen: bad shape");
   B200_CHECK_ARG(head_width_ok(dh), "attention_varlen: dim_head=%d not supported by this build (32, 64, 80 or 128)",
@@ -374,6 +399,7 @@ extern "C" int b200vit_attention_varlen(const void* qkv, void* out, const int32_
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention_varlen: pointers must be 16-byte aligned");
   B200_CHECK_ARG(H <= 65535, "attention_varlen: H=%d exceeds the grid", H);
+  B200_CHECK_ARG((flags & ~B200VIT_ATTN_MASK_SELF) == 0, "attention_varlen: unknown flags 0x%x", flags);
   AttnParams p{};
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.cu_seqlens = cu_seqlens_dev;
@@ -384,6 +410,6 @@ extern "C" int b200vit_attention_varlen(const void* qkv, void* out, const int32_
   p.scale_log2e = scale * 1.4426950408889634f;
   const int mode = g_varlen_mode.load();
   const dim3 grid(total_tiles, H, 1);
-  return launch_attention<true>(qkv, total_tokens, p, dh, mode == 1 ? 128 : 64, mode == 2, grid,
-                                reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention<true>(qkv, total_tokens, p, dh, mode == 1 ? 128 : 64, mode == 2,
+                                (flags & B200VIT_ATTN_MASK_SELF) != 0, grid, reinterpret_cast<cudaStream_t>(stream));
 }

@@ -5,6 +5,9 @@
 // Nothing here touches the device itself: it is the host-side loop, moved below the language boundary so that a Python
 // (ctypes) or C++ host pays one call instead of 5 x depth -- at small batches the forward is host bound.
 // With a rope table (b200vit_encoder_blocks_rope) a sixth launch rotates q and k right after the QKV GEMM.
+// b200vit_encoder_blocks_ex adds a softmax scale per layer and attention flags (LSA: learned temperature, self mask).
+#include <cmath>
+
 #include "../../include/b200vit.h"
 #include "host_util.h"
 
@@ -27,6 +30,15 @@ extern "C" int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int dept
                                            int hidden, float scale, int primed, const int32_t* cu_seqlens_dev,
                                            const int32_t* tile_prefix_dev, int total_tiles, const float* rope_cs,
                                            int rope_rows, void* stream) {
+  return b200vit_encoder_blocks_ex(layers, depth, x, ws, B, N, D, heads, dh, hidden, scale, primed, cu_seqlens_dev,
+                                   tile_prefix_dev, total_tiles, rope_cs, rope_rows, nullptr, 0, stream);
+}
+
+extern "C" int b200vit_encoder_blocks_ex(const b200vit_layer* layers, int depth, float* x,
+                                         const b200vit_encoder_ws* ws, int B, int N, int D, int heads, int dh,
+                                         int hidden, float scale, int primed, const int32_t* cu_seqlens_dev,
+                                         const int32_t* tile_prefix_dev, int total_tiles, const float* rope_cs,
+                                         int rope_rows, const float* layer_scales, int attn_flags, void* stream) {
   B200_CHECK_ARG(layers && x && ws && depth > 0, "encoder_blocks: null pointer / depth %d", depth);
   B200_CHECK_ARG(B > 0 && N > 0 && D > 0 && heads > 0 && hidden > 0, "encoder_blocks: bad shape");
   B200_CHECK_ARG(ws->xb && ws->qkv && ws->o && ws->h && ws->stats_in && ws->stats_a && ws->stats_b,
@@ -34,6 +46,11 @@ extern "C" int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int dept
   B200_CHECK_ARG(N <= 512 || (cu_seqlens_dev && tile_prefix_dev && total_tiles > 0),
                  "encoder_blocks: N = %d > 512 needs the varlen index (cu_seqlens, tile_prefix)", N);
   B200_CHECK_ARG(!rope_cs || rope_rows > 0, "encoder_blocks: rope table with %d rows", rope_rows);
+  B200_CHECK_ARG((attn_flags & ~B200VIT_ATTN_MASK_SELF) == 0, "encoder_blocks: unknown attention flags 0x%x",
+                 attn_flags);
+  if (layer_scales)
+    for (int i = 0; i < depth; ++i)
+      B200_CHECK_ARG(std::isfinite(layer_scales[i]), "encoder_blocks: layer %d has a non-finite scale", i);
   const int M = B * N, I = heads * dh;
   const int parts = b200vit_stats_parts(D);
   int rc = 0;
@@ -61,12 +78,13 @@ extern "C" int b200vit_encoder_blocks_rope(const b200vit_layer* layers, int dept
       rc = b200vit_rope_qk(ws->qkv, rope_cs, rope_rows, M, heads, dh, stream);
       if (rc) return rc;
     }
-    // softmax(q k^T * scale) v, heads merged   (vit.py:55-63)
+    // softmax(q k^T * scale) v, heads merged   (vit.py:55-63; vit_for_small_dataset.py:53-60 with the flags)
+    const float sc = layer_scales ? layer_scales[i] : scale;
     if (N <= 512)
-      rc = b200vit_attention(ws->qkv, ws->o, B, N, heads, dh, scale, stream);
+      rc = b200vit_attention_ex(ws->qkv, ws->o, B, N, heads, dh, sc, attn_flags, stream);
     else
-      rc = b200vit_attention_varlen(ws->qkv, ws->o, cu_seqlens_dev, tile_prefix_dev, B, M, total_tiles, heads, dh,
-                                    scale, stream);
+      rc = b200vit_attention_varlen_ex(ws->qkv, ws->o, cu_seqlens_dev, tile_prefix_dev, B, M, total_tiles, heads, dh,
+                                       sc, attn_flags, stream);
     if (rc) return rc;
     // to_out + residual   (vit.py:64,80)
     rc = b200vit_gemm_bf16(ws->o, I, L.out_w, I, ws->xb, x, D, L.out_b, x, nullptr, 0, 0.f, nullptr, ws->stats_b, M, D,

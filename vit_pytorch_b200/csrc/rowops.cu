@@ -284,10 +284,93 @@ patchify_ln16c3_kernel(const __nv_bfloat16* __restrict__ img, const float* __res
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Shifted patch tokenization + LayerNorm(5 C p^2) (SPT, vit_for_small_dataset.py:81-96).  One CTA per (image, patch
+// row), persistent: the p + 2 image rows the patch row and its vertical shifts read are staged per channel in shared
+// memory, SPT_LPAD columns right of a zero column for x = -1 and with one zero column at x = W, the rows above / below
+// the image zero -- so each of the five sources is a fixed offset into the slab and needs no bounds test.  A table of
+// those offsets per output column (patch-relative, built once per CTA) replaces the (p1 p2 k c) index arithmetic; each
+// warp normalises whole patches (two passes over the slab for mean and variance, one to write) in 16-byte pieces.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int SPT_LPAD = 8;  // slab column of x = 0 (keeps the staged rows 16-byte aligned); x = -1 is column 7
+
+__global__ void __launch_bounds__(256)
+patchify_spt_ln_kernel(const __nv_bfloat16* __restrict__ img, const float* __restrict__ gamma,
+                       const float* __restrict__ beta, __nv_bfloat16* __restrict__ out, long long ldo, int nrows, int C,
+                       int H, int W, int p, int rs, float eps) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  const int pd = 5 * C * p * p, C5 = 5 * C, ps = p + 2;
+  int* offs = reinterpret_cast<int*>(smem_raw);                                  // [pd rounded up to 8]
+  __nv_bfloat16* slab = reinterpret_cast<__nv_bfloat16*>(offs + ((pd + 7) & ~7));  // [C][p + 2][rs]
+  const int gh = H / p, gw = W / p;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int e = threadIdx.x; e < pd; e += blockDim.x) {
+    const int pix = e / C5, kc = e - pix * C5, k = kc / C, c = kc - k * C;
+    const int p1 = pix / p, p2 = pix - p1 * p;
+    const int dx = k == 1 ? -1 : k == 2 ? 1 : 0, dy = k == 3 ? -1 : k == 4 ? 1 : 0;
+    offs[e] = (c * ps + 1 + p1 + dy) * rs + SPT_LPAD + p2 + dx;
+  }
+  const int slab_rows = C * ps;
+  for (int r = threadIdx.x; r < slab_rows; r += blockDim.x) {  // the x = -1 and x = W columns stay zero
+    slab[r * rs + SPT_LPAD - 1] = __float2bfloat16_rn(0.f);
+    slab[r * rs + SPT_LPAD + W] = __float2bfloat16_rn(0.f);
+  }
+  const bool vec = (W & 7) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0;
+  const int vpr = vec ? W >> 3 : W;  // work items per slab row
+  const int nchunks = (int)(ldo >> 3);
+  for (int bh = blockIdx.x; bh < nrows; bh += gridDim.x) {
+    const int b = bh / gh, h = bh % gh;
+    __syncthreads();  // previous slab fully consumed (and the table / pad columns written)
+    for (int i = threadIdx.x; i < slab_rows * vpr; i += blockDim.x) {
+      const int r = i / vpr, v = i - r * vpr;
+      const int c = r / ps, y = h * p - 1 + (r - c * ps);
+      const bool in = y >= 0 && y < H;
+      const __nv_bfloat16* src = img + ((long long)(b * C + c) * H + y) * W;
+      __nv_bfloat16* dst = slab + r * rs + SPT_LPAD;
+      if (vec) {
+        const uint4 u = in ? __ldg(reinterpret_cast<const uint4*>(src) + v) : make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(dst + 8 * v) = u;
+      } else {
+        dst[v] = in ? src[v] : __float2bfloat16_rn(0.f);
+      }
+    }
+    __syncthreads();
+    for (int w = warp; w < gw; w += 8) {
+      const __nv_bfloat16* sl = slab + w * p;
+      float s = 0.f;
+      for (int e = lane; e < pd; e += 32) s += __bfloat162float(sl[offs[e]]);
+      const float mean = warp_sum(s) / (float)pd;
+      float q = 0.f;
+      for (int e = lane; e < pd; e += 32) {
+        const float d = __bfloat162float(sl[offs[e]]) - mean;
+        q = fmaf(d, d, q);
+      }
+      const float rstd = rsqrtf(warp_sum(q) / (float)pd + eps);
+      __nv_bfloat16* orow = out + ((long long)(b * gh + h) * gw + w) * ldo;
+      for (int ch = lane; ch < nchunks; ch += 32) {
+        const int e0 = ch * 8;
+        float y[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int e = e0 + j;  // columns [pd, ldo) are zero (K padding)
+          y[j] = e < pd ? (__bfloat162float(sl[offs[e]]) - mean) * rstd * __ldg(gamma + e) + __ldg(beta + e) : 0.f;
+        }
+        uint4 pk;
+        pk.x = pack_bf16x2(y[0], y[1]);
+        pk.y = pack_bf16x2(y[2], y[3]);
+        pk.z = pack_bf16x2(y[4], y[5]);
+        pk.w = pack_bf16x2(y[6], y[7]);
+        *reinterpret_cast<uint4*>(orow + e0) = pk;
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Token assembly: LN(dim) of the patch projection + positional embedding + cls row  -> fp32 residual stream
 // ---------------------------------------------------------------------------------------------------------------
 // POS = false: no positional term (vit_nd_rotary.py:272-287 has no table; rotary positions act on q / k instead)
-template <bool POS>
+// LN = false: no LayerNorm(dim), the patch rows are y itself (SPT, vit_for_small_dataset.py:127-132)
+template <bool POS, bool LN>
 __global__ void __launch_bounds__(256)
 embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma, const float* __restrict__ beta,
                     const float* __restrict__ cls, const float* __restrict__ pos, float* __restrict__ x,
@@ -320,6 +403,9 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
       emit(i, POS && cls_pos ? cls[(long long)t * D + i] + pr[i] : cls[(long long)t * D + i]);
   } else if (t >= ncls + n) {  // register tokens appended after the patches (simple_vit_with_register_tokens.py:124-126)
     for (int i = lane; i < D; i += 32) emit(i, tail[(long long)(t - ncls - n) * D + i]);
+  } else if (!LN) {
+    const float* yr = y + ((long long)b * n + (t - ncls)) * D;
+    for (int i = lane; i < D; i += 32) emit(i, POS ? yr[i] + pr[i] : yr[i]);
   } else {
     const float* yr = y + ((long long)b * n + (t - ncls)) * D;
     float mean, rstd;
@@ -486,6 +572,31 @@ extern "C" int b200vit_patchify_ln(const void* img, const float* gamma, const fl
   return 0;
 }
 
+extern "C" int b200vit_patchify_spt_ln(const void* img, const float* gamma, const float* beta, void* out_bf16,
+                                       int64_t ldo, int B, int C, int H, int W, int p, float eps, void* stream) {
+  B200_CHECK_ARG(img && gamma && beta && out_bf16, "patchify_spt_ln: null pointer");
+  B200_CHECK_ARG(B > 0 && C > 0 && p > 0 && H > 0 && W > 0 && H % p == 0 && W % p == 0,
+                 "patchify_spt_ln: image %dx%d not divisible by patch %d", H, W, p);
+  const long long pd = 5LL * C * p * p;
+  B200_CHECK_ARG(ldo >= pd && ldo % 8 == 0, "patchify_spt_ln: ldo=%lld must be >= 5*C*p*p=%lld and a multiple of 8",
+                 (long long)ldo, pd);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(out_bf16) & 15) == 0, "patchify_spt_ln: out must be 16-byte aligned");
+  const int rs = (W + SPT_LPAD + 1 + 7) / 8 * 8;  // slab row: zero column, W pixels, zero column, 16-byte multiple
+  const size_t smem = (size_t)((pd + 7) & ~7LL) * sizeof(int) + (size_t)C * (p + 2) * rs * 2;
+  B200_CHECK_ARG(smem <= 200 * 1024, "patchify_spt_ln: patch-row slab of %zu bytes exceeds shared memory", smem);
+  B200_ENSURE_SMEM(patchify_spt_ln_kernel, smem);
+  const int nrows = B * (H / p);
+  const int per_sm = (int)(200 * 1024 / (smem + 1024)) < 8 ? (int)(200 * 1024 / (smem + 1024)) : 8;
+  int grid = num_sms() * (per_sm < 1 ? 1 : per_sm);
+  if (grid > nrows) grid = nrows;
+  patchify_spt_ln_kernel<<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(img), gamma, beta, reinterpret_cast<__nv_bfloat16*>(out_bf16), ldo, nrows,
+      C, H, W, p, rs, eps);
+  B200_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
 extern "C" int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats, int M, int D, void* stream) {
   B200_CHECK_ARG(x && xb_bf16 && stats && M > 0 && D > 0, "rowstats_cast: bad argument");
   rowstats_cast_kernel<<<(M + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
@@ -499,14 +610,15 @@ extern "C" int b200vit_embed_tokens_grouped(const float* y, const float* gamma, 
                                             const float* pos, const float* tail, float* x, void* xb_bf16, float* stats,
                                             int groups, int n, int ncls, int ntail, int D, float eps, int pos_period,
                                             int pos_stride, int cls_pos, void* stream) {
-  B200_CHECK_ARG(y && gamma && beta && x, "embed_tokens: null pointer");
+  B200_CHECK_ARG(y && (beta || !gamma) && x, "embed_tokens: null pointer");
   B200_CHECK_ARG(ncls == 0 || cls, "embed_tokens: ncls=%d without cls", ncls);
   B200_CHECK_ARG(ntail == 0 || tail, "embed_tokens: ntail=%d without tail", ntail);
   B200_CHECK_ARG(groups > 0 && n > 0 && D > 0 && ncls >= 0 && ntail >= 0, "embed_tokens: bad shape");
   B200_CHECK_ARG(pos_period > 0 && pos_stride >= 0, "embed_tokens: bad positional period %d / stride %d", pos_period,
                  pos_stride);
   const long long rows = (long long)groups * (n + ncls + ntail);
-  auto kern = pos ? embed_tokens_kernel<true> : embed_tokens_kernel<false>;
+  auto kern = gamma ? (pos ? embed_tokens_kernel<true, true> : embed_tokens_kernel<false, true>)
+                    : (pos ? embed_tokens_kernel<true, false> : embed_tokens_kernel<false, false>);
   kern<<<(unsigned)((rows + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       y, gamma, beta, cls, pos, x, reinterpret_cast<__nv_bfloat16*>(xb_bf16), stats, groups, n, ncls, D, eps, tail,
       ntail, pos_period, pos_stride, cls_pos != 0);

@@ -17,6 +17,7 @@ Schedule per encoder layer (reference vit.py:78-81), M = B*N token rows, residua
 """
 from __future__ import annotations
 
+import ctypes
 import os
 from dataclasses import dataclass
 from typing import Dict, List, NamedTuple, Optional, Tuple
@@ -167,6 +168,8 @@ class EncoderLayer:
     # attention along the time axis between the attention and the feed-forward block (ViViT's FactorizedTransformer,
     # reference vivit.py:144-150); run_blocks needs `axial` to address its sequences
     temporal: Optional[AttnBlock] = None
+    # each query's own key excluded from its softmax (LSA, vit_for_small_dataset.py:53-57)
+    mask_self: bool = False
 
 
 class _Prepared:
@@ -324,10 +327,12 @@ class TransformerEngine:
         return t
 
     def _c_layers(self, t: Dict[str, torch.Tensor]):
-        """(ctypes array of b200vit_layer, heads, dh, hidden, scale) for the one-call encoder (b200vit_encoder_blocks),
-        or None when it cannot run these layers: they are not uniform, one has a per-head LayerNorm (the one-call
-        encoder has no EPI_HEADLN) or a temporal sub-block.  The pointers stay valid as long as `t` (which holds the tensors)."""
-        sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.scale)      # noqa: E731
+        """(ctypes array of b200vit_layer, (heads, dh, hidden, scale), layer scales, attention flags) for the one-call
+        encoder (b200vit_encoder_blocks), or None when it cannot run these layers: they are not uniform, one has a
+        per-head LayerNorm (the one-call encoder has no EPI_HEADLN) or a temporal sub-block.  Layer scales: None when
+        every layer has the same scale, else a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned
+        temperatures).  The pointers stay valid as long as `t` (which holds the tensors)."""
+        sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
         if any(L.qk_norm == "ln" or L.temporal is not None or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
@@ -340,7 +345,11 @@ class TransformerEngine:
             c.fc1_wg, c.fc1_t, c.fc1_s = p(t[f"{i}.fc1.wg"]), p(t[f"{i}.fc1.t"]), p(t[f"{i}.fc1.s"])
             c.fc2_w, c.fc2_b = p(t[f"{i}.fc2.w"]), p(t[f"{i}.fc2.b"])
             c.ln1_eps, c.ln2_eps = float(L.ln1.eps), float(L.ln2.eps)
-        return arr, sig(self.layers[0])
+        L0 = self.layers[0]
+        scales = [float(L.scale) for L in self.layers]
+        per_layer = None if all(sc == scales[0] for sc in scales) else (ctypes.c_float * len(scales))(*scales)
+        return arr, (L0.heads, L0.dim_head, L0.fc1_w.shape[0], L0.scale), per_layer, \
+            _lib.ATTN_MASK_SELF if L0.mask_self else 0
 
     # -------------------------------------------------------------------------------------------- workspaces
     def workspace(self, M: int, device: torch.device) -> Dict[str, torch.Tensor]:
@@ -404,9 +413,9 @@ class TransformerEngine:
         if (fold and varlen is None and axial is None and t["c_layers"] is not None and not _lib.profiling()
                 and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
             # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
-            arr, (heads, dh, hidden, scale) = t["c_layers"]
+            arr, (heads, dh, hidden, scale), layer_scales, flags = t["c_layers"]
             _lib.encoder_blocks(arr, len(arr), x, self.c_ws, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl,
-                                rope=rope)
+                                rope=rope, layer_scales=layer_scales, attn_flags=flags)
             return
         xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
         if fold and not primed:
@@ -436,9 +445,9 @@ class TransformerEngine:
             if axial is not None and L.temporal is None:
                 axial_attention(L)
             elif vl is None:
-                _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale)
+                _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
             else:
-                _lib.attention_varlen(ws["qkv"], ws["o"], *vl, L.heads, L.dim_head, L.scale)
+                _lib.attention_varlen(ws["qkv"], ws["o"], *vl, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
             if fold:
                 # the residual GEMMs also write the bf16 copy of x and its row statistics for the next folded GEMM
                 _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.out.b"], resid=x,
@@ -489,7 +498,9 @@ class TransformerEngine:
 
 
 class PatchEmbedEngine:
-    """Fused patch embedding + token assembly (reference vit.py:99-104,120-127 / simple_vit.py:90-95,113-114)."""
+    """Fused patch embedding + token assembly (reference vit.py:99-104,120-127 / simple_vit.py:90-95,113-114).  An
+    owner whose to_patch_embedding is an SPT (vit_for_small_dataset.py:81-96: `to_patch_tokens` = Rearrange,
+    LayerNorm, Linear, and no LayerNorm(dim)) gets the shifted-patch kernel instead of the plain patchify."""
 
     def __init__(self, owner: nn.Module) -> None:
         self.owner = owner
@@ -510,17 +521,23 @@ class PatchEmbedEngine:
         key = _version_key(params) + (str(device),)
         if self.prep.key == key:
             return self.prep.t
-        ln1, lin, ln2 = o.to_patch_embedding[1], o.to_patch_embedding[2], o.to_patch_embedding[3]
+        spt = getattr(o.to_patch_embedding, "to_patch_tokens", None)
+        if spt is not None:
+            ln1, lin, ln2 = spt[1], spt[2], None
+        else:
+            ln1, lin, ln2 = o.to_patch_embedding[1], o.to_patch_embedding[2], o.to_patch_embedding[3]
         pd = lin.weight.shape[1]
         kp = (pd + 63) // 64 * 64
         t = {
             "ln1.w": _f32(ln1.weight), "ln1.b": _f32(ln1.bias),
             "w": _bf16_rows(lin.weight, kp), "b": _f32(lin.bias),
-            "ln2.w": _f32(ln2.weight), "ln2.b": _f32(ln2.bias),
+            "ln2.w": None if ln2 is None else _f32(ln2.weight), "ln2.b": None if ln2 is None else _f32(ln2.bias),
         }
         t["kp"] = kp  # type: ignore[assignment]
+        t["spt"] = spt is not None  # type: ignore[assignment]
+        t["ln1.eps"], t["ln2.eps"] = ln1.eps, 1e-5 if ln2 is None else ln2.eps  # type: ignore[assignment]
         ph, pw = getattr(o, "fused_patch_box", None) or o.patch_size
-        if ph == 16 and pw == 16 and pd % 256 == 0:
+        if spt is None and ph == 16 and pw == 16 and pd % 256 == 0:
             # im2col-free path (b200vit_patch_embed_tma): LayerNorm(patch) folded into the projection, weight columns
             # permuted from the reference's (p1 p2 c) order (vit.py:100) to the image's own (c p1 p2)
             C = pd // 256
@@ -573,7 +590,7 @@ class PatchEmbedEngine:
         y = self.project(img, patch)
         x = torch.empty(B * N, D, device=img.device, dtype=torch.float32)
         _lib.embed_tokens(y, t["ln2.w"], t["ln2.b"], t["cls"], pos, x, B, n, ncls, xb=xb, stats=stats,
-                          eps=o.to_patch_embedding[3].eps, tail=t["tail"])
+                          eps=t["ln2.eps"], tail=t["tail"])
         return x, B, N
 
     def project(self, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None) -> torch.Tensor:
@@ -593,11 +610,14 @@ class PatchEmbedEngine:
                 and W // pw <= 128 and D % 8 == 0):
             # the wgmma GEMM reads the image itself: no patch matrix, no LayerNorm pass
             stats_p = torch.empty(B * n, 2, device=dev, dtype=torch.float32)
-            _lib.patch_embed_tma(img.contiguous(), t["tma.w"], t["tma.b"], t["tma.s"], stats_p, y,
-                                 eps=o.to_patch_embedding[1].eps)
+            _lib.patch_embed_tma(img.contiguous(), t["tma.w"], t["tma.b"], t["tma.s"], stats_p, y, eps=t["ln1.eps"])
         else:
             a0 = torch.empty(B * n, t["kp"], device=dev, dtype=torch.bfloat16)
-            _lib.patchify_ln(img.contiguous(), t["ln1.w"], t["ln1.b"], a0, ph, pw, eps=o.to_patch_embedding[1].eps)
+            if t["spt"]:
+                # the five shifted copies are gathered straight from the image (vit_for_small_dataset.py:92-96)
+                _lib.patchify_spt_ln(img.contiguous(), t["ln1.w"], t["ln1.b"], a0, ph, eps=t["ln1.eps"])
+            else:
+                _lib.patchify_ln(img.contiguous(), t["ln1.w"], t["ln1.b"], a0, ph, pw, eps=t["ln1.eps"])
             _lib.gemm(a0, t["w"], out_f32=y, bias=t["b"])
         return y
 
