@@ -353,6 +353,7 @@ extern "C" int b200vit_debug_set(int key, int value) {
     case 11: g_varlen_mode = value; return 0;
     case 12: gemm_set_block_n(value); return 0;
     case 13: g_attn_emul = value; return 0;
+    case 14: gemm_set_direct_store(value); return 0;
     default: return B200VIT_ERR_INVALID;
   }
 }

@@ -5,12 +5,24 @@
 //                     warp 1 (one thread, residual GEMMs only): the fp32 residual tile, TMA -> two 64-column slabs
 //                     warp 2: the tile's bias / col_s slices and LN-fold row sums -> smem (double buffered per tile)
 //   warpgroups 1, 2 : consumers     (wgmma m64 x BLOCK_N x k16, fp32 accumulators in registers, 64 rows each), then
-//                     the epilogue straight from the accumulator registers: bias / LN-fold / GELU / residual -> global
+//                     the epilogue from the accumulator registers: bias / LN-fold / GELU / residual
 //
 // The loaders run ahead into the next tile while the consumers finish the epilogue of the current one, so every
-// epilogue input is already in shared memory when the accumulators are ready: the epilogue's only global-memory
-// instructions are its stores.  (Read from global memory inside the epilogue, each residual load would wait behind the
-// previous column's stores -- resid may be out_f32 itself -- for a full memory latency.)
+// epilogue input is already in shared memory when the accumulators are ready.  (Read from global memory inside the
+// epilogue, each residual load would wait behind the previous column's stores -- resid may be out_f32 itself -- for a
+// full memory latency.)
+// The outputs leave through shared memory too, written by TMA stores that drain while the consumers go on.  Written
+// from the registers instead, every warp store puts 16 bytes into each of 8 rows, and the tile is bound by the rate of
+// store instructions, not by HBM.
+//   bf16 output (QKV, FC1): the epilogue writes 128B-swizzled staging boxes of 64 x 64 for the whole tile, one thread
+//     per warpgroup hands them to TMA stores, and the consumers go straight on to the next tile's MMAs.  Thread 0 waits
+//     for the stores to have read the staging tile during the next tile's first k block, before it is written again.
+//   residual (out-proj, FC2; 128-wide tiles): the fp32 sum goes back into the residual slab at the address its
+//     residual was read from and is TMA-stored from there; the bf16 copy is held in registers until the previous
+//     slab's stores have read the one 16 KB staging chunk.  A slab returns to the residual loader once its stores have
+//     read it: at the next slab, or during the next tile's first k block.
+// The direct-store epilogue remains for non-residual fp32 outputs, patch tiles of fewer than 128 rows, ldo or N not a
+// multiple of 8, 256-wide residual tiles (test hook 12) and every launch under test hook 14.
 // Replaces the nn.Linear call sites listed in include/b200vit.h.
 #include "common.cuh"
 #include "host_util.h"
@@ -56,7 +68,11 @@ struct GemmParams {
 // RES (EPI_RESIDUAL launches): two residual slabs of 128 rows x 64 fp32 columns after the ring.  A slab is two TMA
 // boxes of 32 columns (128 B per row, 128B swizzle: 16-byte chunk c of row r sits at chunk c ^ (r % 8)), so that the
 // epilogue's float2 reads -- 8 rows x 4 column pairs per warp instruction -- touch every bank exactly twice.
-template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false>
+// TMA_OUT: the bf16 output is staged in 128B-swizzled boxes of 64 rows x 64 columns (8 KB) and written by TMA stores.
+// Without RES that is the whole tile (consumer warpgroup c owns boxes [c * BLOCK_N / 64, (c + 1) * BLOCK_N / 64)); with
+// RES one 128 x 64 chunk, the bf16 copy of the slab being stored (warpgroup c owns its c-th box), while the fp32 sums
+// go back into the residual slab they were read from and are stored from there.
+template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false>
 struct GemmSmem {
   static constexpr int A_SLAB = PATCH ? BLOCK_M * 32 : BLOCK_M * BLOCK_K * 2;
   static constexpr int A_BYTES = PATCH ? 4 * A_SLAB : A_SLAB;
@@ -65,8 +81,11 @@ struct GemmSmem {
   static constexpr int RES_BOX = BLOCK_M * 32 * 4;
   static constexpr int RES_SLAB = 2 * RES_BOX;
   static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int OUT_BOX = 64 * 64 * 2;
+  static constexpr int OUT_OFFSET = RES_OFFSET + (RES ? 2 * RES_SLAB : 0);
+  static constexpr int OUT_BYTES = !TMA_OUT ? 0 : RES ? 2 * OUT_BOX : BLOCK_M * BLOCK_N * 2;
   // per tile, double buffered: bias[BLOCK_N], col_s[BLOCK_N], LN-fold row sums [BLOCK_M][2]
-  static constexpr int VEC_OFFSET = RES_OFFSET + (RES ? 2 * RES_SLAB : 0);
+  static constexpr int VEC_OFFSET = OUT_OFFSET + OUT_BYTES;
   static constexpr int VEC_BYTES = (2 * BLOCK_N + 2 * BLOCK_M) * 4;
   static constexpr int BAR_OFFSET = VEC_OFFSET + 2 * VEC_BYTES;
   // full[STAGES], empty[STAGES], res_full[2], res_empty[2], vec_full[2], vec_empty[2]
@@ -74,11 +93,18 @@ struct GemmSmem {
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024B alignment
 };
 
-template <int BLOCK_N, int STAGES, bool PATCH, bool RES>
+// named barrier over the 128 threads of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
+// (the id comes from a register, so ptxas reserves all 16 named barriers; harmless at one CTA per SM)
+__device__ __forceinline__ void warpgroup_sync(int c) { asm volatile("bar.sync %0, 128;" ::"r"(c + 1) : "memory"); }
+
+// tmO / tmF (TMA_OUT only): store maps over out_bf16 (64 x 64 boxes) and out_f32 (32 x 64 boxes), 128B swizzle
+template <int BLOCK_N, int STAGES, bool PATCH, bool RES, bool TMA_OUT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
-  using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES>;
+                 const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO,
+                 const __grid_constant__ CUtensorMap tmF, const GemmParams p) {
+  static_assert(!(TMA_OUT && PATCH), "patch tiles have fewer than 128 rows: a 64-row box would overwrite the next one");
+  using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
   constexpr int NACC = BLOCK_N / 2;          // fp32 accumulators per consumer thread (64 rows x BLOCK_N / 128)
   constexpr int CHUNKS = BLOCK_N / 64;       // 64-column statistics chunks (and residual slabs) per tile
 
@@ -100,13 +126,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (RES) tma_prefetch_desc(&tmR);
+    if (TMA_OUT && p.out_bf16) tma_prefetch_desc(&tmO);
+    if (TMA_OUT && RES && p.out_f32) tma_prefetch_desc(&tmF);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
     for (int s = 0; s < 2; ++s) {
       mbar_init(&res_full[s], 1);
-      mbar_init(&res_empty[s], NUM_CONSUMERS);
+      // TMA_OUT: thread 0 of each consumer warpgroup, once the stores of its half of the slab have read it
+      mbar_init(&res_empty[s], TMA_OUT ? 2 : NUM_CONSUMERS);
       mbar_init(&vec_full[s], 64);  // every thread of loader warps 2 and 3
       mbar_init(&vec_empty[s], NUM_CONSUMERS);
     }
@@ -222,6 +251,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   int stage = 0;
   uint32_t phase = 0;
   int slab_it = 0;  // residual slabs consumed so far (the loader's count)
+  int pend_slab = -1;  // TMA_OUT && RES, thread 0: the slab buffer whose stores may still be reading it
+  uint8_t* const stg_wg = smem + L::OUT_OFFSET + c * (RES ? L::OUT_BOX : 64 * BLOCK_N * 2);
   float acc[NACC];
 
   for (int tile = blockIdx.x, it = 0; tile < num_tiles; tile += gridDim.x, ++it) {
@@ -244,6 +275,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         else wgmma_m64n128k16(acc, ad, bdesc + 2 * k, (kb | k) != 0);
       }
       wgmma_commit();
+      // while the first MMAs run: the previous tile's output stores have read the staging tile (RES: and the last
+      // slab, which goes back to the residual loader so that it can fill it during this main loop)
+      if (TMA_OUT && kb == 0 && t == 0) {
+        tma_store_wait_read<0>();
+        if (RES && pend_slab >= 0) mbar_arrive(&res_empty[pend_slab]);
+        pend_slab = -1;
+      }
       // the MMAs of the previous k block have finished reading their stage once at most one group is in flight
       wgmma_wait<1>();
       if (prev_stage >= 0 && t == 0) mbar_arrive(&empty_bar[prev_stage]);
@@ -256,6 +294,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     wgmma_wait<0>();
     fence_regs(acc);
     if (t == 0) mbar_arrive(&empty_bar[prev_stage]);
+    if (TMA_OUT && !RES) warpgroup_sync(c);  // ... and the whole warpgroup may write it again
 
     // ---------------------------------------------------------------- epilogue
     // accumulator layout (wgmma m64nN, fp32): acc[4j + h] holds row (16 warp + lane/4 + 8 (h >> 1)),
@@ -292,12 +331,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // of box (j % 8) / 4, 8-byte half lane & 1
     const int res_off = tr0 * 128 + (lane & 1) * 8;
     const int res_xor = ((lane & 3) >> 1) ^ (lane >> 2);
+    // TMA_OUT: this thread's bf16 pair in a staging box: row tr0 % 64 (+ 8 h), 16-byte chunk (j % 8) ^ (tr0 % 8),
+    // byte 4 (lane % 4) -- the 8 rows of a warp store land in 8 different chunks, so the stores are conflict free
+    const int stg_off = (tr0 - 64 * c) * 128 + 4 * (lane & 3);
+    // TMA_OUT && RES: the bf16 pairs of the current slab, held until the staging chunk is free again
+    uint32_t pks[8][2] = {};
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
       const int pc = 8 * j + 2 * (lane & 3);  // column of the pair in the tile
       const int col = n0 + pc;
       if (RES && j % 8 == 0 && j / 8 < nslab) mbar_wait(&res_full[slab_it & 1], (slab_it >> 1) & 1);
-      const uint8_t* slab = smem + L::RES_OFFSET + (slab_it & 1) * L::RES_SLAB + ((j % 8) / 4) * L::RES_BOX + res_off;
+      uint8_t* slab = smem + L::RES_OFFSET + (slab_it & 1) * L::RES_SLAB + ((j % 8) / 4) * L::RES_BOX + res_off;
+      uint8_t* stg = stg_wg + (RES ? 0 : (j / 8) * L::OUT_BOX) + stg_off + (((j % 8) ^ (lane >> 2)) << 4);
       const bool pair = vec_ok && col + 1 < p.N;
       float b0 = 0.f, b1 = 0.f, s0 = 0.f, s1 = 0.f;
       if (flags & B200VIT_EPI_BIAS) {
@@ -325,10 +370,25 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         if (flags & B200VIT_EPI_GELU) gelu_erf2(v0, v1);
         const size_t o = (size_t)row[h] * p.ldo + col;
+        float2* rp = reinterpret_cast<float2*>(slab + h * 8 * 128 + ((((j % 4) * 2) ^ res_xor) << 4));
         float2 rr = make_float2(0.f, 0.f);
-        if (RES) rr = *reinterpret_cast<const float2*>(slab + h * 8 * 128 + ((((j % 4) * 2) ^ res_xor) << 4));
+        if (RES) rr = *rp;
         float r0 = 0.f, r1 = 0.f;
-        if (pair) {
+        if (TMA_OUT) {
+          // the same values as below, into shared memory: the fp32 sum where its residual was read (no other thread
+          // touches that address), the bf16 pair into the staging box (rows past M are clipped by the store maps; N is
+          // a multiple of 8, so col + 1 < N)
+          if (RES) {
+            v0 += rr.x;
+            v1 += rr.y;
+            if (p.out_f32) *rp = make_float2(v0, v1);
+          }
+          const uint32_t pk = pack_bf16x2(v0, v1);
+          if (RES) pks[j % 8][h] = pk;
+          else *reinterpret_cast<uint32_t*>(stg + h * 8 * 128) = pk;
+          r0 = __uint_as_float(pk << 16);
+          r1 = __uint_as_float(pk & 0xFFFF0000u);
+        } else if (pair) {
           if (RES) {
             v0 += rr.x;
             v1 += rr.y;
@@ -359,11 +419,54 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
       if (RES && j % 8 == 7 && j / 8 < nslab) {
-        mbar_arrive(&res_empty[slab_it & 1]);
+        if constexpr (TMA_OUT) {
+          // The previous slab's stores have had this slab's arithmetic to read the chunk and their slab: wait for
+          // them, hand that slab back to the loader, then stage this slab's bf16 copy and store the slab and the chunk.
+          if (t == 0) {
+            tma_store_wait_read<0>();
+            if (pend_slab >= 0) mbar_arrive(&res_empty[pend_slab]);
+            pend_slab = -1;
+          }
+          warpgroup_sync(c);
+          if (p.out_bf16)
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<uint32_t*>(stg_wg + stg_off + ((jj ^ (lane >> 2)) << 4) + h * 8 * 128) = pks[jj][h];
+          fence_proxy_async_smem();
+          warpgroup_sync(c);
+          if (t == 0) {
+            const int buf = slab_it & 1, c0 = n0 + 64 * (j / 8), row0 = m_blk * BLOCK_M + 64 * c;
+            if (row0 < p.M) {
+              const uint8_t* half = smem + L::RES_OFFSET + buf * L::RES_SLAB + c * 64 * 128;
+              if (p.out_f32)
+                for (int b = 0; b < 2 && c0 + 32 * b < p.N; ++b)
+                  tma_store_2d(&tmF, half + b * L::RES_BOX, c0 + 32 * b, row0);
+              if (p.out_bf16) tma_store_2d(&tmO, stg_wg, c0, row0);
+            }
+            tma_store_commit();
+            pend_slab = buf;
+          }
+        } else {
+          mbar_arrive(&res_empty[slab_it & 1]);
+        }
         ++slab_it;
       }
     }
     mbar_arrive(&vec_empty[vb]);
+    if constexpr (TMA_OUT && !RES) {
+      // generic-proxy writes -> visible to the TMA unit, then one thread stores the warpgroup's 64 rows, box by box
+      fence_proxy_async_smem();
+      warpgroup_sync(c);
+      if (t == 0) {
+        const int row0 = m_blk * BLOCK_M + 64 * c;
+        if (row0 < p.M)
+          for (int b = 0; b < BLOCK_N / 64 && n0 + 64 * b < p.N; ++b)
+            tma_store_2d(&tmO, stg_wg + b * L::OUT_BOX, n0 + 64 * b, row0);
+        tma_store_commit();
+      }
+    }
     if (flags & B200VIT_EPI_STATS) {
       // the four lanes of a quad hold the same two rows: reduce, then lane 0 of the quad writes every part of the tile
 #pragma unroll
@@ -397,18 +500,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   }
+  if (TMA_OUT && t == 0) tma_store_wait<0>();
 }
 
-// test hook 12: BLOCK_N of b200vit_gemm_bf16 -- 0 = auto (256 when N > 128), 1 = 128, 2 = 256
+// test hook 12: BLOCK_N of b200vit_gemm_bf16 -- 0 = auto, 1 = 128, 2 = 256
 static std::atomic<int> g_gemm_block_n{0};
 void gemm_set_block_n(int v) { g_gemm_block_n = v; }
+// test hook 14: 1 = every b200vit_gemm_bf16 launch takes the direct-store epilogue
+static std::atomic<int> g_gemm_direct_store{0};
+void gemm_set_direct_store(int v) { g_gemm_direct_store = v; }
 
-template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, GemmParams& p,
-                       cudaStream_t stream) {
-  using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES>;
+template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
+                       const CUtensorMap& tmF, GemmParams& p, cudaStream_t stream) {
+  using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
   static_assert(L::DYN_BYTES <= 227 * 1024, "gemm: shared memory budget");
-  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
   B200_ENSURE_SMEM(kern, L::DYN_BYTES);
   if (!p.patch) p.rows_per_tile = BLOCK_M;
   p.num_m_tiles = (p.M + p.rows_per_tile - 1) / p.rows_per_tile;
@@ -417,7 +524,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   p.stats_width = p.N > 128 ? 128 : 64;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(tmA, tmB, tmR, p);
+  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(tmA, tmB, tmR, tmO, tmF, p);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
@@ -472,11 +579,33 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   p.col_s = col_s;
   p.stats_out = stats_out;
 
-  const int force = g_gemm_block_n.load();
-  const bool wide = force == 0 ? N > 128 : force == 2;
-  const uint32_t block_n = wide ? 256 : 128;
   const bool res = (flags & B200VIT_EPI_RESIDUAL) != 0;
-  CUtensorMap tmA, tmB, tmR{};
+  // The TMA-store epilogue takes bf16 outputs and residual launches (fp32 + bf16), with ldo and N multiples of 8 so
+  // that every row and its written part are whole 16-byte units (a precaution at N: the store maps clip there anyway).
+  // A non-residual fp32 output (off the hot path) has no room for its 128 KB staging tile and stores from the
+  // registers, as do patch tiles.  Residual launches run 128-wide tiles: at 256 columns the residual slabs leave no
+  // room for the staging chunk beside the ring.
+  const bool tma_ok = !g_gemm_direct_store.load() && ((ldo | N) & 7) == 0 && (res || !out_f32);
+  const int force = g_gemm_block_n.load();
+  const bool wide = force == 0 ? N > 128 && !(res && tma_ok) : force == 2;
+  const uint32_t block_n = wide ? 256 : 128;
+  const bool tma_out = tma_ok && !(res && wide);
+  CUtensorMap tmA, tmB, tmR{}, tmO{}, tmF{};
+  if (tma_out && out_bf16) {
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
+    const uint64_t strides[1] = {(uint64_t)ldo * 2};
+    const uint32_t box[2] = {64, 64};
+    int rc = encode_tmap_bf16(&tmO, out_bf16, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  if (tma_out && res && out_f32) {
+    // the residual slab's layout: 32-column boxes (128 B rows, 128B swizzle), 64 rows per consumer warpgroup
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
+    const uint64_t strides[1] = {(uint64_t)ldo * 4};
+    const uint32_t box[2] = {32, 64};
+    int rc = encode_tmap_f32(&tmF, out_f32, 2, dims, strides, box, true);
+    if (rc) return rc;
+  }
   if (res) {
     // fp32 residual, 32-column boxes (128 B rows, 128B swizzle) of one tile's 128 rows
     const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
@@ -499,9 +628,17 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
     int rc = encode_tmap_bf16(&tmB, W, 2, dims, strides, box);
     if (rc) return rc;
   }
-  // residual launches trade ring stages for the two 32 KB residual slabs
-  if (wide) return res ? launch_gemm<256, 3, false, true>(tmA, tmB, tmR, p, st) : launch_gemm<256, 4>(tmA, tmB, tmR, p, st);
-  return res ? launch_gemm<128, 4, false, true>(tmA, tmB, tmR, p, st) : launch_gemm<128, 6>(tmA, tmB, tmR, p, st);
+  // residual launches trade ring stages for the two 32 KB residual slabs, TMA-store launches for the staging buffers
+  if (tma_out) {
+    if (res) return launch_gemm<128, 4, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st);
+    return wide ? launch_gemm<256, 3, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st)
+                : launch_gemm<128, 5, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st);
+  }
+  if (wide)
+    return res ? launch_gemm<256, 3, false, true>(tmA, tmB, tmR, tmO, tmF, p, st)
+               : launch_gemm<256, 4>(tmA, tmB, tmR, tmO, tmF, p, st);
+  return res ? launch_gemm<128, 4, false, true>(tmA, tmB, tmR, tmO, tmF, p, st)
+             : launch_gemm<128, 6>(tmA, tmB, tmR, tmO, tmF, p, st);
 }
 
 extern "C" int b200vit_rmsnorm_heads(void* buf, int64_t ld, const float* gamma, int T, int nheads, int dh, void* stream);
@@ -571,7 +708,7 @@ extern "C" int b200vit_patch_embed_tma(const void* img, const void* w_perm, cons
   p.patch_tiles_per_img = gh / ght;
   p.patch_C = C;
   p.rows_per_tile = ght * gw;
-  CUtensorMap tmA, tmB, tmR{};
+  CUtensorMap tmA, tmB, tmR{}, tmO{}, tmF{};
   {
     // innermost first: pixel in a patch row | patch column | patch row | pixel row in the patch | image x channel
     const uint64_t dims[5] = {16, (uint64_t)gw, (uint64_t)gh, 16, (uint64_t)B * C};
@@ -587,5 +724,5 @@ extern "C" int b200vit_patch_embed_tma(const void* img, const void* w_perm, cons
     int rc = encode_tmap_bf16(&tmB, w_perm, 2, dims, strides, box);
     if (rc) return rc;
   }
-  return launch_gemm<256, 4, true>(tmA, tmB, tmR, p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_gemm<256, 4, true>(tmA, tmB, tmR, tmO, tmF, p, reinterpret_cast<cudaStream_t>(stream));
 }

@@ -48,8 +48,9 @@ void tmap_cache_stats(int64_t* hits, int64_t* misses);
 // The head widths (dim_head) the attention, head-norm and pooling kernels are built for.
 inline bool head_width_ok(int dh) { return dh == 32 || dh == 64 || dh == 80 || dh == 128; }
 
-// test hook 12 (gemm.cu)
+// test hooks 12 and 14 (gemm.cu)
 void gemm_set_block_n(int v);
+void gemm_set_direct_store(int v);
 
 // SM count of the CURRENT device (cached per device).
 int num_sms();
