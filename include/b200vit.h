@@ -270,6 +270,22 @@ int b200vit_embed_varlen(const float* y, const float* gamma, const float* pos_h,
 int b200vit_attn_pool(const void* kv, const float* qn, const int32_t* cu_seqlens_dev, void* out, int S, int H, int dh,
                       void* stream);
 
+/*
+ * Class-token cross attention (CrossViT, cross_vit.py:53-71 with kv_include_self = True): one query per image attends
+ * over its own key / value and n context rows of the same image.  For image b < B and head h < H:
+ *   out[b, h*dh:(h+1)*dh] = softmax_j(scale * q_bh . k_jh) v_jh,   j over {self} u {the n context rows of image b}
+ *   qkv_self[B, 3*H*dh] bf16, packed q | k | v as for b200vit_attention: q, the self key and the self value of image b.
+ *   ctx_kv: [k | v] rows 2*H*dh wide (row stride ctx_ld); image b's rows start at row b*ctx_rows_per_image + ctx_first
+ *   (a kv GEMM over every row of the other stream, its cls rows skipped with ctx_first = 1).
+ *   out: bf16 [B, H*dh], row stride ldo.
+ * n = 0..16384 (n = 0: out = v_self), dh = 32, 64, 80 or 128; softmax in fp32.  One CTA of 8 warps per (image, head):
+ * the NaViT pooling kernel above with a per-image bf16 query and a strided context.  ctx_ld and ldo multiples of 8,
+ * pointers 16-byte aligned; ctx_kv may be NULL when n = 0.
+ */
+int b200vit_attention_cls(const void* qkv_self, const void* ctx_kv, int64_t ctx_ld, int64_t ctx_rows_per_image,
+                          int ctx_first, int n, void* out, int64_t ldo, int B, int H, int dh, float scale,
+                          void* stream);
+
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */
 int b200vit_mean_pool(const float* x, float* out, int B, int N, int D, int n_pool, void* stream);

@@ -34,7 +34,7 @@ SYMBOLS = [
     "b200vit_gemm_headnorm_bf16", "b200vit_layernorm_heads", "b200vit_patch_stats", "b200vit_patch_embed_tma",
     "b200vit_encoder_blocks", "b200vit_patchify_nd", "b200vit_rope_qk", "b200vit_encoder_blocks_rope",
     "b200vit_attention_axial", "b200vit_embed_tokens_grouped", "b200vit_patchify_spt_ln", "b200vit_attention_ex",
-    "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex",
+    "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex", "b200vit_attention_cls",
 ]
 
 
@@ -114,6 +114,8 @@ def lib() -> C.CDLL:
     L.b200vit_embed_varlen.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]
     L.b200vit_attn_pool.restype = i32
     L.b200vit_attn_pool.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp]
+    L.b200vit_attention_cls.restype = i32
+    L.b200vit_attention_cls.argtypes = [vp, vp, i64, i64, i32, i32, vp, i64, i32, i32, i32, f32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -643,6 +645,25 @@ def attn_pool(kv: torch.Tensor, qn: torch.Tensor, cu_seqlens: torch.Tensor, out:
     with _Timed("attn_pool", bytes=kv.numel() * 2):
         rc = lib().b200vit_attn_pool(_ptr(kv), _ptr(qn), _ptr(cu_seqlens), _ptr(out), S, H, dh, _stream())
     _check(rc, "b200vit_attn_pool")
+
+
+def attention_cls(qkv_self: torch.Tensor, ctx: Optional[torch.Tensor], out: torch.Tensor, rows_per_image: int,
+                  first: int, n: int, H: int, dh: int, scale: float) -> None:
+    """Class-token cross attention: the query of image b (row b of qkv_self[B, 3*H*dh], q | k | v) attends over its
+    own k / v and rows b*rows_per_image + first + j (j < n) of the [k | v] matrix ctx (row stride ctx.stride(0)).
+    out [B, H*dh] bf16, any row stride."""
+    _chk(qkv_self, torch.bfloat16, "qkv_self"); _chk(ctx, torch.bfloat16, "ctx"); _chk(out, torch.bfloat16, "out")
+    B = qkv_self.shape[0]
+    assert qkv_self.is_contiguous() and qkv_self.shape[1] == 3 * H * dh
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (B, H * dh)
+    assert ctx is None or (ctx.dim() == 2 and ctx.stride(1) == 1 and ctx.shape[1] >= 2 * H * dh
+                           and ctx.shape[0] >= (B - 1) * rows_per_image + first + n)
+    with _Timed("attention_cls", B=B, n=n, H=H, bytes=(B * n * 2 * H * dh + qkv_self.numel() + out.numel()) * 2,
+                flops=4.0 * B * H * (n + 1) * dh):
+        rc = lib().b200vit_attention_cls(_ptr(qkv_self), _ptr(ctx), 0 if ctx is None else ctx.stride(0),
+                                         int(rows_per_image), int(first), int(n), _ptr(out), out.stride(0), B, H, dh,
+                                         float(scale), _stream())
+    _check(rc, "b200vit_attention_cls")
 
 
 def mean_pool(x: torch.Tensor, out: torch.Tensor, B: int, N: int, D: int, n_pool: Optional[int] = None) -> None:

@@ -745,10 +745,18 @@ rmsnorm_heads_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float*
 //   shared memory -- a 1024-token image no longer takes 64x the time of a 16-token one on a single warp.
 //   Lane l owns the element pairs l, l + 32, ... of the head (NP = DH / 64 rounded up); pairs beyond DH / 2 (dh 32
 //   and 80) are masked: zero q, k and v, never stored.
-template <int DH>
+//
+// CLS = true: class-token cross attention (CrossViT, reference cross_vit.py:53-71 with kv_include_self): the query of
+//   image s is row s of the packed qkv_self[S, 3*H*DH] (bf16, q | k | v), multiplied by `scale`; its own k and v (the
+//   same row) are the first key and value, taken by warp 0 before its share of the context.  The n context [k | v]
+//   rows of image s are rows s*ctx_rows + ctx_first + j (j < n) of kv, row stride ctx_ld; out row stride ldo.  cu and
+//   qn are unused.  The CLS = false instances (NaViT) read none of the trailing parameters.
+template <int DH, bool CLS = false>
 __global__ void __launch_bounds__(256)
 attn_pool_kernel(const __nv_bfloat16* __restrict__ kv, const float* __restrict__ qn, const int* __restrict__ cu,
-                 __nv_bfloat16* __restrict__ out, int S, int H) {
+                 __nv_bfloat16* __restrict__ out, int S, int H, const __nv_bfloat16* __restrict__ qkv_self = nullptr,
+                 long long ctx_ld = 0, long long ctx_rows = 0, int ctx_first = 0, int n = 0, long long ldo = 0,
+                 float scale = 1.f) {
   constexpr int NW = 8;
   constexpr int NP = (DH + 63) / 64;   // element pairs per lane
   __shared__ float part[NW][4 + DH];   // m, l, -, -, acc[DH]
@@ -758,22 +766,48 @@ attn_pool_kernel(const __nv_bfloat16* __restrict__ kv, const float* __restrict__
   const int I = H * DH;
   bool act[NP];
   float2 q[NP];
+  const __nv_bfloat16* self = CLS ? qkv_self + (long long)s * 3 * I + h * DH : nullptr;
 #pragma unroll
   for (int c = 0; c < NP; ++c) {
     act[c] = 2 * (32 * c + lane) < DH;
-    q[c] = act[c] ? *reinterpret_cast<const float2*>(qn + h * DH + 2 * (32 * c + lane)) : make_float2(0.f, 0.f);
+    if (CLS) {
+      const float2 z = make_float2(0.f, 0.f);
+      const float2 qq = act[c] ? __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(self) + 32 * c + lane)) : z;
+      q[c] = make_float2(qq.x * scale, qq.y * scale);
+    } else {
+      q[c] = act[c] ? *reinterpret_cast<const float2*>(qn + h * DH + 2 * (32 * c + lane)) : make_float2(0.f, 0.f);
+    }
   }
   float m = -INFINITY, l = 0.f, a0[NP], a1[NP];
 #pragma unroll
   for (int c = 0; c < NP; ++c) a0[c] = a1[c] = 0.f;
-  const int j0 = cu[s], j1 = cu[s + 1];
+  if (CLS && warp == 0) {
+    // the query token's own key and value (kv_include_self, cross_vit.py:58-59) open warp 0's running softmax
+    float sc = 0.f;
+#pragma unroll
+    for (int c = 0; c < NP; ++c) {
+      if (!act[c]) continue;
+      const float2 k = __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(self + I) + 32 * c + lane));
+      const float2 v = __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(self + 2 * I) + 32 * c + lane));
+      sc += q[c].x * k.x + q[c].y * k.y;
+      a0[c] = v.x;
+      a1[c] = v.y;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sc += __shfl_xor_sync(0xffffffffu, sc, o);
+    m = sc;
+    l = 1.f;
+  }
+  const int j0 = CLS ? 0 : cu[s], j1 = CLS ? n : cu[s + 1];
+  const __nv_bfloat16* ctx = CLS ? kv + ((long long)s * ctx_rows + ctx_first) * ctx_ld + h * DH : nullptr;
   // four tokens per step: eight independent loads and four interleaved butterflies, one rescale of the running sums
   for (int j = j0 + 4 * warp; j < j1; j += 4 * NW) {
     const int cnt = j1 - j < 4 ? j1 - j : 4;
     float2 k[4][NP], v[4][NP];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const __nv_bfloat16* r = kv + (long long)(j + (i < cnt ? i : 0)) * 2 * I + h * DH;
+      const __nv_bfloat16* r = CLS ? ctx + (long long)(j + (i < cnt ? i : 0)) * ctx_ld
+                                   : kv + (long long)(j + (i < cnt ? i : 0)) * 2 * I + h * DH;
 #pragma unroll
       for (int c = 0; c < NP; ++c) {
         const float2 z = make_float2(0.f, 0.f);
@@ -844,7 +878,8 @@ attn_pool_kernel(const __nv_bfloat16* __restrict__ kv, const float* __restrict__
         A1 = fmaf(part[w][5 + e], f, A1);
       }
       const float inv = 1.0f / L;
-      *reinterpret_cast<__nv_bfloat162*>(out + (long long)s * I + h * DH + e) = __floats2bfloat162_rn(A0 * inv, A1 * inv);
+      *reinterpret_cast<__nv_bfloat162*>(out + (long long)s * (CLS ? ldo : I) + h * DH + e) =
+          __floats2bfloat162_rn(A0 * inv, A1 * inv);
     }
   }
 }
@@ -997,6 +1032,52 @@ extern "C" int b200vit_attn_pool(const void* kv, const float* qn, const int32_t*
     case 80: attn_pool_kernel<80><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H); break;
     case 128: attn_pool_kernel<128><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H); break;
     default: attn_pool_kernel<64><<<S * H, 256, 0, st>>>(k, qn, cu_seqlens_dev, o, S, H);
+  }
+  B200_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+extern "C" int b200vit_attention_cls(const void* qkv_self, const void* ctx_kv, int64_t ctx_ld,
+                                     int64_t ctx_rows_per_image, int ctx_first, int n, void* out, int64_t ldo, int B,
+                                     int H, int dh, float scale, void* stream) {
+  B200_CHECK_ARG(qkv_self && out && (ctx_kv || n == 0), "attention_cls: null pointer");
+  B200_CHECK_ARG(B > 0 && H > 0, "attention_cls: bad shape B=%d H=%d", B, H);
+  B200_CHECK_ARG(head_width_ok(dh), "attention_cls: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
+  B200_CHECK_ARG(n >= 0 && n <= 16384, "attention_cls: n=%d context rows out of range [0, 16384]", n);
+  B200_CHECK_ARG(ctx_first >= 0 && ctx_rows_per_image >= (int64_t)ctx_first + n,
+                 "attention_cls: context rows [%d, %d) exceed the %lld rows per image", ctx_first, ctx_first + n,
+                 (long long)ctx_rows_per_image);
+  const int64_t I = (int64_t)H * dh;
+  B200_CHECK_ARG(ldo >= I && (ldo % 8) == 0, "attention_cls: ldo=%lld must be >= H*dh and a multiple of 8",
+                 (long long)ldo);
+  B200_CHECK_ARG(n == 0 || (ctx_ld >= 2 * I && (ctx_ld % 8) == 0),
+                 "attention_cls: ctx_ld=%lld must be >= 2*H*dh and a multiple of 8", (long long)ctx_ld);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv_self) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
+                     (reinterpret_cast<uintptr_t>(ctx_kv) & 15) == 0,
+                 "attention_cls: qkv_self, ctx_kv and out must be 16-byte aligned");
+  B200_CHECK_ARG((int64_t)B * H <= 0x7fffffff, "attention_cls: B*H too large");
+  const auto* q = reinterpret_cast<const __nv_bfloat16*>(qkv_self);
+  const auto* k = reinterpret_cast<const __nv_bfloat16*>(ctx_kv);
+  auto* o = reinterpret_cast<__nv_bfloat16*>(out);
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  const long long ld = ctx_ld, rows = ctx_rows_per_image, lo = ldo;
+  switch (dh) {
+    case 32:
+      attn_pool_kernel<32, true><<<B * H, 256, 0, st>>>(k, nullptr, nullptr, o, B, H, q, ld, rows, ctx_first, n, lo,
+                                                        scale);
+      break;
+    case 80:
+      attn_pool_kernel<80, true><<<B * H, 256, 0, st>>>(k, nullptr, nullptr, o, B, H, q, ld, rows, ctx_first, n, lo,
+                                                        scale);
+      break;
+    case 128:
+      attn_pool_kernel<128, true><<<B * H, 256, 0, st>>>(k, nullptr, nullptr, o, B, H, q, ld, rows, ctx_first, n, lo,
+                                                         scale);
+      break;
+    default:
+      attn_pool_kernel<64, true><<<B * H, 256, 0, st>>>(k, nullptr, nullptr, o, B, H, q, ld, rows, ctx_first, n, lo,
+                                                        scale);
   }
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();

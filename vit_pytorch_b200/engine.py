@@ -243,6 +243,16 @@ def _fold(t: Dict[str, torch.Tensor], prefix: str, w: torch.Tensor, b: Optional[
         t[prefix + ".t"] = (tb + b.detach().float() if b is not None else tb).contiguous()
 
 
+class Workspace:
+    """Scratch buffers of a TransformerEngine: `t` by name, `c` the _lib.EncoderWs over them, `key` what they were
+    allocated for (rows, device, stream)."""
+
+    def __init__(self) -> None:
+        self.key: Optional[tuple] = None
+        self.t: Dict[str, torch.Tensor] = {}
+        self.c = None
+
+
 class FusedEncoder:
     """nn.Module mixin of the Transformers the engine runs.  A class using it provides
         encoder_layers() -> (List[EncoderLayer], final Norm or None)
@@ -264,9 +274,7 @@ class TransformerEngine:
         # what prepared() was built from: the layers and the final LayerNorm (simple_flash_attn_vit.py has none)
         self.layers: List[EncoderLayer] = []
         self.norm: Optional[Norm] = None
-        self.ws_key: Optional[tuple] = None
-        self.ws: Dict[str, torch.Tensor] = {}
-        self.c_ws = None                       # _lib.EncoderWs over self.ws
+        self.slot = Workspace()                # may be shared with engines of the same shapes (share_workspace)
         self._vl_key: Optional[tuple] = None
         self._vl = None                        # varlen index of the fixed grid, for N > 512
 
@@ -352,16 +360,22 @@ class TransformerEngine:
             _lib.ATTN_MASK_SELF if L0.mask_self else 0
 
     # -------------------------------------------------------------------------------------------- workspaces
+    def share_workspace(self, other: "TransformerEngine") -> None:
+        """Run on `other`'s workspace from now on.  Only for encoders of identical shapes that never run at the same
+        time: the stages of one CrossViT branch (cross_vit.py:151-153), which would otherwise each hold their own."""
+        self.slot = other.slot
+
     def workspace(self, M: int, device: torch.device) -> Dict[str, torch.Tensor]:
         # one workspace per (rows, stream): two streams running the same model must not share scratch buffers.  The
         # other dimensions are the module's own and do not change.
         key = (M, device, torch.cuda.current_stream(device).cuda_stream)
-        if self.ws_key != key:
+        slot = self.slot
+        if slot.key != key:
             self.prepared()
             L = self.layers[0]
             D, I, Hd = L.qkv_w.shape[1], L.heads * L.dim_head, L.fc1_w.shape[0]
             bf = dict(device=device, dtype=torch.bfloat16)
-            self.ws = {
+            slot.t = {
                 "xn": torch.empty(M, D, **bf),          # exact: LayerNorm output; fold: bf16 copy of x
                 "qkv": torch.empty(M, 3 * I, **bf),
                 "o": torch.empty(M, I, **bf),
@@ -371,11 +385,11 @@ class TransformerEngine:
                 "stats_a": torch.empty(M, _lib.stats_parts(D), 2, device=device, dtype=torch.float32),
                 "stats_b": torch.empty(M, _lib.stats_parts(D), 2, device=device, dtype=torch.float32),
             }
-            w = self.ws
-            self.c_ws = _lib.EncoderWs(w["xn"].data_ptr(), w["qkv"].data_ptr(), w["o"].data_ptr(), w["h"].data_ptr(),
-                                       w["stats_in"].data_ptr(), w["stats_a"].data_ptr(), w["stats_b"].data_ptr())
-            self.ws_key = key
-        return self.ws
+            w = slot.t
+            slot.c = _lib.EncoderWs(w["xn"].data_ptr(), w["qkv"].data_ptr(), w["o"].data_ptr(), w["h"].data_ptr(),
+                                    w["stats_in"].data_ptr(), w["stats_a"].data_ptr(), w["stats_b"].data_ptr())
+            slot.key = key
+        return slot.t
 
     # -------------------------------------------------------------------------------------------- execution
     def _varlen_args(self, B: int, N: int, varlen: Optional[_lib.VarlenIndex], device: torch.device):
@@ -414,7 +428,7 @@ class TransformerEngine:
                 and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
             # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
             arr, (heads, dh, hidden, scale), layer_scales, flags = t["c_layers"]
-            _lib.encoder_blocks(arr, len(arr), x, self.c_ws, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl,
+            _lib.encoder_blocks(arr, len(arr), x, self.slot.c, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl,
                                 rope=rope, layer_scales=layer_scales, attn_flags=flags)
             return
         xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
@@ -650,6 +664,132 @@ class HeadEngine:
         out = torch.empty(pooled_bf16.shape[0], t["w"].shape[0], device=pooled_bf16.device, dtype=torch.bfloat16)
         _lib.gemm(pooled_bf16.contiguous(), t["w"], out_bf16=out, bias=t["b"])
         return out
+
+
+class CrossLayer(NamedTuple):
+    """One direction of one class-token cross-attention layer (CrossViT, reference cross_vit.py:94-130), as the module
+    describes it to CrossAttentionEngine: the cls row of stream A (width D_A) queries the patch rows of stream B
+    (width D_B), in B's width:
+        c    = project_in(cls_A)                                   (Identity when D_A == D_B)
+        cn   = LN(c);  q = cn Wq^T;  [k | v] = [cn; ctx_B] Wkv^T  (kv_include_self)
+        cls_A += project_out(to_out(softmax(q k^T * scale) v))"""
+    proj_in: Optional[Tuple[torch.Tensor, torch.Tensor]]       # (weight [D_B, D_A], bias) or None
+    ln: Norm
+    q_w: torch.Tensor                                           # [heads * dim_head, D_B]
+    kv_w: torch.Tensor                                          # [2 * heads * dim_head, D_B], rows k | v
+    out_w: torch.Tensor                                         # [D_B, heads * dim_head]
+    out_b: Optional[torch.Tensor]
+    proj_out: Optional[Tuple[torch.Tensor, torch.Tensor]]      # (weight [D_A, D_B], bias) or None
+    heads: int
+    dim_head: int
+    scale: float
+
+
+class CrossAttentionEngine:
+    """Fused execution of one direction of a CrossTransformer (cls of stream A attends to stream B's patch rows).
+    The owner module provides cross_layers(direction) -> List[CrossLayer] and cross_params(direction), the parameters
+    they are made of.
+
+    Per call: one GEMM of every layer's to_kv, stacked, over all rows of B's bf16 copy (the context never changes
+    inside a CrossTransformer, cross_vit.py:121-130; B's cls rows are computed and skipped).  Per layer:
+        projection:  project_in GEMM on A's cls rows (+ row statistics) -> LN-folded [to_q; to_kv] GEMM
+        Identity:    LayerNorm of A's fp32 cls rows (row_index)        -> [to_q; to_kv] GEMM
+        b200vit_attention_cls -> to_out GEMM -> project_out GEMM with the residual, in place on A's cls rows of the
+        fp32 stream and its bf16 copy (Identity: to_out carries the residual)."""
+
+    def __init__(self, owner: nn.Module, direction: int) -> None:
+        self.owner, self.direction = owner, direction
+        self.prep = _Prepared()
+        self.layers: List[CrossLayer] = []
+
+    def prepared(self) -> Dict[str, torch.Tensor]:
+        key = _version_key(self.owner.cross_params(self.direction))
+        if self.prep.key == key:
+            return self.prep.t
+        layers = self.owner.cross_layers(self.direction)
+        t: Dict[str, torch.Tensor] = {}
+        for i, L in enumerate(layers):
+            qkv_w = torch.cat([L.q_w.detach(), L.kv_w.detach()])
+            if L.proj_in is not None:
+                t[f"{i}.pin.w"], t[f"{i}.pin.b"] = _bf16_rows(L.proj_in[0]), _f32(L.proj_in[1])
+                _fold(t, f"{i}.qkv", qkv_w, None, L.ln)
+            else:
+                t[f"{i}.ln.w"], t[f"{i}.ln.b"] = _f32(L.ln.gamma), _f32(L.ln.beta)
+                t[f"{i}.qkv.w"] = _bf16_rows(qkv_w)
+            t[f"{i}.out.w"], t[f"{i}.out.b"] = _bf16_rows(L.out_w), _f32(L.out_b)
+            if L.proj_out is not None:
+                t[f"{i}.pout.w"], t[f"{i}.pout.b"] = _bf16_rows(L.proj_out[0]), _f32(L.proj_out[1])
+        t["ctx.w"] = _bf16_rows(torch.cat([L.kv_w.detach() for L in layers]))
+        self.layers = layers
+        self.prep.key, self.prep.t = key, t
+        return t
+
+    def run(self, xa: torch.Tensor, xba: torch.Tensor, Na: int, xbb: torch.Tensor, Nb: int, B: int,
+            cls_rows_a: torch.Tensor) -> None:
+        """xa fp32 [B*Na, D_A] (stream A) and xba, its bf16 copy: cls rows updated in place.  xbb bf16 [B*Nb, D_B]:
+        stream B (row 0 of every image is its cls token, not part of the context).  cls_rows_a int32 [B] = b*Na."""
+        t = self.prepared()
+        dev = xa.device
+        bf = dict(device=dev, dtype=torch.bfloat16)
+        Da = xa.shape[1]
+        ctx = torch.empty(B * Nb, t["ctx.w"].shape[0], **bf)
+        _lib.gemm(xbb, t["ctx.w"], out_bf16=ctx)
+        a_cls, ab_cls = xa.view(B, Na, Da)[:, 0], xba.view(B, Na, Da)[:, 0]      # row stride Na * D_A
+        for i, L in enumerate(self.layers):
+            I, Dc = L.heads * L.dim_head, L.q_w.shape[1]
+            qin = torch.empty(B, Dc, **bf)
+            qkv = torch.empty(B, 3 * I, **bf)
+            if L.proj_in is not None:
+                st = torch.empty(B, _lib.stats_parts(Dc), 2, device=dev, dtype=torch.float32)
+                _lib.gemm(ab_cls, t[f"{i}.pin.w"], out_bf16=qin, bias=t[f"{i}.pin.b"], stats_out=st)
+                _lib.gemm(qin, t[f"{i}.qkv.wg"], out_bf16=qkv, bias=t[f"{i}.qkv.t"], ln_sums=st,
+                          col_s=t[f"{i}.qkv.s"], ln_eps=L.ln.eps)
+            else:
+                _lib.layernorm(xa, t[f"{i}.ln.w"], t[f"{i}.ln.b"], out_bf16=qin, row_index=cls_rows_a, eps=L.ln.eps)
+                _lib.gemm(qin, t[f"{i}.qkv.w"], out_bf16=qkv)
+            o = torch.empty(B, I, **bf)
+            _lib.attention_cls(qkv, ctx[:, 2 * I * i:2 * I * (i + 1)], o, Nb, 1, Nb - 1, L.heads, L.dim_head,
+                               L.scale)
+            if L.proj_out is not None:
+                y = torch.empty(B, Dc, **bf)
+                _lib.gemm(o, t[f"{i}.out.w"], out_bf16=y, bias=t[f"{i}.out.b"])
+                _lib.gemm(y, t[f"{i}.pout.w"], out_f32=a_cls, out_bf16=ab_cls, bias=t[f"{i}.pout.b"], resid=a_cls)
+            else:
+                _lib.gemm(o, t[f"{i}.out.w"], out_f32=a_cls, out_bf16=ab_cls, bias=t[f"{i}.out.b"], resid=a_cls)
+
+
+def cls_row_index(cache: Dict[tuple, torch.Tensor], B: int, N: int, device: torch.device) -> torch.Tensor:
+    """int32 [B] = 0, N, 2N, ...: the cls rows of B images of N tokens, made once per shape so a steady-state forward
+    (and a CUDA-graph capture) issues no allocation-and-fill for it."""
+    key = (B, N, str(device))
+    if key not in cache:
+        cache[key] = torch.arange(0, B * N, N, device=device, dtype=torch.int32)
+    return cache[key]
+
+
+def fused_two_streams(stages, xs: torch.Tensor, xl: torch.Tensor, B: int, Ns: int, Nl: int, primed: bool,
+                      rows: Tuple[torch.Tensor, torch.Tensor]) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+    """CrossViT's MultiScaleEncoder (reference cross_vit.py:157-162) on two fp32 residual streams xs [B*Ns, D_sm] and
+    xl [B*Nl, D_lg].  `stages`: per multi-scale block (sm TransformerEngine, lg TransformerEngine, sm-attends-lg
+    CrossAttentionEngine, lg-attends-sm CrossAttentionEngine); the engines of one branch share one workspace, whose
+    'xn' holds that branch's bf16 copy.  Per block and branch: the encoder layers, then the Transformer's final
+    LayerNorm (cross_vit.py:90), which REPLACES the stream -- written as a new fp32 stream and its bf16 copy; the next
+    block's layers enter the folded chain from it.  Then both cross directions; they are independent (the lg->sm
+    direction reads sm patch rows and lg cls, cross_vit.py:124-126).  `primed`: the embedding already wrote the first
+    block's bf16 copies and row statistics.  `rows`: cls_row_index of either stream.
+    Returns ([x_sm, x_lg], [xb_sm, xb_lg]): the final fp32 streams and their bf16 copies."""
+    x, N = [xs, xl], (Ns, Nl)
+    spare = [torch.empty_like(xs), torch.empty_like(xl)]
+    xb: List[torch.Tensor] = [xs, xl]
+    for i, (enc_s, enc_l, sm_lg, lg_sm) in enumerate(stages):
+        for b, eng in enumerate((enc_s, enc_l)):
+            eng.run_blocks(x[b], B, N[b], primed=primed and i == 0)
+            xb[b] = eng.workspace(B * N[b], x[b].device)["xn"]
+            eng.final_norm(x[b], out_f32=spare[b], out_bf16=xb[b])
+            x[b], spare[b] = spare[b], x[b]
+        sm_lg.run(x[0], xb[0], Ns, xb[1], Nl, B, rows[0])
+        lg_sm.run(x[1], xb[1], Nl, xb[0], Ns, B, rows[1])
+    return x, xb
 
 
 def patch_engine(owner: nn.Module) -> PatchEmbedEngine:
