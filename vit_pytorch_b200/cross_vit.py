@@ -28,9 +28,9 @@ import torch
 from torch import nn
 
 from . import _lib
-from .engine import (CrossAttentionEngine, CrossLayer, FusedWeightsMixin, Norm, _bf16_rows, _f32, _has_hooks,
-                     _version_key, cls_row_index, fused_two_streams, head_width_reason, hooks_inside, ln_mode,
-                     on_device, patch_engine, why_not_fused)
+from .engine import (CrossAttentionEngine, CrossLayer, FusedWeightsMixin, Norm, _bf16_rows, _f32, _has_hooks, cached,
+                     cls_row_index, common_reason, fused_two_streams, head_width_reason, hooks_inside, on_device,
+                     patch_engine, why_not_fused)
 from .vit import FeedForward, FusedTransformer, Patchify
 
 __all__ = ["Attention", "CrossTransformer", "CrossViT", "FeedForward", "ImageEmbedder", "MultiScaleEncoder",
@@ -277,7 +277,6 @@ class ImageEmbedder(nn.Module):
         self.pos_embedding = nn.Parameter(torch.randn(1, num_patches + 1, dim))
         self.cls_token = nn.Parameter(torch.randn(1, 1, dim))
         self.dropout = nn.Dropout(dropout)
-        self._patch_engine = None
 
     def forward(self, img: torch.Tensor) -> torch.Tensor:
         x = self.to_patch_embedding(img)
@@ -337,8 +336,6 @@ class CrossViT(FusedWeightsMixin, nn.Module):
         self.lg_mlp_head = nn.Sequential(nn.LayerNorm(lg_dim), nn.Linear(lg_dim, num_classes))
 
         self._emb_dropout_p = float(emb_dropout)
-        self._heads_key: Optional[tuple] = None
-        self._heads: dict = {}
 
     # ---------------------------------------------------------------------------------------------- dispatch
     def fused_reason(self, img: torch.Tensor) -> Optional[str]:
@@ -346,10 +343,7 @@ class CrossViT(FusedWeightsMixin, nn.Module):
         if img.dim() != 4:
             return "input is not (B, C, H, W)"
         se, le, mse = self.sm_image_embedder, self.lg_image_embedder, self.multi_scale_encoder
-        p_drop = max(self._emb_dropout_p, mse.dropout_p)
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=p_drop)
-        if r is None and hooks_inside(self, skip=(mse,)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, dropout_p=max(self._emb_dropout_p, mse.dropout_p), skip=(mse,))
         for name, emb in (("sm", se), ("lg", le)):
             if r is None:
                 r = emb.fused_reason(img)
@@ -376,15 +370,10 @@ class CrossViT(FusedWeightsMixin, nn.Module):
 
     # ---------------------------------------------------------------------------------------------- fused kernels
     def _head_weights(self) -> dict:
-        params = list(self.sm_mlp_head.parameters()) + list(self.lg_mlp_head.parameters())
-        key = _version_key(params)
-        if self._heads_key != key:
-            t = {}
-            for name, head in (("sm", self.sm_mlp_head), ("lg", self.lg_mlp_head)):
-                t[name] = (_f32(head[0].weight), _f32(head[0].bias), head[0].eps, _bf16_rows(head[1].weight),
-                           _f32(head[1].bias))
-            self._heads, self._heads_key = t, key
-        return self._heads
+        heads = (("sm", self.sm_mlp_head), ("lg", self.lg_mlp_head))
+        build = lambda: {name: (_f32(h[0].weight), _f32(h[0].bias), h[0].eps, _bf16_rows(h[1].weight),   # noqa: E731
+                                _f32(h[1].bias)) for name, h in heads}
+        return cached(self, "_heads", [p for _, h in heads for p in h.parameters()], build)
 
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
         se, le, mse = self.sm_image_embedder, self.lg_image_embedder, self.multi_scale_encoder
@@ -402,13 +391,12 @@ class CrossViT(FusedWeightsMixin, nn.Module):
         else:
             stages = mse.stages()
             Ns, Nl = se.tokens(img), le.tokens(img)
-            primed = ln_mode() == "fold"
-            wss = stages[0][0].workspace(B * Ns, dev) if primed else None
-            wsl = stages[0][1].workspace(B * Nl, dev) if primed else None
-            xs, _, _ = se.embed_fused(img, xb=wss["xn"] if primed else None, stats=wss["stats_in"] if primed else None)
-            xl, _, _ = le.embed_fused(img, xb=wsl["xn"] if primed else None, stats=wsl["stats_in"] if primed else None)
+            xbs, sts = stages[0][0].entry_buffers(B * Ns, dev)
+            xbl, stl = stages[0][1].entry_buffers(B * Nl, dev)
+            xs, _, _ = se.embed_fused(img, xb=xbs, stats=sts)
+            xl, _, _ = le.embed_fused(img, xb=xbl, stats=stl)
             rows = mse.cls_rows(B, Ns, Nl, dev)
-            x, _ = fused_two_streams(stages, xs, xl, B, Ns, Nl, primed, rows)
+            x, _ = fused_two_streams(stages, xs, xl, B, Ns, Nl, xbs is not None, rows)
         heads = self._head_weights()
         nc = heads["sm"][3].shape[0]
         ncp = (nc + 7) // 8 * 8                        # residual row stride: a multiple of 4 (and of 8 for bf16)

@@ -114,6 +114,19 @@ def why_not_fused(params: List[torch.Tensor], x: torch.Tensor, *, training: bool
     return None
 
 
+def common_reason(owner: nn.Module, x: torch.Tensor, *, encoders=(), dropout_p: float = 0.0,
+                  skip: Tuple[nn.Module, ...] = (), inside: str = "model") -> Optional[str]:
+    """The part of every drop-in module's fused_reason that does not depend on its input's shape: an empty encoder in
+    `encoders`, then why_not_fused over all of `owner`'s parameters, then hooks on submodules of `owner` other than
+    `skip` (`inside` names the owner in that reason: "model" or "transformer")."""
+    if any(len(e.layers) == 0 for e in encoders):
+        return "depth == 0"
+    r = why_not_fused(list(owner.parameters()), x, training=owner.training, dropout_p=dropout_p)
+    if r is None and hooks_inside(owner, skip):
+        r = f"forward hooks registered inside the {inside}"
+    return r
+
+
 HEAD_WIDTHS = (32, 64, 80, 128)
 
 
@@ -173,11 +186,26 @@ class EncoderLayer:
 
 
 class _Prepared:
-    """Flat device buffers derived from one module's parameters + the parameter versions they were built from."""
+    """What was derived from some parameters (usually flat device buffers) + the parameter versions it was built from."""
 
     def __init__(self) -> None:
         self.key: Optional[tuple] = None
-        self.t: Dict[str, torch.Tensor] = {}
+        self.t = None
+
+    def get(self, params: List[torch.Tensor], build, *extra_key):
+        """build()'s result, rebuilt only when a version of `params` (or `extra_key`) has changed since the last call."""
+        key = _version_key(params) + extra_key
+        if self.key != key:
+            self.t, self.key = build(), key
+        return self.t
+
+
+def cached(owner, name: str, params: List[torch.Tensor], build, *extra_key):
+    """_Prepared.get on the _Prepared kept on `owner` under `name` (made on first use)."""
+    prep = owner.__dict__.get(name)
+    if prep is None:
+        prep = owner.__dict__[name] = _Prepared()
+    return prep.get(params, build, *extra_key)
 
 
 # bumped by refresh_fused_weights(): part of every prepared-weight key, so one call invalidates every engine of the
@@ -277,6 +305,7 @@ class TransformerEngine:
         self.slot = Workspace()                # may be shared with engines of the same shapes (share_workspace)
         self._vl_key: Optional[tuple] = None
         self._vl = None                        # varlen index of the fixed grid, for N > 512
+        self.rows: Dict[tuple, torch.Tensor] = {}      # cls_row_index of the shapes pool() has seen
 
     def params(self) -> List[torch.Tensor]:
         return list(self.mod.parameters())
@@ -295,10 +324,9 @@ class TransformerEngine:
 
     # -------------------------------------------------------------------------------------------- weights
     def prepared(self) -> Dict[str, torch.Tensor]:
-        params = self.params()
-        key = _version_key(params)
-        if self.prep.key == key:
-            return self.prep.t
+        return self.prep.get(self.params(), self._build)
+
+    def _build(self) -> Dict[str, torch.Tensor]:
         layers, norm = self.mod.encoder_layers()
         t: Dict[str, torch.Tensor] = {}
         for i, L in enumerate(layers):
@@ -331,7 +359,6 @@ class TransformerEngine:
             t["norm.w"], t["norm.b"] = _f32(norm.gamma), _f32(norm.beta)
         self.layers, self.norm = layers, norm
         t["c_layers"] = self._c_layers(t)            # type: ignore[assignment]
-        self.prep.key, self.prep.t = key, t
         return t
 
     def _c_layers(self, t: Dict[str, torch.Tensor]):
@@ -495,6 +522,39 @@ class TransformerEngine:
         _lib.layernorm(x, t["norm.w"], t["norm.b"], out_bf16=out_bf16, out_f32=out_f32, row_index=row_index,
                        eps=self.norm.eps)
 
+    def entry_buffers(self, M: int, device: torch.device) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """(xb, stats) an embedding kernel writes for the first layer so that run_blocks(primed=True) can skip its
+        rowstats_cast pass: the workspace's bf16 copy of x and its row sums in fold mode, (None, None) otherwise."""
+        if ln_mode() != "fold":
+            return None, None
+        ws = self.workspace(M, device)
+        return ws["xn"], ws["stats_in"]
+
+    def pool(self, x: torch.Tensor, B: int, N: int, *, mean: bool, skip: int = 0, n_pool: Optional[int] = None,
+             dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+        """After run_blocks on B sequences of N rows of x: the final LayerNorm (none if the Transformer has none), then
+        per sequence its first row (mean=False) or the mean of `n_pool` rows (default N) from row `skip` on, as a new
+        [B, D] tensor of `dtype`.  LayerNorm is per token, so first-row pooling normalises only those rows."""
+        D, dev = x.shape[1], x.device
+        out = torch.empty(B, D, device=dev, dtype=dtype)
+        if not mean:
+            rows = cls_row_index(self.rows, B, N, dev)
+            if dtype == torch.bfloat16:
+                self.final_norm(x, out_bf16=out, row_index=rows)
+            else:
+                self.final_norm(x, out_f32=out, row_index=rows)
+            return out
+        if self.norm is not None:
+            xf = torch.empty_like(x)
+            self.final_norm(x, out_f32=xf)
+        else:
+            xf = x
+        pm = out if dtype == torch.float32 else torch.empty(B, D, device=dev, dtype=torch.float32)
+        _lib.mean_pool(xf.view(-1)[skip * D:] if skip else xf, pm, B, N, D, n_pool=n_pool)
+        if pm is not out:
+            _lib.cast_f32_bf16(pm, out)
+        return out
+
     def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None,
                        axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
@@ -530,11 +590,10 @@ class PatchEmbedEngine:
         return ps
 
     def prepared(self, device: torch.device) -> Dict[str, torch.Tensor]:
+        return self.prep.get(self.params(), lambda: self._build(device), str(device))
+
+    def _build(self, device: torch.device) -> Dict[str, torch.Tensor]:
         o = self.owner
-        params = self.params()
-        key = _version_key(params) + (str(device),)
-        if self.prep.key == key:
-            return self.prep.t
         spt = getattr(o.to_patch_embedding, "to_patch_tokens", None)
         if spt is not None:
             ln1, lin, ln2 = spt[1], spt[2], None
@@ -566,7 +625,6 @@ class PatchEmbedEngine:
         t["tail"] = _f32(reg) if (reg is not None and reg.shape[0] > 0) else None
         pos = getattr(o, "pos_embedding", None)
         t["pos"] = pos.detach().to(device=device, dtype=torch.float32).contiguous() if pos is not None else None
-        self.prep.key, self.prep.t = key, t
         return t
 
     def _pos_table(self, t: Dict[str, torch.Tensor], gh: int, gw: int, device: torch.device) -> torch.Tensor:
@@ -655,12 +713,7 @@ class HeadEngine:
         return list(self.lin.parameters())
 
     def run(self, pooled_bf16: torch.Tensor) -> torch.Tensor:
-        params = self.params()
-        key = _version_key(params)
-        if self.prep.key != key:
-            self.prep.t = {"w": _bf16_rows(self.lin.weight), "b": _f32(self.lin.bias)}
-            self.prep.key = key
-        t = self.prep.t
+        t = self.prep.get(self.params(), lambda: {"w": _bf16_rows(self.lin.weight), "b": _f32(self.lin.bias)})
         out = torch.empty(pooled_bf16.shape[0], t["w"].shape[0], device=pooled_bf16.device, dtype=torch.bfloat16)
         _lib.gemm(pooled_bf16.contiguous(), t["w"], out_bf16=out, bias=t["b"])
         return out
@@ -703,9 +756,9 @@ class CrossAttentionEngine:
         self.layers: List[CrossLayer] = []
 
     def prepared(self) -> Dict[str, torch.Tensor]:
-        key = _version_key(self.owner.cross_params(self.direction))
-        if self.prep.key == key:
-            return self.prep.t
+        return self.prep.get(self.owner.cross_params(self.direction), self._build)
+
+    def _build(self) -> Dict[str, torch.Tensor]:
         layers = self.owner.cross_layers(self.direction)
         t: Dict[str, torch.Tensor] = {}
         for i, L in enumerate(layers):
@@ -721,7 +774,6 @@ class CrossAttentionEngine:
                 t[f"{i}.pout.w"], t[f"{i}.pout.b"] = _bf16_rows(L.proj_out[0]), _f32(L.proj_out[1])
         t["ctx.w"] = _bf16_rows(torch.cat([L.kv_w.detach() for L in layers]))
         self.layers = layers
-        self.prep.key, self.prep.t = key, t
         return t
 
     def run(self, xa: torch.Tensor, xba: torch.Tensor, Na: int, xbb: torch.Tensor, Nb: int, B: int,
@@ -794,9 +846,29 @@ def fused_two_streams(stages, xs: torch.Tensor, xl: torch.Tensor, B: int, Ns: in
 
 def patch_engine(owner: nn.Module) -> PatchEmbedEngine:
     """The owner's PatchEmbedEngine, made on first use."""
-    if getattr(owner, "_patch_engine", None) is None:
-        owner._patch_engine = PatchEmbedEngine(owner)
-    return owner._patch_engine
+    pe = owner.__dict__.get("_patch_engine")
+    if pe is None:
+        pe = owner._patch_engine = PatchEmbedEngine(owner)
+    return pe
+
+
+def head_engine(owner: nn.Module, linear: nn.Linear) -> HeadEngine:
+    """The owner's HeadEngine over its classifier Linear `linear`, made on first use."""
+    he = owner.__dict__.get("_head_engine")
+    if he is None:
+        he = owner._head_engine = HeadEngine(linear)
+    return he
+
+
+def classify(owner: nn.Module, linear: nn.Linear, pooled: torch.Tensor) -> torch.Tensor:
+    """Logits of bf16 pooled features: owner.to_latent(pooled), which stays a called module (Dino / LeJEPA hook it),
+    then the head GEMM of `linear`."""
+    return head_engine(owner, linear).run(owner.to_latent(pooled))
+
+
+def head_norm(owner: nn.Module, ln: nn.LayerNorm) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """fp32 (weight, bias) of the LayerNorm of the owner's head, cached by parameter version."""
+    return cached(owner, "_head_norm", list(ln.parameters()), lambda: (_f32(ln.weight), _f32(ln.bias)))
 
 
 def fused_encode(owner: nn.Module, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None,
@@ -806,35 +878,27 @@ def fused_encode(owner: nn.Module, img: torch.Tensor, patch: Optional[Tuple[int,
     engine's bf16 copy of x and its row statistics, which the first layer reads.  Must run inside on_device(img)."""
     pe, eng = patch_engine(owner), owner.transformer.engine()
     B, N = pe.geometry(img, patch)
-    primed = ln_mode() == "fold"
-    ws = eng.workspace(B * N, img.device) if primed else None
-    x, B, N = pe.run(img, xb=ws["xn"] if primed else None, stats=ws["stats_in"] if primed else None,
-                     patch=patch, pos=pos)
-    eng.run_blocks(x, B, N, primed=primed)
+    xb, stats = eng.entry_buffers(B * N, img.device)
+    x, B, N = pe.run(img, xb=xb, stats=stats, patch=patch, pos=pos)
+    eng.run_blocks(x, B, N, primed=xb is not None)
     return x, B, N
 
 
 def fused_mean_pooled_features(owner: nn.Module, img: torch.Tensor, pool_tokens: Optional[int] = None,
-                               patch: Optional[Tuple[int, int]] = None,
-                               pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+                               patch: Optional[Tuple[int, int]] = None, pos: Optional[torch.Tensor] = None
+                               ) -> Tuple[torch.Tensor, torch.Tensor]:
     """Shared body of the SimpleViT-family fused forwards (reference simple_vit.py:110-117 and its variants):
     patch embedding (+ register tokens) -> encoder blocks -> final LayerNorm if the Transformer has one -> mean over
-    the first `pool_tokens` tokens of every image (all tokens by default).  Returns fp32 [B, D]; must run inside
-    on_device(img)."""
+    the first `pool_tokens` tokens of every image (all tokens by default).  Returns that mean as fp32 and as bf16,
+    [B, D] each; must run inside on_device(img)."""
     if transformer_is_hooked(owner):
         x, B, N = patch_engine(owner).run(img, patch=patch, pos=pos)
         xf = hooked_transformer_tokens(owner, x, B, N).reshape(B * N, -1).float()
         pm = torch.empty(B, xf.shape[1], device=img.device, dtype=torch.float32)
         _lib.mean_pool(xf, pm, B, N, xf.shape[1], n_pool=pool_tokens)
-        return pm
-    x, B, N = fused_encode(owner, img, patch=patch, pos=pos)
-    D = x.shape[1]
-    eng = owner.transformer.engine()
-    if eng.norm is not None:
-        xf = torch.empty_like(x)
-        eng.final_norm(x, out_f32=xf)
     else:
-        xf = x
-    pm = torch.empty(B, D, device=img.device, dtype=torch.float32)
-    _lib.mean_pool(xf, pm, B, N, D, n_pool=pool_tokens)
-    return pm
+        x, B, N = fused_encode(owner, img, patch=patch, pos=pos)
+        pm = owner.transformer.engine().pool(x, B, N, mean=True, n_pool=pool_tokens, dtype=torch.float32)
+    pooled = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
+    _lib.cast_f32_bf16(pm, pooled)
+    return pm, pooled

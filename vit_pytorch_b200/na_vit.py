@@ -25,8 +25,8 @@ import torch.nn.functional as F
 from torch import Tensor, nn
 
 from . import _lib
-from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, head_width_reason,
-                     hooks_inside, ln_mode, on_device, why_not_fused)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _bf16_rows, _f32, cached, head_width_reason,
+                     hooks_inside, on_device, why_not_fused)
 
 
 def group_images_by_max_seq_len(images: Sequence[Tensor], patch_size: int,
@@ -222,37 +222,32 @@ class NaViT(FusedWeightsMixin, nn.Module):
         """The `beta` buffers are part of the state_dict; the fused path assumes the zeros the reference registers
         (checked once per buffer version, not per forward: the check synchronises)."""
         betas = [b for n, b in self.named_buffers() if n.endswith("beta")]
-        key = _version_key(betas)
-        if getattr(self, "_beta_key", None) != key:
-            self._beta_key, self._beta_nonzero = key, any(bool(b.any()) for b in betas)
-        return self._beta_nonzero
+        return cached(self, "_beta_nonzero", betas, lambda: any(bool(b.any()) for b in betas))
 
     def _prepared(self) -> Dict[str, Tensor]:
         """Device copies of the patch-embedding, positional, pooling and head weights (the encoder layers are the
         transformer engine's)."""
-        params = [p for n, p in self.named_parameters() if not n.startswith("transformer.")]
-        key = _version_key(params)
-        if getattr(self, "_prep_key", None) == key:
-            return self._prep
-        f32 = lambda t: t.detach().float().contiguous()
-        bf = lambda t: t.detach().to(torch.bfloat16).contiguous()
+        return cached(self, "_prep", [p for n, p in self.named_parameters() if not n.startswith("transformer.")],
+                      self._build)
+
+    def _build(self) -> Dict[str, Tensor]:
         t: Dict[str, Tensor] = {}
         pe = self.to_patch_embedding
-        t["pe.ln1"], t["pe.w"], t["pe.b"], t["pe.ln2"] = f32(pe[0].gamma), bf(pe[1].weight), f32(pe[1].bias), f32(pe[2].gamma)
-        t["pos_h"], t["pos_w"] = f32(self.pos_embed_height), f32(self.pos_embed_width)
+        t["pe.ln1"], t["pe.w"], t["pe.b"] = _f32(pe[0].gamma), _bf16_rows(pe[1].weight), _f32(pe[1].bias)
+        t["pe.ln2"] = _f32(pe[2].gamma)
+        t["pos_h"], t["pos_w"] = _f32(self.pos_embed_height), _f32(self.pos_embed_width)
         # the pooling query is the same for every image: LayerNorm -> to_q -> per-head RMSNorm, once per weight version
         pool = self.attn_pool
-        t["pool.kv"] = bf(pool.to_kv.weight)
-        t["pool.gk"] = f32(pool.k_norm.gamma).reshape(-1).contiguous()
-        t["pool.out"] = bf(pool.to_out[0].weight)
+        t["pool.kv"] = _bf16_rows(pool.to_kv.weight)
+        t["pool.gk"] = _f32(pool.k_norm.gamma).reshape(-1).contiguous()
+        t["pool.out"] = _bf16_rows(pool.to_out[0].weight)
         qv = self.attn_pool_queries.detach().float()
         qn = F.layer_norm(qv, qv.shape, pool.norm.gamma.detach().float(), None)
         qh = (pool.to_q.weight.detach().float() @ qn).reshape(pool.heads, -1)
         qh = F.normalize(qh, dim=-1) * pool.q_norm.scale * pool.q_norm.gamma.detach().float().reshape(pool.heads, -1)
         t["pool.qn"] = qh.reshape(-1).contiguous()
         t["pool.queries"] = qv.contiguous()
-        t["head.ln"], t["head.w"] = f32(self.mlp_head[0].gamma), bf(self.mlp_head[1].weight)
-        self._prep_key, self._prep = key, t
+        t["head.ln"], t["head.w"] = _f32(self.mlp_head[0].gamma), _bf16_rows(self.mlp_head[1].weight)
         return t
 
     @torch.no_grad()
@@ -284,7 +279,6 @@ class NaViT(FusedWeightsMixin, nn.Module):
         S, T = ix.S, ix.T
         bf16 = dict(device=dev, dtype=torch.bfloat16)
         f32 = dict(device=dev, dtype=torch.float32)
-        fold = ln_mode() == "fold"
         # ---- patch embedding: patchify + LN(no bias) -> Linear -> LN(no bias) + pos_h + pos_w   (na_vit.py:300,350-359)
         pd = c * p * p
         a0 = torch.empty(T, pd, **bf16)
@@ -292,12 +286,11 @@ class NaViT(FusedWeightsMixin, nn.Module):
         y = torch.empty(T, D, **f32)
         _lib.gemm(a0, t["pe.w"], out_f32=y, bias=t["pe.b"])
         x = torch.empty_like(y)
-        ws = eng.workspace(T, dev)     # fold: the embedding writes the bf16 copy of x and its row sums for layer 0
-        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=ws["xn"] if fold else None,
-                          stats=ws["stats_in"] if fold else None)
+        xb, stats = eng.entry_buffers(T, dev)
+        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=xb, stats=stats)
         # ---- encoder layers on the packed [T, D] matrix                                     (na_vit.py:183-193)
-        eng.run_blocks(x, primed=fold, varlen=ix)
-        xn = ws["xn"]
+        eng.run_blocks(x, primed=xb is not None, varlen=ix)
+        xn = eng.workspace(T, dev)["xn"]
         eng.final_norm(x, out_bf16=xn)
         # ---- attention pooling: one query per image over that image's (un-normalised-again) tokens (na_vit.py:371-387)
         kv = torch.empty(T, 2 * I, **bf16)

@@ -24,8 +24,8 @@ import torch.nn.functional as F
 from torch import Tensor, nn
 
 from . import _lib
-from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _version_key, head_width_reason,
-                     hooks_inside, ln_mode, on_device, why_not_fused)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _bf16_rows, _f32, cached, head_width_reason,
+                     hooks_inside, on_device, why_not_fused)
 
 
 def FeedForward(dim: int, hidden_dim: int, dropout: float = 0.) -> nn.Sequential:
@@ -198,26 +198,24 @@ class NaViT(FusedWeightsMixin, nn.Module):
     def _prepared(self) -> Dict[str, Tensor]:
         """Device copies of the patch-embedding, positional, pooling and head weights (the encoder layers are the
         transformer engine's)."""
-        params = [p for n, p in self.named_parameters() if not n.startswith("transformer.")]
-        key = _version_key(params)
-        if getattr(self, "_prep_key", None) == key:
-            return self._prep
-        f32 = lambda t: t.detach().float().contiguous()
-        bf = lambda t: t.detach().to(torch.bfloat16).contiguous()
+        return cached(self, "_prep", [p for n, p in self.named_parameters() if not n.startswith("transformer.")],
+                      self._build)
+
+    def _build(self) -> Dict[str, Tensor]:
         t: Dict[str, Tensor] = {}
         ln1, lin, ln2 = self.to_patch_embedding
         # LN(x; g1, b1) W^T + c == (x_hat g1) W^T + (W b1 + c): beta_1 moves into the projection's bias
-        t["pe.ln1"], t["pe.w"] = f32(ln1.weight), bf(lin.weight)
+        t["pe.ln1"], t["pe.w"] = _f32(ln1.weight), _bf16_rows(lin.weight)
         t["pe.b"] = (lin.weight.detach().float() @ ln1.bias.detach().float() + lin.bias.detach().float()).contiguous()
         # LN(y; g2, b2) + pos_h + pos_w == y_hat g2 + (pos_h + b2) + pos_w: beta_2 moves into the height table
-        t["pe.ln2"] = f32(ln2.weight)
+        t["pe.ln2"] = _f32(ln2.weight)
         t["pos_h"] = (self.pos_embed_height.detach().float() + ln2.bias.detach().float()[None, :]).contiguous()
-        t["pos_w"] = f32(self.pos_embed_width)
+        t["pos_w"] = _f32(self.pos_embed_width)
         pool = self.attn_pool
-        t["pool.kv"] = bf(torch.cat([pool.to_keys.weight, pool.to_values.weight], dim=0))
+        t["pool.kv"] = _bf16_rows(torch.cat([pool.to_keys.weight, pool.to_values.weight], dim=0))
         t["pool.gk"] = (None if isinstance(pool.key_norm, nn.Identity)
-                        else f32(pool.key_norm.weight).repeat(pool.heads).contiguous())    # same gamma for every head
-        t["pool.out"] = bf(pool.to_out.weight)
+                        else _f32(pool.key_norm.weight).repeat(pool.heads).contiguous())    # same gamma for every head
+        t["pool.out"] = _bf16_rows(pool.to_out.weight)
         # the pooling query is the same for every image: LayerNorm -> to_queries -> per-head LayerNorm, times the
         # softmax scale dim_head ** -0.5 (the pooling kernel uses scale 1)
         qv = self.attn_pool_queries.detach().float()
@@ -226,8 +224,7 @@ class NaViT(FusedWeightsMixin, nn.Module):
         if not isinstance(pool.query_norm, nn.Identity):
             qh = F.layer_norm(qh, qh.shape[-1:], pool.query_norm.weight.detach().float(), None, pool.query_norm.eps)
         t["pool.qn"] = (qh * pool.dim_head ** -0.5).reshape(-1).contiguous()
-        t["head.ln"], t["head.w"] = f32(self.mlp_head[0].weight), bf(self.mlp_head[1].weight)
-        self._prep_key, self._prep = key, t
+        t["head.ln"], t["head.w"] = _f32(self.mlp_head[0].weight), _bf16_rows(self.mlp_head[1].weight)
         return t
 
     @torch.no_grad()
@@ -254,19 +251,18 @@ class NaViT(FusedWeightsMixin, nn.Module):
         S, T = ix.S, ix.T
         bf16 = dict(device=dev, dtype=torch.bfloat16)
         f32 = dict(device=dev, dtype=torch.float32)
-        fold = ln_mode() == "fold"
         # ---- patch embedding (reference :186-192,226-262)
         a0 = torch.empty(T, c * p * p, **bf16)
         _lib.patchify_varlen_ln(images, t["pe.ln1"], a0, ix.cu, p, eps=self.to_patch_embedding[0].eps, index=ix)
         y = torch.empty(T, D, **f32)
         _lib.gemm(a0, t["pe.w"], out_f32=y, bias=t["pe.b"])
         x = torch.empty_like(y)
-        ws = eng.workspace(T, dev)     # fold: the embedding writes the bf16 copy of x and its row sums for layer 0
-        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=ws["xn"] if fold else None,
-                          stats=ws["stats_in"] if fold else None, eps=self.to_patch_embedding[2].eps)
+        xb, stats = eng.entry_buffers(T, dev)
+        _lib.embed_varlen(y, t["pe.ln2"], t["pos_h"], t["pos_w"], ix, x, p, xb=xb, stats=stats,
+                          eps=self.to_patch_embedding[2].eps)
         # ---- encoder layers on the packed [T, D] matrix (reference :121-132)
-        eng.run_blocks(x, primed=fold, varlen=ix)
-        xn = ws["xn"]
+        eng.run_blocks(x, primed=xb is not None, varlen=ix)
+        xn = eng.workspace(T, dev)["xn"]
         eng.final_norm(x, out_bf16=xn)
         # ---- attention pooling, one query per image, no residual (reference :284-296)
         kv = torch.empty(T, 2 * I, **bf16)

@@ -15,7 +15,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib
-from .engine import FusedWeightsMixin, HeadEngine, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
+from .engine import FusedWeightsMixin, common_reason, fused_mean_pooled_features, head_engine, head_norm, on_device
 from .simple_vit import FeedForward, posemb_sincos_2d
 from .simple_vit_with_patch_dropout import GridPatchify
 from .vit import FusedTransformer, pair
@@ -84,8 +84,6 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         self.to_latent = nn.Identity()
         self.linear_head = nn.Sequential(nn.LayerNorm(dim), nn.Linear(dim, num_classes))
         self._dim = dim
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
 
     def fused_pos_table(self, gh: int, gw: int) -> torch.Tensor:
         return posemb_sincos_2d(gh, gw, self._dim)
@@ -95,11 +93,7 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
             return "input is not (B, C, H, W)"
         if img.shape[1] * self.patch_size[0] * self.patch_size[1] != self.to_patch_embedding[1].normalized_shape[0]:
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, encoders=(self.transformer,), skip=(self.to_latent, self.transformer))
         if r is None:
             ph, pw = self.patch_size
             if img.shape[2] % ph or img.shape[3] % pw:
@@ -121,16 +115,11 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         return self.linear_head(self.to_latent(x))
 
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
-        pm = fused_mean_pooled_features(self, img)              # fp32 mean of the un-normalised tokens
-        pooled = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
+        pm, pooled = fused_mean_pooled_features(self, img)      # mean of the un-normalised tokens
         lat = self.to_latent(pooled)
         if lat is not pooled:
             pm = lat.float().contiguous()
         ln, lin = self.linear_head[0], self.linear_head[1]
         normed = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
-        _lib.layernorm(pm, ln.weight.detach().float().contiguous(), ln.bias.detach().float().contiguous(),
-                       out_bf16=normed, eps=ln.eps)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(lin)
-        return self._head_engine.run(normed)
+        _lib.layernorm(pm, *head_norm(self, ln), out_bf16=normed, eps=ln.eps)
+        return head_engine(self, lin).run(normed)

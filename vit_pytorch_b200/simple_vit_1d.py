@@ -14,8 +14,7 @@ from typing import Dict, Optional, Tuple
 import torch
 from torch import nn
 
-from . import _lib
-from .engine import FusedWeightsMixin, HeadEngine, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
+from .engine import FusedWeightsMixin, classify, common_reason, fused_mean_pooled_features, on_device
 from .simple_vit import Attention, FeedForward, Transformer  # noqa: F401  (same block classes, reference :23-76)
 
 
@@ -63,8 +62,6 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         self.linear_head = nn.Linear(dim, num_classes)
         self.fused_patch_box: Tuple[int, int] = (1, patch_size)
         self._channels = channels
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
         self._pos_cache: Dict[Tuple[int, str], torch.Tensor] = {}
 
     def fused_reason(self, series: torch.Tensor) -> Optional[str]:
@@ -75,11 +72,7 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
         if series.shape[2] % p or series.shape[2] == 0:
             return "series length not divisible by the patch size"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), series, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, series, encoders=(self.transformer,), skip=(self.to_latent, self.transformer))
         if r is None:
             r = self.transformer.engine().unsupported_reason(series.shape[2] // p)
         return r
@@ -104,11 +97,6 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         key = (n, str(series.device))
         if key not in self._pos_cache:
             self._pos_cache[key] = sincos_table_1d(n, dim, device=series.device).contiguous()
-        pm = fused_mean_pooled_features(self, series.contiguous().view(b, c, 1, length), patch=self.fused_patch_box,
-                                        pos=self._pos_cache[key])
-        pooled = torch.empty(pm.shape, device=series.device, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.linear_head)
-        return self._head_engine.run(pooled)
+        _, pooled = fused_mean_pooled_features(self, series.contiguous().view(b, c, 1, length),
+                                               patch=self.fused_patch_box, pos=self._pos_cache[key])
+        return classify(self, self.linear_head, pooled)

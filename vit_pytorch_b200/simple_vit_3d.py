@@ -17,8 +17,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import _lib
-from .engine import FusedWeightsMixin, HeadEngine, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
+from .engine import FusedWeightsMixin, classify, common_reason, fused_mean_pooled_features, on_device
 from .simple_vit import Attention, FeedForward, Transformer  # noqa: F401  (same block classes, reference :36-88)
 from .vit import pair
 
@@ -79,8 +78,6 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         self.fused_patch_box: Tuple[int, int] = (frame_patch_size * patch_height, patch_width)
         self._pf = frame_patch_size
         self._channels = channels
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
         self._pos_cache: Dict[Tuple[int, int, int, str], torch.Tensor] = {}
 
     def _grid(self, video: torch.Tensor) -> Tuple[int, int, int]:
@@ -93,11 +90,7 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
         if video.shape[2] % self._pf or video.shape[3] % self.patch_size[0] or video.shape[4] % self.patch_size[1]:
             return "video not divisible by the patch box"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), video, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, video, encoders=(self.transformer,), skip=(self.to_latent, self.transformer))
         if r is None:
             f, h, w = self._grid(video)
             if f * h * w == 0:
@@ -134,10 +127,5 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         key = (f, h, w, str(video.device))
         if key not in self._pos_cache:
             self._pos_cache[key] = sincos_table_3d(f, h, w, dim, device=video.device).contiguous()
-        pm = fused_mean_pooled_features(self, img, patch=self.fused_patch_box, pos=self._pos_cache[key])
-        pooled = torch.empty(pm.shape, device=video.device, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.linear_head)
-        return self._head_engine.run(pooled)
+        _, pooled = fused_mean_pooled_features(self, img, patch=self.fused_patch_box, pos=self._pos_cache[key])
+        return classify(self, self.linear_head, pooled)

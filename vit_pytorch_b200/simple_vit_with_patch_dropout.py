@@ -14,8 +14,7 @@ from typing import Optional
 import torch
 from torch import nn
 
-from . import _lib
-from .engine import FusedWeightsMixin, HeadEngine, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
+from .engine import FusedWeightsMixin, classify, common_reason, fused_mean_pooled_features, on_device
 from .simple_vit import Transformer, posemb_sincos_2d
 from .vit import Patchify, pair
 
@@ -64,8 +63,6 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         self.to_latent = nn.Identity()
         self.linear_head = nn.Linear(dim, num_classes)
         self._dim = dim
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
 
     def fused_pos_table(self, gh: int, gw: int) -> torch.Tensor:
         return posemb_sincos_2d(gh, gw, self._dim)
@@ -79,9 +76,7 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
             return "depth == 0"
         if self.training and self.patch_dropout.prob > 0.:
             return "patch dropout is active (training)"
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, skip=(self.to_latent, self.transformer))
         if r is None:
             ph, pw = self.patch_size
             if img.shape[2] % ph or img.shape[3] % pw:
@@ -105,10 +100,5 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         return self.linear_head(self.to_latent(x))
 
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
-        pm = fused_mean_pooled_features(self, img)
-        pooled = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.linear_head)
-        return self._head_engine.run(pooled)
+        _, pooled = fused_mean_pooled_features(self, img)
+        return classify(self, self.linear_head, pooled)

@@ -17,7 +17,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib
-from .engine import FusedWeightsMixin, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
+from .engine import FusedWeightsMixin, common_reason, fused_mean_pooled_features, head_norm, on_device
 from .simple_vit import FeedForward, posemb_sincos_2d
 from .vit import FusedTransformer, Patchify, pair
 
@@ -84,18 +84,13 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         self.pool = "mean"
         self.to_latent = nn.Identity()
         self.linear_head = nn.LayerNorm(dim)          # sic (reference :128): features, not logits
-        self._patch_engine = None
 
     def fused_reason(self, img: torch.Tensor) -> Optional[str]:
         if img.dim() != 4:
             return "input is not (B, C, H, W)"
         if img.shape[1] * self.patch_size[0] * self.patch_size[1] != self.to_patch_embedding[1].normalized_shape[0]:
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, encoders=(self.transformer,), skip=(self.to_latent, self.transformer))
         if r is None:
             ph, pw = self.patch_size
             if img.shape[2] % ph or img.shape[3] % pw:
@@ -119,14 +114,10 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         return self.linear_head(self.to_latent(x))
 
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
-        pm = fused_mean_pooled_features(self, img)
-        pooled = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
+        pm, pooled = fused_mean_pooled_features(self, img)
         lat = self.to_latent(pooled)                  # stays a called module (Dino / LeJEPA hook it)
         if lat is not pooled:
             pm = lat.float().contiguous()
         out = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
-        h = self.linear_head
-        _lib.layernorm(pm, h.weight.detach().float().contiguous(), h.bias.detach().float().contiguous(),
-                       out_bf16=out, eps=h.eps)
+        _lib.layernorm(pm, *head_norm(self, self.linear_head), out_bf16=out, eps=self.linear_head.eps)
         return out

@@ -14,8 +14,7 @@ from typing import Optional
 import torch
 from torch import nn
 
-from . import _lib
-from .engine import FusedWeightsMixin, HeadEngine, fused_mean_pooled_features, hooks_inside, on_device, why_not_fused
+from .engine import FusedWeightsMixin, classify, common_reason, fused_mean_pooled_features, on_device
 from .simple_vit import Attention, FeedForward, Transformer, posemb_sincos_2d  # noqa: F401  (same block classes)
 from .vit import Patchify, pair
 
@@ -41,19 +40,13 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
         self.pool = "mean"
         self.to_latent = nn.Identity()
         self.linear_head = nn.Linear(dim, num_classes)
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
 
     def fused_reason(self, img: torch.Tensor) -> Optional[str]:
         if img.dim() != 4:
             return "input is not (B, C, H, W)"
         if img.shape[1] * self.patch_size[0] * self.patch_size[1] != self.to_patch_embedding[1].normalized_shape[0]:
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=0.0)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, encoders=(self.transformer,), skip=(self.to_latent, self.transformer))
         if r is None:
             ph, pw = self.patch_size
             if img.shape[2] % ph or img.shape[3] % pw:
@@ -81,10 +74,5 @@ class SimpleViT(FusedWeightsMixin, nn.Module):
 
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
         n = self.pos_embedding.shape[0]
-        pm = fused_mean_pooled_features(self, img, pool_tokens=n)     # mean over the patch tokens only
-        pooled = torch.empty(pm.shape, device=img.device, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.linear_head)
-        return self._head_engine.run(pooled)
+        _, pooled = fused_mean_pooled_features(self, img, pool_tokens=n)     # mean over the patch tokens only
+        return classify(self, self.linear_head, pooled)

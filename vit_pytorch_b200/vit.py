@@ -19,10 +19,8 @@ from typing import List, Optional, Tuple
 import torch
 from torch import nn
 
-from . import _lib
-from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, HeadEngine, Norm, PatchEmbedEngine, fused_encode,
-                     hooked_transformer_tokens, hooks_inside, on_device, patch_engine, transformer_is_hooked,
-                     why_not_fused)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, classify, common_reason, fused_encode,
+                     hooked_transformer_tokens, on_device, patch_engine, transformer_is_hooked)
 
 
 def pair(t):
@@ -129,11 +127,7 @@ class FusedTransformer(FusedEncoder, FusedWeightsMixin, nn.Module):
 
     def fused_reason(self, x: torch.Tensor) -> Optional[str]:
         """None if forward(x) will run the fused kernels, else why not."""
-        if len(self.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), x, training=self.training, dropout_p=self.dropout_p)
-        if r is None and hooks_inside(self):
-            r = "forward hooks registered inside the transformer"
+        r = common_reason(self, x, encoders=(self,), dropout_p=self.dropout_p, inside="transformer")
         if r is None and x.dim() != 3:
             r = "input is not (B, N, D)"
         if r is None:
@@ -194,8 +188,6 @@ class ViT(FusedWeightsMixin, nn.Module):
         self.mlp_head = nn.Linear(dim, num_classes) if num_classes > 0 else None
 
         self._emb_dropout_p = float(emb_dropout)
-        self._patch_engine: Optional[PatchEmbedEngine] = None
-        self._head_engine: Optional[HeadEngine] = None
 
     # ---------------------------------------------------------------------------------------------- dispatch
     def fused_reason(self, img: torch.Tensor) -> Optional[str]:
@@ -204,12 +196,9 @@ class ViT(FusedWeightsMixin, nn.Module):
             return "input is not (B, C, H, W)"
         if img.shape[1] * self.patch_size[0] * self.patch_size[1] != self.to_patch_embedding[1].normalized_shape[0]:
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        p_drop = max(self._emb_dropout_p, self.transformer.dropout_p)
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=p_drop)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, encoders=(self.transformer,),
+                          dropout_p=max(self._emb_dropout_p, self.transformer.dropout_p),
+                          skip=(self.to_latent, self.transformer))
         if r is None:
             ph, pw = self.patch_size
             if img.shape[2] % ph or img.shape[3] % pw:
@@ -244,29 +233,12 @@ class ViT(FusedWeightsMixin, nn.Module):
             if self.mlp_head is None:
                 return out
             pooled = (out.mean(dim=1) if self.pool == 'mean' else out[:, 0]).contiguous()
-            pooled = self.to_latent(pooled)
-            if self._head_engine is None:
-                self._head_engine = HeadEngine(self.mlp_head)
-            return self._head_engine.run(pooled)
+            return classify(self, self.mlp_head, pooled)
         x, B, N = fused_encode(self, img)              # fp32 residual stream [B*N, D]
         D = x.shape[1]
         eng = self.transformer.engine()
-        dev = img.device
         if self.mlp_head is None:                      # reference vit.py:132-133: return the normalised tokens
-            out = torch.empty(B * N, D, device=dev, dtype=torch.bfloat16)
+            out = torch.empty(B * N, D, device=img.device, dtype=torch.bfloat16)
             eng.final_norm(x, out_bf16=out)
             return out.view(B, N, D)
-        pooled = torch.empty(B, D, device=dev, dtype=torch.bfloat16)
-        if self.pool == 'mean':
-            xf = torch.empty_like(x)
-            eng.final_norm(x, out_f32=xf)
-            pm = torch.empty(B, D, device=dev, dtype=torch.float32)
-            _lib.mean_pool(xf, pm, B, N, D)
-            _lib.cast_f32_bf16(pm, pooled)
-        else:                                          # LayerNorm is per token: normalise only the cls rows
-            rows = torch.arange(0, B * N, N, device=dev, dtype=torch.int32)
-            eng.final_norm(x, out_bf16=pooled, row_index=rows)
-        pooled = self.to_latent(pooled)                # stays a called module: Dino / LeJEPA hook it
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.mlp_head)
-        return self._head_engine.run(pooled)
+        return classify(self, self.mlp_head, eng.pool(x, B, N, mean=self.pool == 'mean'))

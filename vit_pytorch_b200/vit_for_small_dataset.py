@@ -27,9 +27,8 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib
-from .engine import (EncoderLayer, FusedWeightsMixin, HeadEngine, Norm, _f32, _version_key, fused_encode,
-                     hooked_transformer_tokens, hooks_inside, on_device, patch_engine, transformer_is_hooked,
-                     why_not_fused)
+from .engine import (EncoderLayer, FusedWeightsMixin, Norm, classify, cls_row_index, common_reason, fused_encode,
+                     head_norm, hooked_transformer_tokens, on_device, patch_engine, transformer_is_hooked)
 from .vit import FeedForward, FusedTransformer, Patchify, pair
 
 __all__ = ["FeedForward", "LSA", "Transformer", "SPT", "ViT"]
@@ -135,10 +134,6 @@ class ViT(FusedWeightsMixin, nn.Module):
         self.mlp_head = nn.Sequential(nn.LayerNorm(dim), nn.Linear(dim, num_classes))
 
         self._emb_dropout_p = float(emb_dropout)
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
-        self._head_norm_key: Optional[tuple] = None     # fp32 copies of mlp_head[0]'s affine parameters
-        self._head_norm: Optional[Tuple[torch.Tensor, Optional[torch.Tensor]]] = None
 
     # ---------------------------------------------------------------------------------------------- dispatch
     def fused_reason(self, img: torch.Tensor) -> Optional[str]:
@@ -148,12 +143,9 @@ class ViT(FusedWeightsMixin, nn.Module):
         ph, pw = self.patch_size
         if img.shape[1] * 5 * ph * pw != self.to_patch_embedding.to_patch_tokens[1].normalized_shape[0]:
             return "channel count differs from the constructor's (the reference's LayerNorm raises)"
-        if len(self.transformer.layers) == 0:
-            return "depth == 0"
-        p_drop = max(self._emb_dropout_p, self.transformer.dropout_p)
-        r = why_not_fused(list(self.parameters()), img, training=self.training, dropout_p=p_drop)
-        if r is None and hooks_inside(self, skip=(self.to_latent, self.transformer)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, img, encoders=(self.transformer,),
+                          dropout_p=max(self._emb_dropout_p, self.transformer.dropout_p),
+                          skip=(self.to_latent, self.transformer))
         if r is not None:
             return r
         if img.shape[2] % ph or img.shape[3] % pw:
@@ -187,18 +179,11 @@ class ViT(FusedWeightsMixin, nn.Module):
         return self.mlp_head(x)
 
     # ---------------------------------------------------------------------------------------------- fused kernels
-    def _head_ln(self) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-        ln = self.mlp_head[0]
-        key = _version_key(list(ln.parameters()))
-        if self._head_norm_key != key:
-            self._head_norm, self._head_norm_key = (_f32(ln.weight), _f32(ln.bias)), key
-        return self._head_norm
-
     def _pool(self, x: torch.Tensor, B: int, N: int) -> torch.Tensor:
         """x fp32 [B*N, D] encoder output -> mlp_head[0](x[:, 0]) or mlp_head[0](x.mean(1)), bf16 [B, D]."""
         D = x.shape[1]
         dev = x.device
-        g, b = self._head_ln()
+        g, b = head_norm(self, self.mlp_head[0])
         eps = self.mlp_head[0].eps
         pooled = torch.empty(B, D, device=dev, dtype=torch.bfloat16)
         if self.pool == 'mean':
@@ -206,7 +191,7 @@ class ViT(FusedWeightsMixin, nn.Module):
             _lib.mean_pool(x, pm, B, N, D)
             _lib.layernorm(pm, g, b, out_bf16=pooled, eps=eps)
         else:                                          # LayerNorm is per token: normalise only the cls rows
-            rows = torch.arange(0, B * N, N, device=dev, dtype=torch.int32)
+            rows = cls_row_index(self.transformer.engine().rows, B, N, dev)
             _lib.layernorm(x, g, b, out_bf16=pooled, row_index=rows, eps=eps)
         return pooled
 
@@ -219,7 +204,4 @@ class ViT(FusedWeightsMixin, nn.Module):
             x = out.reshape(B * N, D).float().contiguous()
         else:
             x, B, N = fused_encode(self, img, pos=pos)  # fp32 residual stream [B*N, D]
-        pooled = self.to_latent(self._pool(x, B, N))   # stays a called module, as in vit.ViT
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.mlp_head[1])
-        return self._head_engine.run(pooled)
+        return classify(self, self.mlp_head[1], self._pool(x, B, N))

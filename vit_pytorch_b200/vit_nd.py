@@ -20,8 +20,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from .engine import (FusedWeightsMixin, HeadEngine, _Prepared, _bf16_rows, _f32, _version_key, hooks_inside, ln_mode,
-                     on_device, why_not_fused)
+from .engine import FusedWeightsMixin, _Prepared, _bf16_rows, _f32, classify, common_reason, on_device
 from .vit import Transformer
 
 MAX_FUSED_PATCH_DIM = 16384      # b200vit_patchify_nd stages at least one whole patch in shared memory
@@ -81,19 +80,17 @@ class NdPatchEngine:
         return ps
 
     def prepared(self, device: torch.device) -> dict:
-        key = _version_key(self.params()) + (str(device),)
-        if self.prep.key == key:
-            return self.prep.t
+        return self.prep.get(self.params(), self._build, str(device))
+
+    def _build(self) -> dict:
         o = self.owner
         lin, ln = o.to_patch_embedding[1], o.to_patch_embedding[2]
         D, pd = lin.weight.shape
         cls, pos = getattr(o, "cls_token", None), getattr(o, "pos_embedding", None)
-        t = {"w": _bf16_rows(lin.weight, (pd + 63) // 64 * 64), "b": _f32(lin.bias),
-             "ln.w": _f32(ln.weight), "ln.b": _f32(ln.bias),
-             "cls": None if cls is None else _f32(cls.reshape(-1, D)),
-             "pos": None if pos is None else _f32(pos.reshape(-1, D))}
-        self.prep.key, self.prep.t = key, t
-        return t
+        return {"w": _bf16_rows(lin.weight, (pd + 63) // 64 * 64), "b": _f32(lin.bias),
+                "ln.w": _f32(ln.weight), "ln.b": _f32(ln.bias),
+                "cls": None if cls is None else _f32(cls.reshape(-1, D)),
+                "pos": None if pos is None else _f32(pos.reshape(-1, D))}
 
     def tokens(self, img: torch.Tensor) -> Tuple[int, int]:
         """(patches per input, tokens per input)."""
@@ -130,11 +127,7 @@ def nd_fused_reason(owner: nn.Module, img: torch.Tensor, patch_size: Tuple[int, 
         return "channel count differs from the constructor's (the reference's Linear raises)"
     if any(s % p for s, p in zip(img.shape[2:], patch_size)):
         return "input not divisible by the patch size"
-    if len(owner.transformer.layers) == 0:
-        return "depth == 0"
-    reason = why_not_fused(list(owner.parameters()), img, training=owner.training, dropout_p=dropout_p)
-    if reason is None and hooks_inside(owner, skip=(owner.to_latent,)):
-        reason = "forward hooks registered inside the model"
+    reason = common_reason(owner, img, encoders=(owner.transformer,), dropout_p=dropout_p, skip=(owner.to_latent,))
     if reason is None and lin.in_features > MAX_FUSED_PATCH_DIM:
         reason = f"patch_dim {lin.in_features} > {MAX_FUSED_PATCH_DIM}"
     return reason
@@ -145,10 +138,9 @@ def nd_encode(owner: nn.Module, pe: NdPatchEngine, img: torch.Tensor,
     """Patch embedding -> encoder blocks: (x fp32 [B*N, D] before the final LayerNorm, B, N).  In fold mode the token
     assembly also writes the engine's bf16 copy of x and its row statistics.  Must run inside on_device(img)."""
     eng = owner.transformer.engine()
-    primed = ln_mode() == "fold"
-    ws = eng.workspace(img.shape[0] * pe.tokens(img)[1], img.device) if primed else None
-    x, B, N = pe.run(img, xb=ws["xn"] if primed else None, stats=ws["stats_in"] if primed else None)
-    eng.run_blocks(x, B, N, primed=primed, rope=rope)
+    xb, stats = eng.entry_buffers(img.shape[0] * pe.tokens(img)[1], img.device)
+    x, B, N = pe.run(img, xb=xb, stats=stats)
+    eng.run_blocks(x, B, N, primed=xb is not None, rope=rope)
     return x, B, N
 
 
@@ -183,7 +175,6 @@ class ViTND(FusedWeightsMixin, nn.Module):
         self._nd_patch = tuple(patch_size)
         self._emb_dropout_p = float(emb_dropout)
         self._nd_engine = NdPatchEngine(self, self._nd_patch)
-        self._head_engine: Optional[HeadEngine] = None
 
     # ---------------------------------------------------------------------------------------------- dispatch
     def fused_reason(self, x: torch.Tensor) -> Optional[str]:
@@ -218,21 +209,9 @@ class ViTND(FusedWeightsMixin, nn.Module):
     # ---------------------------------------------------------------------------------------------- fused kernels
     def forward_fused(self, img: torch.Tensor) -> torch.Tensor:
         x, B, N = nd_encode(self, self._nd_engine, img)
-        D = x.shape[1]
         eng = self.transformer.engine()
-        dev = img.device
-        pooled = torch.empty(B, D, device=dev, dtype=torch.bfloat16)
-        if self.pool == 'mean':
-            # mean over the patch tokens x[:, 1:]: the stream offset by the cls row, N - 1 rows per input
-            xf = torch.empty_like(x)
-            eng.final_norm(x, out_f32=xf)
-            pm = torch.empty(B, D, device=dev, dtype=torch.float32)
-            _lib.mean_pool(xf.view(-1)[D:], pm, B, N, D, n_pool=N - 1)
-            _lib.cast_f32_bf16(pm, pooled)
-        else:                                          # LayerNorm is per token: normalise only the cls rows
-            rows = torch.arange(0, B * N, N, device=dev, dtype=torch.int32)
-            eng.final_norm(x, out_bf16=pooled, row_index=rows)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.mlp_head)
-        return self._head_engine.run(pooled)
+        if self.pool == 'mean':                        # mean over the patch tokens x[:, 1:], N - 1 rows per input
+            pooled = eng.pool(x, B, N, mean=True, skip=1, n_pool=N - 1)
+        else:
+            pooled = eng.pool(x, B, N, mean=False)
+        return classify(self, self.mlp_head, pooled)

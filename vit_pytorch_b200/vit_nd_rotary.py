@@ -22,8 +22,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import _lib
-from .engine import _WEIGHT_EPOCH, FusedWeightsMixin, HeadEngine, on_device
+from .engine import _WEIGHT_EPOCH, FusedWeightsMixin, classify, on_device
 from .vit import FeedForward, FusedTransformer
 from .vit_nd import NdPatchEngine, PatchifyND, ensure_tuple, nd_encode, nd_fused_reason
 
@@ -211,7 +210,6 @@ class ViTND(FusedWeightsMixin, nn.Module):
         self._nd_patch = tuple(patch_size)
         self._emb_dropout_p = float(emb_dropout)
         self._nd_engine = NdPatchEngine(self, self._nd_patch)
-        self._head_engine: Optional[HeadEngine] = None
         self._rope_cache: Dict[tuple, torch.Tensor] = {}
 
     def muon_parameters(self) -> List[nn.Parameter]:
@@ -272,18 +270,8 @@ class ViTND(FusedWeightsMixin, nn.Module):
         x, B, N = nd_encode(self, self._nd_engine, img, rope=(cs, cs.shape[0]))      # table rows = N
         D = x.shape[1]
         eng = self.transformer.engine()
-        dev = img.device
         if return_embed:
-            out = torch.empty(B * N, D, device=dev, dtype=torch.bfloat16)
+            out = torch.empty(B * N, D, device=img.device, dtype=torch.bfloat16)
             eng.final_norm(x, out_bf16=out)
             return out.view(B, *grid, D)
-        xf = torch.empty_like(x)
-        eng.final_norm(x, out_f32=xf)
-        pm = torch.empty(B, D, device=dev, dtype=torch.float32)
-        _lib.mean_pool(xf, pm, B, N, D)
-        pooled = torch.empty(B, D, device=dev, dtype=torch.bfloat16)
-        _lib.cast_f32_bf16(pm, pooled)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.mlp_head)
-        return self._head_engine.run(pooled)
+        return classify(self, self.mlp_head, eng.pool(x, B, N, mean=True))

@@ -31,8 +31,8 @@ from torch import nn
 from torch.nn.attention import SDPBackend, sdpa_kernel
 
 from . import _lib
-from .engine import (AttnBlock, EncoderLayer, FusedEncoder, FusedWeightsMixin, HeadEngine, Norm, _f32, hooks_inside,
-                     ln_mode, on_device, patch_engine, why_not_fused)
+from .engine import (AttnBlock, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _f32, classify, common_reason,
+                     on_device, patch_engine)
 from .simple_vit_3d import VideoPatchify
 from .vit import FeedForward, FusedTransformer, pair
 
@@ -198,11 +198,7 @@ class FactorizedTransformer(FusedEncoder, FusedWeightsMixin, nn.Module):
         return [_encoder_layer(sa, ff, temporal=ta) for sa, ta, ff in self.layers], Norm.of(self.norm)
 
     def fused_reason(self, x: torch.Tensor, mask: Optional[torch.Tensor] = None) -> Optional[str]:
-        if len(self.layers) == 0:
-            return "depth == 0"
-        r = why_not_fused(list(self.parameters()), x, training=self.training, dropout_p=self.dropout_p)
-        if r is None and hooks_inside(self):
-            r = "forward hooks registered inside the transformer"
+        r = common_reason(self, x, encoders=(self,), dropout_p=self.dropout_p, inside="transformer")
         if r is None and x.dim() != 4:
             r = "input is not (B, F, N, D)"
         if r is None:
@@ -289,8 +285,6 @@ class ViViT(FusedWeightsMixin, nn.Module):
         self._emb_dropout_p = float(emb_dropout)
         # the 2-D patch kernels see the video as (B, C, F' * pf * H, W) cut into (pf * p1, p2) boxes
         self.fused_patch_box: Tuple[int, int] = (frame_patch_size * patch_height, patch_width)
-        self._patch_engine = None
-        self._head_engine: Optional[HeadEngine] = None
 
     def _transformers(self) -> List[nn.Module]:
         if self.variant == 'factorized_encoder':
@@ -313,12 +307,9 @@ class ViViT(FusedWeightsMixin, nn.Module):
         if f > self.pos_embedding.shape[1] or n > self.pos_embedding.shape[2]:
             return (f"{f} frame patches x {n} patches exceed the positional table "
                     f"({self.pos_embedding.shape[1]} x {self.pos_embedding.shape[2]})")
-        if any(len(t.layers) == 0 for t in self._transformers()):
-            return "depth == 0"
-        p_drop = max([self._emb_dropout_p] + [t.dropout_p for t in self._transformers()])
-        r = why_not_fused(list(self.parameters()), video, training=self.training, dropout_p=p_drop)
-        if r is None and hooks_inside(self, skip=(self.to_latent,)):
-            r = "forward hooks registered inside the model"
+        r = common_reason(self, video, encoders=self._transformers(),
+                          dropout_p=max([self._emb_dropout_p] + [t.dropout_p for t in self._transformers()]),
+                          skip=(self.to_latent,))
         for t in self._transformers():
             r = r or _attention_reason(t)
         if r is not None:
@@ -393,20 +384,16 @@ class ViViT(FusedWeightsMixin, nn.Module):
         y = pe.project(img, patch=self.fused_patch_box)            # [b*f*n, D], patches in (b, f, h, w) order
         t = pe.prepared(dev)
         D = y.shape[1]
-        primed = ln_mode() == "fold"
-        ws = eng.workspace(b * f * N, dev) if primed else None
+        xb, stats = eng.entry_buffers(b * f * N, dev)
         x = torch.empty(b * f * N, D, device=dev, dtype=torch.float32)
         _lib.embed_tokens_grouped(y, t["ln2.w"], t["ln2.b"], _f32(self.spatial_cls_token.reshape(1, D)) if cls else None,
                                   t["pos"].view(-1, D), x, b * f, n, ncls, pos_period=f,
                                   pos_stride=self.pos_embedding.shape[2], cls_pos=False,
-                                  eps=self.to_patch_embedding[3].eps, xb=ws["xn"] if primed else None,
-                                  stats=ws["stats_in"] if primed else None)
+                                  eps=self.to_patch_embedding[3].eps, xb=xb, stats=stats)
         key_mask = None if mask is None else mask.reshape(b, f, pf).all(dim=-1)
-        pooled = torch.empty(b, D, device=dev, dtype=torch.bfloat16)
         if fe:
-            eng.run_blocks(x, b * f, N, primed=primed)
-            xs = torch.empty(b * f, D, device=dev, dtype=torch.float32)
-            self._pool(eng, x, xs, b * f, N, cls)
+            eng.run_blocks(x, b * f, N, primed=xb is not None)
+            xs = eng.pool(x, b * f, N, mean=not cls, dtype=torch.float32)
             tr = self.temporal_transformer
             if cls:
                 xt = torch.cat((self.temporal_cls_token.detach().float().expand(b, 1, D), xs.view(b, f, D)), dim=1)
@@ -420,33 +407,11 @@ class ViViT(FusedWeightsMixin, nn.Module):
                                                    bool(_flash_mode(tr)))
             teng = tr.engine()
             teng.run_blocks(xt, b, Lt, axial=axial)
-            self._pool(teng, xt, pooled, b, Lt, cls)
+            pooled = teng.pool(xt, b, Lt, mean=not cls)
         else:
             tr = self.factorized_transformer
             axial = (N, f, None if key_mask is None else key_mask.to(torch.uint8).contiguous(),
                      bool(_flash_mode(tr)))
-            eng.run_blocks(x, b * f, N, primed=primed, axial=axial)
-            self._pool(eng, x, pooled, b, f * N, cls)
-        pooled = self.to_latent(pooled)
-        if self._head_engine is None:
-            self._head_engine = HeadEngine(self.mlp_head)
-        return self._head_engine.run(pooled)
-
-    @staticmethod
-    def _pool(eng, x: torch.Tensor, out: torch.Tensor, S: int, N: int, cls: bool) -> None:
-        """Final LayerNorm of the S sequences of N rows of x, then their first row (cls) or the mean of all N rows,
-        into out [S, D] (fp32 or bf16)."""
-        D = x.shape[1]
-        if cls:                                        # LayerNorm is per token: normalise only the first rows
-            rows = torch.arange(0, S * N, N, device=x.device, dtype=torch.int32)
-            if out.dtype == torch.bfloat16:
-                eng.final_norm(x, out_bf16=out, row_index=rows)
-            else:
-                eng.final_norm(x, out_f32=out, row_index=rows)
-            return
-        xf = torch.empty_like(x)
-        eng.final_norm(x, out_f32=xf)
-        pm = out if out.dtype == torch.float32 else torch.empty(S, D, device=x.device, dtype=torch.float32)
-        _lib.mean_pool(xf, pm, S, N, D)
-        if pm is not out:
-            _lib.cast_f32_bf16(pm, out)
+            eng.run_blocks(x, b * f, N, primed=xb is not None, axial=axial)
+            pooled = eng.pool(x, b, f * N, mean=not cls)
+        return classify(self, self.mlp_head, pooled)
