@@ -286,6 +286,27 @@ int b200vit_attention_cls(const void* qkv_self, const void* ctx_kv, int64_t ctx_
                           int ctx_first, int n, void* out, int64_t ldo, int B, int H, int dh, float scale,
                           void* stream);
 
+/*
+ * Attention with the softmax probabilities mixed across heads: DeepViT's re-attention (deepvit.py:56-67).  B sequences
+ * of N tokens, qkv[B*N, 3*H*dh] bf16 packed as for b200vit_attention, out[B*N, H*dh] bf16.  Per sequence, for query i,
+ * key j and heads g, f < H:
+ *   s_g[i,j] = scale * q_g[i] . k_g[j]
+ *   p_g      = softmax_j(s_g)
+ *   p'_f     = sum_g post[g][f] p_g
+ *   p''_f    = gamma_f (p'_f - mean) / sqrt(var + eps) + beta_f, mean / var over the H values p'_. of (i, j)
+ *                                                      (head_ln_gamma NULL: p'' = p')
+ *   out_f[i] = sum_j p''_f[i,j] v_f[j]
+ * post: device fp32 [H][H], indexed [input head][output head] (the einsum 'b h i j, h g -> b g i j');
+ * head_ln_gamma / head_ln_beta: device fp32 [H], both or neither, eps > 0.  Mixing, softmax and the LayerNorm run in
+ * fp32; QK^T and PV on wgmma.  No score or probability tile goes to global memory: each CTA holds the score tiles of
+ * every head for 64 query rows and recomputes them per group of output heads (QK^T costs 3 ceil(H / 2G) times that of
+ * plain attention, G = 1..4 output heads per warpgroup, see csrc/headmix.cu).  N = 1..16384, dh = 32, 48, 64,
+ * 80 or 128, H <= 16, H*dh <= 1024, qkv and out 16-byte aligned.
+ */
+int b200vit_attention_headmix(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
+                              const float* post, const float* head_ln_gamma, const float* head_ln_beta,
+                              float head_ln_eps, void* stream);
+
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */
 int b200vit_mean_pool(const float* x, float* out, int B, int N, int D, int n_pool, void* stream);

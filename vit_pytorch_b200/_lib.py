@@ -35,6 +35,7 @@ SYMBOLS = [
     "b200vit_encoder_blocks", "b200vit_patchify_nd", "b200vit_rope_qk", "b200vit_encoder_blocks_rope",
     "b200vit_attention_axial", "b200vit_embed_tokens_grouped", "b200vit_patchify_spt_ln", "b200vit_attention_ex",
     "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex", "b200vit_attention_cls",
+    "b200vit_attention_headmix",
 ]
 
 
@@ -116,6 +117,8 @@ def lib() -> C.CDLL:
     L.b200vit_attn_pool.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp]
     L.b200vit_attention_cls.restype = i32
     L.b200vit_attention_cls.argtypes = [vp, vp, i64, i64, i32, i32, vp, i64, i32, i32, i32, f32, vp]
+    L.b200vit_attention_headmix.restype = i32
+    L.b200vit_attention_headmix.argtypes = [vp, vp, i32, i32, i32, i32, f32, vp, vp, vp, f32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -664,6 +667,29 @@ def attention_cls(qkv_self: torch.Tensor, ctx: Optional[torch.Tensor], out: torc
                                          int(rows_per_image), int(first), int(n), _ptr(out), out.stride(0), B, H, dh,
                                          float(scale), _stream())
     _check(rc, "b200vit_attention_cls")
+
+
+def attention_headmix(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, H: int, dh: int, scale: float,
+                       post: torch.Tensor, head_ln: Optional[tuple] = None) -> None:
+    """Attention with heads mixed across the head axis (re-attention) over B sequences of N tokens of qkv[B*N, 3*H*dh]:
+    post (fp32 [H, H], indexed [input head, output head]) mixes the softmax probabilities; head_ln = (gamma [H],
+    beta [H], eps) adds a LayerNorm over the heads of every (query, key) pair after the mix."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out")
+    _chk(post, torch.float32, "post")
+    assert qkv.is_contiguous() and out.is_contiguous()
+    assert qkv.shape == (B * N, 3 * H * dh) and out.shape == (B * N, H * dh)
+    assert post.is_contiguous() and post.shape == (H, H)
+    g = b = None
+    eps = 0.0
+    if head_ln is not None:
+        g, b, eps = head_ln
+        _chk(g, torch.float32, "head_ln gamma"); _chk(b, torch.float32, "head_ln beta")
+        assert g.is_contiguous() and b.is_contiguous() and g.numel() == H and b.numel() == H
+    with _Timed("attention_headmix", B=B, N=N, H=H, bytes=(qkv.numel() + out.numel()) * 2,
+                flops=4.0 * B * H * N * N * dh):
+        rc = lib().b200vit_attention_headmix(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), _ptr(post),
+                                             _ptr(g), _ptr(b), float(eps), _stream())
+    _check(rc, "b200vit_attention_headmix")
 
 
 def mean_pool(x: torch.Tensor, out: torch.Tensor, B: int, N: int, D: int, n_pool: Optional[int] = None) -> None:

@@ -128,6 +128,8 @@ def common_reason(owner: nn.Module, x: torch.Tensor, *, encoders=(), dropout_p: 
 
 
 HEAD_WIDTHS = (32, 64, 80, 128)
+HEADMIX_WIDTHS = (32, 48, 64, 80, 128)     # b200vit_attention_headmix
+HEADMIX_MAX_HEADS, HEADMIX_MAX_INNER = 16, 1024
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -135,6 +137,17 @@ def head_width_reason(dh: int) -> Optional[str]:
     PyTorch graph is used.  One rule for every model family."""
     if dh not in HEAD_WIDTHS:
         return f"dim_head={dh} (the attention kernels are built for 32, 64, 80 and 128)"
+    return None
+
+
+def headmix_reason(heads: int, dh: int) -> Optional[str]:
+    """None if b200vit_attention_headmix is built for `heads` heads `dh` wide, else the reason the eager PyTorch graph
+    is used."""
+    if dh not in HEADMIX_WIDTHS:
+        return f"dim_head={dh} (the head-mixing attention kernel is built for 32, 48, 64, 80 and 128)"
+    if heads > HEADMIX_MAX_HEADS or heads * dh > HEADMIX_MAX_INNER:
+        return (f"heads={heads} x dim_head={dh} (the head-mixing attention kernel takes at most "
+                f"{HEADMIX_MAX_HEADS} heads and heads * dim_head <= {HEADMIX_MAX_INNER})")
     return None
 
 
@@ -156,6 +169,14 @@ class AttnBlock(NamedTuple):
     qkv_w: torch.Tensor                            # [3 * heads * dim_head, D], rows q | k | v
     out_w: Optional[torch.Tensor]                  # None: to_out is the identity, as EncoderLayer.out_w
     out_b: Optional[torch.Tensor]
+
+
+class HeadMix(NamedTuple):
+    """Softmax probabilities mixed across the head axis (b200vit_attention_headmix; DeepViT's re-attention,
+    deepvit.py:61-62): post indexed [input head, output head], ln a LayerNorm over the heads of every (query, key)
+    pair after the mix."""
+    post: torch.Tensor                            # [heads, heads]
+    ln: Optional[Norm]                            # over `heads` values, or None
 
 
 @dataclass
@@ -183,6 +204,8 @@ class EncoderLayer:
     temporal: Optional[AttnBlock] = None
     # each query's own key excluded from its softmax (LSA, vit_for_small_dataset.py:53-57)
     mask_self: bool = False
+    # heads mixed across the head axis around the softmax (the attention runs b200vit_attention_headmix)
+    headmix: Optional[HeadMix] = None
 
 
 class _Prepared:
@@ -313,7 +336,7 @@ class TransformerEngine:
     def unsupported_reason(self, N: int) -> Optional[str]:
         # only shapes are read, and a module's shapes are fixed at construction: any description of it serves
         for L in self.layers or self.mod.encoder_layers()[0]:
-            r = head_width_reason(L.dim_head)
+            r = head_width_reason(L.dim_head) if L.headmix is None else headmix_reason(L.heads, L.dim_head)
             if r is not None:
                 return r
             if L.qkv_w.shape[1] % 8 or L.fc1_w.shape[0] % 8:
@@ -351,6 +374,11 @@ class TransformerEngine:
                 t[f"{i}.tout.w"] = (torch.eye(T.qkv_w.shape[1], device=T.qkv_w.device, dtype=torch.bfloat16)
                                     if T.out_w is None else _bf16_rows(T.out_w))
                 t[f"{i}.tout.b"] = _f32(T.out_b)
+            if L.headmix is not None:
+                X = L.headmix
+                t[f"{i}.post"] = _f32(X.post)
+                if X.ln is not None:
+                    t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(X.ln.gamma), _f32(X.ln.beta)
             t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(L.ln2.gamma), _f32(L.ln2.beta)
             _fold(t, f"{i}.fc1", L.fc1_w, L.fc1_b, L.ln2)
             t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(L.fc1_w), _f32(L.fc1_b)
@@ -364,11 +392,13 @@ class TransformerEngine:
     def _c_layers(self, t: Dict[str, torch.Tensor]):
         """(ctypes array of b200vit_layer, (heads, dh, hidden, scale), layer scales, attention flags) for the one-call
         encoder (b200vit_encoder_blocks), or None when it cannot run these layers: they are not uniform, one has a
-        per-head LayerNorm (the one-call encoder has no EPI_HEADLN) or a temporal sub-block.  Layer scales: None when
+        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block or heads mixed across the
+        head axis.  Layer scales: None when
         every layer has the same scale, else a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned
         temperatures).  The pointers stay valid as long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
-        if any(L.qk_norm == "ln" or L.temporal is not None or sig(L) != sig(self.layers[0]) for L in self.layers):
+        if any(L.qk_norm == "ln" or L.temporal is not None or L.headmix is not None or sig(L) != sig(self.layers[0])
+               for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -469,6 +499,8 @@ class TransformerEngine:
         for i, L in enumerate(self.layers):
             if L.temporal is not None and axial is None:
                 raise ValueError("a layer with a temporal attention sub-block needs `axial` to address its sequences")
+            if L.headmix is not None and (axial is not None or varlen is not None):
+                raise ValueError("head-mixing attention runs over B sequences of N tokens only")
             # xb = LN1(x) -> qkv   (fold: xb already holds the bf16 copy of x; LN1 is applied in the GEMM epilogue)
             if fold:
                 w, ln = t[f"{i}.qkv.wg"], dict(bias=t[f"{i}.qkv.t"], ln_sums=ws["stats_in"] if i == 0 else sa,
@@ -483,7 +515,10 @@ class TransformerEngine:
                                    dh=L.dim_head, head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None, **ln)
             if rope is not None:
                 _lib.rope_qk(ws["qkv"], rope[0], rope[1], L.heads, L.dim_head)
-            if axial is not None and L.temporal is None:
+            if L.headmix is not None:
+                hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
+                _lib.attention_headmix(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln)
+            elif axial is not None and L.temporal is None:
                 axial_attention(L)
             elif vl is None:
                 _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
@@ -869,6 +904,23 @@ def classify(owner: nn.Module, linear: nn.Linear, pooled: torch.Tensor) -> torch
 def head_norm(owner: nn.Module, ln: nn.LayerNorm) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """fp32 (weight, bias) of the LayerNorm of the owner's head, cached by parameter version."""
     return cached(owner, "_head_norm", list(ln.parameters()), lambda: (_f32(ln.weight), _f32(ln.bias)))
+
+
+def head_ln_pool(owner: nn.Module, ln: nn.LayerNorm, x: torch.Tensor, B: int, N: int, *, mean: bool) -> torch.Tensor:
+    """x fp32 [B*N, D] encoder output of a Transformer without a final LayerNorm -> ln(x[:, 0]) or ln(x.mean(1)), bf16
+    [B, D]: the models whose mlp_head starts with a LayerNorm (vit_for_small_dataset.py:134-140, deepvit.py:125-129)."""
+    D = x.shape[1]
+    dev = x.device
+    g, b = head_norm(owner, ln)
+    pooled = torch.empty(B, D, device=dev, dtype=torch.bfloat16)
+    if mean:
+        pm = torch.empty(B, D, device=dev, dtype=torch.float32)
+        _lib.mean_pool(x, pm, B, N, D)
+        _lib.layernorm(pm, g, b, out_bf16=pooled, eps=ln.eps)
+    else:                                          # LayerNorm is per token: normalise only the cls rows
+        rows = cls_row_index(owner.transformer.engine().rows, B, N, dev)
+        _lib.layernorm(x, g, b, out_bf16=pooled, row_index=rows, eps=ln.eps)
+    return pooled
 
 
 def fused_encode(owner: nn.Module, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None,
