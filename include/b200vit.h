@@ -307,6 +307,31 @@ int b200vit_attention_headmix(const void* qkv, void* out, int B, int N, int H, i
                               const float* post, const float* head_ln_gamma, const float* head_ln_beta,
                               float head_ln_eps, void* stream);
 
+/*
+ * b200vit_attention_headmix with talking heads before the softmax as well (CaiT, cait.py:92-101): the scores are mixed
+ * across heads before the softmax,
+ *   s'_g[i,j] = sum_h pre[h][g] s_h[i,j],   p_g = softmax_j(s'_g)
+ * and the rest is as above.  pre: device fp32 [H][H], [input head][output head], or NULL (no pre-mix: exactly
+ * b200vit_attention_headmix).  Keys beyond the sequence are masked after the mix.
+ */
+int b200vit_attention_headmix_ex(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
+                                 const float* pre, const float* post, const float* head_ln_gamma,
+                                 const float* head_ln_beta, float head_ln_eps, void* stream);
+
+/*
+ * Class-token attention with talking heads (CaiT's class attention, cait.py:83-103 with a context): the addressing of
+ * b200vit_attention_cls (qkv_self, strided ctx_kv rows, out row stride ldo), with the heads mixed before and after the
+ * softmax.  For image b, key j over {self} u {the n context rows of image b}, heads g, f < H:
+ *   s_h[j] = scale * q_h . k_h[j];   s'_g = sum_h pre[h][g] s_h;   p_g = softmax_j(s'_g);   p'_f = sum_g post[g][f] p_g
+ *   out[b, f*dh:(f+1)*dh] = sum_j p'_f[j] v_f[j]
+ * pre, post: device fp32 [H][H], [input head][output head], both required.  n = 0..16384, dh = 32, 48, 64, 80 or 128,
+ * H <= 16, H*dh <= 1024; scores, softmax and both mixes in fp32.  One CTA of 8 warps per image.  ctx_ld and ldo
+ * multiples of 8, qkv_self / ctx_kv / out 16-byte aligned; ctx_kv may be NULL when n = 0.
+ */
+int b200vit_attention_cls_headmix(const void* qkv_self, const void* ctx_kv, int64_t ctx_ld, int64_t ctx_rows_per_image,
+                                  int ctx_first, int n, void* out, int64_t ldo, int B, int H, int dh, float scale,
+                                  const float* pre, const float* post, void* stream);
+
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */
 int b200vit_mean_pool(const float* x, float* out, int B, int N, int D, int n_pool, void* stream);

@@ -1,0 +1,220 @@
+"""-m gpu: the talking-heads attention kernels (b200vit_attention_headmix_ex with a pre-softmax mix,
+b200vit_attention_cls_headmix) and the fused CaiT on the H100.  The kernels are checked against fp32 torch expressions
+on the same bf16 data; the model against the reference's stored fp32 logits (tests/golden/cait.pt) and the module's
+own eager bf16 graph."""
+import sys
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+from conftest import GOLDEN_DIR, load_golden
+from vit_pytorch_b200 import _lib
+from vit_pytorch_b200.cait import CaiT, Transformer
+
+sys.path.insert(0, GOLDEN_DIR)
+from cait_spec import CAIT_CASES, cait_input, cait_model, seed_layer_dropout, weights_digest  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda"
+
+
+def stats(got, ref, rtol=1e-2, atol=1e-3):
+    d = (got.float().cpu() - ref.float().cpu()).abs()
+    return d.max().item(), (d <= atol + rtol * ref.float().cpu().abs()).float().mean().item()
+
+
+def close_to(out, ref):
+    tol = 1e-2 * ref.abs().max().item() + 1e-3
+    err = (out.float() - ref).abs()
+    assert err.max().item() <= tol + 1e-2 * ref.abs().max().item(), (err.max().item(), ref.abs().max().item())
+    assert (err <= tol + 1e-2 * ref.abs()).float().mean().item() > 0.999
+
+
+# ------------------------------------------------------------------------------------------------ attention_headmix_ex
+def headmix_reference(qkv, B, N, H, dh, scale, pre, post, ln):
+    """fp32 (q k^T scale) mixed by pre, softmax, mixed by post (both 'b h i j, h g -> b g i j'), LayerNorm over the
+    heads of every (i, j) if ln = (gamma, beta, eps), then times v (cait.py:92-101)."""
+    q, k, v = qkv.float().view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
+    s = torch.einsum('b h i j, h g -> b g i j', q @ k.transpose(-1, -2) * scale, pre)
+    p = torch.einsum('b h i j, h g -> b g i j', s.softmax(-1), post)
+    if ln is not None:
+        p = F.layer_norm(p.permute(0, 2, 3, 1), (H,), ln[0], ln[1], ln[2]).permute(0, 3, 1, 2)
+    return (p @ v).permute(0, 2, 1, 3).reshape(B * N, H * dh)
+
+
+def headmix_inputs(B, N, H, dh, seed):
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    qkv = torch.randn(B * N, 3 * H * dh, device=DEV, generator=g).bfloat16()
+    pre = torch.randn(H, H, device=DEV, generator=g)
+    post = torch.randn(H, H, device=DEV, generator=g)
+    ln = (1 + 0.2 * torch.randn(H, device=DEV, generator=g), 0.1 * torch.randn(H, device=DEV, generator=g), 1e-5)
+    return qkv, pre, post, ln
+
+
+@pytest.mark.parametrize("mode", ["pre_post", "pre_post_ln"])
+@pytest.mark.parametrize("N", [1, 2, 63, 64, 65, 196, 197, 577, 1025])
+@pytest.mark.parametrize("dh", [32, 48, 64, 80, 128])
+@pytest.mark.parametrize("H", [1, 2, 3, 8, 16])
+def test_attention_headmix_pre_against_fp32(H, dh, N, mode):
+    if H * dh > 1024:
+        pytest.skip("H * dim_head > 1024 is rejected (test_deepvit.py checks the message)")
+    B = 2
+    qkv, pre, post, ln = headmix_inputs(B, N, H, dh, H * 100000 + dh * 1000 + N + 7)
+    ln = ln if mode == "pre_post_ln" else None
+    scale = dh ** -0.5
+    out = torch.empty(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
+    _lib.attention_headmix(qkv, out, B, N, H, dh, scale, post, ln, pre=pre)
+    close_to(out, headmix_reference(qkv, B, N, H, dh, scale, pre, post, ln))
+
+
+def test_one_head_negative_pre_turns_the_softmax_around():
+    """heads = 1, pre = -1: softmax(-s), so the output differs from plain attention and matches the reference."""
+    B, N, H, dh = 2, 70, 1, 64
+    qkv, _, _, _ = headmix_inputs(B, N, H, dh, 13)
+    pre, post = torch.full((1, 1), -1.0, device=DEV), torch.ones(1, 1, device=DEV)
+    out = torch.empty(B * N, dh, device=DEV, dtype=torch.bfloat16)
+    _lib.attention_headmix(qkv, out, B, N, H, dh, 0.125, post, None, pre=pre)
+    close_to(out, headmix_reference(qkv, B, N, H, dh, 0.125, pre, post, None))
+    plain = headmix_reference(qkv, B, N, H, dh, 0.125, -pre, post, None)
+    assert (out.float() - plain).abs().max().item() > 0.1
+
+
+# ------------------------------------------------------------------------------------------------ attention_cls_headmix
+def cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, scale, pre, post):
+    B = qkv_self.shape[0]
+    I = H * dh
+    q, ks, vs = qkv_self.float().view(B, 3, H, dh).unbind(1)
+    c = ctx.float().view(B, rows, -1)[:, first:first + n, :2 * I]
+    k = torch.cat([ks[:, None], c[..., :I].view(B, n, H, dh)], 1)          # [B, n + 1, H, dh]
+    v = torch.cat([vs[:, None], c[..., I:].view(B, n, H, dh)], 1)
+    s = torch.einsum('b h d, b j h d -> b h j', q, k) * scale
+    p = torch.einsum('b h j, h g -> b g j', torch.einsum('b h j, h g -> b g j', s, pre).softmax(-1), post)
+    return torch.einsum('b h j, b j h d -> b h d', p, v).reshape(B, I)
+
+
+@pytest.mark.parametrize("first", [0, 1])
+@pytest.mark.parametrize("n", [0, 1, 15, 16, 196, 576, 4096])
+@pytest.mark.parametrize("H,dh", [(1, 64), (3, 48), (4, 32), (8, 48), (16, 64), (6, 80), (8, 128)])
+def test_attention_cls_headmix_against_fp32(H, dh, n, first):
+    B, I = 3, H * dh
+    g = torch.Generator(device=DEV).manual_seed(H * 1000 + dh + n)
+    qkv_self = torch.randn(B, 3 * I, device=DEV, generator=g).bfloat16()
+    rows = n + first + 2
+    ld = 2 * I + 24                                   # strided context rows with unused columns
+    ctx = torch.randn(B * rows, ld, device=DEV, generator=g).bfloat16()
+    pre, post = torch.randn(H, H, device=DEV, generator=g), torch.randn(H, H, device=DEV, generator=g)
+    buf = torch.full((B, I + 16), 3.0, device=DEV, dtype=torch.bfloat16)
+    out = buf[:, :I]
+    _lib.attention_cls_headmix(qkv_self, ctx, out, rows, first, n, H, dh, dh ** -0.5, pre, post)
+    first_out = out.clone()
+    _lib.attention_cls_headmix(qkv_self, ctx, out, rows, first, n, H, dh, dh ** -0.5, pre, post)
+    torch.cuda.synchronize()
+    assert torch.equal(out, first_out)                # repeat calls are bit-identical
+    assert (buf[:, I:] == 3.0).all()                  # columns outside out untouched
+    close_to(out, cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, dh ** -0.5, pre, post))
+
+
+# ------------------------------------------------------------------------------------------------ model
+def _eager_bf16(m, x, spec, monkeypatch):
+    """The module's own PyTorch graph in bf16 (every submodule), with the case's layer-dropout seed."""
+    with monkeypatch.context() as mp:
+        mp.setenv("B200VIT_DISABLE_FUSED", "1")
+        seed_layer_dropout(spec)
+        with torch.inference_mode():
+            return m(x)
+
+
+@pytest.mark.parametrize("ln_mode", ["fold", "exact"])
+@pytest.mark.parametrize("name", sorted(CAIT_CASES))
+def test_fused_against_reference_goldens(name, ln_mode, monkeypatch):
+    monkeypatch.setenv("B200VIT_LN_MODE", ln_mode)
+    case, spec = load_golden("cait")["cases"][name], CAIT_CASES[name]
+    ref = cait_model(CaiT, spec)
+    assert weights_digest(ref) == case["weights"]
+    x = cait_input(spec).to(DEV)
+    m = cait_model(CaiT, spec).to(DEV, torch.bfloat16)
+    with torch.inference_mode():
+        assert m.fused_reason(x) is None
+        _lib.reset_launch_count()
+        seed_layer_dropout(spec)
+        out = m(x)
+        torch.cuda.synchronize()
+        assert _lib.launch_count() > 0
+    eager = _eager_bf16(m, x, spec, monkeypatch)
+    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
+        mx, frac = stats(out, want)
+        print(f"{name} {ln_mode} vs {what}: max {mx:.5f} within {frac:.4f}")
+        assert mx < 3e-2, (what, mx, frac)
+
+
+def test_cuda_graph_replay_is_bit_identical():
+    from vit_pytorch_b200.graph import GraphedForward
+    spec = CAIT_CASES["n576_h8"]
+    m = cait_model(CaiT, spec).to(DEV, torch.bfloat16)
+    a = cait_input(spec).to(DEV)
+    b = torch.randn_like(a.float()).bfloat16()
+    with torch.inference_mode():
+        ya, yb = m(a).clone(), m(b).clone()
+        g = GraphedForward(m, a)
+        assert torch.equal(g(b), yb)
+        assert torch.equal(g(a), ya)
+
+
+def test_cuda_graph_refused_with_layer_dropout():
+    from vit_pytorch_b200.graph import GraphedForward
+    spec = CAIT_CASES["dh32_n64"]
+    m = cait_model(CaiT, {**spec, "layer_dropout": 0.1}).to(DEV, torch.bfloat16)
+    with pytest.raises(RuntimeError, match="layer_dropout"):
+        GraphedForward(m, cait_input(spec).to(DEV))
+
+
+def test_direct_patch_transformer_call():
+    torch.manual_seed(3)
+    t = Transformer(128, 2, 4, 48, 256).eval()
+    with torch.no_grad():
+        for p in t.parameters():
+            p.copy_(p.bfloat16().float())
+    ref = Transformer(128, 2, 4, 48, 256).eval()
+    ref.load_state_dict(t.state_dict())
+    t = t.to(DEV, torch.bfloat16)
+    x = torch.randn(5, 33, 128, device=DEV).bfloat16()
+    with torch.inference_mode():
+        assert t.fused_reason(x) is None
+        _lib.reset_launch_count()
+        out = t(x)
+        torch.cuda.synchronize()
+        assert _lib.launch_count() > 0
+        want = ref(x.float().cpu())
+    scale = want.abs().max().item()
+    mx, frac = stats(out, want, rtol=1e-2, atol=1e-2 * scale)
+    assert mx < 1e-2 * scale and frac > 0.99, (mx, frac, scale)
+
+
+FALLBACK_KW = dict(image_size=32, patch_size=4, num_classes=3, dim=64, depth=1, cls_depth=1, mlp_dim=64)
+
+
+def _model(**kw):
+    return CaiT(**{**FALLBACK_KW, "heads": 4, "dim_head": 32, **kw}).eval().to(DEV, torch.bfloat16)
+
+
+def test_fallback_unsupported_head_width():
+    m, x = _model(heads=2, dim_head=96), torch.randn(2, 3, 32, 32, device=DEV).bfloat16()
+    with torch.inference_mode():
+        assert "dim_head=96" in m.fused_reason(x)
+        assert m(x).shape == (2, 3)                        # eager, like the reference
+
+
+def test_fallback_too_many_heads():
+    m, x = _model(heads=17, dim_head=32), torch.randn(2, 3, 32, 32, device=DEV).bfloat16()
+    with torch.inference_mode():
+        assert "heads=17" in m.fused_reason(x)
+        assert m(x).shape == (2, 3)
+
+
+def test_fallback_positional_table_and_divisibility():
+    m = _model()
+    with torch.inference_mode():
+        assert "positional table" in m.fused_reason(torch.randn(2, 3, 36, 36, device=DEV).bfloat16())
+        assert "divisible" in m.fused_reason(torch.randn(2, 3, 30, 30, device=DEV).bfloat16())
+        assert "channel count" in m.fused_reason(torch.randn(2, 1, 32, 32, device=DEV).bfloat16())

@@ -35,7 +35,7 @@ SYMBOLS = [
     "b200vit_encoder_blocks", "b200vit_patchify_nd", "b200vit_rope_qk", "b200vit_encoder_blocks_rope",
     "b200vit_attention_axial", "b200vit_embed_tokens_grouped", "b200vit_patchify_spt_ln", "b200vit_attention_ex",
     "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex", "b200vit_attention_cls",
-    "b200vit_attention_headmix",
+    "b200vit_attention_headmix", "b200vit_attention_headmix_ex", "b200vit_attention_cls_headmix",
 ]
 
 
@@ -119,6 +119,10 @@ def lib() -> C.CDLL:
     L.b200vit_attention_cls.argtypes = [vp, vp, i64, i64, i32, i32, vp, i64, i32, i32, i32, f32, vp]
     L.b200vit_attention_headmix.restype = i32
     L.b200vit_attention_headmix.argtypes = [vp, vp, i32, i32, i32, i32, f32, vp, vp, vp, f32, vp]
+    L.b200vit_attention_headmix_ex.restype = i32
+    L.b200vit_attention_headmix_ex.argtypes = [vp, vp, i32, i32, i32, i32, f32, vp, vp, vp, vp, f32, vp]
+    L.b200vit_attention_cls_headmix.restype = i32
+    L.b200vit_attention_cls_headmix.argtypes = [vp, vp, i64, i64, i32, i32, vp, i64, i32, i32, i32, f32, vp, vp, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -670,15 +674,17 @@ def attention_cls(qkv_self: torch.Tensor, ctx: Optional[torch.Tensor], out: torc
 
 
 def attention_headmix(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, H: int, dh: int, scale: float,
-                       post: torch.Tensor, head_ln: Optional[tuple] = None) -> None:
-    """Attention with heads mixed across the head axis (re-attention) over B sequences of N tokens of qkv[B*N, 3*H*dh]:
-    post (fp32 [H, H], indexed [input head, output head]) mixes the softmax probabilities; head_ln = (gamma [H],
-    beta [H], eps) adds a LayerNorm over the heads of every (query, key) pair after the mix."""
+                       post: torch.Tensor, head_ln: Optional[tuple] = None, pre: Optional[torch.Tensor] = None) -> None:
+    """Attention with heads mixed across the head axis (re-attention, talking heads) over B sequences of N tokens of
+    qkv[B*N, 3*H*dh]: post (fp32 [H, H], indexed [input head, output head]) mixes the softmax probabilities; head_ln =
+    (gamma [H], beta [H], eps) adds a LayerNorm over the heads of every (query, key) pair after the mix; pre (fp32
+    [H, H], same indexing) mixes the scores before the softmax (b200vit_attention_headmix_ex)."""
     _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out")
-    _chk(post, torch.float32, "post")
+    _chk(post, torch.float32, "post"); _chk(pre, torch.float32, "pre")
     assert qkv.is_contiguous() and out.is_contiguous()
     assert qkv.shape == (B * N, 3 * H * dh) and out.shape == (B * N, H * dh)
     assert post.is_contiguous() and post.shape == (H, H)
+    assert pre is None or (pre.is_contiguous() and pre.shape == (H, H))
     g = b = None
     eps = 0.0
     if head_ln is not None:
@@ -687,9 +693,30 @@ def attention_headmix(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, H: i
         assert g.is_contiguous() and b.is_contiguous() and g.numel() == H and b.numel() == H
     with _Timed("attention_headmix", B=B, N=N, H=H, bytes=(qkv.numel() + out.numel()) * 2,
                 flops=4.0 * B * H * N * N * dh):
-        rc = lib().b200vit_attention_headmix(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), _ptr(post),
-                                             _ptr(g), _ptr(b), float(eps), _stream())
-    _check(rc, "b200vit_attention_headmix")
+        rc = lib().b200vit_attention_headmix_ex(_ptr(qkv), _ptr(out), B, N, H, dh, float(scale), _ptr(pre),
+                                                _ptr(post), _ptr(g), _ptr(b), float(eps), _stream())
+    _check(rc, "b200vit_attention_headmix_ex")
+
+
+def attention_cls_headmix(qkv_self: torch.Tensor, ctx: Optional[torch.Tensor], out: torch.Tensor,
+                          rows_per_image: int, first: int, n: int, H: int, dh: int, scale: float, pre: torch.Tensor,
+                          post: torch.Tensor) -> None:
+    """Class-token attention with talking heads: the addressing of attention_cls, with the heads mixed by pre (fp32
+    [H, H], [input head, output head]) before the softmax and by post after it."""
+    _chk(qkv_self, torch.bfloat16, "qkv_self"); _chk(ctx, torch.bfloat16, "ctx"); _chk(out, torch.bfloat16, "out")
+    _chk(pre, torch.float32, "pre"); _chk(post, torch.float32, "post")
+    B = qkv_self.shape[0]
+    assert qkv_self.is_contiguous() and qkv_self.shape[1] == 3 * H * dh
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (B, H * dh)
+    assert ctx is None or (ctx.dim() == 2 and ctx.stride(1) == 1 and ctx.shape[1] >= 2 * H * dh
+                           and ctx.shape[0] >= (B - 1) * rows_per_image + first + n)
+    assert pre.is_contiguous() and pre.shape == (H, H) and post.is_contiguous() and post.shape == (H, H)
+    with _Timed("attention_cls_headmix", B=B, n=n, H=H, bytes=(B * n * 2 * H * dh + qkv_self.numel() + out.numel()) * 2,
+                flops=4.0 * B * H * (n + 1) * dh):
+        rc = lib().b200vit_attention_cls_headmix(_ptr(qkv_self), _ptr(ctx), 0 if ctx is None else ctx.stride(0),
+                                                 int(rows_per_image), int(first), int(n), _ptr(out), out.stride(0), B,
+                                                 H, dh, float(scale), _ptr(pre), _ptr(post), _stream())
+    _check(rc, "b200vit_attention_cls_headmix")
 
 
 def mean_pool(x: torch.Tensor, out: torch.Tensor, B: int, N: int, D: int, n_pool: Optional[int] = None) -> None:

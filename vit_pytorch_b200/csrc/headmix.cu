@@ -1,17 +1,18 @@
 // Attention whose heads are mixed across the head axis, for sm_90a:
 //   b200vit_attention_headmix   B sequences of N tokens (1 <= N <= 16384) out of the packed q | k | v buffer
-//     s_h = scale q_h k_h^T;  p_g = softmax_j(s_g);  p'_f = sum_g post[g][f] p_g;
-//     p''_f = LN over f of p' (gamma, beta, eps; head_ln NULL: p'' = p');  o_f = p''_f v_f
-//   That is DeepViT's re-attention (deepvit.py:56-67: post and the LayerNorm over heads).  Every output head depends on
+//     s_h = scale q_h k_h^T;  s'_g = sum_h pre[h][g] s_h (pre NULL: s' = s);  p_g = softmax_j(s'_g);
+//     p'_f = sum_g post[g][f] p_g;  p''_f = LN over f of p' (gamma, beta, eps; head_ln NULL: p'' = p');  o_f = p''_f v_f
+//   That is DeepViT's re-attention (deepvit.py:56-67: post and the LayerNorm over heads) and CaiT's talking heads
+//   (cait.py:92-101: pre and post, no LayerNorm).  Every output head depends on
 //   every head's probabilities at the same (i, j), so one CTA holds the score tiles of ALL heads for its query rows: no
 //   score or probability tile ever goes to global memory.
 //
 // One CTA = 64 query rows of one sequence and 2 G output heads: two warpgroups over the same 64 rows, warpgroup w
 // producing heads [y 2G + w G, y 2G + (w + 1) G).  Thread 0 loads Q (64 rows, every head) once and streams key blocks of
 // 16 keys (K of every head, plus V of the CTA's 2G heads) through a two-stage TMA/mbarrier ring, twice:
-//   pass 1  (warpgroup 0) S_h = Q_h K_h^T for every head (wgmma m64n16k16, operands in shared memory), online max /
-//           sum per (row, head) -> log2-sum-exp per (row, head) in shared memory
-//   pass 2  S again, p = exp2(s - lse) (exact normalised probabilities), post-mix + LayerNorm over heads in
+//   pass 1  (warpgroup 0) S_h = Q_h K_h^T for every head (wgmma m64n16k16, operands in shared memory), pre-mixed
+//           (PRE), online max / sum per (row, head) -> log2-sum-exp per (row, head) in shared memory
+//   pass 2  S again (pre-mixed), p = exp2(s - lse) (exact normalised probabilities), post-mix + LayerNorm over heads in
 //           fp32 registers, then O_f += P''_f V_f for the warpgroup's heads (wgmma, P'' in bf16 from registers)
 // Each thread holds the same (row, key) positions of every head's tile (the wgmma accumulator layout does not depend on
 // the head), so the mix is per-thread register arithmetic.  The cost of the design: every CTA computes QK^T of all H
@@ -39,21 +40,28 @@ struct HeadmixParams {
   float ln_eps;
   int N, H, I;
   float scale_log2e;
+  const float* pre;       // [H][H] or null (no pre-softmax mix; only the PRE instances read it)
 };
 
-// output heads per warpgroup: HC = head capacity of the instance (H <= HC)
-__host__ __device__ constexpr int hm_group(int dh, int hc) {
-  return hc == 4 ? 2 : hc == 8 ? (dh <= 64 ? 4 : dh == 128 ? 1 : 2) : (dh <= 32 ? 4 : dh <= 64 ? 2 : 1);
+// output heads per warpgroup: HC = head capacity of the instance (H <= HC).  The pre-mix needs registers of its own
+// (hm_pre_span), which the 16-head instances with two or more output heads per warpgroup take from the output
+// accumulators
+__host__ __device__ constexpr int hm_group(int dh, int hc, bool pre = false) {
+  return hc == 4 ? 2 : hc == 8 ? (dh <= 64 ? (pre && dh == 64 ? 2 : 4) : dh == 128 ? 1 : 2)
+                              : (pre ? (dh <= 32 ? 2 : 1) : (dh <= 32 ? 4 : dh <= 64 ? 2 : 1));
 }
+
+// positions of a thread's 8 mixed at a time by the pre-softmax mix: HC x span temporaries
+__host__ __device__ constexpr int hm_pre_span(int hc) { return hc >= 8 ? 16 / hc : 8; }
 
 // shared memory of a CTA (offsets from the 1024B-aligned base): Q64[H][N64] | Q16[H][N16], 2 stages of
 // K64[H][N64] | K16[H][N16] | V64[2G][N64] | V16[2G][N16], then lse[64][HC] | sum[64][HC], post[HC][HC] | coef[HC] |
-// gamma[HC] | beta[HC] (zero-padded beyond H), barriers full[2] empty[2] q.  Slabs: 64-wide = rows x 128 B (128B
-// swizzle), 16-wide = rows x 32 B (32B swizzle).
+// gamma[HC] | beta[HC] (zero-padded beyond H), pre[HC][HC] (PRE instances only), barriers full[2] empty[2] q.
+// Slabs: 64-wide = rows x 128 B (128B swizzle), 16-wide = rows x 32 B (32B swizzle).
 struct HmSmem {
   int q16, stage_off, k16, v64, v16, stage, lse, mix, bar, bytes;
   __host__ __device__ static int al(int x) { return (x + 1023) & ~1023; }
-  __host__ __device__ HmSmem(int dh, int H, int hc, int nvh) {
+  __host__ __device__ HmSmem(int dh, int H, int hc, int nvh, bool pre = false) {
     const int n64 = dh / 64, n16 = (dh % 64) / 16;
     q16 = al(H * n64 * HM_ROWS * 128);
     stage_off = al(q16 + H * n16 * HM_ROWS * 32);
@@ -63,7 +71,7 @@ struct HmSmem {
     stage = al(v16 + nvh * n16 * HM_KB * 32);
     lse = stage_off + 2 * stage;
     mix = lse + 2 * HM_ROWS * hc * 4;  // max / log2-sum-exp and sum
-    bar = mix + (hc * hc + 3 * hc) * 4;
+    bar = mix + ((pre ? 2 : 1) * hc * hc + 3 * hc) * 4;
     bytes = bar + 5 * 8 + 1024;
   }
 };
@@ -86,18 +94,24 @@ __device__ __forceinline__ float lds_keep(const float* p) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_u32(p)));
   return v;
 }
+__device__ __forceinline__ float4 lds_keep4(const float* p) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "r"(smem_u32(p)));
+  return v;
+}
 
-template <int DH, int HC>
+template <int DH, int HC, bool PRE>
 __global__ void __launch_bounds__(HM_THREADS, 1)
 attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                          const __grid_constant__ CUtensorMap tmQ16, const __grid_constant__ CUtensorMap tmKV16,
                          const HeadmixParams p) {
-  constexpr int N64 = DH / 64, N16 = (DH % 64) / 16, G = hm_group(DH, HC);
+  constexpr int N64 = DH / 64, N16 = (DH % 64) / 16, G = hm_group(DH, HC, PRE);
   static_assert(N64 * 64 + N16 * 16 == DH, "dim_head must be a multiple of 16");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int H = p.H;
-  const HmSmem L(DH, H, HC, 2 * G);
+  const HmSmem L(DH, H, HC, 2 * G, PRE);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + L.bar);
   uint64_t* empty = full + 2;
   uint64_t* qbar = full + 4;
@@ -105,6 +119,7 @@ attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
   float* coef_s = post_s + HC * HC;
   float* gamma_s = coef_s + HC;
   float* beta_s = gamma_s + HC;
+  float* pre_s = beta_s + HC;
 
   const int seq_start = blockIdx.z * p.N, len = p.N, q0 = blockIdx.x * HM_ROWS;
   const int tid = threadIdx.x;
@@ -162,6 +177,7 @@ attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     const int a = i / HC, b = i % HC;
     const bool in = a < H && b < H;
     post_s[i] = in ? p.post[a * H + b] : 0.f;
+    if (PRE) pre_s[i] = in ? p.pre[a * H + b] : 0.f;
   }
   for (int g = tid; g < HC; g += HM_THREADS) {
     float c = 0.f;
@@ -232,6 +248,41 @@ attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     for (int h = 0; h < HC; ++h)
 #pragma unroll
       for (int e = 0; e < 8; ++e) s[h][e] *= p.scale_log2e;
+    if constexpr (PRE) {
+      // s'_g = sum_h pre[h][g] s_h, in place, SP positions at a time.  Linear, so it commutes with scale_log2e; it
+      // runs before the key mask (a masked -inf inside the sum would give NaN), heads >= H are 0 with weight 0.  A
+      // rolled loop: each step mixes positions 0..SP-1 and rotates the 8 positions left by SP (register moves), so
+      // that ptxas cannot overlap the steps, whose temporaries together would not fit next to the score tiles
+      constexpr int SP = hm_pre_span(HC), e0 = 0;
+#pragma unroll 1
+      for (int step = 0; step < 8 / SP; ++step) {
+        float m[HC][SP];
+#pragma unroll
+        for (int g = 0; g < HC; ++g)
+#pragma unroll
+          for (int e = 0; e < SP; ++e) m[g][e] = 0.f;
+#pragma unroll
+        for (int h = 0; h < HC; ++h)
+#pragma unroll
+          for (int g = 0; g < HC; g += 4) {
+            const float4 w = lds_keep4(pre_s + h * HC + g);   // pre_s is 16-byte aligned (L.mix + post + 3 HC)
+#pragma unroll
+            for (int e = 0; e < SP; ++e) {
+              m[g][e] = fmaf(w.x, s[h][e0 + e], m[g][e]);
+              m[g + 1][e] = fmaf(w.y, s[h][e0 + e], m[g + 1][e]);
+              m[g + 2][e] = fmaf(w.z, s[h][e0 + e], m[g + 2][e]);
+              m[g + 3][e] = fmaf(w.w, s[h][e0 + e], m[g + 3][e]);
+            }
+          }
+#pragma unroll
+        for (int g = 0; g < HC; ++g) {
+#pragma unroll
+          for (int e = 0; e + SP < 8; ++e) s[g][e] = s[g][e + SP];
+#pragma unroll
+          for (int e = 0; e < SP; ++e) s[g][8 - SP + e] = m[g][e];
+        }
+      }
+    }
   };
   auto key_ok = [&](int kb, int e) { return kb * HM_KB + 8 * (e >> 2) + 2 * (lane & 3) + (e & 1) < len; };
   auto release = [&](int u) {
@@ -434,10 +485,10 @@ attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
   }
 }
 
-template <int DH, int HC>
+template <int DH, int HC, bool PRE>
 static int launch_headmix_t(const void* qkv, int B, const HeadmixParams& p, cudaStream_t stream) {
-  constexpr int G = hm_group(DH, HC);
-  const HmSmem L(DH, p.H, HC, 2 * G);
+  constexpr int G = hm_group(DH, HC, PRE);
+  const HmSmem L(DH, p.H, HC, 2 * G, PRE);
   B200_CHECK_ARG(L.bytes <= 227 * 1024, "attention_headmix: H=%d dh=%d needs %d bytes of shared memory", p.H, DH,
                  L.bytes);
   CUtensorMap tm[4];
@@ -453,7 +504,7 @@ static int launch_headmix_t(const void* qkv, int B, const HeadmixParams& p, cuda
   if (rc) return rc;
   if (!has16) tm[2] = tm[0], tm[3] = tm[1];
   if (!has64) tm[0] = tm[2], tm[1] = tm[3];
-  auto kern = attention_headmix_kernel<DH, HC>;
+  auto kern = attention_headmix_kernel<DH, HC, PRE>;
   B200_ENSURE_SMEM(kern, L.bytes);
   const dim3 grid((p.N + HM_ROWS - 1) / HM_ROWS, (p.H + 2 * G - 1) / (2 * G), B);
   kern<<<grid, HM_THREADS, L.bytes, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
@@ -462,20 +513,25 @@ static int launch_headmix_t(const void* qkv, int B, const HeadmixParams& p, cuda
   return 0;
 }
 
+template <int DH, bool PRE>
+static int launch_headmix_hc(const void* qkv, int B, const HeadmixParams& p, cudaStream_t st) {
+  if (p.H <= 4) return launch_headmix_t<DH, 4, PRE>(qkv, B, p, st);
+  if constexpr (DH == 128) return launch_headmix_t<DH, 8, PRE>(qkv, B, p, st);  // H dh <= 1024: H <= 8
+  else return p.H <= 8 ? launch_headmix_t<DH, 8, PRE>(qkv, B, p, st) : launch_headmix_t<DH, 16, PRE>(qkv, B, p, st);
+}
+
 template <int DH>
 static int launch_headmix_dh(const void* qkv, int B, const HeadmixParams& p, cudaStream_t st) {
-  if (p.H <= 4) return launch_headmix_t<DH, 4>(qkv, B, p, st);
-  if constexpr (DH == 128) return launch_headmix_t<DH, 8>(qkv, B, p, st);  // H dh <= 1024: H <= 8
-  else return p.H <= 8 ? launch_headmix_t<DH, 8>(qkv, B, p, st) : launch_headmix_t<DH, 16>(qkv, B, p, st);
+  return p.pre ? launch_headmix_hc<DH, true>(qkv, B, p, st) : launch_headmix_hc<DH, false>(qkv, B, p, st);
 }
 
 }  // namespace b200
 
 using namespace b200;
 
-extern "C" int b200vit_attention_headmix(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
-                                         const float* post, const float* head_ln_gamma,
-                                         const float* head_ln_beta, float head_ln_eps, void* stream) {
+extern "C" int b200vit_attention_headmix_ex(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
+                                            const float* pre, const float* post, const float* head_ln_gamma,
+                                            const float* head_ln_beta, float head_ln_eps, void* stream) {
   B200_CHECK_ARG(qkv && out && post, "attention_headmix: null pointer");
   B200_CHECK_ARG((head_ln_gamma == nullptr) == (head_ln_beta == nullptr),
                  "attention_headmix: head LayerNorm needs both gamma and beta");
@@ -488,14 +544,15 @@ extern "C" int b200vit_attention_headmix(const void* qkv, void* out, int B, int 
   B200_CHECK_ARG(B <= 65535, "attention_headmix: B=%d exceeds the grid", B);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention_headmix: qkv and out must be 16-byte aligned");
-  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(post) & 3) == 0 &&
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(post) & 3) == 0 && (reinterpret_cast<uintptr_t>(pre) & 3) == 0 &&
                      (reinterpret_cast<uintptr_t>(head_ln_gamma) & 3) == 0 &&
                      (reinterpret_cast<uintptr_t>(head_ln_beta) & 3) == 0,
-                 "attention_headmix: post and head LayerNorm vectors must be 4-byte aligned");
+                 "attention_headmix: pre, post and head LayerNorm vectors must be 4-byte aligned");
   B200_CHECK_ARG(head_ln_gamma == nullptr || head_ln_eps > 0.f, "attention_headmix: head LayerNorm eps must be > 0");
   HeadmixParams p{};
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.post = post;
+  p.pre = pre;
   p.ln_gamma = head_ln_gamma;
   p.ln_beta = head_ln_beta;
   p.ln_eps = head_ln_eps;
@@ -511,4 +568,11 @@ extern "C" int b200vit_attention_headmix(const void* qkv, void* out, int B, int 
     case 128: return launch_headmix_dh<128>(qkv, B, p, st);
     default: return launch_headmix_dh<64>(qkv, B, p, st);
   }
+}
+
+extern "C" int b200vit_attention_headmix(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
+                                         const float* post, const float* head_ln_gamma,
+                                         const float* head_ln_beta, float head_ln_eps, void* stream) {
+  return b200vit_attention_headmix_ex(qkv, out, B, N, H, dh, scale, nullptr, post, head_ln_gamma, head_ln_beta,
+                                      head_ln_eps, stream);
 }

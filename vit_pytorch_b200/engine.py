@@ -20,7 +20,7 @@ from __future__ import annotations
 import ctypes
 import os
 from dataclasses import dataclass
-from typing import Dict, List, NamedTuple, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 from torch import nn
@@ -174,9 +174,10 @@ class AttnBlock(NamedTuple):
 class HeadMix(NamedTuple):
     """Softmax probabilities mixed across the head axis (b200vit_attention_headmix; DeepViT's re-attention,
     deepvit.py:61-62): post indexed [input head, output head], ln a LayerNorm over the heads of every (query, key)
-    pair after the mix."""
+    pair after the mix; pre (CaiT's talking heads, cait.py:94) mixes the scores the same way before the softmax."""
     post: torch.Tensor                            # [heads, heads]
     ln: Optional[Norm]                            # over `heads` values, or None
+    pre: Optional[torch.Tensor] = None            # [heads, heads], or None
 
 
 @dataclass
@@ -206,6 +207,10 @@ class EncoderLayer:
     mask_self: bool = False
     # heads mixed across the head axis around the softmax (the attention runs b200vit_attention_headmix)
     headmix: Optional[HeadMix] = None
+    # LayerScale (cait.py:31-45): the attention and feed-forward outputs multiplied by these [D] vectors before their
+    # residual adds, folded into the rows and biases of out_w and fc2_w
+    out_scale: Optional[torch.Tensor] = None
+    ff_scale: Optional[torch.Tensor] = None
 
 
 class _Prepared:
@@ -276,6 +281,17 @@ def _bf16_rows(p: torch.Tensor, k_pad: Optional[int] = None) -> torch.Tensor:
         wp[:, : w.shape[1]] = w
         return wp
     return w.to(torch.bfloat16).contiguous()
+
+
+def _scaled_rows(w: torch.Tensor, b: Optional[torch.Tensor], scale: Optional[torch.Tensor]
+                 ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """(bf16 weight, fp32 bias) of a Linear whose output is multiplied by `scale` [out] (LayerScale): rows and bias
+    scaled in fp32, then rounded."""
+    if scale is None:
+        return _bf16_rows(w), _f32(b)
+    s = scale.detach().float().reshape(-1)
+    ws = (w.detach().float() * s[:, None]).to(torch.bfloat16).contiguous()
+    return ws, None if b is None else (b.detach().float() * s).contiguous()
 
 
 def _fold(t: Dict[str, torch.Tensor], prefix: str, w: torch.Tensor, b: Optional[torch.Tensor], ln: Norm) -> None:
@@ -362,10 +378,10 @@ class TransformerEngine:
             if L.out_w is None:
                 # reference vit.py:34,46-49: heads == 1 and dim_head == dim -> to_out is nn.Identity.  The residual
                 # GEMM then runs with an identity weight: bf16 x 1.0 products accumulate exactly, so x += o bit for bit
-                t[f"{i}.out.w"] = torch.eye(L.qkv_w.shape[1], device=L.qkv_w.device, dtype=torch.bfloat16)
+                eye = torch.eye(L.qkv_w.shape[1], device=L.qkv_w.device, dtype=torch.bfloat16)
+                t[f"{i}.out.w"], t[f"{i}.out.b"] = _scaled_rows(eye, L.out_b, L.out_scale)
             else:
-                t[f"{i}.out.w"] = _bf16_rows(L.out_w)
-            t[f"{i}.out.b"] = _f32(L.out_b)
+                t[f"{i}.out.w"], t[f"{i}.out.b"] = _scaled_rows(L.out_w, L.out_b, L.out_scale)
             if L.temporal is not None:
                 T = L.temporal
                 t[f"{i}.tln.w"], t[f"{i}.tln.b"] = _f32(T.ln.gamma), _f32(T.ln.beta)
@@ -377,12 +393,14 @@ class TransformerEngine:
             if L.headmix is not None:
                 X = L.headmix
                 t[f"{i}.post"] = _f32(X.post)
+                if X.pre is not None:
+                    t[f"{i}.pre"] = _f32(X.pre)
                 if X.ln is not None:
                     t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(X.ln.gamma), _f32(X.ln.beta)
             t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(L.ln2.gamma), _f32(L.ln2.beta)
             _fold(t, f"{i}.fc1", L.fc1_w, L.fc1_b, L.ln2)
             t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(L.fc1_w), _f32(L.fc1_b)
-            t[f"{i}.fc2.w"], t[f"{i}.fc2.b"] = _bf16_rows(L.fc2_w), _f32(L.fc2_b)
+            t[f"{i}.fc2.w"], t[f"{i}.fc2.b"] = _scaled_rows(L.fc2_w, L.fc2_b, L.ff_scale)
         if norm is not None:
             t["norm.w"], t["norm.b"] = _f32(norm.gamma), _f32(norm.beta)
         self.layers, self.norm = layers, norm
@@ -464,8 +482,10 @@ class TransformerEngine:
     def run_blocks(self, x: torch.Tensor, B: int = 0, N: int = 0, primed: bool = False,
                    varlen: Optional[_lib.VarlenIndex] = None,
                    rope: Optional[Tuple[torch.Tensor, int]] = None,
-                   axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None) -> None:
-        """All encoder layers, in place on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
+                   axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
+                   layers: Optional[Sequence[int]] = None) -> None:
+        """The encoder layers (all, or the indices in `layers`, in order: CaiT's layer dropout, cait.py:14-27), in place
+        on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
         B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
         `rope` = (table, rows): rotary positions on q and k after every QKV projection (and its head norm), token t
         using table row t % rows (_lib.rope_qk; the rotary ViTND, vit_nd_rotary.py:143-147).
@@ -481,8 +501,8 @@ class TransformerEngine:
         ws = self.workspace(x.shape[0], x.device)
         vl = self._varlen_args(B, N, varlen, x.device)
         fold = ln_mode() == "fold"
-        if (fold and varlen is None and axial is None and t["c_layers"] is not None and not _lib.profiling()
-                and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
+        if (fold and varlen is None and axial is None and layers is None and t["c_layers"] is not None
+                and not _lib.profiling() and os.environ.get(_HOST_LOOP_ENV, "c") == "c"):
             # the whole layer loop below the language boundary: one ctypes call instead of 5 x depth
             arr, (heads, dh, hidden, scale), layer_scales, flags = t["c_layers"]
             _lib.encoder_blocks(arr, len(arr), x, self.slot.c, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl,
@@ -496,14 +516,17 @@ class TransformerEngine:
             _lib.attention_axial(ws["qkv"], ws["o"], key_mask, x.shape[0] // (Lt * G), Lt, G, L.heads, L.dim_head,
                                  L.scale, zero)
 
-        for i, L in enumerate(self.layers):
+        run = range(len(self.layers)) if layers is None else layers
+        for k, i in enumerate(run):
+            L = self.layers[i]
             if L.temporal is not None and axial is None:
                 raise ValueError("a layer with a temporal attention sub-block needs `axial` to address its sequences")
             if L.headmix is not None and (axial is not None or varlen is not None):
                 raise ValueError("head-mixing attention runs over B sequences of N tokens only")
             # xb = LN1(x) -> qkv   (fold: xb already holds the bf16 copy of x; LN1 is applied in the GEMM epilogue)
             if fold:
-                w, ln = t[f"{i}.qkv.wg"], dict(bias=t[f"{i}.qkv.t"], ln_sums=ws["stats_in"] if i == 0 else sa,
+                # the first layer that runs reads the entry statistics, every later one those of the last fc2 GEMM
+                w, ln = t[f"{i}.qkv.wg"], dict(bias=t[f"{i}.qkv.t"], ln_sums=ws["stats_in"] if k == 0 else sa,
                                                col_s=t[f"{i}.qkv.s"], ln_eps=L.ln1.eps)
             else:
                 _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
@@ -517,7 +540,8 @@ class TransformerEngine:
                 _lib.rope_qk(ws["qkv"], rope[0], rope[1], L.heads, L.dim_head)
             if L.headmix is not None:
                 hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
-                _lib.attention_headmix(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln)
+                _lib.attention_headmix(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln,
+                                       pre=t.get(f"{i}.pre"))
             elif axial is not None and L.temporal is None:
                 axial_attention(L)
             elif vl is None:
@@ -557,6 +581,15 @@ class TransformerEngine:
         _lib.layernorm(x, t["norm.w"], t["norm.b"], out_bf16=out_bf16, out_f32=out_f32, row_index=row_index,
                        eps=self.norm.eps)
 
+    def stream_bf16(self, x: torch.Tensor) -> torch.Tensor:
+        """The bf16 copy of the residual stream x after run_blocks: in fold mode the workspace's, which the last
+        residual GEMM wrote; otherwise a new cast of x."""
+        if ln_mode() == "fold":
+            return self.workspace(x.shape[0], x.device)["xn"]
+        xb = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)
+        _lib.cast_f32_bf16(x.view(-1), xb.view(-1))
+        return xb
+
     def entry_buffers(self, M: int, device: torch.device) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
         """(xb, stats) an embedding kernel writes for the first layer so that run_blocks(primed=True) can skip its
         rowstats_cast pass: the workspace's bf16 copy of x and its row sums in fold mode, (None, None) otherwise."""
@@ -591,13 +624,14 @@ class TransformerEngine:
         return out
 
     def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None,
-                       axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None) -> torch.Tensor:
+                       axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
+                       layers: Optional[Sequence[int]] = None) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
-        reference mae.py:74, simmim.py:70, distill.py:66); `rope` and `axial` as in run_blocks."""
+        reference mae.py:74, simmim.py:70, distill.py:66); `rope`, `axial` and `layers` as in run_blocks."""
         B, N, D = tokens.shape
         with on_device(tokens):
             x = tokens.reshape(B * N, D).float().contiguous()
-            self.run_blocks(x, B, N, rope=rope, axial=axial)
+            self.run_blocks(x, B, N, rope=rope, axial=axial, layers=layers)
             out = torch.empty(B * N, D, device=tokens.device, dtype=torch.bfloat16)
             if self.norm is not None:
                 self.final_norm(x, out_bf16=out)
@@ -614,6 +648,11 @@ class PatchEmbedEngine:
     def __init__(self, owner: nn.Module) -> None:
         self.owner = owner
         self.prep = _Prepared()
+
+    def cls_row(self) -> Optional[torch.Tensor]:
+        """The owner's cls token if it opens every sequence: not for an owner with `cls_in_sequence = False` (CaiT's
+        cls token joins only in its class-attention stage, cait.py:175-176)."""
+        return getattr(self.owner, "cls_token", None) if getattr(self.owner, "cls_in_sequence", True) else None
 
     def params(self) -> List[torch.Tensor]:
         o = self.owner
@@ -654,7 +693,7 @@ class PatchEmbedEngine:
             t["tma.w"] = wg.view(-1, 256, C).permute(0, 2, 1).reshape(-1, pd).to(torch.bfloat16).contiguous()
             t["tma.s"] = t["tma.w"].float().sum(dim=1).contiguous()           # from the ROUNDED weights the MMA sees
             t["tma.b"] = (w32 @ ln1.bias.detach().float() + lin.bias.detach().float()).contiguous()
-        cls = getattr(o, "cls_token", None)
+        cls = self.cls_row()
         t["cls"] = _f32(cls) if (cls is not None and cls.shape[0] > 0) else None
         reg = getattr(o, "register_tokens", None)          # simple_vit_with_register_tokens.py:103,124-126
         t["tail"] = _f32(reg) if (reg is not None and reg.shape[0] > 0) else None
@@ -731,7 +770,7 @@ class PatchEmbedEngine:
     def geometry(self, img: torch.Tensor, patch: Optional[Tuple[int, int]] = None) -> Tuple[int, int]:
         """(B, N) the image batch will produce, without running anything."""
         ph, pw = patch if patch is not None else self.owner.patch_size
-        cls = getattr(self.owner, "cls_token", None)
+        cls = self.cls_row()
         reg = getattr(self.owner, "register_tokens", None)
         extra = (cls.shape[0] if cls is not None else 0) + (reg.shape[0] if reg is not None else 0)
         return img.shape[0], (img.shape[2] // ph) * (img.shape[3] // pw) + extra
@@ -754,13 +793,25 @@ class HeadEngine:
         return out
 
 
+class FeedForwardBlock(NamedTuple):
+    """x += fc2(GELU(fc1(LN(x)))) (reference vit.py:15-28)."""
+    ln: Norm
+    fc1_w: torch.Tensor
+    fc1_b: torch.Tensor
+    fc2_w: torch.Tensor
+    fc2_b: torch.Tensor
+
+
 class CrossLayer(NamedTuple):
     """One direction of one class-token cross-attention layer (CrossViT, reference cross_vit.py:94-130), as the module
     describes it to CrossAttentionEngine: the cls row of stream A (width D_A) queries the patch rows of stream B
     (width D_B), in B's width:
         c    = project_in(cls_A)                                   (Identity when D_A == D_B)
         cn   = LN(c);  q = cn Wq^T;  [k | v] = [cn; ctx_B] Wkv^T  (kv_include_self)
-        cls_A += project_out(to_out(softmax(q k^T * scale) v))"""
+        cls_A += project_out(to_out(softmax(q k^T * scale) v))
+    Optional parts (CaiT's class attention, cait.py:83-122): talking heads `pre` / `post` around the softmax
+    (b200vit_attention_cls_headmix), LayerScale `out_scale` on the to_out output, and a feed-forward sub-block `ff`
+    on the cls rows afterwards, its output scaled by `ff_scale`.  They need D_A == D_B."""
     proj_in: Optional[Tuple[torch.Tensor, torch.Tensor]]       # (weight [D_B, D_A], bias) or None
     ln: Norm
     q_w: torch.Tensor                                           # [heads * dim_head, D_B]
@@ -771,6 +822,11 @@ class CrossLayer(NamedTuple):
     heads: int
     dim_head: int
     scale: float
+    pre: Optional[torch.Tensor] = None                          # [heads, heads], [input head, output head]
+    post: Optional[torch.Tensor] = None                         # (pre and post: both or neither)
+    out_scale: Optional[torch.Tensor] = None                    # [D_B]
+    ff: Optional[FeedForwardBlock] = None
+    ff_scale: Optional[torch.Tensor] = None                     # [D_A]
 
 
 class CrossAttentionEngine:
@@ -783,7 +839,8 @@ class CrossAttentionEngine:
         projection:  project_in GEMM on A's cls rows (+ row statistics) -> LN-folded [to_q; to_kv] GEMM
         Identity:    LayerNorm of A's fp32 cls rows (row_index)        -> [to_q; to_kv] GEMM
         b200vit_attention_cls -> to_out GEMM -> project_out GEMM with the residual, in place on A's cls rows of the
-        fp32 stream and its bf16 copy (Identity: to_out carries the residual)."""
+        fp32 stream and its bf16 copy (Identity: to_out carries the residual);
+        with a feed-forward sub-block: LayerNorm of the cls rows -> fc1 GEMM + GELU -> fc2 GEMM with the residual."""
 
     def __init__(self, owner: nn.Module, direction: int) -> None:
         self.owner, self.direction = owner, direction
@@ -804,17 +861,25 @@ class CrossAttentionEngine:
             else:
                 t[f"{i}.ln.w"], t[f"{i}.ln.b"] = _f32(L.ln.gamma), _f32(L.ln.beta)
                 t[f"{i}.qkv.w"] = _bf16_rows(qkv_w)
-            t[f"{i}.out.w"], t[f"{i}.out.b"] = _bf16_rows(L.out_w), _f32(L.out_b)
+            t[f"{i}.out.w"], t[f"{i}.out.b"] = _scaled_rows(L.out_w, L.out_b, L.out_scale)
             if L.proj_out is not None:
                 t[f"{i}.pout.w"], t[f"{i}.pout.b"] = _bf16_rows(L.proj_out[0]), _f32(L.proj_out[1])
+            if L.pre is not None:
+                t[f"{i}.pre"], t[f"{i}.post"] = _f32(L.pre), _f32(L.post)
+            if L.ff is not None:
+                F = L.ff
+                t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(F.ln.gamma), _f32(F.ln.beta)
+                t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(F.fc1_w), _f32(F.fc1_b)
+                t[f"{i}.fc2.w"], t[f"{i}.fc2.b"] = _scaled_rows(F.fc2_w, F.fc2_b, L.ff_scale)
         t["ctx.w"] = _bf16_rows(torch.cat([L.kv_w.detach() for L in layers]))
         self.layers = layers
         return t
 
     def run(self, xa: torch.Tensor, xba: torch.Tensor, Na: int, xbb: torch.Tensor, Nb: int, B: int,
-            cls_rows_a: torch.Tensor) -> None:
+            cls_rows_a: torch.Tensor, skip: int = 1, layers: Optional[Sequence[int]] = None) -> None:
         """xa fp32 [B*Na, D_A] (stream A) and xba, its bf16 copy: cls rows updated in place.  xbb bf16 [B*Nb, D_B]:
-        stream B (row 0 of every image is its cls token, not part of the context).  cls_rows_a int32 [B] = b*Na."""
+        stream B, whose first `skip` rows per image are not part of the context (1: its cls token).  cls_rows_a int32
+        [B] = b*Na.  `layers`: the indices of the layers to run, in order (default all)."""
         t = self.prepared()
         dev = xa.device
         bf = dict(device=dev, dtype=torch.bfloat16)
@@ -822,7 +887,8 @@ class CrossAttentionEngine:
         ctx = torch.empty(B * Nb, t["ctx.w"].shape[0], **bf)
         _lib.gemm(xbb, t["ctx.w"], out_bf16=ctx)
         a_cls, ab_cls = xa.view(B, Na, Da)[:, 0], xba.view(B, Na, Da)[:, 0]      # row stride Na * D_A
-        for i, L in enumerate(self.layers):
+        for i in range(len(self.layers)) if layers is None else layers:
+            L = self.layers[i]
             I, Dc = L.heads * L.dim_head, L.q_w.shape[1]
             qin = torch.empty(B, Dc, **bf)
             qkv = torch.empty(B, 3 * I, **bf)
@@ -835,14 +901,24 @@ class CrossAttentionEngine:
                 _lib.layernorm(xa, t[f"{i}.ln.w"], t[f"{i}.ln.b"], out_bf16=qin, row_index=cls_rows_a, eps=L.ln.eps)
                 _lib.gemm(qin, t[f"{i}.qkv.w"], out_bf16=qkv)
             o = torch.empty(B, I, **bf)
-            _lib.attention_cls(qkv, ctx[:, 2 * I * i:2 * I * (i + 1)], o, Nb, 1, Nb - 1, L.heads, L.dim_head,
-                               L.scale)
+            ctx_i = ctx[:, 2 * I * i:2 * I * (i + 1)]
+            if L.pre is not None:
+                _lib.attention_cls_headmix(qkv, ctx_i, o, Nb, skip, Nb - skip, L.heads, L.dim_head, L.scale,
+                                           t[f"{i}.pre"], t[f"{i}.post"])
+            else:
+                _lib.attention_cls(qkv, ctx_i, o, Nb, skip, Nb - skip, L.heads, L.dim_head, L.scale)
             if L.proj_out is not None:
                 y = torch.empty(B, Dc, **bf)
                 _lib.gemm(o, t[f"{i}.out.w"], out_bf16=y, bias=t[f"{i}.out.b"])
                 _lib.gemm(y, t[f"{i}.pout.w"], out_f32=a_cls, out_bf16=ab_cls, bias=t[f"{i}.pout.b"], resid=a_cls)
             else:
                 _lib.gemm(o, t[f"{i}.out.w"], out_f32=a_cls, out_bf16=ab_cls, bias=t[f"{i}.out.b"], resid=a_cls)
+            if L.ff is not None:
+                h = torch.empty(B, L.ff.fc1_w.shape[0], **bf)
+                _lib.layernorm(xa, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=qin, row_index=cls_rows_a,
+                               eps=L.ff.ln.eps)
+                _lib.gemm(qin, t[f"{i}.fc1.w"], out_bf16=h, bias=t[f"{i}.fc1.b"], gelu=True)
+                _lib.gemm(h, t[f"{i}.fc2.w"], out_f32=a_cls, out_bf16=ab_cls, bias=t[f"{i}.fc2.b"], resid=a_cls)
 
 
 def cls_row_index(cache: Dict[tuple, torch.Tensor], B: int, N: int, device: torch.device) -> torch.Tensor:
@@ -917,6 +993,8 @@ def head_ln_pool(owner: nn.Module, ln: nn.LayerNorm, x: torch.Tensor, B: int, N:
         pm = torch.empty(B, D, device=dev, dtype=torch.float32)
         _lib.mean_pool(x, pm, B, N, D)
         _lib.layernorm(pm, g, b, out_bf16=pooled, eps=ln.eps)
+    elif N == 1:                                   # x holds the cls rows only (CaiT's class-attention stage)
+        _lib.layernorm(x, g, b, out_bf16=pooled, eps=ln.eps)
     else:                                          # LayerNorm is per token: normalise only the cls rows
         rows = cls_row_index(owner.transformer.engine().rows, B, N, dev)
         _lib.layernorm(x, g, b, out_bf16=pooled, row_index=rows, eps=ln.eps)

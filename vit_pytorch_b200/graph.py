@@ -23,6 +23,10 @@ class GraphedForward:
             reason = model.fused_reason(example) if hasattr(model, "fused_reason") else reason
         if reason is not None:
             raise RuntimeError(f"GraphedForward needs a call that takes the fused path: {reason}")
+        # a model whose fused forward varies from call to call at a fixed shape (CaiT's layer dropout) says why here
+        reason = model.graph_reason() if hasattr(model, "graph_reason") else None
+        if reason is not None:
+            raise RuntimeError(f"GraphedForward cannot replay this model: {reason}")
         self.model = model
         self.static_in = example.clone()
         self.graph = torch.cuda.CUDAGraph()
