@@ -164,6 +164,9 @@ int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats, int M, in
  * online softmax in fp32; S = QK^T and O = PV on the tensor cores (bf16 operands, fp32 accumulation).
  * dh = 32, 64, 80 (canonical ViT-H/14) or 128; a head is split into 64- and 16-column slabs (a 96-wide head would
  * fall out of the same scheme as 64 + 2 x 16, but is not built).
+ * Isolation (this and every attention entry point below): each sequence's output is computed from its own rows only,
+ * so a NaN or Inf in one sequence (image, packed sequence, batch element of b200vit_attention_axial) leaves every other
+ * sequence's output bit-identical, and no row past the buffer's addressed rows is read.
  */
 int b200vit_attention(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* stream);
 /* ... with flags: B200VIT_ATTN_MASK_SELF excludes each query's own key (masked_fill(eye, -finfo.max),

@@ -40,7 +40,7 @@ def test_gemm_k_padding_zero_fill():
     a = torch.randn(256, 64, device=DEV).bfloat16()
     w = torch.randn(192, 64, device=DEV).bfloat16()
     a[:, 48:] = 7.0                 # garbage beyond K=48 must not be read as data: pass k=48 explicitly
-    w[:, 48:] = 0.0
+    w[:, 48:] = 7.0
     out = torch.zeros(256, 192, device=DEV)
     _lib.gemm(a, w, out_f32=out, k=48)
     ref = a[:, :48].float() @ w[:, :48].float().t()

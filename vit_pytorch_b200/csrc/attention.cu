@@ -8,7 +8,11 @@
 // S = Q K^T with wgmma (both operands in shared memory), runs an online softmax in fp32 on the accumulator registers
 // and accumulates O += P V with wgmma, P (bf16) taken from registers as the A operand and V read as the transposed
 // (MN-major) B operand.  dh = 32, 64, 80 or 128: a head is split into 64-wide (128B swizzle) and 16-wide (32B swizzle)
-// slabs (AttnSmem).  Keys of a block beyond the sequence get probability 0; TMA zero-fills rows beyond the buffer.
+// slabs (AttnSmem).  Keys of a block beyond the sequence get probability 0, and their V rows are zero, so that a NaN or
+// Inf in one sequence cannot reach another through 0 x NaN in O += P V: the fixed-length kernel reads Q, K and V
+// through 3-D tensor maps (column, token, sequence), which zero-fill past the end of each sequence; the varlen kernel
+// reads the packed rows through 2-D maps and zeroes the V rows beyond the sequence of its last key block in shared
+// memory.
 // MASK_SELF instances (b200vit_attention_ex / _varlen_ex with B200VIT_ATTN_MASK_SELF) also give key i of query i
 // probability 0 -- LSA, vit_for_small_dataset.py:53-57 -- except in a sequence of one token, where the reference's
 // -finfo.max fill leaves that token's own key with weight 1.
@@ -90,20 +94,25 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int tid = threadIdx.x;
   const int wg = tid >> 7, t = tid & 127, warp = t >> 5, lane = t & 31;
 
+  // rows from token `tok` of this sequence: packed rows (varlen), or the (column, token, sequence) view
+  auto load = [&](void* dst, const CUtensorMap* tm, uint64_t* bar, int col, int tok) {
+    if (VARLEN) tma_load_2d(dst, tm, bar, col, seq_start + tok);
+    else tma_load_3d(dst, tm, bar, col, tok, blockIdx.z);
+  };
   auto issue_kv = [&](int blk) {
     const int st = blk & 1;
     uint8_t* sb = smem + L::STAGE_OFF + st * L::STAGE;
-    const int row = seq_start + blk * KB;
+    const int tok = blk * KB;
     mbar_arrive_expect_tx(&full[st], L::STAGE);
 #pragma unroll
     for (int c = 0; c < N64; ++c) {
-      tma_load_2d(sb + c * L::KV64, &tmKV, &full[st], colk + 64 * c, row);
-      tma_load_2d(sb + (N64 + c) * L::KV64, &tmKV, &full[st], colv + 64 * c, row);
+      load(sb + c * L::KV64, &tmKV, &full[st], colk + 64 * c, tok);
+      load(sb + (N64 + c) * L::KV64, &tmKV, &full[st], colv + 64 * c, tok);
     }
 #pragma unroll
     for (int c = 0; c < N16; ++c) {
-      tma_load_2d(sb + L::K16_OFF + c * L::KV16, &tmKV16, &full[st], colk + 64 * N64 + 16 * c, row);
-      tma_load_2d(sb + L::V16_OFF + c * L::KV16, &tmKV16, &full[st], colv + 64 * N64 + 16 * c, row);
+      load(sb + L::K16_OFF + c * L::KV16, &tmKV16, &full[st], colk + 64 * N64 + 16 * c, tok);
+      load(sb + L::V16_OFF + c * L::KV16, &tmKV16, &full[st], colv + 64 * N64 + 16 * c, tok);
     }
   };
 
@@ -121,10 +130,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   if (tid == 0) {
     mbar_arrive_expect_tx(qbar, L::STAGE_OFF);
 #pragma unroll
-    for (int c = 0; c < N64; ++c) tma_load_2d(smem + c * L::Q64, &tmQ, qbar, colq + 64 * c, seq_start + q0);
+    for (int c = 0; c < N64; ++c) load(smem + c * L::Q64, &tmQ, qbar, colq + 64 * c, q0);
 #pragma unroll
-    for (int c = 0; c < N16; ++c)
-      tma_load_2d(smem + N64 * L::Q64 + c * L::Q16, &tmQ16, qbar, colq + 64 * N64 + 16 * c, seq_start + q0);
+    for (int c = 0; c < N16; ++c) load(smem + N64 * L::Q64 + c * L::Q16, &tmQ16, qbar, colq + 64 * N64 + 16 * c, q0);
     issue_kv(0);
     if (nblocks > 1) issue_kv(1);
   }
@@ -152,6 +160,27 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const uint32_t ph = (kb >> 1) & 1;
     mbar_wait(&full[st], ph);
     const uint32_t sb = smem_u32(smem + L::STAGE_OFF + st * L::STAGE);
+    if (VARLEN && kb == nblocks - 1 && len % KB != 0) {
+      // the last block's rows beyond the sequence are the next sequence's tokens: zero their V (P is 0 there, but
+      // 0 x NaN is NaN), then make the writes visible to the wgmma reads of both warpgroups
+      const int r0 = len - kb * KB;
+      uint8_t* stage = smem + L::STAGE_OFF + st * L::STAGE;
+      const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+      // the swizzles permute 16-byte chunks within a row: row r of a slab is bytes [128 r, 128 r + 128) (64 wide) or
+      // [32 r, 32 r + 32) (16 wide)
+#pragma unroll
+      for (int c = 0; c < N64; ++c) {
+        uint4* sl = reinterpret_cast<uint4*>(stage + (N64 + c) * L::KV64);
+        for (int i = r0 * 8 + tid; i < KB * 8; i += ATT_THREADS) sl[i] = z;
+      }
+#pragma unroll
+      for (int c = 0; c < N16; ++c) {
+        uint4* sl = reinterpret_cast<uint4*>(stage + L::V16_OFF + c * L::KV16);
+        for (int i = r0 * 2 + tid; i < KB * 2; i += ATT_THREADS) sl[i] = z;
+      }
+      fence_proxy_async_smem();
+      __syncthreads();
+    }
 
     // S = Q K^T (64 rows x KB keys per warpgroup): one k16 step per 16 columns, the 64-wide slabs first
     float s[NS];
@@ -288,21 +317,24 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   }
 }
 
-// Tensor maps over qkv[T, 3 I]: 64-column boxes (128B swizzle) of 128 query rows / KB key rows for the 64-wide slabs,
-// and the same with 16 columns (32B swizzle) for the 16-wide ones.  A kind the head does not use gets a copy of the
-// other (never read).
+// Tensor maps over qkv[T, 3 I] (varlen) or its [B][N][3 I] view (fixed length, T = B N): 64-column boxes (128B swizzle)
+// of 128 query rows / KB key rows for the 64-wide slabs, and the same with 16 columns (32B swizzle) for the 16-wide
+// ones.  A kind the head does not use gets a copy of the other (never read).
 template <int DH, int KB, bool VARLEN, bool EMUL, bool MASK_SELF>
 static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 grid, cudaStream_t stream) {
   using L = AttnSmem<DH, KB>;
   CUtensorMap tm[4];
-  const uint64_t dims[2] = {(uint64_t)3 * p.I, (uint64_t)T};
-  const uint64_t strides[1] = {(uint64_t)3 * p.I * 2};
-  const uint32_t qbox[2] = {64, ATT_QROWS}, kvbox[2] = {64, KB}, qbox16[2] = {16, ATT_QROWS}, kvbox16[2] = {16, KB};
+  const int rank = VARLEN ? 2 : 3;
+  const uint64_t ld = (uint64_t)3 * p.I;
+  const uint64_t dims[3] = {ld, (uint64_t)(VARLEN ? T : p.N), (uint64_t)(VARLEN ? 1 : T / p.N)};
+  const uint64_t strides[2] = {ld * 2, ld * 2 * (VARLEN ? T : p.N)};
+  const uint32_t qbox[3] = {64, ATT_QROWS, 1}, kvbox[3] = {64, KB, 1}, qbox16[3] = {16, ATT_QROWS, 1},
+                 kvbox16[3] = {16, KB, 1};
   int rc = 0;
-  if (L::N64) rc = encode_tmap_bf16(&tm[0], qkv, 2, dims, strides, qbox);
-  if (!rc && L::N64) rc = encode_tmap_bf16(&tm[1], qkv, 2, dims, strides, kvbox);
-  if (!rc && L::N16) rc = encode_tmap_bf16_sw(&tm[2], qkv, 2, dims, strides, qbox16, 32);
-  if (!rc && L::N16) rc = encode_tmap_bf16_sw(&tm[3], qkv, 2, dims, strides, kvbox16, 32);
+  if (L::N64) rc = encode_tmap_bf16(&tm[0], qkv, rank, dims, strides, qbox);
+  if (!rc && L::N64) rc = encode_tmap_bf16(&tm[1], qkv, rank, dims, strides, kvbox);
+  if (!rc && L::N16) rc = encode_tmap_bf16_sw(&tm[2], qkv, rank, dims, strides, qbox16, 32);
+  if (!rc && L::N16) rc = encode_tmap_bf16_sw(&tm[3], qkv, rank, dims, strides, kvbox16, 32);
   if (rc) return rc;
   if (!L::N16) tm[2] = tm[0], tm[3] = tm[1];
   if (!L::N64) tm[0] = tm[2], tm[1] = tm[3];

@@ -2,9 +2,11 @@
 //   b200vit_attention_axial   ViViT's attention along the time axis (reference vivit.py:144-150) and the masked
 //                             temporal transformer (vivit.py:268), with an optional per-sequence key mask
 // Tokens are [B][L][G] rows: token j of sequence s = b*G + p is row b*L*G + j*G + p of qkv[T, 3*H*dh] and of out.
-// One CTA = one warpgroup = one 64-row tile of one head that holds SP x SB whole sequences (SP adjacent p of SB adjacent
-// b, all L tokens of each).  Thread 0 loads Q, K and V with one TMA box per slab over the 4-D view (column, p, j, b) of
-// qkv: box row r = (ib * L + j) * SP + ip; out-of-range p / b are zero-filled.  S = Q K^T (64 x 64) with wgmma, then a
+// One CTA = one warpgroup = one 64-row tile of one head that holds SP whole sequences (SP adjacent p of one b, all L
+// tokens of each).  Thread 0 loads Q, K and V with one TMA box per slab over the 4-D view (column, p, j, b) of qkv: box
+// row r = j * SP + ip; out-of-range p are zero-filled.  A tile never holds two batch elements: O = P V meets every V
+// row of the tile, and a masked key's zero probability times a NaN or Inf value would carry one video's non-finite
+// input into another's output.  S = Q K^T (64 x 64) with wgmma, then a
 // block-diagonal mask (same sequence) and the key mask in registers and a plain softmax in fp32 (every key of a row is
 // in the tile), and O = P V with wgmma, P (bf16) taken from registers as the A operand and V read as the transposed
 // (MN-major) B operand, as in attention.cu.  dh = 32, 64, 80 or 128 in 64-wide (128B swizzle) and 16-wide (32B swizzle)
@@ -22,7 +24,7 @@ struct AxialParams {
   __nv_bfloat16* out;
   const uint8_t* key_mask;  // NULL, or [B][L] with 1 = keep
   int B, L, G, I;           // I = H * dh
-  int sp, sb, tiles_p;      // sequences per tile along p and along b; tiles along p
+  int sp, tiles_p;          // sequences per tile along p; tiles along p
   float scale_log2e;
   int zero_masked_rows;
 };
@@ -51,9 +53,9 @@ attention_axial_kernel(const __grid_constant__ CUtensorMap tm64, const __grid_co
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFF);
 
   const int h = blockIdx.y;
-  const int tp = blockIdx.x % p.tiles_p, tb = blockIdx.x / p.tiles_p;
-  const int p0 = tp * p.sp, b0 = tb * p.sb;
-  const int rows = p.sp * p.L * p.sb;  // rows the box covers (<= 64)
+  const int tp = blockIdx.x % p.tiles_p, b0 = blockIdx.x / p.tiles_p;
+  const int p0 = tp * p.sp;
+  const int rows = p.sp * p.L;  // rows the box covers (<= 64)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   // rows beyond the box: their keys are masked, but V meets a zero probability in O = P V and must be finite
@@ -93,29 +95,18 @@ attention_axial_kernel(const __grid_constant__ CUtensorMap tm64, const __grid_co
 
   // this thread's rows r = 16 warp + lane/4 + 8 rh and key columns c = 8 jj + 2 (lane % 4) + e1 (wgmma m64 layout):
   // sequence within the tile, and whether the key is in range and kept by the mask
-  auto decode = [&](int r, int& ip, int& j, int& ib) {
-    ip = r % p.sp;
-    const int t = r / p.sp;
-    j = t % p.L;
-    ib = t / p.L;
-  };
   int rseq[2];
 #pragma unroll
-  for (int rh = 0; rh < 2; ++rh) {
-    int ip, j, ib;
-    decode(warp * 16 + (lane >> 2) + 8 * rh, ip, j, ib);
-    rseq[rh] = ib * p.sp + ip;
-  }
+  for (int rh = 0; rh < 2; ++rh) rseq[rh] = (warp * 16 + (lane >> 2) + 8 * rh) % p.sp;
   int cseq[16];
   uint32_t kept = 0;
 #pragma unroll
   for (int ci = 0; ci < 16; ++ci) {
     const int c = 8 * (ci >> 1) + 2 * (lane & 3) + (ci & 1);
-    int ip, j, ib;
-    decode(c, ip, j, ib);
-    cseq[ci] = ib * p.sp + ip;
-    bool ok = c < rows && p0 + ip < p.G && b0 + ib < p.B;
-    if (ok && p.key_mask) ok = p.key_mask[(long long)(b0 + ib) * p.L + j] != 0;
+    const int ip = c % p.sp, j = c / p.sp;
+    cseq[ci] = c < rows ? ip : -1;  // columns beyond the box belong to no sequence (an all-masked row averages its own)
+    bool ok = c < rows && p0 + ip < p.G;
+    if (ok && p.key_mask) ok = p.key_mask[(long long)b0 * p.L + j] != 0;
     kept |= (ok ? 1u : 0u) << ci;
   }
 
@@ -208,11 +199,9 @@ attention_axial_kernel(const __grid_constant__ CUtensorMap tm64, const __grid_co
 #pragma unroll
   for (int rh = 0; rh < 2; ++rh) {
     const int r = warp * 16 + (lane >> 2) + 8 * rh;
-    int ip, j, ib;
-    decode(r, ip, j, ib);
-    const int pp = p0 + ip, bb = b0 + ib;
-    if (r >= rows || pp >= p.G || bb >= p.B) continue;
-    __nv_bfloat16* op = p.out + (((long long)bb * p.L + j) * p.G + pp) * p.I + h * DH + 2 * (lane & 3);
+    const int ip = r % p.sp, j = r / p.sp, pp = p0 + ip;
+    if (r >= rows || pp >= p.G) continue;
+    __nv_bfloat16* op = p.out + (((long long)b0 * p.L + j) * p.G + pp) * p.I + h * DH + 2 * (lane & 3);
 #pragma unroll
     for (int c = 0; c < N64; ++c)
 #pragma unroll
@@ -229,7 +218,7 @@ attention_axial_kernel(const __grid_constant__ CUtensorMap tm64, const __grid_co
 }
 
 // Tensor maps over the 4-D view (column, p, j, b) of qkv: boxes of 64 columns (128B swizzle) and 16 columns (32B
-// swizzle) by SP x L x SB tokens.  A kind the head does not use gets a copy of the other (never read).
+// swizzle) by SP x L x 1 tokens.  A kind the head does not use gets a copy of the other (never read).
 template <int DH>
 static int launch_axial_t(const void* qkv, const AxialParams& p, int H, int tiles, cudaStream_t stream) {
   using S = AxialSmem<DH>;
@@ -237,8 +226,8 @@ static int launch_axial_t(const void* qkv, const AxialParams& p, int H, int tile
   const uint64_t ld = (uint64_t)3 * p.I;
   const uint64_t dims[4] = {ld, (uint64_t)p.G, (uint64_t)p.L, (uint64_t)p.B};
   const uint64_t strides[3] = {ld * 2, ld * 2 * p.G, ld * 2 * p.G * p.L};
-  const uint32_t box64[4] = {64, (uint32_t)p.sp, (uint32_t)p.L, (uint32_t)p.sb};
-  const uint32_t box16[4] = {16, (uint32_t)p.sp, (uint32_t)p.L, (uint32_t)p.sb};
+  const uint32_t box64[4] = {64, (uint32_t)p.sp, (uint32_t)p.L, 1};
+  const uint32_t box16[4] = {16, (uint32_t)p.sp, (uint32_t)p.L, 1};
   int rc = 0;
   if (S::N64) rc = encode_tmap_bf16(&tm[0], qkv, 4, dims, strides, box64);
   if (!rc && S::N16) rc = encode_tmap_bf16_sw(&tm[1], qkv, 4, dims, strides, box16, 32);
@@ -275,9 +264,8 @@ extern "C" int b200vit_attention_axial(const void* qkv, void* out, const uint8_t
   p.G = G;
   p.I = H * dh;
   p.sp = G < AX_ROWS / L ? G : AX_ROWS / L;
-  p.sb = B < AX_ROWS / (L * p.sp) ? B : AX_ROWS / (L * p.sp);
   p.tiles_p = (G + p.sp - 1) / p.sp;
-  const long long tiles = (long long)p.tiles_p * ((B + p.sb - 1) / p.sb);
+  const long long tiles = (long long)p.tiles_p * B;
   B200_CHECK_ARG(tiles <= 0x7fffffffLL, "attention_axial: %lld tiles exceed the grid", tiles);
   p.scale_log2e = scale * 1.4426950408889634f;
   p.zero_masked_rows = zero_masked_rows != 0;

@@ -137,26 +137,26 @@ attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     const int st = u & 1;
     const bool second = u >= nblocks;
     uint8_t* sb = smem + L.stage_off + st * L.stage;
-    const int row = seq_start + (second ? u - nblocks : u) * HM_KB;
+    const int tok = (second ? u - nblocks : u) * HM_KB, z = blockIdx.z;
     mbar_arrive_expect_tx(&full[st], kbytes + (second ? vbytes : 0));
     for (int h = 0; h < H; ++h) {
 #pragma unroll
       for (int c = 0; c < N64; ++c)
-        tma_load_2d(sb + (h * N64 + c) * HM_KB * 128, &tmKV, &full[st], p.I + h * DH + 64 * c, row);
+        tma_load_3d(sb + (h * N64 + c) * HM_KB * 128, &tmKV, &full[st], p.I + h * DH + 64 * c, tok, z);
 #pragma unroll
       for (int c = 0; c < N16; ++c)
-        tma_load_2d(sb + L.k16 + (h * N16 + c) * HM_KB * 32, &tmKV16, &full[st], p.I + h * DH + 64 * N64 + 16 * c,
-                    row);
+        tma_load_3d(sb + L.k16 + (h * N16 + c) * HM_KB * 32, &tmKV16, &full[st], p.I + h * DH + 64 * N64 + 16 * c,
+                    tok, z);
     }
     if (second)
       for (int j = 0; j < nv; ++j) {
         const int col = 2 * p.I + (hv0 + j) * DH;
 #pragma unroll
         for (int c = 0; c < N64; ++c)
-          tma_load_2d(sb + L.v64 + (j * N64 + c) * HM_KB * 128, &tmKV, &full[st], col + 64 * c, row);
+          tma_load_3d(sb + L.v64 + (j * N64 + c) * HM_KB * 128, &tmKV, &full[st], col + 64 * c, tok, z);
 #pragma unroll
         for (int c = 0; c < N16; ++c)
-          tma_load_2d(sb + L.v16 + (j * N16 + c) * HM_KB * 32, &tmKV16, &full[st], col + 64 * N64 + 16 * c, row);
+          tma_load_3d(sb + L.v16 + (j * N16 + c) * HM_KB * 32, &tmKV16, &full[st], col + 64 * N64 + 16 * c, tok, z);
       }
   };
 
@@ -192,11 +192,11 @@ attention_headmix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     for (int h = 0; h < H; ++h) {
 #pragma unroll
       for (int c = 0; c < N64; ++c)
-        tma_load_2d(smem + (h * N64 + c) * HM_ROWS * 128, &tmQ, qbar, h * DH + 64 * c, seq_start + q0);
+        tma_load_3d(smem + (h * N64 + c) * HM_ROWS * 128, &tmQ, qbar, h * DH + 64 * c, q0, blockIdx.z);
 #pragma unroll
       for (int c = 0; c < N16; ++c)
-        tma_load_2d(smem + L.q16 + (h * N16 + c) * HM_ROWS * 32, &tmQ16, qbar, h * DH + 64 * N64 + 16 * c,
-                    seq_start + q0);
+        tma_load_3d(smem + L.q16 + (h * N16 + c) * HM_ROWS * 32, &tmQ16, qbar, h * DH + 64 * N64 + 16 * c, q0,
+                    blockIdx.z);
     }
     issue(0);
     issue(1);  // 2 nblocks >= 2 loads
@@ -491,16 +491,20 @@ static int launch_headmix_t(const void* qkv, int B, const HeadmixParams& p, cuda
   const HmSmem L(DH, p.H, HC, 2 * G, PRE);
   B200_CHECK_ARG(L.bytes <= 227 * 1024, "attention_headmix: H=%d dh=%d needs %d bytes of shared memory", p.H, DH,
                  L.bytes);
+  // the [B][N][3 I] view (column, token, sequence): boxes past the end of a sequence are zero-filled, so that a
+  // sequence never reads another's rows (0 x NaN in O += P'' V would be NaN)
   CUtensorMap tm[4];
-  const uint64_t dims[2] = {(uint64_t)3 * p.I, (uint64_t)B * p.N};
-  const uint64_t strides[1] = {(uint64_t)3 * p.I * 2};
-  const uint32_t qbox[2] = {64, HM_ROWS}, kvbox[2] = {64, HM_KB}, qbox16[2] = {16, HM_ROWS}, kvbox16[2] = {16, HM_KB};
+  const uint64_t ld = (uint64_t)3 * p.I;
+  const uint64_t dims[3] = {ld, (uint64_t)p.N, (uint64_t)B};
+  const uint64_t strides[2] = {ld * 2, ld * 2 * p.N};
+  const uint32_t qbox[3] = {64, HM_ROWS, 1}, kvbox[3] = {64, HM_KB, 1}, qbox16[3] = {16, HM_ROWS, 1},
+                 kvbox16[3] = {16, HM_KB, 1};
   constexpr bool has64 = DH / 64 > 0, has16 = (DH % 64) / 16 > 0;
   int rc = 0;
-  if (has64) rc = encode_tmap_bf16(&tm[0], qkv, 2, dims, strides, qbox);
-  if (!rc && has64) rc = encode_tmap_bf16(&tm[1], qkv, 2, dims, strides, kvbox);
-  if (!rc && has16) rc = encode_tmap_bf16_sw(&tm[2], qkv, 2, dims, strides, qbox16, 32);
-  if (!rc && has16) rc = encode_tmap_bf16_sw(&tm[3], qkv, 2, dims, strides, kvbox16, 32);
+  if (has64) rc = encode_tmap_bf16(&tm[0], qkv, 3, dims, strides, qbox);
+  if (!rc && has64) rc = encode_tmap_bf16(&tm[1], qkv, 3, dims, strides, kvbox);
+  if (!rc && has16) rc = encode_tmap_bf16_sw(&tm[2], qkv, 3, dims, strides, qbox16, 32);
+  if (!rc && has16) rc = encode_tmap_bf16_sw(&tm[3], qkv, 3, dims, strides, kvbox16, 32);
   if (rc) return rc;
   if (!has16) tm[2] = tm[0], tm[3] = tm[1];
   if (!has64) tm[0] = tm[2], tm[1] = tm[3];
