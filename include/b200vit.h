@@ -281,7 +281,7 @@ int b200vit_attn_pool(const void* kv, const float* qn, const int32_t* cu_seqlens
  *   ctx_kv: [k | v] rows 2*H*dh wide (row stride ctx_ld); image b's rows start at row b*ctx_rows_per_image + ctx_first
  *   (a kv GEMM over every row of the other stream, its cls rows skipped with ctx_first = 1).
  *   out: bf16 [B, H*dh], row stride ldo.
- * n = 0..16384 (n = 0: out = v_self), dh = 32, 64, 80 or 128; softmax in fp32.  One CTA of 8 warps per (image, head):
+ * n = 0..16384 (n = 0: out = v_self), dh = 32, 48, 64, 80 or 128; softmax in fp32.  One CTA of 8 warps per (image, head):
  * the NaViT pooling kernel above with a per-image bf16 query and a strided context.  ctx_ld and ldo multiples of 8,
  * pointers 16-byte aligned; ctx_kv may be NULL when n = 0.
  */
@@ -334,6 +334,36 @@ int b200vit_attention_headmix_ex(const void* qkv, void* out, int B, int N, int H
 int b200vit_attention_cls_headmix(const void* qkv_self, const void* ctx_kv, int64_t ctx_ld, int64_t ctx_rows_per_image,
                                   int ctx_first, int n, void* out, int64_t ldo, int B, int H, int dh, float scale,
                                   const float* pre, const float* post, void* stream);
+
+/*
+ * Cross-covariance attention (XCiT's XCA, xcit.py:109-148): attention over the dh channels of each head, not over its
+ * tokens.  qkv[B*N, 3*H*dh] bf16 packed as for b200vit_attention; tau: device fp32 [H] (temperature.exp()).  For image
+ * b and head h, with q, k, v its [N, dh] slices:
+ *   G = q^T k,  A_ij = softmax_j(tau_h G_ij / (max(|q_:,i|, 1e-12) max(|k_:,j|, 1e-12))),  out_ni = sum_j A_ij v_nj
+ * (F.normalize's eps rule: an all-zero q or k column gives zero scores, never NaN).  out[B*N, H*dh] bf16, (h d) column
+ * order.  The cost is linear in N; accumulation, norms and softmax are fp32 with fixed summation orders and no atomics,
+ * so repeated calls give the same bits.  One CTA per (image, head).  N = 1..16384, dh = 32, 48, 64, 80 or 128,
+ * H*dh a multiple of 8, qkv and out 16-byte aligned.
+ */
+int b200vit_attention_xca(const void* qkv, const float* tau, void* out, int B, int N, int H, int dh, void* stream);
+
+/*
+ * Local patch interaction (XCiT's LPI, xcit.py:150-167) over B images of gh x gw tokens, out of place:
+ *   y = x + conv2'(GELU(conv1'(LayerNorm(x))))
+ * x, y: fp32 [B*gh*gw, D], token (b, r, c) at row b*gh*gw + r*gw + c; y must not overlap x (every token reads its
+ * neighbours' rows of x).  LayerNorm: ln_gamma, ln_beta [D], ln_eps.  conv1', conv2': depthwise k x k, zero padding
+ * k / 2, weights w1, w2 fp32 [k*k][D] (tap dy*k + dx major, channel minor) and biases b1, b2 [D]; the caller folds
+ * BatchNorm (eval) into conv1' and LayerScale into conv2'.  Both paddings are zeros of the padded tensor: of the
+ * LayerNorm output for conv1', of the GELU output for conv2'.  GELU is the erf form.
+ * y_bf16 [M, D] bf16 and y_stats [M][2] fp32 (both, or both NULL): the bf16 copy of y and per row the (sum, sum of
+ * squares) of that copy, exactly as b200vit_rowstats_cast writes them, for an LN-folded GEMM on y.
+ * ln_scratch: fp32 [M][2] scratch (the LayerNorm statistics of x), overwritten.  k = 1, 3, 5 or 7; D a multiple of 4;
+ * x, y 16-byte aligned, y_bf16 8-byte aligned.
+ */
+int b200vit_local_patch_interaction(const float* x, float* y, void* y_bf16, float* y_stats, float* ln_scratch,
+                                    const float* ln_gamma, const float* ln_beta, float ln_eps, const float* w1,
+                                    const float* b1, const float* w2, const float* b2, int B, int gh, int gw, int D,
+                                    int k, void* stream);
 
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */

@@ -36,6 +36,7 @@ SYMBOLS = [
     "b200vit_attention_axial", "b200vit_embed_tokens_grouped", "b200vit_patchify_spt_ln", "b200vit_attention_ex",
     "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex", "b200vit_attention_cls",
     "b200vit_attention_headmix", "b200vit_attention_headmix_ex", "b200vit_attention_cls_headmix",
+    "b200vit_attention_xca", "b200vit_local_patch_interaction",
 ]
 
 
@@ -123,6 +124,11 @@ def lib() -> C.CDLL:
     L.b200vit_attention_headmix_ex.argtypes = [vp, vp, i32, i32, i32, i32, f32, vp, vp, vp, vp, f32, vp]
     L.b200vit_attention_cls_headmix.restype = i32
     L.b200vit_attention_cls_headmix.argtypes = [vp, vp, i64, i64, i32, i32, vp, i64, i32, i32, i32, f32, vp, vp, vp]
+    L.b200vit_attention_xca.restype = i32
+    L.b200vit_attention_xca.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp]
+    L.b200vit_local_patch_interaction.restype = i32
+    L.b200vit_local_patch_interaction.argtypes = [vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, vp, vp, i32, i32, i32, i32,
+                                                  i32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -717,6 +723,47 @@ def attention_cls_headmix(qkv_self: torch.Tensor, ctx: Optional[torch.Tensor], o
                                                  int(rows_per_image), int(first), int(n), _ptr(out), out.stride(0), B,
                                                  H, dh, float(scale), _ptr(pre), _ptr(post), _stream())
     _check(rc, "b200vit_attention_cls_headmix")
+
+
+def attention_xca(qkv: torch.Tensor, tau: torch.Tensor, out: torch.Tensor, B: int, N: int, H: int, dh: int) -> None:
+    """Cross-covariance attention over the channels of every head (XCiT): qkv[B*N, 3*H*dh] packed q | k | v, tau fp32
+    [H] (temperature.exp()), out[B*N, H*dh]."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(tau, torch.float32, "tau"); _chk(out, torch.bfloat16, "out")
+    assert qkv.is_contiguous() and out.is_contiguous() and tau.is_contiguous() and tau.numel() == H
+    assert qkv.shape == (B * N, 3 * H * dh) and out.shape == (B * N, H * dh)
+    with _Timed("attention_xca", B=B, N=N, H=H, bytes=(qkv.numel() + out.numel()) * 2, flops=4.0 * B * H * N * dh * dh):
+        rc = lib().b200vit_attention_xca(_ptr(qkv), _ptr(tau), _ptr(out), B, N, H, dh, _stream())
+    _check(rc, "b200vit_attention_xca")
+
+
+def local_patch_interaction(x: torch.Tensor, y: torch.Tensor, ln_scratch: torch.Tensor, ln: tuple, w1: torch.Tensor,
+                            b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor, B: int, gh: int, gw: int, k: int,
+                            y_bf16: Optional[torch.Tensor] = None, y_stats: Optional[torch.Tensor] = None) -> None:
+    """y = x + conv2'(GELU(conv1'(LayerNorm(x)))) on B grids of gh x gw tokens of x fp32 [B*gh*gw, D] (XCiT's LPI).
+    ln = (gamma, beta, eps); w1, w2 fp32 [k*k, D] tap-major depthwise weights, BatchNorm folded into w1 / b1 and
+    LayerScale into w2 / b2.  y_bf16 / y_stats [M, 2]: the bf16 copy of y and its rowstats_cast statistics.
+    ln_scratch fp32 [M, 2] is overwritten."""
+    g, bt, eps = ln
+    for nm, t in (("x", x), ("y", y), ("ln_scratch", ln_scratch), ("ln gamma", g), ("ln beta", bt), ("w1", w1),
+                  ("b1", b1), ("w2", w2), ("b2", b2), ("y_stats", y_stats)):
+        _chk(t, torch.float32, nm)
+    _chk(y_bf16, torch.bfloat16, "y_bf16")
+    M, D = x.shape
+    assert M == B * gh * gw and y.shape == x.shape and x.is_contiguous() and y.is_contiguous()
+    assert ln_scratch.is_contiguous() and ln_scratch.numel() >= 2 * M
+    for t in (g, bt, b1, b2):
+        assert t.is_contiguous() and t.numel() == D
+    for t in (w1, w2):
+        assert t.is_contiguous() and t.shape == (k * k, D)
+    assert (y_bf16 is None) == (y_stats is None)
+    assert y_bf16 is None or (y_bf16.is_contiguous() and y_bf16.shape == x.shape and y_stats.is_contiguous()
+                              and y_stats.numel() == 2 * M)
+    with _Timed("local_patch_interaction", B=B, h=gh, w=gw, D=D, k=k,
+                bytes=M * D * (4 + 4 + (2 if y_bf16 is not None else 0))):
+        rc = lib().b200vit_local_patch_interaction(_ptr(x), _ptr(y), _ptr(y_bf16), _ptr(y_stats), _ptr(ln_scratch),
+                                                   _ptr(g), _ptr(bt), float(eps), _ptr(w1), _ptr(b1), _ptr(w2),
+                                                   _ptr(b2), B, gh, gw, D, int(k), _stream())
+    _check(rc, "b200vit_local_patch_interaction")
 
 
 def mean_pool(x: torch.Tensor, out: torch.Tensor, B: int, N: int, D: int, n_pool: Optional[int] = None) -> None:

@@ -402,4 +402,78 @@ __device__ __forceinline__ void gelu_erf2(float& a, float& b) {
   f2_get(f2_mul(x, f2_make(fast_rcp(d0), fast_rcp(d1))), a, b);
 }
 
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// One warp: mean and 1 / sqrt(var + eps) of the fp32 row xr[D], two-pass variance with eps inside the sqrt (the
+// semantics of torch.nn.LayerNorm).
+__device__ __forceinline__ void ln_row_stats(const float* __restrict__ xr, int D, int lane, float& mean, float& rstd,
+                                             float eps) {
+  float s = 0.f;
+  if ((D & 3) == 0) {
+    for (int i = lane * 4; i < D; i += 128) {
+      const float4 v = *reinterpret_cast<const float4*>(xr + i);
+      s += (v.x + v.y) + (v.z + v.w);
+    }
+  } else {
+    for (int i = lane; i < D; i += 32) s += xr[i];
+  }
+  mean = warp_sum(s) / (float)D;
+  float q = 0.f;
+  if ((D & 3) == 0) {
+    for (int i = lane * 4; i < D; i += 128) {
+      const float4 v = *reinterpret_cast<const float4*>(xr + i);
+      const float a = v.x - mean, b = v.y - mean, c = v.z - mean, d = v.w - mean;
+      q += (a * a + b * b) + (c * c + d * d);
+    }
+  } else {
+    for (int i = lane; i < D; i += 32) {
+      const float a = xr[i] - mean;
+      q += a * a;
+    }
+  }
+  rstd = rsqrtf(warp_sum(q) / (float)D + eps);
+}
+
+// One warp: fp32 row xr[D] -> its bf16 copy br[D] and, written by lane 0, st[0] = sum and st[1] = sum of squares of
+// the bf16-ROUNDED values: the row statistics the LN-folded GEMMs read (b200vit_rowstats_cast).  Every kernel that
+// hands such statistics to a folded GEMM goes through this function, so they are the same bits whoever writes them.
+__device__ __forceinline__ void rowstats_cast_row(const float* __restrict__ xr, __nv_bfloat16* __restrict__ br,
+                                                  float* __restrict__ st, int D, int lane) {
+  float s1 = 0.f, s2 = 0.f;
+  if ((D & 3) == 0) {
+    for (int i = lane * 4; i < D; i += 128) {
+      const float4 v = *reinterpret_cast<const float4*>(xr + i);
+      uint2 pk;
+      pk.x = pack_bf16x2(v.x, v.y);
+      pk.y = pack_bf16x2(v.z, v.w);
+      *reinterpret_cast<uint2*>(br + i) = pk;
+      const float a0 = __uint_as_float(pk.x << 16), a1 = __uint_as_float(pk.x & 0xFFFF0000u);
+      const float a2 = __uint_as_float(pk.y << 16), a3 = __uint_as_float(pk.y & 0xFFFF0000u);
+      s1 += (a0 + a1) + (a2 + a3);
+      s2 = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, fmaf(a3, a3, s2))));
+    }
+  } else {
+    for (int i = lane; i < D; i += 32) {
+      const __nv_bfloat16 vb = __float2bfloat16_rn(xr[i]);
+      br[i] = vb;
+      const float vr = __bfloat162float(vb);
+      s1 += vr;
+      s2 = fmaf(vr, vr, s2);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+  }
+  if (lane == 0) {
+    st[0] = s1;
+    st[1] = s2;
+  }
+}
+
 }  // namespace b200

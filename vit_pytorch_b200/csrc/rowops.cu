@@ -6,43 +6,9 @@
 
 namespace b200 {
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// LayerNorm: x fp32 [*, D] -> bf16 and/or fp32
+// LayerNorm: x fp32 [*, D] -> bf16 and/or fp32 (row statistics: ln_row_stats, common.cuh)
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ln_row_stats(const float* __restrict__ xr, int D, int lane, float& mean, float& rstd,
-                                             float eps) {
-  float s = 0.f;
-  if ((D & 3) == 0) {
-    for (int i = lane * 4; i < D; i += 128) {
-      const float4 v = *reinterpret_cast<const float4*>(xr + i);
-      s += (v.x + v.y) + (v.z + v.w);
-    }
-  } else {
-    for (int i = lane; i < D; i += 32) s += xr[i];
-  }
-  mean = warp_sum(s) / (float)D;
-  float q = 0.f;
-  if ((D & 3) == 0) {
-    for (int i = lane * 4; i < D; i += 128) {
-      const float4 v = *reinterpret_cast<const float4*>(xr + i);
-      const float a = v.x - mean, b = v.y - mean, c = v.z - mean, d = v.w - mean;
-      q += (a * a + b * b) + (c * c + d * d);
-    }
-  } else {
-    for (int i = lane; i < D; i += 32) {
-      const float a = xr[i] - mean;
-      q += a * a;
-    }
-  }
-  rstd = rsqrtf(warp_sum(q) / (float)D + eps);
-}
-
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ gamma,
                  const float* __restrict__ beta, __nv_bfloat16* __restrict__ out_bf16, float* __restrict__ out_f32,
@@ -463,36 +429,7 @@ rowstats_cast_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ xb
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= M) return;
-  const float* xr = x + row * D;
-  __nv_bfloat16* br = xb + row * D;
-  float s1 = 0.f, s2 = 0.f;
-  if ((D & 3) == 0) {
-    for (int i = lane * 4; i < D; i += 128) {
-      const float4 v = *reinterpret_cast<const float4*>(xr + i);
-      uint2 pk;
-      pk.x = pack_bf16x2(v.x, v.y);
-      pk.y = pack_bf16x2(v.z, v.w);
-      *reinterpret_cast<uint2*>(br + i) = pk;
-      const float a0 = __uint_as_float(pk.x << 16), a1 = __uint_as_float(pk.x & 0xFFFF0000u);
-      const float a2 = __uint_as_float(pk.y << 16), a3 = __uint_as_float(pk.y & 0xFFFF0000u);
-      s1 += (a0 + a1) + (a2 + a3);
-      s2 = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, fmaf(a3, a3, s2))));
-    }
-  } else {
-    for (int i = lane; i < D; i += 32) {
-      const __nv_bfloat16 vb = __float2bfloat16_rn(xr[i]);
-      br[i] = vb;
-      const float vr = __bfloat162float(vb);
-      s1 += vr;
-      s2 = fmaf(vr, vr, s2);
-    }
-  }
-  s1 = warp_sum(s1);
-  s2 = warp_sum(s2);
-  if (lane == 0) {
-    stats[2 * row] = s1;
-    stats[2 * row + 1] = s2;
-  }
+  rowstats_cast_row(x + row * D, xb + row * D, stats + 2 * row, D, lane);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1043,7 +980,8 @@ extern "C" int b200vit_attention_cls(const void* qkv_self, const void* ctx_kv, i
                                      int H, int dh, float scale, void* stream) {
   B200_CHECK_ARG(qkv_self && out && (ctx_kv || n == 0), "attention_cls: null pointer");
   B200_CHECK_ARG(B > 0 && H > 0, "attention_cls: bad shape B=%d H=%d", B, H);
-  B200_CHECK_ARG(head_width_ok(dh), "attention_cls: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
+  B200_CHECK_ARG(head_width_ok(dh) || dh == 48,
+                 "attention_cls: dim_head=%d not supported by this build (32, 48, 64, 80 or 128)", dh);
   B200_CHECK_ARG(n >= 0 && n <= 16384, "attention_cls: n=%d context rows out of range [0, 16384]", n);
   B200_CHECK_ARG(ctx_first >= 0 && ctx_rows_per_image >= (int64_t)ctx_first + n,
                  "attention_cls: context rows [%d, %d) exceed the %lld rows per image", ctx_first, ctx_first + n,
@@ -1065,6 +1003,10 @@ extern "C" int b200vit_attention_cls(const void* qkv_self, const void* ctx_kv, i
   switch (dh) {
     case 32:
       attn_pool_kernel<32, true><<<B * H, 256, 0, st>>>(k, nullptr, nullptr, o, B, H, q, ld, rows, ctx_first, n, lo,
+                                                        scale);
+      break;
+    case 48:
+      attn_pool_kernel<48, true><<<B * H, 256, 0, st>>>(k, nullptr, nullptr, o, B, H, q, ld, rows, ctx_first, n, lo,
                                                         scale);
       break;
     case 80:

@@ -130,6 +130,8 @@ def common_reason(owner: nn.Module, x: torch.Tensor, *, encoders=(), dropout_p: 
 HEAD_WIDTHS = (32, 64, 80, 128)
 HEADMIX_WIDTHS = (32, 48, 64, 80, 128)     # b200vit_attention_headmix
 HEADMIX_MAX_HEADS, HEADMIX_MAX_INNER = 16, 1024
+XCA_WIDTHS = (32, 48, 64, 80, 128)         # b200vit_attention_xca
+LPI_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_local_patch_interaction
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -148,6 +150,24 @@ def headmix_reason(heads: int, dh: int) -> Optional[str]:
     if heads > HEADMIX_MAX_HEADS or heads * dh > HEADMIX_MAX_INNER:
         return (f"heads={heads} x dim_head={dh} (the head-mixing attention kernel takes at most "
                 f"{HEADMIX_MAX_HEADS} heads and heads * dim_head <= {HEADMIX_MAX_INNER})")
+    return None
+
+
+def xca_reason(dh: int) -> Optional[str]:
+    """None if b200vit_attention_xca is built for heads `dh` wide, else the reason the eager PyTorch graph is used."""
+    if dh not in XCA_WIDTHS:
+        return f"dim_head={dh} (the cross-covariance attention kernel is built for 32, 48, 64, 80 and 128)"
+    return None
+
+
+def lpi_reason(kernel_size: int, grid_w: int) -> Optional[str]:
+    """None if b200vit_local_patch_interaction runs a k x k kernel over grid rows of `grid_w` tokens, else the reason
+    the eager PyTorch graph is used.  The kernel keeps (3k - 1) padded grid rows of at least 4 channels in 100 KB of
+    shared memory."""
+    if kernel_size not in LPI_KERNEL_SIZES:
+        return f"local_patch_kernel_size={kernel_size} (the local patch interaction kernel is built for 1, 3, 5 and 7)"
+    if (3 * kernel_size - 1) * (grid_w + 2 * (kernel_size // 2)) * 4 * 4 > 100 * 1024:
+        return f"a grid row of {grid_w} tokens is too wide for the local patch interaction kernel"
     return None
 
 
@@ -178,6 +198,41 @@ class HeadMix(NamedTuple):
     post: torch.Tensor                            # [heads, heads]
     ln: Optional[Norm]                            # over `heads` values, or None
     pre: Optional[torch.Tensor] = None            # [heads, heads], or None
+
+
+class LPIBlock(NamedTuple):
+    """XCiT's local patch interaction between the attention and the feed-forward block (xcit.py:150-167, 208-211), on
+    the h x w token grid:  x += scale * conv2(GELU(BatchNorm(conv1(LN(x))))), conv1 / conv2 depthwise k x k with zero
+    padding k // 2 (b200vit_local_patch_interaction).  BatchNorm runs on its running statistics (eval)."""
+    ln: Norm
+    conv1_w: torch.Tensor                         # [D, 1, k, k]
+    conv1_b: Optional[torch.Tensor]
+    bn_w: torch.Tensor
+    bn_b: torch.Tensor
+    bn_mean: torch.Tensor                         # running_mean, a buffer
+    bn_var: torch.Tensor                          # running_var, a buffer
+    bn_eps: float
+    conv2_w: torch.Tensor                         # [D, 1, k, k]
+    conv2_b: Optional[torch.Tensor]
+    scale: Optional[torch.Tensor]                 # LayerScale [D], or None
+    kernel_size: int
+
+
+def lpi_weights(P: LPIBlock) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(w1, b1, w2, b2) fp32 of b200vit_local_patch_interaction: BatchNorm (eval) folded into conv1,
+        w1' = w1 g / sqrt(var + eps),  b1' = (b1 - mean) g / sqrt(var + eps) + beta,
+    LayerScale s into conv2, w2' = s w2, b2' = s b2 (all per channel: the convolutions are depthwise); the weights
+    tap-major [k*k, D]."""
+    D, kk = P.conv1_w.shape[0], P.kernel_size * P.kernel_size
+    f = lambda t: t.detach().float()                                                    # noqa: E731
+    zeros = torch.zeros(D, device=P.conv1_w.device, dtype=torch.float32)
+    inv = f(P.bn_w) / torch.sqrt(f(P.bn_var) + P.bn_eps)
+    w1 = f(P.conv1_w).reshape(D, kk) * inv[:, None]
+    b1 = ((f(P.conv1_b) if P.conv1_b is not None else zeros) - f(P.bn_mean)) * inv + f(P.bn_b)
+    s = f(P.scale).reshape(D) if P.scale is not None else torch.ones_like(zeros)
+    w2 = f(P.conv2_w).reshape(D, kk) * s[:, None]
+    b2 = (f(P.conv2_b) if P.conv2_b is not None else zeros) * s
+    return w1.t().contiguous(), b1.contiguous(), w2.t().contiguous(), b2.contiguous()
 
 
 @dataclass
@@ -211,6 +266,11 @@ class EncoderLayer:
     # residual adds, folded into the rows and biases of out_w and fc2_w
     out_scale: Optional[torch.Tensor] = None
     ff_scale: Optional[torch.Tensor] = None
+    # cross-covariance attention (XCiT, xcit.py:109-148): the per-head temperature parameter [heads, 1, 1]; the
+    # attention runs b200vit_attention_xca with tau = exp(xca_tau), read when the prepared weights are rebuilt
+    xca_tau: Optional[torch.Tensor] = None
+    # local patch interaction between the attention and the feed-forward block (XCiT); run_blocks needs `grid`
+    lpi: Optional[LPIBlock] = None
 
 
 class _Prepared:
@@ -347,12 +407,20 @@ class TransformerEngine:
         self.rows: Dict[tuple, torch.Tensor] = {}      # cls_row_index of the shapes pool() has seen
 
     def params(self) -> List[torch.Tensor]:
-        return list(self.mod.parameters())
+        """What the prepared weights are built from: the module's parameters and the buffers it names in
+        `prepared_buffers()` (BatchNorm running statistics), so an in-place update of either rebuilds them."""
+        extra = getattr(self.mod, "prepared_buffers", None)
+        return list(self.mod.parameters()) + (list(extra()) if extra is not None else [])
 
     def unsupported_reason(self, N: int) -> Optional[str]:
         # only shapes are read, and a module's shapes are fixed at construction: any description of it serves
         for L in self.layers or self.mod.encoder_layers()[0]:
-            r = head_width_reason(L.dim_head) if L.headmix is None else headmix_reason(L.heads, L.dim_head)
+            if L.xca_tau is not None:
+                r = xca_reason(L.dim_head)
+            else:
+                r = head_width_reason(L.dim_head) if L.headmix is None else headmix_reason(L.heads, L.dim_head)
+            if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
+                r = lpi_reason(L.lpi.kernel_size, 1)
             if r is not None:
                 return r
             if L.qkv_w.shape[1] % 8 or L.fc1_w.shape[0] % 8:
@@ -397,6 +465,12 @@ class TransformerEngine:
                     t[f"{i}.pre"] = _f32(X.pre)
                 if X.ln is not None:
                     t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(X.ln.gamma), _f32(X.ln.beta)
+            if L.xca_tau is not None:
+                t[f"{i}.tau"] = L.xca_tau.detach().float().exp().reshape(-1).contiguous()
+            if L.lpi is not None:
+                P = L.lpi
+                t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"] = _f32(P.ln.gamma), _f32(P.ln.beta)
+                t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"], t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"] = lpi_weights(P)
             t[f"{i}.ln2.w"], t[f"{i}.ln2.b"] = _f32(L.ln2.gamma), _f32(L.ln2.beta)
             _fold(t, f"{i}.fc1", L.fc1_w, L.fc1_b, L.ln2)
             t[f"{i}.fc1.w"], t[f"{i}.fc1.b"] = _bf16_rows(L.fc1_w), _f32(L.fc1_b)
@@ -410,13 +484,13 @@ class TransformerEngine:
     def _c_layers(self, t: Dict[str, torch.Tensor]):
         """(ctypes array of b200vit_layer, (heads, dh, hidden, scale), layer scales, attention flags) for the one-call
         encoder (b200vit_encoder_blocks), or None when it cannot run these layers: they are not uniform, one has a
-        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block or heads mixed across the
-        head axis.  Layer scales: None when
+        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block, heads mixed across the
+        head axis, cross-covariance attention or a local patch interaction.  Layer scales: None when
         every layer has the same scale, else a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned
         temperatures).  The pointers stay valid as long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
-        if any(L.qk_norm == "ln" or L.temporal is not None or L.headmix is not None or sig(L) != sig(self.layers[0])
-               for L in self.layers):
+        if any(L.qk_norm == "ln" or L.temporal is not None or L.headmix is not None or L.xca_tau is not None
+               or L.lpi is not None or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -460,6 +534,11 @@ class TransformerEngine:
                 "stats_a": torch.empty(M, _lib.stats_parts(D), 2, device=device, dtype=torch.float32),
                 "stats_b": torch.empty(M, _lib.stats_parts(D), 2, device=device, dtype=torch.float32),
             }
+            if any(L.lpi is not None for L in self.layers):
+                # the local patch interaction's output stream, its row statistics and its LayerNorm scratch
+                slot.t["y"] = torch.empty(M, D, device=device, dtype=torch.float32)
+                slot.t["stats_l"] = torch.empty(M, 2, device=device, dtype=torch.float32)
+                slot.t["lnst"] = torch.empty(M, 2, device=device, dtype=torch.float32)
             w = slot.t
             slot.c = _lib.EncoderWs(w["xn"].data_ptr(), w["qkv"].data_ptr(), w["o"].data_ptr(), w["h"].data_ptr(),
                                     w["stats_in"].data_ptr(), w["stats_a"].data_ptr(), w["stats_b"].data_ptr())
@@ -483,7 +562,7 @@ class TransformerEngine:
                    varlen: Optional[_lib.VarlenIndex] = None,
                    rope: Optional[Tuple[torch.Tensor, int]] = None,
                    axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
-                   layers: Optional[Sequence[int]] = None) -> None:
+                   layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None) -> None:
         """The encoder layers (all, or the indices in `layers`, in order: CaiT's layer dropout, cait.py:14-27), in place
         on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
         B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
@@ -494,6 +573,11 @@ class TransformerEngine:
         sub-block run it there (the factorized layers of ViViT: spatial attention over the B sequences of N tokens,
         G = N); layers without one run their attention there instead of over the B x N sequences (ViViT's masked
         temporal transformer, G = 1).  These calls take the per-kernel loop below.
+        `grid` = (h, w): the token grid of every sequence (N = h*w, token r*w + c), which layers with a local patch
+        interaction need (XCiT).  Such a layer runs
+            QKV GEMM -> attention -> out GEMM (+ residual) -> local patch interaction x -> y (second fp32 stream, its
+            bf16 copy and row statistics) -> fc1 GEMM (+ GELU) on y -> fc2 GEMM with residual y, written to x,
+        so the stream stays in x.
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
         the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
@@ -523,6 +607,10 @@ class TransformerEngine:
                 raise ValueError("a layer with a temporal attention sub-block needs `axial` to address its sequences")
             if L.headmix is not None and (axial is not None or varlen is not None):
                 raise ValueError("head-mixing attention runs over B sequences of N tokens only")
+            if L.xca_tau is not None and (axial is not None or varlen is not None):
+                raise ValueError("cross-covariance attention runs over B sequences of N tokens only")
+            if L.lpi is not None and (grid is None or grid[0] * grid[1] != N or axial is not None or varlen is not None):
+                raise ValueError("a layer with a local patch interaction needs `grid` = (h, w) with h * w == N")
             # xb = LN1(x) -> qkv   (fold: xb already holds the bf16 copy of x; LN1 is applied in the GEMM epilogue)
             if fold:
                 # the first layer that runs reads the entry statistics, every later one those of the last fc2 GEMM
@@ -538,7 +626,9 @@ class TransformerEngine:
                                    dh=L.dim_head, head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None, **ln)
             if rope is not None:
                 _lib.rope_qk(ws["qkv"], rope[0], rope[1], L.heads, L.dim_head)
-            if L.headmix is not None:
+            if L.xca_tau is not None:
+                _lib.attention_xca(ws["qkv"], t[f"{i}.tau"], ws["o"], B, N, L.heads, L.dim_head)
+            elif L.headmix is not None:
                 hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
                 _lib.attention_headmix(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln,
                                        pre=t.get(f"{i}.pre"))
@@ -548,7 +638,17 @@ class TransformerEngine:
                 _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
             else:
                 _lib.attention_varlen(ws["qkv"], ws["o"], *vl, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
-            if fold:
+            # the stream the feed-forward block reads: x, or the local patch interaction's output
+            ff_in = x if L.lpi is None else ws["y"]
+            if fold and L.lpi is not None:
+                # the local patch interaction reads x in fp32 and writes y, its bf16 copy and its row statistics
+                _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
+                self._lpi(t, i, L, x, ws, B, grid, xb, ws["stats_l"])
+                _lib.gemm(xb, t[f"{i}.fc1.wg"], out_bf16=ws["h"], bias=t[f"{i}.fc1.t"], gelu=True,
+                          ln_sums=ws["stats_l"], col_s=t[f"{i}.fc1.s"], ln_eps=L.ln2.eps)
+                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.fc2.b"], resid=ff_in,
+                          stats_out=sa)
+            elif fold:
                 # the residual GEMMs also write the bf16 copy of x and its row statistics for the next folded GEMM
                 _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.out.b"], resid=x,
                           stats_out=sb)
@@ -565,14 +665,25 @@ class TransformerEngine:
                           stats_out=sa)
             else:
                 _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
+                if L.lpi is not None:
+                    self._lpi(t, i, L, x, ws, B, grid)
                 if L.temporal is not None:
                     _lib.layernorm(x, t[f"{i}.tln.w"], t[f"{i}.tln.b"], out_bf16=xb, eps=L.temporal.ln.eps)
                     _lib.gemm(xb, t[f"{i}.tqkv.w"], out_bf16=ws["qkv"])
                     axial_attention(L)
                     _lib.gemm(ws["o"], t[f"{i}.tout.w"], out_f32=x, bias=t[f"{i}.tout.b"], resid=x)
-                _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=xb, eps=L.ln2.eps)
+                _lib.layernorm(ff_in, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=xb, eps=L.ln2.eps)
                 _lib.gemm(xb, t[f"{i}.fc1.w"], out_bf16=ws["h"], bias=t[f"{i}.fc1.b"], gelu=True)
-                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, bias=t[f"{i}.fc2.b"], resid=x)
+                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, bias=t[f"{i}.fc2.b"], resid=ff_in)
+
+    @staticmethod
+    def _lpi(t: Dict[str, torch.Tensor], i: int, L: EncoderLayer, x: torch.Tensor, ws: Dict[str, torch.Tensor], B: int,
+             grid: Tuple[int, int], y_bf16: Optional[torch.Tensor] = None,
+             y_stats: Optional[torch.Tensor] = None) -> None:
+        """ws['y'] = x + local patch interaction of layer i (and, given, its bf16 copy and row statistics)."""
+        _lib.local_patch_interaction(x, ws["y"], ws["lnst"], (t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"], L.lpi.ln.eps),
+                                     t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"], t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"], B,
+                                     grid[0], grid[1], L.lpi.kernel_size, y_bf16=y_bf16, y_stats=y_stats)
 
     def final_norm(self, x: torch.Tensor, *, out_bf16: Optional[torch.Tensor] = None,
                    out_f32: Optional[torch.Tensor] = None, row_index: Optional[torch.Tensor] = None) -> None:
@@ -625,13 +736,13 @@ class TransformerEngine:
 
     def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None,
                        axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
-                       layers: Optional[Sequence[int]] = None) -> torch.Tensor:
+                       layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
-        reference mae.py:74, simmim.py:70, distill.py:66); `rope`, `axial` and `layers` as in run_blocks."""
+        reference mae.py:74, simmim.py:70, distill.py:66); `rope`, `axial`, `layers` and `grid` as in run_blocks."""
         B, N, D = tokens.shape
         with on_device(tokens):
             x = tokens.reshape(B * N, D).float().contiguous()
-            self.run_blocks(x, B, N, rope=rope, axial=axial, layers=layers)
+            self.run_blocks(x, B, N, rope=rope, axial=axial, layers=layers, grid=grid)
             out = torch.empty(B * N, D, device=tokens.device, dtype=torch.bfloat16)
             if self.norm is not None:
                 self.final_norm(x, out_bf16=out)
