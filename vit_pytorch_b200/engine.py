@@ -6,14 +6,14 @@ family.  This file turns them into the flat bf16 / fp32 device buffers the C ABI
 issues the launches on torch's current stream.  Nothing here computes on the host and nothing falls back: a missing
 library or a failing call raises.
 
-Schedule per encoder layer (reference vit.py:78-81), M = B*N token rows, residual stream x kept in fp32:
-    xn  = LayerNorm(x)                         b200vit_layernorm      fp32 -> bf16              (vit.py:52)
-    qkv = xn Wqkv^T                            b200vit_gemm_bf16      wgmma, bf16 out           (vit.py:54)
+Schedule per encoder layer (reference vit.py:78-81) in the default LayerNorm mode, fold (see ln_mode), M = B*N token
+rows, residual stream x in fp32 and xb, its bf16 copy, which the LN-folded GEMMs read with its per-row (sum, sum^2):
+    qkv = LN1(x) Wqkv^T                        b200vit_gemm_bf16      LN-folded, bf16 out       (vit.py:52,54)
     o   = softmax(q k^T * scale) v             b200vit_attention      wgmma, online softmax     (vit.py:55-63)
-    x  += o Wout^T + b                         b200vit_gemm_bf16      residual epilogue, fp32   (vit.py:64,80)
-    xn  = LayerNorm(x)                         b200vit_layernorm                               (vit.py:19)
-    h   = GELU(xn W1^T + b1)                   b200vit_gemm_bf16      bias+GELU epilogue        (vit.py:20-21)
-    x  += h W2^T + b2                          b200vit_gemm_bf16      residual epilogue         (vit.py:23,81)
+    x  += o Wout^T + b                         b200vit_gemm_bf16      residual epilogue, + xb   (vit.py:64,80)
+    h   = GELU(LN2(x) W1^T + b1)               b200vit_gemm_bf16      LN-folded, GELU epilogue  (vit.py:19-21)
+    x  += h W2^T + b2                          b200vit_gemm_bf16      residual epilogue, + xb   (vit.py:23,81)
+exact: b200vit_layernorm (x -> xb) and the plain GEMM in place of each LN-folded one, the reference's operator sequence.
 """
 from __future__ import annotations
 
@@ -273,6 +273,20 @@ class EncoderLayer:
     lpi: Optional[LPIBlock] = None
 
 
+def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
+    """Which kernel runs layer L's attention: 'xca', 'headmix', 'axial' (a run_blocks call with `axial`, unless the
+    layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys) or 'plain'.
+    ValueError for cross-covariance or head-mixing attention with `axial` or over a `packed` batch."""
+    if L.xca_tau is not None or L.headmix is not None:
+        if axial or packed:
+            what = "cross-covariance" if L.xca_tau is not None else "head-mixing"
+            raise ValueError(f"{what} attention runs over B sequences of N tokens only")
+        return "xca" if L.xca_tau is not None else "headmix"
+    if axial and L.temporal is None:
+        return "axial"
+    return "varlen" if key_blocks else "plain"
+
+
 class _Prepared:
     """What was derived from some parameters (usually flat device buffers) + the parameter versions it was built from."""
 
@@ -415,10 +429,9 @@ class TransformerEngine:
     def unsupported_reason(self, N: int) -> Optional[str]:
         # only shapes are read, and a module's shapes are fixed at construction: any description of it serves
         for L in self.layers or self.mod.encoder_layers()[0]:
-            if L.xca_tau is not None:
-                r = xca_reason(L.dim_head)
-            else:
-                r = head_width_reason(L.dim_head) if L.headmix is None else headmix_reason(L.heads, L.dim_head)
+            kernel = attention_kernel(L)
+            r = (xca_reason(L.dim_head) if kernel == "xca" else
+                 headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else head_width_reason(L.dim_head))
             if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
                 r = lpi_reason(L.lpi.kernel_size, 1)
             if r is not None:
@@ -484,13 +497,13 @@ class TransformerEngine:
     def _c_layers(self, t: Dict[str, torch.Tensor]):
         """(ctypes array of b200vit_layer, (heads, dh, hidden, scale), layer scales, attention flags) for the one-call
         encoder (b200vit_encoder_blocks), or None when it cannot run these layers: they are not uniform, one has a
-        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block, heads mixed across the
-        head axis, cross-covariance attention or a local patch interaction.  Layer scales: None when
-        every layer has the same scale, else a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned
-        temperatures).  The pointers stay valid as long as `t` (which holds the tensors)."""
+        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block, an attention kernel other
+        than the plain one or a local patch interaction.  Layer scales: None when every layer has the same scale, else
+        a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned temperatures).  The pointers stay valid as
+        long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
-        if any(L.qk_norm == "ln" or L.temporal is not None or L.headmix is not None or L.xca_tau is not None
-               or L.lpi is not None or sig(L) != sig(self.layers[0]) for L in self.layers):
+        if any(L.qk_norm == "ln" or L.temporal is not None or attention_kernel(L) != "plain" or L.lpi is not None
+               or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -574,10 +587,9 @@ class TransformerEngine:
         G = N); layers without one run their attention there instead of over the B x N sequences (ViViT's masked
         temporal transformer, G = 1).  These calls take the per-kernel loop below.
         `grid` = (h, w): the token grid of every sequence (N = h*w, token r*w + c), which layers with a local patch
-        interaction need (XCiT).  Such a layer runs
-            QKV GEMM -> attention -> out GEMM (+ residual) -> local patch interaction x -> y (second fp32 stream, its
-            bf16 copy and row statistics) -> fc1 GEMM (+ GELU) on y -> fc2 GEMM with residual y, written to x,
-        so the stream stays in x.
+        interaction need (XCiT).  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
+        axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
+        onto that stream, written to x.  The call is checked first: a ValueError leaves x as it was.
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
         the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
@@ -592,98 +604,84 @@ class TransformerEngine:
             _lib.encoder_blocks(arr, len(arr), x, self.slot.c, B, N, x.shape[1], heads, dh, hidden, scale, primed, vl,
                                 rope=rope, layer_scales=layer_scales, attn_flags=flags)
             return
-        xb, sa, sb = ws["xn"], ws["stats_a"], ws["stats_b"]
-        if fold and not primed:
-            _lib.rowstats_cast(x, xb, ws["stats_in"])
-        def axial_attention(L: EncoderLayer) -> None:
-            G, Lt, key_mask, zero = axial
-            _lib.attention_axial(ws["qkv"], ws["o"], key_mask, x.shape[0] // (Lt * G), Lt, G, L.heads, L.dim_head,
-                                 L.scale, zero)
-
         run = range(len(self.layers)) if layers is None else layers
-        for k, i in enumerate(run):
+        kernels = []
+        for i in run:
             L = self.layers[i]
             if L.temporal is not None and axial is None:
                 raise ValueError("a layer with a temporal attention sub-block needs `axial` to address its sequences")
-            if L.headmix is not None and (axial is not None or varlen is not None):
-                raise ValueError("head-mixing attention runs over B sequences of N tokens only")
-            if L.xca_tau is not None and (axial is not None or varlen is not None):
-                raise ValueError("cross-covariance attention runs over B sequences of N tokens only")
+            kernels.append(attention_kernel(L, axial is not None, varlen is not None, vl is not None))
             if L.lpi is not None and (grid is None or grid[0] * grid[1] != N or axial is not None or varlen is not None):
                 raise ValueError("a layer with a local patch interaction needs `grid` = (h, w) with h * w == N")
-            # xb = LN1(x) -> qkv   (fold: xb already holds the bf16 copy of x; LN1 is applied in the GEMM epilogue)
-            if fold:
-                # the first layer that runs reads the entry statistics, every later one those of the last fc2 GEMM
-                w, ln = t[f"{i}.qkv.wg"], dict(bias=t[f"{i}.qkv.t"], ln_sums=ws["stats_in"] if k == 0 else sa,
-                                               col_s=t[f"{i}.qkv.s"], ln_eps=L.ln1.eps)
-            else:
-                _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
-                w, ln = t[f"{i}.qkv.w"], {}
-            if L.qk_norm is None:
-                _lib.gemm(xb, w, out_bf16=ws["qkv"], **ln)
-            else:
-                _lib.gemm_headnorm(xb, w, out_bf16=ws["qkv"], head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads,
-                                   dh=L.dim_head, head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None, **ln)
-            if rope is not None:
-                _lib.rope_qk(ws["qkv"], rope[0], rope[1], L.heads, L.dim_head)
-            if L.xca_tau is not None:
-                _lib.attention_xca(ws["qkv"], t[f"{i}.tau"], ws["o"], B, N, L.heads, L.dim_head)
-            elif L.headmix is not None:
-                hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
-                _lib.attention_headmix(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln,
-                                       pre=t.get(f"{i}.pre"))
-            elif axial is not None and L.temporal is None:
-                axial_attention(L)
-            elif vl is None:
-                _lib.attention(ws["qkv"], ws["o"], B, N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
-            else:
-                _lib.attention_varlen(ws["qkv"], ws["o"], *vl, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
-            # the stream the feed-forward block reads: x, or the local patch interaction's output
-            ff_in = x if L.lpi is None else ws["y"]
-            if fold and L.lpi is not None:
-                # the local patch interaction reads x in fp32 and writes y, its bf16 copy and its row statistics
-                _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
-                self._lpi(t, i, L, x, ws, B, grid, xb, ws["stats_l"])
-                _lib.gemm(xb, t[f"{i}.fc1.wg"], out_bf16=ws["h"], bias=t[f"{i}.fc1.t"], gelu=True,
-                          ln_sums=ws["stats_l"], col_s=t[f"{i}.fc1.s"], ln_eps=L.ln2.eps)
-                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.fc2.b"], resid=ff_in,
-                          stats_out=sa)
-            elif fold:
-                # the residual GEMMs also write the bf16 copy of x and its row statistics for the next folded GEMM
-                _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.out.b"], resid=x,
-                          stats_out=sb)
-                if L.temporal is not None:
-                    # temporal sub-block: LN folded into its QKV GEMM on the statistics the out-projection just wrote
-                    _lib.gemm(xb, t[f"{i}.tqkv.wg"], out_bf16=ws["qkv"], bias=t[f"{i}.tqkv.t"], ln_sums=sb,
-                              col_s=t[f"{i}.tqkv.s"], ln_eps=L.temporal.ln.eps)
-                    axial_attention(L)
-                    _lib.gemm(ws["o"], t[f"{i}.tout.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.tout.b"], resid=x,
-                              stats_out=sb)
-                _lib.gemm(xb, t[f"{i}.fc1.wg"], out_bf16=ws["h"], bias=t[f"{i}.fc1.t"], gelu=True, ln_sums=sb,
-                          col_s=t[f"{i}.fc1.s"], ln_eps=L.ln2.eps)
-                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, out_bf16=xb, bias=t[f"{i}.fc2.b"], resid=x,
-                          stats_out=sa)
-            else:
-                _lib.gemm(ws["o"], t[f"{i}.out.w"], out_f32=x, bias=t[f"{i}.out.b"], resid=x)
-                if L.lpi is not None:
-                    self._lpi(t, i, L, x, ws, B, grid)
-                if L.temporal is not None:
-                    _lib.layernorm(x, t[f"{i}.tln.w"], t[f"{i}.tln.b"], out_bf16=xb, eps=L.temporal.ln.eps)
-                    _lib.gemm(xb, t[f"{i}.tqkv.w"], out_bf16=ws["qkv"])
-                    axial_attention(L)
-                    _lib.gemm(ws["o"], t[f"{i}.tout.w"], out_f32=x, bias=t[f"{i}.tout.b"], resid=x)
-                _lib.layernorm(ff_in, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_bf16=xb, eps=L.ln2.eps)
-                _lib.gemm(xb, t[f"{i}.fc1.w"], out_bf16=ws["h"], bias=t[f"{i}.fc1.b"], gelu=True)
-                _lib.gemm(ws["h"], t[f"{i}.fc2.w"], out_f32=x, bias=t[f"{i}.fc2.b"], resid=ff_in)
+        xb, qkv, o, h = ws["xn"], ws["qkv"], ws["o"], ws["h"]
+        sums = ws["stats_in"] if primed else None          # fold: the row sums of xb the next LN-folded GEMM reads
 
-    @staticmethod
-    def _lpi(t: Dict[str, torch.Tensor], i: int, L: EncoderLayer, x: torch.Tensor, ws: Dict[str, torch.Tensor], B: int,
-             grid: Tuple[int, int], y_bf16: Optional[torch.Tensor] = None,
-             y_stats: Optional[torch.Tensor] = None) -> None:
-        """ws['y'] = x + local patch interaction of layer i (and, given, its bf16 copy and row statistics)."""
-        _lib.local_patch_interaction(x, ws["y"], ws["lnst"], (t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"], L.lpi.ln.eps),
-                                     t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"], t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"], B,
-                                     grid[0], grid[1], L.lpi.kernel_size, y_bf16=y_bf16, y_stats=y_stats)
+        def normed(src: torch.Tensor, ln: str, norm: Norm, w: str, out: torch.Tensor, **epi) -> None:
+            """out = LN(src) W^T, LN = t[ln + '.w' / '.b'] with norm.eps, W the Linear t[w + ...].  fold: the LN-folded
+            GEMM on xb and `sums` (made by one rowstats_cast pass if not primed); exact: layernorm(src -> xb), then the
+            plain GEMM with the Linear's bias if it has one.  `epi` with head_gamma (a q / k norm): gemm_headnorm."""
+            nonlocal sums
+            if fold:
+                if sums is None:
+                    sums = ws["stats_in"]
+                    _lib.rowstats_cast(src, xb, sums)
+                wt, ln_kw = t[w + ".wg"], dict(bias=t[w + ".t"], ln_sums=sums, col_s=t[w + ".s"], ln_eps=norm.eps)
+            else:
+                _lib.layernorm(src, t[ln + ".w"], t[ln + ".b"], out_bf16=xb, eps=norm.eps)
+                wt, ln_kw = t[w + ".w"], dict(bias=t.get(w + ".b"))
+            (_lib.gemm_headnorm if "head_gamma" in epi else _lib.gemm)(xb, wt, out_bf16=out, **epi, **ln_kw)
+
+        def stream_copy(slot: str) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+            """(bf16 copy, row sums) the kernel writing the stream also writes: fold (xb, ws[slot]), exact none."""
+            nonlocal sums
+            if fold:
+                sums = ws[slot]
+                return xb, sums
+            return None, None
+
+        def residual(a: torch.Tensor, w: str, resid: torch.Tensor, slot: Optional[str]) -> None:
+            """x = resid + a W^T + b (t[w + '.w' / '.b']) and stream_copy(slot); None: a local patch interaction
+            follows and writes the copy of its own output."""
+            copy, stats = stream_copy(slot) if slot is not None else (None, None)
+            _lib.gemm(a, t[w + ".w"], out_f32=x, out_bf16=copy, bias=t[w + ".b"], resid=resid, stats_out=stats)
+
+        def attend(kernel: str, L: EncoderLayer, i: int) -> None:
+            if kernel == "xca":
+                _lib.attention_xca(qkv, t[f"{i}.tau"], o, B, N, L.heads, L.dim_head)
+            elif kernel == "headmix":
+                hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
+                _lib.attention_headmix(qkv, o, B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln,
+                                       pre=t.get(f"{i}.pre"))
+            elif kernel == "axial":
+                G, T, key_mask, zero = axial
+                _lib.attention_axial(qkv, o, key_mask, x.shape[0] // (T * G), T, G, L.heads, L.dim_head, L.scale, zero)
+            elif kernel == "varlen":
+                _lib.attention_varlen(qkv, o, *vl, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
+            else:
+                _lib.attention(qkv, o, B, N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
+
+        for i, kernel in zip(run, kernels):
+            L = self.layers[i]
+            head = {} if L.qk_norm is None else dict(head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
+                                                     head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
+            normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv, **head)
+            if rope is not None:
+                _lib.rope_qk(qkv, rope[0], rope[1], L.heads, L.dim_head)
+            attend(kernel, L, i)
+            residual(o, f"{i}.out", x, "stats_b" if L.lpi is None else None)
+            if L.temporal is not None:
+                normed(x, f"{i}.tln", L.temporal.ln, f"{i}.tqkv", qkv)
+                attend("axial", L, i)
+                residual(o, f"{i}.tout", x, "stats_b")
+            ff_in = x if L.lpi is None else ws["y"]
+            if L.lpi is not None:
+                yb, ys = stream_copy("stats_l")
+                ln = (t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"], L.lpi.ln.eps)
+                _lib.local_patch_interaction(x, ff_in, ws["lnst"], ln, t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"],
+                                             t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"], B, grid[0], grid[1],
+                                             L.lpi.kernel_size, y_bf16=yb, y_stats=ys)
+            normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, gelu=True)
+            residual(h, f"{i}.fc2", ff_in, "stats_a")
 
     def final_norm(self, x: torch.Tensor, *, out_bf16: Optional[torch.Tensor] = None,
                    out_f32: Optional[torch.Tensor] = None, row_index: Optional[torch.Tensor] = None) -> None:
