@@ -11,6 +11,7 @@ import subprocess
 import pytest
 import torch
 
+from oracle import bounds as Bd
 from vit_pytorch_b200 import _lib
 
 DEV = "cuda"
@@ -117,11 +118,8 @@ def test_tma_store_matches_reference(block_n):
     M, N, ldo = 300, 392, 400
     ob_full, _, _, _ = _run("bias_lnfold_gelu", M, N, ldo, False, block_n, seed=11)
     a, w, b, col_s, parts, _ = _inputs(M, N, 11, ldo)
-    af = a.float()
-    mu = af.mean(1, keepdim=True)
-    rstd = torch.rsqrt((af * af).mean(1, keepdim=True) - mu * mu + 1e-5)
-    ref = torch.nn.functional.gelu(rstd * (af @ w.float().t() - mu * col_s[None]) + b[None])
-    assert torch.allclose(ob_full[:M, :N].float(), ref, rtol=2e-2, atol=2e-2)
+    Bd.check(ob_full[:M, :N], *Bd.gemm_reference(a, w, bias=b, ln_sums=parts, col_s=col_s, gelu=True, bf16_out=True),
+             f"TMA store, hook 12 = {block_n}")
 
 
 @pytest.mark.gpu

@@ -5,6 +5,7 @@ import math
 import pytest
 import torch
 
+from oracle import bounds as Bd
 from oracle import vit_oracle as O
 from vit_pytorch_b200 import _lib
 
@@ -58,11 +59,12 @@ def test_gemm_epilogues_bias_gelu_residual():
     # bias + GELU -> bf16  (FeedForward first half, vit.py:20-21)
     ob = torch.zeros(M, N, device=DEV, dtype=torch.bfloat16)
     _lib.gemm(a, w, out_bf16=ob, bias=b, gelu=True)
-    assert within(ob, O.gelu_erf(lin)) > 0.999          # bf16 output rounding only (rtol 1e-2 / atol 1e-3)
+    Bd.check(ob, *Bd.gemm_reference(a, w, bias=b, gelu=True, bf16_out=True), "bias + GELU -> bf16")
     # bias + residual, in place on the fp32 stream (vit.py:80-81)
     x = r.clone()
     _lib.gemm(a, w, out_f32=x, bias=b, resid=x)
     assert torch.allclose(x.cpu(), lin + r.cpu(), rtol=1e-4, atol=1e-4)
+    Bd.check(x, *Bd.gemm_reference(a, w, bias=b, resid=r), "bias + residual")
 
 
 def test_gemm_lnfold_and_stats():
@@ -84,15 +86,20 @@ def test_gemm_lnfold_and_stats():
     sums2 = torch.stack([sums * 0.25, sums * 0.75], 1).contiguous()
     _lib.gemm(a, wg, out_f32=out, out_bf16=ob, bias=t.contiguous(), ln_sums=sums2, col_s=col_s.contiguous(),
               stats_out=st)
-    st = st.sum(1)
+    st_parts, st = st, st.sum(1)
     # (a) the kernel's arithmetic, against the same folded formula evaluated in fp32 on the host
     mu = af.mean(1, keepdim=True)
     rstd = torch.rsqrt((af * af).mean(1, keepdim=True) - mu * mu + 1e-5)
     same = (rstd * (af @ wg.float().t() - mu * col_s[None]) + t[None]).cpu()
     assert torch.allclose(out.cpu(), same, rtol=2e-3, atol=2e-3)
-    # (b) against the oracle's exact LayerNorm -> Linear: only the bf16 rounding of gamma*W separates them
+    # (b) every element within its bound of the fp64 LayerNorm-folded GEMM of the same inputs (oracle/bounds.py), and
+    # near the oracle's exact LayerNorm -> Linear: only the bf16 rounding of gamma*W separates the two
+    ref, e = Bd.gemm_reference(a, wg, bias=t, ln_sums=sums2, col_s=col_s)
+    Bd.check(out, ref, e, "LN fold fp32")
+    Bd.check(ob, ref, Bd.bf16_bound(ref, e), "LN fold bf16")
+    Bd.check(st_parts, *Bd.stats_reference(ob, st_parts.shape[1]), "stats")
     ref = O.linear(O.layer_norm(af.cpu(), g.cpu(), be.cpu()), w.float().cpu())
-    assert within(out, ref) > 0.95 and (out.cpu() - ref).abs().max() < 0.05
+    assert (out.cpu() - ref).abs().max() < 0.05
     rb = ob.float()
     assert torch.allclose(st[:, 0], rb.sum(1), rtol=1e-4, atol=1e-2)
     assert torch.allclose(st[:, 1], (rb * rb).sum(1), rtol=1e-4, atol=1e-2)
@@ -131,8 +138,8 @@ def test_patchify_ln(C, H, W, p):
     g, b = torch.randn(pd, device=DEV), torch.randn(pd, device=DEV)
     out = torch.full((3 * (H // p) * (W // p), ldo), 7.0, device=DEV, dtype=torch.bfloat16)
     _lib.patchify_ln(img, g, b, out, p, p)
-    ref = O.layer_norm(O.patchify(img.float().cpu(), p, p), g.cpu(), b.cpu()).reshape(-1, pd)
-    assert torch.equal(out[:, :pd].cpu(), ref.bfloat16()) or within(out[:, :pd], ref) > 0.9999
+    # within one bf16 ulp (plus the fp32 error of the LayerNorm) of the fp64 LayerNorm of every patch
+    Bd.check(out[:, :pd], *Bd.layernorm_reference(O.patchify(img, p, p).reshape(-1, pd), g, b), "patchify_ln")
     assert (out[:, pd:] == 0).all()
 
 
@@ -375,11 +382,13 @@ def test_gemm_long_k_block_n_variants_agree():
         finally:
             L.b200vit_debug_set(12, 0)
         res[ew] = (x, xb, st.sum(dim=1), y)
-    ref = x0.cpu() + a.float().cpu() @ w.float().cpu().t() + bias.cpu()
+    ref, e = Bd.gemm_reference(a, w, bias=bias, resid=x0)
+    ref_y, e_y = Bd.gemm_reference(a, w, bias=bias)
     for ew in (1, 2):
         x, xb, st, y = res[ew]
         assert torch.isfinite(st).all()
-        assert within(x, ref, rtol=1e-3, atol=2e-3) > 0.999
+        Bd.check(x, ref, e, f"long K, residual, hook 12 = {ew}")
+        Bd.check(y, ref_y, e_y, f"long K, fp32, hook 12 = {ew}")
         assert torch.equal(xb, x.bfloat16())
         assert torch.allclose(st[:, 0].cpu(), xb.float().sum(1).cpu(), rtol=1e-3, atol=1e-2)
         assert torch.allclose(st[:, 1].cpu(), (xb.float() ** 2).sum(1).cpu(), rtol=1e-3, atol=1e-2)
