@@ -365,6 +365,34 @@ int b200vit_local_patch_interaction(const float* x, float* y, void* y_bf16, floa
                                     const float* b1, const float* w2, const float* b2, int B, int gh, int gw, int D,
                                     int k, void* stream);
 
+/*
+ * Overlapping patch extraction (PiT's nn.Unfold(kernel_size=p, stride=s) + Rearrange('b c n -> b n c'),
+ * pit.py:140-147): img[B, C, H, W] bf16 (NCHW, contiguous) -> out[B*oh*ow, ldo] bf16, oh = (H - p) / s + 1,
+ * ow = (W - p) / s + 1 (trailing pixels that do not fill a stride step are dropped), with
+ *   out[b*oh*ow + r*ow + c, (ch*p + i)*p + j] = img[b, ch, r*s + i, c*s + j]
+ * as bit copies (Unfold's column order: channel slowest).  Columns [C*p*p, ldo) are zero filled (K padding for the
+ * GEMM).  p >= 2, s >= 1, H and W >= p; ldo a multiple of 8 and >= C*p*p; out_bf16 16-byte aligned.  Each CTA stages the
+ * image rows of one patch row in shared memory, so a pixel covered by several patches of that row is read once.
+ */
+int b200vit_unfold_patches(const void* img, void* out_bf16, int64_t ldo, int B, int C, int H, int W, int p, int s,
+                           void* stream);
+
+/*
+ * PiT's pooling layer up to its 1 x 1 convolution (Pool, pit.py:98-113): x[M, D] fp32 is the residual stream of B
+ * images of 1 + h*w rows (row b*(1 + h*w) the cls row, then token r*w + c of the h x w grid; M = B*(1 + h*w)).
+ *   a[b*(1 + oh*ow) + 1 + t, o] = bias[o] + sum_{dy, dx < 3} w9[dy*3 + dx][o] x_grid[b, 2*r - 1 + dy, 2*q - 1 + dx, o / 2]
+ * for output token t = r*ow + q of the oh x ow = ceil(h / 2) x ceil(w / 2) grid and o < 2D: the depthwise 3 x 3,
+ * stride 2, zero padding 1 convolution with channel multiplier 2 (Conv2d(D, 2D, 3, 2, 1, groups=D): output channel o
+ * reads input channel o / 2), accumulated in fp32 and rounded to bf16 -- the A operand of the 1 x 1 convolution's GEMM.
+ * Row b*(1 + oh*ow) of a (the cls slot) is zero filled, so one GEMM over all B*(1 + oh*ow) rows writes the next
+ * stage's stream, whose cls rows cls_ff then overwrites.  cls[b, :D] = bf16 copy of x's cls row of image b: the A
+ * operand of the cls_ff GEMM.  w9: fp32 [9][2D] (tap major, output channel minor), bias fp32 [2D].
+ * D a multiple of 8; lda >= 2D and ldc >= D, multiples of 8; x, w9, bias, a_bf16, cls_bf16 16-byte aligned.  Each
+ * image's outputs are computed from its own rows only, and repeated calls give the same bits.
+ */
+int b200vit_pit_pool(const float* x, int64_t M, int B, int h, int w, int D, const float* w9, const float* bias,
+                     void* a_bf16, int64_t lda, void* cls_bf16, int64_t ldc, void* stream);
+
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */
 int b200vit_mean_pool(const float* x, float* out, int B, int N, int D, int n_pool, void* stream);

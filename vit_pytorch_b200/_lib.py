@@ -36,7 +36,7 @@ SYMBOLS = [
     "b200vit_attention_axial", "b200vit_embed_tokens_grouped", "b200vit_patchify_spt_ln", "b200vit_attention_ex",
     "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex", "b200vit_attention_cls",
     "b200vit_attention_headmix", "b200vit_attention_headmix_ex", "b200vit_attention_cls_headmix",
-    "b200vit_attention_xca", "b200vit_local_patch_interaction",
+    "b200vit_attention_xca", "b200vit_local_patch_interaction", "b200vit_unfold_patches", "b200vit_pit_pool",
 ]
 
 
@@ -129,6 +129,10 @@ def lib() -> C.CDLL:
     L.b200vit_local_patch_interaction.restype = i32
     L.b200vit_local_patch_interaction.argtypes = [vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, vp, vp, i32, i32, i32, i32,
                                                   i32, vp]
+    L.b200vit_unfold_patches.restype = i32
+    L.b200vit_unfold_patches.argtypes = [vp, vp, i64, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_pit_pool.restype = i32
+    L.b200vit_pit_pool.argtypes = [vp, i64, i32, i32, i32, i32, vp, vp, vp, i64, vp, i64, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -764,6 +768,43 @@ def local_patch_interaction(x: torch.Tensor, y: torch.Tensor, ln_scratch: torch.
                                                    _ptr(g), _ptr(bt), float(eps), _ptr(w1), _ptr(b1), _ptr(w2),
                                                    _ptr(b2), B, gh, gw, D, int(k), _stream())
     _check(rc, "b200vit_local_patch_interaction")
+
+
+def unfold_patches(img: torch.Tensor, out_bf16: torch.Tensor, p: int, s: int) -> None:
+    """img [B, C, H, W] bf16 -> out [B*oh*ow, ldo] bf16 rows of F.unfold(img, p, stride=s).transpose(1, 2) (columns
+    (c, i, j), channel slowest), zero K padding up to ldo = out.stride(0)."""
+    _chk(img, torch.bfloat16, "img"); _chk(out_bf16, torch.bfloat16, "out")
+    assert img.is_contiguous() and img.dim() == 4 and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    B, Cc, H, W = img.shape
+    rows = B * ((H - p) // s + 1) * ((W - p) // s + 1)
+    assert out_bf16.shape[0] == rows and out_bf16.shape[1] >= Cc * p * p, \
+        f"out must be [{rows}, >= {Cc * p * p}], got {tuple(out_bf16.shape)}"
+    with _Timed("unfold_patches", bytes=img.numel() * 2 + rows * out_bf16.stride(0) * 2):
+        rc = lib().b200vit_unfold_patches(_ptr(img), _ptr(out_bf16), out_bf16.stride(0), B, Cc, H, W, int(p), int(s),
+                                          _stream())
+    _check(rc, "b200vit_unfold_patches")
+
+
+def pit_pool(x: torch.Tensor, B: int, h: int, w: int, w9: torch.Tensor, bias: torch.Tensor, a_bf16: torch.Tensor,
+             cls_bf16: torch.Tensor) -> None:
+    """PiT's Pool before its 1 x 1 convolution: x fp32 [B*(1 + h*w), D] (cls row, then the h x w grid) -> a_bf16
+    [B*(1 + oh*ow), >= 2D] = the depthwise 3 x 3 / stride 2 / pad 1 convolution with channel multiplier 2 (+ bias) of
+    every grid, cls slots zero filled, and cls_bf16 [B, >= D] = the bf16 cls rows.  w9 fp32 [9, 2D] tap major, bias
+    fp32 [2D]."""
+    for nm, t in (("x", x), ("w9", w9), ("bias", bias)):
+        _chk(t, torch.float32, nm)
+    _chk(a_bf16, torch.bfloat16, "a"); _chk(cls_bf16, torch.bfloat16, "cls")
+    M, D = x.shape
+    oh, ow = (h + 1) // 2, (w + 1) // 2
+    assert x.is_contiguous() and w9.is_contiguous() and bias.is_contiguous()
+    assert w9.shape == (9, 2 * D) and bias.numel() == 2 * D
+    assert a_bf16.dim() == 2 and a_bf16.stride(1) == 1 and a_bf16.shape[0] == B * (1 + oh * ow) \
+        and a_bf16.shape[1] >= 2 * D
+    assert cls_bf16.dim() == 2 and cls_bf16.stride(1) == 1 and cls_bf16.shape[0] == B and cls_bf16.shape[1] >= D
+    with _Timed("pit_pool", B=B, h=h, w=w, D=D, bytes=M * D * 4 + B * (1 + oh * ow) * 2 * D * 2):
+        rc = lib().b200vit_pit_pool(_ptr(x), M, B, int(h), int(w), D, _ptr(w9), _ptr(bias), _ptr(a_bf16),
+                                    a_bf16.stride(0), _ptr(cls_bf16), cls_bf16.stride(0), _stream())
+    _check(rc, "b200vit_pit_pool")
 
 
 def mean_pool(x: torch.Tensor, out: torch.Tensor, B: int, N: int, D: int, n_pool: Optional[int] = None) -> None:
