@@ -8,6 +8,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR, load_golden
+from oracle import attention_bounds as AB
 from oracle import bounds as Bd
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.vit import Patchify
@@ -99,9 +100,11 @@ def test_masked_attention_against_fp32(dh, N):
     want = masked_reference(qkv, [N] * B, H, dh, scale)
     assert torch.isfinite(out.float()).all()
     assert close(out, want), (out.float() - want).abs().max().item()
+    Bd.check(out, *AB.qkv_attention_reference(qkv, [N] * B, H, dh, scale, mask_self=True), "MASK_SELF")
     # flags = 0 is the existing entry point, bit for bit
     plain, ex0 = torch.empty_like(out), torch.empty_like(out)
     _lib.attention(qkv, plain, B, N, H, dh, scale)
+    Bd.check(plain, *AB.qkv_attention_reference(qkv, [N] * B, H, dh, scale), "flags = 0")
     _ex(qkv, ex0, B, N, H, dh, scale, 0)
     assert torch.equal(plain, ex0)
     if N == 1:                                             # the reference's fill leaves the only key: out = v
@@ -124,8 +127,10 @@ def test_masked_varlen_attention_against_fp32(dh, lengths):
     want = masked_reference(qkv, lengths, H, dh, scale)
     assert torch.isfinite(out.float()).all()
     assert close(out, want), (out.float() - want).abs().max().item()
+    Bd.check(out, *AB.qkv_attention_reference(qkv, lengths, H, dh, scale, mask_self=True), "MASK_SELF")
     plain, ex0 = torch.empty_like(out), torch.empty_like(out)
     _lib.attention_varlen(qkv, plain, cu, tp, tiles, H, dh, scale)
+    Bd.check(plain, *AB.qkv_attention_reference(qkv, lengths, H, dh, scale), "flags = 0")
     rc = _lib.lib().b200vit_attention_varlen_ex(qkv.data_ptr(), ex0.data_ptr(), cu.data_ptr(), tp.data_ptr(),
                                                 len(lengths), T, tiles, H, dh, scale, 0,
                                                 torch.cuda.current_stream().cuda_stream)
