@@ -41,6 +41,12 @@ extern "C" {
 /* attention flags (b200vit_attention_ex, b200vit_attention_varlen_ex, b200vit_encoder_blocks_ex) */
 #define B200VIT_ATTN_MASK_SELF 1  /* key i of query i gets probability 0 (LSA, vit_for_small_dataset.py:53-57) */
 
+/* what the convolutional tokenizer's kernels are built for (b200vit_conv_im2col_*, b200vit_relu_maxpool,
+ * b200vit_seq_pool) */
+#define B200VIT_CONV_MAX_KERNEL 16   /* Conv2d kernel size k */
+#define B200VIT_POOL_MAX_KERNEL 16   /* MaxPool2d kernel size */
+#define B200VIT_SEQ_POOL_MAX_DIM 1024  /* embedding width D of b200vit_seq_pool */
+
 const char* b200vit_last_error(void);
 int b200vit_version(void);
 /* number of kernels this library has launched in the calling process (all threads) since load / last reset */
@@ -392,6 +398,49 @@ int b200vit_unfold_patches(const void* img, void* out_bf16, int64_t ldo, int B, 
  */
 int b200vit_pit_pool(const float* x, int64_t M, int B, int h, int w, int D, const float* w9, const float* bias,
                      void* a_bf16, int64_t lda, void* cls_bf16, int64_t ldc, void* stream);
+
+/*
+ * The A operand of a zero-padded Conv2d(C, Cout, k, stride s, padding p) as a GEMM (CCT's tokenizer, cct.py:181-190),
+ * oh = (H + 2p - k) / s + 1, ow = (W + 2p - k) / s + 1, one row per output pixel b*oh*ow + r*ow + q, written as bit
+ * copies; a tap outside the image is zero and so are columns [K, ldo) (K padding for the GEMM).
+ *   _nchw: img[B, C, H, W] bf16 (NCHW, contiguous), column (c*k + i)*k + j = img[b, c, r*s - p + i, q*s - p + j]
+ *          (F.unfold's order: channel slowest, the layout of the Conv2d weight itself), K = C*k*k.  Each CTA stages the
+ *          image rows one output row covers, zero halo included, in shared memory.
+ *   _nhwc: x[M, C] bf16 channels-last (pixel (b, y, x) at row (b*H + y)*W + x, M = B*H*W), column (i*k + j)*C + c =
+ *          x[(b, r*s - p + i, q*s - p + j), c] (channel fastest, 16-byte vectors: C a multiple of 8), K = k*k*C.  The
+ *          caller permutes the weight to [Cout, k, k, C] to match.
+ * 1 <= k <= B200VIT_CONV_MAX_KERNEL, s >= 1, 0 <= p < k, H + 2p and W + 2p >= k; ldo a multiple of 8 and >= K;
+ * out_bf16 16-byte aligned (and x for _nhwc).
+ */
+int b200vit_conv_im2col_nchw(const void* img, void* out_bf16, int64_t ldo, int B, int C, int H, int W, int k, int s,
+                             int p, void* stream);
+int b200vit_conv_im2col_nhwc(const void* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W, int C, int k,
+                             int s, int p, void* stream);
+
+/*
+ * ReLU then MaxPool2d(pk, stride ps, padding pp) in one pass (CCT's tokenizer, cct.py:187-190): y[M, C] bf16
+ * channels-last (M = B*H*W, as b200vit_conv_im2col_nhwc's x) ->
+ *   out[b*oh*ow + r*ow + q, c] = relu(max_{i, j < pk} y[(b, r*ps - pp + i, q*ps - pp + j), c]),
+ * oh = (H + 2pp - pk) / ps + 1 (likewise ow), the padding counting as -inf; NaN propagates as in F.max_pool2d.
+ * Exactly one output: out_bf16 (the next conv layer's channels-last input; ldo a multiple of 8) or out_f32 (the
+ * tokens [B*oh*ow, C] b200vit_embed_tokens takes; ldo a multiple of 4), row stride ldo >= C elements.  C a multiple of
+ * 8; 1 <= pk <= B200VIT_POOL_MAX_KERNEL, ps >= 1, 0 <= pp <= pk / 2, H + 2pp and W + 2pp >= pk; y and the output
+ * 16-byte aligned.  Bit exact: every output is one of the inputs, or zero.
+ */
+int b200vit_relu_maxpool(const void* y, int64_t M, int B, int H, int W, int C, int pk, int ps, int pp, void* out_bf16,
+                         float* out_f32, int64_t ldo, void* stream);
+
+/*
+ * Sequence pooling (CCT's TransformerClassifier with seq_pool, cct.py:284-288): x[B*n, D] fp32, token t of image b at
+ * row b*n + t ->
+ *   y_t = LayerNorm(x_t) (gamma, beta, eps),  z_t = y_t . w + bias[0],  out[b, :D] = sum_t softmax_t(z)_t y_t
+ * as bf16 (the A operand of the classifier GEMM), row stride ldo.  fp32 throughout with an online max; each image's
+ * tokens are shared by a cluster of up to 8 CTAs, merged in a fixed order (repeated calls give the same bits).  An
+ * image's NaN or Inf reaches only its own output row.  D a multiple of 8 and <= B200VIT_SEQ_POOL_MAX_DIM, B <= 65535;
+ * ldo a multiple of 8 and >= D; x, gamma, beta, w, out_bf16 16-byte aligned; bias a device pointer to one float.
+ */
+int b200vit_seq_pool(const float* x, int B, int n, int D, const float* gamma, const float* beta, float eps,
+                     const float* w, const float* bias, void* out_bf16, int64_t ldo, void* stream);
 
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */

@@ -37,6 +37,7 @@ SYMBOLS = [
     "b200vit_attention_varlen_ex", "b200vit_encoder_blocks_ex", "b200vit_attention_cls",
     "b200vit_attention_headmix", "b200vit_attention_headmix_ex", "b200vit_attention_cls_headmix",
     "b200vit_attention_xca", "b200vit_local_patch_interaction", "b200vit_unfold_patches", "b200vit_pit_pool",
+    "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
 ]
 
 
@@ -133,6 +134,14 @@ def lib() -> C.CDLL:
     L.b200vit_unfold_patches.argtypes = [vp, vp, i64, i32, i32, i32, i32, i32, i32, vp]
     L.b200vit_pit_pool.restype = i32
     L.b200vit_pit_pool.argtypes = [vp, i64, i32, i32, i32, i32, vp, vp, vp, i64, vp, i64, vp]
+    L.b200vit_conv_im2col_nchw.restype = i32
+    L.b200vit_conv_im2col_nchw.argtypes = [vp, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_conv_im2col_nhwc.restype = i32
+    L.b200vit_conv_im2col_nhwc.argtypes = [vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_relu_maxpool.restype = i32
+    L.b200vit_relu_maxpool.argtypes = [vp, i64, i32, i32, i32, i32, i32, i32, i32, vp, vp, i64, vp]
+    L.b200vit_seq_pool.restype = i32
+    L.b200vit_seq_pool.argtypes = [vp, i32, i32, i32, vp, vp, f32, vp, vp, vp, i64, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -805,6 +814,77 @@ def pit_pool(x: torch.Tensor, B: int, h: int, w: int, w9: torch.Tensor, bias: to
         rc = lib().b200vit_pit_pool(_ptr(x), M, B, int(h), int(w), D, _ptr(w9), _ptr(bias), _ptr(a_bf16),
                                     a_bf16.stride(0), _ptr(cls_bf16), cls_bf16.stride(0), _stream())
     _check(rc, "b200vit_pit_pool")
+
+
+def conv_out_size(n: int, k: int, s: int, p: int) -> int:
+    """Output length of a Conv2d / MaxPool2d window along one axis (dilation 1, floor mode)."""
+    return (n + 2 * p - k) // s + 1
+
+
+def conv_im2col_nchw(img: torch.Tensor, out_bf16: torch.Tensor, k: int, s: int, p: int) -> None:
+    """img [B, C, H, W] bf16 -> out [B*oh*ow, ldo] bf16 rows of F.unfold(img, k, padding=p, stride=s).transpose(1, 2)
+    (columns (c, i, j), channel slowest), zero K padding up to ldo = out.stride(0)."""
+    _chk(img, torch.bfloat16, "img"); _chk(out_bf16, torch.bfloat16, "out")
+    assert img.is_contiguous() and img.dim() == 4 and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    B, Cc, H, W = img.shape
+    rows = B * conv_out_size(H, k, s, p) * conv_out_size(W, k, s, p)
+    assert out_bf16.shape[0] == rows and out_bf16.shape[1] >= Cc * k * k, \
+        f"out must be [{rows}, >= {Cc * k * k}], got {tuple(out_bf16.shape)}"
+    with _Timed("conv_im2col", bytes=img.numel() * 2 + rows * out_bf16.stride(0) * 2):
+        rc = lib().b200vit_conv_im2col_nchw(_ptr(img), _ptr(out_bf16), out_bf16.stride(0), B, Cc, H, W, int(k), int(s),
+                                            int(p), _stream())
+    _check(rc, "b200vit_conv_im2col_nchw")
+
+
+def conv_im2col_nhwc(x: torch.Tensor, out_bf16: torch.Tensor, B: int, H: int, W: int, k: int, s: int, p: int) -> None:
+    """x [B*H*W, C] bf16 channels-last -> out [B*oh*ow, ldo] bf16, column (i*k + j)*C + c the channel c of tap (i, j)
+    of the zero-padded k x k window at stride s, zero K padding up to ldo = out.stride(0)."""
+    _chk(x, torch.bfloat16, "x"); _chk(out_bf16, torch.bfloat16, "out")
+    assert x.is_contiguous() and x.dim() == 2 and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    M, Cc = x.shape
+    rows = B * conv_out_size(H, k, s, p) * conv_out_size(W, k, s, p)
+    assert out_bf16.shape[0] == rows and out_bf16.shape[1] >= Cc * k * k, \
+        f"out must be [{rows}, >= {Cc * k * k}], got {tuple(out_bf16.shape)}"
+    with _Timed("conv_im2col", bytes=x.numel() * 2 + rows * out_bf16.stride(0) * 2):
+        rc = lib().b200vit_conv_im2col_nhwc(_ptr(x), M, _ptr(out_bf16), out_bf16.stride(0), B, H, W, Cc, int(k), int(s),
+                                            int(p), _stream())
+    _check(rc, "b200vit_conv_im2col_nhwc")
+
+
+def relu_maxpool(y: torch.Tensor, B: int, H: int, W: int, pk: int, ps: int, pp: int, *,
+                 out_bf16: Optional[torch.Tensor] = None, out_f32: Optional[torch.Tensor] = None) -> None:
+    """y [B*H*W, C] bf16 channels-last -> relu(max_pool2d(y, pk, ps, pp)) channels-last [B*oh*ow, C] into exactly one
+    of out_bf16 / out_f32 (row stride out.stride(0))."""
+    _chk(y, torch.bfloat16, "y"); _chk(out_bf16, torch.bfloat16, "out_bf16"); _chk(out_f32, torch.float32, "out_f32")
+    assert (out_bf16 is None) != (out_f32 is None)
+    out = out_bf16 if out_bf16 is not None else out_f32
+    assert y.is_contiguous() and y.dim() == 2 and out.dim() == 2 and out.stride(1) == 1
+    M, Cc = y.shape
+    rows = B * conv_out_size(H, pk, ps, pp) * conv_out_size(W, pk, ps, pp)
+    assert out.shape[0] == rows and out.shape[1] >= Cc, f"out must be [{rows}, >= {Cc}], got {tuple(out.shape)}"
+    with _Timed("relu_maxpool", bytes=M * Cc * 2 + rows * Cc * out.element_size()):
+        rc = lib().b200vit_relu_maxpool(_ptr(y), M, B, H, W, Cc, int(pk), int(ps), int(pp), _ptr(out_bf16),
+                                        _ptr(out_f32), out.stride(0), _stream())
+    _check(rc, "b200vit_relu_maxpool")
+
+
+def seq_pool(x: torch.Tensor, B: int, n: int, gamma: torch.Tensor, beta: torch.Tensor, w: torch.Tensor,
+             bias: torch.Tensor, out_bf16: torch.Tensor, eps: float = 1e-5) -> None:
+    """x fp32 [B*n, D] -> out_bf16 [B, D] (any row stride) = sum_t softmax_t(LN(x_t) . w + bias) LN(x_t) per image
+    (CCT's sequence pooling).  gamma, beta, w fp32 [D], bias fp32 [1]."""
+    for nm, t in (("x", x), ("gamma", gamma), ("beta", beta), ("w", w), ("bias", bias)):
+        _chk(t, torch.float32, nm)
+    _chk(out_bf16, torch.bfloat16, "out")
+    M, D = x.shape
+    assert M == B * n and x.is_contiguous()
+    for t in (gamma, beta, w):
+        assert t.is_contiguous() and t.numel() == D
+    assert bias.numel() == 1
+    assert out_bf16.dim() == 2 and out_bf16.stride(1) == 1 and out_bf16.shape == (B, D)
+    with _Timed("seq_pool", B=B, n=n, D=D, bytes=M * D * 4):
+        rc = lib().b200vit_seq_pool(_ptr(x), B, n, D, _ptr(gamma), _ptr(beta), float(eps), _ptr(w), _ptr(bias),
+                                    _ptr(out_bf16), out_bf16.stride(0), _stream())
+    _check(rc, "b200vit_seq_pool")
 
 
 def mean_pool(x: torch.Tensor, out: torch.Tensor, B: int, N: int, D: int, n_pool: Optional[int] = None) -> None:

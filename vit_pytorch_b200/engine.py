@@ -271,6 +271,8 @@ class EncoderLayer:
     xca_tau: Optional[torch.Tensor] = None
     # local patch interaction between the attention and the feed-forward block (XCiT); run_blocks needs `grid`
     lpi: Optional[LPIBlock] = None
+    # `ln2` replaces the stream: x = LN2(x); x += fc2(GELU(fc1(x))) (cct.py:137-142)
+    post_norm: bool = False
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
@@ -498,12 +500,12 @@ class TransformerEngine:
         """(ctypes array of b200vit_layer, (heads, dh, hidden, scale), layer scales, attention flags) for the one-call
         encoder (b200vit_encoder_blocks), or None when it cannot run these layers: they are not uniform, one has a
         per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block, an attention kernel other
-        than the plain one or a local patch interaction.  Layer scales: None when every layer has the same scale, else
+        than the plain one, a local patch interaction or a post-norm step.  Layer scales: None when every layer has the same scale, else
         a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned temperatures).  The pointers stay valid as
         long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
         if any(L.qk_norm == "ln" or L.temporal is not None or attention_kernel(L) != "plain" or L.lpi is not None
-               or sig(L) != sig(self.layers[0]) for L in self.layers):
+               or L.post_norm or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -547,9 +549,11 @@ class TransformerEngine:
                 "stats_a": torch.empty(M, _lib.stats_parts(D), 2, device=device, dtype=torch.float32),
                 "stats_b": torch.empty(M, _lib.stats_parts(D), 2, device=device, dtype=torch.float32),
             }
-            if any(L.lpi is not None for L in self.layers):
-                # the local patch interaction's output stream, its row statistics and its LayerNorm scratch
+            if any(L.lpi is not None or L.post_norm for L in self.layers):
+                # the stream the feed-forward block reads: the local patch interaction's or the post-norm's output
                 slot.t["y"] = torch.empty(M, D, device=device, dtype=torch.float32)
+            if any(L.lpi is not None for L in self.layers):
+                # the local patch interaction's row statistics and its LayerNorm scratch
                 slot.t["stats_l"] = torch.empty(M, 2, device=device, dtype=torch.float32)
                 slot.t["lnst"] = torch.empty(M, 2, device=device, dtype=torch.float32)
             w = slot.t
@@ -589,7 +593,8 @@ class TransformerEngine:
         `grid` = (h, w): the token grid of every sequence (N = h*w, token r*w + c), which layers with a local patch
         interaction need (XCiT).  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
         axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
-        onto that stream, written to x.  The call is checked first: a ValueError leaves x as it was.
+        onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
+        fc1 is the plain GEMM on that copy.  The call is checked first: a ValueError leaves x as it was.
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
         the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
@@ -668,19 +673,24 @@ class TransformerEngine:
             if rope is not None:
                 _lib.rope_qk(qkv, rope[0], rope[1], L.heads, L.dim_head)
             attend(kernel, L, i)
-            residual(o, f"{i}.out", x, "stats_b" if L.lpi is None else None)
+            residual(o, f"{i}.out", x, "stats_b" if L.lpi is None and not L.post_norm else None)
             if L.temporal is not None:
                 normed(x, f"{i}.tln", L.temporal.ln, f"{i}.tqkv", qkv)
                 attend("axial", L, i)
                 residual(o, f"{i}.tout", x, "stats_b")
-            ff_in = x if L.lpi is None else ws["y"]
+            ff_in = x if L.lpi is None and not L.post_norm else ws["y"]
             if L.lpi is not None:
                 yb, ys = stream_copy("stats_l")
                 ln = (t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"], L.lpi.ln.eps)
                 _lib.local_patch_interaction(x, ff_in, ws["lnst"], ln, t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"],
                                              t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"], B, grid[0], grid[1],
                                              L.lpi.kernel_size, y_bf16=yb, y_stats=ys)
-            normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, gelu=True)
+            if L.post_norm:
+                # the normalised stream and its bf16 copy; fc1 reads that copy as it is, with no LayerNorm of its own
+                _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_f32=ff_in, out_bf16=xb, eps=L.ln2.eps)
+                _lib.gemm(xb, t[f"{i}.fc1.w"], out_bf16=h, bias=t[f"{i}.fc1.b"], gelu=True)
+            else:
+                normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, gelu=True)
             residual(h, f"{i}.fc2", ff_in, "stats_a")
 
     def final_norm(self, x: torch.Tensor, *, out_bf16: Optional[torch.Tensor] = None,
