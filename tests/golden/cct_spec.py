@@ -1,11 +1,6 @@
-"""Recipe of the CCT parity cases (reference cct.py), shared by make_cct_golden.py, which runs the UNMODIFIED reference
-on them, and by the tests, which rebuild the same weights and inputs from the seeds.  The weights are not stored: the
-drop-in's constructor consumes the RNG exactly like the reference's (tests/test_cct.py checks the seeded-init digest),
-and cct.pt keeps a digest of every rebuilt case so a drift in the recipe fails loudly instead of comparing different
-models."""
-import hashlib
-
-import torch
+"""CCT parity cases (reference cct.py), on the shared recipe of parity.py.  A case with a `preset` builds that cct_*
+function instead of CCT; the fixture also stores the presets' and _cct's signatures and each case's sequence_length."""
+from parity import Family, load, signature
 
 BASE = dict(embedding_dim=64, n_input_channels=3, num_layers=2, num_heads=1, mlp_ratio=2, num_classes=7,
             dropout_rate=0., attention_dropout=0.1, stochastic_depth_rate=0.1)
@@ -54,43 +49,16 @@ def case_kwargs(spec: dict) -> dict:
     return kw
 
 
-def input_channels(spec: dict) -> int:
-    return case_kwargs(spec).get("n_input_channels", 3)
+def signatures(package: str) -> dict:
+    return {"signature": signature(load(package, "cct.CCT")),
+            "presets": {p: signature(load(package, f"cct.{p}")) for p in PRESETS},
+            "cct_defaults": signature(load(package, "cct._cct"))}
 
 
-def cct_model(module, spec: dict):
-    """`module` = the reference's vit_pytorch.cct (generator) or vit_pytorch_b200.cct (tests): the same fp32 model from
-    the same seeds.  LayerNorm affine parameters and every bias are perturbed so they are exercised, then every
-    parameter is rounded to a bf16-representable value, so a bf16 copy of the model holds the same numbers."""
-    torch.manual_seed(spec["seed"])
-    ctor = getattr(module, spec["preset"]) if "preset" in spec else module.CCT
-    model = ctor(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        for p in model.parameters():
-            p.copy_(p.bfloat16().float())
-    return model
-
-
-def cct_input(spec: dict) -> torch.Tensor:
-    """bf16 images [BATCH, channels, height, width]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    return torch.randn(BATCH, input_channels(spec), *spec["input"], generator=g).bfloat16()
-
-
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="cct", model="cct.CCT", cases=CCT_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, case_kwargs(spec).get("n_input_channels", 3), *spec["input"]),
+    init_seed=INIT_SEED, init={None: INIT_KWARGS},
+    make=lambda package, spec: load(package, "cct." + spec.get("preset", "CCT")),
+    signatures=signatures,
+    stored=lambda model, spec: {"sequence_length": model.classifier.sequence_length})

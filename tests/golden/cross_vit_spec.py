@@ -1,11 +1,5 @@
-"""Recipe of the CrossViT parity cases (reference cross_vit.py), shared by make_cross_vit_golden.py, which runs the
-UNMODIFIED reference on them, and by the tests, which rebuild the same weights and inputs from the seeds.  The weights
-are not stored: the drop-in's constructor consumes the RNG exactly like the reference's (tests/test_cross_vit.py checks
-the seeded-init digests), and cross_vit.pt keeps a digest of every rebuilt case so a drift in the recipe fails loudly
-instead of comparing different models."""
-import hashlib
-
-import torch
+"""CrossViT parity cases (reference cross_vit.py), on the shared recipe of parity.py."""
+from parity import Family
 
 BASE = dict(num_classes=7, sm_dim=32, lg_dim=64, sm_patch_size=4, lg_patch_size=8, sm_enc_depth=1, sm_enc_heads=2,
             sm_enc_mlp_dim=64, sm_enc_dim_head=32, lg_enc_depth=2, lg_enc_heads=2, lg_enc_mlp_dim=96,
@@ -42,39 +36,7 @@ def case_kwargs(spec: dict) -> dict:
     return kw
 
 
-def cross_vit_model(cls, spec: dict):
-    """`cls` = the reference's CrossViT (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm affine parameters are perturbed so they are exercised, then every parameter is rounded to
-    bf16-representable values, so a bf16 copy of the model holds the same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        for t in model.parameters():
-            t.copy_(t.bfloat16().float())
-    return model
-
-
-def cross_vit_input(spec: dict) -> torch.Tensor:
-    """bf16 images [BATCH, channels, input, input]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    c = spec.get("channels", BASE["channels"])
-    return torch.randn(BATCH, c, spec["input"], spec["input"], generator=g).bfloat16()
-
-
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="cross_vit", model="cross_vit.CrossViT", cases=CROSS_VIT_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, spec.get("channels", BASE["channels"]), spec["input"], spec["input"]),
+    init_seed=INIT_SEED, init={"widths": INIT_KWARGS, "equal": dict(INIT_KWARGS, lg_dim=INIT_KWARGS["sm_dim"])})

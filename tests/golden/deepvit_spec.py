@@ -1,11 +1,8 @@
-"""Recipe of the DeepViT parity cases (reference deepvit.py), shared by make_deepvit_golden.py, which runs the
-UNMODIFIED reference on them, and by the tests, which rebuild the same weights and inputs from the seeds.  The weights
-are not stored: the drop-in's constructor consumes the RNG exactly like the reference's (tests/test_deepvit.py checks
-the seeded-init digests), and deepvit.pt keeps a digest of every rebuilt case so a drift in the recipe fails loudly
-instead of comparing different models."""
-import hashlib
-
+"""DeepViT parity cases (reference deepvit.py), on the shared recipe of parity.py.  Its own rule: each layer's
+re-attention matrix gets `mix` times N(0, 1) noise (the LayerNorm over the heads is perturbed by the shared rule)."""
 import torch
+
+from parity import Family
 
 BASE = dict(num_classes=7, dim=64, depth=2, heads=4, mlp_dim=96, dim_head=32, pool='cls', channels=3, dropout=0.,
             emb_dropout=0.)
@@ -43,42 +40,12 @@ def case_kwargs(spec: dict) -> dict:
     return kw
 
 
-def deepvit_model(cls, spec: dict):
-    """`cls` = the reference's DeepViT (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm affine parameters (the one over heads included) are perturbed so they are exercised, each layer's
-    re-attention matrix gets `mix` times N(0, 1) noise, then every parameter is rounded to bf16-representable values,
-    so a bf16 copy of the model holds the same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-            elif n.endswith("reattn_weights"):
-                p.add_(spec["mix"] * torch.randn(p.shape, generator=g))
-        for t in model.parameters():
-            t.copy_(t.bfloat16().float())
-    return model
+def extra(n, p, g, spec) -> None:
+    if n.endswith("reattn_weights"):
+        p.add_(spec["mix"] * torch.randn(p.shape, generator=g))
 
 
-def deepvit_input(spec: dict) -> torch.Tensor:
-    """bf16 images [BATCH, channels, input, input]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    c = spec.get("channels", BASE["channels"])
-    return torch.randn(BATCH, c, spec["input"], spec["input"], generator=g).bfloat16()
-
-
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="deepvit", model="deepvit.DeepViT", cases=DEEPVIT_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, spec.get("channels", BASE["channels"]), spec["input"], spec["input"]),
+    init_seed=INIT_SEED, init={pool: dict(INIT_KWARGS, pool=pool) for pool in ("cls", "mean")}, extra=extra)

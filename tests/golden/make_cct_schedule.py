@@ -4,18 +4,17 @@ on CPU without a GPU:
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_cct_schedule.py
 
-The recording machinery is make_pit_schedule.py's (itself make_engine_schedule.py's): every _lib entry point the
-forward reaches is replaced by a recorder and torch.cuda.current_stream is stubbed, so CCT.forward_fused runs on CPU
-tensors and nothing computes.  A tensor is stored as the input image (`img`), as a buffer of the classifier's workspace
-(`ws.<name>`), as a prepared weight (its key -- `conv<i>`, `seq.*`, `enc.*`, `head.*` -- and a digest of its bytes), or
-as the k-th intermediate buffer the forward allocated (`tmp<k>`), with byte offset, shape and stride.
+The recording machinery is make_engine_schedule.recording, with make_pit_schedule.py's Recorder: every _lib entry
+point the forward reaches is replaced by a recorder and torch.cuda.current_stream is stubbed, so CCT.forward_fused
+runs on CPU tensors and nothing computes.  A tensor is stored as the input image (`img`), as a buffer of the
+classifier's workspace (`ws.<name>`), as a prepared weight (its key -- `conv<i>`, `seq.*`, `enc.*`, `head.*` -- and a
+digest of its bytes), or as the k-th intermediate buffer the forward allocated (`tmp<k>`), with byte offset, shape and
+stride.
 """
 from __future__ import annotations
 
-import contextlib
 import os
 import sys
-import types
 from typing import Dict, List
 
 import torch
@@ -64,37 +63,13 @@ class _Weights:
         return out
 
 
-@contextlib.contextmanager
-def recording(model, img: torch.Tensor, ln_mode: str, host_loop: str):
-    """make_pit_schedule.recording over this file's entry points and buffers."""
-    def owners():
-        return [("img", img)] + [(f"ws.{k}", v) for k, v in model.classifier.engine().slot.t.items()]
-    rec = PS.Recorder(_Weights(model), owners)
-    names = S.ENTRY_POINTS + EXTRA_ENTRY_POINTS
-    saved = {n: getattr(_lib, n) for n in names}
-    saved_stream = torch.cuda.current_stream
-    saved_env = {k: os.environ.get(k) for k in ("B200VIT_LN_MODE", "B200VIT_HOST_LOOP")}
-    try:
-        for n, f in saved.items():
-            setattr(_lib, n, rec.recorder(n, f))
-        torch.cuda.current_stream = lambda device=None: types.SimpleNamespace(cuda_stream=0)
-        os.environ["B200VIT_LN_MODE"], os.environ["B200VIT_HOST_LOOP"] = ln_mode, host_loop
-        yield rec
-    finally:
-        for n, f in saved.items():
-            setattr(_lib, n, f)
-        torch.cuda.current_stream = saved_stream
-        for k, v in saved_env.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-
-
 def record(ln_mode: str, host_loop: str) -> List[dict]:
     model = build()
     img = torch.zeros(*INPUT, dtype=torch.bfloat16)
-    with recording(model, img, ln_mode, host_loop) as rec:
+
+    def owners():
+        return [("img", img)] + [(f"ws.{k}", v) for k, v in model.classifier.engine().slot.t.items()]
+    with S.recording(_Weights(model), owners, ln_mode, host_loop, EXTRA_ENTRY_POINTS, PS.Recorder) as rec:
         model.forward_fused(img)
     return rec.calls
 

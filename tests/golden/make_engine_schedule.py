@@ -239,11 +239,12 @@ class Recorder:
 
 
 @contextlib.contextmanager
-def recording(eng, owners: Callable[[], List[tuple]], ln_mode: str, host_loop: str):
-    """Within: the _lib entry points record into the yielded Recorder's `calls`, torch.cuda.current_stream is stubbed
-    and B200VIT_LN_MODE / B200VIT_HOST_LOOP are set."""
-    rec = Recorder(eng, owners)
-    saved = {n: getattr(_lib, n) for n in ENTRY_POINTS}
+def recording(eng, owners: Callable[[], List[tuple]], ln_mode: str, host_loop: str, extra_entry_points=(),
+              recorder=Recorder):
+    """Within: ENTRY_POINTS and `extra_entry_points` of _lib record into the yielded `recorder(eng, owners)`'s
+    `calls`, torch.cuda.current_stream is stubbed and B200VIT_LN_MODE / B200VIT_HOST_LOOP are set."""
+    rec = recorder(eng, owners)
+    saved = {n: getattr(_lib, n) for n in ENTRY_POINTS + tuple(extra_entry_points)}
     saved_stream = torch.cuda.current_stream
     saved_env = {k: os.environ.get(k) for k in ("B200VIT_LN_MODE", "B200VIT_HOST_LOOP")}
     try:

@@ -1,11 +1,5 @@
-"""Recipe of the PiT parity cases (reference pit.py), shared by make_pit_golden.py, which runs the UNMODIFIED reference
-on them, and by the tests, which rebuild the same weights and inputs from the seeds.  The weights are not stored: the
-drop-in's constructor consumes the RNG exactly like the reference's (tests/test_pit.py checks the seeded-init digest),
-and pit.pt keeps a digest of every rebuilt case so a drift in the recipe fails loudly instead of comparing different
-models."""
-import hashlib
-
-import torch
+"""PiT parity cases (reference pit.py), on the shared recipe of parity.py."""
+from parity import Family
 
 BASE = dict(num_classes=7, dim=32, depth=(1, 1), heads=2, mlp_dim=64, dim_head=32, dropout=0., emb_dropout=0.,
             channels=3)
@@ -53,38 +47,7 @@ def case_kwargs(spec: dict) -> dict:
     return kw
 
 
-def pit_model(cls, spec: dict):
-    """`cls` = the reference's PiT (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm affine parameters and every bias are perturbed so they are exercised, then every parameter is rounded to
-    a bf16-representable value, so a bf16 copy of the model holds the same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        for p in model.parameters():
-            p.copy_(p.bfloat16().float())
-    return model
-
-
-def pit_input(spec: dict) -> torch.Tensor:
-    """bf16 images [BATCH, channels, height, width]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    return torch.randn(BATCH, case_kwargs(spec)["channels"], *spec["input"], generator=g).bfloat16()
-
-
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="pit", model="pit.PiT", cases=PIT_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, case_kwargs(spec)["channels"], *spec["input"]),
+    init_seed=INIT_SEED, init={None: INIT_KWARGS})

@@ -1,11 +1,8 @@
-"""Recipe of the N-dimensional ViT parity cases (reference vit_nd.py / vit_nd_rotary.py), shared by
-make_vit_nd_golden.py, which runs the UNMODIFIED reference on them, and by the tests, which rebuild the same weights and
-inputs from the seeds.  The weights are not stored: the drop-ins' constructors consume the RNG exactly like the
-reference's (tests/test_vit_nd.py checks the seeded-init digests), and vit_nd.pt keeps a digest of every rebuilt case
-so a drift in the recipe fails loudly instead of comparing different models."""
-import hashlib
-
-import torch
+"""N-dimensional ViT parity cases (reference vit_nd.py / vit_nd_rotary.py), on the shared recipe of parity.py.  A case's
+`kind` picks the module; the fixture stores both classes' signatures and seeded-init digests by kind.  Its own rules:
+the rotary `freqs` buffer is rounded to bf16 like the parameters, and the rotary model's return_embed output for the
+first sample is stored too."""
+from parity import Family, load, round_buffers, signature
 
 # every case: ViT dims below; `shape` is the input without (batch, channels)
 BASE = dict(num_classes=7, dim=64, depth=2, heads=2, dim_head=32, mlp_dim=96)
@@ -34,38 +31,18 @@ def case_kwargs(spec: dict) -> dict:
     return kw
 
 
-def vit_nd_model(cls, spec: dict):
-    """`cls` = the reference's ViTND (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm affine parameters are perturbed so they are exercised; every parameter AND buffer (the rotary `freqs`)
-    is rounded to bf16-representable values, so a bf16 copy of the model holds the very same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        for t in list(model.parameters()) + list(model.buffers()):
-            t.copy_(t.bfloat16().float())
-    return model
+KINDS = ("vit_nd", "vit_nd_rotary")
 
 
-def vit_nd_input(spec: dict) -> torch.Tensor:
-    """bf16 input [BATCH, channels, *shape]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    return torch.randn(BATCH, spec["channels"], *spec["shape"], generator=g).bfloat16()
+def embed(model, x, spec) -> dict:
+    rotary = spec["kind"] == "vit_nd_rotary"
+    return {"embed0_fp32": model(x.float(), return_embed=True)[:1].clone() if rotary else None}
 
 
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="vit_nd", model="vit_nd.ViTND", cases=VIT_ND_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, spec["channels"], *spec["shape"]),
+    init_seed=INIT_SEED, init={kind: INIT_KWARGS for kind in KINDS},
+    make=lambda package, spec: load(package, f"{spec['kind']}.ViTND"),
+    signatures=lambda package: {"signature": {k: signature(load(package, f"{k}.ViTND")) for k in KINDS}},
+    after=lambda model, g, spec: round_buffers(model), embed=embed)

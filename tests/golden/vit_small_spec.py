@@ -1,11 +1,7 @@
-"""Recipe of the vit_for_small_dataset parity cases (reference vit_for_small_dataset.py), shared by
-make_vit_small_golden.py, which runs the UNMODIFIED reference on them, and by the tests, which rebuild the same weights
-and inputs from the seeds.  The weights are not stored: the drop-in's constructor consumes the RNG exactly like the
-reference's (tests/test_vit_small_dataset.py checks the seeded-init digests), and vit_small.pt keeps a digest of every
-rebuilt case so a drift in the recipe fails loudly instead of comparing different models."""
-import hashlib
-
-import torch
+"""vit_for_small_dataset parity cases (reference vit_for_small_dataset.py), on the shared recipe of parity.py.  Its own
+rule: every layer's `temperature` moves by a different amount per layer, since its default is exactly
+log(dim_head ** -0.5) and a path that ignored it would match."""
+from parity import Family
 
 BASE = dict(num_classes=7, dim=64, depth=2, heads=2, dim_head=32, mlp_dim=96)
 BATCH = 3
@@ -37,41 +33,12 @@ def case_kwargs(spec: dict) -> dict:
                 pool=spec["pool"], **kw)
 
 
-def vit_small_model(cls, spec: dict):
-    """`cls` = the reference's ViT (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm affine parameters are perturbed so they are exercised, and so is every layer's `temperature`, by a
-    different amount per layer: its default is exactly log(dim_head ** -0.5), so a path that ignored it would match.
-    Every parameter is then rounded to bf16-representable values, so a bf16 copy of the model holds the same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        for i, layer in enumerate(model.transformer.layers):
-            layer[0].temperature.add_(0.3 * (i + 1) * (-1) ** i)
-        for t in model.parameters():
-            t.copy_(t.bfloat16().float())
-    return model
+def after(model, g, spec) -> None:
+    for i, layer in enumerate(model.transformer.layers):
+        layer[0].temperature.add_(0.3 * (i + 1) * (-1) ** i)
 
 
-def vit_small_input(spec: dict) -> torch.Tensor:
-    """bf16 images [BATCH, channels, height, width]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    return torch.randn(BATCH, spec["channels"], *spec["input"], generator=g).bfloat16()
-
-
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="vit_small", model="vit_for_small_dataset.ViT", cases=VIT_SMALL_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, spec["channels"], *spec["input"]),
+    init_seed=INIT_SEED, init={pool: dict(INIT_KWARGS, pool=pool) for pool in ("cls", "mean")}, after=after)

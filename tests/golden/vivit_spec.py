@@ -1,11 +1,8 @@
-"""Recipe of the ViViT parity cases (reference vivit.py), shared by make_vivit_golden.py, which runs the UNMODIFIED
-reference on them, and by the tests, which rebuild the same weights, inputs and frame masks from the seeds.  The weights
-are not stored: the drop-in's constructor consumes the RNG exactly like the reference's (tests/test_vivit.py checks the
-seeded-init digests), and vivit.pt keeps a digest of every rebuilt case so a drift in the recipe fails loudly instead of
-comparing different models."""
-import hashlib
-
+"""ViViT parity cases (reference vivit.py), on the shared recipe of parity.py.  Every case stores the logits of each
+frame-mask kind."""
 import torch
+
+from parity import Family
 
 BASE = dict(num_classes=7, dim=64, spatial_depth=2, temporal_depth=2, heads=2, dim_head=32, mlp_dim=96)
 BATCH = 3
@@ -31,6 +28,7 @@ VIVIT_CASES["fe_cls_pf1_p16"] = dict(seed=53, variant="factorized_encoder", pool
                                      input=(3, 32, 32), image_size=32, image_patch_size=16, frames=3,
                                      frame_patch_size=1, channels=3)
 MASK_KINDS = ("none", "partial", "full")
+VARIANTS = ("factorized_encoder", "factorized_self_attention")
 # the seeded-init (unperturbed) comparison
 INIT_SEED = 123
 INIT_KWARGS = dict(image_size=(16, 24), image_patch_size=8, frames=8, frame_patch_size=2, channels=3, **BASE)
@@ -40,30 +38,6 @@ def case_kwargs(spec: dict) -> dict:
     return dict(image_size=spec["image_size"], image_patch_size=spec["image_patch_size"], frames=spec["frames"],
                 frame_patch_size=spec["frame_patch_size"], channels=spec["channels"], pool=spec["pool"],
                 variant=spec["variant"], use_flash_attn=spec["use_flash_attn"], **BASE)
-
-
-def vivit_model(cls, spec: dict):
-    """`cls` = the reference's ViViT (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm affine parameters are perturbed so they are exercised; every parameter is rounded to bf16-representable
-    values, so a bf16 copy of the model holds the very same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        for t in model.parameters():
-            t.copy_(t.bfloat16().float())
-    return model
-
-
-def vivit_input(spec: dict) -> torch.Tensor:
-    """bf16 video [BATCH, channels, frames, height, width]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    return torch.randn(BATCH, spec["channels"], *spec["input"], generator=g).bfloat16()
 
 
 def vivit_mask(spec: dict, kind: str):
@@ -84,14 +58,8 @@ def vivit_mask(spec: dict, kind: str):
     return m
 
 
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="vivit", model="vivit.ViViT", cases=VIVIT_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, spec["channels"], *spec["input"]),
+    init_seed=INIT_SEED, init={v: dict(INIT_KWARGS, variant=v) for v in VARIANTS},
+    forwards=lambda spec: [(kind, {"mask": vivit_mask(spec, kind)}) for kind in MASK_KINDS])

@@ -1,12 +1,9 @@
-"""Recipe of the XCiT parity cases (reference xcit.py), shared by make_xcit_golden.py, which runs the UNMODIFIED
-reference on them, and by the tests, which rebuild the same weights and inputs from the seeds.  The weights are not
-stored: the drop-in's constructor consumes the RNG exactly like the reference's (tests/test_xcit.py checks the
-seeded-init digests), and xcit.pt keeps a digest of every rebuilt case so a drift in the recipe fails loudly instead of
-comparing different models."""
-import hashlib
-import random
-
+"""XCiT parity cases (reference xcit.py), on the shared recipe of parity.py.  Its own rules: the LayerScale vectors
+are scaled by 1 + 0.5 N(0, 1), every temperature gets `tau` plus N(0, 0.3), the BatchNorm running statistics are
+perturbed and rounded to bf16 like the parameters, and layer dropout is seeded right before every forward."""
 import torch
+
+from parity import Family, round_buffers, seed_layer_dropout
 
 BASE = dict(num_classes=7, dim=64, depth=2, cls_depth=2, heads=4, mlp_dim=96, dim_head=32, dropout=0.,
             emb_dropout=0., local_patch_kernel_size=3, layer_dropout=0.)
@@ -57,56 +54,23 @@ def case_kwargs(spec: dict) -> dict:
     return kw
 
 
-def xcit_model(cls, spec: dict):
-    """`cls` = the reference's XCiT (generator) or the drop-in's (tests): the same fp32 model from the same seeds.
-    LayerNorm and BatchNorm affine parameters, LayerScale vectors, temperatures and the BatchNorm running statistics are
-    perturbed so they are exercised, then every parameter and floating-point buffer is rounded to bf16-representable
-    values, so a bf16 copy of the model holds the same numbers."""
-    torch.manual_seed(spec["seed"])
-    model = cls(**case_kwargs(spec)).eval()
-    g = torch.Generator().manual_seed(1000 + spec["seed"])
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if p.dim() == 1 and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 and n.endswith("bias"):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-            elif n.endswith(".scale"):                          # LayerScale (dim,)
-                p.mul_(1 + 0.5 * torch.randn(p.shape, generator=g))
-            elif n.endswith("temperature"):
-                p.add_(spec.get("tau", 0.0) + 0.3 * torch.randn(p.shape, generator=g))
-        for n, b in model.named_buffers():
-            if n.endswith("running_mean"):
-                b.add_(0.2 * torch.randn(b.shape, generator=g))
-            elif n.endswith("running_var"):
-                b.mul_(0.5 + torch.rand(b.shape, generator=g))
-        for t in list(model.parameters()) + [b for b in model.buffers() if b.is_floating_point()]:
-            t.copy_(t.bfloat16().float())
-    return model
+def extra(n, p, g, spec) -> None:
+    if n.endswith(".scale"):                                    # LayerScale (dim,)
+        p.mul_(1 + 0.5 * torch.randn(p.shape, generator=g))
+    elif n.endswith("temperature"):
+        p.add_(spec.get("tau", 0.0) + 0.3 * torch.randn(p.shape, generator=g))
 
 
-def seed_layer_dropout(spec: dict) -> None:
-    """Seed the generators layer dropout draws from (torch's CPU generator, and `random` when every layer would be
-    dropped) right before a forward, so that every run of the case keeps the same layers."""
-    if "drop_seed" in spec:
-        torch.manual_seed(spec["drop_seed"])
-        random.seed(spec["drop_seed"])
+def after(model, g, spec) -> None:
+    for n, b in model.named_buffers():
+        if n.endswith("running_mean"):
+            b.add_(0.2 * torch.randn(b.shape, generator=g))
+        elif n.endswith("running_var"):
+            b.mul_(0.5 + torch.rand(b.shape, generator=g))
+    round_buffers(model)
 
 
-def xcit_input(spec: dict) -> torch.Tensor:
-    """bf16 images [BATCH, 3, height, width]."""
-    g = torch.Generator().manual_seed(100 + spec["seed"])
-    return torch.randn(BATCH, 3, *spec["input"], generator=g).bfloat16()
-
-
-def weights_digest(model) -> str:
-    """One sha256 over every state_dict entry (name, shape, dtype, bytes) in registration order."""
-    h = hashlib.sha256()
-    for k, v in model.state_dict().items():
-        h.update(f"{k}{tuple(v.shape)}{v.dtype}".encode())
-        h.update(v.detach().float().contiguous().cpu().numpy().tobytes())
-    return h.hexdigest()
-
-
-def input_digest(x: torch.Tensor) -> str:
-    return hashlib.sha256(x.float().contiguous().numpy().tobytes()).hexdigest()
+FAMILY = Family(
+    name="xcit", model="xcit.XCiT", cases=XCIT_CASES, case_kwargs=case_kwargs,
+    input_shape=lambda spec: (BATCH, 3, *spec["input"]),
+    init_seed=INIT_SEED, init={None: INIT_KWARGS}, extra=extra, after=after, before_forward=seed_layer_dropout)

@@ -1,6 +1,6 @@
-"""CaiT (vit_pytorch_b200.cait) without a GPU: drop-in surface against the reference's stored signature, init digest
-and fp32 logits (tests/golden/cait.pt, made by make_cait_golden.py), the eager graph's hooks, and the argument checks
-of the two talking-heads attention entry points."""
+"""CaiT (vit_pytorch_b200.cait) without a GPU: the attribute surface, the seeded cases' layer dropout and mixing-matrix
+orientation, the eager graph's hooks, and the argument checks of the two talking-heads attention entry points.  The
+reference-parity tests are in test_family_parity.py."""
 import ctypes
 import os
 import sys
@@ -8,29 +8,17 @@ import sys
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, ROOT, load_golden, signature, state_digest
+from conftest import GOLDEN_DIR, ROOT, load_golden
 from vit_pytorch_b200 import _lib, build
 from vit_pytorch_b200.cait import Attention, CaiT, LayerScale, Transformer
 
 sys.path.insert(0, GOLDEN_DIR)
-from cait_spec import (CAIT_CASES, INIT_KWARGS, INIT_SEED, cait_input, cait_model, input_digest,  # noqa: E402
-                       seed_layer_dropout, weights_digest)
+from cait_spec import CAIT_CASES, FAMILY, INIT_KWARGS  # noqa: E402
 
 
 @pytest.fixture(scope="module")
 def golden():
     return load_golden("cait")
-
-
-def test_signature_matches_reference(golden):
-    assert signature(CaiT) == golden["signature"]
-
-
-def test_seeded_init_matches_reference(golden):
-    torch.manual_seed(INIT_SEED)
-    sd = CaiT(**INIT_KWARGS).state_dict()
-    assert list(sd) == list(golden["init"])                # names and registration order
-    assert state_digest(sd) == golden["init"]              # shapes, dtypes and the bytes of every tensor
 
 
 def test_layer_scale_init_follows_the_layer_index():
@@ -51,28 +39,13 @@ def test_attribute_surface():
     assert isinstance(m.cls_transformer, Transformer) and not hasattr(m.patch_transformer, "norm")
 
 
-@pytest.mark.parametrize("name", sorted(CAIT_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    """Weights (LayerNorms, LayerScale vectors and mixing matrices perturbed) and input rebuilt from the seeds are the
-    ones the reference ran; the drop-in's PyTorch graph reproduces its fp32 logits, the layer-dropout case included."""
-    case, spec = golden["cases"][name], CAIT_CASES[name]
-    assert case["spec"] == spec
-    m = cait_model(CaiT, spec)
-    x = cait_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    seed_layer_dropout(spec)
-    with torch.inference_mode():
-        out = m(x.float())
-    assert torch.allclose(out, case["logits_fp32"], atol=1e-5, rtol=1e-5), (out - case["logits_fp32"]).abs().max()
-
-
 def test_layer_dropout_case_drops_layers(golden):
     """The seeded layer-dropout case runs a strict subset: with every layer it gives other logits."""
     spec = dict(CAIT_CASES["readme_layer_dropout"])
-    m = cait_model(CaiT, spec)
+    m = FAMILY.build(spec)
     m.patch_transformer.layer_dropout = m.cls_transformer.layer_dropout = 0.0
     with torch.inference_mode():
-        out = m(cait_input(spec).float())
+        out = m(FAMILY.input(spec).float())
     assert (out - golden["cases"]["readme_layer_dropout"]["logits_fp32"]).abs().max() > 1e-3
 
 
@@ -81,14 +54,14 @@ def test_transposed_mixing_matrix_changes_the_logits(golden, which):
     """The einsums 'b h i j, h g -> b g i j' index both matrices [input head][output head]: a transpose is a different
     model, so the goldens pin the orientation of each."""
     spec = CAIT_CASES["dh32_n64"]
-    m = cait_model(CaiT, spec)
+    m = FAMILY.build(spec)
     with torch.no_grad():
         for t in (m.patch_transformer, m.cls_transformer):
             for ls, _ in t.layers:
                 w = getattr(ls.fn, which)
                 w.copy_(w.t().contiguous())
     with torch.inference_mode():
-        out = m(cait_input(spec).float())
+        out = m(FAMILY.input(spec).float())
     assert (out - golden["cases"]["dh32_n64"]["logits_fp32"]).abs().max() > 1e-3
 
 

@@ -1,9 +1,8 @@
-"""CCT (vit_pytorch_b200.cct) without a GPU: drop-in surface against the reference's stored signatures, init digest and
-fp32 logits (tests/golden/cct.pt, made by make_cct_golden.py), the fallback rules, the prepared conv-weight layout,
-the argument checks of the im2col, ReLU max-pool and sequence-pooling entry points, the post-norm layer's schedule and
-the launch sequence of the whole fused forward (tests/golden/cct_schedule.json, made by make_cct_schedule.py)."""
+"""CCT (vit_pytorch_b200.cct) without a GPU: the sine table and presets, the fallback rules, the prepared conv-weight
+layout, the argument checks of the im2col, ReLU max-pool and sequence-pooling entry points, the post-norm layer's
+schedule and the launch sequence of the whole fused forward (tests/golden/cct_schedule.json, made by
+make_cct_schedule.py).  The reference-parity tests are in test_family_parity.py."""
 import ctypes
-import inspect
 import json
 import os
 import sys
@@ -12,24 +11,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, ROOT, load_golden, state_digest
+from conftest import GOLDEN_DIR, ROOT
 from vit_pytorch_b200 import _lib, build, cct as cct_mod
 from vit_pytorch_b200.cct import CCT, conv_weights, sinusoidal_embedding
 
 sys.path.insert(0, GOLDEN_DIR)
-from cct_spec import CCT_CASES, INIT_KWARGS, INIT_SEED, PRESETS, cct_input, cct_model, input_digest, weights_digest  # noqa: E402,E501
 import make_cct_schedule as CS  # noqa: E402
-
-
-def signature(fn) -> list:
-    """As make_cct_golden.signature: of cls.__init__ for a class, of the function itself otherwise."""
-    target = fn.__init__ if inspect.isclass(fn) else fn
-    return [(k, repr(v.default)) for k, v in inspect.signature(target).parameters.items() if k != "self"]
-
-
-@pytest.fixture(scope="module")
-def golden():
-    return load_golden("cct")
 
 
 @pytest.fixture(scope="module")
@@ -37,34 +24,6 @@ def lib():
     if not _lib.LIB_PATH.exists():
         build.build()
     return _lib.lib()
-
-
-def test_signatures_match_reference(golden):
-    sig = signature
-    assert sig(CCT) == golden["signature"]
-    assert sig(cct_mod._cct) == golden["cct_defaults"]
-    for p in PRESETS:
-        assert sig(getattr(cct_mod, p)) == golden["presets"][p], p
-
-
-def test_seeded_init_matches_reference(golden):
-    torch.manual_seed(INIT_SEED)
-    sd = CCT(**INIT_KWARGS).state_dict()
-    assert list(sd) == list(golden["init"])                # names and registration order
-    assert state_digest(sd) == golden["init"]              # shapes, dtypes and the bytes of every tensor
-
-
-@pytest.mark.parametrize("name", sorted(CCT_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    case, spec = golden["cases"][name], CCT_CASES[name]
-    assert case["spec"] == spec
-    m = cct_model(cct_mod, spec)
-    x = cct_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    assert m.classifier.sequence_length == case["sequence_length"]
-    with torch.inference_mode():
-        out = m(x.float())
-    assert torch.allclose(out, case["logits_fp32"], atol=1e-5, rtol=1e-5), (out - case["logits_fp32"]).abs().max()
 
 
 def test_sine_table_and_presets():

@@ -1,6 +1,5 @@
-"""CrossViT (vit_pytorch_b200.cross_vit) without a GPU: drop-in surface against the reference's stored signature, init
-digests and fp32 logits (tests/golden/cross_vit.pt, made by make_cross_vit_golden.py), the eager graph's hooks, and
-the argument checks of b200vit_attention_cls."""
+"""CrossViT (vit_pytorch_b200.cross_vit) without a GPU: the attribute surface, the eager graph's hooks, and the
+argument checks of b200vit_attention_cls.  The reference-parity tests are in test_family_parity.py."""
 import ctypes
 import os
 import sys
@@ -9,33 +8,13 @@ import pytest
 import torch
 from torch import nn
 
-from conftest import GOLDEN_DIR, ROOT, load_golden, signature, state_digest
+from conftest import GOLDEN_DIR, ROOT
 from vit_pytorch_b200 import _lib, build
 from vit_pytorch_b200.cross_vit import (Attention, CrossTransformer, CrossViT, ImageEmbedder, MultiScaleEncoder,
                                         ProjectInOut, Transformer)
 
 sys.path.insert(0, GOLDEN_DIR)
-from cross_vit_spec import (CROSS_VIT_CASES, INIT_KWARGS, INIT_SEED, cross_vit_input, cross_vit_model,  # noqa: E402
-                            input_digest, weights_digest)
-
-
-@pytest.fixture(scope="module")
-def golden():
-    return load_golden("cross_vit")
-
-
-def test_signature_matches_reference(golden):
-    assert signature(CrossViT) == golden["signature"]
-
-
-@pytest.mark.parametrize("name", ["widths", "equal"])
-def test_seeded_init_matches_reference(golden, name):
-    init = golden["init"][name]
-    kw = dict(INIT_KWARGS, **({} if name == "widths" else dict(lg_dim=INIT_KWARGS["sm_dim"])))
-    torch.manual_seed(INIT_SEED)
-    sd = CrossViT(**kw).state_dict()
-    assert list(sd) == list(init)                          # names and registration order
-    assert state_digest(sd) == init                        # shapes, dtypes and the bytes of every tensor
+from cross_vit_spec import CROSS_VIT_CASES, FAMILY, INIT_KWARGS  # noqa: E402
 
 
 def test_attribute_surface():
@@ -58,32 +37,18 @@ def test_attribute_surface():
     assert m.sm_mlp_head[1].out_features == 7 and m.lg_mlp_head[0].normalized_shape == (64,)
 
 
-@pytest.mark.parametrize("name", sorted(CROSS_VIT_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    """Weights and input rebuilt from the seeds are the ones the reference ran; the drop-in's PyTorch graph
-    reproduces its fp32 logits."""
-    case, spec = golden["cases"][name], CROSS_VIT_CASES[name]
-    assert case["spec"] == spec
-    m = cross_vit_model(CrossViT, spec)
-    x = cross_vit_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    with torch.inference_mode():
-        assert m.fused_reason(x.float()) == "input is not on a CUDA device"
-        torch.testing.assert_close(m(x.float()), case["logits_fp32"], rtol=0, atol=1e-5)
-
-
 def test_eager_graph_keeps_hooks_observable():
     """Recorder-style hooks on the cross-attention softmax fire on the PyTorch graph: one query row over the query
     token itself plus the other stream's patch tokens."""
     spec = CROSS_VIT_CASES["widths_32_64"]
-    m = cross_vit_model(CrossViT, spec)
+    m = FAMILY.build(spec)
     seen = []
     for mse_layer in m.multi_scale_encoder.layers:
         for sm_lg, lg_sm in mse_layer[2].layers:
             sm_lg.fn.attend.register_forward_hook(lambda mod, i, o: seen.append(("sm", o)))
             lg_sm.fn.attend.register_forward_hook(lambda mod, i, o: seen.append(("lg", o)))
     with torch.inference_mode():
-        m(cross_vit_input(spec).float())
+        m(FAMILY.input(spec).float())
     assert len(seen) == 2 * 2 * 2
     assert seen[0][0] == "sm" and seen[0][1].shape == (3, 2, 1, 1 + 16)     # self + 16 lg patches
     assert seen[1][0] == "lg" and seen[1][1].shape == (3, 2, 1, 1 + 64)     # self + 64 sm patches

@@ -1,6 +1,6 @@
-"""DeepViT (vit_pytorch_b200.deepvit) without a GPU: drop-in surface against the reference's stored signature, init
-digests and fp32 logits (tests/golden/deepvit.pt, made by make_deepvit_golden.py), the eager graph's hooks, and the
-argument checks of the head-mixing attention entry point."""
+"""DeepViT (vit_pytorch_b200.deepvit) without a GPU: the attribute surface, the mixing-matrix orientation, the eager
+graph's hooks, and the argument checks of the head-mixing attention entry point.  The reference-parity tests are in
+test_family_parity.py."""
 import ctypes
 import os
 import sys
@@ -8,31 +8,17 @@ import sys
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, ROOT, load_golden, signature, state_digest
+from conftest import GOLDEN_DIR, ROOT, load_golden
 from vit_pytorch_b200 import _lib, build
 from vit_pytorch_b200.deepvit import Attention, DeepViT, Transformer
 
 sys.path.insert(0, GOLDEN_DIR)
-from deepvit_spec import (DEEPVIT_CASES, INIT_KWARGS, INIT_SEED, deepvit_input, deepvit_model,  # noqa: E402
-                          input_digest, weights_digest)
+from deepvit_spec import DEEPVIT_CASES, FAMILY, INIT_KWARGS  # noqa: E402
 
 
 @pytest.fixture(scope="module")
 def golden():
     return load_golden("deepvit")
-
-
-def test_signature_matches_reference(golden):
-    assert signature(DeepViT) == golden["signature"]
-
-
-@pytest.mark.parametrize("pool", ["cls", "mean"])
-def test_seeded_init_matches_reference(golden, pool):
-    init = golden["init"][pool]
-    torch.manual_seed(INIT_SEED)
-    sd = DeepViT(**{**INIT_KWARGS, "pool": pool}).state_dict()
-    assert list(sd) == list(init)                          # names and registration order
-    assert state_digest(sd) == init                        # shapes, dtypes and the bytes of every tensor
 
 
 def test_attribute_surface():
@@ -47,30 +33,16 @@ def test_attribute_surface():
     assert names[:2] == ["reattn_weights", "norm.weight"]
 
 
-@pytest.mark.parametrize("name", sorted(DEEPVIT_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    """Weights (re-attention matrices and head LayerNorms perturbed per layer) and input rebuilt from the seeds are the
-    ones the reference ran; the drop-in's PyTorch graph reproduces its fp32 logits."""
-    case, spec = golden["cases"][name], DEEPVIT_CASES[name]
-    assert case["spec"] == spec
-    m = deepvit_model(DeepViT, spec)
-    x = deepvit_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    with torch.inference_mode():
-        out = m(x.float())
-    assert torch.allclose(out, case["logits_fp32"], atol=1e-5, rtol=1e-5), (out - case["logits_fp32"]).abs().max()
-
-
 def test_transposed_mixing_matrix_changes_the_logits(golden):
     """The einsum 'b h i j, h g -> b g i j' indexes the matrix [input head][output head]: its transpose is a different
     model, so the goldens pin the orientation."""
     spec = DEEPVIT_CASES["dh32_n65"]
-    m = deepvit_model(DeepViT, spec)
+    m = FAMILY.build(spec)
     with torch.no_grad():
         for attn, _ in m.transformer.layers:
             attn.reattn_weights.copy_(attn.reattn_weights.t().contiguous())
     with torch.inference_mode():
-        out = m(deepvit_input(spec).float())
+        out = m(FAMILY.input(spec).float())
     assert (out - golden["cases"]["dh32_n65"]["logits_fp32"]).abs().max() > 1e-2
 
 

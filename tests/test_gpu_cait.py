@@ -1,19 +1,19 @@
 """-m gpu: the talking-heads attention kernels (b200vit_attention_headmix_ex with a pre-softmax mix,
 b200vit_attention_cls_headmix) and the fused CaiT on the H100.  The kernels are checked against fp32 torch expressions
-on the same bf16 data; the model against the reference's stored fp32 logits (tests/golden/cait.pt) and the module's
-own eager bf16 graph."""
+on the same bf16 data; the model's CUDA-graph replay and fallback rules (its reference parity is in
+test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.cait import CaiT, Transformer
 
 sys.path.insert(0, GOLDEN_DIR)
-from cait_spec import CAIT_CASES, cait_input, cait_model, seed_layer_dropout, weights_digest  # noqa: E402
+from cait_spec import CAIT_CASES, FAMILY  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -116,43 +116,11 @@ def test_attention_cls_headmix_against_fp32(H, dh, n, first):
 
 
 # ------------------------------------------------------------------------------------------------ model
-def _eager_bf16(m, x, spec, monkeypatch):
-    """The module's own PyTorch graph in bf16 (every submodule), with the case's layer-dropout seed."""
-    with monkeypatch.context() as mp:
-        mp.setenv("B200VIT_DISABLE_FUSED", "1")
-        seed_layer_dropout(spec)
-        with torch.inference_mode():
-            return m(x)
-
-
-@pytest.mark.parametrize("ln_mode", ["fold", "exact"])
-@pytest.mark.parametrize("name", sorted(CAIT_CASES))
-def test_fused_against_reference_goldens(name, ln_mode, monkeypatch):
-    monkeypatch.setenv("B200VIT_LN_MODE", ln_mode)
-    case, spec = load_golden("cait")["cases"][name], CAIT_CASES[name]
-    ref = cait_model(CaiT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = cait_input(spec).to(DEV)
-    m = cait_model(CaiT, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        seed_layer_dropout(spec)
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0
-    eager = _eager_bf16(m, x, spec, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} {ln_mode} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 3e-2, (what, mx, frac)
-
-
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = CAIT_CASES["n576_h8"]
-    m = cait_model(CaiT, spec).to(DEV, torch.bfloat16)
-    a = cait_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()
@@ -164,9 +132,9 @@ def test_cuda_graph_replay_is_bit_identical():
 def test_cuda_graph_refused_with_layer_dropout():
     from vit_pytorch_b200.graph import GraphedForward
     spec = CAIT_CASES["dh32_n64"]
-    m = cait_model(CaiT, {**spec, "layer_dropout": 0.1}).to(DEV, torch.bfloat16)
+    m = FAMILY.build({**spec, "layer_dropout": 0.1}).to(DEV, torch.bfloat16)
     with pytest.raises(RuntimeError, match="layer_dropout"):
-        GraphedForward(m, cait_input(spec).to(DEV))
+        GraphedForward(m, FAMILY.input(spec).to(DEV))
 
 
 def test_direct_patch_transformer_call():

@@ -1,20 +1,20 @@
 """-m gpu: the convolutional tokenizer's kernels (b200vit_conv_im2col_nchw / _nhwc, b200vit_relu_maxpool), the
 sequence-pooling kernel (b200vit_seq_pool), the post-norm encoder layer and the fused CCT on the H100.  The im2col
 and the pool are checked bit for bit against F.unfold and F.max_pool2d; the sequence pooling and the post-norm layer
-against fp64 references; the model against the reference's stored fp32 logits (tests/golden/cct.pt) and the module's
-own eager bf16 graph."""
+against fp64 references; the model's CUDA-graph replay and weight updates (its reference parity is in
+test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib, cct as cct_mod
 from vit_pytorch_b200.cct import CCT, TransformerClassifier
 
 sys.path.insert(0, GOLDEN_DIR)
-from cct_spec import CCT_CASES, cct_input, cct_model, weights_digest  # noqa: E402
+from cct_spec import CCT_CASES, FAMILY  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -238,35 +238,6 @@ def test_post_norm_layer_against_fp64(ln_mode, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ model
-def _eager_bf16(m, x, monkeypatch):
-    with monkeypatch.context() as mp:
-        mp.setenv("B200VIT_DISABLE_FUSED", "1")
-        with torch.inference_mode():
-            return m(x)
-
-
-@pytest.mark.parametrize("ln_mode", ["fold", "exact"])
-@pytest.mark.parametrize("name", sorted(CCT_CASES))
-def test_fused_against_reference_goldens(name, ln_mode, monkeypatch):
-    monkeypatch.setenv("B200VIT_LN_MODE", ln_mode)
-    case, spec = load_golden("cct")["cases"][name], CCT_CASES[name]
-    ref = cct_model(cct_mod, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = cct_input(spec).to(DEV)
-    m = cct_model(cct_mod, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0
-    eager = _eager_bf16(m, x, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} {ln_mode} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 3e-2, (what, mx, frac)
-
-
 README_CCT = dict(img_size=(224, 448), embedding_dim=384, n_conv_layers=2, kernel_size=7, stride=2, padding=3,
                   pooling_kernel_size=3, pooling_stride=2, pooling_padding=1, num_layers=14, num_heads=6, mlp_ratio=3.,
                   num_classes=1000, positional_embedding='learnable')
@@ -288,8 +259,8 @@ def test_readme_configs_take_the_fused_path():
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = CCT_CASES["two_layers_k7_nonsquare"]
-    m = cct_model(cct_mod, spec).to(DEV, torch.bfloat16)
-    a = cct_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()
@@ -302,15 +273,15 @@ def test_weight_updates_reach_the_fused_output():
     """load_state_dict and in-place updates of a conv weight, the pooling Linear and the positional table all rebuild
     the prepared weights: afterwards the fused output equals, bit for bit, that of a fresh model with the same state."""
     spec = CCT_CASES["learnable"]
-    m = cct_model(cct_mod, spec).to(DEV, torch.bfloat16)
-    x = cct_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         before = m(x).clone()
     with torch.no_grad():
         m.tokenizer.conv_layers[0][0].weight.mul_(-1.0)
         m.classifier.attention_pool.weight.mul_(3.0)
         m.classifier.positional_emb.add_(0.25)
-    fresh = cct_model(cct_mod, spec).to(DEV, torch.bfloat16)
+    fresh = FAMILY.build(spec).to(DEV, torch.bfloat16)
     with torch.inference_mode():
         fresh(x)                                          # prepares fresh's weights from the old state first
     fresh.load_state_dict(m.state_dict())

@@ -1,18 +1,18 @@
 """-m gpu: the class-token cross-attention kernel and the fused CrossViT on the H100.  The kernel is checked against an
-fp32 torch expression on the same bf16 data; the model against the reference's stored fp32 logits
-(tests/golden/cross_vit.pt) and the module's own eager bf16 graph."""
+fp32 torch expression on the same bf16 data; the model at batch one and its fallback rules
+(its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.cross_vit import CrossViT, Transformer
 from vit_pytorch_b200.extractor import Extractor
 
 sys.path.insert(0, GOLDEN_DIR)
-from cross_vit_spec import CROSS_VIT_CASES, cross_vit_input, cross_vit_model, weights_digest  # noqa: E402
+from cross_vit_spec import CROSS_VIT_CASES, FAMILY  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -83,33 +83,13 @@ def _eager_bf16(m, x, monkeypatch, *args):
             return m(x, *args)
 
 
-@pytest.mark.parametrize("name", sorted(CROSS_VIT_CASES))
-def test_fused_against_reference_goldens(name, monkeypatch):
-    case, spec = load_golden("cross_vit")["cases"][name], CROSS_VIT_CASES[name]
-    ref = cross_vit_model(CrossViT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = cross_vit_input(spec).to(DEV)
-    m = cross_vit_model(CrossViT, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0 and out.shape == (3, 7)
-    eager = _eager_bf16(m, x, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 2e-2, (what, mx, frac)
-
-
 def test_batch_one(monkeypatch):
     spec = CROSS_VIT_CASES["widths_32_64"]
-    m = cross_vit_model(CrossViT, spec).to(DEV, torch.bfloat16)
-    x = cross_vit_input(spec).to(DEV)[:1]
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)[:1]
     with torch.inference_mode():
         out = m(x)
-        batched = m(cross_vit_input(spec).to(DEV))[:1]
+        batched = m(FAMILY.input(spec).to(DEV))[:1]
     eager = _eager_bf16(m, x, monkeypatch)
     assert out.shape == (1, 7)
     assert stats(out, eager)[0] < 3e-2 and stats(out, batched)[0] < 3e-2
@@ -117,7 +97,7 @@ def test_batch_one(monkeypatch):
 
 def test_direct_multi_scale_encoder_and_transformer_calls(monkeypatch):
     spec = CROSS_VIT_CASES["widths_32_64"]
-    m = cross_vit_model(CrossViT, spec).to(DEV, torch.bfloat16)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
     mse = m.multi_scale_encoder
     torch.manual_seed(0)
     sm = torch.randn(3, 65, 32, device=DEV).bfloat16()
@@ -144,8 +124,8 @@ def test_direct_multi_scale_encoder_and_transformer_calls(monkeypatch):
 
 def test_extractor_on_multi_scale_encoder_stays_fused(monkeypatch):
     spec = CROSS_VIT_CASES["widths_32_64"]
-    m = cross_vit_model(CrossViT, spec).to(DEV, torch.bfloat16)
-    x = cross_vit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         plain = m(x)
     v = Extractor(m, layer_name='multi_scale_encoder')
@@ -172,8 +152,8 @@ def test_extractor_on_multi_scale_encoder_stays_fused(monkeypatch):
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = CROSS_VIT_CASES["widths_32_64"]
-    m = cross_vit_model(CrossViT, spec).to(DEV, torch.bfloat16)
-    a = cross_vit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()

@@ -1,18 +1,18 @@
 """-m gpu: the head-mixing attention kernel (b200vit_attention_headmix) and the fused DeepViT on the H100.  The kernel
-is checked against an fp32 torch expression on the same bf16 data; the model against the reference's stored fp32
-logits (tests/golden/deepvit.pt) and the module's own eager bf16 graph."""
+is checked against an fp32 torch expression on the same bf16 data; the model at batch one, its CUDA-graph replay
+and fallback rules (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.deepvit import DeepViT, Transformer
 
 sys.path.insert(0, GOLDEN_DIR)
-from deepvit_spec import DEEPVIT_CASES, deepvit_input, deepvit_model, weights_digest  # noqa: E402
+from deepvit_spec import DEEPVIT_CASES, FAMILY  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -98,32 +98,10 @@ def _eager_bf16(m, x, monkeypatch):
             return m(x)
 
 
-@pytest.mark.parametrize("ln_mode", ["fold", "exact"])
-@pytest.mark.parametrize("name", sorted(DEEPVIT_CASES))
-def test_fused_against_reference_goldens(name, ln_mode, monkeypatch):
-    monkeypatch.setenv("B200VIT_LN_MODE", ln_mode)
-    case, spec = load_golden("deepvit")["cases"][name], DEEPVIT_CASES[name]
-    ref = deepvit_model(DeepViT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = deepvit_input(spec).to(DEV)
-    m = deepvit_model(DeepViT, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0
-    eager = _eager_bf16(m, x, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} {ln_mode} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 3e-2, (what, mx, frac)
-
-
 def test_batch_one(monkeypatch):
     spec = DEEPVIT_CASES["dh48_n197"]
-    m = deepvit_model(DeepViT, spec).to(DEV, torch.bfloat16)
-    x = deepvit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         both = m(x)
         one = m(x[1:2])
@@ -135,8 +113,8 @@ def test_batch_one(monkeypatch):
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = DEEPVIT_CASES["n577_h8"]
-    m = deepvit_model(DeepViT, spec).to(DEV, torch.bfloat16)
-    a = deepvit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()
@@ -148,8 +126,8 @@ def test_cuda_graph_replay_is_bit_identical():
 def test_transformer_hook_keeps_the_fused_path():
     """A hook on .transformer (the Extractor pattern) sees the encoder output while the blocks still run fused."""
     spec = DEEPVIT_CASES["dh32_n65"]
-    m = deepvit_model(DeepViT, spec).to(DEV, torch.bfloat16)
-    x = deepvit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     seen = []
     h = m.transformer.register_forward_hook(lambda mod, i, o: seen.append(o.shape))
     with torch.inference_mode():

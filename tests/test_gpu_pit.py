@@ -1,19 +1,19 @@
 """-m gpu: the overlapping-patch unfold kernel (b200vit_unfold_patches), the pooling kernel (b200vit_pit_pool) and the fused
 PiT on the H100.  The unfold is checked bit for bit against F.unfold; the pool against an fp64 conv2d with a
-per-element bound; the model against the reference's stored fp32 logits (tests/golden/pit.pt) and the module's own
-eager bf16 graph."""
+per-element bound; the model's CUDA-graph replay, weight updates and fallback rules (its reference parity is in
+test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.pit import PiT, Transformer
 
 sys.path.insert(0, GOLDEN_DIR)
-from pit_spec import PIT_CASES, pit_input, pit_model, weights_digest  # noqa: E402
+from pit_spec import FAMILY, PIT_CASES  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -137,35 +137,6 @@ def test_pit_pool_keeps_each_image_to_itself_and_repeats_bits():
 
 
 # ------------------------------------------------------------------------------------------------ model
-def _eager_bf16(m, x, monkeypatch):
-    with monkeypatch.context() as mp:
-        mp.setenv("B200VIT_DISABLE_FUSED", "1")
-        with torch.inference_mode():
-            return m(x)
-
-
-@pytest.mark.parametrize("ln_mode", ["fold", "exact"])
-@pytest.mark.parametrize("name", sorted(PIT_CASES))
-def test_fused_against_reference_goldens(name, ln_mode, monkeypatch):
-    monkeypatch.setenv("B200VIT_LN_MODE", ln_mode)
-    case, spec = load_golden("pit")["cases"][name], PIT_CASES[name]
-    ref = pit_model(PiT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = pit_input(spec).to(DEV)
-    m = pit_model(PiT, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0
-    eager = _eager_bf16(m, x, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} {ln_mode} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 3e-2, (what, mx, frac)
-
-
 def test_readme_config_takes_the_fused_path():
     m = PiT(image_size=224, patch_size=14, dim=256, num_classes=1000, depth=(3, 3, 3), heads=16, mlp_dim=2048,
             dropout=0.1, emb_dropout=0.1).eval().to(DEV, torch.bfloat16)
@@ -200,8 +171,8 @@ def test_direct_transformer_call_runs_fused():
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = PIT_CASES["heads_tuple"]
-    m = pit_model(PiT, spec).to(DEV, torch.bfloat16)
-    a = pit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()
@@ -214,14 +185,14 @@ def test_weight_updates_reach_the_fused_output():
     """load_state_dict and an in-place update of a pool weight both rebuild the prepared weights: afterwards the fused
     output equals, bit for bit, that of a fresh model loaded with the same state."""
     spec = PIT_CASES["heads_tuple"]
-    m = pit_model(PiT, spec).to(DEV, torch.bfloat16)
-    x = pit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         before = m(x).clone()
     with torch.no_grad():
         m.layers[1].downsample.net[0].weight.mul_(-1.0)
         m.layers[3].cls_ff.bias.add_(0.5)
-    fresh = pit_model(PiT, spec).to(DEV, torch.bfloat16)
+    fresh = FAMILY.build(spec).to(DEV, torch.bfloat16)
     with torch.inference_mode():
         fresh(x)                                          # prepares fresh's weights from the old state first
     fresh.load_state_dict(m.state_dict())

@@ -1,13 +1,13 @@
 """-m gpu: the shifted-patch tokenizer, the self-masked attention, token assembly without a LayerNorm and the fused
-ViT for small datasets on the H100.  Kernels are checked against torch expressions on the same bf16 data; the model
-against the reference's stored fp32 logits (tests/golden/vit_small.pt) and the module's own eager bf16 graph."""
+ViT for small datasets on the H100.  Kernels are checked against torch expressions on the same bf16 data; the model's
+two host loops against each other (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from oracle import attention_bounds as AB
 from oracle import bounds as Bd
 from vit_pytorch_b200 import _lib
@@ -15,7 +15,7 @@ from vit_pytorch_b200.vit import Patchify
 from vit_pytorch_b200.vit_for_small_dataset import SPT_SHIFTS, Transformer, ViT
 
 sys.path.insert(0, GOLDEN_DIR)
-from vit_small_spec import VIT_SMALL_CASES, vit_small_input, vit_small_model, weights_digest  # noqa: E402
+from vit_small_spec import FAMILY, VIT_SMALL_CASES  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -165,35 +165,13 @@ def _eager_bf16(m, x, monkeypatch):
             return m(x)
 
 
-@pytest.mark.parametrize("name", sorted(VIT_SMALL_CASES))
-def test_fused_against_reference_goldens(name, monkeypatch):
-    """Weights (per-layer temperatures perturbed) and input rebuilt from the seeds, against the reference's fp32 logits
-    and the module's own eager bf16 graph."""
-    case, spec = load_golden("vit_small")["cases"][name], VIT_SMALL_CASES[name]
-    ref = vit_small_model(ViT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = vit_small_input(spec).to(DEV)
-    m = vit_small_model(ViT, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0
-    eager = _eager_bf16(m, x, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 2e-2, (what, mx, frac)
-
-
 @pytest.mark.parametrize("name", ["c32_p4_cls", "long_577"])
 def test_c_and_python_layer_loops_agree(name, monkeypatch):
     """b200vit_encoder_blocks_ex (per-layer scales, self mask) against the per-kernel Python loop: the same launches,
     the same bits."""
     spec = VIT_SMALL_CASES[name]
-    m = vit_small_model(ViT, spec).to(DEV, torch.bfloat16)
-    x = vit_small_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         m(x)
         _lib.reset_launch_count()
@@ -211,8 +189,8 @@ def test_c_and_python_layer_loops_agree(name, monkeypatch):
 
 def test_in_place_temperature_change_reaches_the_fused_path(monkeypatch):
     spec = VIT_SMALL_CASES["c32_p4_mean"]
-    m = vit_small_model(ViT, spec).to(DEV, torch.bfloat16)
-    x = vit_small_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         before = m(x).clone()
     with torch.no_grad():
@@ -229,8 +207,8 @@ def test_in_place_temperature_change_reaches_the_fused_path(monkeypatch):
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = VIT_SMALL_CASES["c32_p4_cls"]
-    m = vit_small_model(ViT, spec).to(DEV, torch.bfloat16)
-    a = vit_small_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()
@@ -242,8 +220,8 @@ def test_cuda_graph_replay_is_bit_identical():
 def test_transformer_hook_keeps_the_fused_path():
     """A hook on .transformer (the Extractor pattern) sees the encoder output while the blocks still run fused."""
     spec = VIT_SMALL_CASES["c32_p4_cls"]
-    m = vit_small_model(ViT, spec).to(DEV, torch.bfloat16)
-    x = vit_small_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     seen = {}
     with torch.inference_mode():
         plain = m(x)

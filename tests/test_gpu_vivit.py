@@ -1,17 +1,17 @@
 """-m gpu: the strided short-sequence attention kernel, the grouped token assembly and the fused ViViT on the H100.
-The kernels are checked against torch expressions on the same bf16 data; the model against the reference's stored fp32
-logits (tests/golden/vivit.pt) and the module's own fp32 graph, with and without frame masks."""
+The kernels are checked against torch expressions on the same bf16 data; the model's fallback rules, direct
+transformer calls and LayerNorm modes (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.vivit import FactorizedTransformer, Transformer, ViViT
 
 sys.path.insert(0, GOLDEN_DIR)
-from vivit_spec import MASK_KINDS, VIVIT_CASES, vivit_input, vivit_mask, vivit_model, weights_digest  # noqa: E402
+from vivit_spec import FAMILY, VIVIT_CASES, vivit_mask  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -96,31 +96,6 @@ def test_embed_tokens_grouped(ncls, n, n_max):
 
 
 # ------------------------------------------------------------------------------------------------------ model
-@pytest.mark.parametrize("name", sorted(VIVIT_CASES))
-def test_fused_against_reference_goldens(name):
-    """Weights and input rebuilt from the seeds against the reference's fp32 logits and the module's own fp32 graph,
-    for every mask kind; the two attention modes' fully masked clip included."""
-    case, spec = load_golden("vivit")["cases"][name], VIVIT_CASES[name]
-    ref = vivit_model(ViViT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = vivit_input(spec)
-    m = vivit_model(ViViT, spec).to(DEV, torch.bfloat16)
-    for kind in MASK_KINDS:
-        mask = vivit_mask(spec, kind)
-        xd, md = x.to(DEV), None if mask is None else mask.to(DEV)
-        with torch.inference_mode():
-            assert m.fused_reason(xd, md) is None
-            _lib.reset_launch_count()
-            out = m(xd, mask=md)
-            torch.cuda.synchronize()
-            assert _lib.launch_count() > 0
-            own = ref(x.float(), mask=mask)                # the module's fp32 graph (CPU)
-        for want in (case["logits_fp32"][kind], own):
-            mx, frac = stats(out, want)
-            print(f"{name} {kind}: max {mx:.5f} within {frac:.4f}")
-            assert mx < 2e-2, (kind, mx, frac)
-
-
 def test_fallback_reasons():
     kw = dict(image_size=16, image_patch_size=8, num_classes=3, dim=64, spatial_depth=1, temporal_depth=1, heads=2,
               dim_head=32, mlp_dim=64)
@@ -204,8 +179,8 @@ def test_direct_factorized_transformer_call(masked):
 
 def test_exact_layernorm_mode_matches_fold(monkeypatch):
     spec = VIVIT_CASES["fsa_cls_softmax"]
-    m = vivit_model(ViViT, spec).to(DEV, torch.bfloat16)
-    x = vivit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     mask = vivit_mask(spec, "partial").to(DEV)
     with torch.inference_mode():
         fold = m(x, mask).float()

@@ -1,19 +1,19 @@
 """-m gpu: the cross-covariance attention kernel (b200vit_attention_xca), the local patch interaction kernel
 (b200vit_local_patch_interaction), class attention at dim_head 48 and the fused XCiT on the H100.  The kernels are checked
-against fp32 torch expressions on the same data; the model against the reference's stored fp32 logits
-(tests/golden/xcit.pt) and the module's own eager bf16 graph."""
+against fp32 torch expressions on the same data; the model's CUDA-graph replay and fallback rules
+(its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, load_golden
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.xcit import XCATransformer, XCiT
 
 sys.path.insert(0, GOLDEN_DIR)
-from xcit_spec import XCIT_CASES, seed_layer_dropout, weights_digest, xcit_input, xcit_model  # noqa: E402
+from xcit_spec import FAMILY, XCIT_CASES  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -161,43 +161,11 @@ def test_attention_cls_dim_head_48():
 
 
 # ------------------------------------------------------------------------------------------------ model
-def _eager_bf16(m, x, spec, monkeypatch):
-    """The module's own PyTorch graph in bf16 (every submodule), with the case's layer-dropout seed."""
-    with monkeypatch.context() as mp:
-        mp.setenv("B200VIT_DISABLE_FUSED", "1")
-        seed_layer_dropout(spec)
-        with torch.inference_mode():
-            return m(x)
-
-
-@pytest.mark.parametrize("ln_mode", ["fold", "exact"])
-@pytest.mark.parametrize("name", sorted(XCIT_CASES))
-def test_fused_against_reference_goldens(name, ln_mode, monkeypatch):
-    monkeypatch.setenv("B200VIT_LN_MODE", ln_mode)
-    case, spec = load_golden("xcit")["cases"][name], XCIT_CASES[name]
-    ref = xcit_model(XCiT, spec)
-    assert weights_digest(ref) == case["weights"]
-    x = xcit_input(spec).to(DEV)
-    m = xcit_model(XCiT, spec).to(DEV, torch.bfloat16)
-    with torch.inference_mode():
-        assert m.fused_reason(x) is None
-        _lib.reset_launch_count()
-        seed_layer_dropout(spec)
-        out = m(x)
-        torch.cuda.synchronize()
-        assert _lib.launch_count() > 0
-    eager = _eager_bf16(m, x, spec, monkeypatch)
-    for what, want in (("reference fp32", case["logits_fp32"]), ("eager bf16", eager)):
-        mx, frac = stats(out, want)
-        print(f"{name} {ln_mode} vs {what}: max {mx:.5f} within {frac:.4f}")
-        assert mx < 3e-2, (what, mx, frac)
-
-
 def test_cuda_graph_replay_is_bit_identical():
     from vit_pytorch_b200.graph import GraphedForward
     spec = XCIT_CASES["dh48_n196"]
-    m = xcit_model(XCiT, spec).to(DEV, torch.bfloat16)
-    a = xcit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    a = FAMILY.input(spec).to(DEV)
     b = torch.randn_like(a.float()).bfloat16()
     with torch.inference_mode():
         ya, yb = m(a).clone(), m(b).clone()
@@ -209,9 +177,9 @@ def test_cuda_graph_replay_is_bit_identical():
 def test_cuda_graph_refused_with_layer_dropout():
     from vit_pytorch_b200.graph import GraphedForward
     spec = XCIT_CASES["dh32"]
-    m = xcit_model(XCiT, {**spec, "layer_dropout": 0.1}).to(DEV, torch.bfloat16)
+    m = FAMILY.build({**spec, "layer_dropout": 0.1}).to(DEV, torch.bfloat16)
     with pytest.raises(RuntimeError, match="layer_dropout"):
-        GraphedForward(m, xcit_input(spec).to(DEV))
+        GraphedForward(m, FAMILY.input(spec).to(DEV))
 
 
 def test_direct_xcit_transformer_call():
@@ -241,14 +209,14 @@ def test_running_var_change_reaches_the_fused_output():
     """BatchNorm's running statistics are buffers, not parameters: an in-place update must still rebuild the folded
     conv1 weights.  After it the fused output equals, bit for bit, that of a fresh model loaded with the same state."""
     spec = XCIT_CASES["dh32"]
-    m = xcit_model(XCiT, spec).to(DEV, torch.bfloat16)
-    x = xcit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         before = m(x).clone()
     with torch.no_grad():
         for _, lpi, _ in m.xcit_transformer.layers:
             lpi.fn.net[3].running_var.mul_(0.01)          # BatchNorm now scales conv1 by 10
-    fresh = xcit_model(XCiT, spec).to(DEV, torch.bfloat16)
+    fresh = FAMILY.build(spec).to(DEV, torch.bfloat16)
     fresh.load_state_dict(m.state_dict())
     with torch.inference_mode():
         assert m.fused_reason(x) is None
@@ -262,15 +230,15 @@ def test_train_mode_forward_reaches_the_fused_output():
     statistics in place without bumping their version counters.  The next eval forward runs fused and equals, bit for
     bit, a fresh model loaded with the same state."""
     spec = XCIT_CASES["dh32"]
-    m = xcit_model(XCiT, spec).to(DEV, torch.bfloat16)
-    x = xcit_input(spec).to(DEV)
+    m = FAMILY.build(spec).to(DEV, torch.bfloat16)
+    x = FAMILY.input(spec).to(DEV)
     with torch.inference_mode():
         before = m(x).clone()
     m.train()
     with torch.no_grad():
         m(3 * torch.randn(8, *x.shape[1:], device=DEV).bfloat16())
     m.eval()
-    fresh = xcit_model(XCiT, spec).to(DEV, torch.bfloat16)
+    fresh = FAMILY.build(spec).to(DEV, torch.bfloat16)
     fresh.load_state_dict(m.state_dict())
     with torch.inference_mode():
         assert m.fused_reason(x) is None

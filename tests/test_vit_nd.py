@@ -1,56 +1,18 @@
-"""The N-dimensional ViTs (vit_pytorch_b200.vit_nd / vit_nd_rotary) without a GPU: drop-in surface against the
-reference's stored signatures, init digests and fp32 outputs (tests/golden/vit_nd.pt, made by make_vit_nd_golden.py), the
-eager graph's hooks, and the argument checks of the new C entry points."""
+"""The N-dimensional ViTs (vit_pytorch_b200.vit_nd / vit_nd_rotary) without a GPU: the shared rotary buffer, the eager
+graph's hooks, and the argument checks of the new C entry points.  The reference-parity tests are in
+test_family_parity.py."""
 import ctypes
 import sys
 
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, load_golden, signature, state_digest
+from conftest import GOLDEN_DIR
 from vit_pytorch_b200 import _lib, build
-from vit_pytorch_b200.vit_nd import ViTND
 from vit_pytorch_b200.vit_nd_rotary import ViTND as RotaryViTND
 
 sys.path.insert(0, GOLDEN_DIR)
-from vit_nd_spec import (INIT_KWARGS, INIT_SEED, VIT_ND_CASES, input_digest, vit_nd_input, vit_nd_model,  # noqa: E402
-                         weights_digest)
-
-CLASSES = {"vit_nd": ViTND, "vit_nd_rotary": RotaryViTND}
-
-
-@pytest.fixture(scope="module")
-def golden():
-    return load_golden("vit_nd")
-
-
-@pytest.mark.parametrize("kind", sorted(CLASSES))
-def test_signature_and_seeded_init_match_reference(golden, kind):
-    assert signature(CLASSES[kind]) == golden["signature"][kind]
-    init = golden["init"][kind]
-    torch.manual_seed(INIT_SEED)
-    sd = CLASSES[kind](**INIT_KWARGS).state_dict()
-    assert list(sd) == list(init)                          # names and registration order
-    assert state_digest(sd) == init                        # shapes, dtypes and the bytes of every tensor
-
-
-@pytest.mark.parametrize("name", sorted(VIT_ND_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    """Weights and input rebuilt from the seeds are the ones the reference ran; the drop-in's PyTorch graph
-    reproduces its fp32 logits (and the rotary model's return_embed output)."""
-    case, spec = golden["cases"][name], VIT_ND_CASES[name]
-    assert case["spec"] == spec
-    m = vit_nd_model(CLASSES[spec["kind"]], spec)
-    x = vit_nd_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    x = x.float()
-    with torch.inference_mode():
-        assert m.fused_reason(x) == "input is not on a CUDA device"
-        torch.testing.assert_close(m(x), case["logits_fp32"], rtol=0, atol=1e-5)
-        if case["embed0_fp32"] is not None:
-            e = m(x, return_embed=True)[:1]
-            assert e.shape == case["embed0_fp32"].shape     # (1, *grid, dim)
-            torch.testing.assert_close(e, case["embed0_fp32"], rtol=0, atol=1e-5)
+from vit_nd_spec import FAMILY, INIT_KWARGS, VIT_ND_CASES  # noqa: E402
 
 
 def test_rotary_buffer_is_shared_and_muon_parameters():
@@ -69,17 +31,17 @@ def test_rotary_buffer_is_shared_and_muon_parameters():
 def test_eager_graph_keeps_hooks_observable():
     """Recorder-style hooks on the attention softmax fire on the PyTorch graph, once per layer."""
     spec = VIT_ND_CASES["rot_r2"]
-    m = vit_nd_model(RotaryViTND, spec)
+    m = FAMILY.build(spec)
     seen = []
     for attn, _ in m.transformer.layers:
         attn.attend.register_forward_hook(lambda mod, i, o: seen.append(o.shape))
     with torch.inference_mode():
-        m(vit_nd_input(spec).float())
+        m(FAMILY.input(spec).float())
     assert len(seen) == len(m.transformer.layers) and seen[0][-1] == seen[0][-2]
 
 
 def test_positional_table_overflow_raises_like_the_reference():
-    m = vit_nd_model(ViTND, VIT_ND_CASES["nd_r2_cls"])
+    m = FAMILY.build(VIT_ND_CASES["nd_r2_cls"])
     big = torch.randn(1, 3, 32, 24)                       # more patches than the learned table holds
     with pytest.raises(RuntimeError):
         m(big)

@@ -1,6 +1,6 @@
-"""ViViT (vit_pytorch_b200.vivit) without a GPU: drop-in surface against the reference's stored signature, init digests
-and fp32 logits (tests/golden/vivit.pt, made by make_vivit_golden.py) with and without frame masks, the state_dict
-round trip with the reference package, the eager graph's hooks, and the argument checks of the new C entry points."""
+"""ViViT (vit_pytorch_b200.vivit) without a GPU: the attribute surface, the stored logits of a fully masked clip, the
+state_dict round trip with the reference package, the eager graph's hooks, and the argument checks of the new C entry
+points.  The reference-parity tests are in test_family_parity.py."""
 import ctypes
 import os
 import sys
@@ -8,33 +8,17 @@ import sys
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, ROOT, import_reference, load_golden, reference_available, signature, state_digest
+from conftest import GOLDEN_DIR, ROOT, import_reference, load_golden, reference_available
 from vit_pytorch_b200 import _lib, build
 from vit_pytorch_b200.vivit import FactorizedTransformer, Transformer, ViViT
 
 sys.path.insert(0, GOLDEN_DIR)
-from vivit_spec import (INIT_KWARGS, INIT_SEED, MASK_KINDS, VIVIT_CASES, input_digest, vivit_input,  # noqa: E402
-                        vivit_mask, vivit_model, weights_digest)
-
-VARIANTS = ("factorized_encoder", "factorized_self_attention")
+from vivit_spec import FAMILY, INIT_KWARGS, VARIANTS, VIVIT_CASES  # noqa: E402
 
 
 @pytest.fixture(scope="module")
 def golden():
     return load_golden("vivit")
-
-
-def test_signature_matches_reference(golden):
-    assert signature(ViViT) == golden["signature"]
-
-
-@pytest.mark.parametrize("variant", VARIANTS)
-def test_seeded_init_matches_reference(golden, variant):
-    init = golden["init"][variant]
-    torch.manual_seed(INIT_SEED)
-    sd = ViViT(variant=variant, **INIT_KWARGS).state_dict()
-    assert list(sd) == list(init)                          # names and registration order
-    assert state_digest(sd) == init                        # shapes, dtypes and the bytes of every tensor
 
 
 @pytest.mark.parametrize("pool", ["cls", "mean"])
@@ -48,24 +32,6 @@ def test_attribute_surface(pool):
     assert (fe.temporal_cls_token is None) == (pool == "mean")
     assert isinstance(fe.spatial_transformer, Transformer) and isinstance(fsa.factorized_transformer,
                                                                           FactorizedTransformer)
-
-
-@pytest.mark.parametrize("name", sorted(VIVIT_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    """Weights and input rebuilt from the seeds are the ones the reference ran; the drop-in's PyTorch graph
-    reproduces its fp32 logits without a mask, with a partial frame mask and with one clip fully masked (where the
-    use_flash_attn modes differ)."""
-    case, spec = golden["cases"][name], VIVIT_CASES[name]
-    assert case["spec"] == spec
-    m = vivit_model(ViViT, spec)
-    x = vivit_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    x = x.float()
-    with torch.inference_mode():
-        assert m.fused_reason(x) == "input is not on a CUDA device"
-        for kind in MASK_KINDS:
-            torch.testing.assert_close(m(x, mask=vivit_mask(spec, kind)), case["logits_fp32"][kind], rtol=0,
-                                       atol=1e-5)
 
 
 def test_fully_masked_clip_modes_differ(golden):
@@ -99,13 +65,13 @@ def test_state_dict_round_trip_with_reference(variant):
 def test_eager_graph_keeps_hooks_observable():
     """Recorder-style hooks on the attention softmax fire on the PyTorch graph: spatial and temporal, every layer."""
     spec = VIVIT_CASES["fsa_cls_softmax"]
-    m = vivit_model(ViViT, spec)
+    m = FAMILY.build(spec)
     seen = []
     for sa, ta, _ in m.factorized_transformer.layers:
         for a in (sa, ta):
             a.attend.register_forward_hook(lambda mod, i, o: seen.append(tuple(o.shape)))
     with torch.inference_mode():
-        m(vivit_input(spec).float())
+        m(FAMILY.input(spec).float())
     n, f = 6 + 1, 4
     assert seen[0] == (3 * f, 2, n, n) and seen[1] == (3 * n, 2, f, f) and len(seen) == 4
 
@@ -120,7 +86,7 @@ def test_direct_transformer_calls_take_masks():
 
 
 def test_positional_table_overflow_raises_like_the_reference():
-    m = vivit_model(ViViT, VIVIT_CASES["fe_cls_sdpa"])
+    m = FAMILY.build(VIVIT_CASES["fe_cls_sdpa"])
     with pytest.raises(RuntimeError):
         m(torch.randn(1, 3, 8, 32, 24))                   # more patches per frame than the table holds
 

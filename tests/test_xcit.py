@@ -1,7 +1,7 @@
-"""XCiT (vit_pytorch_b200.xcit) without a GPU: drop-in surface against the reference's stored signature, init digest and
-fp32 logits (tests/golden/xcit.pt, made by make_xcit_golden.py), the BatchNorm / LayerScale fold of the local patch
-interaction, the fallback rules, and the argument checks of the cross-covariance attention, local patch interaction and
-class attention entry points."""
+"""XCiT (vit_pytorch_b200.xcit) without a GPU: the attribute surface, the seeded layer-dropout case, the BatchNorm /
+LayerScale fold of the local patch interaction, the fallback rules, and the argument checks of the cross-covariance
+attention, local patch interaction and class attention entry points.  The reference-parity tests are in
+test_family_parity.py."""
 import ctypes
 import os
 import sys
@@ -10,31 +10,19 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, ROOT, load_golden, signature, state_digest
+from conftest import GOLDEN_DIR, ROOT, load_golden
 from vit_pytorch_b200 import _lib, build
 from vit_pytorch_b200.engine import LPIBlock, Norm, lpi_reason, lpi_weights, xca_reason
 from vit_pytorch_b200.xcit import (LayerScale, LocalPatchInteraction, XCATransformer, XCAttention, XCiT,
                                    batchnorm_reason)
 
 sys.path.insert(0, GOLDEN_DIR)
-from xcit_spec import (INIT_KWARGS, INIT_SEED, XCIT_CASES, input_digest, seed_layer_dropout,  # noqa: E402
-                       weights_digest, xcit_input, xcit_model)
+from xcit_spec import FAMILY, INIT_KWARGS, XCIT_CASES  # noqa: E402
 
 
 @pytest.fixture(scope="module")
 def golden():
     return load_golden("xcit")
-
-
-def test_signature_matches_reference(golden):
-    assert signature(XCiT) == golden["signature"]
-
-
-def test_seeded_init_matches_reference(golden):
-    torch.manual_seed(INIT_SEED)
-    sd = XCiT(**INIT_KWARGS).state_dict()
-    assert list(sd) == list(golden["init"])                # names and registration order, BatchNorm buffers included
-    assert state_digest(sd) == golden["init"]              # shapes, dtypes and the bytes of every tensor
 
 
 def test_layer_scale_init_follows_the_reference_condition():
@@ -58,28 +46,12 @@ def test_attribute_surface():
     assert isinstance(m.xcit_transformer, XCATransformer) and not hasattr(m.xcit_transformer, "norm")
 
 
-@pytest.mark.parametrize("name", sorted(XCIT_CASES))
-def test_eager_forward_matches_reference(golden, name):
-    """Weights (LayerNorms, LayerScale vectors, temperatures and BatchNorm statistics perturbed) and input rebuilt from
-    the seeds are the ones the reference ran; the drop-in's PyTorch graph reproduces its fp32 logits, the layer-dropout
-    case included."""
-    case, spec = golden["cases"][name], XCIT_CASES[name]
-    assert case["spec"] == spec
-    m = xcit_model(XCiT, spec)
-    x = xcit_input(spec)
-    assert weights_digest(m) == case["weights"] and input_digest(x) == case["input"]
-    seed_layer_dropout(spec)
-    with torch.inference_mode():
-        out = m(x.float())
-    assert torch.allclose(out, case["logits_fp32"], atol=1e-5, rtol=1e-5), (out - case["logits_fp32"]).abs().max()
-
-
 def test_layer_dropout_case_drops_layers(golden):
     spec = dict(XCIT_CASES["readme_layer_dropout"])
-    m = xcit_model(XCiT, spec)
+    m = FAMILY.build(spec)
     m.xcit_transformer.layer_dropout = m.cls_transformer.layer_dropout = 0.0
     with torch.inference_mode():
-        out = m(xcit_input(spec).float())
+        out = m(FAMILY.input(spec).float())
     assert (out - golden["cases"]["readme_layer_dropout"]["logits_fp32"]).abs().max() > 1e-3
 
 
