@@ -46,6 +46,7 @@ extern "C" {
 #define B200VIT_CONV_MAX_KERNEL 16   /* Conv2d kernel size k */
 #define B200VIT_POOL_MAX_KERNEL 16   /* MaxPool2d kernel size */
 #define B200VIT_SEQ_POOL_MAX_DIM 1024  /* embedding width D of b200vit_seq_pool */
+#define B200VIT_ATTN_KV_MAX_KEYS 16384  /* keys per image of b200vit_attention_kv */
 
 const char* b200vit_last_error(void);
 int b200vit_version(void);
@@ -207,6 +208,36 @@ int b200vit_attention_varlen_ex(const void* qkv, void* out, const int32_t* cu_se
  */
 int b200vit_attention_axial(const void* qkv, void* out, const uint8_t* key_mask, int B, int L, int G, int H, int dh,
                             float scale, int zero_masked_rows, void* stream);
+
+/*
+ * Softmax attention inside non-overlapping p x p windows of a token map (Twins-SVT's locally-grouped attention,
+ * twins_svt.py:85-120): B maps of gh x gw tokens, token (b, y, x) at row (b*gh + y)*gw + x of
+ *   qkv[B*gh*gw, 3*H*dh] bf16 packed as for b200vit_attention; out[B*gh*gw, H*dh] bf16.
+ * Window (b, wy, wx) is the p*p rows (b*gh + wy*p + i)*gw + wx*p + j, i, j < p; each head attends among them and the
+ * result goes back to the same rows.  One 64-row tile holds as many whole windows of one image as fit (1 for p >= 6,
+ * 64 for p = 1).  p*p <= 64, gh and gw multiples of p, dh = 32, 64, 80 or 128; qkv and out 16-byte aligned.
+ * Isolation: a window's output is computed from its own rows only and nothing outside the B*gh*gw rows is read or
+ * written.  A NaN or Inf stays within its image, and within its window when the window has a tile of its own
+ * (p*p > 32); windows that share a tile give each other's values the probability 0, so any finite change in one
+ * leaves the others bit-identical.
+ */
+int b200vit_attention_window(const void* qkv, void* out, int B, int gh, int gw, int p, int H, int dh, float scale,
+                             void* stream);
+
+/*
+ * Attention of every query of an image over keys and values that live in another buffer and have another length
+ * (Twins-SVT's global sub-sampled attention, twins_svt.py:122-157, where they come from a strided convolution):
+ *   q[B*Nq, H*dh] bf16 (row stride ldq), kv[B*Nk, 2*H*dh] bf16 packed k | v (row stride ldkv), both head-major;
+ *   out[B*Nq, H*dh] bf16 (contiguous) = softmax(scale * q k^T) v per image and head.
+ * 128-row query tiles, keys in blocks of 64 with an fp32 online softmax, both products on wgmma, keys past Nk masked.
+ * When the key blocks of an (image, head) fit in shared memory they are loaded once per CTA and the CTA's query tiles
+ * loop over them (up to 1024 / 704 / 576 / 320 keys for dh = 32 / 64 / 80 / 128); longer key sets stream through a
+ * ring of block slots once per query tile.  Nq >= 1, 1 <= Nk <= B200VIT_ATTN_KV_MAX_KEYS (Nk = 1: out is that value
+ * row), dh = 32, 64, 80 or 128, B and H <= 65535; ldq and ldkv multiples of 8; q, kv and out 16-byte aligned.  Each
+ * image's output is computed from its own rows only, and no row past B*Nq or B*Nk is read.
+ */
+int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq, int Nk,
+                         int H, int dh, float scale, void* stream);
 
 /*
  * NaViT patch extraction over a LIST of images of different resolutions + LayerNorm(patch_dim) without bias, one launch:
@@ -416,6 +447,31 @@ int b200vit_conv_im2col_nchw(const void* img, void* out_bf16, int64_t ldo, int B
                              int p, void* stream);
 int b200vit_conv_im2col_nhwc(const void* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W, int C, int k,
                              int s, int p, void* stream);
+
+/*
+ * Patch merging + LayerNorm between the stages of a hierarchical model (Twins-SVT's PatchEmbedding up to its 1 x 1
+ * convolution, twins_svt.py:59-75): x[M, C] fp32 is the token map of B images of gh x gw tokens (token (b, y, x) at
+ * row (b*gh + y)*gw + x, M = B*gh*gw); output row b*(gh/p)*(gw/p) + oy*(gw/p) + ox holds the p x p block's tokens,
+ *   out[row, (p1*p + p2)*C + c] = LN(x[(b, oy*p + p1, ox*p + p2), c]) * gamma[(p1*p + p2)*C + c] + beta[...],
+ * the LayerNorm over all p*p*C values of the row (fp32, biased variance, eps inside the square root), rounded to bf16:
+ * the A operand of the convolution's GEMM.  The reference orders the merged features (c p1 p2); the caller permutes
+ * its gamma, beta and weight columns to (p1 p2 c), the order of contiguous reads.  Columns [p*p*C, ldo) are zero
+ * filled (K padding).  gh and gw multiples of p, C a multiple of 4; ldo a multiple of 8 and >= p*p*C; x, gamma, beta
+ * and out_bf16 16-byte aligned.
+ */
+int b200vit_merge_patches_ln(const float* x, int64_t M, const float* gamma, const float* beta, void* out_bf16,
+                             int64_t ldo, int B, int gh, int gw, int C, int p, float eps, void* stream);
+
+/*
+ * Positional encoding generator (Twins-SVT's PEG, twins_svt.py:77-83) on the token map x[M, C] fp32 of B images of
+ * gh x gw tokens, out of place:
+ *   y[(b, i, j), c] = x[(b, i, j), c] + bias[c] + sum_{dy, dx < k} w[dy*k + dx][c] x[(b, i + dy - k/2, j + dx - k/2), c]
+ * the depthwise k x k convolution with zero padding k / 2, plus the identity.  w fp32 [k*k][C] (tap major, channel
+ * minor), bias fp32 [C]; y must not be x (every token reads its neighbours).  k = 1, 3, 5 or 7, C a multiple of 4;
+ * x, w, bias and y 16-byte aligned.  Each image's output is computed from its own rows only.
+ */
+int b200vit_peg(const float* x, int64_t M, const float* w, const float* bias, float* y, int B, int gh, int gw, int C,
+                int k, void* stream);
 
 /*
  * ReLU then MaxPool2d(pk, stride ps, padding pp) in one pass (CCT's tokenizer, cct.py:187-190): y[M, C] bf16

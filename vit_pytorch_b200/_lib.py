@@ -38,6 +38,7 @@ SYMBOLS = [
     "b200vit_attention_headmix", "b200vit_attention_headmix_ex", "b200vit_attention_cls_headmix",
     "b200vit_attention_xca", "b200vit_local_patch_interaction", "b200vit_unfold_patches", "b200vit_pit_pool",
     "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
+    "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
 ]
 
 
@@ -142,6 +143,14 @@ def lib() -> C.CDLL:
     L.b200vit_relu_maxpool.argtypes = [vp, i64, i32, i32, i32, i32, i32, i32, i32, vp, vp, i64, vp]
     L.b200vit_seq_pool.restype = i32
     L.b200vit_seq_pool.argtypes = [vp, i32, i32, i32, vp, vp, f32, vp, vp, vp, i64, vp]
+    L.b200vit_attention_window.restype = i32
+    L.b200vit_attention_window.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_attention_kv.restype = i32
+    L.b200vit_attention_kv.argtypes = [vp, i64, vp, i64, vp, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_merge_patches_ln.restype = i32
+    L.b200vit_merge_patches_ln.argtypes = [vp, i64, vp, vp, vp, i64, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_peg.restype = i32
+    L.b200vit_peg.argtypes = [vp, i64, vp, vp, vp, i32, i32, i32, i32, i32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -544,6 +553,34 @@ def attention_axial(qkv: torch.Tensor, out: torch.Tensor, key_mask: Optional[tor
     _check(rc, "b200vit_attention_axial")
 
 
+def attention_window(qkv: torch.Tensor, out: torch.Tensor, B: int, gh: int, gw: int, p: int, H: int, dh: int,
+                     scale: float) -> None:
+    """Attention inside the p x p windows of B token maps of gh x gw tokens: qkv[B*gh*gw, 3*H*dh] packed q | k | v,
+    token (b, y, x) at row (b*gh + y)*gw + x; out[B*gh*gw, H*dh]."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out")
+    assert qkv.is_contiguous() and out.is_contiguous()
+    assert qkv.shape == (B * gh * gw, 3 * H * dh) and out.shape == (B * gh * gw, H * dh)
+    with _Timed("attention_window", B=B, h=gh, w=gw, p=p, H=H, bytes=(qkv.numel() + out.numel()) * 2,
+                flops=4.0 * B * gh * gw * H * p * p * dh):
+        rc = lib().b200vit_attention_window(_ptr(qkv), _ptr(out), B, int(gh), int(gw), int(p), H, dh, float(scale),
+                                            _stream())
+    _check(rc, "b200vit_attention_window")
+
+
+def attention_kv(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, B: int, Nq: int, Nk: int, H: int, dh: int,
+                 scale: float) -> None:
+    """out[B*Nq, H*dh] = softmax(scale q k^T) v per image and head: q[B*Nq, H*dh] (any row stride), kv[B*Nk, 2*H*dh]
+    packed k | v (any row stride), Nq and Nk independent."""
+    _chk(q, torch.bfloat16, "q"); _chk(kv, torch.bfloat16, "kv"); _chk(out, torch.bfloat16, "out")
+    assert q.dim() == 2 and q.stride(1) == 1 and kv.dim() == 2 and kv.stride(1) == 1 and out.is_contiguous()
+    assert q.shape == (B * Nq, H * dh) and kv.shape == (B * Nk, 2 * H * dh) and out.shape == (B * Nq, H * dh)
+    with _Timed("attention_kv", B=B, Nq=Nq, Nk=Nk, H=H, bytes=(q.numel() + kv.numel() + out.numel()) * 2,
+                flops=4.0 * B * H * Nq * Nk * dh):
+        rc = lib().b200vit_attention_kv(_ptr(q), q.stride(0), _ptr(kv), kv.stride(0), _ptr(out), B, int(Nq), int(Nk),
+                                        H, dh, float(scale), _stream())
+    _check(rc, "b200vit_attention_kv")
+
+
 def varlen_index(lengths, device) -> tuple:
     """(cu_seqlens, tile_prefix, total_tiles) device int32 tensors for b200vit_attention_varlen."""
     cu, tp = [0], [0]
@@ -849,6 +886,38 @@ def conv_im2col_nhwc(x: torch.Tensor, out_bf16: torch.Tensor, B: int, H: int, W:
         rc = lib().b200vit_conv_im2col_nhwc(_ptr(x), M, _ptr(out_bf16), out_bf16.stride(0), B, H, W, Cc, int(k), int(s),
                                             int(p), _stream())
     _check(rc, "b200vit_conv_im2col_nhwc")
+
+
+def merge_patches_ln(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out_bf16: torch.Tensor, B: int, gh: int,
+                     gw: int, p: int, eps: float = 1e-5) -> None:
+    """x fp32 [B*gh*gw, C] token map -> out [B*(gh/p)*(gw/p), ldo] bf16: every p x p block's tokens concatenated in
+    (p1 p2 c) order, LayerNorm over all p*p*C values (gamma, beta in that order), zero K padding up to ldo."""
+    for nm, t in (("x", x), ("gamma", gamma), ("beta", beta)):
+        _chk(t, torch.float32, nm)
+    _chk(out_bf16, torch.bfloat16, "out")
+    M, Cc = x.shape
+    K = p * p * Cc
+    rows = B * (gh // p) * (gw // p)
+    assert x.is_contiguous() and gamma.is_contiguous() and beta.is_contiguous() and gamma.numel() == beta.numel() == K
+    assert out_bf16.dim() == 2 and out_bf16.stride(1) == 1 and out_bf16.shape[0] == rows and out_bf16.shape[1] >= K, \
+        f"out must be [{rows}, >= {K}], got {tuple(out_bf16.shape)}"
+    with _Timed("merge_patches_ln", B=B, h=gh, w=gw, C=Cc, p=p, bytes=M * Cc * 4 + rows * out_bf16.stride(0) * 2):
+        rc = lib().b200vit_merge_patches_ln(_ptr(x), M, _ptr(gamma), _ptr(beta), _ptr(out_bf16), out_bf16.stride(0), B,
+                                            int(gh), int(gw), Cc, int(p), float(eps), _stream())
+    _check(rc, "b200vit_merge_patches_ln")
+
+
+def peg(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, y: torch.Tensor, B: int, gh: int, gw: int, k: int) -> None:
+    """y = x + depthwise k x k convolution (zero padding k // 2, + bias) of the B token maps x fp32 [B*gh*gw, C];
+    w fp32 [k*k, C] tap major, bias fp32 [C]; y is another buffer."""
+    for nm, t in (("x", x), ("w", w), ("bias", bias), ("y", y)):
+        _chk(t, torch.float32, nm)
+    M, Cc = x.shape
+    assert x.is_contiguous() and y.is_contiguous() and y.shape == x.shape and w.is_contiguous() and bias.is_contiguous()
+    assert w.shape == (k * k, Cc) and bias.numel() == Cc
+    with _Timed("peg", B=B, h=gh, w=gw, C=Cc, k=k, bytes=M * Cc * 8):
+        rc = lib().b200vit_peg(_ptr(x), M, _ptr(w), _ptr(bias), _ptr(y), B, int(gh), int(gw), Cc, int(k), _stream())
+    _check(rc, "b200vit_peg")
 
 
 def relu_maxpool(y: torch.Tensor, B: int, H: int, W: int, pk: int, ps: int, pp: int, *,

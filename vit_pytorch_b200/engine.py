@@ -132,6 +132,8 @@ HEADMIX_WIDTHS = (32, 48, 64, 80, 128)     # b200vit_attention_headmix
 HEADMIX_MAX_HEADS, HEADMIX_MAX_INNER = 16, 1024
 XCA_WIDTHS = (32, 48, 64, 80, 128)         # b200vit_attention_xca
 LPI_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_local_patch_interaction
+WINDOW_MAX_TOKENS = 64                     # b200vit_attention_window: tokens of one window
+PEG_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_peg
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -273,12 +275,25 @@ class EncoderLayer:
     lpi: Optional[LPIBlock] = None
     # `ln2` replaces the stream: x = LN2(x); x += fc2(GELU(fc1(x))) (cct.py:137-142)
     post_norm: bool = False
+    # attention inside non-overlapping window x window blocks of the token grid (Twins-SVT's LocalAttention,
+    # twins_svt.py:85-120; b200vit_attention_window); run_blocks needs `grid`
+    window: Optional[int] = None
+    # keys and values from a kv_stride x kv_stride, stride-kv_stride convolution of the normalised token grid
+    # (Twins-SVT's GlobalAttention, twins_svt.py:122-157; b200vit_attention_kv): kv_w is that Conv2d's weight
+    # [2 * heads * dim_head, D, k, k], rows k | v, and qkv_w holds the query rows only; run_blocks needs `grid`
+    kv_stride: Optional[int] = None
+    kv_w: Optional[torch.Tensor] = None
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
-    """Which kernel runs layer L's attention: 'xca', 'headmix', 'axial' (a run_blocks call with `axial`, unless the
-    layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys) or 'plain'.
-    ValueError for cross-covariance or head-mixing attention with `axial` or over a `packed` batch."""
+    """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'kv' (sub-sampled keys), 'axial' (a
+    run_blocks call with `axial`, unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed
+    batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed or sub-sampled-key
+    attention with `axial` or over a `packed` batch."""
+    if L.window is not None or L.kv_stride is not None:
+        if axial or packed:
+            raise ValueError("windowed and sub-sampled-key attention run over B token grids only")
+        return "window" if L.window is not None else "kv"
     if L.xca_tau is not None or L.headmix is not None:
         if axial or packed:
             what = "cross-covariance" if L.xca_tau is not None else "head-mixing"
@@ -436,6 +451,9 @@ class TransformerEngine:
                  headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else head_width_reason(L.dim_head))
             if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
                 r = lpi_reason(L.lpi.kernel_size, 1)
+            if r is None and L.window is not None and L.window ** 2 > WINDOW_MAX_TOKENS:
+                r = (f"local_patch_size={L.window}: a window of {L.window ** 2} tokens (the window attention kernel "
+                     f"takes at most {WINDOW_MAX_TOKENS})")
             if r is not None:
                 return r
             if L.qkv_w.shape[1] % 8 or L.fc1_w.shape[0] % 8:
@@ -482,6 +500,9 @@ class TransformerEngine:
                     t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(X.ln.gamma), _f32(X.ln.beta)
             if L.xca_tau is not None:
                 t[f"{i}.tau"] = L.xca_tau.detach().float().exp().reshape(-1).contiguous()
+            if L.kv_stride is not None:
+                # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
+                t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.detach().permute(0, 2, 3, 1).reshape(L.kv_w.shape[0], -1))
             if L.lpi is not None:
                 P = L.lpi
                 t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"] = _f32(P.ln.gamma), _f32(P.ln.beta)
@@ -591,7 +612,10 @@ class TransformerEngine:
         G = N); layers without one run their attention there instead of over the B x N sequences (ViViT's masked
         temporal transformer, G = 1).  These calls take the per-kernel loop below.
         `grid` = (h, w): the token grid of every sequence (N = h*w, token r*w + c), which layers with a local patch
-        interaction need (XCiT).  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
+        interaction, windowed attention or sub-sampled keys need (XCiT, Twins-SVT).  A layer with sub-sampled keys cannot
+        fold its LayerNorm into the key / value projection (one convolution window spans tokens with different
+        statistics): in both LayerNorm modes it runs layernorm(x -> xb), the query GEMM on xb, conv_im2col_nhwc of xb
+        and the key / value GEMM (kernel size 1: the GEMM on xb itself), then attention_kv.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
         axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
         onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
         fc1 is the plain GEMM on that copy.  The call is checked first: a ValueError leaves x as it was.
@@ -618,6 +642,13 @@ class TransformerEngine:
             kernels.append(attention_kernel(L, axial is not None, varlen is not None, vl is not None))
             if L.lpi is not None and (grid is None or grid[0] * grid[1] != N or axial is not None or varlen is not None):
                 raise ValueError("a layer with a local patch interaction needs `grid` = (h, w) with h * w == N")
+            if kernels[-1] in ("window", "kv"):
+                if grid is None or grid[0] * grid[1] != N:
+                    raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
+                step = L.window if kernels[-1] == "window" else L.kv_stride
+                if (grid[0] % step or grid[1] % step) if kernels[-1] == "window" else min(grid) < step:
+                    raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {step} x {step} "
+                                     f"{'windows' if kernels[-1] == 'window' else 'key patches'}")
         xb, qkv, o, h = ws["xn"], ws["qkv"], ws["o"], ws["h"]
         sums = ws["stats_in"] if primed else None          # fold: the row sums of xb the next LN-folded GEMM reads
 
@@ -650,8 +681,26 @@ class TransformerEngine:
             copy, stats = stream_copy(slot) if slot is not None else (None, None)
             _lib.gemm(a, t[w + ".w"], out_f32=x, out_bf16=copy, bias=t[w + ".b"], resid=resid, stats_out=stats)
 
+        def subsampled(L: EncoderLayer, i: int) -> None:
+            """o = attention of LN1(x)'s queries over the keys / values of its strided convolution."""
+            I, k = L.heads * L.dim_head, L.kv_stride
+            kh, kw = grid[0] // k, grid[1] // k
+            _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
+            q = qkv[:, :I]
+            _lib.gemm(xb, t[f"{i}.qkv.w"], out_bf16=q)
+            if k == 1:
+                col = xb
+            else:
+                col = torch.empty(B * kh * kw, k * k * x.shape[1], device=x.device, dtype=torch.bfloat16)
+                _lib.conv_im2col_nhwc(xb, col, B, grid[0], grid[1], k, k, 0)
+            kv = torch.empty(B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
+            _lib.gemm(col, t[f"{i}.kv.w"], out_bf16=kv)
+            _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
+
         def attend(kernel: str, L: EncoderLayer, i: int) -> None:
-            if kernel == "xca":
+            if kernel == "window":
+                _lib.attention_window(qkv, o, B, grid[0], grid[1], L.window, L.heads, L.dim_head, L.scale)
+            elif kernel == "xca":
                 _lib.attention_xca(qkv, t[f"{i}.tau"], o, B, N, L.heads, L.dim_head)
             elif kernel == "headmix":
                 hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
@@ -669,10 +718,13 @@ class TransformerEngine:
             L = self.layers[i]
             head = {} if L.qk_norm is None else dict(head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
                                                      head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
-            normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv, **head)
-            if rope is not None:
-                _lib.rope_qk(qkv, rope[0], rope[1], L.heads, L.dim_head)
-            attend(kernel, L, i)
+            if kernel == "kv":
+                subsampled(L, i)
+            else:
+                normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv, **head)
+                if rope is not None:
+                    _lib.rope_qk(qkv, rope[0], rope[1], L.heads, L.dim_head)
+                attend(kernel, L, i)
             residual(o, f"{i}.out", x, "stats_b" if L.lpi is None and not L.post_norm else None)
             if L.temporal is not None:
                 normed(x, f"{i}.tln", L.temporal.ln, f"{i}.tqkv", qkv)
