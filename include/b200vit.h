@@ -171,6 +171,12 @@ int b200vit_rowstats_cast(const float* x, void* xb_bf16, float* stats, int M, in
  * online softmax in fp32; S = QK^T and O = PV on the tensor cores (bf16 operands, fp32 accumulation).
  * dh = 32, 64, 80 (canonical ViT-H/14) or 128; a head is split into 64- and 16-column slabs (a 96-wide head would
  * fall out of the same scheme as 64 + 2 x 16, but is not built).
+ * 128 < N <= 256 with dh = 32 or 64 (ViT-B/16 and ViT-L/16 at 224^2: 197 tokens) runs a persistent kernel instead: one
+ * CTA per SM loops over (sequence, head) items, each head's Q, K and V are staged in shared memory once while the
+ * next head loads underneath, four warpgroups take 64 query rows each, the last key block runs at its real width
+ * rounded up to 16 keys, and the output leaves through TMA stores.  It keeps the per-block arithmetic and its order,
+ * so both kernels give the same bits.  dh = 80 and 128 do not fit two heads in shared memory and, like calls with
+ * B200VIT_ATTN_MASK_SELF, keep the tiled kernel at every N.
  * Isolation (this and every attention entry point below): each sequence's output is computed from its own rows only,
  * so a NaN or Inf in one sequence (image, packed sequence, batch element of b200vit_attention_axial) leaves every other
  * sequence's output bit-identical, and no row past the buffer's addressed rows is read.
@@ -567,6 +573,9 @@ int b200vit_encoder_blocks_ex(const b200vit_layer* layers, int depth, float* x, 
  *   key 14: b200vit_gemm_bf16 epilogue: 0 = bf16 outputs and residual launches with ldo and N multiples of 8 are staged
  *           in shared memory and written by TMA stores (default; 256-wide residual tiles excepted), 1 = every launch
  *           stores straight from the accumulator registers.  Both give the same bits.
+ *   key 15: b200vit_attention: 0 = launches with 128 < N <= 256 and dh = 32 or 64 run the persistent kernel (default),
+ *           1 = every launch runs the tiled kernel.  Both give the same bits.  Keys 1 and 13 select instances of the
+ *           tiled kernel: while either is non-zero every launch runs it, as with key 15.
  * Keys 1, 11 and 13 select real attention instances for every head width (32, 64, 80, 128): all (key block, FMA
  * exponential) combinations are built without register spills, so no setting falls back to a width's default.
  * They do not apply to calls with B200VIT_ATTN_MASK_SELF: those always run 64-key blocks with every exponential on MUFU.

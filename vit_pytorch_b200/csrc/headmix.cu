@@ -76,17 +76,6 @@ struct HmSmem {
   }
 };
 
-// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]^T, both operands K-major in shared memory
-__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
-}
-
 // shared-memory load the compiler may not hoist out of the key loop: the mixing weights are re-read per use instead of
 // occupying H^2 registers
 __device__ __forceinline__ float lds_keep(const float* p) {

@@ -48,6 +48,11 @@ void tmap_cache_stats(int64_t* hits, int64_t* misses);
 // The head widths (dim_head) the attention, head-norm and pooling kernels are built for.
 inline bool head_width_ok(int dh) { return dh == 32 || dh == 64 || dh == 80 || dh == 128; }
 
+// The persistent fixed-length attention kernel (attention_short.cu): the lengths and head widths it is built for, and
+// its launch.  Same bits as the tiled kernel of attention.cu; b200vit_attention_ex chooses between them.
+bool attention_short_ok(int N, int dh);
+int attention_short(const void* qkv, void* out, int B, int N, int H, int dh, float scale_log2e, cudaStream_t stream);
+
 // test hooks 12 and 14 (gemm.cu)
 void gemm_set_block_n(int v);
 void gemm_set_direct_store(int v);
