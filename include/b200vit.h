@@ -36,10 +36,16 @@ extern "C" {
                                    itself (in-place residual stream) or does not overlap it */
 #define B200VIT_EPI_LNFOLD 8    /* A is the un-normalised bf16 row, W carries gamma: y = rstd_m*(acc - mu_m*s_n) + bias_n */
 #define B200VIT_EPI_STATS 16    /* write per-row partial (sum, sum^2) of the bf16-rounded result into stats_out */
+#define B200VIT_EPI_HARDSWISH 32  /* y * clamp(y + 3, 0, 6) / 6 after the bias, where GELU would be (nn.Hardswish,
+                                     levit.py:32); not with B200VIT_EPI_GELU */
 #define B200VIT_EPI_HEADLN 64   /* b200vit_gemm_headnorm_bf16: per-head LayerNorm (no bias) instead of the RMS norm */
 
 /* attention flags (b200vit_attention_ex, b200vit_attention_varlen_ex, b200vit_encoder_blocks_ex) */
 #define B200VIT_ATTN_MASK_SELF 1  /* key i of query i gets probability 0 (LSA, vit_for_small_dataset.py:53-57) */
+/* b200vit_attention_posbias only (the entry points above reject it): exact-erf GELU on every fp32 output before it is
+ * rounded to bf16 (LeViT's to_out, levit.py:60-61) */
+#define B200VIT_ATTN_GELU_OUT 4
+#define B200VIT_ATTN_POSBIAS_MAX_KEYS 4096  /* keys per image (F*F) of b200vit_attention_posbias */
 
 /* what the convolutional tokenizer's kernels are built for (b200vit_conv_im2col_*, b200vit_relu_maxpool,
  * b200vit_seq_pool) */
@@ -244,6 +250,24 @@ int b200vit_attention_window(const void* qkv, void* out, int B, int gh, int gw, 
  */
 int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq, int Nk,
                          int H, int dh, float scale, void* stream);
+
+/*
+ * Attention with a learned relative-position bias over an F x F token map (LeViT, levit.py:40-108):
+ *   qkv[B*F*F, ld] bf16, token (b, y, x) at row (b*F + y)*F + x; columns q (H*dk) | k (H*dk) | v (H*dv), head-major.
+ *   Queries are the tokens (s*i, s*j), i, j < Fq = ceil(F / s), s = 1 or 2 (the downsampling attention's stride-2
+ *   to_q, gathered from the same full-grid qkv).
+ *   out[B*Fq*Fq, H*dv] bf16 (contiguous), row (b*Fq + i)*Fq + j:
+ *     softmax_j(scale * q.k_j + table[h][|dy|*F + |dx|]) v,  (dy, dx) the offset between the query's and key j's
+ *     positions on the F x F grid.  table fp32 [H][F*F] (the caller passes pos_bias.weight^T / scale).
+ *   flags: B200VIT_ATTN_GELU_OUT applies exact-erf GELU to each output before rounding.
+ * One CTA per 64 queries of an (image, head); keys and values stream through two shared-memory slots in blocks of 64,
+ * fp32 online softmax, both products on wgmma.  dk = 16, 32 or 64; dv = 32, 64 or 128; F*F <=
+ * B200VIT_ATTN_POSBIAS_MAX_KEYS; ld a multiple of 8; qkv, out and table 16-byte aligned; B and H <= 65535.
+ * Isolation as b200vit_attention: each image's output is computed from its own rows only, no row past B*F*F is read,
+ * and no output row outside the B*Fq*Fq addressed is written.
+ */
+int b200vit_attention_posbias(const void* qkv, int64_t ld, void* out, const float* table, int B, int F, int s, int H,
+                              int dk, int dv, float scale, int flags, void* stream);
 
 /*
  * NaViT patch extraction over a LIST of images of different resolutions + LayerNorm(patch_dim) without bias, one launch:

@@ -21,8 +21,11 @@ EPI_GELU = 2
 EPI_RESIDUAL = 4
 EPI_LNFOLD = 8
 EPI_STATS = 16
+EPI_HARDSWISH = 32
 EPI_HEADLN = 64
 ATTN_MASK_SELF = 1
+ATTN_GELU_OUT = 4
+ATTN_POSBIAS_MAX_KEYS = 4096    # B200VIT_ATTN_POSBIAS_MAX_KEYS
 
 # every symbol include/b200vit.h declares (tests check that the library exports each of them)
 SYMBOLS = [
@@ -39,6 +42,7 @@ SYMBOLS = [
     "b200vit_attention_xca", "b200vit_local_patch_interaction", "b200vit_unfold_patches", "b200vit_pit_pool",
     "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
     "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
+    "b200vit_attention_posbias",
 ]
 
 
@@ -151,6 +155,8 @@ def lib() -> C.CDLL:
     L.b200vit_merge_patches_ln.argtypes = [vp, i64, vp, vp, vp, i64, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_peg.restype = i32
     L.b200vit_peg.argtypes = [vp, i64, vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    L.b200vit_attention_posbias.restype = i32
+    L.b200vit_attention_posbias.argtypes = [vp, i64, vp, vp, i32, i32, i32, i32, i32, i32, f32, i32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -306,6 +312,16 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, out_bf16: Optional[torch.Tensor] =
     """out = epilogue(a[M,K] @ w[N,K]^T).  a, w bf16 row-major (last stride 1).
 
     ln_sums: [M, parts, 2] (or [M, 2]) partial row sums of `a`; stats_out: [M, stats_parts(N), 2], fully overwritten."""
+    _gemm(a, w, out_bf16, out_f32, bias, resid, gelu, ln_sums, ln_eps, col_s, stats_out, n, k, 0)
+
+
+def gemm_hardswish(a: torch.Tensor, w: torch.Tensor, *, out_bf16: torch.Tensor, bias: Optional[torch.Tensor] = None
+                   ) -> None:
+    """out_bf16 = hardswish(a @ w^T + bias) (EPI_HARDSWISH: y * clamp(y + 3, 0, 6) / 6; LeViT's FeedForward)."""
+    _gemm(a, w, out_bf16, None, bias, None, False, None, 1e-5, None, None, None, None, EPI_HARDSWISH)
+
+
+def _gemm(a, w, out_bf16, out_f32, bias, resid, gelu, ln_sums, ln_eps, col_s, stats_out, n, k, extra_flags) -> None:
     _chk(a, torch.bfloat16, "a"); _chk(w, torch.bfloat16, "w")
     _chk(out_bf16, torch.bfloat16, "out_bf16"); _chk(out_f32, torch.float32, "out_f32")
     for nm, t in (("bias", bias), ("resid", resid), ("ln_sums", ln_sums), ("col_s", col_s), ("stats_out", stats_out)):
@@ -318,7 +334,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, out_bf16: Optional[torch.Tensor] =
     assert out is not None and out.stride(1) == 1
     if out_bf16 is not None and out_f32 is not None:
         assert out_bf16.stride(0) == out_f32.stride(0)
-    flags = 0
+    flags = extra_flags
     if bias is not None:
         flags |= EPI_BIAS
     if gelu:
@@ -579,6 +595,24 @@ def attention_kv(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, B: int, N
         rc = lib().b200vit_attention_kv(_ptr(q), q.stride(0), _ptr(kv), kv.stride(0), _ptr(out), B, int(Nq), int(Nk),
                                         H, dh, float(scale), _stream())
     _check(rc, "b200vit_attention_kv")
+
+
+def attention_posbias(qkv: torch.Tensor, out: torch.Tensor, table: torch.Tensor, B: int, F: int, s: int, H: int,
+                      dk: int, dv: int, scale: float, gelu_out: bool = False) -> None:
+    """LeViT attention over B F x F token maps: qkv[B*F*F, ld] packed q (H*dk) | k (H*dk) | v (H*dv), any row stride;
+    queries the tokens (s*i, s*j); out[B*Fq*Fq, H*dv] (Fq = ceil(F / s)) = [GELU] softmax(scale q k^T + bias) v, the
+    bias table[h][|dy|*F + |dx|] from table fp32 [H, F*F]."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out"); _chk(table, torch.float32, "table")
+    Fq = -(-F // s)
+    assert qkv.dim() == 2 and qkv.stride(1) == 1 and out.is_contiguous() and table.is_contiguous()
+    assert qkv.shape == (B * F * F, H * (2 * dk + dv)) and out.shape == (B * Fq * Fq, H * dv)
+    assert table.shape == (H, F * F)
+    with _Timed("attention_posbias", B=B, F=F, s=s, H=H, bytes=(qkv.numel() + out.numel()) * 2,
+                flops=2.0 * B * H * Fq * Fq * F * F * (dk + dv)):
+        rc = lib().b200vit_attention_posbias(_ptr(qkv), qkv.stride(0), _ptr(out), _ptr(table), B, int(F), int(s), H,
+                                             int(dk), int(dv), float(scale), ATTN_GELU_OUT if gelu_out else 0,
+                                             _stream())
+    _check(rc, "b200vit_attention_posbias")
 
 
 def varlen_index(lengths, device) -> tuple:

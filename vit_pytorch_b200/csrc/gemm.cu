@@ -369,6 +369,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           v1 = fmaf(v1, rs, c1);
         }
         if (flags & B200VIT_EPI_GELU) gelu_erf2(v0, v1);
+        if (flags & B200VIT_EPI_HARDSWISH) {  // y * clamp(y + 3, 0, 6) / 6 (nn.Hardswish, levit.py:32)
+          v0 = v0 * fminf(fmaxf(v0 + 3.0f, 0.0f), 6.0f) * (1.0f / 6.0f);
+          v1 = v1 * fminf(fmaxf(v1 + 3.0f, 0.0f), 6.0f) * (1.0f / 6.0f);
+        }
         const size_t o = (size_t)row[h] * p.ldo + col;
         float2* rp = reinterpret_cast<float2*>(slab + h * 8 * 128 + ((((j % 4) * 2) ^ res_xor) << 4));
         float2 rr = make_float2(0.f, 0.f);
@@ -557,6 +561,8 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   B200_CHECK_ARG(!(flags & B200VIT_EPI_LNFOLD) || (ln_sums && col_s && ln_parts >= 1 && ln_parts <= 64),
                  "gemm: EPI_LNFOLD needs ln_sums, col_s and 1 <= ln_parts <= 64");
   B200_CHECK_ARG(!(flags & B200VIT_EPI_STATS) || stats_out, "gemm: EPI_STATS without stats_out");
+  B200_CHECK_ARG((flags & (B200VIT_EPI_GELU | B200VIT_EPI_HARDSWISH)) != (B200VIT_EPI_GELU | B200VIT_EPI_HARDSWISH),
+                 "gemm: EPI_GELU and EPI_HARDSWISH are exclusive");
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   B200_CHECK_ARG(al16(bias) && al16(resid) && al16(col_s) && al16(out_bf16) && al16(out_f32) && al16(ln_sums),
                  "gemm: epilogue pointers must be 16-byte aligned");
