@@ -9,6 +9,8 @@ import torch
 import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR
+from oracle import attention_fp32_bounds as FB
+from oracle import bounds as Bd
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.cait import CaiT, Transformer
 
@@ -81,18 +83,6 @@ def test_one_head_negative_pre_turns_the_softmax_around():
 
 
 # ------------------------------------------------------------------------------------------------ attention_cls_headmix
-def cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, scale, pre, post):
-    B = qkv_self.shape[0]
-    I = H * dh
-    q, ks, vs = qkv_self.float().view(B, 3, H, dh).unbind(1)
-    c = ctx.float().view(B, rows, -1)[:, first:first + n, :2 * I]
-    k = torch.cat([ks[:, None], c[..., :I].view(B, n, H, dh)], 1)          # [B, n + 1, H, dh]
-    v = torch.cat([vs[:, None], c[..., I:].view(B, n, H, dh)], 1)
-    s = torch.einsum('b h d, b j h d -> b h j', q, k) * scale
-    p = torch.einsum('b h j, h g -> b g j', torch.einsum('b h j, h g -> b g j', s, pre).softmax(-1), post)
-    return torch.einsum('b h j, b j h d -> b h d', p, v).reshape(B, I)
-
-
 @pytest.mark.parametrize("first", [0, 1])
 @pytest.mark.parametrize("n", [0, 1, 15, 16, 196, 576, 4096])
 @pytest.mark.parametrize("H,dh", [(1, 64), (3, 48), (4, 32), (8, 48), (16, 64), (6, 80), (8, 128)])
@@ -105,6 +95,7 @@ def test_attention_cls_headmix_against_fp32(H, dh, n, first):
     ctx = torch.randn(B * rows, ld, device=DEV, generator=g).bfloat16()
     pre, post = torch.randn(H, H, device=DEV, generator=g), torch.randn(H, H, device=DEV, generator=g)
     buf = torch.full((B, I + 16), 3.0, device=DEV, dtype=torch.bfloat16)
+    buf[:, :I] = float("nan")
     out = buf[:, :I]
     _lib.attention_cls_headmix(qkv_self, ctx, out, rows, first, n, H, dh, dh ** -0.5, pre, post)
     first_out = out.clone()
@@ -112,7 +103,8 @@ def test_attention_cls_headmix_against_fp32(H, dh, n, first):
     torch.cuda.synchronize()
     assert torch.equal(out, first_out)                # repeat calls are bit-identical
     assert (buf[:, I:] == 3.0).all()                  # columns outside out untouched
-    close_to(out, cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, dh ** -0.5, pre, post))
+    ref, bound = FB.cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, dh ** -0.5, pre, post)
+    Bd.check(out, ref, bound, f"attention_cls_headmix H{H} dh{dh} n{n} first{first}")
 
 
 # ------------------------------------------------------------------------------------------------ model

@@ -1,5 +1,5 @@
-"""-m gpu: the class-token cross-attention kernel and the fused CrossViT on the H100.  The kernel is checked against an
-fp32 torch expression on the same bf16 data; the model at batch one and its fallback rules
+"""-m gpu: the class-token cross-attention kernel and the fused CrossViT on the H100.  The kernel is checked against the
+fp64 reference and per-element bound of oracle/attention_fp32_bounds.py; the model at batch one and its fallback rules
 (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
@@ -7,6 +7,8 @@ import pytest
 import torch
 
 from conftest import GOLDEN_DIR
+from oracle import attention_fp32_bounds as FB
+from oracle import bounds as Bd
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.cross_vit import CrossViT, Transformer
 from vit_pytorch_b200.extractor import Extractor
@@ -37,20 +39,6 @@ def tokens_close(got, want):
 
 
 # ------------------------------------------------------------------------------------------------------ attention_cls
-def cls_reference(qkv_self, ctx, rows, first, n, H, dh, scale):
-    """fp32 softmax(scale * q k^T) v per image over [self; context rows first .. first + n of the image]."""
-    B, I = qkv_self.shape[0], H * dh
-    q, ks, vs = (qkv_self[:, i * I:(i + 1) * I].float().view(B, H, 1, dh) for i in range(3))
-    if n:
-        c = ctx[:B * rows].float().view(B, rows, -1)[:, first:first + n, :2 * I]
-        kc, vc = (c[..., i * I:(i + 1) * I].reshape(B, n, H, dh).transpose(1, 2) for i in range(2))
-        k, v = torch.cat((ks, kc), dim=2), torch.cat((vs, vc), dim=2)
-    else:
-        k, v = ks, vs
-    p = (q @ k.transpose(-1, -2) * scale).softmax(-1)
-    return (p @ v).reshape(B, I)
-
-
 @pytest.mark.parametrize("dh", [32, 64, 80, 128])
 @pytest.mark.parametrize("n", [0, 1, 16, 255, 1024, 4096])
 @pytest.mark.parametrize("H", [1, 3, 8])
@@ -65,10 +53,8 @@ def test_attention_cls_against_fp32(dh, n, H, B):
     out = torch.full((B, I + 8), 5.0, device=DEV).bfloat16()
     scale = 0.9 * dh ** -0.5
     _lib.attention_cls(qkv, ctx[:, :2 * I] if n else None, out[:, :I], rows, 1, n, H, dh, scale)
-    want = cls_reference(qkv, ctx, rows, 1, n, H, dh, scale)
-    got = out[:, :I].float()
-    assert torch.isfinite(got).all()
-    assert ((got - want).abs() <= 2e-2 + 1e-2 * want.abs()).all(), (got - want).abs().max().item()
+    ref, bound = FB.cls_reference(qkv, ctx, rows, 1, n, H, dh, scale)
+    Bd.check(out[:, :I], ref, bound, f"attention_cls B{B} H{H} n{n} dh{dh}")
     assert (out[:, I:] == 5.0).all()                     # row stride ldo: the padding columns are untouched
     if n == 0:
         assert torch.equal(out[:, :I], qkv[:, 2 * I:])

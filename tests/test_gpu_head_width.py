@@ -6,6 +6,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import attention_bounds as AB
+from oracle import attention_fp32_bounds as FB
 from oracle import bounds as Bd
 from oracle import navit_oracle as NO
 from vit_pytorch_b200 import NaViT, SimpleViT, ViT, _lib
@@ -180,17 +181,11 @@ def test_attn_pool_new_widths(dh, H):
     kv = torch.randn(T, 2 * I, device=DEV).bfloat16()
     qn = torch.randn(I, device=DEV) * dh ** -0.5
     cu, _, _ = _lib.varlen_index(lengths, DEV)
-    out = torch.zeros(len(lengths), I, device=DEV, dtype=torch.bfloat16)
+    out = torch.full((len(lengths), I), float("nan"), device=DEV, dtype=torch.bfloat16)
     _lib.attn_pool(kv, qn, cu, out, H, dh)
     torch.cuda.synchronize()
-    o = 0
-    for i, n in enumerate(lengths):
-        k = kv[o:o + n, :I].float().view(n, H, dh)
-        v = kv[o:o + n, I:].float().view(n, H, dh)
-        sc = torch.einsum("hd,nhd->hn", qn.view(H, dh), k)
-        want = torch.einsum("hn,nhd->hd", sc.softmax(-1), v).reshape(-1)
-        assert torch.allclose(out[i].float(), want, rtol=2e-2, atol=2e-2), (i, n)
-        o += n
+    ref, bound = FB.navit_pool_reference(kv, qn, lengths, H, dh)
+    Bd.check(out, ref, bound, f"attn_pool H{H} dh{dh}")
 
 
 # ---------------------------------------------------------------------------------------------------- whole models

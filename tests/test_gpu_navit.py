@@ -6,6 +6,7 @@ import torch
 
 from conftest import load_golden
 from oracle import attention_bounds as AB
+from oracle import attention_fp32_bounds as FB
 from oracle import bounds as Bd
 from oracle import navit_oracle as NO
 from oracle import vit_oracle as O
@@ -174,16 +175,10 @@ def test_qk_rmsnorm_and_attn_pool_kernels(H):
     cu, _, _ = _lib.varlen_index(lengths, DEV)
     kv = qkv[:, I:].contiguous()
     qn = torch.randn(I, device=DEV)
-    out = torch.zeros(3, I, device=DEV, dtype=torch.bfloat16)
+    out = torch.full((3, I), float("nan"), device=DEV, dtype=torch.bfloat16)
     _lib.attn_pool(kv, qn, cu, out, H, dh)
-    o = 0
-    for i, n in enumerate(lengths):
-        k = kv[o:o + n, :I].float().view(n, H, dh)
-        v = kv[o:o + n, I:].float().view(n, H, dh)
-        sc = torch.einsum("hd,nhd->hn", qn.view(H, dh), k)
-        want = torch.einsum("hn,nhd->hd", sc.softmax(-1), v).reshape(-1)
-        assert torch.allclose(out[i].float(), want, rtol=2e-2, atol=2e-2)
-        o += n
+    ref, bound = FB.navit_pool_reference(kv, qn, lengths, H, dh)
+    Bd.check(out, ref, bound, f"attn_pool H{H}")
 
 
 def test_rmsnorm_heads_on_the_k_half_of_a_kv_buffer():

@@ -1,6 +1,7 @@
 """-m gpu: the cross-covariance attention kernel (b200vit_attention_xca), the local patch interaction kernel
-(b200vit_local_patch_interaction), class attention at dim_head 48 and the fused XCiT on the H100.  The kernels are checked
-against fp32 torch expressions on the same data; the model's CUDA-graph replay and fallback rules
+(b200vit_local_patch_interaction), class attention at dim_head 48 and the fused XCiT on the H100.  The attention kernels
+are checked against the fp64 references and per-element bounds of oracle/attention_fp32_bounds.py, the patch
+interaction against an fp32 torch expression on the same data; the model's CUDA-graph replay and fallback rules
 (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
@@ -9,6 +10,8 @@ import torch
 import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR
+from oracle import attention_fp32_bounds as FB
+from oracle import bounds as Bd
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.xcit import XCATransformer, XCiT
 
@@ -25,14 +28,6 @@ def stats(got, ref, rtol=1e-2, atol=1e-3):
 
 
 # ------------------------------------------------------------------------------------------------ attention_xca
-def xca_reference(qkv, tau, B, N, H, dh):
-    """fp32 softmax_j(tau q^_i . k^_j) over the channels, q^ / k^ the L2-normalised columns (F.normalize), times v."""
-    q, k, v = qkv.float().view(B, N, 3, H, dh).permute(2, 0, 3, 4, 1)                 # b h d n
-    q, k = F.normalize(q, dim=-1), F.normalize(k, dim=-1)
-    a = (torch.einsum('b h i n, b h j n -> b h i j', q, k) * tau.view(1, H, 1, 1)).softmax(-1)
-    return torch.einsum('b h i j, b h j n -> b h i n', a, v).permute(0, 3, 1, 2).reshape(B * N, H * dh)
-
-
 @pytest.mark.parametrize("N", [1, 63, 64, 65, 196, 197, 784, 3136])
 @pytest.mark.parametrize("dh", [32, 48, 64, 80, 128])
 @pytest.mark.parametrize("H", [1, 3, 8, 16])
@@ -41,12 +36,10 @@ def test_attention_xca_against_fp32(H, dh, N):
     B = 2
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV).bfloat16()
     tau = torch.exp(torch.randn(H, device=DEV))
-    out = torch.empty(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
+    out = torch.full((B * N, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
     _lib.attention_xca(qkv, tau, out, B, N, H, dh)
-    want = xca_reference(qkv, tau, B, N, H, dh)
-    mx, frac = stats(out, want, rtol=1e-2, atol=1e-2)
-    assert torch.isfinite(out.float()).all()
-    assert mx < 3e-2 and frac > 0.999, (mx, frac)
+    ref, bound = FB.xca_reference(qkv, tau, B, N, H, dh)
+    Bd.check(out, ref, bound, f"xca H{H} dh{dh} N{N}")
 
 
 def test_attention_xca_zero_columns_and_peaky_tau():
@@ -58,15 +51,10 @@ def test_attention_xca_zero_columns_and_peaky_tau():
     qkv[:, 5] = 0                                          # q column 5 of head 0
     qkv[:, H * dh + 2 * dh + 7] = 0                        # k column 7 of head 2
     tau = torch.tensor([1.0, 30.0, 2.0, 0.5], device=DEV)
-    out = torch.empty(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
+    out = torch.full((B * N, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
     _lib.attention_xca(qkv, tau, out, B, N, H, dh)
-    want = xca_reference(qkv, tau, B, N, H, dh)
-    assert torch.isfinite(out.float()).all()
-    mx, frac = stats(out, want, rtol=1e-2, atol=1e-2)
-    assert mx < 3e-2 and frac > 0.999, (mx, frac)
-    # row 5 of head 0 is uniform: its output is the mean of head 0's v columns
-    v0 = qkv.float().view(B, N, 3, H, dh)[:, :, 2, 0]
-    assert torch.allclose(out.float().view(B, N, H, dh)[:, :, 0, 5], v0.mean(-1), atol=2e-2)
+    ref, bound = FB.xca_reference(qkv, tau, B, N, H, dh)
+    Bd.check(out, ref, bound, "xca zero columns")
 
 
 def test_attention_xca_repeat_calls_are_bit_identical_and_stay_in_place():
@@ -150,14 +138,8 @@ def test_attention_cls_dim_head_48():
     out = torch.full((B, I), 5.0, device=DEV).bfloat16()
     scale = dh ** -0.5
     _lib.attention_cls(qkv, ctx, out, rows, 1, n, H, dh, scale)
-    q, ks, vs = qkv.float().view(B, 3, H, dh).unbind(1)
-    c = ctx.float().view(B, rows, 2, H, dh)[:, 1:1 + n]
-    k = torch.cat([ks[:, None], c[:, :, 0]], 1)            # b j h d
-    v = torch.cat([vs[:, None], c[:, :, 1]], 1)
-    p = (torch.einsum('b h d, b j h d -> b h j', q, k) * scale).softmax(-1)
-    want = torch.einsum('b h j, b j h d -> b h d', p, v).reshape(B, I)
-    mx, frac = stats(out, want, rtol=1e-2, atol=1e-2)
-    assert mx < 3e-2 and frac > 0.999, (mx, frac)
+    ref, bound = FB.cls_reference(qkv, ctx, rows, 1, n, H, dh, scale)
+    Bd.check(out, ref, bound, "attention_cls dh48")
 
 
 # ------------------------------------------------------------------------------------------------ model
