@@ -1,6 +1,7 @@
 """Where the time of the four ViT-B/16 layer GEMMs goes: main loop against the fixed cost of each output tile.
 
-    python scripts/bench_gemm_epilogue.py [--launches 50] [--warmup 5] [--m 100864]
+    python scripts/bench_gemm_epilogue.py [--launches 50] [--warmup 5] [--m 100864] [--block-n 0 [1 2]]
+                                          [--rounds 1] [--residual-only]
 
 Times QKV, out-proj, FC1 and FC2 through _lib.gemm at M = 512 * 197 rows, with the flags and outputs that
 b200vit_encoder_blocks_ex passes (LN-fold row sums over stats_parts(768) parts for QKV and FC1, an in-place fp32
@@ -8,8 +9,10 @@ residual with a bf16 copy and row statistics for out-proj and FC2).  Each GEMM a
 fit of time against K splits a launch into the main loop (slope * K) and a fixed cost (intercept: the epilogue and
 the pipeline fill of every tile).  Per-tile figures are per 128 x 256 block of output spread over the SMs, so that
 builds with different tile widths compare directly.  CUDA events around --launches launches after --warmup.
-B200VIT_LIB selects the library.  Prints one JSON object with the card's name, power limit and maximum SM clock.
-Needs a GPU; writes nothing.
+--block-n sets the tile width (test hook 12: 0 = the library's choice, 1 = 128, 2 = 256); with several widths, each
+of --rounds rounds times every width in turn, and the figures are medians over the rounds.  --residual-only times
+out-proj and FC2 alone.  B200VIT_LIB selects the library.  Prints one JSON object with the card's name, power limit
+and maximum SM clock.  Needs a GPU; writes nothing.
 """
 from __future__ import annotations
 
@@ -62,6 +65,9 @@ def main() -> None:
     ap.add_argument("--launches", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--m", type=int, default=512 * 197)
+    ap.add_argument("--block-n", type=int, nargs="+", default=[0], choices=[0, 1, 2])
+    ap.add_argument("--rounds", type=int, default=1)
+    ap.add_argument("--residual-only", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_gemm_epilogue: needs a CUDA device")
@@ -94,21 +100,40 @@ def main() -> None:
         "fc2": (D, HIDDEN, lambda k: _lib.gemm(a_d, w[D], out_bf16=xb, out_f32=x, bias=bias[D], resid=x,
                                                  stats_out=stats, k=k)),
     }
+    if args.residual_only:
+        gemms = {name: gemms[name] for name in ("out_proj", "fc2")}
     info = card()
     blocks_per_sm = lambda n: M * n / (128 * 256) / info["num_sms"]  # noqa: E731
+    L = _lib.lib()
+    rounds = {bn: {name: [] for name in gemms} for bn in args.block_n}  # [ms at k, 2k, 4k] per round
+    try:
+        for _ in range(args.rounds):
+            for bn in args.block_n:
+                L.b200vit_debug_set(12, bn)
+                for name, (n, k, fn) in gemms.items():
+                    ks = [k, 2 * k, 4 * k]
+                    rounds[bn][name].append([timed(lambda kk=kk: fn(kk), args.launches, args.warmup) for kk in ks])
+                    assert math.isfinite(float(x.sum())), "residual stream overflowed"
+    finally:
+        L.b200vit_debug_set(12, 0)
     res = {}
-    for name, (n, k, fn) in gemms.items():
-        ks = [k, 2 * k, 4 * k]
-        ms = [timed(lambda kk=kk: fn(kk), args.launches, args.warmup) for kk in ks]
-        slope, icpt = np.polyfit(np.array(ks, dtype=float), np.array(ms), 1)
-        per = blocks_per_sm(n)
-        res[name] = {
-            "M": M, "N": n, "K": k, "ms_per_launch": ms[0], "tflops": 2.0 * M * n * k / ms[0] / 1e9,
-            "ms_at_2k_4k": ms[1:], "main_loop_ms": slope * k, "fixed_ms": icpt,
-            "main_loop_us_per_block": 1e3 * slope * k / per, "fixed_us_per_block": 1e3 * icpt / per,
-        }
-        assert math.isfinite(float(x.sum())), "residual stream overflowed"
-    print(json.dumps({"lib": str(_lib.LIB_PATH), "card": info, "launches": args.launches, "gemms": res}), flush=True)
+    for bn in args.block_n:
+        res[bn] = {}
+        for name, (n, k, _) in gemms.items():
+            ms = np.median(np.array(rounds[bn][name]), axis=0)
+            ks = np.array([k, 2 * k, 4 * k], dtype=float)
+            fits = [np.polyfit(ks, np.array(r), 1) for r in rounds[bn][name]]
+            slope, icpt = np.median([f[0] for f in fits]), np.median([f[1] for f in fits])
+            per = blocks_per_sm(n)
+            res[bn][name] = {
+                "M": M, "N": n, "K": k, "ms_per_launch": ms[0], "tflops": 2.0 * M * n * k / ms[0] / 1e9,
+                "ms_at_2k_4k": list(ms[1:]), "main_loop_ms": slope * k, "fixed_ms": icpt,
+                "main_loop_us_per_block": 1e3 * slope * k / per, "fixed_us_per_block": 1e3 * icpt / per,
+                "ms_per_launch_rounds": [r[0] for r in rounds[bn][name]],
+                "main_loop_ms_rounds": [f[0] * k for f in fits], "fixed_ms_rounds": [f[1] for f in fits],
+            }
+    print(json.dumps({"lib": str(_lib.LIB_PATH), "card": info, "launches": args.launches, "rounds": args.rounds,
+                      "gemms_by_block_n": res}), flush=True)
 
 
 if __name__ == "__main__":

@@ -2,7 +2,9 @@
 //
 //   warpgroup 0     : loaders
 //                     warp 0 (one thread): A / W tiles, cp.async.bulk.tensor -> 128B-swizzled smem ring
-//                     warp 1 (one thread, residual GEMMs only): the fp32 residual tile, TMA -> two 64-column slabs
+//                     warp 1 (one thread, residual GEMMs only): the fp32 residual tile, TMA -> two 64-column slab
+//                     buffers (256-wide tiles with TMA stores: none; warp 0 loads the four slabs into the four ring
+//                     stages after the tile's last k block)
 //                     warp 2: the tile's bias / col_s slices and LN-fold row sums -> smem (double buffered per tile)
 //   warpgroups 1, 2 : consumers     (wgmma m64 x BLOCK_N x k16, fp32 accumulators in registers, 64 rows each), then
 //                     the epilogue from the accumulator registers: bias / LN-fold / GELU / residual
@@ -17,12 +19,14 @@
 //   bf16 output (QKV, FC1): the epilogue writes 128B-swizzled staging boxes of 64 x 64 for the whole tile, one thread
 //     per warpgroup hands them to TMA stores, and the consumers go straight on to the next tile's MMAs.  Thread 0 waits
 //     for the stores to have read the staging tile during the next tile's first k block, before it is written again.
-//   residual (out-proj, FC2; 128-wide tiles): the fp32 sum goes back into the residual slab at the address its
-//     residual was read from and is TMA-stored from there; the bf16 copy is held in registers until the previous
-//     slab's stores have read the one 16 KB staging chunk.  A slab returns to the residual loader once its stores have
-//     read it: at the next slab, or during the next tile's first k block.
+//   residual (out-proj, FC2): the fp32 sum goes back into the residual slab at the address its residual was read
+//     from and is TMA-stored from there; once the previous slab's stores have read the one 16 KB staging chunk, the
+//     bf16 copy is rounded from those sums into it.  A slab returns to its loader once its stores have read it: at the
+//     next slab, or during the next tile's first k block.  Out-proj and FC2 run 256-wide tiles when the grid has at
+//     least one per SM; their vector buffer holds the bias slice alone, so residual launches with an LN fold stay
+//     128 wide.
 // The direct-store epilogue remains for non-residual fp32 outputs, patch tiles of fewer than 128 rows, ldo or N not a
-// multiple of 8, 256-wide residual tiles (test hook 12) and every launch under test hook 14.
+// multiple of 8, 256-wide residual tiles with an LN fold (test hook 12) and every launch under test hook 14.
 // Replaces the nn.Linear call sites listed in include/b200vit.h.
 #include "common.cuh"
 #include "host_util.h"
@@ -72,8 +76,15 @@ struct GemmParams {
 // Without RES that is the whole tile (consumer warpgroup c owns boxes [c * BLOCK_N / 64, (c + 1) * BLOCK_N / 64)); with
 // RES one 128 x 64 chunk, the bf16 copy of the slab being stored (warpgroup c owns its c-th box), while the fp32 sums
 // go back into the residual slab they were read from and are stored from there.
+// BIAS_ONLY (256-wide residual tiles with TMA stores): the vector buffer holds the bias slice alone, once; such
+// launches never carry an LN fold.
 template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false>
 struct GemmSmem {
+  static constexpr bool BIAS_ONLY = RES && TMA_OUT && BLOCK_N == 256;
+  // ... and its four slabs load into the ring, a 32 KB slab per 48 KB stage, under the tile's last k blocks: with no
+  // slab buffers the ring has 4 stages instead of 3
+  static constexpr bool RING_SLABS = BIAS_ONLY;
+  static constexpr int BUF_SLABS = RING_SLABS ? 0 : BLOCK_N / 64;  // slabs of a tile in the two slab buffers
   static constexpr int A_SLAB = PATCH ? BLOCK_M * 32 : BLOCK_M * BLOCK_K * 2;
   static constexpr int A_BYTES = PATCH ? 4 * A_SLAB : A_SLAB;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
@@ -82,12 +93,14 @@ struct GemmSmem {
   static constexpr int RES_SLAB = 2 * RES_BOX;
   static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int OUT_BOX = 64 * 64 * 2;
-  static constexpr int OUT_OFFSET = RES_OFFSET + (RES ? 2 * RES_SLAB : 0);
+  static constexpr int OUT_OFFSET = RES_OFFSET + (RES && !RING_SLABS ? 2 * RES_SLAB : 0);
   static constexpr int OUT_BYTES = !TMA_OUT ? 0 : RES ? 2 * OUT_BOX : BLOCK_M * BLOCK_N * 2;
-  // per tile, double buffered: bias[BLOCK_N], col_s[BLOCK_N], LN-fold row sums [BLOCK_M][2]
+  // per tile, double buffered: bias[BLOCK_N], col_s[BLOCK_N], LN-fold row sums [BLOCK_M][2] (BIAS_ONLY: bias[BLOCK_N],
+  // one buffer)
   static constexpr int VEC_OFFSET = OUT_OFFSET + OUT_BYTES;
-  static constexpr int VEC_BYTES = (2 * BLOCK_N + 2 * BLOCK_M) * 4;
-  static constexpr int BAR_OFFSET = VEC_OFFSET + 2 * VEC_BYTES;
+  static constexpr int VEC_BYTES = (BIAS_ONLY ? BLOCK_N : 2 * BLOCK_N + 2 * BLOCK_M) * 4;
+  static constexpr int VEC_BUFS = BIAS_ONLY ? 1 : 2;
+  static constexpr int BAR_OFFSET = VEC_OFFSET + VEC_BUFS * VEC_BYTES;
   // full[STAGES], empty[STAGES], res_full[2], res_empty[2], vec_full[2], vec_empty[2]
   static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 8) * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024B alignment
@@ -174,6 +187,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             phase ^= 1;
           }
         }
+        if (L::RING_SLABS) {
+          const int n0 = n_blk * BLOCK_N;
+          const int nslab = min(BLOCK_N / 64, (p.N - n0 + 63) / 64);
+          for (int q = L::BUF_SLABS; q < nslab; ++q) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            const int c0 = n0 + 64 * q;
+            const int nbox = c0 + 32 < p.N ? 2 : 1;
+            mbar_arrive_expect_tx(&full_bar[stage], nbox * L::RES_BOX);
+            uint8_t* slab = smem + stage * L::STAGE_BYTES;
+            for (int b = 0; b < nbox; ++b)
+              tma_load_2d(slab + b * L::RES_BOX, &tmR, &full_bar[stage], c0 + 32 * b, m_blk * BLOCK_M);
+            if (++stage == STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
       }
     } else if (RES && threadIdx.x == 32) {
       // residual slabs: the consumers release slab q of a tile after its last column group, so the first two slabs
@@ -182,7 +212,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
         const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-        const int nslab = min(CHUNKS, (p.N - n0 + 63) / 64);
+        const int nslab = min(L::BUF_SLABS, (p.N - n0 + 63) / 64);
         for (int q = 0; q < nslab; ++q, ++it) {
           const int buf = it & 1;
           mbar_wait(&res_empty[buf], ((it >> 1) & 1) ^ 1);
@@ -201,8 +231,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
         const int m_blk = tile / p.num_n_tiles;
         const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
-        const int vb = it & 1;
-        mbar_wait(&vec_empty[vb], ((it >> 1) & 1) ^ 1);
+        const int vb = it % L::VEC_BUFS;
+        mbar_wait(&vec_empty[vb], ((it / L::VEC_BUFS) & 1) ^ 1);
         float* vbias = reinterpret_cast<float*>(smem + L::VEC_OFFSET + vb * L::VEC_BYTES);
         float* vcs = vbias + BLOCK_N;
         float2* vln = reinterpret_cast<float2*>(vcs + BLOCK_N);
@@ -211,9 +241,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int i = lane; i < BLOCK_N; i += 32) {
             const int col = n0 + i;
             vbias[i] = (p.flags & B200VIT_EPI_BIAS) && col < p.N ? p.bias[col] : 0.f;
-            vcs[i] = (p.flags & B200VIT_EPI_LNFOLD) && col < p.N ? p.col_s[col] : 0.f;
+            if (!L::BIAS_ONLY) vcs[i] = (p.flags & B200VIT_EPI_LNFOLD) && col < p.N ? p.col_s[col] : 0.f;
           }
-        } else if (p.flags & B200VIT_EPI_LNFOLD) {
+        } else if (!L::BIAS_ONLY && (p.flags & B200VIT_EPI_LNFOLD)) {
           float s1[BLOCK_M / 32], s2[BLOCK_M / 32];
           bool ok[BLOCK_M / 32];
 #pragma unroll
@@ -246,12 +276,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int c = wg - 1;                       // rows [64c, 64c + 64) of the tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
-  const int flags = p.flags;
+  const int flags = L::BIAS_ONLY ? p.flags & ~B200VIT_EPI_LNFOLD : p.flags;  // the host routes LN folds elsewhere
   const bool vec_ok = (p.ldo & 1) == 0;
   int stage = 0;
   uint32_t phase = 0;
   int slab_it = 0;  // residual slabs consumed so far (the loader's count)
-  int pend_slab = -1;  // TMA_OUT && RES, thread 0: the slab buffer whose stores may still be reading it
+  // TMA_OUT && RES, thread 0: the slab its stores may still be reading, as the index of its empty barrier from
+  // empty_bar (a ring stage s: s; slab buffer b: STAGES + 2 + b, past res_full), or -1
+  int pend_slab = -1;
   uint8_t* const stg_wg = smem + L::OUT_OFFSET + c * (RES ? L::OUT_BOX : 64 * BLOCK_N * 2);
   float acc[NACC];
 
@@ -279,7 +311,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       // slab, which goes back to the residual loader so that it can fill it during this main loop)
       if (TMA_OUT && kb == 0 && t == 0) {
         tma_store_wait_read<0>();
-        if (RES && pend_slab >= 0) mbar_arrive(&res_empty[pend_slab]);
+        if (RES && pend_slab >= 0) mbar_arrive(&empty_bar[pend_slab]);
         pend_slab = -1;
       }
       // the MMAs of the previous k block have finished reading their stage once at most one group is in flight
@@ -300,8 +332,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // accumulator layout (wgmma m64nN, fp32): acc[4j + h] holds row (16 warp + lane/4 + 8 (h >> 1)),
     // column (8 j + 2 (lane % 4) + (h & 1)) of this warpgroup's 64 x BLOCK_N block
     const int tr0 = c * 64 + warp * 16 + (lane >> 2);
-    const int vb = it & 1;
-    mbar_wait(&vec_full[vb], (it >> 1) & 1);
+    const int vb = it % L::VEC_BUFS;
+    mbar_wait(&vec_full[vb], (it / L::VEC_BUFS) & 1);
     const float* vbias = reinterpret_cast<const float*>(smem + L::VEC_OFFSET + vb * L::VEC_BYTES);
     const float* vcs = vbias + BLOCK_N;
     const float2* vln = reinterpret_cast<const float2*>(vcs + BLOCK_N);
@@ -334,14 +366,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // TMA_OUT: this thread's bf16 pair in a staging box: row tr0 % 64 (+ 8 h), 16-byte chunk (j % 8) ^ (tr0 % 8),
     // byte 4 (lane % 4) -- the 8 rows of a warp store land in 8 different chunks, so the stores are conflict free
     const int stg_off = (tr0 - 64 * c) * 128 + 4 * (lane & 3);
-    // TMA_OUT && RES: the bf16 pairs of the current slab, held until the staging chunk is free again
-    uint32_t pks[8][2] = {};
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
       const int pc = 8 * j + 2 * (lane & 3);  // column of the pair in the tile
       const int col = n0 + pc;
-      if (RES && j % 8 == 0 && j / 8 < nslab) mbar_wait(&res_full[slab_it & 1], (slab_it >> 1) & 1);
-      uint8_t* slab = smem + L::RES_OFFSET + (slab_it & 1) * L::RES_SLAB + ((j % 8) / 4) * L::RES_BOX + res_off;
+      // RING_SLABS: the slabs sit in the ring stages after the tile's last k block
+      const bool ring_slab = L::RING_SLABS && j / 8 >= L::BUF_SLABS;
+      if (RES && j % 8 == 0 && j / 8 < nslab) {
+        if (ring_slab) mbar_wait(&full_bar[stage], phase);
+        else mbar_wait(&res_full[slab_it & 1], (slab_it >> 1) & 1);
+      }
+      uint8_t* const slab_base =
+          smem + (ring_slab ? stage * L::STAGE_BYTES : L::RES_OFFSET + (slab_it & 1) * L::RES_SLAB);
+      uint8_t* slab = slab_base + ((j % 8) / 4) * L::RES_BOX + res_off;
       uint8_t* stg = stg_wg + (RES ? 0 : (j / 8) * L::OUT_BOX) + stg_off + (((j % 8) ^ (lane >> 2)) << 4);
       const bool pair = vec_ok && col + 1 < p.N;
       float b0 = 0.f, b1 = 0.f, s0 = 0.f, s1 = 0.f;
@@ -380,16 +417,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         float r0 = 0.f, r1 = 0.f;
         if (TMA_OUT) {
           // the same values as below, into shared memory: the fp32 sum where its residual was read (no other thread
-          // touches that address), the bf16 pair into the staging box (rows past M are clipped by the store maps; N is
-          // a multiple of 8, so col + 1 < N)
+          // touches that address; RES: its bf16 copy is made from there once the staging chunk is free), the bf16
+          // pair into the staging box (rows past M are clipped by the store maps; N is a multiple of 8, so
+          // col + 1 < N)
           if (RES) {
             v0 += rr.x;
             v1 += rr.y;
-            if (p.out_f32) *rp = make_float2(v0, v1);
+            *rp = make_float2(v0, v1);
           }
           const uint32_t pk = pack_bf16x2(v0, v1);
-          if (RES) pks[j % 8][h] = pk;
-          else *reinterpret_cast<uint32_t*>(stg + h * 8 * 128) = pk;
+          if (!RES) *reinterpret_cast<uint32_t*>(stg + h * 8 * 128) = pk;
           r0 = __uint_as_float(pk << 16);
           r1 = __uint_as_float(pk & 0xFFFF0000u);
         } else if (pair) {
@@ -425,10 +462,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (RES && j % 8 == 7 && j / 8 < nslab) {
         if constexpr (TMA_OUT) {
           // The previous slab's stores have had this slab's arithmetic to read the chunk and their slab: wait for
-          // them, hand that slab back to the loader, then stage this slab's bf16 copy and store the slab and the chunk.
+          // them, hand that slab back to its loader, then stage this slab's bf16 copy -- rounded from the fp32 sums
+          // this thread wrote into the slab, rather than held in registers -- and store the slab and the chunk.
           if (t == 0) {
             tma_store_wait_read<0>();
-            if (pend_slab >= 0) mbar_arrive(&res_empty[pend_slab]);
+            if (pend_slab >= 0) mbar_arrive(&empty_bar[pend_slab]);
             pend_slab = -1;
           }
           warpgroup_sync(c);
@@ -436,26 +474,37 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-              for (int h = 0; h < 2; ++h)
-                *reinterpret_cast<uint32_t*>(stg_wg + stg_off + ((jj ^ (lane >> 2)) << 4) + h * 8 * 128) = pks[jj][h];
+              for (int h = 0; h < 2; ++h) {
+                const float2 s = *reinterpret_cast<const float2*>(slab_base + (jj / 4) * L::RES_BOX + res_off +
+                                                                  h * 8 * 128 + ((((jj % 4) * 2) ^ res_xor) << 4));
+                *reinterpret_cast<uint32_t*>(stg_wg + stg_off + ((jj ^ (lane >> 2)) << 4) + h * 8 * 128) =
+                    pack_bf16x2(s.x, s.y);
+              }
           fence_proxy_async_smem();
           warpgroup_sync(c);
           if (t == 0) {
-            const int buf = slab_it & 1, c0 = n0 + 64 * (j / 8), row0 = m_blk * BLOCK_M + 64 * c;
+            const int c0 = n0 + 64 * (j / 8), row0 = m_blk * BLOCK_M + 64 * c;
             if (row0 < p.M) {
-              const uint8_t* half = smem + L::RES_OFFSET + buf * L::RES_SLAB + c * 64 * 128;
+              const uint8_t* half = slab_base + c * 64 * 128;
               if (p.out_f32)
                 for (int b = 0; b < 2 && c0 + 32 * b < p.N; ++b)
                   tma_store_2d(&tmF, half + b * L::RES_BOX, c0 + 32 * b, row0);
               if (p.out_bf16) tma_store_2d(&tmO, stg_wg, c0, row0);
             }
             tma_store_commit();
-            pend_slab = buf;
+            pend_slab = ring_slab ? stage : STAGES + 2 + (slab_it & 1);
           }
         } else {
           mbar_arrive(&res_empty[slab_it & 1]);
         }
-        ++slab_it;
+        if (ring_slab) {
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        } else {
+          ++slab_it;
+        }
       }
     }
     mbar_arrive(&vec_empty[vb]);
@@ -489,7 +538,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (!row_ok[h]) continue;
-          float* so = p.stats_out + 2 * (size_t)row[h] * p.stats_parts;
+          // (row[0] + 8 h rather than row[h]: holding row[1] through the epilogue spills at 256 columns)
+          float* so = p.stats_out + 2 * (size_t)(row[0] + 8 * h) * p.stats_parts;
           for (int part = first; part < last; ++part) {
             float a = 0.f, b = 0.f;
 #pragma unroll
@@ -518,7 +568,10 @@ template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TM
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
                        const CUtensorMap& tmF, GemmParams& p, cudaStream_t stream) {
   using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
+  // 256 x 4 residual with TMA stores (slabs in the ring): 4 x 48 KB ring + 16 KB staging chunk + 1 KB bias + 128 B
+  // barriers + 1 KB alignment slack = 215 168 of the 232 448 bytes
   static_assert(L::DYN_BYTES <= 227 * 1024, "gemm: shared memory budget");
+  static_assert(!L::BIAS_ONLY || L::DYN_BYTES == 215168, "gemm: 256 x 4 residual TMA-store layout changed");
   auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
   B200_ENSURE_SMEM(kern, L::DYN_BYTES);
   if (!p.patch) p.rows_per_tile = BLOCK_M;
@@ -589,13 +642,18 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   // The TMA-store epilogue takes bf16 outputs and residual launches (fp32 + bf16), with ldo and N multiples of 8 so
   // that every row and its written part are whole 16-byte units (a precaution at N: the store maps clip there anyway).
   // A non-residual fp32 output (off the hot path) has no room for its 128 KB staging tile and stores from the
-  // registers, as do patch tiles.  Residual launches run 128-wide tiles: at 256 columns the residual slabs leave no
-  // room for the staging chunk beside the ring.
+  // registers, as do patch tiles.  A 256-wide residual tile with TMA stores has room for the bias slice only, so a
+  // residual launch with an LN fold runs 128-wide tiles (or, forced wide by test hook 12, stores directly).
   const bool tma_ok = !g_gemm_direct_store.load() && ((ldo | N) & 7) == 0 && (res || !out_f32);
+  const bool lnfold = (flags & B200VIT_EPI_LNFOLD) != 0;
   const int force = g_gemm_block_n.load();
-  const bool wide = force == 0 ? N > 128 && !(res && tma_ok) : force == 2;
+  // Residual launches take 256-wide tiles when there is at least one wide tile per SM (fewer would leave SMs idle).
+  // Measured on an H100 SXM at 700 W, M = 100 864, N = 768: K 768 (out-proj) 0.42-0.44 ms against 0.48-0.50 at 128
+  // columns, K 3072 (FC2) 0.91-0.93 ms against 0.95-0.97.
+  const bool res_wide_pays = (long long)((M + BLOCK_M - 1) / BLOCK_M) * ((N + 255) / 256) >= num_sms();
+  const bool wide = force == 0 ? N > 128 && (!(res && tma_ok) || (!lnfold && res_wide_pays)) : force == 2;
   const uint32_t block_n = wide ? 256 : 128;
-  const bool tma_out = tma_ok && !(res && wide);
+  const bool tma_out = tma_ok && !(res && wide && lnfold);
   CUtensorMap tmA, tmB, tmR{}, tmO{}, tmF{};
   if (tma_out && out_bf16) {
     const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
@@ -636,7 +694,9 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   }
   // residual launches trade ring stages for the two 32 KB residual slabs, TMA-store launches for the staging buffers
   if (tma_out) {
-    if (res) return launch_gemm<128, 4, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st);
+    if (res)
+      return wide ? launch_gemm<256, 4, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st)
+                  : launch_gemm<128, 4, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st);
     return wide ? launch_gemm<256, 3, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st)
                 : launch_gemm<128, 5, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st);
   }
