@@ -39,6 +39,10 @@ extern "C" {
 #define B200VIT_EPI_HARDSWISH 32  /* y * clamp(y + 3, 0, 6) / 6 after the bias, where GELU would be (nn.Hardswish,
                                      levit.py:32); not with B200VIT_EPI_GELU */
 #define B200VIT_EPI_HEADLN 64   /* b200vit_gemm_headnorm_bf16: per-head LayerNorm (no bias) instead of the RMS norm */
+#define B200VIT_EPI_SILU 128    /* y / (1 + exp(-y)) after the bias, where GELU would be (nn.SiLU, max_vit.py:55) */
+#define B200VIT_EPI_SIGMOID 256 /* 1 / (1 + exp(-y)) after the bias, where GELU would be (nn.Sigmoid, max_vit.py:57);
+                                   at most one of EPI_GELU, EPI_HARDSWISH, EPI_SILU and EPI_SIGMOID per call, and
+                                   neither EPI_SILU nor EPI_SIGMOID with EPI_RESIDUAL */
 
 /* attention flags (b200vit_attention_ex, b200vit_attention_varlen_ex, b200vit_encoder_blocks_ex) */
 #define B200VIT_ATTN_MASK_SELF 1  /* key i of query i gets probability 0 (LSA, vit_for_small_dataset.py:53-57) */
@@ -268,6 +272,51 @@ int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldk
  */
 int b200vit_attention_posbias(const void* qkv, int64_t ld, void* out, const float* table, int B, int F, int s, int H,
                               int dk, int dv, float scale, int flags, void* stream);
+
+/*
+ * MaxViT's window attention with a relative-position bias (max_vit.py:121-206) over B maps of gh x gw tokens, token
+ * (b, y, x) at row (b*gh + y)*gw + x of qkv[B*gh*gw, 3*H*dh] bf16 (packed as for b200vit_attention) and of
+ * out[B*gh*gw, H*dh] bf16.  With X = gh / w and Y = gw / w windows along each axis, window (b, i, j) holds the w*w
+ * tokens of local coordinates (u, v), u, v < w, at map position
+ *   grid = 0 (block, 'b d (x w1) (y w2)'):  (i*w + u, j*w + v)
+ *   grid = 1 (grid,  'b d (w1 x) (w2 y)'):  (u*X + i, v*Y + j)
+ * and each head attends among them:  softmax_k(scale * q.k + table[h][(du + w-1)*(2w-1) + (dv + w-1)]) v,  (du, dv)
+ * the query's local coordinates minus the key's.  table fp32 [H][(2w-1)^2] = rel_pos_bias.weight^T.
+ * One CTA per (window, head): the window's rows are gathered with cp.async into one 64-row tile, the head's bias
+ * table is staged in shared memory, both products on wgmma, an fp32 softmax over the w*w keys.
+ * 1 <= w <= 8, gh and gw multiples of w, dh = 32, 64, 80 or 128, H <= 65535; qkv, out and table 16-byte aligned.
+ * Isolation: a window's output is computed from its own rows only and nothing outside the B*gh*gw rows is read or
+ * written; a NaN or Inf stays within its window.
+ */
+int b200vit_attention_window_relpos(const void* qkv, void* out, const float* table, int B, int gh, int gw, int w,
+                                    int grid, int H, int dh, float scale, void* stream);
+
+/* rows of the token map one CTA of b200vit_mbconv_dwconv sums per (image, channel): the partial sums have
+ * ceil(oh*ow / B200VIT_MBCONV_PART_ROWS) parts per image */
+#define B200VIT_MBCONV_PART_ROWS 64
+
+/*
+ * MBConv's depthwise 3 x 3 convolution + BatchNorm + GELU (max_vit.py:106-108) on B channels-last maps:
+ *   x[B*h*w, C] bf16 -> y[B*oh*ow, C] bf16, oh = ceil(h / stride), ow = ceil(w / stride), zero padding 1,
+ *   y = GELU_erf(bias[c] + sum_taps w9[tap][c] * x),  w9 fp32 [9][C] tap-major and bias fp32 [C] with the BatchNorm
+ *   folded in by the caller.
+ * part[B][P][C] fp32, P = ceil(oh*ow / B200VIT_MBCONV_PART_ROWS): part[b][p][c] = the sum of the bf16-rounded y of
+ * rows p*PART_ROWS .. of image b in channel c, each slot written once in a fixed order (no atomics), so repeated calls
+ * give the same bits.  stride 1 or 2; C a multiple of 8; all pointers 16-byte aligned; x and y do not overlap.
+ */
+int b200vit_mbconv_dwconv(const void* x, int64_t M, const float* w9, const float* bias, void* y, float* part, int B,
+                          int h, int w, int C, int stride, void* stream);
+
+/*
+ * Squeeze-excitation around two bias-free GEMMs (max_vit.py:47-62):
+ *   b200vit_se_pool:   pooled[b][c] bf16 = (sum_p part[b][p][c]) * inv_n, the parts added in index order (the mean of
+ *                      b200vit_mbconv_dwconv's output); the gate then runs as GEMM(EPI_SILU), GEMM(EPI_SIGMOID) over
+ *                      the B pooled rows, so each SE weight matrix is read once per batch
+ *   b200vit_se_scale:  h[b*n + t][c] = bf16(h[b*n + t][c] * gate[b][c]), in place, gate bf16 [B][C]
+ * C a multiple of 8; all pointers 16-byte aligned.
+ */
+int b200vit_se_pool(const float* part, void* pooled, int B, int P, int C, float inv_n, void* stream);
+int b200vit_se_scale(void* h, const void* gate, int B, int n, int C, void* stream);
 
 /*
  * NaViT patch extraction over a LIST of images of different resolutions + LayerNorm(patch_dim) without bias, one launch:

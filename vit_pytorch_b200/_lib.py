@@ -23,9 +23,12 @@ EPI_LNFOLD = 8
 EPI_STATS = 16
 EPI_HARDSWISH = 32
 EPI_HEADLN = 64
+EPI_SILU = 128
+EPI_SIGMOID = 256
 ATTN_MASK_SELF = 1
 ATTN_GELU_OUT = 4
 ATTN_POSBIAS_MAX_KEYS = 4096    # B200VIT_ATTN_POSBIAS_MAX_KEYS
+MBCONV_PART_ROWS = 64           # B200VIT_MBCONV_PART_ROWS
 
 # every symbol include/b200vit.h declares (tests check that the library exports each of them)
 SYMBOLS = [
@@ -42,7 +45,8 @@ SYMBOLS = [
     "b200vit_attention_xca", "b200vit_local_patch_interaction", "b200vit_unfold_patches", "b200vit_pit_pool",
     "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
     "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
-    "b200vit_attention_posbias",
+    "b200vit_attention_posbias", "b200vit_attention_window_relpos", "b200vit_mbconv_dwconv", "b200vit_se_pool",
+    "b200vit_se_scale",
 ]
 
 
@@ -157,6 +161,14 @@ def lib() -> C.CDLL:
     L.b200vit_peg.argtypes = [vp, i64, vp, vp, vp, i32, i32, i32, i32, i32, vp]
     L.b200vit_attention_posbias.restype = i32
     L.b200vit_attention_posbias.argtypes = [vp, i64, vp, vp, i32, i32, i32, i32, i32, i32, f32, i32, vp]
+    L.b200vit_attention_window_relpos.restype = i32
+    L.b200vit_attention_window_relpos.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_mbconv_dwconv.restype = i32
+    L.b200vit_mbconv_dwconv.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    L.b200vit_se_pool.restype = i32
+    L.b200vit_se_pool.argtypes = [vp, vp, i32, i32, i32, f32, vp]
+    L.b200vit_se_scale.restype = i32
+    L.b200vit_se_scale.argtypes = [vp, vp, i32, i32, i32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -319,6 +331,18 @@ def gemm_hardswish(a: torch.Tensor, w: torch.Tensor, *, out_bf16: torch.Tensor, 
                    ) -> None:
     """out_bf16 = hardswish(a @ w^T + bias) (EPI_HARDSWISH: y * clamp(y + 3, 0, 6) / 6; LeViT's FeedForward)."""
     _gemm(a, w, out_bf16, None, bias, None, False, None, 1e-5, None, None, None, None, EPI_HARDSWISH)
+
+
+def gemm_silu(a: torch.Tensor, w: torch.Tensor, *, out_bf16: torch.Tensor, bias: Optional[torch.Tensor] = None
+              ) -> None:
+    """out_bf16 = silu(a @ w^T + bias) (EPI_SILU: y / (1 + exp(-y)); MaxViT's squeeze-excitation)."""
+    _gemm(a, w, out_bf16, None, bias, None, False, None, 1e-5, None, None, None, None, EPI_SILU)
+
+
+def gemm_sigmoid(a: torch.Tensor, w: torch.Tensor, *, out_bf16: torch.Tensor, bias: Optional[torch.Tensor] = None
+                 ) -> None:
+    """out_bf16 = sigmoid(a @ w^T + bias) (EPI_SIGMOID: 1 / (1 + exp(-y)); MaxViT's squeeze-excitation gate)."""
+    _gemm(a, w, out_bf16, None, bias, None, False, None, 1e-5, None, None, None, None, EPI_SIGMOID)
 
 
 def _gemm(a, w, out_bf16, out_f32, bias, resid, gelu, ln_sums, ln_eps, col_s, stats_out, n, k, extra_flags) -> None:
@@ -613,6 +637,66 @@ def attention_posbias(qkv: torch.Tensor, out: torch.Tensor, table: torch.Tensor,
                                              int(dk), int(dv), float(scale), ATTN_GELU_OUT if gelu_out else 0,
                                              _stream())
     _check(rc, "b200vit_attention_posbias")
+
+
+def attention_window_relpos(qkv: torch.Tensor, out: torch.Tensor, table: torch.Tensor, B: int, gh: int, gw: int,
+                            w: int, grid: bool, H: int, dh: int, scale: float) -> None:
+    """MaxViT attention inside the w x w windows of B token maps of gh x gw tokens with a relative-position bias:
+    qkv[B*gh*gw, 3*H*dh] packed q | k | v, token (b, y, x) at row (b*gh + y)*gw + x; out[B*gh*gw, H*dh].  grid False:
+    window (i, j) is the block of map positions (i*w + u, j*w + v); True: the dilated grid (u*gh/w + i, v*gw/w + j).
+    table fp32 [H, (2w-1)^2] = rel_pos_bias.weight^T, indexed by the local offset (du + w-1)*(2w-1) + dv + w-1."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out"); _chk(table, torch.float32, "table")
+    assert qkv.is_contiguous() and out.is_contiguous() and table.is_contiguous()
+    assert qkv.shape == (B * gh * gw, 3 * H * dh) and out.shape == (B * gh * gw, H * dh)
+    assert table.shape == (H, (2 * w - 1) ** 2)
+    with _Timed("attention_window_relpos", B=B, h=gh, w=gw, window=w, grid=bool(grid), H=H,
+                bytes=(qkv.numel() + out.numel()) * 2, flops=4.0 * B * gh * gw * H * w * w * dh):
+        rc = lib().b200vit_attention_window_relpos(_ptr(qkv), _ptr(out), _ptr(table), B, int(gh), int(gw), int(w),
+                                                   1 if grid else 0, H, dh, float(scale), _stream())
+    _check(rc, "b200vit_attention_window_relpos")
+
+
+def mbconv_parts(oh: int, ow: int) -> int:
+    """Partial sums per image that mbconv_dwconv writes for an oh x ow output map."""
+    return -(-(oh * ow) // MBCONV_PART_ROWS)
+
+
+def mbconv_dwconv(x: torch.Tensor, w9: torch.Tensor, bias: torch.Tensor, y: torch.Tensor, part: torch.Tensor, B: int,
+                  h: int, w: int, stride: int) -> None:
+    """y = GELU(depthwise 3 x 3 convolution of x, zero padding 1, stride 1 or 2, + bias): x bf16 [B*h*w, C]
+    channels-last, y bf16 [B*ceil(h/s)*ceil(w/s), C], w9 fp32 [9, C] tap-major and bias fp32 [C] with the BatchNorm
+    folded in; part fp32 [B, mbconv_parts(oh, ow), C] gets the per-image channel sums of the rounded y, part by part."""
+    _chk(x, torch.bfloat16, "x"); _chk(y, torch.bfloat16, "y")
+    for nm, t in (("w9", w9), ("bias", bias), ("part", part)):
+        _chk(t, torch.float32, nm)
+    M, Cc = x.shape
+    oh, ow = -(-h // stride), -(-w // stride)
+    assert x.is_contiguous() and y.is_contiguous() and w9.is_contiguous() and bias.is_contiguous()
+    assert y.shape == (B * oh * ow, Cc) and w9.shape == (9, Cc) and bias.numel() == Cc
+    assert part.is_contiguous() and part.shape == (B, mbconv_parts(oh, ow), Cc)
+    with _Timed("mbconv_dwconv", B=B, h=h, w=w, C=Cc, s=stride, bytes=(M + y.shape[0]) * Cc * 2):
+        rc = lib().b200vit_mbconv_dwconv(_ptr(x), M, _ptr(w9), _ptr(bias), _ptr(y), _ptr(part), B, int(h), int(w), Cc,
+                                         int(stride), _stream())
+    _check(rc, "b200vit_mbconv_dwconv")
+
+
+def se_pool(part: torch.Tensor, pooled: torch.Tensor, n: int) -> None:
+    """pooled bf16 [B, C] = the sum over the parts of part fp32 [B, P, C], in part order, divided by n."""
+    _chk(part, torch.float32, "part"); _chk(pooled, torch.bfloat16, "pooled")
+    B, P, Cc = part.shape
+    assert part.is_contiguous() and pooled.is_contiguous() and pooled.shape == (B, Cc)
+    with _Timed("se_pool", B=B, C=Cc, bytes=part.numel() * 4):
+        rc = lib().b200vit_se_pool(_ptr(part), _ptr(pooled), B, P, Cc, 1.0 / n, _stream())
+    _check(rc, "b200vit_se_pool")
+
+
+def se_scale(h: torch.Tensor, gate: torch.Tensor, B: int, n: int) -> None:
+    """In place h[b*n + t, c] *= gate[b, c], rounded to bf16: h bf16 [B*n, C], gate bf16 [B, C]."""
+    _chk(h, torch.bfloat16, "h"); _chk(gate, torch.bfloat16, "gate")
+    assert h.is_contiguous() and gate.is_contiguous() and h.shape[0] == B * n and gate.shape == (B, h.shape[1])
+    with _Timed("se_scale", B=B, n=n, C=h.shape[1], bytes=h.numel() * 4):
+        rc = lib().b200vit_se_scale(_ptr(h), _ptr(gate), B, int(n), h.shape[1], _stream())
+    _check(rc, "b200vit_se_scale")
 
 
 def varlen_index(lengths, device) -> tuple:

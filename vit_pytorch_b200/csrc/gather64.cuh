@@ -1,0 +1,90 @@
+// 64-row attention tiles whose rows are gathered from arbitrary rows of a packed qkv buffer (levit.cu, max_vit.cu):
+// every thread copies its 16-byte pieces with cp.async straight into the wgmma operand layouts -- 64-column slabs with
+// the 128B swizzle, then 16-column slabs with the 32B swizzle -- and the two products of one 64 x 64 score block.
+#pragma once
+#include "common.cuh"
+
+namespace b200 {
+namespace gather64 {
+
+constexpr int PB_ROWS = 64;
+constexpr int PB_THREADS = 128;
+
+// One operand block of 64 rows: N64 slabs 64 columns wide (128B swizzle), then N16 slabs 16 columns wide (32B swizzle).
+template <int D>
+struct PbSlabs {
+  static constexpr int N64 = D / 64;
+  static constexpr int N16 = (D % 64) / 16;
+  static_assert(N64 * 64 + N16 * 16 == D, "head width must be a multiple of 16");
+  static constexpr int S64 = PB_ROWS * 128;
+  static constexpr int S16 = PB_ROWS * 32;
+  static constexpr int OP = N64 * S64 + N16 * S16;
+};
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// shared-memory address of the 16-byte piece c (columns 8c .. 8c + 7) of row r of an operand block at `base`
+template <int D>
+__device__ __forceinline__ uint32_t piece_addr(uint32_t base, int r, int c) {
+  using S = PbSlabs<D>;
+  if (c < S::N64 * 8) return base + (c >> 3) * S::S64 + r * 128 + (((c & 7) ^ (r & 7)) << 4);
+  const int j = c - S::N64 * 8;
+  return base + S::N64 * S::S64 + (j >> 1) * S::S16 + r * 32 + (((j & 1) ^ ((r >> 2) & 1)) << 4);
+}
+
+// rows r of an operand block from global rows src(r) (negative: zero-fill without a read), D columns from `col`
+template <int D, typename RowFn>
+__device__ __forceinline__ void load_block(uint32_t base, const __nv_bfloat16* qkv, long long ld, int col, RowFn src,
+                                           int tid) {
+  constexpr int P = D / 8;
+  for (int i = tid; i < PB_ROWS * P; i += PB_THREADS) {
+    const int r = i / P, c = i - r * P;
+    const long long row = src(r);
+    const bool ok = row >= 0;
+    cp_async16(piece_addr<D>(base, r, c), ok ? qkv + row * ld + col + 8 * c : qkv, ok);
+  }
+}
+
+// S[64 x 64] = Q K^T over the slabs of one operand block each
+template <int DK>
+__device__ __forceinline__ void qk_mma(float (&s)[32], uint32_t sq, uint32_t sk) {
+  using S = PbSlabs<DK>;
+#pragma unroll
+  for (int c = 0; c < S::N64; ++c)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_m64n64k16(s, make_wgmma_desc(sq + c * S::S64, 1024, WGMMA_SW128) + 2 * k,
+                      make_wgmma_desc(sk + c * S::S64, 1024, WGMMA_SW128) + 2 * k, c != 0 || k != 0);
+#pragma unroll
+  for (int c = 0; c < S::N16; ++c)
+    wgmma_m64n64k16(s, make_wgmma_desc(sq + S::N64 * S::S64 + c * S::S16, 256, WGMMA_SW32),
+                    make_wgmma_desc(sk + S::N64 * S::S64 + c * S::S16, 256, WGMMA_SW32), S::N64 != 0 || c != 0);
+}
+
+// O[64 x DV] += P V, P the 64 x 64 probabilities in this thread's S registers, V one operand block
+template <int DV>
+__device__ __forceinline__ void pv_mma(float (&o)[PbSlabs<DV>::N64 > 0 ? PbSlabs<DV>::N64 : 1][32],
+                                       float (&o16)[PbSlabs<DV>::N16 > 0 ? PbSlabs<DV>::N16 : 1][8],
+                                       const float (&s)[32], uint32_t sv) {
+  using S = PbSlabs<DV>;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const uint32_t a[4] = {pack_bf16x2(s[8 * kk], s[8 * kk + 1]), pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]),
+                           pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7])};
+#pragma unroll
+    for (int c = 0; c < S::N64; ++c)
+      wgmma_m64n64k16_rs_tb(o[c], a, make_wgmma_desc_lbo(sv + c * S::S64 + kk * 2048, 1024, 1024, WGMMA_SW128));
+#pragma unroll
+    for (int c = 0; c < S::N16; ++c)
+      wgmma_m64n16k16_rs_tb(o16[c], a,
+                            make_wgmma_desc_lbo(sv + S::N64 * S::S64 + c * S::S16 + kk * 512, 256, 256, WGMMA_SW32));
+  }
+}
+
+}  // namespace gather64
+}  // namespace b200

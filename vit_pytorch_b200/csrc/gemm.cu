@@ -111,7 +111,9 @@ struct GemmSmem {
 __device__ __forceinline__ void warpgroup_sync(int c) { asm volatile("bar.sync %0, 128;" ::"r"(c + 1) : "memory"); }
 
 // tmO / tmF (TMA_OUT only): store maps over out_bf16 (64 x 64 boxes) and out_f32 (32 x 64 boxes), 128B swizzle
-template <int BLOCK_N, int STAGES, bool PATCH, bool RES, bool TMA_OUT>
+// SIG: the instances that take EPI_SILU / EPI_SIGMOID (the squeeze-excitation GEMMs); every other instance is compiled
+// without that branch
+template <int BLOCK_N, int STAGES, bool PATCH, bool RES, bool TMA_OUT, bool SIG = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO,
@@ -410,6 +412,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           v0 = v0 * fminf(fmaxf(v0 + 3.0f, 0.0f), 6.0f) * (1.0f / 6.0f);
           v1 = v1 * fminf(fmaxf(v1 + 3.0f, 0.0f), 6.0f) * (1.0f / 6.0f);
         }
+        if (SIG && (flags & (B200VIT_EPI_SILU | B200VIT_EPI_SIGMOID))) {
+          // sigmoid(y) = 1 / (1 + 2^(-y log2 e)) (nn.Sigmoid, max_vit.py:57); SiLU is y sigmoid(y) (max_vit.py:55)
+          const float g0 = fast_rcp(1.0f + fast_ex2(-1.4426950408889634f * v0));
+          const float g1 = fast_rcp(1.0f + fast_ex2(-1.4426950408889634f * v1));
+          const bool silu = (flags & B200VIT_EPI_SILU) != 0;
+          v0 = silu ? v0 * g0 : g0;
+          v1 = silu ? v1 * g1 : g1;
+        }
         const size_t o = (size_t)row[h] * p.ldo + col;
         float2* rp = reinterpret_cast<float2*>(slab + h * 8 * 128 + ((((j % 4) * 2) ^ res_xor) << 4));
         float2 rr = make_float2(0.f, 0.f);
@@ -564,7 +574,7 @@ void gemm_set_block_n(int v) { g_gemm_block_n = v; }
 static std::atomic<int> g_gemm_direct_store{0};
 void gemm_set_direct_store(int v) { g_gemm_direct_store = v; }
 
-template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false>
+template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false, bool SIG = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
                        const CUtensorMap& tmF, GemmParams& p, cudaStream_t stream) {
   using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
@@ -572,7 +582,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   // barriers + 1 KB alignment slack = 215 168 of the 232 448 bytes
   static_assert(L::DYN_BYTES <= 227 * 1024, "gemm: shared memory budget");
   static_assert(!L::BIAS_ONLY || L::DYN_BYTES == 215168, "gemm: 256 x 4 residual TMA-store layout changed");
-  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES, TMA_OUT, SIG>;
   B200_ENSURE_SMEM(kern, L::DYN_BYTES);
   if (!p.patch) p.rows_per_tile = BLOCK_M;
   p.num_m_tiles = (p.M + p.rows_per_tile - 1) / p.rows_per_tile;
@@ -614,8 +624,11 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   B200_CHECK_ARG(!(flags & B200VIT_EPI_LNFOLD) || (ln_sums && col_s && ln_parts >= 1 && ln_parts <= 64),
                  "gemm: EPI_LNFOLD needs ln_sums, col_s and 1 <= ln_parts <= 64");
   B200_CHECK_ARG(!(flags & B200VIT_EPI_STATS) || stats_out, "gemm: EPI_STATS without stats_out");
-  B200_CHECK_ARG((flags & (B200VIT_EPI_GELU | B200VIT_EPI_HARDSWISH)) != (B200VIT_EPI_GELU | B200VIT_EPI_HARDSWISH),
-                 "gemm: EPI_GELU and EPI_HARDSWISH are exclusive");
+  B200_CHECK_ARG(!(flags & B200VIT_EPI_RESIDUAL) || !(flags & (B200VIT_EPI_SILU | B200VIT_EPI_SIGMOID)),
+                 "gemm: EPI_SILU and EPI_SIGMOID do not combine with EPI_RESIDUAL");
+  const int act = flags & (B200VIT_EPI_GELU | B200VIT_EPI_HARDSWISH | B200VIT_EPI_SILU | B200VIT_EPI_SIGMOID);
+  B200_CHECK_ARG((act & (act - 1)) == 0,
+                 "gemm: EPI_GELU, EPI_HARDSWISH, EPI_SILU and EPI_SIGMOID are exclusive (flags 0x%x)", flags);
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   B200_CHECK_ARG(al16(bias) && al16(resid) && al16(col_s) && al16(out_bf16) && al16(out_f32) && al16(ln_sums),
                  "gemm: epilogue pointers must be 16-byte aligned");
@@ -651,7 +664,9 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   // Measured on an H100 SXM at 700 W, M = 100 864, N = 768: K 768 (out-proj) 0.42-0.44 ms against 0.48-0.50 at 128
   // columns, K 3072 (FC2) 0.91-0.93 ms against 0.95-0.97.
   const bool res_wide_pays = (long long)((M + BLOCK_M - 1) / BLOCK_M) * ((N + 255) / 256) >= num_sms();
-  const bool wide = force == 0 ? N > 128 && (!(res && tma_ok) || (!lnfold && res_wide_pays)) : force == 2;
+  // SiLU / sigmoid launches (squeeze-excitation over a few pooled rows) take their own 128-wide instances
+  const bool sig = (flags & (B200VIT_EPI_SILU | B200VIT_EPI_SIGMOID)) != 0;
+  const bool wide = !sig && (force == 0 ? N > 128 && (!(res && tma_ok) || (!lnfold && res_wide_pays)) : force == 2);
   const uint32_t block_n = wide ? 256 : 128;
   const bool tma_out = tma_ok && !(res && wide && lnfold);
   CUtensorMap tmA, tmB, tmR{}, tmO{}, tmF{};
@@ -692,6 +707,9 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
     int rc = encode_tmap_bf16(&tmB, W, 2, dims, strides, box);
     if (rc) return rc;
   }
+  if (sig)
+    return tma_out ? launch_gemm<128, 5, false, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st)
+                   : launch_gemm<128, 6, false, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st);
   // residual launches trade ring stages for the two 32 KB residual slabs, TMA-store launches for the staging buffers
   if (tma_out) {
     if (res)

@@ -283,17 +283,25 @@ class EncoderLayer:
     # [2 * heads * dim_head, D, k, k], rows k | v, and qkv_w holds the query rows only; run_blocks needs `grid`
     kv_stride: Optional[int] = None
     kv_w: Optional[torch.Tensor] = None
+    # with `window`: a learned relative-position bias inside every window (MaxViT, max_vit.py:148-159;
+    # b200vit_attention_window_relpos): the Embedding weight [(2 window - 1)^2, heads]; `grid_windows` cuts the map into
+    # dilated grids instead of contiguous blocks ('b d (w1 x) (w2 y)', max_vit.py:269)
+    rel_pos_bias: Optional[torch.Tensor] = None
+    grid_windows: bool = False
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
-    """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'kv' (sub-sampled keys), 'axial' (a
-    run_blocks call with `axial`, unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed
+    """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'window_relpos' (windows with a
+    relative-position bias), 'kv' (sub-sampled keys), 'axial' (a run_blocks call with `axial`, unless the layer's
+    temporal sub-block runs there), 'varlen' (`key_blocks`: a packed
     batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed or sub-sampled-key
     attention with `axial` or over a `packed` batch."""
     if L.window is not None or L.kv_stride is not None:
         if axial or packed:
             raise ValueError("windowed and sub-sampled-key attention run over B token grids only")
-        return "window" if L.window is not None else "kv"
+        if L.window is None:
+            return "kv"
+        return "window" if L.rel_pos_bias is None else "window_relpos"
     if L.xca_tau is not None or L.headmix is not None:
         if axial or packed:
             what = "cross-covariance" if L.xca_tau is not None else "head-mixing"
@@ -451,6 +459,9 @@ class TransformerEngine:
                  headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else head_width_reason(L.dim_head))
             if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
                 r = lpi_reason(L.lpi.kernel_size, 1)
+            if r is None and kernel == "window_relpos" and L.window ** 2 > WINDOW_MAX_TOKENS:
+                r = (f"window_size={L.window}: a window of {L.window ** 2} tokens (the relative-position window "
+                     f"attention kernel takes at most {WINDOW_MAX_TOKENS})")
             if r is None and L.window is not None and L.window ** 2 > WINDOW_MAX_TOKENS:
                 r = (f"local_patch_size={L.window}: a window of {L.window ** 2} tokens (the window attention kernel "
                      f"takes at most {WINDOW_MAX_TOKENS})")
@@ -500,6 +511,8 @@ class TransformerEngine:
                     t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(X.ln.gamma), _f32(X.ln.beta)
             if L.xca_tau is not None:
                 t[f"{i}.tau"] = L.xca_tau.detach().float().exp().reshape(-1).contiguous()
+            if L.rel_pos_bias is not None:
+                t[f"{i}.relpos"] = L.rel_pos_bias.detach().float().t().contiguous()
             if L.kv_stride is not None:
                 # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
                 t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.detach().permute(0, 2, 3, 1).reshape(L.kv_w.shape[0], -1))
@@ -642,13 +655,14 @@ class TransformerEngine:
             kernels.append(attention_kernel(L, axial is not None, varlen is not None, vl is not None))
             if L.lpi is not None and (grid is None or grid[0] * grid[1] != N or axial is not None or varlen is not None):
                 raise ValueError("a layer with a local patch interaction needs `grid` = (h, w) with h * w == N")
-            if kernels[-1] in ("window", "kv"):
+            if kernels[-1] in ("window", "window_relpos", "kv"):
                 if grid is None or grid[0] * grid[1] != N:
                     raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
-                step = L.window if kernels[-1] == "window" else L.kv_stride
-                if (grid[0] % step or grid[1] % step) if kernels[-1] == "window" else min(grid) < step:
+                windowed = kernels[-1] != "kv"
+                step = L.window if windowed else L.kv_stride
+                if (grid[0] % step or grid[1] % step) if windowed else min(grid) < step:
                     raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {step} x {step} "
-                                     f"{'windows' if kernels[-1] == 'window' else 'key patches'}")
+                                     f"{'windows' if windowed else 'key patches'}")
         xb, qkv, o, h = ws["xn"], ws["qkv"], ws["o"], ws["h"]
         sums = ws["stats_in"] if primed else None          # fold: the row sums of xb the next LN-folded GEMM reads
 
@@ -700,6 +714,9 @@ class TransformerEngine:
         def attend(kernel: str, L: EncoderLayer, i: int) -> None:
             if kernel == "window":
                 _lib.attention_window(qkv, o, B, grid[0], grid[1], L.window, L.heads, L.dim_head, L.scale)
+            elif kernel == "window_relpos":
+                _lib.attention_window_relpos(qkv, o, t[f"{i}.relpos"], B, grid[0], grid[1], L.window, L.grid_windows,
+                                             L.heads, L.dim_head, L.scale)
             elif kernel == "xca":
                 _lib.attention_xca(qkv, t[f"{i}.tau"], o, B, N, L.heads, L.dim_head)
             elif kernel == "headmix":
