@@ -199,6 +199,64 @@ def test_attention_axial_isolation_under_poisoning(dh, L, G):
             assert torch.equal(run_axial(buf[:T], km, B, L, G, H, dh, zero), clean)
 
 
+def assert_nan_query_row(run, qkv, row, dh, what):
+    """A NaN query in one row: every score of that row is NaN, so the row is NaN (the reference's softmax); every
+    other row, and the row's other heads, are bit-identical to the clean run."""
+    clean = run(qkv)
+    assert torch.isfinite(clean.float()).all()
+    bad = qkv.clone()
+    bad[row, :dh] = NAN                  # head 0's query
+    got = run(bad)
+    assert torch.isnan(got[row, :dh].float()).all(), f"{what}: the NaN query row is not NaN"
+    keep = torch.ones(got.shape[0], dtype=torch.bool, device=DEV)
+    keep[row] = False
+    assert_rows_equal(got, clean, keep, what)
+    assert torch.equal(got[row, dh:], clean[row, dh:]), f"{what}: the other heads of the NaN query row changed"
+
+
+@pytest.mark.parametrize("dh", [32, 64, 80, 128])
+def test_attention_axial_nan_query_row(dh):
+    B, L, G, H = 3, 8, 3, 2
+    g = torch.Generator(device=DEV).manual_seed(dh)
+    qkv = torch.randn(B * L * G, 3 * H * dh, device=DEV, generator=g).bfloat16()
+    for name, km in axial_masks(B, L, g).items():
+        for zero in (True, False):
+            assert_nan_query_row(lambda x: run_axial(x, km, B, L, G, H, dh, zero), qkv, 2 * L * G + 5, dh,
+                                 f"{name} zero={zero}")
+
+
+@pytest.mark.parametrize("dh", [32, 64, 80, 128])
+@pytest.mark.parametrize("p", [2, 7])                 # several windows per tile, one window per tile
+def test_attention_window_nan_query_row(dh, p):
+    B, H, gh, gw = 2, 2, 2 * p, 3 * p
+    g = torch.Generator(device=DEV).manual_seed(dh * 10 + p)
+    qkv = torch.randn(B * gh * gw, 3 * H * dh, device=DEV, generator=g).bfloat16()
+
+    def run(x):
+        out = torch.full((B * gh * gw, H * dh), 5.0, device=DEV, dtype=torch.bfloat16)
+        _lib.attention_window(x, out, B, gh, gw, p, H, dh, dh ** -0.5)
+        torch.cuda.synchronize()
+        return out
+    assert_nan_query_row(run, qkv, gh * gw + gw + 1, dh, f"p={p}")
+
+
+@pytest.mark.parametrize("dh", [32, 64, 80, 128])
+@pytest.mark.parametrize("grid", [False, True])
+def test_attention_window_relpos_nan_query_row(dh, grid):
+    B, H, w = 2, 2, 7
+    gh = gw = 2 * w
+    g = torch.Generator(device=DEV).manual_seed(dh * 10 + grid)
+    qkv = torch.randn(B * gh * gw, 3 * H * dh, device=DEV, generator=g).bfloat16()
+    table = torch.randn(H, (2 * w - 1) ** 2, device=DEV, generator=g)
+
+    def run(x):
+        out = torch.full((B * gh * gw, H * dh), 5.0, device=DEV, dtype=torch.bfloat16)
+        _lib.attention_window_relpos(x, out, table, B, gh, gw, w, grid, H, dh, dh ** -0.5)
+        torch.cuda.synchronize()
+        return out
+    assert_nan_query_row(run, qkv, gh * gw + gw + 1, dh, f"grid={grid}")
+
+
 def cls_inputs(B, n, first, H, dh, g):
     I = H * dh
     rows = n + first + 2                  # every image: `first` skipped rows, n context rows, 2 unused rows

@@ -1,4 +1,5 @@
-"""-m gpu: Twins-SVT on the H100.  The four kernels of csrc/twins.cu against fp64 references with per-element bounds
+"""-m gpu: Twins-SVT on the H100.  Its four kernels (window attention in csrc/attention_tile64.cu, the other three in
+csrc/twins.cu) against fp64 references with per-element bounds
 (the attention kernels through oracle/attention_bounds.py, the patch merging through oracle.bounds.layernorm_reference,
 the positional encoding with a bound built like test_gpu_pit.pool_reference), what they write and which rows they
 read; then the model: every case of tests/golden/twins_svt_spec.py through the comparison of

@@ -6,21 +6,21 @@
 // One CTA = one warpgroup = 64 consecutive queries of one (image, head).  The queries are gathered from the full-grid
 // qkv buffer: query n of the tile is the token (s i, s j), i = n / Fq, j = n % Fq, so the downsampling layer's q comes
 // out of the same full-grid QKV GEMM as its keys and values.  Keys and values run in blocks of 64 through two shared-
-// memory slots: every thread copies its 16-byte pieces with cp.async straight into the wgmma operand layouts (64-column
-// slabs with the 128B swizzle, 16-column slabs with the 32B swizzle), block kb + 1 in flight while block kb is
-// computed.  Rows past the image's tokens are zero-filled without a read, so nothing outside the image is touched.
+// memory slots: every thread copies its 16-byte pieces with cp.async straight into the wgmma operand tiles of
+// tile64.cuh, block kb + 1 in flight while block kb is computed.  Rows past the image's tokens are zero-filled without
+// a read, so nothing outside the image is touched.
 // The head's F*F bias values (times log2 e) are staged in shared memory once; each (query, key) index is formed from
 // the coordinates in registers, so no [H, Nq, Nk] bias exists anywhere.  Per block: S = Q K^T with wgmma, the bias
 // gathered and added, keys past Nk masked to -inf, the online softmax of attention.cu in fp32, O += P V with wgmma (P
 // from registers, V as the transposed B operand).  Streaming every block (instead of keeping an image's keys
 // resident) and the 64-query tile are untuned choices: no measurement preceded them.
-#include "gather64.cuh"
+#include "tile64.cuh"
 #include "host_util.h"
 
 namespace {
 
 using namespace b200;
-using namespace b200::gather64;
+using namespace b200::tile64;
 
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
@@ -45,10 +45,10 @@ struct PosBiasParams {
 };
 
 template <int DK, int DV>
-__global__ void __launch_bounds__(PB_THREADS)
+__global__ void __launch_bounds__(THREADS)
 attention_posbias_kernel(const PosBiasParams p) {
-  using SK = PbSlabs<DK>;
-  using SV = PbSlabs<DV>;
+  using SK = Slabs<DK>;
+  using SV = Slabs<DV>;
   constexpr int KV = SK::OP + SV::OP;  // one slot: K block | V block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -56,9 +56,9 @@ attention_posbias_kernel(const PosBiasParams p) {
   float* tab = reinterpret_cast<float*>(smem + SK::OP + 2 * KV);
 
   const int h = blockIdx.y, b = blockIdx.z;
-  const int q0 = blockIdx.x * PB_ROWS;
+  const int q0 = blockIdx.x * ROWS;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int F = p.F, Nk = p.Nk, nkb = (Nk + PB_ROWS - 1) / PB_ROWS;
+  const int F = p.F, Nk = p.Nk, nkb = (Nk + ROWS - 1) / ROWS;
   const long long img0 = (long long)b * Nk;  // first row of this image in qkv
   const uint32_t sq = smem_u32(smem), slot0 = sq + SK::OP;
   const int kcol = p.H * DK + h * DK, vcol = 2 * p.H * DK + h * DV;
@@ -73,7 +73,7 @@ attention_posbias_kernel(const PosBiasParams p) {
   auto load_kv = [&](int kb) {
     const uint32_t base = slot0 + (kb & 1) * KV;
     auto key_row = [&](int r) -> long long {
-      const int m = kb * PB_ROWS + r;
+      const int m = kb * ROWS + r;
       return m < Nk ? img0 + m : -1;
     };
     load_block<DK>(base, p.qkv, p.ld, kcol, key_row, tid);
@@ -82,7 +82,7 @@ attention_posbias_kernel(const PosBiasParams p) {
   load_kv(0);
   cp_async_commit();
   const float* th = p.table + (long long)h * Nk;
-  for (int i = tid; i < Nk; i += PB_THREADS) tab[i] = th[i] * 1.4426950408889634f;
+  for (int i = tid; i < Nk; i += THREADS) tab[i] = th[i] * 1.4426950408889634f;
 
   // this thread's two query rows r = 16 warp + lane/4 + 8 rh: their coordinates on the input grid
   int qy[2], qx[2];
@@ -207,11 +207,11 @@ attention_posbias_kernel(const PosBiasParams p) {
 
 template <int DK, int DV>
 int launch_posbias(const PosBiasParams& p, cudaStream_t stream) {
-  constexpr int KV = PbSlabs<DK>::OP + PbSlabs<DV>::OP;
-  const int bytes = PbSlabs<DK>::OP + 2 * KV + B200VIT_ATTN_POSBIAS_MAX_KEYS * 4 + 1024;  // slack for 1024B alignment
+  constexpr int KV = Slabs<DK>::OP + Slabs<DV>::OP;
+  const int bytes = Slabs<DK>::OP + 2 * KV + B200VIT_ATTN_POSBIAS_MAX_KEYS * 4 + 1024;  // slack for 1024B alignment
   auto kern = attention_posbias_kernel<DK, DV>;
   B200_ENSURE_SMEM(kern, bytes);
-  kern<<<dim3((p.Nq + PB_ROWS - 1) / PB_ROWS, p.H, p.B), PB_THREADS, bytes, stream>>>(p);
+  kern<<<dim3((p.Nq + ROWS - 1) / ROWS, p.H, p.B), THREADS, bytes, stream>>>(p);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
