@@ -553,6 +553,24 @@ int b200vit_peg(const float* x, int64_t M, const float* w, const float* bias, fl
                 int k, void* stream);
 
 /*
+ * CvT's convolutional projections, depthwise halves (DepthWiseConv2d up to its 1 x 1 convolution, cvt.py:51-60, 74-75),
+ * on the LayerNorm'ed token map x[M, C] bf16 of B images of h x w tokens (token (b, y, x) at row (b*h + y)*w + x,
+ * M = B*h*w), both outputs from one read of x:
+ *   q_out[(b, y, x), c]  = bq[c]  + sum_{i, j < k} wq[i*k + j][c]  x[(b, y + i - k/2, x + j - k/2), c]
+ *   kv_out[(b, r, q), c] = bkv[c] + sum_{i, j < k} wkv[i*k + j][c] x[(b, s*r + i - k/2, s*q + j - k/2), c]
+ * q_out [M, C] bf16 (stride 1), kv_out [B*oh*ow, C] bf16 with oh = (h - 1)/s + 1, ow = (w - 1)/s + 1, row
+ * (b*oh + r)*ow + q (stride s).  Taps outside the map are zero (padding k / 2).  wq, wkv fp32 [k*k][C] tap major and
+ * bq, bkv fp32 [C], with the BatchNorm (eval) folded in by the caller: w * g / sqrt(var + eps), beta - mean * g /
+ * sqrt(var + eps).  Sums in fp32 in tap order, rounded to bf16 once; no atomics, so repeated calls give the same bits.
+ * k = 1, 3, 5 or 7, s >= 1, C a multiple of 8, B, h, w >= 1; all pointers 16-byte aligned; x overlaps neither output.
+ * Each image's outputs come from its own rows only; nothing outside the B*h*w / B*oh*ow addressed rows is read or
+ * written.
+ */
+int b200vit_conv_proj_dw(const void* x, int64_t M, const float* wq, const float* bq, const float* wkv,
+                         const float* bkv, void* q_out, void* kv_out, int B, int h, int w, int C, int k, int s,
+                         void* stream);
+
+/*
  * ReLU then MaxPool2d(pk, stride ps, padding pp) in one pass (CCT's tokenizer, cct.py:187-190): y[M, C] bf16
  * channels-last (M = B*H*W, as b200vit_conv_im2col_nhwc's x) ->
  *   out[b*oh*ow + r*ow + q, c] = relu(max_{i, j < pk} y[(b, r*ps - pp + i, q*ps - pp + j), c]),

@@ -46,7 +46,7 @@ SYMBOLS = [
     "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
     "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
     "b200vit_attention_posbias", "b200vit_attention_window_relpos", "b200vit_mbconv_dwconv", "b200vit_se_pool",
-    "b200vit_se_scale",
+    "b200vit_se_scale", "b200vit_conv_proj_dw",
 ]
 
 
@@ -169,6 +169,8 @@ def lib() -> C.CDLL:
     L.b200vit_se_pool.argtypes = [vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_se_scale.restype = i32
     L.b200vit_se_scale.argtypes = [vp, vp, i32, i32, i32, vp]
+    L.b200vit_conv_proj_dw.restype = i32
+    L.b200vit_conv_proj_dw.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -1036,6 +1038,27 @@ def peg(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, y: torch.Tensor, B
     with _Timed("peg", B=B, h=gh, w=gw, C=Cc, k=k, bytes=M * Cc * 8):
         rc = lib().b200vit_peg(_ptr(x), M, _ptr(w), _ptr(bias), _ptr(y), B, int(gh), int(gw), Cc, int(k), _stream())
     _check(rc, "b200vit_peg")
+
+
+def conv_proj_dw(x: torch.Tensor, wq: torch.Tensor, bq: torch.Tensor, wkv: torch.Tensor, bkv: torch.Tensor,
+                 q_out: torch.Tensor, kv_out: torch.Tensor, B: int, h: int, w: int, k: int, s: int) -> None:
+    """CvT's depthwise convolutional projections from one read of x bf16 [B*h*w, C] channels-last: q_out bf16
+    [B*h*w, C] the k x k depthwise convolution (zero padding k // 2) at stride 1, kv_out bf16 [B*oh*ow, C]
+    (oh = (h - 1) // s + 1, likewise ow) the same at stride s; wq, wkv fp32 [k*k, C] tap major and bq, bkv fp32 [C]
+    with the BatchNorm folded in."""
+    _chk(x, torch.bfloat16, "x"); _chk(q_out, torch.bfloat16, "q_out"); _chk(kv_out, torch.bfloat16, "kv_out")
+    for nm, t in (("wq", wq), ("bq", bq), ("wkv", wkv), ("bkv", bkv)):
+        _chk(t, torch.float32, nm)
+    M, Cc = x.shape
+    oh, ow = (h - 1) // s + 1, (w - 1) // s + 1
+    assert x.is_contiguous() and q_out.is_contiguous() and kv_out.is_contiguous()
+    assert q_out.shape == (M, Cc) and kv_out.shape == (B * oh * ow, Cc)
+    for wt, bt in ((wq, bq), (wkv, bkv)):
+        assert wt.is_contiguous() and bt.is_contiguous() and wt.shape == (k * k, Cc) and bt.numel() == Cc
+    with _Timed("conv_proj_dw", B=B, h=h, w=w, C=Cc, k=k, s=s, bytes=(2 * M + kv_out.shape[0]) * Cc * 2):
+        rc = lib().b200vit_conv_proj_dw(_ptr(x), M, _ptr(wq), _ptr(bq), _ptr(wkv), _ptr(bkv), _ptr(q_out),
+                                        _ptr(kv_out), B, int(h), int(w), Cc, int(k), int(s), _stream())
+    _check(rc, "b200vit_conv_proj_dw")
 
 
 def relu_maxpool(y: torch.Tensor, B: int, H: int, W: int, pk: int, ps: int, pp: int, *,

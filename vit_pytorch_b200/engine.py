@@ -134,6 +134,7 @@ XCA_WIDTHS = (32, 48, 64, 80, 128)         # b200vit_attention_xca
 LPI_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_local_patch_interaction
 WINDOW_MAX_TOKENS = 64                     # b200vit_attention_window: tokens of one window
 PEG_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_peg
+CONV_PROJ_KERNEL_SIZES = (1, 3, 5, 7)      # b200vit_conv_proj_dw
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -237,6 +238,44 @@ def lpi_weights(P: LPIBlock) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, 
     return w1.t().contiguous(), b1.contiguous(), w2.t().contiguous(), b2.contiguous()
 
 
+class ConvProj(NamedTuple):
+    """CvT's convolutional projections (cvt.py:51-60, 74-75) of the normalised h x w token grid: for the queries a
+    depthwise k x k convolution at stride 1, for the keys / values one at stride `stride`, both bias-free with zero
+    padding k // 2 and followed by a BatchNorm (eval, on its running statistics); the bias-free 1 x 1 convolutions
+    after them are EncoderLayer.qkv_w (queries) and kv_w (keys | values)."""
+    q_w: torch.Tensor                             # [D, 1, k, k]
+    q_bn_w: torch.Tensor
+    q_bn_b: torch.Tensor
+    q_bn_mean: torch.Tensor                       # running_mean, a buffer
+    q_bn_var: torch.Tensor                        # running_var, a buffer
+    q_bn_eps: float
+    kv_w: torch.Tensor                            # [D, 1, k, k]
+    kv_bn_w: torch.Tensor
+    kv_bn_b: torch.Tensor
+    kv_bn_mean: torch.Tensor
+    kv_bn_var: torch.Tensor
+    kv_bn_eps: float
+    kernel_size: int
+    stride: int
+
+    def grid(self, h: int, w: int) -> Tuple[int, int]:
+        """The (h, w) of the key / value map of an h x w token grid."""
+        return (h - 1) // self.stride + 1, (w - 1) // self.stride + 1
+
+
+def conv_proj_weights(P: ConvProj) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(wq, bq, wkv, bkv) fp32 of b200vit_conv_proj_dw: each BatchNorm (eval) folded into its bias-free depthwise
+    convolution, w' = w g / sqrt(var + eps), b' = beta - mean g / sqrt(var + eps); the weights tap-major [k*k, D]."""
+    f = lambda t: t.detach().float()                                                    # noqa: E731
+    out = []
+    for w, g, beta, mean, var, eps in ((P.q_w, P.q_bn_w, P.q_bn_b, P.q_bn_mean, P.q_bn_var, P.q_bn_eps),
+                                       (P.kv_w, P.kv_bn_w, P.kv_bn_b, P.kv_bn_mean, P.kv_bn_var, P.kv_bn_eps)):
+        inv = f(g) / torch.sqrt(f(var) + eps)
+        out.append((f(w).reshape(w.shape[0], -1) * inv[:, None]).t().contiguous())
+        out.append((f(beta) - f(mean) * inv).contiguous())
+    return out[0], out[1], out[2], out[3]
+
+
 @dataclass
 class EncoderLayer:
     """One pre-LN encoder layer as a model family describes it to the engine (reference vit.py:78-81):
@@ -288,15 +327,19 @@ class EncoderLayer:
     # dilated grids instead of contiguous blocks ('b d (w1 x) (w2 y)', max_vit.py:269)
     rel_pos_bias: Optional[torch.Tensor] = None
     grid_windows: bool = False
+    # queries and keys / values from CvT's convolutional projections of the normalised token grid (cvt.py:74-75,
+    # 86-87; b200vit_conv_proj_dw, then b200vit_attention_kv): qkv_w holds the queries' 1 x 1 rows [I, D] and kv_w the
+    # keys' and values' [2I, D], rows k | v; run_blocks needs `grid`
+    conv_proj: Optional[ConvProj] = None
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
     """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'window_relpos' (windows with a
-    relative-position bias), 'kv' (sub-sampled keys), 'axial' (a run_blocks call with `axial`, unless the layer's
-    temporal sub-block runs there), 'varlen' (`key_blocks`: a packed
-    batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed or sub-sampled-key
+    relative-position bias), 'kv' (sub-sampled keys: a strided convolution or CvT's convolutional projections), 'axial'
+    (a run_blocks call with `axial`, unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a
+    packed batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed or sub-sampled-key
     attention with `axial` or over a `packed` batch."""
-    if L.window is not None or L.kv_stride is not None:
+    if L.window is not None or L.kv_stride is not None or L.conv_proj is not None:
         if axial or packed:
             raise ValueError("windowed and sub-sampled-key attention run over B token grids only")
         if L.window is None:
@@ -462,6 +505,9 @@ class TransformerEngine:
             if r is None and kernel == "window_relpos" and L.window ** 2 > WINDOW_MAX_TOKENS:
                 r = (f"window_size={L.window}: a window of {L.window ** 2} tokens (the relative-position window "
                      f"attention kernel takes at most {WINDOW_MAX_TOKENS})")
+            if r is None and L.conv_proj is not None and L.conv_proj.kernel_size not in CONV_PROJ_KERNEL_SIZES:
+                r = (f"proj_kernel={L.conv_proj.kernel_size} (the convolutional-projection kernel is built for 1, 3, 5 "
+                     f"and 7)")
             if r is None and L.window is not None and L.window ** 2 > WINDOW_MAX_TOKENS:
                 r = (f"local_patch_size={L.window}: a window of {L.window ** 2} tokens (the window attention kernel "
                      f"takes at most {WINDOW_MAX_TOKENS})")
@@ -513,7 +559,11 @@ class TransformerEngine:
                 t[f"{i}.tau"] = L.xca_tau.detach().float().exp().reshape(-1).contiguous()
             if L.rel_pos_bias is not None:
                 t[f"{i}.relpos"] = L.rel_pos_bias.detach().float().t().contiguous()
-            if L.kv_stride is not None:
+            if L.conv_proj is not None:
+                # the depthwise halves with their BatchNorms folded (tap-major) and the keys' / values' 1 x 1 rows
+                t[f"{i}.cpq.w"], t[f"{i}.cpq.b"], t[f"{i}.cpkv.w"], t[f"{i}.cpkv.b"] = conv_proj_weights(L.conv_proj)
+                t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.reshape(L.kv_w.shape[0], -1))
+            elif L.kv_stride is not None:
                 # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
                 t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.detach().permute(0, 2, 3, 1).reshape(L.kv_w.shape[0], -1))
             if L.lpi is not None:
@@ -628,7 +678,9 @@ class TransformerEngine:
         interaction, windowed attention or sub-sampled keys need (XCiT, Twins-SVT).  A layer with sub-sampled keys cannot
         fold its LayerNorm into the key / value projection (one convolution window spans tokens with different
         statistics): in both LayerNorm modes it runs layernorm(x -> xb), the query GEMM on xb, conv_im2col_nhwc of xb
-        and the key / value GEMM (kernel size 1: the GEMM on xb itself), then attention_kv.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
+        and the key / value GEMM (kernel size 1: the GEMM on xb itself), then attention_kv.  A layer with convolutional
+        projections (CvT) runs layernorm(x -> xb), conv_proj_dw of xb into the query and key / value operands, their
+        1 x 1 GEMMs, then attention_kv; the projections pad, so any h, w >= 1 will do.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
         axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
         onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
         fc1 is the plain GEMM on that copy.  The call is checked first: a ValueError leaves x as it was.
@@ -658,6 +710,8 @@ class TransformerEngine:
             if kernels[-1] in ("window", "window_relpos", "kv"):
                 if grid is None or grid[0] * grid[1] != N:
                     raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
+                if L.conv_proj is not None:
+                    continue                   # the projections pad: any h, w >= 1
                 windowed = kernels[-1] != "kv"
                 step = L.window if windowed else L.kv_stride
                 if (grid[0] % step or grid[1] % step) if windowed else min(grid) < step:
@@ -696,7 +750,11 @@ class TransformerEngine:
             _lib.gemm(a, t[w + ".w"], out_f32=x, out_bf16=copy, bias=t[w + ".b"], resid=resid, stats_out=stats)
 
         def subsampled(L: EncoderLayer, i: int) -> None:
-            """o = attention of LN1(x)'s queries over the keys / values of its strided convolution."""
+            """o = attention of LN1(x)'s queries over the keys / values of its strided convolution, or of its
+            convolutional projections (CvT)."""
+            if L.conv_proj is not None:
+                conv_projected(L, i)
+                return
             I, k = L.heads * L.dim_head, L.kv_stride
             kh, kw = grid[0] // k, grid[1] // k
             _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
@@ -709,6 +767,22 @@ class TransformerEngine:
                 _lib.conv_im2col_nhwc(xb, col, B, grid[0], grid[1], k, k, 0)
             kv = torch.empty(B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
             _lib.gemm(col, t[f"{i}.kv.w"], out_bf16=kv)
+            _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
+
+        def conv_projected(L: EncoderLayer, i: int) -> None:
+            """CvT: layernorm(x -> xb), both depthwise projections of xb in one pass (the LayerNorm cannot be folded:
+            the padding taps must read zeros of the normalised map), the 1 x 1 GEMMs, attention_kv."""
+            P, I, D = L.conv_proj, L.heads * L.dim_head, x.shape[1]
+            kh, kw = P.grid(*grid)
+            _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
+            aq = torch.empty(x.shape[0], D, device=x.device, dtype=torch.bfloat16)
+            akv = torch.empty(B * kh * kw, D, device=x.device, dtype=torch.bfloat16)
+            _lib.conv_proj_dw(xb, t[f"{i}.cpq.w"], t[f"{i}.cpq.b"], t[f"{i}.cpkv.w"], t[f"{i}.cpkv.b"], aq, akv, B,
+                              grid[0], grid[1], P.kernel_size, P.stride)
+            q = qkv[:, :I]
+            _lib.gemm(aq, t[f"{i}.qkv.w"], out_bf16=q)
+            kv = torch.empty(B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
+            _lib.gemm(akv, t[f"{i}.kv.w"], out_bf16=kv)
             _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
 
         def attend(kernel: str, L: EncoderLayer, i: int) -> None:
