@@ -162,6 +162,15 @@ def layernorm_reference(x: Tensor, gamma: Tensor, beta: Optional[Tensor] = None,
                         depth: Optional[int] = None) -> Tuple[Tensor, Tensor]:
     """(ref, bound) of the bf16 LayerNorm of the rows x[m, pd] (the patch pixels, in the output's column order) as
     the patch kernels compute it.  depth: the deepest fp32 sum of a row (default ceil(pd / 32) + 5, one warp)."""
+    ref, e32 = layernorm_e32(x, gamma, beta, eps, depth)
+    # the rounding of y32 is within half its ulp: at most one ulp of ref plus 2^-8 E32
+    return ref, bf16_ulp(ref) + (1 + U_BF16) * e32
+
+
+def layernorm_e32(x: Tensor, gamma: Tensor, beta: Optional[Tensor] = None, eps: float = 1e-5,
+                  depth: Optional[int] = None) -> Tuple[Tensor, Tensor]:
+    """(ref, E32): the fp64 LayerNorm of the rows x[m, pd] and the bound E32 of the fp32 value a one-warp two-pass
+    LayerNorm computes before any output rounding (module docstring).  depth as in layernorm_reference."""
     x = x.double()
     pd = x.shape[1]
     d = depth if depth is not None else -(-pd // 32) + 5
@@ -175,8 +184,7 @@ def layernorm_reference(x: Tensor, gamma: Tensor, beta: Optional[Tensor] = None,
     d_mu = (d + 2) * U * x.abs().mean(1, keepdim=True)
     rel = (d + 3) * U / 2 + d_mu * d_mu / (2 * (var + eps)) + 5 * U
     e32 = g.abs() * (xh.abs() * (rel + 3 * U) + rstd * d_mu) + U * ((xh * g).abs() + bt.abs())
-    # the rounding of y32 is within half its ulp: at most one ulp of ref plus 2^-8 E32
-    return ref, bf16_ulp(ref) + (1 + U_BF16) * e32
+    return ref, e32
 
 
 def excess(got: Tensor, ref: Tensor, bound: Tensor) -> float:

@@ -3,12 +3,11 @@ pass and key-block, every test-hook instance), the per-head norms, the NaViT att
 against the fp32 oracle or the module's own fp32 graph."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import attention_bounds as AB
 from oracle import attention_fp32_bounds as FB
 from oracle import bounds as Bd
-from oracle import navit_oracle as NO
+from oracle import row_bounds as RB
 from vit_pytorch_b200 import NaViT, SimpleViT, ViT, _lib
 from vit_pytorch_b200.na_vit_nested_tensor import NaViT as NestedNaViT
 from vit_pytorch_b200.simple_vit_with_qk_norm import SimpleViT as QKNormViT
@@ -108,11 +107,6 @@ def _layernorm_heads(buf, gamma, nheads, dh, eps):
     assert rc == 0, _lib.lib().b200vit_last_error()
 
 
-def _ln_heads_ref(x, gamma, eps):
-    """x [T, H, dh], gamma [H, dh]: nn.LayerNorm(dh, bias=False) per head with a per-head gain."""
-    return F.layer_norm(x, x.shape[-1:], None, None, eps) * gamma
-
-
 @pytest.mark.parametrize("dh", [32, 80, 128])
 @pytest.mark.parametrize("H", [3, 5, 16])
 def test_head_norms_new_widths(dh, H):
@@ -122,27 +116,23 @@ def test_head_norms_new_widths(dh, H):
     T, I = 301, H * dh
     kv = torch.randn(T, 2 * I, device=DEV).bfloat16()
     g = torch.randn(H, dh, device=DEV)
-    want_rms = NO.rms_norm_heads(kv[:, :I].float().view(T, H, dh).permute(1, 0, 2).cpu(), g.cpu()[:, None, :])
-    want_ln = _ln_heads_ref(kv[:, :I].float().view(T, H, dh).cpu(), g.cpu(), 1e-5)
+    k = kv[:, :I].view(T, H, dh)
     buf = kv.clone()
     _lib.rmsnorm_heads(buf, g.reshape(-1).contiguous(), H, dh)
-    torch.cuda.synchronize()
-    assert torch.allclose(buf[:, :I].float().view(T, H, dh).permute(1, 0, 2).cpu(), want_rms, rtol=1e-2, atol=1e-2)
+    RB.check(buf[:, :I].view(T, H, dh), *RB.rmsnorm_heads_reference(k, g), "rmsnorm_heads")
     assert torch.equal(buf[:, I:], kv[:, I:])                             # v untouched
     buf = kv.clone()
     _layernorm_heads(buf, g.reshape(-1).contiguous(), H, dh, 1e-5)
-    torch.cuda.synchronize()
-    assert torch.allclose(buf[:, :I].float().view(T, H, dh).cpu(), want_ln, rtol=1e-2, atol=2e-2)
+    RB.check(buf[:, :I].view(T, H, dh), *RB.layernorm_heads_reference(k, g, 1e-5), "layernorm_heads")
     assert torch.equal(buf[:, I:], kv[:, I:])
     # q / k RMSNorm in place on qkv[T, 3 H dh]
     qkv = torch.randn(T, 3 * I, device=DEV).bfloat16()
     gqk = torch.randn(2, H, dh, device=DEV)
-    ref = qkv.float().cpu().view(T, 3, H, dh).clone()
+    got = qkv.clone()
+    _lib.qk_rmsnorm(got, gqk.reshape(-1).contiguous(), H, dh)
     for s in (0, 1):
-        ref[:, s] = NO.rms_norm_heads(ref[:, s].permute(1, 0, 2), gqk[s].cpu()[:, None, :]).permute(1, 0, 2)
-    _lib.qk_rmsnorm(qkv, gqk.reshape(-1).contiguous(), H, dh)
-    torch.cuda.synchronize()
-    assert torch.allclose(qkv.float().cpu().view(T, 3, H, dh), ref, rtol=1e-2, atol=1e-2)
+        RB.check(got.view(T, 3, H, dh)[:, s], *RB.rmsnorm_heads_reference(qkv.view(T, 3, H, dh)[:, s], gqk[s]), "qk")
+    assert torch.equal(got[:, 2 * I:], qkv[:, 2 * I:])
 
 
 @pytest.mark.parametrize("dh", [32, 80, 128])
@@ -162,13 +152,9 @@ def test_gemm_headnorm_new_widths(dh, headln):
     _lib.gemm_headnorm(a, w, out_bf16=got, head_gamma=g.reshape(-1).contiguous(), norm_heads=2 * H, dh=dh,
                        head_layernorm_eps=1e-5 if headln else None)
     torch.cuda.synchronize()
-    x = plain[:, :2 * I].float().cpu().view(M, 2 * H, dh)
-    if headln:
-        want = _ln_heads_ref(x, g.cpu(), 1e-5)
-    else:
-        want = NO.rms_norm_heads(x.permute(1, 0, 2), g.cpu()[:, None, :]).permute(1, 0, 2)
-    d = (got[:, :2 * I].float().cpu().view(M, 2 * H, dh) - want).abs()
-    assert (d <= 1e-2 + 1e-2 * want.abs()).float().mean() > 0.999, d.max()
+    x = plain[:, :2 * I].view(M, 2 * H, dh)
+    ref, bound = RB.layernorm_heads_reference(x, g, 1e-5) if headln else RB.rmsnorm_heads_reference(x, g)
+    RB.check(got[:, :2 * I].view(M, 2 * H, dh), ref, bound, "gemm_headnorm")
     assert torch.equal(got[:, 2 * I:], plain[:, 2 * I:])                  # v columns untouched
 
 

@@ -7,6 +7,7 @@ import torch
 
 from oracle import attention_bounds as AB
 from oracle import bounds as Bd
+from oracle import row_bounds as RB
 from oracle import vit_oracle as O
 from vit_pytorch_b200 import _lib
 
@@ -101,19 +102,6 @@ def test_gemm_lnfold_and_stats():
     assert torch.allclose(st[:, 1], (rb * rb).sum(1), rtol=1e-4, atol=1e-2)
 
 
-@pytest.mark.parametrize("M,D", [(1000, 768), (77, 50), (513, 1280)])
-def test_layernorm(M, D):
-    torch.manual_seed(3)
-    x = torch.randn(M, D, device=DEV) * 3 + 1
-    g, b = torch.randn(D, device=DEV), torch.randn(D, device=DEV)
-    of = torch.zeros(M, D, device=DEV)
-    ob = torch.zeros(M, D, device=DEV, dtype=torch.bfloat16)
-    _lib.layernorm(x, g, b, out_bf16=ob, out_f32=of)
-    ref = O.layer_norm(x.cpu(), g.cpu(), b.cpu())
-    assert torch.allclose(of.cpu(), ref, rtol=1e-5, atol=1e-5)
-    assert torch.equal(ob.cpu(), of.cpu().bfloat16())
-
-
 def test_layernorm_row_gather_no_bias():
     torch.manual_seed(4)
     x = torch.randn(197 * 4, 256, device=DEV)
@@ -164,43 +152,6 @@ def test_patch_embed_tma_matches_patchify_layernorm_linear(B, C, H, W, D):
     d = (y.cpu() - ref).abs()
     print(f"patch_embed_tma {B}x{C}x{H}x{W} -> {D}: max {d.max():.4f} mean {d.mean():.5f}")
     assert torch.isfinite(y).all() and d.max() < 3e-2 and d.mean() < 4e-3     # gamma (.) W is rounded to bf16
-
-
-@pytest.mark.parametrize("ncls", [0, 1])
-def test_embed_tokens(ncls):
-    torch.manual_seed(6)
-    B, n, D = 3, 49, 192
-    y = torch.randn(B * n, D, device=DEV)
-    g, be = torch.randn(D, device=DEV), torch.randn(D, device=DEV)
-    cls = torch.randn(ncls, D, device=DEV) if ncls else None
-    pos = torch.randn(n + ncls, D, device=DEV)
-    x = torch.zeros(B * (n + ncls), D, device=DEV)
-    xb = torch.zeros(B * (n + ncls), D, device=DEV, dtype=torch.bfloat16)
-    st = torch.zeros(B * (n + ncls), 1, 2, device=DEV)
-    _lib.embed_tokens(y, g, be, cls, pos, x, B, n, ncls, xb=xb, stats=st)
-    st = st[:, 0]
-    t = O.layer_norm(y.cpu(), g.cpu(), be.cpu()).view(B, n, D)
-    if ncls:
-        t = torch.cat([cls.cpu()[None].expand(B, -1, -1), t], 1)
-    assert torch.allclose(x.cpu(), (t + pos.cpu()[None]).reshape(-1, D), rtol=1e-5, atol=1e-5)
-    # bf16 copy and its row statistics (inputs of the first LN-folded GEMM)
-    assert torch.equal(xb, x.bfloat16())
-    xr = xb.float()
-    assert torch.allclose(st[:, 0], xr.sum(1), rtol=1e-5, atol=1e-3)
-    assert torch.allclose(st[:, 1], (xr * xr).sum(1), rtol=1e-5, atol=1e-3)
-
-
-def test_rowstats_cast():
-    torch.manual_seed(8)
-    x = torch.randn(333, 768, device=DEV) * 2 + 0.5
-    xb = torch.zeros(333, 768, device=DEV, dtype=torch.bfloat16)
-    st = torch.zeros(333, 1, 2, device=DEV)
-    _lib.rowstats_cast(x, xb, st)
-    st = st[:, 0]
-    assert torch.equal(xb, x.bfloat16())
-    xr = xb.float()
-    assert torch.allclose(st[:, 0], xr.sum(1), rtol=1e-5, atol=1e-3)
-    assert torch.allclose(st[:, 1], (xr * xr).sum(1), rtol=1e-5, atol=1e-3)
 
 
 @pytest.mark.parametrize("M,N,K", [(2048, 768, 768), (1300, 1024, 512),
@@ -398,15 +349,68 @@ def test_attention_large_logits_are_stable():
     Bd.check(out, *AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5), "large logits")
 
 
+def _same_bits(a, b):
+    """bit equality, NaN payloads included."""
+    return torch.equal(a.view(torch.int16 if a.dtype == torch.bfloat16 else torch.int32),
+                       b.view(torch.int16 if b.dtype == torch.bfloat16 else torch.int32))
+
+
+def test_rowstats_cast():
+    """The bf16 copy bit for bit, the (sum, sum of squares) within the depth-based bound of
+    oracle/row_bounds.py at D on the float4 path (768, 192) and the scalar path (50); rows past M untouched."""
+    for D in (768, 192, 50):
+        torch.manual_seed(D)
+        M = 333
+        x = torch.randn(M, D, device=DEV) * 2 + 0.5
+        xb = torch.full((M + 2, D), float("nan"), device=DEV, dtype=torch.bfloat16)
+        st = torch.full((M + 2, 2), float("nan"), device=DEV)
+        _lib.rowstats_cast(x, xb[:M], st[:M])
+        assert _same_bits(xb[:M], x.bfloat16())
+        r = RB.check(st[:M], *RB.row_stats_reference(xb[:M]), f"rowstats_cast D={D}")
+        print(f"excess rowstats_cast D={D}: {r:.3f}")
+        assert torch.isnan(xb[M:].float()).all() and torch.isnan(st[M:]).all()
+        xb2, st2 = torch.empty_like(xb[:M]), torch.empty_like(st[:M])
+        _lib.rowstats_cast(x, xb2, st2)
+        assert _same_bits(xb2, xb[:M]) and _same_bits(st2, st[:M])
+
+
 def test_mean_pool_and_cast():
-    torch.manual_seed(10)
-    x = torch.randn(8, 197, 768, device=DEV)
-    o = torch.zeros(8, 768, device=DEV)
-    _lib.mean_pool(x, o, 8, 197, 768)
-    assert torch.allclose(o.cpu(), x.cpu().mean(1), rtol=1e-5, atol=1e-6)
-    xb = torch.zeros(x.numel(), device=DEV, dtype=torch.bfloat16)
-    _lib.cast_f32_bf16(x.view(-1), xb)
-    assert torch.equal(xb.cpu(), x.view(-1).cpu().bfloat16())
+    """mean_pool within the bound of oracle/row_bounds.py (n_pool < N as with register tokens, n_pool = 1, D not a
+    multiple of 256): repeat calls give the same bits, a NaN stays in its image, rows past n_pool are not read.
+    cast_f32_bf16 equals torch's round-to-nearest-even bit for bit at n % 8 = 0 .. 7, n < 8, +-0, subnormals,
+    +-Inf and NaN, and writes nothing past n."""
+    nan = float("nan")
+    for B, N, D, n_pool in [(8, 197, 768, 197), (5, 21, 200, 17), (3, 9, 100, 1), (4, 65, 300, 64)]:
+        torch.manual_seed(N + D)
+        x = torch.randn(B, N, D, device=DEV) + 0.3
+        o = torch.full((B + 1, D), nan, device=DEV)
+        _lib.mean_pool(x, o[:B], B, N, D, n_pool)
+        r = RB.check(o[:B], *RB.mean_pool_reference(x, n_pool), f"mean_pool {B}x{N}x{D} n_pool={n_pool}")
+        print(f"excess mean_pool {B}x{N}x{D} n_pool={n_pool}: {r:.3f}")
+        assert torch.isnan(o[B:]).all()
+        o2 = torch.full((B + 1, D), nan, device=DEV)
+        _lib.mean_pool(x, o2[:B], B, N, D, n_pool)
+        assert _same_bits(o2, o)
+        xn = x.clone()
+        xn[1, n_pool - 1, 3] = nan
+        if n_pool < N:
+            xn[2, n_pool:] = nan                                     # rows past n_pool (register tokens)
+        on = torch.full((B + 1, D), nan, device=DEV)
+        _lib.mean_pool(xn, on[:B], B, N, D, n_pool)
+        others = [0] + list(range(2, B))
+        assert torch.isnan(on[1, 3]) and _same_bits(on[others], o[others])
+    special = torch.tensor([0.0, -0.0, 1e-40, -1e-40, 1.17e-38, float("inf"), float("-inf"), nan,
+                            1.0 + 2.0 ** -8, 1.0 + 3 * 2.0 ** -8, 3.4e38], device=DEV)
+    for n in [1, 3, 7, 8, 9, 15, 16, 17, 1000, 1001, 1002, 1003, 1004, 1005, 1006, 1007, 4096 + 5, 8 * 197 * 768]:
+        g = torch.Generator(device=DEV).manual_seed(n)
+        x = torch.randn(n, generator=g, device=DEV) * 100
+        x[:min(n, special.numel())] = special[:min(n, special.numel())]
+        out = torch.full((n + 8,), nan, device=DEV, dtype=torch.bfloat16)
+        _lib.cast_f32_bf16(x, out[:n])
+        want = x.bfloat16()
+        ok = ~torch.isnan(want)
+        assert torch.equal(out[:n].view(torch.int16)[ok], want.view(torch.int16)[ok]), n
+        assert torch.equal(torch.isnan(out[:n]), torch.isnan(want)) and torch.isnan(out[n:].float()).all(), n
 
 
 def test_kernels_were_launched_by_the_library():

@@ -479,19 +479,23 @@ __device__ __forceinline__ void ln_row_stats(const float* __restrict__ xr, int D
   rstd = rsqrtf(warp_sum(q) / (float)D + eps);
 }
 
-// One warp: fp32 row xr[D] -> its bf16 copy br[D] and, written by lane 0, st[0] = sum and st[1] = sum of squares of
-// the bf16-ROUNDED values: the row statistics the LN-folded GEMMs read (b200vit_rowstats_cast).  Every kernel that
-// hands such statistics to a folded GEMM goes through this function, so they are the same bits whoever writes them.
-__device__ __forceinline__ void rowstats_cast_row(const float* __restrict__ xr, __nv_bfloat16* __restrict__ br,
-                                                  float* __restrict__ st, int D, int lane) {
+// One warp writes the D values of a row -- fp32 to xr (F32) and their bf16 copy to br (when given) -- and, written by
+// lane 0 when st is given, st[0] = sum and st[1] = sum of squares of the bf16-ROUNDED values: the row statistics the
+// LN-folded GEMMs read.  D % 4 == 0: lane l produces v4(i) = values i .. i + 3 for i = 4 l, 4 l + 128, ...; otherwise
+// v1(i) for i = l, l + 32, ...  The sums run in that order, then a 5-level butterfly.  Every kernel that hands such
+// statistics to a folded GEMM writes its rows through this function, so they are the same bits whoever writes them.
+template <bool F32, class V4, class V1>
+__device__ __forceinline__ void emit_row_stats(int D, int lane, float* __restrict__ xr, __nv_bfloat16* __restrict__ br,
+                                               float* __restrict__ st, V4 v4, V1 v1) {
   float s1 = 0.f, s2 = 0.f;
   if ((D & 3) == 0) {
     for (int i = lane * 4; i < D; i += 128) {
-      const float4 v = *reinterpret_cast<const float4*>(xr + i);
+      const float4 v = v4(i);
+      if (F32) *reinterpret_cast<float4*>(xr + i) = v;
       uint2 pk;
       pk.x = pack_bf16x2(v.x, v.y);
       pk.y = pack_bf16x2(v.z, v.w);
-      *reinterpret_cast<uint2*>(br + i) = pk;
+      if (br) *reinterpret_cast<uint2*>(br + i) = pk;
       const float a0 = __uint_as_float(pk.x << 16), a1 = __uint_as_float(pk.x & 0xFFFF0000u);
       const float a2 = __uint_as_float(pk.y << 16), a3 = __uint_as_float(pk.y & 0xFFFF0000u);
       s1 += (a0 + a1) + (a2 + a3);
@@ -499,13 +503,16 @@ __device__ __forceinline__ void rowstats_cast_row(const float* __restrict__ xr, 
     }
   } else {
     for (int i = lane; i < D; i += 32) {
-      const __nv_bfloat16 vb = __float2bfloat16_rn(xr[i]);
-      br[i] = vb;
+      const float v = v1(i);
+      if (F32) xr[i] = v;
+      const __nv_bfloat16 vb = __float2bfloat16_rn(v);
+      if (br) br[i] = vb;
       const float vr = __bfloat162float(vb);
       s1 += vr;
       s2 = fmaf(vr, vr, s2);
     }
   }
+  if (!st) return;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     s1 += __shfl_xor_sync(0xffffffffu, s1, o);
@@ -515,6 +522,14 @@ __device__ __forceinline__ void rowstats_cast_row(const float* __restrict__ xr, 
     st[0] = s1;
     st[1] = s2;
   }
+}
+
+// One warp: fp32 row xr[D] -> its bf16 copy br[D] and its row statistics st[2] (b200vit_rowstats_cast).
+__device__ __forceinline__ void rowstats_cast_row(const float* __restrict__ xr, __nv_bfloat16* __restrict__ br,
+                                                  float* __restrict__ st, int D, int lane) {
+  emit_row_stats<false>(
+      D, lane, nullptr, br, st, [&](int i) { return *reinterpret_cast<const float4*>(xr + i); },
+      [&](int i) { return xr[i]; });
 }
 
 }  // namespace b200

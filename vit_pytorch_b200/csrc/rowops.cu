@@ -1,6 +1,7 @@
 // HBM-bound row kernels around the GEMMs: LayerNorm, patchify + LayerNorm, token assembly, mean pool, cast.
 // One warp per row, float4 / 16-byte accesses, fp32 statistics (two-pass variance, eps inside the sqrt -- the
-// semantics of torch.nn.LayerNorm used at vit.py:19,39,69,101,103).
+// semantics of torch.nn.LayerNorm used at vit.py:19,39,69,101,103).  The token rows that leave embed_tokens,
+// embed_varlen and rowstats_cast with LN-fold statistics are all written through emit_row_stats (common.cuh).
 #include "common.cuh"
 #include "host_util.h"
 
@@ -355,69 +356,47 @@ embed_tokens_kernel(const float* __restrict__ y, const float* __restrict__ gamma
   const int tc = min(t, n + ncls - 1);
   const long long prow = (long long)(b % pos_period) * pos_stride + (cls_pos ? tc : max(tc - ncls, 0));
   const float* pr = POS ? pos + prow * D : nullptr;
-  float s1 = 0.f, s2 = 0.f;  // sum / sum of squares of the bf16-rounded row (LN-fold statistics for the first layer)
-  auto emit = [&](int i, float v) {
-    xr[i] = v;
-    const __nv_bfloat16 vb = __float2bfloat16_rn(v);
-    if (xbr) xbr[i] = vb;
-    const float vr = __bfloat162float(vb);
-    s1 += vr;
-    s2 = fmaf(vr, vr, s2);
-  };
+  // every row kind goes through emit_row_stats: the first layer's LN-fold statistics are the bits rowstats_cast
+  // would write for the same fp32 row
+  float* st = stats ? stats + 2 * row : nullptr;
+  auto ld4 = [](const float* p) { return *reinterpret_cast<const float4*>(p); };
+  auto add4 = [](float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); };
   if (t < ncls) {
-    for (int i = lane; i < D; i += 32)
-      emit(i, POS && cls_pos ? cls[(long long)t * D + i] + pr[i] : cls[(long long)t * D + i]);
+    const float* cr = cls + (long long)t * D;
+    if (POS && cls_pos)
+      emit_row_stats<true>(D, lane, xr, xbr, st, [&](int i) { return add4(ld4(cr + i), ld4(pr + i)); },
+                     [&](int i) { return cr[i] + pr[i]; });
+    else
+      emit_row_stats<true>(D, lane, xr, xbr, st, [&](int i) { return ld4(cr + i); }, [&](int i) { return cr[i]; });
   } else if (t >= ncls + n) {  // register tokens appended after the patches (simple_vit_with_register_tokens.py:124-126)
-    for (int i = lane; i < D; i += 32) emit(i, tail[(long long)(t - ncls - n) * D + i]);
+    const float* tr = tail + (long long)(t - ncls - n) * D;
+    emit_row_stats<true>(D, lane, xr, xbr, st, [&](int i) { return ld4(tr + i); }, [&](int i) { return tr[i]; });
   } else if (!LN) {
     const float* yr = y + ((long long)b * n + (t - ncls)) * D;
-    for (int i = lane; i < D; i += 32) emit(i, POS ? yr[i] + pr[i] : yr[i]);
+    if (POS)
+      emit_row_stats<true>(D, lane, xr, xbr, st, [&](int i) { return add4(ld4(yr + i), ld4(pr + i)); },
+                     [&](int i) { return yr[i] + pr[i]; });
+    else
+      emit_row_stats<true>(D, lane, xr, xbr, st, [&](int i) { return ld4(yr + i); }, [&](int i) { return yr[i]; });
   } else {
     const float* yr = y + ((long long)b * n + (t - ncls)) * D;
     float mean, rstd;
     ln_row_stats(yr, D, lane, mean, rstd, eps);
-    if ((D & 3) == 0) {
-      for (int i = lane * 4; i < D; i += 128) {
-        const float4 v = *reinterpret_cast<const float4*>(yr + i);
-        const float4 g = *reinterpret_cast<const float4*>(gamma + i);
-        const float4 be = *reinterpret_cast<const float4*>(beta + i);
-        float4 o;
-        if (POS) {
-          const float4 p = *reinterpret_cast<const float4*>(pr + i);
-          o.x = ((v.x - mean) * rstd * g.x + be.x) + p.x;
-          o.y = ((v.y - mean) * rstd * g.y + be.y) + p.y;
-          o.z = ((v.z - mean) * rstd * g.z + be.z) + p.z;
-          o.w = ((v.w - mean) * rstd * g.w + be.w) + p.w;
-        } else {
-          o.x = (v.x - mean) * rstd * g.x + be.x;
-          o.y = (v.y - mean) * rstd * g.y + be.y;
-          o.z = (v.z - mean) * rstd * g.z + be.z;
-          o.w = (v.w - mean) * rstd * g.w + be.w;
-        }
-        *reinterpret_cast<float4*>(xr + i) = o;
-        uint2 pk;
-        pk.x = pack_bf16x2(o.x, o.y);
-        pk.y = pack_bf16x2(o.z, o.w);
-        if (xbr) *reinterpret_cast<uint2*>(xbr + i) = pk;
-        const float a0 = __uint_as_float(pk.x << 16), a1 = __uint_as_float(pk.x & 0xFFFF0000u);
-        const float a2 = __uint_as_float(pk.y << 16), a3 = __uint_as_float(pk.y & 0xFFFF0000u);
-        s1 += (a0 + a1) + (a2 + a3);
-        s2 = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, fmaf(a3, a3, s2))));
-      }
-    } else {
-      for (int i = lane; i < D; i += 32) {
-        const float v = (yr[i] - mean) * rstd * gamma[i] + beta[i];
-        emit(i, POS ? v + pr[i] : v);
-      }
-    }
-  }
-  if (stats) {
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    if (lane == 0) {
-      stats[2 * row] = s1;
-      stats[2 * row + 1] = s2;
-    }
+    // ((LN . gamma + beta) + pos): the association of the reference's x + pos_embedding
+    auto ln1 = [&](int i) {
+      const float v = (yr[i] - mean) * rstd * gamma[i] + beta[i];
+      return POS ? v + pr[i] : v;
+    };
+    auto ln4 = [&](int i) {
+      const float4 v = ld4(yr + i), g = ld4(gamma + i), be = ld4(beta + i);
+      float4 o;
+      o.x = (v.x - mean) * rstd * g.x + be.x;
+      o.y = (v.y - mean) * rstd * g.y + be.y;
+      o.z = (v.z - mean) * rstd * g.z + be.z;
+      o.w = (v.w - mean) * rstd * g.w + be.w;
+      return POS ? add4(o, ld4(pr + i)) : o;
+    };
+    emit_row_stats<true>(D, lane, xr, xbr, st, ln4, ln1);
   }
 }
 
@@ -611,11 +590,13 @@ struct HeadLanes {
 
 // buf[T, ld] bf16: the `nheads` consecutive DH-wide heads starting at the row's column 0 are normalised in place.
 // One warp per token; LPH lanes per head (8 bf16 = 16 B each; dh 80 = 10 chunks leaves 6 of its 16 lanes idle, their
-// zeros join the sums), so HPS heads are normalised per step with a butterfly inside each LPH-lane group; the loads of
-// U steps are issued before the first reduction (a serial load -> shuffle -> store chain per step left the kernel
-// latency bound at a quarter of the HBM rate).
-// LN = true: LayerNorm over the head's DH values without bias, (v - mean) * rsqrt(var + eps) * gamma -- the q / k norm
-// of the nested-tensor NaViT (na_vit_nested_tensor.py:61-62,101-102) -- instead of the RMS norm.
+// zeros join the sums of the values), so HPS heads are normalised per step with a butterfly inside each LPH-lane
+// group; the loads of U steps are issued before the first reduction (a serial load -> shuffle -> store chain per step
+// left the kernel latency bound at a quarter of the HBM rate).  Each lane's part of a sum is a chain of 8 fp32 adds or
+// fmas, then log2(LPH) butterfly levels.
+// LN = true: LayerNorm over the head's DH values without bias, (v - mean) * rsqrt(var + eps) * gamma with a two-pass
+// variance (the idle lanes of dh 80 masked out of the second pass) -- the q / k norm of the nested-tensor NaViT
+// (na_vit_nested_tensor.py:61-62,101-102) -- instead of the RMS norm.
 template <int DH, int U, bool LN>
 __global__ void __launch_bounds__(256)
 rmsnorm_heads_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float* __restrict__ gamma, int T,
@@ -641,26 +622,39 @@ rmsnorm_heads_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float*
       const int hh = base + HPS * u + grp;
       __nv_bfloat162* h2 = reinterpret_cast<__nv_bfloat162*>(&raw[u]);
       float2 f[4];
-      float ss = 0.f, s1 = 0.f;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        f[i] = __bfloat1622float2(h2[i]);
-        ss = fmaf(f[i].x, f[i].x, fmaf(f[i].y, f[i].y, ss));
-        s1 += f[i].x + f[i].y;
-      }
-#pragma unroll
-      for (int o = LPH / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      float inv = HL::SQRT_DH / fmaxf(sqrtf(ss), 1e-12f);
+      for (int i = 0; i < 4; ++i) f[i] = __bfloat1622float2(h2[i]);
+      float inv;
       if (LN) {
+        // two-pass variance over the values held in registers: E[x^2] - mean^2 loses var to cancellation in fp32 once
+        // |mean| / std reaches the hundreds
+        float s1 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) s1 += f[i].x + f[i].y;
 #pragma unroll
         for (int o = LPH / 2; o > 0; o >>= 1) s1 += __shfl_xor_sync(0xffffffffu, s1, o);
         const float mean = s1 * (1.0f / (float)DH);
-        inv = rsqrtf(fmaxf(ss * (1.0f / (float)DH) - mean * mean, 0.f) + eps);
+        float q = 0.f;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           f[i].x -= mean;
           f[i].y -= mean;
+          q = fmaf(f[i].x, f[i].x, fmaf(f[i].y, f[i].y, q));
         }
+        if (!act) q = 0.f;  // dh 80: an idle lane's zeros would add (0 - mean)^2
+#pragma unroll
+        for (int o = LPH / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+        inv = rsqrtf(q * (1.0f / (float)DH) + eps);
+      } else {
+        float ss = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ss = fmaf(f[i].x, f[i].x, fmaf(f[i].y, f[i].y, ss));
+#pragma unroll
+        for (int o = LPH / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        // max(||v||, 1e-12) as torch's clamp_min: a NaN norm stays NaN (fmaxf would return 1e-12 and turn the head's
+        // other values into finite garbage)
+        const float nrm = sqrtf(ss);
+        inv = HL::SQRT_DH / (nrm < 1e-12f ? 1e-12f : nrm);
       }
       if (hh < nheads && act) {
         const float4 g0 = *reinterpret_cast<const float4*>(gamma + hh * DH + 8 * sub);
@@ -849,35 +843,19 @@ embed_varlen_kernel(const float* __restrict__ y, const float* __restrict__ gamma
   __nv_bfloat16* xbr = xb ? xb + row * D : nullptr;
   float mean, rstd;
   ln_row_stats(yr, D, lane, mean, rstd, eps);
-  float s1 = 0.f, s2 = 0.f;
-  for (int i = lane * 4; i < D; i += 128) {  // D % 4 == 0 (checked by the launcher)
-    const float4 v = *reinterpret_cast<const float4*>(yr + i);
-    const float4 g = *reinterpret_cast<const float4*>(gamma + i);
-    const float4 a = *reinterpret_cast<const float4*>(ph + i);
-    const float4 b = *reinterpret_cast<const float4*>(pw + i);
-    float4 o;  // same association as the reference: (LN + pos_h) + pos_w
-    o.x = ((v.x - mean) * rstd * g.x + a.x) + b.x;
-    o.y = ((v.y - mean) * rstd * g.y + a.y) + b.y;
-    o.z = ((v.z - mean) * rstd * g.z + a.z) + b.z;
-    o.w = ((v.w - mean) * rstd * g.w + a.w) + b.w;
-    *reinterpret_cast<float4*>(xr + i) = o;
-    uint2 pk;
-    pk.x = pack_bf16x2(o.x, o.y);
-    pk.y = pack_bf16x2(o.z, o.w);
-    if (xbr) *reinterpret_cast<uint2*>(xbr + i) = pk;
-    const float a0 = __uint_as_float(pk.x << 16), a1 = __uint_as_float(pk.x & 0xFFFF0000u);
-    const float a2 = __uint_as_float(pk.y << 16), a3 = __uint_as_float(pk.y & 0xFFFF0000u);
-    s1 += (a0 + a1) + (a2 + a3);
-    s2 = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, fmaf(a3, a3, s2))));
-  }
-  if (stats) {
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    if (lane == 0) {
-      stats[2 * row] = s1;
-      stats[2 * row + 1] = s2;
-    }
-  }
+  // same association as the reference: (LN + pos_h) + pos_w.  D % 4 == 0 (checked by the launcher): only the float4
+  // form runs.
+  emit_row_stats<true>(
+      D, lane, xr, xbr, stats ? stats + 2 * row : nullptr,
+      [&](int i) {
+        const float4 v = *reinterpret_cast<const float4*>(yr + i);
+        const float4 g = *reinterpret_cast<const float4*>(gamma + i);
+        const float4 a = *reinterpret_cast<const float4*>(ph + i);
+        const float4 b = *reinterpret_cast<const float4*>(pw + i);
+        return make_float4(((v.x - mean) * rstd * g.x + a.x) + b.x, ((v.y - mean) * rstd * g.y + a.y) + b.y,
+                           ((v.z - mean) * rstd * g.z + a.z) + b.z, ((v.w - mean) * rstd * g.w + a.w) + b.w);
+      },
+      [&](int i) { return ((yr[i] - mean) * rstd * gamma[i] + ph[i]) + pw[i]; });
 }
 
 }  // namespace b200
