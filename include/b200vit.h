@@ -58,6 +58,13 @@ extern "C" {
 #define B200VIT_SEQ_POOL_MAX_DIM 1024  /* embedding width D of b200vit_seq_pool */
 #define B200VIT_ATTN_KV_MAX_KEYS 16384  /* keys per image of b200vit_attention_kv */
 
+/* what b200vit_cross_embed_nchw (CrossFormer's stage-1 cross-scale embedding) is built for */
+#define B200VIT_CROSS_EMBED_MAX_SCALES 4     /* convolutions (scales) per call */
+#define B200VIT_CROSS_EMBED_MAX_KERNEL 32    /* kernel size k of a scale */
+#define B200VIT_CROSS_EMBED_MAX_CHANNELS 4   /* image channels C */
+#define B200VIT_CROSS_EMBED_MAX_STRIDE 8     /* the shared stride s */
+#define B200VIT_CROSS_EMBED_MAX_WIDTH 64     /* output channels n of a scale (a multiple of 8) */
+
 const char* b200vit_last_error(void);
 int b200vit_version(void);
 /* number of kernels this library has launched in the calling process (all threads) since load / last reset */
@@ -569,6 +576,27 @@ int b200vit_peg(const float* x, int64_t M, const float* w, const float* bias, fl
 int b200vit_conv_proj_dw(const void* x, int64_t M, const float* wq, const float* bq, const float* wkv,
                          const float* bkv, void* q_out, void* kv_out, int B, int h, int w, int C, int k, int s,
                          void* stream);
+
+/*
+ * CrossFormer's cross-scale embedding of the image (CrossEmbedLayer, crossformer.py:14-36) in one launch: S
+ * convolutions of img [B, C, H, W] bf16 (NCHW, contiguous) with kernel sizes ks[0..S) and the one stride s, padding
+ * p_i = (ks[i] - s) / 2, their outputs concatenated along the channels and written channels-last as fp32:
+ *   out[(b*oh + r)*ow + q, off_i + n] = bias[off_i + n]
+ *       + sum_{c, y, x < ks[i]} W_i[n, c, y, x] * img[b, c, r*s - p_i + y, q*s - p_i + x]
+ * off_i = ns[0] + ... + ns[i-1], n < ns[i]; taps outside the image read zero.  Every scale must give the same oh x ow
+ * map (the reference's torch.cat raises otherwise).  `w` holds the scales one after another, scale i as bf16
+ * [ns[i], Kp_i] row-major with Kp_i = C*ks[i]^2 rounded up to a multiple of 64, columns (c, y, x) as in
+ * Conv2d.weight.reshape(ns[i], -1), zeros past C*ks[i]^2; `bias` fp32 [sum ns] in output column order.  ks and ns are
+ * host arrays.  An implicit GEMM on wgmma with fp32 accumulation: each CTA stages the input band of its output tokens
+ * once in shared memory and gathers every scale's A k-blocks from it, so no im2col matrix is written.  Sums run in a
+ * fixed order with no atomics, so repeated calls give the same bits.
+ * 1 <= S <= B200VIT_CROSS_EMBED_MAX_SCALES, 1 <= C <= B200VIT_CROSS_EMBED_MAX_CHANNELS,
+ * 1 <= s <= B200VIT_CROSS_EMBED_MAX_STRIDE, s <= ks[i] <= B200VIT_CROSS_EMBED_MAX_KERNEL, ns[i] a multiple of 8 up to
+ * B200VIT_CROSS_EMBED_MAX_WIDTH; ldo even and >= sum ns; w 16-byte, out and bias 8-byte aligned.  Each image's outputs
+ * come from its own pixels only; nothing outside the B*oh*ow addressed rows and their columns [0, sum ns) is written.
+ */
+int b200vit_cross_embed_nchw(const void* img, const void* w, const float* bias, float* out, int64_t ldo, int B, int C,
+                             int H, int W, int S, const int* ks, const int* ns, int s, void* stream);
 
 /*
  * ReLU then MaxPool2d(pk, stride ps, padding pp) in one pass (CCT's tokenizer, cct.py:187-190): y[M, C] bf16

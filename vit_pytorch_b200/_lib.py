@@ -46,7 +46,7 @@ SYMBOLS = [
     "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
     "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
     "b200vit_attention_posbias", "b200vit_attention_window_relpos", "b200vit_mbconv_dwconv", "b200vit_se_pool",
-    "b200vit_se_scale", "b200vit_conv_proj_dw",
+    "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw",
 ]
 
 
@@ -171,6 +171,9 @@ def lib() -> C.CDLL:
     L.b200vit_se_scale.argtypes = [vp, vp, i32, i32, i32, vp]
     L.b200vit_conv_proj_dw.restype = i32
     L.b200vit_conv_proj_dw.argtypes = [vp, i64, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_cross_embed_nchw.restype = i32
+    L.b200vit_cross_embed_nchw.argtypes = [vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, C.POINTER(i32),
+                                           C.POINTER(i32), i32, vp]
     L.b200vit_mean_pool.restype = i32
     L.b200vit_mean_pool.argtypes = [vp, vp, i32, i32, i32, i32, vp]
     L.b200vit_cast_f32_bf16.restype = i32
@@ -1059,6 +1062,48 @@ def conv_proj_dw(x: torch.Tensor, wq: torch.Tensor, bq: torch.Tensor, wkv: torch
         rc = lib().b200vit_conv_proj_dw(_ptr(x), M, _ptr(wq), _ptr(bq), _ptr(wkv), _ptr(bkv), _ptr(q_out),
                                         _ptr(kv_out), B, int(h), int(w), Cc, int(k), int(s), _stream())
     _check(rc, "b200vit_conv_proj_dw")
+
+
+CROSS_EMBED_MAX_SCALES, CROSS_EMBED_MAX_KERNEL, CROSS_EMBED_MAX_CHANNELS = 4, 32, 4   # include/b200vit.h
+CROSS_EMBED_MAX_STRIDE, CROSS_EMBED_MAX_WIDTH = 8, 64
+
+
+def cross_embed_pack(weights) -> torch.Tensor:
+    """The packed weight of b200vit_cross_embed_nchw from the scales' Conv2d weights [n_i, C, k_i, k_i]: bf16, scale
+    after scale [n_i, Kp_i] with Kp_i = C*k_i^2 rounded up to a multiple of 64, columns (c, y, x), zeros past
+    C*k_i^2."""
+    parts = []
+    for w in weights:
+        w = w.detach().reshape(w.shape[0], -1)
+        kp = (w.shape[1] + 63) // 64 * 64
+        wp = torch.zeros(w.shape[0], kp, device=w.device, dtype=torch.bfloat16)
+        wp[:, : w.shape[1]] = w
+        parts.append(wp.reshape(-1))
+    return torch.cat(parts)
+
+
+def cross_embed_nchw(img: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, out: torch.Tensor,
+                     kernel_sizes, widths, s: int) -> None:
+    """CrossFormer's cross-scale embedding: img [B, C, H, W] bf16 -> out fp32 [B*oh*ow, ldo = out.stride(0)], columns
+    [off_i, off_i + widths[i]) the Conv2d of kernel kernel_sizes[i], stride s, padding (k_i - s) // 2, plus its bias
+    (bias fp32 [sum widths], output column order); w_packed from cross_embed_pack."""
+    _chk(img, torch.bfloat16, "img"); _chk(w_packed, torch.bfloat16, "w"); _chk(bias, torch.float32, "bias")
+    _chk(out, torch.float32, "out")
+    assert img.is_contiguous() and img.dim() == 4 and out.dim() == 2 and out.stride(1) == 1
+    assert w_packed.is_contiguous() and bias.is_contiguous() and len(kernel_sizes) == len(widths)
+    B, Cc, H, W = img.shape
+    S, D = len(kernel_sizes), sum(widths)
+    p = (kernel_sizes[0] - s) // 2
+    oh, ow = conv_out_size(H, kernel_sizes[0], s, p), conv_out_size(W, kernel_sizes[0], s, p)
+    assert out.shape[0] == B * oh * ow and out.shape[1] >= D and bias.numel() == D
+    assert w_packed.numel() == sum(n * ((Cc * k * k + 63) // 64 * 64) for k, n in zip(kernel_sizes, widths))
+    ks = (C.c_int * S)(*[int(k) for k in kernel_sizes])
+    ns = (C.c_int * S)(*[int(n) for n in widths])
+    flops = 2.0 * B * oh * ow * sum(n * Cc * k * k for k, n in zip(kernel_sizes, widths))
+    with _Timed("cross_embed_nchw", B=B, C=Cc, H=H, W=W, ks=tuple(kernel_sizes), ns=tuple(widths), s=s, flops=flops):
+        rc = lib().b200vit_cross_embed_nchw(_ptr(img), _ptr(w_packed), _ptr(bias), _ptr(out), out.stride(0), B, Cc, H,
+                                            W, S, ks, ns, int(s), _stream())
+    _check(rc, "b200vit_cross_embed_nchw")
 
 
 def relu_maxpool(y: torch.Tensor, B: int, H: int, W: int, pk: int, ps: int, pp: int, *,
