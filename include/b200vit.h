@@ -313,6 +313,35 @@ int b200vit_attention_window_relpos(const void* qkv, void* out, const float* tab
  */
 int b200vit_mbconv_dwconv(const void* x, int64_t M, const float* w9, const float* bias, void* y, float* part, int B,
                           int h, int w, int C, int stride, void* stream);
+/* ... with the activation `act` = B200VIT_EPI_GELU or B200VIT_EPI_SILU (y / (1 + exp(-y)), MobileViT's MV2Block,
+ * mobile_vit.py:108-127, as the GEMM's EPI_SILU computes it), and `part` optional: NULL skips the channel sums
+ * (MobileViT has no squeeze-excitation).  b200vit_mbconv_dwconv is this call with B200VIT_EPI_GELU and `part`
+ * required; both give the same bits. */
+int b200vit_mbconv_dwconv_ex(const void* x, int64_t M, const float* w9, const float* bias, void* y, float* part, int B,
+                             int h, int w, int C, int stride, int act, void* stream);
+
+/* tokens per group b200vit_attention_groups takes, (gh/ph)*(gw/pw) */
+#define B200VIT_ATTN_GROUPS_MAX_TOKENS 4096
+
+/*
+ * MobileViT attention over strided patch groups (mobile_vit.py:64-72, 150-152):  B channels-last token maps of
+ * gh x gw tokens, token (b, y, x) at row (b*gh + y)*gw + x of qkv[B*gh*gw, 3*H*dh] (packed q | k | v, head-major, as
+ * for b200vit_attention) and of out[B*gh*gw, H*dh].  Group (b, i, j), i < ph, j < pw, is the set of tokens
+ * (y'*ph + i, x'*pw + j); each head attends only within its group and each result goes back to the token's own row:
+ *   out = softmax(scale * q k^T) v  over the group's (gh/ph)*(gw/pw) tokens.
+ * Rows are gathered by this address map; no token is copied into group order.  ph = pw = 1 with gw = 1 gives B
+ * contiguous sequences of gh tokens.
+ * Numerics as b200vit_attention: scores q.k * scale in fp32, an fp32 online softmax over 64-key blocks with exp2 and
+ * scale*log2(e) folded in, probabilities rounded to bf16 before P V, fp32 accumulation, one bf16 rounding of the
+ * output.  mma.sync m16n8k8 for Q K^T and for P V (8 keys per MMA); one CTA stages one head's K and V of one or more groups in
+ * shared memory once.
+ * dh = 8 only; any H >= 1 (<= 65535); gh % ph == gw % pw == 0; 1 <= group length <= B200VIT_ATTN_GROUPS_MAX_TOKENS;
+ * qkv and out 16-byte aligned.
+ * Isolation: a group's output is computed from its own rows only; a NaN or Inf stays within its group; nothing outside
+ * the B*gh*gw rows is read or written; repeated calls give the same bits.
+ */
+int b200vit_attention_groups(const void* qkv, void* out, int B, int gh, int gw, int ph, int pw, int H, int dh,
+                             float scale, void* stream);
 
 /*
  * Squeeze-excitation around two bias-free GEMMs (max_vit.py:47-62):
@@ -533,6 +562,11 @@ int b200vit_conv_im2col_nchw(const void* img, void* out_bf16, int64_t ldo, int B
                              int p, void* stream);
 int b200vit_conv_im2col_nhwc(const void* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W, int C, int k,
                              int s, int p, void* stream);
+/* ... with x's rows ldx elements apart (ldx a multiple of 8, >= C): the channels-last map may be a column slice of a
+ * wider buffer (MobileViT's concatenation, mobile_vit.py:155-157).  b200vit_conv_im2col_nhwc is this call with
+ * ldx = C. */
+int b200vit_conv_im2col_nhwc_ex(const void* x, int64_t ldx, int64_t M, void* out_bf16, int64_t ldo, int B, int H,
+                                int W, int C, int k, int s, int p, void* stream);
 
 /*
  * Patch merging + LayerNorm between the stages of a hierarchical model (Twins-SVT's PatchEmbedding up to its 1 x 1

@@ -29,6 +29,7 @@ ATTN_MASK_SELF = 1
 ATTN_GELU_OUT = 4
 ATTN_POSBIAS_MAX_KEYS = 4096    # B200VIT_ATTN_POSBIAS_MAX_KEYS
 MBCONV_PART_ROWS = 64           # B200VIT_MBCONV_PART_ROWS
+ATTN_GROUPS_MAX_TOKENS = 4096   # B200VIT_ATTN_GROUPS_MAX_TOKENS
 
 # every symbol include/b200vit.h declares (tests check that the library exports each of them)
 SYMBOLS = [
@@ -46,7 +47,8 @@ SYMBOLS = [
     "b200vit_conv_im2col_nchw", "b200vit_conv_im2col_nhwc", "b200vit_relu_maxpool", "b200vit_seq_pool",
     "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
     "b200vit_attention_posbias", "b200vit_attention_window_relpos", "b200vit_mbconv_dwconv", "b200vit_se_pool",
-    "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw",
+    "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw", "b200vit_mbconv_dwconv_ex",
+    "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex",
 ]
 
 
@@ -147,6 +149,8 @@ def lib() -> C.CDLL:
     L.b200vit_conv_im2col_nchw.argtypes = [vp, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]
     L.b200vit_conv_im2col_nhwc.restype = i32
     L.b200vit_conv_im2col_nhwc.argtypes = [vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_conv_im2col_nhwc_ex.restype = i32
+    L.b200vit_conv_im2col_nhwc_ex.argtypes = [vp, i64, i64, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]
     L.b200vit_relu_maxpool.restype = i32
     L.b200vit_relu_maxpool.argtypes = [vp, i64, i32, i32, i32, i32, i32, i32, i32, vp, vp, i64, vp]
     L.b200vit_seq_pool.restype = i32
@@ -165,6 +169,10 @@ def lib() -> C.CDLL:
     L.b200vit_attention_window_relpos.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_mbconv_dwconv.restype = i32
     L.b200vit_mbconv_dwconv.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    L.b200vit_mbconv_dwconv_ex.restype = i32
+    L.b200vit_mbconv_dwconv_ex.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_attention_groups.restype = i32
+    L.b200vit_attention_groups.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_se_pool.restype = i32
     L.b200vit_se_pool.argtypes = [vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_se_scale.restype = i32
@@ -330,6 +338,19 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, out_bf16: Optional[torch.Tensor] =
 
     ln_sums: [M, parts, 2] (or [M, 2]) partial row sums of `a`; stats_out: [M, stats_parts(N), 2], fully overwritten."""
     _gemm(a, w, out_bf16, out_f32, bias, resid, gelu, ln_sums, ln_eps, col_s, stats_out, n, k, 0)
+
+
+def gemm_act(a: torch.Tensor, w: torch.Tensor, *, act: str, out_bf16: Optional[torch.Tensor] = None,
+             out_f32: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None,
+             ln_sums: Optional[torch.Tensor] = None, ln_eps: float = 1e-5, col_s: Optional[torch.Tensor] = None,
+             stats_out: Optional[torch.Tensor] = None) -> None:
+    """gemm with the activation `act` after the bias / LayerNorm fold: "gelu" (EPI_GELU) or "silu" (EPI_SILU:
+    y / (1 + exp(-y)); MobileViT's convolutions and FeedForward), at any M, with the LN fold, fp32 / bf16 outputs and
+    row statistics as gemm takes them (no residual)."""
+    if act not in ("gelu", "silu"):
+        raise B200VitError(f"gemm_act: act={act!r} (gelu or silu)")
+    _gemm(a, w, out_bf16, out_f32, bias, None, act == "gelu", ln_sums, ln_eps, col_s, stats_out, None, None,
+          EPI_SILU if act == "silu" else 0)
 
 
 def gemm_hardswish(a: torch.Tensor, w: torch.Tensor, *, out_bf16: torch.Tensor, bias: Optional[torch.Tensor] = None
@@ -685,6 +706,42 @@ def mbconv_dwconv(x: torch.Tensor, w9: torch.Tensor, bias: torch.Tensor, y: torc
     _check(rc, "b200vit_mbconv_dwconv")
 
 
+def mbconv_dwconv_ex(x: torch.Tensor, w9: torch.Tensor, bias: torch.Tensor, y: torch.Tensor,
+                     part: Optional[torch.Tensor], B: int, h: int, w: int, stride: int, act: str = "gelu") -> None:
+    """mbconv_dwconv with the activation `act` ("gelu" or "silu": y / (1 + exp(-y)), as the GEMM's EPI_SILU) and
+    `part` optional (None: no channel sums; MobileViT's MV2Block, mobile_vit.py:108-127)."""
+    _chk(x, torch.bfloat16, "x"); _chk(y, torch.bfloat16, "y")
+    for nm, t in (("w9", w9), ("bias", bias), ("part", part)):
+        _chk(t, torch.float32, nm)
+    if act not in ("gelu", "silu"):
+        raise B200VitError(f"mbconv_dwconv_ex: act={act!r} (gelu or silu)")
+    M, Cc = x.shape
+    oh, ow = -(-h // stride), -(-w // stride)
+    assert x.is_contiguous() and y.is_contiguous() and w9.is_contiguous() and bias.is_contiguous()
+    assert y.shape == (B * oh * ow, Cc) and w9.shape == (9, Cc) and bias.numel() == Cc
+    assert part is None or (part.is_contiguous() and part.shape == (B, mbconv_parts(oh, ow), Cc))
+    with _Timed("mbconv_dwconv", B=B, h=h, w=w, C=Cc, s=stride, act=act, bytes=(M + y.shape[0]) * Cc * 2):
+        rc = lib().b200vit_mbconv_dwconv_ex(_ptr(x), M, _ptr(w9), _ptr(bias), _ptr(y), _ptr(part), B, int(h), int(w),
+                                            Cc, int(stride), EPI_GELU if act == "gelu" else EPI_SILU, _stream())
+    _check(rc, "b200vit_mbconv_dwconv_ex")
+
+
+def attention_groups(qkv: torch.Tensor, out: torch.Tensor, B: int, gh: int, gw: int, ph: int, pw: int, H: int,
+                     dh: int, scale: float) -> None:
+    """MobileViT attention inside the strided patch groups of B token maps of gh x gw tokens: qkv[B*gh*gw, 3*H*dh]
+    packed q | k | v, token (b, y, x) at row (b*gh + y)*gw + x; out[B*gh*gw, H*dh].  Group (b, i, j) is the tokens
+    (y'*ph + i, x'*pw + j) (mobile_vit.py:150); dh = 8."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out")
+    assert qkv.is_contiguous() and out.is_contiguous()
+    assert qkv.shape == (B * gh * gw, 3 * H * dh) and out.shape == (B * gh * gw, H * dh)
+    n = (gh // ph) * (gw // pw) if ph > 0 and pw > 0 else 0
+    with _Timed("attention_groups", B=B, h=gh, w=gw, ph=ph, pw=pw, H=H, n=n, bytes=(qkv.numel() + out.numel()) * 2,
+                exps=B * ph * pw * H * n * n, flops=4.0 * B * ph * pw * H * n * n * dh):
+        rc = lib().b200vit_attention_groups(_ptr(qkv), _ptr(out), B, int(gh), int(gw), int(ph), int(pw), H, dh,
+                                            float(scale), _stream())
+    _check(rc, "b200vit_attention_groups")
+
+
 def se_pool(part: torch.Tensor, pooled: torch.Tensor, n: int) -> None:
     """pooled bf16 [B, C] = the sum over the parts of part fp32 [B, P, C], in part order, divided by n."""
     _chk(part, torch.float32, "part"); _chk(pooled, torch.bfloat16, "pooled")
@@ -998,16 +1055,21 @@ def conv_im2col_nchw(img: torch.Tensor, out_bf16: torch.Tensor, k: int, s: int, 
 
 def conv_im2col_nhwc(x: torch.Tensor, out_bf16: torch.Tensor, B: int, H: int, W: int, k: int, s: int, p: int) -> None:
     """x [B*H*W, C] bf16 channels-last -> out [B*oh*ow, ldo] bf16, column (i*k + j)*C + c the channel c of tap (i, j)
-    of the zero-padded k x k window at stride s, zero K padding up to ldo = out.stride(0)."""
+    of the zero-padded k x k window at stride s, zero K padding up to ldo = out.stride(0).  x may be a column slice of
+    a wider buffer (rows x.stride(0) apart: b200vit_conv_im2col_nhwc_ex)."""
     _chk(x, torch.bfloat16, "x"); _chk(out_bf16, torch.bfloat16, "out")
-    assert x.is_contiguous() and x.dim() == 2 and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    assert x.dim() == 2 and x.stride(1) == 1 and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
     M, Cc = x.shape
     rows = B * conv_out_size(H, k, s, p) * conv_out_size(W, k, s, p)
     assert out_bf16.shape[0] == rows and out_bf16.shape[1] >= Cc * k * k, \
         f"out must be [{rows}, >= {Cc * k * k}], got {tuple(out_bf16.shape)}"
     with _Timed("conv_im2col", bytes=x.numel() * 2 + rows * out_bf16.stride(0) * 2):
-        rc = lib().b200vit_conv_im2col_nhwc(_ptr(x), M, _ptr(out_bf16), out_bf16.stride(0), B, H, W, Cc, int(k), int(s),
-                                            int(p), _stream())
+        if x.is_contiguous():
+            rc = lib().b200vit_conv_im2col_nhwc(_ptr(x), M, _ptr(out_bf16), out_bf16.stride(0), B, H, W, Cc, int(k),
+                                                int(s), int(p), _stream())
+        else:
+            rc = lib().b200vit_conv_im2col_nhwc_ex(_ptr(x), x.stride(0), M, _ptr(out_bf16), out_bf16.stride(0), B, H,
+                                                   W, Cc, int(k), int(s), int(p), _stream())
     _check(rc, "b200vit_conv_im2col_nhwc")
 
 

@@ -73,12 +73,12 @@ im2col_nchw_kernel(const __nv_bfloat16* __restrict__ img, __nv_bfloat16* __restr
     for (int q = 0; q < nq; ++q) out[(row0 + q) * ldo + K + t] = zero;
 }
 
-// x [B*H*W, C] bf16 channels-last (pixel (b, y, x) at row (b*H + y)*W + x), as CV = C / 8 16-byte vectors per row;
-// out row (b*oh + r)*ow + q, vector (i*k + j)*CV + v = x[(b, r*s - p + i, q*s - p + j), vector v], or zeros outside
+// x [B*H*W, C] bf16 channels-last (pixel (b, y, x) at row (b*H + y)*W + x), as CV = C / 8 16-byte vectors per row
+// and LX8 16-byte vectors from one row to the next (LX8 >= CV: the rows may be a column slice of a wider buffer); out row (b*oh + r)*ow + q, vector (i*k + j)*CV + v = x[(b, r*s - p + i, q*s - p + j), vector v], or zeros outside
 // the image; vectors [k*k*CV, ldo8) zero.  One warp per output row.
 __global__ void __launch_bounds__(256)
-im2col_nhwc_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, long long ldo8, int H, int W, int CV, int k,
-                   int s, int p, int oh, int ow, long long rows) {
+im2col_nhwc_kernel(const uint4* __restrict__ x, long long lx8, uint4* __restrict__ out, long long ldo8, int H, int W,
+                   int CV, int k, int s, int p, int oh, int ow, long long rows) {
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -87,14 +87,14 @@ im2col_nhwc_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, long lo
   const int r = (int)(t % oh);
   const long long b = t / oh;
   const int y0 = r * s - p, x0 = q * s - p, kv = k * k * CV;
-  const uint4* img = x + b * H * W * CV;
+  const uint4* img = x + b * H * W * lx8;
   uint4* dst = out + row * ldo8;
   for (int v = lane; v < ldo8; v += 32) {
     uint4 val = make_uint4(0u, 0u, 0u, 0u);
     if (v < kv) {
       const int tap = v / CV, cv = v - tap * CV, i = tap / k, j = tap - i * k;
       const int y = y0 + i, xx = x0 + j;
-      if (y >= 0 && y < H && xx >= 0 && xx < W) val = __ldg(img + ((long long)y * W + xx) * CV + cv);
+      if (y >= 0 && y < H && xx >= 0 && xx < W) val = __ldg(img + ((long long)y * W + xx) * lx8 + cv);
     }
     dst[v] = val;
   }
@@ -333,31 +333,38 @@ extern "C" int b200vit_conv_im2col_nchw(const void* img, void* out_bf16, int64_t
   return 0;
 }
 
-extern "C" int b200vit_conv_im2col_nhwc(const void* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W,
-                                        int C, int k, int s, int p, void* stream) {
+extern "C" int b200vit_conv_im2col_nhwc_ex(const void* x, int64_t ldx, int64_t M, void* out_bf16, int64_t ldo, int B,
+                                           int H, int W, int C, int k, int s, int p, void* stream) {
   B200_CHECK_ARG(x && out_bf16, "conv_im2col_nhwc: null pointer");
   B200_CHECK_ARG(B > 0 && C > 0 && H > 0 && W > 0 && k >= 1 && k <= B200VIT_CONV_MAX_KERNEL && s >= 1 && p >= 0 &&
                      p < k && H + 2 * p >= k && W + 2 * p >= k,
                  "conv_im2col_nhwc: bad shape B=%d H=%d W=%d C=%d k=%d s=%d p=%d (1 <= k <= %d, s >= 1, 0 <= p < k, "
                  "H + 2p and W + 2p >= k)", B, H, W, C, k, s, p, B200VIT_CONV_MAX_KERNEL);
   B200_CHECK_ARG(C % 8 == 0, "conv_im2col_nhwc: C=%d must be a multiple of 8", C);
+  B200_CHECK_ARG(ldx >= C && (ldx & 7) == 0, "conv_im2col_nhwc: ldx=%lld must be a multiple of 8 and >= C=%d",
+                 (long long)ldx, C);
   B200_CHECK_ARG(M == (long long)B * H * W, "conv_im2col_nhwc: x has %lld rows, B*H*W = %lld expected", (long long)M,
                  (long long)B * H * W);
   const int oh = (H + 2 * p - k) / s + 1, ow = (W + 2 * p - k) / s + 1;
   const long long K = (long long)C * k * k, rows = (long long)B * oh * ow;
   B200_CHECK_ARG(ldo >= K && (ldo & 7) == 0, "conv_im2col_nhwc: ldo=%lld must be a multiple of 8 and >= k*k*C=%lld",
                  (long long)ldo, K);
-  B200_CHECK_ARG(rows * ldo <= (1LL << 40) && M * C <= (1LL << 40), "conv_im2col_nhwc: %lld output pixels too many",
+  B200_CHECK_ARG(rows * ldo <= (1LL << 40) && M * ldx <= (1LL << 40), "conv_im2col_nhwc: %lld output pixels too many",
                  rows);
   B200_CHECK_ARG(al16(x) && al16(out_bf16), "conv_im2col_nhwc: x and out_bf16 must be 16-byte aligned");
   const long long grid = (rows + 7) / 8;
   B200_CHECK_ARG(grid <= 0x7fffffff, "conv_im2col_nhwc: %lld CTAs too many", grid);
   im2col_nhwc_kernel<<<(unsigned)grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out_bf16), (long long)ldo / 8, H, W, C / 8, k, s, p,
-      oh, ow, rows);
+      reinterpret_cast<const uint4*>(x), (long long)ldx / 8, reinterpret_cast<uint4*>(out_bf16), (long long)ldo / 8, H,
+      W, C / 8, k, s, p, oh, ow, rows);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
+}
+
+extern "C" int b200vit_conv_im2col_nhwc(const void* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W,
+                                        int C, int k, int s, int p, void* stream) {
+  return b200vit_conv_im2col_nhwc_ex(x, C, M, out_bf16, ldo, B, H, W, C, k, s, p, stream);
 }
 
 extern "C" int b200vit_relu_maxpool(const void* y, int64_t M, int B, int H, int W, int C, int pk, int ps, int pp,

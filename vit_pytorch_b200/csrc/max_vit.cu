@@ -3,6 +3,8 @@
 // window attention with its relative-position bias, b200vit_attention_window_relpos, is in attention_tile64.cu.
 //   b200vit_mbconv_dwconv             depthwise 3 x 3 convolution, BatchNorm folded, GELU, and the per-image channel
 //                                     sums squeeze-excitation averages (max_vit.py:106-109)
+//   b200vit_mbconv_dwconv_ex          the same with GELU or SiLU and the sums optional (MobileViT's MV2Block,
+//                                     mobile_vit.py:108-127)
 //   b200vit_se_pool / b200vit_se_scale  the squeeze-excitation mean and gate around its two GEMMs (max_vit.py:47-62)
 //
 // mbconv_dwconv: one thread = two adjacent channels of one image over a run of B200VIT_MBCONV_PART_ROWS output
@@ -18,6 +20,13 @@ using namespace b200;
 // ------------------------------------------------------------------------------------------------ mbconv_dwconv
 constexpr int DW_THREADS = 128;
 
+// y sigmoid(y), sigmoid(y) = 1 / (1 + 2^(-y log2 e)): the GEMM epilogue's EPI_SILU, so both give the same bits
+__device__ __forceinline__ float silu_fast(float y) {
+  return y * fast_rcp(1.0f + fast_ex2(-1.4426950408889634f * y));
+}
+
+// ACT: B200VIT_EPI_GELU or B200VIT_EPI_SILU; part NULL: no channel sums
+template <int ACT>
 __global__ void __launch_bounds__(DW_THREADS)
 mbconv_dwconv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w9, const float* __restrict__ bias,
                      __nv_bfloat16* __restrict__ y, float* __restrict__ part, int h, int w, int oh, int ow, int C,
@@ -51,13 +60,18 @@ mbconv_dwconv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restric
         a1 = fmaf(wt[3 * ky + kx].y, v.y, a1);
       }
     }
-    gelu_erf2(a0, a1);
+    if (ACT == B200VIT_EPI_GELU) {
+      gelu_erf2(a0, a1);
+    } else {
+      a0 = silu_fast(a0);
+      a1 = silu_fast(a1);
+    }
     const uint32_t pk = pack_bf16x2(a0, a1);
     *reinterpret_cast<uint32_t*>(yb + (long long)t * C) = pk;
     sum0 += __uint_as_float(pk << 16);
     sum1 += __uint_as_float(pk & 0xFFFF0000u);
   }
-  *reinterpret_cast<float2*>(part + ((long long)b * P + pi) * C + c) = make_float2(sum0, sum1);
+  if (part) *reinterpret_cast<float2*>(part + ((long long)b * P + pi) * C + c) = make_float2(sum0, sum1);
 }
 
 // ------------------------------------------------------------------------------------------------ se_pool / se_scale
@@ -99,9 +113,11 @@ se_scale_kernel(__nv_bfloat16* __restrict__ hbuf, const __nv_bfloat16* __restric
 
 static inline bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
-extern "C" int b200vit_mbconv_dwconv(const void* x, int64_t M, const float* w9, const float* bias, void* y, float* part,
-                                     int B, int h, int w, int C, int stride, void* stream) {
-  B200_CHECK_ARG(x && w9 && bias && y && part, "mbconv_dwconv: null pointer");
+extern "C" int b200vit_mbconv_dwconv_ex(const void* x, int64_t M, const float* w9, const float* bias, void* y,
+                                        float* part, int B, int h, int w, int C, int stride, int act, void* stream) {
+  B200_CHECK_ARG(x && w9 && bias && y, "mbconv_dwconv: null pointer");
+  B200_CHECK_ARG(act == B200VIT_EPI_GELU || act == B200VIT_EPI_SILU,
+                 "mbconv_dwconv: act=%d (B200VIT_EPI_GELU or B200VIT_EPI_SILU)", act);
   B200_CHECK_ARG(B > 0 && h > 0 && w > 0 && C > 0, "mbconv_dwconv: bad shape B=%d h=%d w=%d C=%d", B, h, w, C);
   B200_CHECK_ARG(stride == 1 || stride == 2, "mbconv_dwconv: stride=%d (1 or 2)", stride);
   B200_CHECK_ARG(M == (int64_t)B * h * w, "mbconv_dwconv: x has %lld rows, %lld expected", (long long)M,
@@ -114,12 +130,19 @@ extern "C" int b200vit_mbconv_dwconv(const void* x, int64_t M, const float* w9, 
   const long long P = ((long long)oh * ow + B200VIT_MBCONV_PART_ROWS - 1) / B200VIT_MBCONV_PART_ROWS;
   B200_CHECK_ARG(B <= 65535 && P <= 65535, "mbconv_dwconv: B=%d, %lld parts exceed the grid", B, P);
   const dim3 grid((C / 2 + DW_THREADS - 1) / DW_THREADS, (unsigned)P, B);
-  mbconv_dwconv_kernel<<<grid, DW_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  auto kern = act == B200VIT_EPI_GELU ? mbconv_dwconv_kernel<B200VIT_EPI_GELU> : mbconv_dwconv_kernel<B200VIT_EPI_SILU>;
+  kern<<<grid, DW_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), w9, bias, reinterpret_cast<__nv_bfloat16*>(y), part, h, w, oh, ow, C,
       stride, (int)P);
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
+}
+
+extern "C" int b200vit_mbconv_dwconv(const void* x, int64_t M, const float* w9, const float* bias, void* y, float* part,
+                                     int B, int h, int w, int C, int stride, void* stream) {
+  B200_CHECK_ARG(part, "mbconv_dwconv: null pointer");
+  return b200vit_mbconv_dwconv_ex(x, M, w9, bias, y, part, B, h, w, C, stride, B200VIT_EPI_GELU, stream);
 }
 
 extern "C" int b200vit_se_pool(const float* part, void* pooled, int B, int P, int C, float inv_n, void* stream) {

@@ -135,6 +135,8 @@ LPI_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_local_patch_interaction
 WINDOW_MAX_TOKENS = 64                     # b200vit_attention_window: tokens of one window
 PEG_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_peg
 CONV_PROJ_KERNEL_SIZES = (1, 3, 5, 7)      # b200vit_conv_proj_dw
+GROUPS_WIDTHS = (8,)                       # b200vit_attention_groups
+GROUPS_MAX_TOKENS = _lib.ATTN_GROUPS_MAX_TOKENS    # b200vit_attention_groups: tokens of one group
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -171,6 +173,14 @@ def lpi_reason(kernel_size: int, grid_w: int) -> Optional[str]:
         return f"local_patch_kernel_size={kernel_size} (the local patch interaction kernel is built for 1, 3, 5 and 7)"
     if (3 * kernel_size - 1) * (grid_w + 2 * (kernel_size // 2)) * 4 * 4 > 100 * 1024:
         return f"a grid row of {grid_w} tokens is too wide for the local patch interaction kernel"
+    return None
+
+
+def groups_reason(dh: int) -> Optional[str]:
+    """None if b200vit_attention_groups is built for heads `dh` wide, else the reason the eager PyTorch graph is
+    used."""
+    if dh not in GROUPS_WIDTHS:
+        return f"dim_head={dh} (the patch-group attention kernel is built for 8)"
     return None
 
 
@@ -331,14 +341,24 @@ class EncoderLayer:
     # 86-87; b200vit_conv_proj_dw, then b200vit_attention_kv): qkv_w holds the queries' 1 x 1 rows [I, D] and kv_w the
     # keys' and values' [2I, D], rows k | v; run_blocks needs `grid`
     conv_proj: Optional[ConvProj] = None
+    # the feed-forward block's activation: "gelu" (vit.py:21) or "silu" (MobileViT's FeedForward, mobile_vit.py:28-34)
+    ff_act: str = "gelu"
+    # attention inside the strided patch groups of the token grid, token (y'*ph + i, x'*pw + j) in group (i, j)
+    # (MobileViT, mobile_vit.py:150; b200vit_attention_groups); run_blocks needs `grid` and `groups` = (ph, pw)
+    patch_groups: bool = False
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
     """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'window_relpos' (windows with a
-    relative-position bias), 'kv' (sub-sampled keys: a strided convolution or CvT's convolutional projections), 'axial'
-    (a run_blocks call with `axial`, unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a
-    packed batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed or sub-sampled-key
-    attention with `axial` or over a `packed` batch."""
+    relative-position bias), 'kv' (sub-sampled keys: a strided convolution or CvT's convolutional projections),
+    'groups' (strided patch groups), 'axial' (a run_blocks call with `axial`, unless the layer's temporal sub-block runs
+    there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys) or 'plain'.  ValueError for
+    cross-covariance, head-mixing, windowed, patch-group or sub-sampled-key attention with `axial` or over a `packed`
+    batch."""
+    if L.patch_groups:
+        if axial or packed:
+            raise ValueError("patch-group attention runs over B token grids only")
+        return "groups"
     if L.window is not None or L.kv_stride is not None or L.conv_proj is not None:
         if axial or packed:
             raise ValueError("windowed and sub-sampled-key attention run over B token grids only")
@@ -499,7 +519,8 @@ class TransformerEngine:
         for L in self.layers or self.mod.encoder_layers()[0]:
             kernel = attention_kernel(L)
             r = (xca_reason(L.dim_head) if kernel == "xca" else
-                 headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else head_width_reason(L.dim_head))
+                 headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else
+                 groups_reason(L.dim_head) if kernel == "groups" else head_width_reason(L.dim_head))
             if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
                 r = lpi_reason(L.lpi.kernel_size, 1)
             if r is None and kernel == "window_relpos" and L.window ** 2 > WINDOW_MAX_TOKENS:
@@ -589,7 +610,7 @@ class TransformerEngine:
         long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
         if any(L.qk_norm == "ln" or L.temporal is not None or attention_kernel(L) != "plain" or L.lpi is not None
-               or L.post_norm or sig(L) != sig(self.layers[0]) for L in self.layers):
+               or L.post_norm or L.ff_act != "gelu" or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -663,7 +684,8 @@ class TransformerEngine:
                    varlen: Optional[_lib.VarlenIndex] = None,
                    rope: Optional[Tuple[torch.Tensor, int]] = None,
                    axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
-                   layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None) -> None:
+                   layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None,
+                   groups: Optional[Tuple[int, int]] = None) -> None:
         """The encoder layers (all, or the indices in `layers`, in order: CaiT's layer dropout, cait.py:14-27), in place
         on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
         B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
@@ -680,7 +702,9 @@ class TransformerEngine:
         statistics): in both LayerNorm modes it runs layernorm(x -> xb), the query GEMM on xb, conv_im2col_nhwc of xb
         and the key / value GEMM (kernel size 1: the GEMM on xb itself), then attention_kv.  A layer with convolutional
         projections (CvT) runs layernorm(x -> xb), conv_proj_dw of xb into the query and key / value operands, their
-        1 x 1 GEMMs, then attention_kv; the projections pad, so any h, w >= 1 will do.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
+        1 x 1 GEMMs, then attention_kv; the projections pad, so any h, w >= 1 will do.  Layers with patch-group attention
+        (MobileViT) need `groups` = (ph, pw) dividing `grid` as well (attention_groups).  A layer's feed-forward block
+        applies its `ff_act`.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
         axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
         onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
         fc1 is the plain GEMM on that copy.  The call is checked first: a ValueError leaves x as it was.
@@ -707,6 +731,12 @@ class TransformerEngine:
             kernels.append(attention_kernel(L, axial is not None, varlen is not None, vl is not None))
             if L.lpi is not None and (grid is None or grid[0] * grid[1] != N or axial is not None or varlen is not None):
                 raise ValueError("a layer with a local patch interaction needs `grid` = (h, w) with h * w == N")
+            if kernels[-1] == "groups":
+                if grid is None or grid[0] * grid[1] != N or groups is None:
+                    raise ValueError("patch-group attention needs `grid` = (h, w) with h * w == N and `groups`")
+                if grid[0] % groups[0] or grid[1] % groups[1]:
+                    raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {groups[0]} x {groups[1]} "
+                                     f"patches")
             if kernels[-1] in ("window", "window_relpos", "kv"):
                 if grid is None or grid[0] * grid[1] != N:
                     raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
@@ -733,7 +763,8 @@ class TransformerEngine:
             else:
                 _lib.layernorm(src, t[ln + ".w"], t[ln + ".b"], out_bf16=xb, eps=norm.eps)
                 wt, ln_kw = t[w + ".w"], dict(bias=t.get(w + ".b"))
-            (_lib.gemm_headnorm if "head_gamma" in epi else _lib.gemm)(xb, wt, out_bf16=out, **epi, **ln_kw)
+            fn = _lib.gemm_headnorm if "head_gamma" in epi else _lib.gemm_act if "act" in epi else _lib.gemm
+            fn(xb, wt, out_bf16=out, **epi, **ln_kw)
 
         def stream_copy(slot: str) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
             """(bf16 copy, row sums) the kernel writing the stream also writes: fold (xb, ws[slot]), exact none."""
@@ -791,6 +822,8 @@ class TransformerEngine:
             elif kernel == "window_relpos":
                 _lib.attention_window_relpos(qkv, o, t[f"{i}.relpos"], B, grid[0], grid[1], L.window, L.grid_windows,
                                              L.heads, L.dim_head, L.scale)
+            elif kernel == "groups":
+                _lib.attention_groups(qkv, o, B, grid[0], grid[1], groups[0], groups[1], L.heads, L.dim_head, L.scale)
             elif kernel == "xca":
                 _lib.attention_xca(qkv, t[f"{i}.tau"], o, B, N, L.heads, L.dim_head)
             elif kernel == "headmix":
@@ -807,6 +840,7 @@ class TransformerEngine:
 
         for i, kernel in zip(run, kernels):
             L = self.layers[i]
+            act = dict(act="silu") if L.ff_act == "silu" else dict(gelu=True)
             head = {} if L.qk_norm is None else dict(head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
                                                      head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
             if kernel == "kv":
@@ -831,9 +865,10 @@ class TransformerEngine:
             if L.post_norm:
                 # the normalised stream and its bf16 copy; fc1 reads that copy as it is, with no LayerNorm of its own
                 _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_f32=ff_in, out_bf16=xb, eps=L.ln2.eps)
-                _lib.gemm(xb, t[f"{i}.fc1.w"], out_bf16=h, bias=t[f"{i}.fc1.b"], gelu=True)
+                (_lib.gemm_act if "act" in act else _lib.gemm)(xb, t[f"{i}.fc1.w"], out_bf16=h, bias=t[f"{i}.fc1.b"],
+                                                                **act)
             else:
-                normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, gelu=True)
+                normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, **act)
             residual(h, f"{i}.fc2", ff_in, "stats_a")
 
     def final_norm(self, x: torch.Tensor, *, out_bf16: Optional[torch.Tensor] = None,
@@ -887,13 +922,15 @@ class TransformerEngine:
 
     def forward_tokens(self, tokens: torch.Tensor, rope: Optional[Tuple[torch.Tensor, int]] = None,
                        axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
-                       layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None) -> torch.Tensor:
+                       layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None,
+                       groups: Optional[Tuple[int, int]] = None) -> torch.Tensor:
         """Transformer.forward on arbitrary bf16 tokens [B, N, D] (what MAE / SimMIM / Distill call,
-        reference mae.py:74, simmim.py:70, distill.py:66); `rope`, `axial`, `layers` and `grid` as in run_blocks."""
+        reference mae.py:74, simmim.py:70, distill.py:66); `rope`, `axial`, `layers`, `grid` and `groups` as in
+        run_blocks."""
         B, N, D = tokens.shape
         with on_device(tokens):
             x = tokens.reshape(B * N, D).float().contiguous()
-            self.run_blocks(x, B, N, rope=rope, axial=axial, layers=layers, grid=grid)
+            self.run_blocks(x, B, N, rope=rope, axial=axial, layers=layers, grid=grid, groups=groups)
             out = torch.empty(B * N, D, device=tokens.device, dtype=torch.bfloat16)
             if self.norm is not None:
                 self.final_norm(x, out_bf16=out)
