@@ -113,12 +113,15 @@ __device__ __forceinline__ void warpgroup_sync(int c) { asm volatile("bar.sync %
 // tmO / tmF (TMA_OUT only): store maps over out_bf16 (64 x 64 boxes) and out_f32 (32 x 64 boxes), 128B swizzle
 // SIG: the instances that take EPI_SILU / EPI_SIGMOID (the squeeze-excitation GEMMs); every other instance is compiled
 // without that branch
-template <int BLOCK_N, int STAGES, bool PATCH, bool RES, bool TMA_OUT, bool SIG = false>
+// EPI >= 0 (TMA_OUT only): the instance runs launches whose flags are exactly EPI -- the encoder layer's flag sets, see
+// launch_tma_out -- so that every flag test of the epilogue is resolved at compile time; -1: the flags of the launch
+template <int BLOCK_N, int STAGES, bool PATCH, bool RES, bool TMA_OUT, bool SIG = false, int EPI = -1>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO,
                  const __grid_constant__ CUtensorMap tmF, const GemmParams p) {
   static_assert(!(TMA_OUT && PATCH), "patch tiles have fewer than 128 rows: a 64-row box would overwrite the next one");
+  static_assert(EPI < 0 || (TMA_OUT && !SIG), "compiled flag sets are for the TMA-store epilogue");
   using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
   constexpr int NACC = BLOCK_N / 2;          // fp32 accumulators per consumer thread (64 rows x BLOCK_N / 128)
   constexpr int CHUNKS = BLOCK_N / 64;       // 64-column statistics chunks (and residual slabs) per tile
@@ -278,7 +281,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int c = wg - 1;                       // rows [64c, 64c + 64) of the tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
-  const int flags = L::BIAS_ONLY ? p.flags & ~B200VIT_EPI_LNFOLD : p.flags;  // the host routes LN folds elsewhere
+  // (BIAS_ONLY: the host routes LN folds elsewhere)
+  const int flags = EPI >= 0 ? EPI : L::BIAS_ONLY ? p.flags & ~B200VIT_EPI_LNFOLD : p.flags;
   const bool vec_ok = (p.ldo & 1) == 0;
   int stage = 0;
   uint32_t phase = 0;
@@ -368,6 +372,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // TMA_OUT: this thread's bf16 pair in a staging box: row tr0 % 64 (+ 8 h), 16-byte chunk (j % 8) ^ (tr0 % 8),
     // byte 4 (lane % 4) -- the 8 rows of a warp store land in 8 different chunks, so the stores are conflict free
     const int stg_off = (tr0 - 64 * c) * 128 + 4 * (lane & 3);
+    // GUARD: skip the pairs outside M x N.  A compiled flag set without a residual needs no such test: whatever lands
+    // in the staging tile past M or N stays there, because the store maps clip both edges, and these flag sets collect
+    // no statistics.  (It is finite, too: TMA zero-fills A and W outside their maps, vbias / vcs are zero past N, and
+    // the LN sums of rows past M are zero, so their rstd is rsqrt(eps).)  With a residual, a slab's columns past N
+    // hold stale data that would enter the row statistics.  Without the tests, and with the flags known at compile
+    // time, the loop is straight-line code whose pairs the compiler interleaves.
+    constexpr bool GUARD = EPI < 0 || RES;
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
       const int pc = 8 * j + 2 * (lane & 3);  // column of the pair in the tile
@@ -396,7 +407,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (!row_ok[h] || col >= p.N) continue;
+        if (GUARD && (!row_ok[h] || col >= p.N)) continue;
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
         if (flags & (B200VIT_EPI_LNFOLD | B200VIT_EPI_BIAS)) {
           // y = acc * rstd + (bias - rstd*mu * s)
@@ -574,7 +585,8 @@ void gemm_set_block_n(int v) { g_gemm_block_n = v; }
 static std::atomic<int> g_gemm_direct_store{0};
 void gemm_set_direct_store(int v) { g_gemm_direct_store = v; }
 
-template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false, bool SIG = false>
+template <int BLOCK_N, int STAGES, bool PATCH = false, bool RES = false, bool TMA_OUT = false, bool SIG = false,
+          int EPI = -1>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR, const CUtensorMap& tmO,
                        const CUtensorMap& tmF, GemmParams& p, cudaStream_t stream) {
   using L = GemmSmem<BLOCK_N, STAGES, PATCH, RES, TMA_OUT>;
@@ -582,7 +594,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   // barriers + 1 KB alignment slack = 215 168 of the 232 448 bytes
   static_assert(L::DYN_BYTES <= 227 * 1024, "gemm: shared memory budget");
   static_assert(!L::BIAS_ONLY || L::DYN_BYTES == 215168, "gemm: 256 x 4 residual TMA-store layout changed");
-  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES, TMA_OUT, SIG>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, STAGES, PATCH, RES, TMA_OUT, SIG, EPI>;
   B200_ENSURE_SMEM(kern, L::DYN_BYTES);
   if (!p.patch) p.rows_per_tile = BLOCK_M;
   p.num_m_tiles = (p.M + p.rows_per_tile - 1) / p.rows_per_tile;
@@ -595,6 +607,28 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   B200_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
+}
+
+// TMA-store launches with the encoder layer's flag sets -- QKV (bias + LN fold), FC1 (the same + GELU), out-proj and
+// FC2 (residual + statistics, with or without a bias) -- run instances compiled for exactly those flags; any other set
+// runs the generic instance
+template <int BLOCK_N, int STAGES, bool RES>
+static int launch_tma_out(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmR,
+                          const CUtensorMap& tmO, const CUtensorMap& tmF, GemmParams& p, cudaStream_t stream) {
+  constexpr int QKV = B200VIT_EPI_BIAS | B200VIT_EPI_LNFOLD, FC1 = QKV | B200VIT_EPI_GELU;
+  constexpr int RES_STATS = B200VIT_EPI_RESIDUAL | B200VIT_EPI_STATS, RES_STATS_BIAS = RES_STATS | B200VIT_EPI_BIAS;
+  if constexpr (RES) {
+    if (p.flags == RES_STATS_BIAS)
+      return launch_gemm<BLOCK_N, STAGES, false, true, true, false, RES_STATS_BIAS>(tmA, tmB, tmR, tmO, tmF, p, stream);
+    if (p.flags == RES_STATS)
+      return launch_gemm<BLOCK_N, STAGES, false, true, true, false, RES_STATS>(tmA, tmB, tmR, tmO, tmF, p, stream);
+  } else {
+    if (p.flags == QKV)
+      return launch_gemm<BLOCK_N, STAGES, false, false, true, false, QKV>(tmA, tmB, tmR, tmO, tmF, p, stream);
+    if (p.flags == FC1)
+      return launch_gemm<BLOCK_N, STAGES, false, false, true, false, FC1>(tmA, tmB, tmR, tmO, tmF, p, stream);
+  }
+  return launch_gemm<BLOCK_N, STAGES, false, RES, true>(tmA, tmB, tmR, tmO, tmF, p, stream);
 }
 
 }  // namespace b200
@@ -713,10 +747,10 @@ extern "C" int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int6
   // residual launches trade ring stages for the two 32 KB residual slabs, TMA-store launches for the staging buffers
   if (tma_out) {
     if (res)
-      return wide ? launch_gemm<256, 4, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st)
-                  : launch_gemm<128, 4, false, true, true>(tmA, tmB, tmR, tmO, tmF, p, st);
-    return wide ? launch_gemm<256, 3, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st)
-                : launch_gemm<128, 5, false, false, true>(tmA, tmB, tmR, tmO, tmF, p, st);
+      return wide ? launch_tma_out<256, 4, true>(tmA, tmB, tmR, tmO, tmF, p, st)
+                  : launch_tma_out<128, 4, true>(tmA, tmB, tmR, tmO, tmF, p, st);
+    return wide ? launch_tma_out<256, 3, false>(tmA, tmB, tmR, tmO, tmF, p, st)
+                : launch_tma_out<128, 5, false>(tmA, tmB, tmR, tmO, tmF, p, st);
   }
   if (wide)
     return res ? launch_gemm<256, 3, false, true>(tmA, tmB, tmR, tmO, tmF, p, st)
