@@ -344,6 +344,43 @@ int b200vit_attention_groups(const void* qkv, void* out, int B, int gh, int gw, 
                              float scale, void* stream);
 
 /*
+ * SepViT's window attention with a window token (sep_vit.py:139-168) over B maps of gh x gw tokens, token (b, y, x) at
+ * row (b*gh + y)*gw + x of qkv[B*gh*gw, 3*H*dh] bf16 (packed as for b200vit_attention) and of out[B*gh*gw, H*dh] bf16.
+ * Window (b, wy, wx) of the (gh/p) x (gw/p) grid holds the p*p tokens (wy*p + u, wx*p + v) and one more token whose
+ * q | k | v is tok_qkv[3*H*dh] bf16 (the layer's to_qkv applied to its window_tokens parameter, the same for every
+ * window); each head attends among these p*p + 1 tokens:  softmax(scale * q k^T) v.  The window's own tokens' results
+ * go to their rows of out; if tok_out is not NULL, the window token's result goes to row (b*(gh/p) + wy)*(gw/p) + wx
+ * of tok_out[B*(gh/p)*(gw/p), H*dh] bf16, the reference's '(b x y)' window order.
+ * One CTA per (window, head): row 0 of the 64-row tile is the window token, rows 1 .. p*p the window's tokens gathered
+ * with cp.async; both products on wgmma.  Numerics as b200vit_attention_window: fp32 scores, exp2 with scale*log2(e)
+ * folded in, probabilities rounded to bf16, fp32 accumulation, one bf16 rounding of the output.
+ * p*p + 1 <= 64 (p <= 7), gh and gw multiples of p, dh = 32, 64, 80 or 128, H <= 65535; every pointer 16-byte aligned.
+ * Isolation: a window's outputs are computed from its own rows and tok_qkv only and nothing outside the B*gh*gw rows
+ * of qkv / out and the addressed rows of tok_out is read or written; a NaN or Inf stays within its window.
+ */
+int b200vit_attention_window_token(const void* qkv, const void* tok_qkv, void* out, void* tok_out, int B, int gh,
+                                   int gw, int p, int H, int dh, float scale, void* stream);
+
+/*
+ * SepViT's attention across windows (sep_vit.py:182-205), out of place on B maps laid out as for
+ * b200vit_attention_window_token, with nw = (gh/p)*(gw/p) windows per map:
+ *   wqk[B*nw, 2*H*dh] bf16, row b*nw + j the window-token projection of window j of image b; head h's query is columns
+ *   [2h*dh, 2h*dh + dh) and its key [2h*dh + dh, 2(h+1)*dh) (the per-head interleave of 'b (h c) n -> b h n c' then
+ *   .chunk(2, -1));
+ *   P = softmax_j(scale * wq_i . wk_j) per (image, head), over the nw windows;
+ *   out[(window i, position w)] = sum_j P_ij o[(window j, position w)]  for every window position w < p*p, o and out
+ *   [B*gh*gw, H*dh] bf16, head h's columns [h*dh, (h+1)*dh).
+ * One CTA per (image, head, slice of up to 8 window positions): S = wq wk^T on one 64 x 64 wgmma and the softmax once,
+ * then per position the nw rows of o through a two-buffer cp.async ring and O_w = P V_w on wgmma.  Numerics as
+ * b200vit_attention_window_token.
+ * 2 <= nw <= 64, gh and gw multiples of p, dh = 32, 64, 80 or 128; out != o; every pointer 16-byte aligned.
+ * Isolation: an (image, head)'s output is computed from its own rows of wqk and o only, and nothing outside the
+ * B*nw rows of wqk and the B*gh*gw rows of o / out is read or written; a NaN or Inf stays within its image and head.
+ */
+int b200vit_window_mix(const void* wqk, const void* o, void* out, int B, int gh, int gw, int p, int H, int dh,
+                       float scale, void* stream);
+
+/*
  * Squeeze-excitation around two bias-free GEMMs (max_vit.py:47-62):
  *   b200vit_se_pool:   pooled[b][c] bf16 = (sum_p part[b][p][c]) * inv_n, the parts added in index order (the mean of
  *                      b200vit_mbconv_dwconv's output); the gate then runs as GEMM(EPI_SILU), GEMM(EPI_SIGMOID) over
@@ -405,6 +442,12 @@ int b200vit_rmsnorm_heads(void* buf, int64_t ld, const float* gamma, int T, int 
 /* ... and its LayerNorm (no bias) flavour: (v - mean) * rsqrt(var + eps) * gamma[h, d] over each dh-wide head. */
 int b200vit_layernorm_heads(void* buf, int64_t ld, const float* gamma, int T, int nheads, int dh, float eps,
                             void* stream);
+/* ... and with a shift and exact-erf GELU after it, SepViT's window-token pre-norm (sep_vit.py:96-98):
+ *   v <- GELU_erf((v - mean) * rsqrt(var + eps) * gamma[d] + beta[d]),  gamma, beta fp32 [dh] shared by the heads,
+ * statistics in fp32 with the two-pass variance.  In place on the nheads heads from column 0 of every row buf[t*ld
+ * ...]; ld a multiple of 8, buf, gamma and beta 16-byte aligned.  Each row is read and written only by its own warp. */
+int b200vit_head_layernorm_gelu(void* buf, int64_t ld, const float* gamma, const float* beta, int T, int nheads, int dh,
+                                float eps, void* stream);
 
 /*
  * NaViT token assembly on the packed [T, D] matrix (na_vit.py:228,350-359): x = LayerNorm(y; gamma, no bias)

@@ -7,6 +7,7 @@ The fused path lives in csrc/ (CUDA, C ABI in include/b200vit.h) and is bound wi
 from .vit import ViT
 from .simple_vit import SimpleViT
 from .na_vit import NaViT           # padding-free fused path (varlen attention) + the reference's packed PyTorch graph
+from .sep_vit import SepViT         # window attention with window tokens, then attention across windows
 
-__all__ = ["ViT", "SimpleViT", "NaViT"]
+__all__ = ["ViT", "SimpleViT", "NaViT", "SepViT"]
 __version__ = "0.1.0"

@@ -48,7 +48,8 @@ SYMBOLS = [
     "b200vit_attention_window", "b200vit_attention_kv", "b200vit_merge_patches_ln", "b200vit_peg",
     "b200vit_attention_posbias", "b200vit_attention_window_relpos", "b200vit_mbconv_dwconv", "b200vit_se_pool",
     "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw", "b200vit_mbconv_dwconv_ex",
-    "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex",
+    "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex", "b200vit_attention_window_token",
+    "b200vit_window_mix", "b200vit_head_layernorm_gelu",
 ]
 
 
@@ -173,6 +174,12 @@ def lib() -> C.CDLL:
     L.b200vit_mbconv_dwconv_ex.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200vit_attention_groups.restype = i32
     L.b200vit_attention_groups.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_attention_window_token.restype = i32
+    L.b200vit_attention_window_token.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_window_mix.restype = i32
+    L.b200vit_window_mix.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_head_layernorm_gelu.restype = i32
+    L.b200vit_head_layernorm_gelu.argtypes = [vp, i64, vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_se_pool.restype = i32
     L.b200vit_se_pool.argtypes = [vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_se_scale.restype = i32
@@ -740,6 +747,61 @@ def attention_groups(qkv: torch.Tensor, out: torch.Tensor, B: int, gh: int, gw: 
         rc = lib().b200vit_attention_groups(_ptr(qkv), _ptr(out), B, int(gh), int(gw), int(ph), int(pw), H, dh,
                                             float(scale), _stream())
     _check(rc, "b200vit_attention_groups")
+
+
+def attention_window_token(qkv: torch.Tensor, tok_qkv: torch.Tensor, out: torch.Tensor,
+                           tok_out: Optional[torch.Tensor], B: int, gh: int, gw: int, p: int, H: int, dh: int,
+                           scale: float) -> None:
+    """SepViT attention inside the p x p windows of B token maps of gh x gw tokens, each window with one more token
+    whose q | k | v is tok_qkv[3*H*dh] (the same for every window): qkv[B*gh*gw, 3*H*dh] packed q | k | v, token
+    (b, y, x) at row (b*gh + y)*gw + x; out[B*gh*gw, H*dh]; tok_out None or [B*nw, H*dh], the window token's output
+    of window (b, wy, wx) at row (b*gh/p + wy)*gw/p + wx (sep_vit.py:139-172)."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(tok_qkv, torch.bfloat16, "tok_qkv"); _chk(out, torch.bfloat16, "out")
+    _chk(tok_out, torch.bfloat16, "tok_out")
+    I = H * dh
+    assert qkv.is_contiguous() and out.is_contiguous() and tok_qkv.is_contiguous() and tok_qkv.numel() == 3 * I
+    assert qkv.shape == (B * gh * gw, 3 * I) and out.shape == (B * gh * gw, I)
+    nw = (gh // p) * (gw // p) if p > 0 else 0
+    assert tok_out is None or (tok_out.is_contiguous() and tok_out.shape == (B * nw, I))
+    n = p * p + 1
+    with _Timed("attention_window_token", B=B, h=gh, w=gw, p=p, H=H,
+                bytes=(qkv.numel() + out.numel() + (0 if tok_out is None else tok_out.numel())) * 2,
+                flops=4.0 * B * nw * H * n * n * dh):
+        rc = lib().b200vit_attention_window_token(_ptr(qkv), _ptr(tok_qkv), _ptr(out), _ptr(tok_out), B, int(gh),
+                                                  int(gw), int(p), H, dh, float(scale), _stream())
+    _check(rc, "b200vit_attention_window_token")
+
+
+def window_mix(wqk: torch.Tensor, o: torch.Tensor, out: torch.Tensor, B: int, gh: int, gw: int, p: int, H: int,
+               dh: int, scale: float) -> None:
+    """SepViT attention across the nw windows of each map (sep_vit.py:182-205): per image and head P =
+    softmax(scale wq wk^T) over the windows, wqk[B*nw, 2*H*dh] with head h's query at columns [2h dh, 2h dh + dh) and
+    its key right after; out[(window i, position w)] = sum_j P_ij o[(window j, position w)], o and out [B*gh*gw, H*dh]
+    in the map's row order, out of place."""
+    _chk(wqk, torch.bfloat16, "wqk"); _chk(o, torch.bfloat16, "o"); _chk(out, torch.bfloat16, "out")
+    I = H * dh
+    nw = (gh // p) * (gw // p) if p > 0 else 0
+    assert wqk.is_contiguous() and o.is_contiguous() and out.is_contiguous()
+    assert wqk.shape == (B * nw, 2 * I) and o.shape == (B * gh * gw, I) and out.shape == (B * gh * gw, I)
+    with _Timed("window_mix", B=B, h=gh, w=gw, p=p, H=H, nw=nw, bytes=(wqk.numel() + o.numel() + out.numel()) * 2,
+                flops=2.0 * B * H * nw * nw * (dh + p * p * dh)):
+        rc = lib().b200vit_window_mix(_ptr(wqk), _ptr(o), _ptr(out), B, int(gh), int(gw), int(p), H, dh, float(scale),
+                                      _stream())
+    _check(rc, "b200vit_window_mix")
+
+
+def head_layernorm_gelu(buf: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, nheads: int, dh: int,
+                        eps: float = 1e-5) -> None:
+    """In place on buf[T, >= nheads*dh] bf16: every dh-wide head from column 0 <- GELU_erf(LayerNorm(head) gamma +
+    beta), gamma and beta fp32 [dh] shared by the heads (SepViT's window_tokens_to_qk, sep_vit.py:96-98)."""
+    _chk(buf, torch.bfloat16, "buf"); _chk(gamma, torch.float32, "gamma"); _chk(beta, torch.float32, "beta")
+    assert buf.dim() == 2 and buf.stride(1) == 1 and gamma.is_contiguous() and beta.is_contiguous()
+    assert gamma.numel() == dh and beta.numel() == dh
+    T = buf.shape[0]
+    with _Timed("head_layernorm_gelu", T=T, H=nheads, bytes=T * nheads * dh * 4):
+        rc = lib().b200vit_head_layernorm_gelu(_ptr(buf), buf.stride(0), _ptr(gamma), _ptr(beta), T, int(nheads),
+                                               int(dh), float(eps), _stream())
+    _check(rc, "b200vit_head_layernorm_gelu")
 
 
 def se_pool(part: torch.Tensor, pooled: torch.Tensor, n: int) -> None:

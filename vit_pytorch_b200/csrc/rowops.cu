@@ -669,6 +669,69 @@ rmsnorm_heads_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float*
   }
 }
 
+// SepViT's window-token pre-norm and activation (reference sep_vit.py:96-98), in place on buf[T, ld] bf16:
+//   v <- GELU_erf((v - mean) * rsqrt(var + eps) * gamma[d] + beta[d])  over each of the `nheads` DH-wide heads, one
+// nn.LayerNorm(dh) shared by the heads.  The lane layout, the sums and the two-pass variance are those of
+// rmsnorm_heads_kernel<DH, 1, true>; GELU is common.cuh's gelu_erf, as the GEMM epilogue's.
+template <int DH>
+__global__ void __launch_bounds__(256)
+head_layernorm_gelu_kernel(__nv_bfloat16* __restrict__ buf, long long ld, const float* __restrict__ gamma,
+                           const float* __restrict__ beta, int T, int nheads, float eps) {
+  using HL = HeadLanes<DH>;
+  constexpr int LPH = HL::LPH, HPS = HL::HPS;
+  const long long t = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (t >= T) return;
+  __nv_bfloat16* row = buf + t * ld;
+  const int sub = lane % LPH, grp = lane / LPH;
+  const bool act = sub < HL::CH;  // (always true unless dh = 80)
+  float4 g[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)}, be[2] = {g[0], g[1]};
+  if (act) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      g[i] = *reinterpret_cast<const float4*>(gamma + 8 * sub + 4 * i);
+      be[i] = *reinterpret_cast<const float4*>(beta + 8 * sub + 4 * i);
+    }
+  }
+  for (int base = 0; base < nheads; base += HPS) {
+    const int hh = base + grp;  // (heads beyond nheads: the group only joins the shuffles)
+    uint4 raw = act ? *(reinterpret_cast<const uint4*>(row + (hh < nheads ? hh : 0) * DH) + sub)
+                    : make_uint4(0, 0, 0, 0);
+    __nv_bfloat162* h2 = reinterpret_cast<__nv_bfloat162*>(&raw);
+    float2 f[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) f[i] = __bfloat1622float2(h2[i]);
+    float s1 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) s1 += f[i].x + f[i].y;
+#pragma unroll
+    for (int o = LPH / 2; o > 0; o >>= 1) s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+    const float mean = s1 * (1.0f / (float)DH);
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      f[i].x -= mean;
+      f[i].y -= mean;
+      q = fmaf(f[i].x, f[i].x, fmaf(f[i].y, f[i].y, q));
+    }
+    if (!act) q = 0.f;  // dh 80: an idle lane's zeros would add (0 - mean)^2
+#pragma unroll
+    for (int o = LPH / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    const float inv = rsqrtf(q * (1.0f / (float)DH) + eps);
+    if (hh < nheads && act) {
+      const float gg[8] = {g[0].x, g[0].y, g[0].z, g[0].w, g[1].x, g[1].y, g[1].z, g[1].w};
+      const float bb[8] = {be[0].x, be[0].y, be[0].z, be[0].w, be[1].x, be[1].y, be[1].z, be[1].w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        float a = f[i].x * inv * gg[2 * i] + bb[2 * i], c = f[i].y * inv * gg[2 * i + 1] + bb[2 * i + 1];
+        gelu_erf2(a, c);
+        h2[i] = __floats2bfloat162_rn(a, c);
+      }
+      *(reinterpret_cast<uint4*>(row + hh * DH) + sub) = raw;
+    }
+  }
+}
+
 // NaViT attention pooling (reference na_vit.py:371-387): one learned query per image attends to that image's tokens.
 //   kv[T, 2*H*DH] bf16 (k already RMS-normalised, then v), qn[H*DH] fp32 (normalised query), sequences by cu_seqlens;
 //   out[S, H*DH] bf16 = softmax_j(qn_h . k_jh) v_jh   (scale 1).  One CTA of 8 warps per (image, head): warp w walks the
@@ -894,6 +957,31 @@ extern "C" int b200vit_layernorm_heads(void* buf, int64_t ld, const float* gamma
                  "layernorm_heads: rows must be 16-byte aligned and hold nheads*dh columns (ld=%lld)", (long long)ld);
   launch_heads_norm<true>(reinterpret_cast<__nv_bfloat16*>(buf), ld, gamma, T, nheads, dh, eps,
                           reinterpret_cast<cudaStream_t>(stream));
+  B200_CHECK_CUDA(cudaGetLastError());
+  b200::count_launch();
+  return 0;
+}
+
+extern "C" int b200vit_head_layernorm_gelu(void* buf, int64_t ld, const float* gamma, const float* beta, int T,
+                                           int nheads, int dh, float eps, void* stream) {
+  B200_CHECK_ARG(buf && gamma && beta, "head_layernorm_gelu: null pointer");
+  B200_CHECK_ARG(T > 0 && nheads > 0, "head_layernorm_gelu: bad shape T=%d nheads=%d", T, nheads);
+  B200_CHECK_ARG(head_width_ok(dh), "head_layernorm_gelu: dim_head=%d not supported by this build (32, 64, 80 or 128)",
+                 dh);
+  B200_CHECK_ARG(ld >= (int64_t)nheads * dh && (ld % 8) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0,
+                 "head_layernorm_gelu: rows must be 16-byte aligned and hold nheads*dh columns (ld=%lld)",
+                 (long long)ld);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(gamma) & 15) == 0 && (reinterpret_cast<uintptr_t>(beta) & 15) == 0,
+                 "head_layernorm_gelu: gamma and beta must be 16-byte aligned");
+  auto* b = reinterpret_cast<__nv_bfloat16*>(buf);
+  const dim3 grid((T + 7) / 8);
+  const auto st = reinterpret_cast<cudaStream_t>(stream);
+  switch (dh) {
+    case 32: b200::head_layernorm_gelu_kernel<32><<<grid, 256, 0, st>>>(b, ld, gamma, beta, T, nheads, eps); break;
+    case 80: b200::head_layernorm_gelu_kernel<80><<<grid, 256, 0, st>>>(b, ld, gamma, beta, T, nheads, eps); break;
+    case 128: b200::head_layernorm_gelu_kernel<128><<<grid, 256, 0, st>>>(b, ld, gamma, beta, T, nheads, eps); break;
+    default: b200::head_layernorm_gelu_kernel<64><<<grid, 256, 0, st>>>(b, ld, gamma, beta, T, nheads, eps);
+  }
   B200_CHECK_CUDA(cudaGetLastError());
   b200::count_launch();
   return 0;

@@ -137,6 +137,8 @@ PEG_KERNEL_SIZES = (1, 3, 5, 7)            # b200vit_peg
 CONV_PROJ_KERNEL_SIZES = (1, 3, 5, 7)      # b200vit_conv_proj_dw
 GROUPS_WIDTHS = (8,)                       # b200vit_attention_groups
 GROUPS_MAX_TOKENS = _lib.ATTN_GROUPS_MAX_TOKENS    # b200vit_attention_groups: tokens of one group
+WINDOW_TOKEN_MAX_WINDOW = 7                # b200vit_attention_window_token: p*p tokens + the window token <= 64
+WINDOW_MIX_MAX_WINDOWS = 64                # b200vit_window_mix: windows of one map
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -286,6 +288,20 @@ def conv_proj_weights(P: ConvProj) -> Tuple[torch.Tensor, torch.Tensor, torch.Te
     return out[0], out[1], out[2], out[3]
 
 
+class WindowTokenBlock(NamedTuple):
+    """SepViT's window token and the attention across windows it drives (DSSA, sep_vit.py:91-102, 139-205): `token`
+    [D] joins every p x p window as one more key, value and query of the layer's own (bias-free) qkv projection, not
+    normalised; its per-head outputs pass `ln` (nn.LayerNorm(dim_head), shared by the heads), GELU and the 1 x 1
+    convolution wqk_w [2I, I] + wqk_b over the heads' channels, whose output columns interleave per head (q of head h
+    at [2h dh, 2h dh + dh), its k right after); softmax(scale wq wk^T) over the windows then mixes the windows' outputs
+    position by position (b200vit_attention_window_token, b200vit_head_layernorm_gelu, GEMM, b200vit_window_mix)."""
+    token: torch.Tensor                           # [D], a parameter
+    ln: Norm                                      # over dim_head values
+    wqk_w: torch.Tensor                           # [2I, I] (the Conv1d weight [2I, I, 1] reshaped)
+    wqk_b: torch.Tensor                           # [2I]
+    window: int
+
+
 @dataclass
 class EncoderLayer:
     """One pre-LN encoder layer as a model family describes it to the engine (reference vit.py:78-81):
@@ -346,15 +362,22 @@ class EncoderLayer:
     # attention inside the strided patch groups of the token grid, token (y'*ph + i, x'*pw + j) in group (i, j)
     # (MobileViT, mobile_vit.py:150; b200vit_attention_groups); run_blocks needs `grid` and `groups` = (ph, pw)
     patch_groups: bool = False
+    # attention inside non-overlapping window x window blocks with one learned window token each, then across the
+    # windows (SepViT's DSSA, sep_vit.py:65-206); run_blocks needs `grid`
+    window_token: Optional[WindowTokenBlock] = None
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
     """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'window_relpos' (windows with a
     relative-position bias), 'kv' (sub-sampled keys: a strided convolution or CvT's convolutional projections),
-    'groups' (strided patch groups), 'axial' (a run_blocks call with `axial`, unless the layer's temporal sub-block runs
+    'groups' (strided patch groups), 'window_token' (SepViT's windows with a window token, then across windows), 'axial' (a run_blocks call with `axial`, unless the layer's temporal sub-block runs
     there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys) or 'plain'.  ValueError for
     cross-covariance, head-mixing, windowed, patch-group or sub-sampled-key attention with `axial` or over a `packed`
     batch."""
+    if L.window_token is not None:
+        if axial or packed:
+            raise ValueError("window-token attention runs over B token grids only")
+        return "window_token"
     if L.patch_groups:
         if axial or packed:
             raise ValueError("patch-group attention runs over B token grids only")
@@ -529,6 +552,10 @@ class TransformerEngine:
             if r is None and L.conv_proj is not None and L.conv_proj.kernel_size not in CONV_PROJ_KERNEL_SIZES:
                 r = (f"proj_kernel={L.conv_proj.kernel_size} (the convolutional-projection kernel is built for 1, 3, 5 "
                      f"and 7)")
+            if r is None and kernel == "window_token" and L.window_token.window > WINDOW_TOKEN_MAX_WINDOW:
+                r = (f"window_size={L.window_token.window}: a window of {L.window_token.window ** 2} tokens and its "
+                     f"window token (the window-token attention kernel takes windows up to "
+                     f"{WINDOW_TOKEN_MAX_WINDOW} x {WINDOW_TOKEN_MAX_WINDOW})")
             if r is None and L.window is not None and L.window ** 2 > WINDOW_MAX_TOKENS:
                 r = (f"local_patch_size={L.window}: a window of {L.window ** 2} tokens (the window attention kernel "
                      f"takes at most {WINDOW_MAX_TOKENS})")
@@ -587,6 +614,12 @@ class TransformerEngine:
             elif L.kv_stride is not None:
                 # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
                 t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.detach().permute(0, 2, 3, 1).reshape(L.kv_w.shape[0], -1))
+            if L.window_token is not None:
+                T = L.window_token
+                # the window token's q | k | v: the same for every window, so projected once, in fp32, then rounded
+                t[f"{i}.tok_qkv"] = (L.qkv_w.detach().float() @ T.token.detach().float()).to(torch.bfloat16)
+                t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"] = _f32(T.ln.gamma), _f32(T.ln.beta)
+                t[f"{i}.wqk.w"], t[f"{i}.wqk.b"] = _bf16_rows(T.wqk_w), _f32(T.wqk_b)
             if L.lpi is not None:
                 P = L.lpi
                 t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"] = _f32(P.ln.gamma), _f32(P.ln.beta)
@@ -657,6 +690,9 @@ class TransformerEngine:
             if any(L.lpi is not None or L.post_norm for L in self.layers):
                 # the stream the feed-forward block reads: the local patch interaction's or the post-norm's output
                 slot.t["y"] = torch.empty(M, D, device=device, dtype=torch.float32)
+            if any(L.window_token is not None for L in self.layers):
+                # the attention across windows, out of place from "o"
+                slot.t["o2"] = torch.empty(M, I, **bf)
             if any(L.lpi is not None for L in self.layers):
                 # the local patch interaction's row statistics and its LayerNorm scratch
                 slot.t["stats_l"] = torch.empty(M, 2, device=device, dtype=torch.float32)
@@ -703,7 +739,9 @@ class TransformerEngine:
         and the key / value GEMM (kernel size 1: the GEMM on xb itself), then attention_kv.  A layer with convolutional
         projections (CvT) runs layernorm(x -> xb), conv_proj_dw of xb into the query and key / value operands, their
         1 x 1 GEMMs, then attention_kv; the projections pad, so any h, w >= 1 will do.  Layers with patch-group attention
-        (MobileViT) need `groups` = (ph, pw) dividing `grid` as well (attention_groups).  A layer's feed-forward block
+        (MobileViT) need `groups` = (ph, pw) dividing `grid` as well (attention_groups).  Layers with window-token attention
+        (SepViT) need `grid` cut into at most 64 windows: attention_window_token into o, and with more than one window
+        head_layernorm_gelu, the window q | k GEMM and window_mix into ws['o2'], which the out-projection then reads.  A layer's feed-forward block
         applies its `ff_act`.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
         axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
         onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
@@ -737,6 +775,15 @@ class TransformerEngine:
                 if grid[0] % groups[0] or grid[1] % groups[1]:
                     raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {groups[0]} x {groups[1]} "
                                      f"patches")
+            if kernels[-1] == "window_token":
+                p = L.window_token.window
+                if grid is None or grid[0] * grid[1] != N:
+                    raise ValueError("window-token attention needs `grid` = (h, w) with h * w == N")
+                if grid[0] % p or grid[1] % p:
+                    raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {p} x {p} windows")
+                if (grid[0] // p) * (grid[1] // p) > WINDOW_MIX_MAX_WINDOWS:
+                    raise ValueError(f"a {grid[0]} x {grid[1]} grid has more than {WINDOW_MIX_MAX_WINDOWS} "
+                                     f"{p} x {p} windows")
             if kernels[-1] in ("window", "window_relpos", "kv"):
                 if grid is None or grid[0] * grid[1] != N:
                     raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
@@ -816,6 +863,26 @@ class TransformerEngine:
             _lib.gemm(akv, t[f"{i}.kv.w"], out_bf16=kv)
             _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
 
+        def window_token(L: EncoderLayer, i: int) -> torch.Tensor:
+            """SepViT's DSSA after its QKV projection: the windows' attention with their window token into o; with more
+            than one window, the window tokens' outputs -> LayerNorm + GELU -> their q | k GEMM -> the attention across
+            windows into a second buffer.  Returns the buffer that holds the result."""
+            T, I = L.window_token, L.heads * L.dim_head
+            gh, gw, p = grid[0], grid[1], T.window
+            nw = (gh // p) * (gw // p)
+            if nw == 1:           # the window token is a key and a value, its own output unused (sep_vit.py:176-178)
+                _lib.attention_window_token(qkv, t[f"{i}.tok_qkv"], o, None, B, gh, gw, p, L.heads, L.dim_head,
+                                            L.scale)
+                return o
+            tok = torch.empty(B * nw, I, device=x.device, dtype=torch.bfloat16)
+            _lib.attention_window_token(qkv, t[f"{i}.tok_qkv"], o, tok, B, gh, gw, p, L.heads, L.dim_head, L.scale)
+            _lib.head_layernorm_gelu(tok, t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"], L.heads, L.dim_head, eps=T.ln.eps)
+            wqk = torch.empty(B * nw, 2 * I, device=x.device, dtype=torch.bfloat16)
+            _lib.gemm(tok, t[f"{i}.wqk.w"], out_bf16=wqk, bias=t[f"{i}.wqk.b"])
+            mixed = ws["o2"]
+            _lib.window_mix(wqk, o, mixed, B, gh, gw, p, L.heads, L.dim_head, L.scale)
+            return mixed
+
         def attend(kernel: str, L: EncoderLayer, i: int) -> None:
             if kernel == "window":
                 _lib.attention_window(qkv, o, B, grid[0], grid[1], L.window, L.heads, L.dim_head, L.scale)
@@ -843,14 +910,18 @@ class TransformerEngine:
             act = dict(act="silu") if L.ff_act == "silu" else dict(gelu=True)
             head = {} if L.qk_norm is None else dict(head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
                                                      head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
+            attn_out = o
             if kernel == "kv":
                 subsampled(L, i)
             else:
                 normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv, **head)
                 if rope is not None:
                     _lib.rope_qk(qkv, rope[0], rope[1], L.heads, L.dim_head)
-                attend(kernel, L, i)
-            residual(o, f"{i}.out", x, "stats_b" if L.lpi is None and not L.post_norm else None)
+                if kernel == "window_token":
+                    attn_out = window_token(L, i)
+                else:
+                    attend(kernel, L, i)
+            residual(attn_out, f"{i}.out", x, "stats_b" if L.lpi is None and not L.post_norm else None)
             if L.temporal is not None:
                 normed(x, f"{i}.tln", L.temporal.ln, f"{i}.tqkv", qkv)
                 attend("axial", L, i)
