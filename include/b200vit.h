@@ -381,6 +381,26 @@ int b200vit_window_mix(const void* wqk, const void* o, void* out, int B, int gh,
                        float scale, void* stream);
 
 /*
+ * RegionViT's region-to-local attention (regionvit.py:167-176) over one buffer of both token maps of B images:
+ * qkv[B*lh*lw + B*rh*rw, 3*H*dh] bf16 (packed as for b200vit_attention) holds the local tokens first, token (b, y, x)
+ * at row (b*lh + y)*lw + x, then the region tokens, token (b, i, j) at row B*lh*lw + (b*rh + i)*rw + j; out
+ * [same rows, H*dh] bf16 has the same layout.  Window (b, i, j) is the region token (b, i, j) and the wh x ww local
+ * tokens (i*wh + u, j*ww + v), wh = lh/rh, ww = lw/rw; per head its n = 1 + wh*ww tokens attend together,
+ *   softmax(scale * q k^T + bias) v,
+ * bias = table[h*(2W-1)^2 + (u1-u2 + W-1) + (v1-v2 + W-1)*(2W-1)] between local tokens (u1, v1) (query) and (u2, v2)
+ * (key), 0 for every pair that involves the region token.  table fp32 [H][(2W-1)^2] is the transposed
+ * local_rel_pos_bias.weight of an R2LTransformer built with window_size W.  Each result goes to its own row of out.
+ * One CTA per (window, head, 64-row query tile): the window's <= 4 key / value blocks gathered with cp.async, both
+ * products on wgmma.  Numerics as b200vit_attention_window_relpos: fp32 scores, exp2 with scale*log2(e) folded in,
+ * probabilities rounded to bf16, fp32 accumulation, one bf16 rounding of the output.
+ * dh = 32, lh % rh == 0, lw % rw == 0, wh <= W, ww <= W, wh*ww + 1 <= 256, H <= 65535; every pointer 16-byte aligned.
+ * Isolation: a window's outputs are computed from its own rows only and nothing outside the B*(lh*lw + rh*rw) rows
+ * of qkv / out is read or written; a NaN or Inf stays within its window.
+ */
+int b200vit_attention_region_local(const void* qkv, void* out, const float* table, int B, int lh, int lw, int rh,
+                                   int rw, int W, int H, int dh, float scale, void* stream);
+
+/*
  * Squeeze-excitation around two bias-free GEMMs (max_vit.py:47-62):
  *   b200vit_se_pool:   pooled[b][c] bf16 = (sum_p part[b][p][c]) * inv_n, the parts added in index order (the mean of
  *                      b200vit_mbconv_dwconv's output); the gate then runs as GEMM(EPI_SILU), GEMM(EPI_SIGMOID) over

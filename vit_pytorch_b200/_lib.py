@@ -49,7 +49,7 @@ SYMBOLS = [
     "b200vit_attention_posbias", "b200vit_attention_window_relpos", "b200vit_mbconv_dwconv", "b200vit_se_pool",
     "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw", "b200vit_mbconv_dwconv_ex",
     "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex", "b200vit_attention_window_token",
-    "b200vit_window_mix", "b200vit_head_layernorm_gelu",
+    "b200vit_window_mix", "b200vit_head_layernorm_gelu", "b200vit_attention_region_local",
 ]
 
 
@@ -180,6 +180,8 @@ def lib() -> C.CDLL:
     L.b200vit_window_mix.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_head_layernorm_gelu.restype = i32
     L.b200vit_head_layernorm_gelu.argtypes = [vp, i64, vp, vp, i32, i32, i32, f32, vp]
+    L.b200vit_attention_region_local.restype = i32
+    L.b200vit_attention_region_local.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_se_pool.restype = i32
     L.b200vit_se_pool.argtypes = [vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_se_scale.restype = i32
@@ -770,6 +772,27 @@ def attention_window_token(qkv: torch.Tensor, tok_qkv: torch.Tensor, out: torch.
         rc = lib().b200vit_attention_window_token(_ptr(qkv), _ptr(tok_qkv), _ptr(out), _ptr(tok_out), B, int(gh),
                                                   int(gw), int(p), H, dh, float(scale), _stream())
     _check(rc, "b200vit_attention_window_token")
+
+
+def attention_region_local(qkv: torch.Tensor, out: torch.Tensor, table: torch.Tensor, B: int, lh: int, lw: int,
+                           rh: int, rw: int, W: int, H: int, dh: int, scale: float) -> None:
+    """RegionViT's region-to-local attention (regionvit.py:167-176): qkv[B*lh*lw + B*rh*rw, 3*H*dh] packed q | k | v,
+    the local tokens (b, y, x) at rows (b*lh + y)*lw + x, then the region tokens (b, i, j) at rows
+    B*lh*lw + (b*rh + i)*rw + j; window (b, i, j) is that region token and the (lh/rh) x (lw/rw) local tokens of its
+    cell, attending together under table[H, (2W-1)^2] (the transposed local_rel_pos_bias weight) between local tokens;
+    out [same rows, H*dh]."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out"); _chk(table, torch.float32, "table")
+    I = H * dh
+    rows = B * (lh * lw + rh * rw)
+    assert qkv.is_contiguous() and out.is_contiguous() and table.is_contiguous()
+    assert qkv.shape == (rows, 3 * I) and out.shape == (rows, I) and table.shape == (H, (2 * W - 1) ** 2)
+    n = (lh // rh) * (lw // rw) + 1 if rh > 0 and rw > 0 else 0
+    with _Timed("attention_region_local", B=B, lh=lh, lw=lw, rh=rh, rw=rw, H=H, n=n,
+                bytes=(qkv.numel() + out.numel()) * 2 + table.numel() * 4,
+                flops=4.0 * B * rh * rw * H * n * n * dh):
+        rc = lib().b200vit_attention_region_local(_ptr(qkv), _ptr(out), _ptr(table), B, int(lh), int(lw), int(rh),
+                                                  int(rw), int(W), H, dh, float(scale), _stream())
+    _check(rc, "b200vit_attention_region_local")
 
 
 def window_mix(wqk: torch.Tensor, o: torch.Tensor, out: torch.Tensor, B: int, gh: int, gw: int, p: int, H: int,

@@ -40,51 +40,6 @@ struct WinTokParams {
   float scale_log2e;
 };
 
-// the plain softmax of a 64 x 64 score tile in place, keys c >= n dropped; l: this thread's two row sums
-__device__ __forceinline__ void tile_softmax(float (&s)[32], float (&l)[2], int n, float scale_log2e, int lane) {
-  float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-  for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int c = 8 * jj + 2 * (lane & 3) + (e & 1);
-      s[4 * jj + e] = c < n ? s[4 * jj + e] * scale_log2e : -INFINITY;
-      mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * jj + e]);
-    }
-#pragma unroll
-  for (int rh = 0; rh < 2; ++rh) {
-    mx[rh] = fmaxf(mx[rh], __shfl_xor_sync(0xffffffffu, mx[rh], 1));
-    mx[rh] = fmaxf(mx[rh], __shfl_xor_sync(0xffffffffu, mx[rh], 2));
-    l[rh] = 0.f;
-  }
-#pragma unroll
-  for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float v = fast_ex2(s[4 * jj + e] - mx[e >> 1]);
-      s[4 * jj + e] = v;
-      l[e >> 1] += v;
-    }
-#pragma unroll
-  for (int rh = 0; rh < 2; ++rh) {
-    l[rh] += __shfl_xor_sync(0xffffffffu, l[rh], 1);
-    l[rh] += __shfl_xor_sync(0xffffffffu, l[rh], 2);
-  }
-}
-
-template <int DH>
-__device__ __forceinline__ void zero_acc(float (&o)[Slabs<DH>::N64 > 0 ? Slabs<DH>::N64 : 1][32],
-                                         float (&o16)[Slabs<DH>::N16 > 0 ? Slabs<DH>::N16 : 1][8]) {
-#pragma unroll
-  for (int c = 0; c < Slabs<DH>::N64; ++c)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
-#pragma unroll
-  for (int c = 0; c < Slabs<DH>::N16; ++c)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o16[c][i] = 0.f;
-}
-
 template <int DH>
 __global__ void __launch_bounds__(THREADS)
 attention_window_token_kernel(const WinTokParams p) {

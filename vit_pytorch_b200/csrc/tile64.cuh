@@ -1,5 +1,5 @@
 // The 64-row operand tile of the wgmma attention kernels that compute one 64 x 64 score block at a time
-// (attention_tile64.cu, levit.cu, twins.cu's attention_kv).  An operand block is 64 rows of one head's D columns:
+// (attention_tile64.cu, levit.cu, twins.cu's attention_kv, sep_vit.cu, regionvit.cu).  An operand block is 64 rows of one head's D columns:
 // D / 64 slabs 64 columns wide with the 128B swizzle, then (D % 64) / 16 slabs 16 columns wide with the 32B swizzle.
 // TMA boxes of 64 or 16 columns land in a slab as they are; cp.async gathers place 16-byte pieces at piece_addr.
 // S = Q K^T reads Q and K blocks as K-major operands; O += P V takes P (bf16) from registers as the A operand and V as
@@ -88,6 +88,66 @@ __device__ __forceinline__ void pv_mma(float (&o)[Slabs<DV>::N64 > 0 ? Slabs<DV>
       wgmma_m64n16k16_rs_tb(o16[c], a,
                             make_wgmma_desc_lbo(sv + S::N64 * S::S64 + c * S::S16 + kk * 512, 256, 256, WGMMA_SW32));
   }
+}
+
+// this thread's two row maxima, resp. row sums (rh), reduced over the four lanes that hold the row
+__device__ __forceinline__ void quad_max(float (&mx)[2]) {
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh) {
+    mx[rh] = fmaxf(mx[rh], __shfl_xor_sync(0xffffffffu, mx[rh], 1));
+    mx[rh] = fmaxf(mx[rh], __shfl_xor_sync(0xffffffffu, mx[rh], 2));
+  }
+}
+__device__ __forceinline__ void quad_sum(float (&l)[2]) {
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh) {
+    l[rh] += __shfl_xor_sync(0xffffffffu, l[rh], 1);
+    l[rh] += __shfl_xor_sync(0xffffffffu, l[rh], 2);
+  }
+}
+
+// s <- exp2(s - mx) over a 64 x 64 score block in log2 units (s[4 jj + e]: row half e >> 1); l += this thread's part
+// of each row's sum
+__device__ __forceinline__ void tile_exp2(float (&s)[32], const float (&mx)[2], float (&l)[2]) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float v = fast_ex2(s[4 * jj + e] - mx[e >> 1]);
+      s[4 * jj + e] = v;
+      l[e >> 1] += v;
+    }
+}
+
+// the plain softmax of a 64 x 64 score tile in place, keys c >= n dropped; l: this thread's two row sums
+__device__ __forceinline__ void tile_softmax(float (&s)[32], float (&l)[2], int n, float scale_log2e, int lane) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = 8 * jj + 2 * (lane & 3) + (e & 1);
+      s[4 * jj + e] = c < n ? s[4 * jj + e] * scale_log2e : -INFINITY;
+      mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * jj + e]);
+    }
+  quad_max(mx);
+  l[0] = l[1] = 0.f;
+  tile_exp2(s, mx, l);
+  quad_sum(l);
+}
+
+// O accumulators (pv_mma's) set to zero
+template <int DH>
+__device__ __forceinline__ void zero_acc(float (&o)[Slabs<DH>::N64 > 0 ? Slabs<DH>::N64 : 1][32],
+                                         float (&o16)[Slabs<DH>::N16 > 0 ? Slabs<DH>::N16 : 1][8]) {
+#pragma unroll
+  for (int c = 0; c < Slabs<DH>::N64; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
+#pragma unroll
+  for (int c = 0; c < Slabs<DH>::N16; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o16[c][i] = 0.f;
 }
 
 // this thread's two output rows (rh) of O, scaled by inv, to op (the row's first column of this head)

@@ -139,6 +139,9 @@ GROUPS_WIDTHS = (8,)                       # b200vit_attention_groups
 GROUPS_MAX_TOKENS = _lib.ATTN_GROUPS_MAX_TOKENS    # b200vit_attention_groups: tokens of one group
 WINDOW_TOKEN_MAX_WINDOW = 7                # b200vit_attention_window_token: p*p tokens + the window token <= 64
 WINDOW_MIX_MAX_WINDOWS = 64                # b200vit_window_mix: windows of one map
+REGION_LOCAL_WIDTHS = (32,)                # b200vit_attention_region_local
+REGION_LOCAL_MAX_TOKENS = 256              # b200vit_attention_region_local: a window's local tokens + its region token
+REGION_MAX_TOKENS = 512                    # b200vit_attention over one image's region tokens
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -302,6 +305,15 @@ class WindowTokenBlock(NamedTuple):
     window: int
 
 
+class RegionLocalBlock(NamedTuple):
+    """RegionViT's region-to-local attention (R2LTransformer, regionvit.py:114-190): the layer's attention runs over
+    the region tokens alone, then inside every window of local tokens together with the window's region token, with
+    the learned relative-position bias `bias` between local tokens (b200vit_attention, then
+    b200vit_attention_region_local); `window` is the W the bias table was built for, (2W-1)^2 offsets."""
+    bias: torch.Tensor                            # local_rel_pos_bias.weight [(2W-1)^2, heads], a parameter
+    window: int
+
+
 @dataclass
 class EncoderLayer:
     """One pre-LN encoder layer as a model family describes it to the engine (reference vit.py:78-81):
@@ -365,15 +377,22 @@ class EncoderLayer:
     # attention inside non-overlapping window x window blocks with one learned window token each, then across the
     # windows (SepViT's DSSA, sep_vit.py:65-206); run_blocks needs `grid`
     window_token: Optional[WindowTokenBlock] = None
+    # region-to-local attention over a stream of local token rows followed by region token rows (RegionViT's
+    # R2LTransformer, regionvit.py:163-186); run_blocks needs `grid` (the local map) and `regions` (the region map)
+    region_local: Optional[RegionLocalBlock] = None
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
     """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'window_relpos' (windows with a
     relative-position bias), 'kv' (sub-sampled keys: a strided convolution or CvT's convolutional projections),
     'groups' (strided patch groups), 'window_token' (SepViT's windows with a window token, then across windows), 'axial' (a run_blocks call with `axial`, unless the layer's temporal sub-block runs
-    there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys) or 'plain'.  ValueError for
-    cross-covariance, head-mixing, windowed, patch-group or sub-sampled-key attention with `axial` or over a `packed`
-    batch."""
+    there), 'region_local' (RegionViT's regional, then region-to-local attention), 'varlen' (`key_blocks`: a packed
+    batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed, patch-group,
+    region-to-local or sub-sampled-key attention with `axial` or over a `packed` batch."""
+    if L.region_local is not None:
+        if axial or packed:
+            raise ValueError("region-to-local attention runs over B local and region token maps only")
+        return "region_local"
     if L.window_token is not None:
         if axial or packed:
             raise ValueError("window-token attention runs over B token grids only")
@@ -396,6 +415,35 @@ def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False,
     if axial and L.temporal is None:
         return "axial"
     return "varlen" if key_blocks else "plain"
+
+
+def region_local_reason(lh: int, lw: int, rh: int, rw: int, W: int) -> Optional[str]:
+    """None if an lh x lw local map and an rh x rw region map run region-to-local attention with a bias table built for
+    window_size W, else the reason."""
+    if lh % rh or lw % rw:
+        return f"the {lh} x {lw} local map does not split into the {rh} x {rw} region map"
+    wh, ww = lh // rh, lw // rw
+    if wh > W or ww > W:
+        return f"a {wh} x {ww} window is larger than window_size={W} of the relative-position bias"
+    if wh * ww + 1 > REGION_LOCAL_MAX_TOKENS:
+        return (f"a {wh} x {ww} window of {wh * ww} local tokens (the region-to-local attention kernel takes at most "
+                f"{REGION_LOCAL_MAX_TOKENS - 1})")
+    if rh * rw > REGION_MAX_TOKENS:
+        return f"a {rh} x {rw} region map (regional attention takes at most {REGION_MAX_TOKENS} tokens)"
+    return None
+
+
+def region_local_check(L: EncoderLayer, grid, regions, B: int, N: int, rows: int) -> None:
+    """ValueError unless run_blocks' arguments describe B local maps `grid` (N tokens each) followed by B region maps
+    `regions` in `rows` rows that layer L's region-to-local attention can run on."""
+    if grid is None or regions is None or grid[0] * grid[1] != N:
+        raise ValueError("region-to-local attention needs `grid` = (h, w) with h * w == N and `regions` = (rh, rw)")
+    if rows != B * (N + regions[0] * regions[1]):
+        raise ValueError(f"x has {rows} rows, not the B * (N + rh * rw) = {B * (N + regions[0] * regions[1])} of B "
+                         f"local and region maps")
+    r = region_local_reason(grid[0], grid[1], regions[0], regions[1], L.region_local.window)
+    if r is not None:
+        raise ValueError(r)
 
 
 class _Prepared:
@@ -544,6 +592,8 @@ class TransformerEngine:
             r = (xca_reason(L.dim_head) if kernel == "xca" else
                  headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else
                  groups_reason(L.dim_head) if kernel == "groups" else head_width_reason(L.dim_head))
+            if r is None and kernel == "region_local" and L.dim_head not in REGION_LOCAL_WIDTHS:
+                r = f"dim_head={L.dim_head} (the region-to-local attention kernel is built for 32)"
             if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
                 r = lpi_reason(L.lpi.kernel_size, 1)
             if r is None and kernel == "window_relpos" and L.window ** 2 > WINDOW_MAX_TOKENS:
@@ -620,6 +670,8 @@ class TransformerEngine:
                 t[f"{i}.tok_qkv"] = (L.qkv_w.detach().float() @ T.token.detach().float()).to(torch.bfloat16)
                 t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"] = _f32(T.ln.gamma), _f32(T.ln.beta)
                 t[f"{i}.wqk.w"], t[f"{i}.wqk.b"] = _bf16_rows(T.wqk_w), _f32(T.wqk_b)
+            if L.region_local is not None:
+                t[f"{i}.r2l"] = L.region_local.bias.detach().float().t().contiguous()     # [heads, (2W-1)^2]
             if L.lpi is not None:
                 P = L.lpi
                 t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"] = _f32(P.ln.gamma), _f32(P.ln.beta)
@@ -721,7 +773,7 @@ class TransformerEngine:
                    rope: Optional[Tuple[torch.Tensor, int]] = None,
                    axial: Optional[Tuple[int, int, Optional[torch.Tensor], bool]] = None,
                    layers: Optional[Sequence[int]] = None, grid: Optional[Tuple[int, int]] = None,
-                   groups: Optional[Tuple[int, int]] = None) -> None:
+                   groups: Optional[Tuple[int, int]] = None, regions: Optional[Tuple[int, int]] = None) -> None:
         """The encoder layers (all, or the indices in `layers`, in order: CaiT's layer dropout, cait.py:14-27), in place
         on the fp32 residual stream x[M, D] (no final LayerNorm).  Attention runs over
         B sequences of N tokens (M = B*N) or, `varlen` given, over the packed sequences it describes (M = varlen.T).
@@ -741,7 +793,14 @@ class TransformerEngine:
         1 x 1 GEMMs, then attention_kv; the projections pad, so any h, w >= 1 will do.  Layers with patch-group attention
         (MobileViT) need `groups` = (ph, pw) dividing `grid` as well (attention_groups).  Layers with window-token attention
         (SepViT) need `grid` cut into at most 64 windows: attention_window_token into o, and with more than one window
-        head_layernorm_gelu, the window q | k GEMM and window_mix into ws['o2'], which the out-projection then reads.  A layer's feed-forward block
+        head_layernorm_gelu, the window q | k GEMM and window_mix into ws['o2'], which the out-projection then reads.
+        Layers with region-to-local attention (RegionViT) take x = B*N local rows (the `grid` maps, N = h*w) followed
+        by the B*rh*rw rows of the `regions` = (rh, rw) maps, and run the QKV GEMM, attention over each image's region
+        tokens and the out-projection residual on the region rows alone (pointer offsets into x, its bf16 copy and its
+        statistics), then the QKV GEMM over all rows and attention_region_local; the windows are (h/rh) x (w/rw) local
+        tokens, at most 255.  In fold mode the region residual writes the region rows' statistics where the next QKV
+        GEMM reads them; right after a rowstats_cast prime (one part per row) the region rows take the exact LayerNorm
+        and one rowstats_cast of the region rows writes their statistics instead.  A layer's feed-forward block
         applies its `ff_act`.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
         axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
         onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
@@ -784,6 +843,8 @@ class TransformerEngine:
                 if (grid[0] // p) * (grid[1] // p) > WINDOW_MIX_MAX_WINDOWS:
                     raise ValueError(f"a {grid[0]} x {grid[1]} grid has more than {WINDOW_MIX_MAX_WINDOWS} "
                                      f"{p} x {p} windows")
+            if kernels[-1] == "region_local":
+                region_local_check(L, grid, regions, B, N, x.shape[0])
             if kernels[-1] in ("window", "window_relpos", "kv"):
                 if grid is None or grid[0] * grid[1] != N:
                     raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
@@ -863,6 +924,34 @@ class TransformerEngine:
             _lib.gemm(akv, t[f"{i}.kv.w"], out_bf16=kv)
             _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
 
+        def region_local(L: EncoderLayer, i: int) -> None:
+            """RegionViT's regional attention on the region rows (x[B*N:]) with its residual, then the QKV GEMM over
+            all rows and the region-to-local attention into o."""
+            nonlocal sums
+            Ml, (rh, rw) = B * N, regions
+            xr, xbr = x[Ml:], xb[Ml:]
+            if fold and sums is None:
+                sums = ws["stats_in"]
+                _lib.rowstats_cast(x, xb, sums)
+            # the residual GEMMs' statistics: the folded GEMM reads them from row Ml on.  A rowstats_cast prime (one
+            # part per row) is read there only 8 bytes per row in, which the GEMM's 16-byte rule does not allow for odd
+            # Ml: the region rows then take the exact LayerNorm, and their new statistics a rowstats_cast
+            gemm_stats = fold and sums is not ws["stats_in"]
+            if gemm_stats:
+                _lib.gemm(xbr, t[f"{i}.qkv.wg"], out_bf16=qkv[Ml:], bias=t[f"{i}.qkv.t"], ln_sums=sums[Ml:],
+                          col_s=t[f"{i}.qkv.s"], ln_eps=L.ln1.eps)
+            else:
+                _lib.layernorm(xr, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xbr, eps=L.ln1.eps)
+                _lib.gemm(xbr, t[f"{i}.qkv.w"], out_bf16=qkv[Ml:])
+            _lib.attention(qkv[Ml:], o[Ml:], B, rh * rw, L.heads, L.dim_head, L.scale)
+            _lib.gemm(o[Ml:], t[f"{i}.out.w"], out_f32=xr, out_bf16=xbr if gemm_stats else None, bias=t[f"{i}.out.b"],
+                      resid=xr, stats_out=sums[Ml:] if gemm_stats else None)
+            if fold and not gemm_stats:
+                _lib.rowstats_cast(xr, xbr, sums[Ml:])
+            normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv)
+            _lib.attention_region_local(qkv, o, t[f"{i}.r2l"], B, grid[0], grid[1], rh, rw, L.region_local.window,
+                                        L.heads, L.dim_head, L.scale)
+
         def window_token(L: EncoderLayer, i: int) -> torch.Tensor:
             """SepViT's DSSA after its QKV projection: the windows' attention with their window token into o; with more
             than one window, the window tokens' outputs -> LayerNorm + GELU -> their q | k GEMM -> the attention across
@@ -913,6 +1002,8 @@ class TransformerEngine:
             attn_out = o
             if kernel == "kv":
                 subsampled(L, i)
+            elif kernel == "region_local":
+                region_local(L, i)
             else:
                 normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv, **head)
                 if rope is not None:
