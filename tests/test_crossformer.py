@@ -132,17 +132,17 @@ def test_stage_maps_match_the_convolutions():
 
 
 # ------------------------------------------------------------------------------------------------ engine description
-def test_engine_description_of_the_readme_config():
+def test_window_records_of_the_readme_config():
     m = CrossFormer(**README)
     layers = [L for _, t in m.layers for L in t.encoder_layers()[0]]
     assert len(layers) == 28
-    assert [L.grid_windows for L in layers] == [False, True] * 14
-    wins = [(L.window, L.grid_windows) for _, t in m.layers for L in t.encoder_layers()[0][:2]]
+    assert [L.attention.dilated for L in layers] == [False, True] * 14
+    wins = [(L.attention.size, L.attention.dilated) for _, t in m.layers for L in t.encoder_layers()[0][:2]]
     assert wins == [(7, False), (8, True), (7, False), (4, True), (7, False), (2, True), (7, False), (1, True)]
     assert {attention_kernel(L) for L in layers} == {"window_relpos"}
     assert [(L.heads, L.dim_head) for L in layers[::4]][:4] == [(2, 32), (4, 32), (8, 32), (8, 32)]
     L = layers[0]
-    assert L.rel_pos_bias.shape == (13 * 13, 2) and L.qkv_w.shape == (192, 64) and L.out_w.shape == (64, 64)
+    assert L.attention.rel_pos_bias.shape == (13 * 13, 2) and L.qkv_w.shape == (192, 64) and L.out_w.shape == (64, 64)
     assert L.fc1_w.shape == (256, 64) and L.fc2_w.shape == (64, 256) and L.ln1.eps == 1e-5
 
 
@@ -160,7 +160,7 @@ def eligible(monkeypatch):
     monkeypatch.setattr(cf, "common_reason", lambda *a, **k: None)
 
 
-def test_fused_reason_rules(eligible):
+def test_fused_reason_rules_with_the_engine_window_limit(eligible):
     img = lambda h, w, c=3: torch.zeros(2, c, h, w)                        # noqa: E731
     mk = lambda **kw: CrossFormer(**dict(SMALL, **kw)).eval()               # noqa: E731
     m = mk()
@@ -169,8 +169,8 @@ def test_fused_reason_rules(eligible):
     assert "not (B, 3, H, W)" in m.fused_reason(torch.zeros(3, 64, 64))
     assert "not (B, 3, H, W)" in m.fused_reason(img(64, 64, c=1))
     assert mk(channels=1).fused_reason(img(64, 64, c=1)) is None
-    assert "local window 9" in mk(local_window_size=9).fused_reason(img(576, 576))
-    assert "global window 9" in mk(global_window_size=(9, 1, 1, 1)).fused_reason(img(576, 576))
+    assert "window_size=9: a window of 81 tokens" in mk(local_window_size=9).fused_reason(img(576, 576))
+    assert "window_size=9: a window of 81 tokens" in mk(global_window_size=(9, 1, 1, 1)).fused_reason(img(576, 576))
     assert "not divisible" in m.fused_reason(img(48, 48))
     assert "not divisible" in mk(global_window_size=(3, 1, 1, 1)).fused_reason(img(64, 64))
     assert "torch.cat raises" in mk(cross_embed_kernel_sizes=((4, 8), (2, 3), (2, 4), (2, 4))).fused_reason(

@@ -118,18 +118,19 @@ def test_map_geometry_matches_the_convolutions(k, s, h, w):
 
 
 # ------------------------------------------------------------------------------------------------ engine
-def test_encoder_layers_describe_conv_projections():
+def test_encoder_layers_carry_conv_projection_records():
     m = CvT(**INIT_KWARGS).eval()
     layers, norm = m.layers[2][2].encoder_layers()
     assert norm is None and len(layers) == 2
     a = m.layers[2][2].layers[0][0]
     L = layers[0]
-    assert attention_kernel(L) == "kv" and L.kv_stride is None and L.window is None
-    assert L.qkv_w.shape == (128, 48) and L.kv_w.shape == (256, 48) and L.out_w.shape == (48, 128)
-    assert L.conv_proj.kernel_size == 3 and L.conv_proj.stride == 2 and L.conv_proj.q_bn_var is a.to_q.net[1].running_var
+    assert attention_kernel(L) == "kv" and isinstance(L.attention, ConvProj)
+    assert L.qkv_w.shape == (128, 48) and L.attention.kv_proj_w.shape == (256, 48) and L.out_w.shape == (48, 128)
+    assert L.attention.kernel_size == 3 and L.attention.stride == 2
+    assert L.attention.q_bn_var is a.to_q.net[1].running_var
     assert L.heads == 2 and L.dim_head == 64 and L.scale == a.scale
     eng = m.layers[2][2].engine()
-    assert eng.unsupported_reason(49) is None
+    assert eng.unsupported_reason(49, grid=(7, 7)) is None
     t = eng.prepared()
     assert t["0.cpq.w"].shape == (9, 48) and t["0.cpkv.b"].shape == (48,) and t["0.kv.w"].shape == (256, 48)
     assert t["0.kv.w"].dtype == torch.bfloat16 and t["c_layers"] is None

@@ -136,13 +136,14 @@ def test_kernel_bias_index_reproduces_rel_pos_indices(w):
     assert torch.equal(idx, a.rel_pos_indices)
 
 
-def test_encoder_layers_describe_block_then_grid_windows():
+def test_window_records_describe_block_then_grid_windows():
     m = MaxViT(**INIT_KWARGS).eval()
     layers, norm = m._encoders()[1].encoder_layers()
-    assert norm is None and [L.grid_windows for L in layers] == [False, True]
+    assert norm is None and [L.attention.dilated for L in layers] == [False, True]
     a = m.layers[1][2].fn
     L = layers[0]
-    assert L.window == 2 and L.rel_pos_bias is a.rel_pos_bias.weight and L.out_b is None and L.scale == a.scale
+    assert L.attention.size == 2 and L.attention.rel_pos_bias is a.rel_pos_bias.weight
+    assert L.out_b is None and L.scale == a.scale
     from vit_pytorch_b200.engine import attention_kernel
     assert [attention_kernel(L) for L in layers] == ["window_relpos"] * 2
     engines = [e.engine() for e in m._encoders()]

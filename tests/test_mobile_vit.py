@@ -14,7 +14,7 @@ import torch
 
 from conftest import GOLDEN_DIR, ROOT
 from vit_pytorch_b200 import _lib, build, mobile_vit as mvit
-from vit_pytorch_b200.engine import attention_kernel
+from vit_pytorch_b200.engine import PatchGroups, attention_kernel
 from vit_pytorch_b200.mobile_vit import MobileViT, conv_bn_weights, from_groups, to_groups
 
 sys.path.insert(0, GOLDEN_DIR)
@@ -124,21 +124,21 @@ def test_fused_reason_hooks(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ engine description
-def test_engine_describes_the_readme_config():
+def test_patch_group_records_of_the_readme_config():
     torch.manual_seed(0)
     m = MobileViT(**README).eval()
     for (_, blk), depth, dim, mlp in zip(m.trunk, (2, 4, 3), (96, 120, 144), (192, 480, 576)):
         layers, norm = blk.transformer.encoder_layers()
         assert norm is None and len(layers) == depth
         for L in layers:
-            assert (L.heads, L.dim_head, L.ff_act, L.patch_groups) == (4, 8, "silu", True)
+            assert (L.heads, L.dim_head, L.ff_act, L.attention) == (4, 8, "silu", PatchGroups())
             assert L.scale == 8 ** -0.5 and L.qkv_w.shape == (96, dim) and L.fc1_w.shape == (mlp, dim)
             assert attention_kernel(L) == "groups"
             with pytest.raises(ValueError):
                 attention_kernel(L, axial=True)
         assert (blk.ph, blk.pw) == (2, 2)
         eng = blk.transformer.engine()
-        assert eng.unsupported_reason(256) is None
+        assert eng.unsupported_reason(256, grid=(16, 16), groups=(2, 2)) is None
         assert eng.prepared()["c_layers"] is None                 # the per-kernel loop
     assert m.block_maps(256, 256) == [(32, 32), (16, 16), (8, 8)]
 

@@ -186,7 +186,7 @@ def test_fused_reason_names_dtype_device_and_hooks(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ engine description
-def test_engine_describes_the_readme_config():
+def test_region_local_records_of_the_readme_config():
     torch.manual_seed(0)
     m = RegionViT().eval()
     assert m.stage_maps(224, 224) == [(56, 56, 8, 8), (28, 28, 4, 4), (14, 14, 2, 2), (7, 7, 1, 1)]
@@ -197,7 +197,7 @@ def test_engine_describes_the_readme_config():
         for L in layers:
             assert (L.heads, L.dim_head, L.scale) == (4, 32, 32 ** -0.5)
             assert L.qkv_w.shape == (3 * 128, dim) and L.fc1_w.shape == (4 * dim, dim)
-            assert L.region_local.window == 7 and L.region_local.bias is tr.local_rel_pos_bias.weight
+            assert L.attention.window == 7 and L.attention.bias is tr.local_rel_pos_bias.weight
             assert attention_kernel(L) == "region_local"
             with pytest.raises(ValueError):
                 attention_kernel(L, axial=True)

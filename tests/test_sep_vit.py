@@ -170,7 +170,7 @@ def test_fused_reason_names_dtype_device_and_hooks(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ engine description
-def test_engine_describes_the_readme_config():
+def test_window_token_records_of_the_readme_config():
     torch.manual_seed(0)
     m = SepViT(**README).eval()
     assert m.stage_maps(224, 224) == [(56, 56), (28, 28), (14, 14), (7, 7)]
@@ -180,16 +180,16 @@ def test_engine_describes_the_readme_config():
         for L in layers:
             assert (L.heads, L.dim_head, L.scale) == (heads, 32, 32 ** -0.5)
             assert L.qkv_w.shape == (3 * heads * 32, dim) and L.fc1_w.shape == (4 * dim, dim)
-            assert L.window_token.window == 7 and L.window_token.wqk_w.shape == (2 * heads * 32, heads * 32)
+            assert L.attention.window == 7 and L.attention.wqk_w.shape == (2 * heads * 32, heads * 32)
             assert attention_kernel(L) == "window_token"
             with pytest.raises(ValueError):
                 attention_kernel(L, axial=True)
         eng = tr.engine()
-        assert eng.unsupported_reason(56 * 56) is None
+        assert eng.unsupported_reason(56 * 56, grid=(56, 56)) is None
         t = eng.prepared()
         assert t["c_layers"] is None                                   # the per-kernel loop
         L, W = layers[0], layers[0].qkv_w.float()
-        assert torch.equal(t["0.tok_qkv"], (W @ L.window_token.token.float()).bfloat16())
+        assert torch.equal(t["0.tok_qkv"], (W @ L.attention.token.float()).bfloat16())
 
 
 def test_run_blocks_rejects_grids_before_touching_x(monkeypatch):

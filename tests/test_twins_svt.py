@@ -15,7 +15,7 @@ import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR, ROOT
 from vit_pytorch_b200 import _lib, build, twins_svt as tw
-from vit_pytorch_b200.engine import attention_kernel
+from vit_pytorch_b200.engine import StridedKV, Windows, attention_kernel
 from vit_pytorch_b200.twins_svt import PEG, PatchEmbedding, Transformer, TwinsSVT, merge_weights, peg_weights
 
 sys.path.insert(0, GOLDEN_DIR)
@@ -55,12 +55,13 @@ def test_attribute_surface():
                                                                        if k.startswith("layers.3."))
 
 
-def test_encoder_layers_describe_two_pairs_per_layer():
+def test_encoder_layers_carry_window_and_strided_kv_records():
     t = Transformer(16, 2, local_patch_size=4, global_k=3).eval()
     layers, norm = t.encoder_layers()
     assert norm is None and [attention_kernel(L) for L in layers] == ["window", "kv", "window", "kv"]
-    assert layers[0].window == 4 and layers[0].qkv_w.shape == (3 * 512, 16) and layers[0].kv_w is None
-    assert layers[1].kv_stride == 3 and layers[1].qkv_w.shape == (512, 16) and layers[1].kv_w.shape == (1024, 16, 3, 3)
+    assert layers[0].attention == Windows(4) and layers[0].qkv_w.shape == (3 * 512, 16)
+    assert isinstance(layers[1].attention, StridedKV) and layers[1].attention.stride == 3
+    assert layers[1].qkv_w.shape == (512, 16) and layers[1].attention.kv_w.shape == (1024, 16, 3, 3)
     assert torch.equal(layers[0].qkv_w[512:], t.layers[0][0].fn.to_kv.weight.reshape(1024, 16))
     assert [attention_kernel(L) for L in Transformer(16, 1, has_local=False).encoder_layers()[0]] == ["kv"]
     with pytest.raises(ValueError):

@@ -148,7 +148,7 @@ class Transformer(FusedTransformer):
                 out_w=out.weight, out_b=out.bias,
                 ln2=Norm.of(ff.net[0]), fc1_w=fc1.weight, fc1_b=fc1.bias, fc2_w=fc2.weight, fc2_b=fc2.bias,
                 heads=attn.heads, dim_head=attn.dim_head, scale=float(attn.scale),
-                headmix=HeadMix(post=attn.mix_heads_post_attn, ln=None, pre=attn.mix_heads_pre_attn),
+                attention=HeadMix(post=attn.mix_heads_post_attn, ln=None, pre=attn.mix_heads_pre_attn),
                 out_scale=ls_attn.scale, ff_scale=ls_ff.scale))
         return layers, None
 

@@ -36,7 +36,7 @@ from torch import einsum, nn
 
 from . import _lib
 from .cct import CONV_MAX_KERNEL
-from .engine import (WINDOW_MAX_TOKENS, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _bf16_rows, _f32, cached,
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, Windows, _bf16_rows, _f32, cached,
                      common_reason, head_engine, on_device)
 from .max_vit import _MeanHW
 
@@ -301,8 +301,8 @@ class Transformer(FusedEncoder, nn.Module):
                     ln1=_norm(a.norm), qkv_w=a.to_qkv.weight.reshape(3 * I, D),
                     out_w=a.to_out.weight.reshape(D, I), out_b=a.to_out.bias, ln2=_norm(f[0]),
                     fc1_w=f[1].weight.reshape(-1, D), fc1_b=f[1].bias, fc2_w=f[4].weight.reshape(D, -1),
-                    fc2_b=f[4].bias, heads=a.heads, dim_head=I // a.heads, scale=a.scale, window=a.window_size,
-                    rel_pos_bias=dpb_table(a), grid_windows=a.attn_type == 'long'))
+                    fc2_b=f[4].bias, heads=a.heads, dim_head=I // a.heads, scale=a.scale,
+                    attention=Windows(a.window_size, rel_pos_bias=dpb_table(a), dilated=a.attn_type == 'long')))
         return layers, None
 
 
@@ -444,13 +444,10 @@ class CrossFormer(FusedWeightsMixin, nn.Module):
                 return f"stage {i + 1}: the map of a {img.shape[2]} x {img.shape[3]} image is empty"
             for name, a in (("local", t.layers[0][0]), ("global", t.layers[0][2])):
                 ws = a.window_size
-                if ws * ws > WINDOW_MAX_TOKENS:
-                    return (f"stage {i + 1}: {name} window {ws} (the relative-position window attention kernel takes "
-                            f"at most {WINDOW_MAX_TOKENS} tokens)")
                 if h % ws or w % ws:
                     return (f"stage {i + 1}: the {h} x {w} map is not divisible into {name} {ws} x {ws} windows (the "
                             f"reference raises)")
-            r = t.engine().unsupported_reason(h * w)
+            r = t.engine().unsupported_reason(h * w, grid=(h, w))
             if r is not None:
                 return r
         return None

@@ -174,7 +174,7 @@ class Transformer(FusedEncoder, nn.Module):
         return x
 
     def encoder_layers(self) -> Tuple[List[EncoderLayer], Optional[Norm]]:
-        """One EncoderLayer per (Attention, FeedForward) pair, with `conv_proj`: qkv_w the queries' 1 x 1 rows, kv_w
+        """One EncoderLayer per (Attention, FeedForward) pair, with ConvProj: qkv_w the queries' 1 x 1 rows, kv_proj_w
         the keys' and values' (rows k | v, the order of chunk(2, dim=1))."""
         layers = []
         for a, ff in self.layers:
@@ -185,12 +185,12 @@ class Transformer(FusedEncoder, nn.Module):
             P = ConvProj(q_w=dq.weight, q_bn_w=bq.weight, q_bn_b=bq.bias, q_bn_mean=bq.running_mean,
                          q_bn_var=bq.running_var, q_bn_eps=bq.eps, kv_w=dkv.weight, kv_bn_w=bkv.weight,
                          kv_bn_b=bkv.bias, kv_bn_mean=bkv.running_mean, kv_bn_var=bkv.running_var, kv_bn_eps=bkv.eps,
-                         kernel_size=dq.kernel_size[0], stride=dkv.stride[0])
+                         kernel_size=dq.kernel_size[0], stride=dkv.stride[0], kv_proj_w=pkv.weight.reshape(2 * I, D))
             layers.append(EncoderLayer(
                 ln1=_norm(a.norm), qkv_w=pq.weight.reshape(I, D), out_w=a.to_out[0].weight.reshape(D, I),
                 out_b=a.to_out[0].bias, ln2=_norm(f[0]), fc1_w=f[1].weight.reshape(-1, D), fc1_b=f[1].bias,
                 fc2_w=f[4].weight.reshape(D, -1), fc2_b=f[4].bias, heads=a.heads, dim_head=I // a.heads,
-                scale=a.scale, kv_w=pkv.weight.reshape(2 * I, D), conv_proj=P))
+                scale=a.scale, attention=P))
         return layers, None
 
     def prepared_buffers(self) -> List[torch.Tensor]:
@@ -309,7 +309,7 @@ class CvT(FusedWeightsMixin, nn.Module):
                 return f"stage {i + 1}: the map of a {img.shape[2]} x {img.shape[3]} image is empty"
             # the engine's rules: proj_kernel 1, 3, 5 or 7 (an even one also makes the reference raise), dim_head,
             # at most 16384 tokens (and so keys) per map
-            r = stage[2].engine().unsupported_reason(h * w)
+            r = stage[2].engine().unsupported_reason(h * w, grid=(h, w))
             if r is not None:
                 return r
         return None

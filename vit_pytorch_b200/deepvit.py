@@ -97,7 +97,7 @@ class Transformer(FusedTransformer):
                 ln1=Norm.of(attn.norm), qkv_w=attn.to_qkv.weight, out_w=out.weight, out_b=out.bias,
                 ln2=Norm.of(ff.net[0]), fc1_w=fc1.weight, fc1_b=fc1.bias, fc2_w=fc2.weight, fc2_b=fc2.bias,
                 heads=attn.heads, dim_head=attn.dim_head, scale=float(attn.scale),
-                headmix=HeadMix(post=attn.reattn_weights, ln=Norm.of(attn.reattn_norm[1]))))
+                attention=HeadMix(post=attn.reattn_weights, ln=Norm.of(attn.reattn_norm[1]))))
         return layers, None
 
 

@@ -20,7 +20,7 @@ from __future__ import annotations
 import ctypes
 import os
 from dataclasses import dataclass
-from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import nn
@@ -181,14 +181,6 @@ def lpi_reason(kernel_size: int, grid_w: int) -> Optional[str]:
     return None
 
 
-def groups_reason(dh: int) -> Optional[str]:
-    """None if b200vit_attention_groups is built for heads `dh` wide, else the reason the eager PyTorch graph is
-    used."""
-    if dh not in GROUPS_WIDTHS:
-        return f"dim_head={dh} (the patch-group attention kernel is built for 8)"
-    return None
-
-
 class Norm(NamedTuple):
     """A LayerNorm over the feature dim.  beta None: the norm has no shift."""
     gamma: torch.Tensor
@@ -207,15 +199,6 @@ class AttnBlock(NamedTuple):
     qkv_w: torch.Tensor                            # [3 * heads * dim_head, D], rows q | k | v
     out_w: Optional[torch.Tensor]                  # None: to_out is the identity, as EncoderLayer.out_w
     out_b: Optional[torch.Tensor]
-
-
-class HeadMix(NamedTuple):
-    """Softmax probabilities mixed across the head axis (b200vit_attention_headmix; DeepViT's re-attention,
-    deepvit.py:61-62): post indexed [input head, output head], ln a LayerNorm over the heads of every (query, key)
-    pair after the mix; pre (CaiT's talking heads, cait.py:94) mixes the scores the same way before the softmax."""
-    post: torch.Tensor                            # [heads, heads]
-    ln: Optional[Norm]                            # over `heads` values, or None
-    pre: Optional[torch.Tensor] = None            # [heads, heads], or None
 
 
 class LPIBlock(NamedTuple):
@@ -253,11 +236,197 @@ def lpi_weights(P: LPIBlock) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, 
     return w1.t().contiguous(), b1.contiguous(), w2.t().contiguous(), b2.contiguous()
 
 
+# ------------------------------------------------------------------------------------------------ attention variants
+# EncoderLayer.attention is None (softmax attention over the layer's sequences) or one of the records below, each of
+# which holds its variant's parameters and what the engine knows about it:
+#   kernel, rejects   the name attention_kernel() reports, and its ValueError for `axial` or a packed batch
+#   reason(L)         why the kernels are not built for layer L's widths or window, or None
+#   geometry_reason(L, N, grid, groups, regions, rows)   why run_blocks' token geometry does not suit it, or None;
+#                     `rows` = (B, rows of x) in run_blocks, None in unsupported_reason
+#   prepare(t, i, L)  its prepared weights of layer i, into t
+#   launch(c, L, i)   its launches in the BlocksCall c up to the attention output; returns the buffer holding it
+#   o2 = True         (WindowTokenBlock only) launch() needs the workspace's second attention output
+
+
+class HeadMix(NamedTuple):
+    """Softmax probabilities mixed across the head axis (b200vit_attention_headmix; DeepViT's re-attention,
+    deepvit.py:61-62): post indexed [input head, output head], ln a LayerNorm over the heads of every (query, key)
+    pair after the mix; pre (CaiT's talking heads, cait.py:94) mixes the scores the same way before the softmax."""
+    post: torch.Tensor                            # [heads, heads]
+    ln: Optional[Norm]                            # over `heads` values, or None
+    pre: Optional[torch.Tensor] = None            # [heads, heads], or None
+    kernel = "headmix"
+    rejects = "head-mixing attention runs over B sequences of N tokens only"
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        return headmix_reason(L.heads, L.dim_head)
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        t[f"{i}.post"] = _f32(self.post)
+        if self.pre is not None:
+            t[f"{i}.pre"] = _f32(self.pre)
+        if self.ln is not None:
+            t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(self.ln.gamma), _f32(self.ln.beta)
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        c.project(L, i)
+        hln = None if self.ln is None else (c.t[f"{i}.hln.w"], c.t[f"{i}.hln.b"], self.ln.eps)
+        _lib.attention_headmix(c.qkv, c.o, c.B, c.N, L.heads, L.dim_head, L.scale, c.t[f"{i}.post"], hln,
+                               pre=c.t.get(f"{i}.pre"))
+        return c.o
+
+
+class CrossCovariance(NamedTuple):
+    """Cross-covariance attention (XCiT, xcit.py:109-148; b200vit_attention_xca) with the per-head temperature
+    exp(tau), read when the prepared weights are rebuilt."""
+    tau: torch.Tensor                             # the temperature parameter [heads, 1, 1]
+    kernel = "xca"
+    rejects = "cross-covariance attention runs over B sequences of N tokens only"
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        return xca_reason(L.dim_head)
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        t[f"{i}.tau"] = self.tau.detach().float().exp().reshape(-1).contiguous()
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        c.project(L, i)
+        _lib.attention_xca(c.qkv, c.t[f"{i}.tau"], c.o, c.B, c.N, L.heads, L.dim_head)
+        return c.o
+
+
+class Windows(NamedTuple):
+    """Attention inside non-overlapping size x size blocks of the token grid (Twins-SVT's LocalAttention,
+    twins_svt.py:85-120; b200vit_attention_window).  With `rel_pos_bias`, the Embedding weight [(2 size - 1)^2, heads],
+    a learned relative-position bias inside every window (MaxViT, max_vit.py:148-159; b200vit_attention_window_relpos);
+    `dilated` then cuts the map into dilated grids instead of contiguous blocks ('b d (w1 x) (w2 y)', max_vit.py:269).
+    run_blocks needs `grid`."""
+    size: int
+    rel_pos_bias: Optional[torch.Tensor] = None
+    dilated: bool = False
+    rejects = "windowed and sub-sampled-key attention run over B token grids only"
+
+    @property
+    def kernel(self) -> str:
+        return "window" if self.rel_pos_bias is None else "window_relpos"
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        r = head_width_reason(L.dim_head)
+        if r is None and self.size ** 2 > WINDOW_MAX_TOKENS:
+            name, what = ("local_patch_size", "window") if self.rel_pos_bias is None else \
+                ("window_size", "relative-position window")
+            r = (f"{name}={self.size}: a window of {self.size ** 2} tokens (the {what} attention kernel takes at "
+                 f"most {WINDOW_MAX_TOKENS})")
+        return r
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        if grid is None or grid[0] * grid[1] != N:
+            return "windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N"
+        if grid[0] % self.size or grid[1] % self.size:
+            return f"a {grid[0]} x {grid[1]} grid cannot be cut into {self.size} x {self.size} windows"
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        if self.rel_pos_bias is not None:
+            t[f"{i}.relpos"] = self.rel_pos_bias.detach().float().t().contiguous()
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        c.project(L, i)
+        if self.rel_pos_bias is None:
+            _lib.attention_window(c.qkv, c.o, c.B, c.grid[0], c.grid[1], self.size, L.heads, L.dim_head, L.scale)
+        else:
+            _lib.attention_window_relpos(c.qkv, c.o, c.t[f"{i}.relpos"], c.B, c.grid[0], c.grid[1], self.size,
+                                         self.dilated, L.heads, L.dim_head, L.scale)
+        return c.o
+
+
+class StridedKV(NamedTuple):
+    """Keys and values from a stride x stride, stride-`stride` convolution of the normalised token grid (Twins-SVT's
+    GlobalAttention, twins_svt.py:122-157; b200vit_attention_kv); EncoderLayer.qkv_w holds the query rows only.
+    run_blocks needs `grid`.  The LayerNorm cannot be folded into the key / value projection (one convolution window
+    spans tokens with different statistics): in both LayerNorm modes the layer runs layernorm(x -> xb), the query GEMM
+    on xb, conv_im2col_nhwc of xb and the key / value GEMM (stride 1: the GEMM on xb itself), then attention_kv."""
+    stride: int
+    kv_w: torch.Tensor                            # the Conv2d weight [2 * heads * dim_head, D, k, k], rows k | v
+    kernel = "kv"
+    rejects = Windows.rejects
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        return head_width_reason(L.dim_head)
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        if grid is None or grid[0] * grid[1] != N:
+            return "windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N"
+        if min(grid) < self.stride:
+            return f"a {grid[0]} x {grid[1]} grid cannot be cut into {self.stride} x {self.stride} key patches"
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
+        t[f"{i}.kv.w"] = _bf16_rows(self.kv_w.detach().permute(0, 2, 3, 1).reshape(self.kv_w.shape[0], -1))
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        x, xb, t, k = c.x, c.xb, c.t, self.stride
+        I, (gh, gw) = L.heads * L.dim_head, c.grid
+        kh, kw = gh // k, gw // k
+        _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
+        q = c.qkv[:, :I]
+        _lib.gemm(xb, t[f"{i}.qkv.w"], out_bf16=q)
+        if k == 1:
+            col = xb
+        else:
+            col = torch.empty(c.B * kh * kw, k * k * x.shape[1], device=x.device, dtype=torch.bfloat16)
+            _lib.conv_im2col_nhwc(xb, col, c.B, gh, gw, k, k, 0)
+        kv = torch.empty(c.B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
+        _lib.gemm(col, t[f"{i}.kv.w"], out_bf16=kv)
+        _lib.attention_kv(q, kv, c.o, c.B, c.N, kh * kw, L.heads, L.dim_head, L.scale)
+        return c.o
+
+
+class PatchGroups(NamedTuple):
+    """Attention inside the strided patch groups of the token grid, token (y'*ph + i, x'*pw + j) in group (i, j)
+    (MobileViT, mobile_vit.py:150; b200vit_attention_groups); run_blocks needs `grid` and `groups` = (ph, pw).  It has
+    no fields, so it is an empty tuple: test EncoderLayer.attention against None, never for truth."""
+    kernel = "groups"
+    rejects = "patch-group attention runs over B token grids only"
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        if L.dim_head not in GROUPS_WIDTHS:
+            return f"dim_head={L.dim_head} (the patch-group attention kernel is built for 8)"
+        return None
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        if grid is None or grid[0] * grid[1] != N or groups is None:
+            return "patch-group attention needs `grid` = (h, w) with h * w == N and `groups`"
+        if grid[0] % groups[0] or grid[1] % groups[1]:
+            return f"a {grid[0]} x {grid[1]} grid cannot be cut into {groups[0]} x {groups[1]} patches"
+        n = (grid[0] // groups[0]) * (grid[1] // groups[1])
+        if not 1 <= n <= GROUPS_MAX_TOKENS:
+            return f"{n} tokens per group (the patch-group attention kernel takes 1 to {GROUPS_MAX_TOKENS})"
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        pass
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        c.project(L, i)
+        _lib.attention_groups(c.qkv, c.o, c.B, c.grid[0], c.grid[1], c.groups[0], c.groups[1], L.heads, L.dim_head,
+                              L.scale)
+        return c.o
+
+
 class ConvProj(NamedTuple):
     """CvT's convolutional projections (cvt.py:51-60, 74-75) of the normalised h x w token grid: for the queries a
     depthwise k x k convolution at stride 1, for the keys / values one at stride `stride`, both bias-free with zero
     padding k // 2 and followed by a BatchNorm (eval, on its running statistics); the bias-free 1 x 1 convolutions
-    after them are EncoderLayer.qkv_w (queries) and kv_w (keys | values)."""
+    after them are EncoderLayer.qkv_w (queries) and kv_proj_w (keys | values).  The attention runs b200vit_conv_proj_dw,
+    then b200vit_attention_kv; run_blocks needs `grid`, of any h, w >= 1 (the projections pad)."""
     q_w: torch.Tensor                             # [D, 1, k, k]
     q_bn_w: torch.Tensor
     q_bn_b: torch.Tensor
@@ -272,10 +441,47 @@ class ConvProj(NamedTuple):
     kv_bn_eps: float
     kernel_size: int
     stride: int
+    kv_proj_w: Optional[torch.Tensor] = None      # [2 * heads * dim_head, D], rows k | v; an encoder layer needs it
+    kernel = "kv"
+    rejects = Windows.rejects
 
     def grid(self, h: int, w: int) -> Tuple[int, int]:
         """The (h, w) of the key / value map of an h x w token grid."""
         return (h - 1) // self.stride + 1, (w - 1) // self.stride + 1
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        r = head_width_reason(L.dim_head)
+        if r is None and self.kernel_size not in CONV_PROJ_KERNEL_SIZES:
+            r = f"proj_kernel={self.kernel_size} (the convolutional-projection kernel is built for 1, 3, 5 and 7)"
+        return r
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        if grid is None or grid[0] * grid[1] != N:
+            return "windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N"
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        # the depthwise halves with their BatchNorms folded (tap-major) and the keys' / values' 1 x 1 rows
+        t[f"{i}.cpq.w"], t[f"{i}.cpq.b"], t[f"{i}.cpkv.w"], t[f"{i}.cpkv.b"] = conv_proj_weights(self)
+        t[f"{i}.kv.w"] = _bf16_rows(self.kv_proj_w.reshape(self.kv_proj_w.shape[0], -1))
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        """layernorm(x -> xb), both depthwise projections of xb in one pass (the LayerNorm cannot be folded: the
+        padding taps must read zeros of the normalised map), the 1 x 1 GEMMs, attention_kv."""
+        x, xb, t = c.x, c.xb, c.t
+        I, D = L.heads * L.dim_head, x.shape[1]
+        kh, kw = self.grid(*c.grid)
+        _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
+        aq = torch.empty(x.shape[0], D, device=x.device, dtype=torch.bfloat16)
+        akv = torch.empty(c.B * kh * kw, D, device=x.device, dtype=torch.bfloat16)
+        _lib.conv_proj_dw(xb, t[f"{i}.cpq.w"], t[f"{i}.cpq.b"], t[f"{i}.cpkv.w"], t[f"{i}.cpkv.b"], aq, akv, c.B,
+                          c.grid[0], c.grid[1], self.kernel_size, self.stride)
+        q = c.qkv[:, :I]
+        _lib.gemm(aq, t[f"{i}.qkv.w"], out_bf16=q)
+        kv = torch.empty(c.B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
+        _lib.gemm(akv, t[f"{i}.kv.w"], out_bf16=kv)
+        _lib.attention_kv(q, kv, c.o, c.B, c.N, kh * kw, L.heads, L.dim_head, L.scale)
+        return c.o
 
 
 def conv_proj_weights(P: ConvProj) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -297,21 +503,139 @@ class WindowTokenBlock(NamedTuple):
     normalised; its per-head outputs pass `ln` (nn.LayerNorm(dim_head), shared by the heads), GELU and the 1 x 1
     convolution wqk_w [2I, I] + wqk_b over the heads' channels, whose output columns interleave per head (q of head h
     at [2h dh, 2h dh + dh), its k right after); softmax(scale wq wk^T) over the windows then mixes the windows' outputs
-    position by position (b200vit_attention_window_token, b200vit_head_layernorm_gelu, GEMM, b200vit_window_mix)."""
+    position by position (b200vit_attention_window_token, b200vit_head_layernorm_gelu, GEMM, b200vit_window_mix).
+    run_blocks needs `grid`, cut into at most 64 windows."""
     token: torch.Tensor                           # [D], a parameter
     ln: Norm                                      # over dim_head values
     wqk_w: torch.Tensor                           # [2I, I] (the Conv1d weight [2I, I, 1] reshaped)
     wqk_b: torch.Tensor                           # [2I]
     window: int
+    kernel = "window_token"
+    rejects = "window-token attention runs over B token grids only"
+    o2 = True                                     # launch() writes the workspace's second attention output
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        r, p = head_width_reason(L.dim_head), self.window
+        if r is None and p > WINDOW_TOKEN_MAX_WINDOW:
+            r = (f"window_size={p}: a window of {p ** 2} tokens and its window token (the window-token attention "
+                 f"kernel takes windows up to {WINDOW_TOKEN_MAX_WINDOW} x {WINDOW_TOKEN_MAX_WINDOW})")
+        return r
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        p = self.window
+        if grid is None or grid[0] * grid[1] != N:
+            return "window-token attention needs `grid` = (h, w) with h * w == N"
+        if grid[0] % p or grid[1] % p:
+            return f"a {grid[0]} x {grid[1]} grid cannot be cut into {p} x {p} windows"
+        nw = (grid[0] // p) * (grid[1] // p)
+        if nw > WINDOW_MIX_MAX_WINDOWS:
+            return (f"a {grid[0]} x {grid[1]} grid has {nw} windows of {p} x {p}, more than {WINDOW_MIX_MAX_WINDOWS} "
+                    f"(the window-mixing kernel's limit)")
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        # the window token's q | k | v: the same for every window, so projected once, in fp32, then rounded
+        t[f"{i}.tok_qkv"] = (L.qkv_w.detach().float() @ self.token.detach().float()).to(torch.bfloat16)
+        t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"] = _f32(self.ln.gamma), _f32(self.ln.beta)
+        t[f"{i}.wqk.w"], t[f"{i}.wqk.b"] = _bf16_rows(self.wqk_w), _f32(self.wqk_b)
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        """The QKV projection, then the windows' attention with their window token into o; with more than one window,
+        the window tokens' outputs -> LayerNorm + GELU -> their q | k GEMM -> the attention across windows into o2."""
+        c.project(L, i)
+        t, I = c.t, L.heads * L.dim_head
+        (gh, gw), p = c.grid, self.window
+        nw = (gh // p) * (gw // p)
+        if nw == 1:           # the window token is a key and a value, its own output unused (sep_vit.py:176-178)
+            _lib.attention_window_token(c.qkv, t[f"{i}.tok_qkv"], c.o, None, c.B, gh, gw, p, L.heads, L.dim_head,
+                                        L.scale)
+            return c.o
+        tok = torch.empty(c.B * nw, I, device=c.x.device, dtype=torch.bfloat16)
+        _lib.attention_window_token(c.qkv, t[f"{i}.tok_qkv"], c.o, tok, c.B, gh, gw, p, L.heads, L.dim_head, L.scale)
+        _lib.head_layernorm_gelu(tok, t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"], L.heads, L.dim_head, eps=self.ln.eps)
+        wqk = torch.empty(c.B * nw, 2 * I, device=c.x.device, dtype=torch.bfloat16)
+        _lib.gemm(tok, t[f"{i}.wqk.w"], out_bf16=wqk, bias=t[f"{i}.wqk.b"])
+        mixed = c.ws["o2"]
+        _lib.window_mix(wqk, c.o, mixed, c.B, gh, gw, p, L.heads, L.dim_head, L.scale)
+        return mixed
 
 
 class RegionLocalBlock(NamedTuple):
     """RegionViT's region-to-local attention (R2LTransformer, regionvit.py:114-190): the layer's attention runs over
     the region tokens alone, then inside every window of local tokens together with the window's region token, with
     the learned relative-position bias `bias` between local tokens (b200vit_attention, then
-    b200vit_attention_region_local); `window` is the W the bias table was built for, (2W-1)^2 offsets."""
+    b200vit_attention_region_local); `window` is the W the bias table was built for, (2W-1)^2 offsets.  run_blocks
+    takes x = B*N local rows (the `grid` maps, N = h*w) followed by the B*rh*rw rows of the `regions` = (rh, rw) maps;
+    the windows are (h/rh) x (w/rw) local tokens, at most 255."""
     bias: torch.Tensor                            # local_rel_pos_bias.weight [(2W-1)^2, heads], a parameter
     window: int
+    kernel = "region_local"
+    rejects = "region-to-local attention runs over B local and region token maps only"
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        r = head_width_reason(L.dim_head)
+        if r is None and L.dim_head not in REGION_LOCAL_WIDTHS:
+            r = f"dim_head={L.dim_head} (the region-to-local attention kernel is built for 32)"
+        return r
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        if grid is None or regions is None or grid[0] * grid[1] != N:
+            return "region-to-local attention needs `grid` = (h, w) with h * w == N and `regions` = (rh, rw)"
+        (lh, lw), (rh, rw) = grid, regions
+        if rows is not None and rows[1] != rows[0] * (N + rh * rw):
+            return (f"x has {rows[1]} rows, not the B * (N + rh * rw) = {rows[0] * (N + rh * rw)} of B local and "
+                    f"region maps")
+        if lh % rh or lw % rw:
+            return f"the {lh} x {lw} local map does not split into the {rh} x {rw} region map"
+        wh, ww = lh // rh, lw // rw
+        if wh > self.window or ww > self.window:
+            return f"a {wh} x {ww} window is larger than window_size={self.window} of the relative-position bias"
+        if wh * ww + 1 > REGION_LOCAL_MAX_TOKENS:
+            return (f"a {wh} x {ww} window of {wh * ww} local tokens (the region-to-local attention kernel takes at "
+                    f"most {REGION_LOCAL_MAX_TOKENS - 1})")
+        if rh * rw > REGION_MAX_TOKENS:
+            return f"a {rh} x {rw} region map (regional attention takes at most {REGION_MAX_TOKENS} tokens)"
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        t[f"{i}.r2l"] = self.bias.detach().float().t().contiguous()     # [heads, (2W-1)^2]
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        """The QKV GEMM, attention over each image's region tokens and the out-projection residual on the region rows
+        alone (pointer offsets into x, its bf16 copy and its statistics), then the QKV GEMM over all rows and the
+        region-to-local attention into o.  In fold mode the region residual writes the region rows' statistics where
+        the next QKV GEMM reads them; right after a rowstats_cast prime (one part per row) the region rows take the
+        exact LayerNorm and one rowstats_cast of the region rows writes their statistics instead."""
+        t, x, xb, qkv, o = c.t, c.x, c.xb, c.qkv, c.o
+        Ml, (rh, rw) = c.B * c.N, c.regions
+        xr, xbr = x[Ml:], xb[Ml:]
+        if c.fold and c.sums is None:
+            c.sums = c.ws["stats_in"]
+            _lib.rowstats_cast(x, xb, c.sums)
+        sums = c.sums
+        # the residual GEMMs' statistics: the folded GEMM reads them from row Ml on.  A rowstats_cast prime (one part
+        # per row) is read there only 8 bytes per row in, which the GEMM's 16-byte rule does not allow for odd Ml: the
+        # region rows then take the exact LayerNorm, and their new statistics a rowstats_cast
+        gemm_stats = c.fold and sums is not c.ws["stats_in"]
+        if gemm_stats:
+            _lib.gemm(xbr, t[f"{i}.qkv.wg"], out_bf16=qkv[Ml:], bias=t[f"{i}.qkv.t"], ln_sums=sums[Ml:],
+                      col_s=t[f"{i}.qkv.s"], ln_eps=L.ln1.eps)
+        else:
+            _lib.layernorm(xr, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xbr, eps=L.ln1.eps)
+            _lib.gemm(xbr, t[f"{i}.qkv.w"], out_bf16=qkv[Ml:])
+        _lib.attention(qkv[Ml:], o[Ml:], c.B, rh * rw, L.heads, L.dim_head, L.scale)
+        _lib.gemm(o[Ml:], t[f"{i}.out.w"], out_f32=xr, out_bf16=xbr if gemm_stats else None, bias=t[f"{i}.out.b"],
+                  resid=xr, stats_out=sums[Ml:] if gemm_stats else None)
+        if c.fold and not gemm_stats:
+            _lib.rowstats_cast(xr, xbr, sums[Ml:])
+        c.normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv)
+        _lib.attention_region_local(qkv, o, t[f"{i}.r2l"], c.B, c.grid[0], c.grid[1], rh, rw, self.window, L.heads,
+                                    L.dim_head, L.scale)
+        return o
+
+
+AttentionVariant = Union[HeadMix, CrossCovariance, Windows, StridedKV, ConvProj, PatchGroups, WindowTokenBlock,
+                         RegionLocalBlock]
 
 
 @dataclass
@@ -339,111 +663,33 @@ class EncoderLayer:
     temporal: Optional[AttnBlock] = None
     # each query's own key excluded from its softmax (LSA, vit_for_small_dataset.py:53-57)
     mask_self: bool = False
-    # heads mixed across the head axis around the softmax (the attention runs b200vit_attention_headmix)
-    headmix: Optional[HeadMix] = None
+    # the attention variant: None for softmax attention over the layer's sequences, else its record (see above)
+    attention: Optional[AttentionVariant] = None
     # LayerScale (cait.py:31-45): the attention and feed-forward outputs multiplied by these [D] vectors before their
     # residual adds, folded into the rows and biases of out_w and fc2_w
     out_scale: Optional[torch.Tensor] = None
     ff_scale: Optional[torch.Tensor] = None
-    # cross-covariance attention (XCiT, xcit.py:109-148): the per-head temperature parameter [heads, 1, 1]; the
-    # attention runs b200vit_attention_xca with tau = exp(xca_tau), read when the prepared weights are rebuilt
-    xca_tau: Optional[torch.Tensor] = None
     # local patch interaction between the attention and the feed-forward block (XCiT); run_blocks needs `grid`
     lpi: Optional[LPIBlock] = None
     # `ln2` replaces the stream: x = LN2(x); x += fc2(GELU(fc1(x))) (cct.py:137-142)
     post_norm: bool = False
-    # attention inside non-overlapping window x window blocks of the token grid (Twins-SVT's LocalAttention,
-    # twins_svt.py:85-120; b200vit_attention_window); run_blocks needs `grid`
-    window: Optional[int] = None
-    # keys and values from a kv_stride x kv_stride, stride-kv_stride convolution of the normalised token grid
-    # (Twins-SVT's GlobalAttention, twins_svt.py:122-157; b200vit_attention_kv): kv_w is that Conv2d's weight
-    # [2 * heads * dim_head, D, k, k], rows k | v, and qkv_w holds the query rows only; run_blocks needs `grid`
-    kv_stride: Optional[int] = None
-    kv_w: Optional[torch.Tensor] = None
-    # with `window`: a learned relative-position bias inside every window (MaxViT, max_vit.py:148-159;
-    # b200vit_attention_window_relpos): the Embedding weight [(2 window - 1)^2, heads]; `grid_windows` cuts the map into
-    # dilated grids instead of contiguous blocks ('b d (w1 x) (w2 y)', max_vit.py:269)
-    rel_pos_bias: Optional[torch.Tensor] = None
-    grid_windows: bool = False
-    # queries and keys / values from CvT's convolutional projections of the normalised token grid (cvt.py:74-75,
-    # 86-87; b200vit_conv_proj_dw, then b200vit_attention_kv): qkv_w holds the queries' 1 x 1 rows [I, D] and kv_w the
-    # keys' and values' [2I, D], rows k | v; run_blocks needs `grid`
-    conv_proj: Optional[ConvProj] = None
     # the feed-forward block's activation: "gelu" (vit.py:21) or "silu" (MobileViT's FeedForward, mobile_vit.py:28-34)
     ff_act: str = "gelu"
-    # attention inside the strided patch groups of the token grid, token (y'*ph + i, x'*pw + j) in group (i, j)
-    # (MobileViT, mobile_vit.py:150; b200vit_attention_groups); run_blocks needs `grid` and `groups` = (ph, pw)
-    patch_groups: bool = False
-    # attention inside non-overlapping window x window blocks with one learned window token each, then across the
-    # windows (SepViT's DSSA, sep_vit.py:65-206); run_blocks needs `grid`
-    window_token: Optional[WindowTokenBlock] = None
-    # region-to-local attention over a stream of local token rows followed by region token rows (RegionViT's
-    # R2LTransformer, regionvit.py:163-186); run_blocks needs `grid` (the local map) and `regions` (the region map)
-    region_local: Optional[RegionLocalBlock] = None
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
-    """Which kernel runs layer L's attention: 'xca', 'headmix', 'window', 'window_relpos' (windows with a
-    relative-position bias), 'kv' (sub-sampled keys: a strided convolution or CvT's convolutional projections),
-    'groups' (strided patch groups), 'window_token' (SepViT's windows with a window token, then across windows), 'axial' (a run_blocks call with `axial`, unless the layer's temporal sub-block runs
-    there), 'region_local' (RegionViT's regional, then region-to-local attention), 'varlen' (`key_blocks`: a packed
-    batch, or more than 512 keys) or 'plain'.  ValueError for cross-covariance, head-mixing, windowed, patch-group,
-    region-to-local or sub-sampled-key attention with `axial` or over a `packed` batch."""
-    if L.region_local is not None:
+    """Which kernel runs layer L's attention: its record's `kernel` ('headmix', 'xca', 'window', 'window_relpos', 'kv',
+    'groups', 'window_token' or 'region_local'), or for softmax attention 'axial' (a run_blocks call with `axial`,
+    unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys)
+    or 'plain'.  ValueError for an attention variant with `axial` or over a `packed` batch."""
+    A = L.attention
+    if A is not None:
         if axial or packed:
-            raise ValueError("region-to-local attention runs over B local and region token maps only")
-        return "region_local"
-    if L.window_token is not None:
-        if axial or packed:
-            raise ValueError("window-token attention runs over B token grids only")
-        return "window_token"
-    if L.patch_groups:
-        if axial or packed:
-            raise ValueError("patch-group attention runs over B token grids only")
-        return "groups"
-    if L.window is not None or L.kv_stride is not None or L.conv_proj is not None:
-        if axial or packed:
-            raise ValueError("windowed and sub-sampled-key attention run over B token grids only")
-        if L.window is None:
-            return "kv"
-        return "window" if L.rel_pos_bias is None else "window_relpos"
-    if L.xca_tau is not None or L.headmix is not None:
-        if axial or packed:
-            what = "cross-covariance" if L.xca_tau is not None else "head-mixing"
-            raise ValueError(f"{what} attention runs over B sequences of N tokens only")
-        return "xca" if L.xca_tau is not None else "headmix"
+            raise ValueError(A.rejects)
+        return A.kernel
     if axial and L.temporal is None:
         return "axial"
     return "varlen" if key_blocks else "plain"
-
-
-def region_local_reason(lh: int, lw: int, rh: int, rw: int, W: int) -> Optional[str]:
-    """None if an lh x lw local map and an rh x rw region map run region-to-local attention with a bias table built for
-    window_size W, else the reason."""
-    if lh % rh or lw % rw:
-        return f"the {lh} x {lw} local map does not split into the {rh} x {rw} region map"
-    wh, ww = lh // rh, lw // rw
-    if wh > W or ww > W:
-        return f"a {wh} x {ww} window is larger than window_size={W} of the relative-position bias"
-    if wh * ww + 1 > REGION_LOCAL_MAX_TOKENS:
-        return (f"a {wh} x {ww} window of {wh * ww} local tokens (the region-to-local attention kernel takes at most "
-                f"{REGION_LOCAL_MAX_TOKENS - 1})")
-    if rh * rw > REGION_MAX_TOKENS:
-        return f"a {rh} x {rw} region map (regional attention takes at most {REGION_MAX_TOKENS} tokens)"
-    return None
-
-
-def region_local_check(L: EncoderLayer, grid, regions, B: int, N: int, rows: int) -> None:
-    """ValueError unless run_blocks' arguments describe B local maps `grid` (N tokens each) followed by B region maps
-    `regions` in `rows` rows that layer L's region-to-local attention can run on."""
-    if grid is None or regions is None or grid[0] * grid[1] != N:
-        raise ValueError("region-to-local attention needs `grid` = (h, w) with h * w == N and `regions` = (rh, rw)")
-    if rows != B * (N + regions[0] * regions[1]):
-        raise ValueError(f"x has {rows} rows, not the B * (N + rh * rw) = {B * (N + regions[0] * regions[1])} of B "
-                         f"local and region maps")
-    r = region_local_reason(grid[0], grid[1], regions[0], regions[1], L.region_local.window)
-    if r is not None:
-        raise ValueError(r)
 
 
 class _Prepared:
@@ -565,6 +811,69 @@ class FusedEncoder:
         return eng
 
 
+class BlocksCall:
+    """What the launches of one run_blocks call on the per-kernel loop share: the prepared weights `t`, the workspace
+    `ws` and its buffers xb (the bf16 copy of x), qkv, o and h, the fp32 residual stream x, the call's arguments and
+    `sums`, in fold mode the row sums of xb that the next LN-folded GEMM reads (None until a pass writes them)."""
+
+    def __init__(self, t: Dict[str, torch.Tensor], ws: Dict[str, torch.Tensor], x: torch.Tensor, B: int, N: int,
+                 grid, groups, regions, rope, axial, vl, fold: bool, primed: bool) -> None:
+        self.t, self.ws, self.x, self.fold = t, ws, x, fold
+        self.xb, self.qkv, self.o, self.h = ws["xn"], ws["qkv"], ws["o"], ws["h"]
+        self.B, self.N, self.grid, self.groups, self.regions = B, N, grid, groups, regions
+        self.rope, self.axial, self.vl = rope, axial, vl
+        self.sums = ws["stats_in"] if primed else None
+
+    def normed(self, src: torch.Tensor, ln: str, norm: Norm, w: str, out: torch.Tensor, **epi) -> None:
+        """out = LN(src) W^T, LN = t[ln + '.w' / '.b'] with norm.eps, W the Linear t[w + ...].  fold: the LN-folded
+        GEMM on xb and `sums` (made by one rowstats_cast pass if not primed); exact: layernorm(src -> xb), then the
+        plain GEMM with the Linear's bias if it has one.  `epi` with head_gamma (a q / k norm): gemm_headnorm."""
+        t, xb = self.t, self.xb
+        if self.fold:
+            if self.sums is None:
+                self.sums = self.ws["stats_in"]
+                _lib.rowstats_cast(src, xb, self.sums)
+            wt, ln_kw = t[w + ".wg"], dict(bias=t[w + ".t"], ln_sums=self.sums, col_s=t[w + ".s"], ln_eps=norm.eps)
+        else:
+            _lib.layernorm(src, t[ln + ".w"], t[ln + ".b"], out_bf16=xb, eps=norm.eps)
+            wt, ln_kw = t[w + ".w"], dict(bias=t.get(w + ".b"))
+        fn = _lib.gemm_headnorm if "head_gamma" in epi else _lib.gemm_act if "act" in epi else _lib.gemm
+        fn(xb, wt, out_bf16=out, **epi, **ln_kw)
+
+    def stream_copy(self, slot: str) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """(bf16 copy, row sums) the kernel writing the stream also writes: fold (xb, ws[slot]), exact none."""
+        if self.fold:
+            self.sums = self.ws[slot]
+            return self.xb, self.sums
+        return None, None
+
+    def residual(self, a: torch.Tensor, w: str, resid: torch.Tensor, slot: Optional[str]) -> None:
+        """x = resid + a W^T + b (t[w + '.w' / '.b']) and stream_copy(slot); None: a local patch interaction
+        follows and writes the copy of its own output."""
+        copy, stats = self.stream_copy(slot) if slot is not None else (None, None)
+        _lib.gemm(a, self.t[w + ".w"], out_f32=self.x, out_bf16=copy, bias=self.t[w + ".b"], resid=resid,
+                  stats_out=stats)
+
+    def project(self, L: EncoderLayer, i: int) -> None:
+        """qkv = LN1(x) Wqkv^T with layer L's q / k head norm, then the call's rotary positions."""
+        head = {} if L.qk_norm is None else dict(head_gamma=self.t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
+                                                 head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
+        self.normed(self.x, f"{i}.ln1", L.ln1, f"{i}.qkv", self.qkv, **head)
+        if self.rope is not None:
+            _lib.rope_qk(self.qkv, self.rope[0], self.rope[1], L.heads, L.dim_head)
+
+    def attend(self, kernel: str, L: EncoderLayer, i: int) -> None:
+        """o = softmax attention of qkv through the kernel attention_kernel chose: 'axial', 'varlen' or 'plain'."""
+        if kernel == "axial":
+            G, T, key_mask, zero = self.axial
+            _lib.attention_axial(self.qkv, self.o, key_mask, self.x.shape[0] // (T * G), T, G, L.heads, L.dim_head,
+                                 L.scale, zero)
+        elif kernel == "varlen":
+            _lib.attention_varlen(self.qkv, self.o, *self.vl, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
+        else:
+            _lib.attention(self.qkv, self.o, self.B, self.N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
+
+
 class TransformerEngine:
     """Fused execution of the encoder layers a FusedEncoder module describes (reference vit.py:66-83)."""
 
@@ -585,30 +894,20 @@ class TransformerEngine:
         extra = getattr(self.mod, "prepared_buffers", None)
         return list(self.mod.parameters()) + (list(extra()) if extra is not None else [])
 
-    def unsupported_reason(self, N: int) -> Optional[str]:
+    def unsupported_reason(self, N: int, grid: Optional[Tuple[int, int]] = None,
+                           groups: Optional[Tuple[int, int]] = None,
+                           regions: Optional[Tuple[int, int]] = None) -> Optional[str]:
+        """None if the kernels are built for these layers over sequences of N tokens, else the reason the eager
+        PyTorch graph is used.  Layers with an attention variant also check the token geometry, `grid`, `groups` and
+        `regions` as run_blocks takes them, with the rule run_blocks raises on."""
         # only shapes are read, and a module's shapes are fixed at construction: any description of it serves
         for L in self.layers or self.mod.encoder_layers()[0]:
-            kernel = attention_kernel(L)
-            r = (xca_reason(L.dim_head) if kernel == "xca" else
-                 headmix_reason(L.heads, L.dim_head) if kernel == "headmix" else
-                 groups_reason(L.dim_head) if kernel == "groups" else head_width_reason(L.dim_head))
-            if r is None and kernel == "region_local" and L.dim_head not in REGION_LOCAL_WIDTHS:
-                r = f"dim_head={L.dim_head} (the region-to-local attention kernel is built for 32)"
+            A = L.attention
+            r = head_width_reason(L.dim_head) if A is None else A.reason(L)
             if r is None and L.lpi is not None and L.lpi.kernel_size not in LPI_KERNEL_SIZES:
                 r = lpi_reason(L.lpi.kernel_size, 1)
-            if r is None and kernel == "window_relpos" and L.window ** 2 > WINDOW_MAX_TOKENS:
-                r = (f"window_size={L.window}: a window of {L.window ** 2} tokens (the relative-position window "
-                     f"attention kernel takes at most {WINDOW_MAX_TOKENS})")
-            if r is None and L.conv_proj is not None and L.conv_proj.kernel_size not in CONV_PROJ_KERNEL_SIZES:
-                r = (f"proj_kernel={L.conv_proj.kernel_size} (the convolutional-projection kernel is built for 1, 3, 5 "
-                     f"and 7)")
-            if r is None and kernel == "window_token" and L.window_token.window > WINDOW_TOKEN_MAX_WINDOW:
-                r = (f"window_size={L.window_token.window}: a window of {L.window_token.window ** 2} tokens and its "
-                     f"window token (the window-token attention kernel takes windows up to "
-                     f"{WINDOW_TOKEN_MAX_WINDOW} x {WINDOW_TOKEN_MAX_WINDOW})")
-            if r is None and L.window is not None and L.window ** 2 > WINDOW_MAX_TOKENS:
-                r = (f"local_patch_size={L.window}: a window of {L.window ** 2} tokens (the window attention kernel "
-                     f"takes at most {WINDOW_MAX_TOKENS})")
+            if r is None and A is not None:
+                r = A.geometry_reason(L, N, grid, groups, regions)
             if r is not None:
                 return r
             if L.qkv_w.shape[1] % 8 or L.fc1_w.shape[0] % 8:
@@ -646,32 +945,8 @@ class TransformerEngine:
                 t[f"{i}.tout.w"] = (torch.eye(T.qkv_w.shape[1], device=T.qkv_w.device, dtype=torch.bfloat16)
                                     if T.out_w is None else _bf16_rows(T.out_w))
                 t[f"{i}.tout.b"] = _f32(T.out_b)
-            if L.headmix is not None:
-                X = L.headmix
-                t[f"{i}.post"] = _f32(X.post)
-                if X.pre is not None:
-                    t[f"{i}.pre"] = _f32(X.pre)
-                if X.ln is not None:
-                    t[f"{i}.hln.w"], t[f"{i}.hln.b"] = _f32(X.ln.gamma), _f32(X.ln.beta)
-            if L.xca_tau is not None:
-                t[f"{i}.tau"] = L.xca_tau.detach().float().exp().reshape(-1).contiguous()
-            if L.rel_pos_bias is not None:
-                t[f"{i}.relpos"] = L.rel_pos_bias.detach().float().t().contiguous()
-            if L.conv_proj is not None:
-                # the depthwise halves with their BatchNorms folded (tap-major) and the keys' / values' 1 x 1 rows
-                t[f"{i}.cpq.w"], t[f"{i}.cpq.b"], t[f"{i}.cpkv.w"], t[f"{i}.cpkv.b"] = conv_proj_weights(L.conv_proj)
-                t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.reshape(L.kv_w.shape[0], -1))
-            elif L.kv_stride is not None:
-                # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
-                t[f"{i}.kv.w"] = _bf16_rows(L.kv_w.detach().permute(0, 2, 3, 1).reshape(L.kv_w.shape[0], -1))
-            if L.window_token is not None:
-                T = L.window_token
-                # the window token's q | k | v: the same for every window, so projected once, in fp32, then rounded
-                t[f"{i}.tok_qkv"] = (L.qkv_w.detach().float() @ T.token.detach().float()).to(torch.bfloat16)
-                t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"] = _f32(T.ln.gamma), _f32(T.ln.beta)
-                t[f"{i}.wqk.w"], t[f"{i}.wqk.b"] = _bf16_rows(T.wqk_w), _f32(T.wqk_b)
-            if L.region_local is not None:
-                t[f"{i}.r2l"] = L.region_local.bias.detach().float().t().contiguous()     # [heads, (2W-1)^2]
+            if L.attention is not None:
+                L.attention.prepare(t, i, L)
             if L.lpi is not None:
                 P = L.lpi
                 t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"] = _f32(P.ln.gamma), _f32(P.ln.beta)
@@ -689,12 +964,12 @@ class TransformerEngine:
     def _c_layers(self, t: Dict[str, torch.Tensor]):
         """(ctypes array of b200vit_layer, (heads, dh, hidden, scale), layer scales, attention flags) for the one-call
         encoder (b200vit_encoder_blocks), or None when it cannot run these layers: they are not uniform, one has a
-        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block, an attention kernel other
-        than the plain one, a local patch interaction or a post-norm step.  Layer scales: None when every layer has the same scale, else
+        per-head LayerNorm (the one-call encoder has no EPI_HEADLN), a temporal sub-block, an attention variant, a
+        local patch interaction or a post-norm step.  Layer scales: None when every layer has the same scale, else
         a ctypes float array for b200vit_encoder_blocks_ex (LSA's learned temperatures).  The pointers stay valid as
         long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
-        if any(L.qk_norm == "ln" or L.temporal is not None or attention_kernel(L) != "plain" or L.lpi is not None
+        if any(L.qk_norm == "ln" or L.temporal is not None or L.attention is not None or L.lpi is not None
                or L.post_norm or L.ff_act != "gelu" or sig(L) != sig(self.layers[0]) for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
@@ -742,8 +1017,8 @@ class TransformerEngine:
             if any(L.lpi is not None or L.post_norm for L in self.layers):
                 # the stream the feed-forward block reads: the local patch interaction's or the post-norm's output
                 slot.t["y"] = torch.empty(M, D, device=device, dtype=torch.float32)
-            if any(L.window_token is not None for L in self.layers):
-                # the attention across windows, out of place from "o"
+            if any(getattr(L.attention, "o2", False) for L in self.layers):
+                # a second attention output, out of place from "o" (the attention across windows)
                 slot.t["o2"] = torch.empty(M, I, **bf)
             if any(L.lpi is not None for L in self.layers):
                 # the local patch interaction's row statistics and its LayerNorm scratch
@@ -785,26 +1060,12 @@ class TransformerEngine:
         G = N); layers without one run their attention there instead of over the B x N sequences (ViViT's masked
         temporal transformer, G = 1).  These calls take the per-kernel loop below.
         `grid` = (h, w): the token grid of every sequence (N = h*w, token r*w + c), which layers with a local patch
-        interaction, windowed attention or sub-sampled keys need (XCiT, Twins-SVT).  A layer with sub-sampled keys cannot
-        fold its LayerNorm into the key / value projection (one convolution window spans tokens with different
-        statistics): in both LayerNorm modes it runs layernorm(x -> xb), the query GEMM on xb, conv_im2col_nhwc of xb
-        and the key / value GEMM (kernel size 1: the GEMM on xb itself), then attention_kv.  A layer with convolutional
-        projections (CvT) runs layernorm(x -> xb), conv_proj_dw of xb into the query and key / value operands, their
-        1 x 1 GEMMs, then attention_kv; the projections pad, so any h, w >= 1 will do.  Layers with patch-group attention
-        (MobileViT) need `groups` = (ph, pw) dividing `grid` as well (attention_groups).  Layers with window-token attention
-        (SepViT) need `grid` cut into at most 64 windows: attention_window_token into o, and with more than one window
-        head_layernorm_gelu, the window q | k GEMM and window_mix into ws['o2'], which the out-projection then reads.
-        Layers with region-to-local attention (RegionViT) take x = B*N local rows (the `grid` maps, N = h*w) followed
-        by the B*rh*rw rows of the `regions` = (rh, rw) maps, and run the QKV GEMM, attention over each image's region
-        tokens and the out-projection residual on the region rows alone (pointer offsets into x, its bf16 copy and its
-        statistics), then the QKV GEMM over all rows and attention_region_local; the windows are (h/rh) x (w/rw) local
-        tokens, at most 255.  In fold mode the region residual writes the region rows' statistics where the next QKV
-        GEMM reads them; right after a rowstats_cast prime (one part per row) the region rows take the exact LayerNorm
-        and one rowstats_cast of the region rows writes their statistics instead.  A layer's feed-forward block
-        applies its `ff_act`.  A layer runs QKV -> rope -> attention -> out-projection -> temporal sub-block (QKV,
-        axial attention, out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2
-        onto that stream, written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its
-        fc1 is the plain GEMM on that copy.  The call is checked first: a ValueError leaves x as it was.
+        interaction (XCiT) or an attention variant on the grid need; `groups` and `regions` as those variants describe
+        them (PatchGroups, RegionLocalBlock).  A layer's feed-forward block applies its `ff_act`.  A layer runs QKV ->
+        rope -> attention (or its variant's launches) -> out-projection -> temporal sub-block (QKV, axial attention,
+        out) -> local patch interaction x -> y, the stream the feed-forward block reads -> fc1 -> fc2 onto that stream,
+        written to x.  A post-norm layer (CCT) writes y = LN2(x) and its bf16 copy instead, and its fc1 is the plain
+        GEMM on that copy.  The call is checked first: a ValueError leaves x as it was.
 
         fold mode needs ws['xn'] (bf16 copy of x) and ws['stats_in'] (row sums of that copy) on entry: `primed` says
         the caller (embed_tokens / embed_varlen) already wrote them, otherwise one rowstats_cast pass produces them."""
@@ -828,198 +1089,29 @@ class TransformerEngine:
             kernels.append(attention_kernel(L, axial is not None, varlen is not None, vl is not None))
             if L.lpi is not None and (grid is None or grid[0] * grid[1] != N or axial is not None or varlen is not None):
                 raise ValueError("a layer with a local patch interaction needs `grid` = (h, w) with h * w == N")
-            if kernels[-1] == "groups":
-                if grid is None or grid[0] * grid[1] != N or groups is None:
-                    raise ValueError("patch-group attention needs `grid` = (h, w) with h * w == N and `groups`")
-                if grid[0] % groups[0] or grid[1] % groups[1]:
-                    raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {groups[0]} x {groups[1]} "
-                                     f"patches")
-            if kernels[-1] == "window_token":
-                p = L.window_token.window
-                if grid is None or grid[0] * grid[1] != N:
-                    raise ValueError("window-token attention needs `grid` = (h, w) with h * w == N")
-                if grid[0] % p or grid[1] % p:
-                    raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {p} x {p} windows")
-                if (grid[0] // p) * (grid[1] // p) > WINDOW_MIX_MAX_WINDOWS:
-                    raise ValueError(f"a {grid[0]} x {grid[1]} grid has more than {WINDOW_MIX_MAX_WINDOWS} "
-                                     f"{p} x {p} windows")
-            if kernels[-1] == "region_local":
-                region_local_check(L, grid, regions, B, N, x.shape[0])
-            if kernels[-1] in ("window", "window_relpos", "kv"):
-                if grid is None or grid[0] * grid[1] != N:
-                    raise ValueError("windowed and sub-sampled-key attention need `grid` = (h, w) with h * w == N")
-                if L.conv_proj is not None:
-                    continue                   # the projections pad: any h, w >= 1
-                windowed = kernels[-1] != "kv"
-                step = L.window if windowed else L.kv_stride
-                if (grid[0] % step or grid[1] % step) if windowed else min(grid) < step:
-                    raise ValueError(f"a {grid[0]} x {grid[1]} grid cannot be cut into {step} x {step} "
-                                     f"{'windows' if windowed else 'key patches'}")
-        xb, qkv, o, h = ws["xn"], ws["qkv"], ws["o"], ws["h"]
-        sums = ws["stats_in"] if primed else None          # fold: the row sums of xb the next LN-folded GEMM reads
-
-        def normed(src: torch.Tensor, ln: str, norm: Norm, w: str, out: torch.Tensor, **epi) -> None:
-            """out = LN(src) W^T, LN = t[ln + '.w' / '.b'] with norm.eps, W the Linear t[w + ...].  fold: the LN-folded
-            GEMM on xb and `sums` (made by one rowstats_cast pass if not primed); exact: layernorm(src -> xb), then the
-            plain GEMM with the Linear's bias if it has one.  `epi` with head_gamma (a q / k norm): gemm_headnorm."""
-            nonlocal sums
-            if fold:
-                if sums is None:
-                    sums = ws["stats_in"]
-                    _lib.rowstats_cast(src, xb, sums)
-                wt, ln_kw = t[w + ".wg"], dict(bias=t[w + ".t"], ln_sums=sums, col_s=t[w + ".s"], ln_eps=norm.eps)
-            else:
-                _lib.layernorm(src, t[ln + ".w"], t[ln + ".b"], out_bf16=xb, eps=norm.eps)
-                wt, ln_kw = t[w + ".w"], dict(bias=t.get(w + ".b"))
-            fn = _lib.gemm_headnorm if "head_gamma" in epi else _lib.gemm_act if "act" in epi else _lib.gemm
-            fn(xb, wt, out_bf16=out, **epi, **ln_kw)
-
-        def stream_copy(slot: str) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-            """(bf16 copy, row sums) the kernel writing the stream also writes: fold (xb, ws[slot]), exact none."""
-            nonlocal sums
-            if fold:
-                sums = ws[slot]
-                return xb, sums
-            return None, None
-
-        def residual(a: torch.Tensor, w: str, resid: torch.Tensor, slot: Optional[str]) -> None:
-            """x = resid + a W^T + b (t[w + '.w' / '.b']) and stream_copy(slot); None: a local patch interaction
-            follows and writes the copy of its own output."""
-            copy, stats = stream_copy(slot) if slot is not None else (None, None)
-            _lib.gemm(a, t[w + ".w"], out_f32=x, out_bf16=copy, bias=t[w + ".b"], resid=resid, stats_out=stats)
-
-        def subsampled(L: EncoderLayer, i: int) -> None:
-            """o = attention of LN1(x)'s queries over the keys / values of its strided convolution, or of its
-            convolutional projections (CvT)."""
-            if L.conv_proj is not None:
-                conv_projected(L, i)
-                return
-            I, k = L.heads * L.dim_head, L.kv_stride
-            kh, kw = grid[0] // k, grid[1] // k
-            _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
-            q = qkv[:, :I]
-            _lib.gemm(xb, t[f"{i}.qkv.w"], out_bf16=q)
-            if k == 1:
-                col = xb
-            else:
-                col = torch.empty(B * kh * kw, k * k * x.shape[1], device=x.device, dtype=torch.bfloat16)
-                _lib.conv_im2col_nhwc(xb, col, B, grid[0], grid[1], k, k, 0)
-            kv = torch.empty(B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
-            _lib.gemm(col, t[f"{i}.kv.w"], out_bf16=kv)
-            _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
-
-        def conv_projected(L: EncoderLayer, i: int) -> None:
-            """CvT: layernorm(x -> xb), both depthwise projections of xb in one pass (the LayerNorm cannot be folded:
-            the padding taps must read zeros of the normalised map), the 1 x 1 GEMMs, attention_kv."""
-            P, I, D = L.conv_proj, L.heads * L.dim_head, x.shape[1]
-            kh, kw = P.grid(*grid)
-            _lib.layernorm(x, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xb, eps=L.ln1.eps)
-            aq = torch.empty(x.shape[0], D, device=x.device, dtype=torch.bfloat16)
-            akv = torch.empty(B * kh * kw, D, device=x.device, dtype=torch.bfloat16)
-            _lib.conv_proj_dw(xb, t[f"{i}.cpq.w"], t[f"{i}.cpq.b"], t[f"{i}.cpkv.w"], t[f"{i}.cpkv.b"], aq, akv, B,
-                              grid[0], grid[1], P.kernel_size, P.stride)
-            q = qkv[:, :I]
-            _lib.gemm(aq, t[f"{i}.qkv.w"], out_bf16=q)
-            kv = torch.empty(B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
-            _lib.gemm(akv, t[f"{i}.kv.w"], out_bf16=kv)
-            _lib.attention_kv(q, kv, o, B, N, kh * kw, L.heads, L.dim_head, L.scale)
-
-        def region_local(L: EncoderLayer, i: int) -> None:
-            """RegionViT's regional attention on the region rows (x[B*N:]) with its residual, then the QKV GEMM over
-            all rows and the region-to-local attention into o."""
-            nonlocal sums
-            Ml, (rh, rw) = B * N, regions
-            xr, xbr = x[Ml:], xb[Ml:]
-            if fold and sums is None:
-                sums = ws["stats_in"]
-                _lib.rowstats_cast(x, xb, sums)
-            # the residual GEMMs' statistics: the folded GEMM reads them from row Ml on.  A rowstats_cast prime (one
-            # part per row) is read there only 8 bytes per row in, which the GEMM's 16-byte rule does not allow for odd
-            # Ml: the region rows then take the exact LayerNorm, and their new statistics a rowstats_cast
-            gemm_stats = fold and sums is not ws["stats_in"]
-            if gemm_stats:
-                _lib.gemm(xbr, t[f"{i}.qkv.wg"], out_bf16=qkv[Ml:], bias=t[f"{i}.qkv.t"], ln_sums=sums[Ml:],
-                          col_s=t[f"{i}.qkv.s"], ln_eps=L.ln1.eps)
-            else:
-                _lib.layernorm(xr, t[f"{i}.ln1.w"], t[f"{i}.ln1.b"], out_bf16=xbr, eps=L.ln1.eps)
-                _lib.gemm(xbr, t[f"{i}.qkv.w"], out_bf16=qkv[Ml:])
-            _lib.attention(qkv[Ml:], o[Ml:], B, rh * rw, L.heads, L.dim_head, L.scale)
-            _lib.gemm(o[Ml:], t[f"{i}.out.w"], out_f32=xr, out_bf16=xbr if gemm_stats else None, bias=t[f"{i}.out.b"],
-                      resid=xr, stats_out=sums[Ml:] if gemm_stats else None)
-            if fold and not gemm_stats:
-                _lib.rowstats_cast(xr, xbr, sums[Ml:])
-            normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv)
-            _lib.attention_region_local(qkv, o, t[f"{i}.r2l"], B, grid[0], grid[1], rh, rw, L.region_local.window,
-                                        L.heads, L.dim_head, L.scale)
-
-        def window_token(L: EncoderLayer, i: int) -> torch.Tensor:
-            """SepViT's DSSA after its QKV projection: the windows' attention with their window token into o; with more
-            than one window, the window tokens' outputs -> LayerNorm + GELU -> their q | k GEMM -> the attention across
-            windows into a second buffer.  Returns the buffer that holds the result."""
-            T, I = L.window_token, L.heads * L.dim_head
-            gh, gw, p = grid[0], grid[1], T.window
-            nw = (gh // p) * (gw // p)
-            if nw == 1:           # the window token is a key and a value, its own output unused (sep_vit.py:176-178)
-                _lib.attention_window_token(qkv, t[f"{i}.tok_qkv"], o, None, B, gh, gw, p, L.heads, L.dim_head,
-                                            L.scale)
-                return o
-            tok = torch.empty(B * nw, I, device=x.device, dtype=torch.bfloat16)
-            _lib.attention_window_token(qkv, t[f"{i}.tok_qkv"], o, tok, B, gh, gw, p, L.heads, L.dim_head, L.scale)
-            _lib.head_layernorm_gelu(tok, t[f"{i}.wt.ln.w"], t[f"{i}.wt.ln.b"], L.heads, L.dim_head, eps=T.ln.eps)
-            wqk = torch.empty(B * nw, 2 * I, device=x.device, dtype=torch.bfloat16)
-            _lib.gemm(tok, t[f"{i}.wqk.w"], out_bf16=wqk, bias=t[f"{i}.wqk.b"])
-            mixed = ws["o2"]
-            _lib.window_mix(wqk, o, mixed, B, gh, gw, p, L.heads, L.dim_head, L.scale)
-            return mixed
-
-        def attend(kernel: str, L: EncoderLayer, i: int) -> None:
-            if kernel == "window":
-                _lib.attention_window(qkv, o, B, grid[0], grid[1], L.window, L.heads, L.dim_head, L.scale)
-            elif kernel == "window_relpos":
-                _lib.attention_window_relpos(qkv, o, t[f"{i}.relpos"], B, grid[0], grid[1], L.window, L.grid_windows,
-                                             L.heads, L.dim_head, L.scale)
-            elif kernel == "groups":
-                _lib.attention_groups(qkv, o, B, grid[0], grid[1], groups[0], groups[1], L.heads, L.dim_head, L.scale)
-            elif kernel == "xca":
-                _lib.attention_xca(qkv, t[f"{i}.tau"], o, B, N, L.heads, L.dim_head)
-            elif kernel == "headmix":
-                hln = None if L.headmix.ln is None else (t[f"{i}.hln.w"], t[f"{i}.hln.b"], L.headmix.ln.eps)
-                _lib.attention_headmix(qkv, o, B, N, L.heads, L.dim_head, L.scale, t[f"{i}.post"], hln,
-                                       pre=t.get(f"{i}.pre"))
-            elif kernel == "axial":
-                G, T, key_mask, zero = axial
-                _lib.attention_axial(qkv, o, key_mask, x.shape[0] // (T * G), T, G, L.heads, L.dim_head, L.scale, zero)
-            elif kernel == "varlen":
-                _lib.attention_varlen(qkv, o, *vl, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
-            else:
-                _lib.attention(qkv, o, B, N, L.heads, L.dim_head, L.scale, mask_self=L.mask_self)
-
+            if L.attention is not None:
+                r = L.attention.geometry_reason(L, N, grid, groups, regions, rows=(B, x.shape[0]))
+                if r is not None:
+                    raise ValueError(r)
+        c = BlocksCall(t, ws, x, B, N, grid, groups, regions, rope, axial, vl, fold, primed)
+        xb, h = c.xb, c.h
         for i, kernel in zip(run, kernels):
             L = self.layers[i]
             act = dict(act="silu") if L.ff_act == "silu" else dict(gelu=True)
-            head = {} if L.qk_norm is None else dict(head_gamma=t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
-                                                     head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
-            attn_out = o
-            if kernel == "kv":
-                subsampled(L, i)
-            elif kernel == "region_local":
-                region_local(L, i)
+            if L.attention is None:
+                c.project(L, i)
+                c.attend(kernel, L, i)
+                attn_out = c.o
             else:
-                normed(x, f"{i}.ln1", L.ln1, f"{i}.qkv", qkv, **head)
-                if rope is not None:
-                    _lib.rope_qk(qkv, rope[0], rope[1], L.heads, L.dim_head)
-                if kernel == "window_token":
-                    attn_out = window_token(L, i)
-                else:
-                    attend(kernel, L, i)
-            residual(attn_out, f"{i}.out", x, "stats_b" if L.lpi is None and not L.post_norm else None)
+                attn_out = L.attention.launch(c, L, i)
+            c.residual(attn_out, f"{i}.out", x, "stats_b" if L.lpi is None and not L.post_norm else None)
             if L.temporal is not None:
-                normed(x, f"{i}.tln", L.temporal.ln, f"{i}.tqkv", qkv)
-                attend("axial", L, i)
-                residual(o, f"{i}.tout", x, "stats_b")
+                c.normed(x, f"{i}.tln", L.temporal.ln, f"{i}.tqkv", c.qkv)
+                c.attend("axial", L, i)
+                c.residual(c.o, f"{i}.tout", x, "stats_b")
             ff_in = x if L.lpi is None and not L.post_norm else ws["y"]
             if L.lpi is not None:
-                yb, ys = stream_copy("stats_l")
+                yb, ys = c.stream_copy("stats_l")
                 ln = (t[f"{i}.lpi.ln.w"], t[f"{i}.lpi.ln.b"], L.lpi.ln.eps)
                 _lib.local_patch_interaction(x, ff_in, ws["lnst"], ln, t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"],
                                              t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"], B, grid[0], grid[1],
@@ -1030,8 +1122,8 @@ class TransformerEngine:
                 (_lib.gemm_act if "act" in act else _lib.gemm)(xb, t[f"{i}.fc1.w"], out_bf16=h, bias=t[f"{i}.fc1.b"],
                                                                 **act)
             else:
-                normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, **act)
-            residual(h, f"{i}.fc2", ff_in, "stats_a")
+                c.normed(ff_in, f"{i}.ln2", L.ln2, f"{i}.fc1", h, **act)
+            c.residual(h, f"{i}.fc2", ff_in, "stats_a")
 
     def final_norm(self, x: torch.Tensor, *, out_bf16: Optional[torch.Tensor] = None,
                    out_f32: Optional[torch.Tensor] = None, row_index: Optional[torch.Tensor] = None) -> None:

@@ -21,7 +21,7 @@ partition, as an address map.
     rows, b200vit_se_scale; the last 1 x 1 GEMM with its BatchNorm folded, added into the stream (MBConvResidual) or
     starting the stage's fresh fp32 stream;
   * block attention + FeedForward, then grid attention + FeedForward: two EncoderLayers through
-    TransformerEngine.run_blocks with b200vit_attention_window_relpos (grid_windows False, then True);
+    TransformerEngine.run_blocks with b200vit_attention_window_relpos (Windows.dilated False, then True);
   * head: b200vit_mean_pool, b200vit_layernorm (the reference normalises after pooling), the classifier GEMM.
 BatchNorm runs on its running statistics: a BatchNorm2d in training mode sends the call to the PyTorch graph.
 """
@@ -33,8 +33,8 @@ import torch
 from torch import einsum, nn
 
 from . import _lib
-from .engine import (WINDOW_MAX_TOKENS, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _bf16_rows, cached,
-                     common_reason, head_engine, head_norm, on_device)
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, Windows, _bf16_rows, cached, common_reason,
+                     head_engine, head_norm, on_device)
 from .levit import _conv_weight, fold_bn
 from .xcit import batchnorm_reason
 
@@ -318,8 +318,8 @@ class _BlockAttention(FusedEncoder):
             layers.append(EncoderLayer(
                 ln1=Norm.of(a.norm), qkv_w=a.to_qkv.weight, out_w=a.to_out[0].weight, out_b=None, ln2=Norm.of(f[0]),
                 fc1_w=f[1].weight, fc1_b=f[1].bias, fc2_w=f[4].weight, fc2_b=f[4].bias, heads=a.heads,
-                dim_head=a.dim_head, scale=a.scale, window=a.window_size, rel_pos_bias=a.rel_pos_bias.weight,
-                grid_windows=grid))
+                dim_head=a.dim_head, scale=a.scale,
+                attention=Windows(a.window_size, rel_pos_bias=a.rel_pos_bias.weight, dilated=grid)))
         return layers, None
 
 
@@ -443,9 +443,6 @@ class MaxViT(FusedWeightsMixin, nn.Module):
         r = batchnorm_reason(self)
         if r is not None:
             return r
-        if self.window_size ** 2 > WINDOW_MAX_TOKENS:
-            return (f"window_size={self.window_size}: a window of {self.window_size ** 2} tokens (the relative-position "
-                    f"window attention kernel takes at most {WINDOW_MAX_TOKENS})")
         if self.conv_stem[0].out_channels % 8:
             return f"dim_conv_stem={self.conv_stem[0].out_channels} (the GEMMs need multiples of 8)"
         w = self.window_size
@@ -459,7 +456,7 @@ class MaxViT(FusedWeightsMixin, nn.Module):
                 return (f"block {i}: MBConv widths {widths[0]} -> {widths[1]} (squeeze-excitation {widths[2]}) -> "
                         f"{widths[3]} (the GEMMs need multiples of 8)")
         for e, (h, ww) in zip(self._encoders(), self.stage_maps(img.shape[2], img.shape[3])):
-            r = e.engine().unsupported_reason(h * ww)
+            r = e.engine().unsupported_reason(h * ww, grid=(h, ww))
             if r is not None:
                 return r
         return None

@@ -31,7 +31,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from .engine import (GROUPS_MAX_TOKENS, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, _bf16_rows, cached,
+from .engine import (EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, PatchGroups, _bf16_rows, cached,
                      common_reason, head_engine, on_device)
 from .levit import fold_bn
 from .xcit import batchnorm_reason
@@ -131,7 +131,7 @@ class Transformer(FusedEncoder, nn.Module):
                 ln1=Norm.of(attn.norm), qkv_w=attn.to_qkv.weight, out_w=attn.to_out[0].weight,
                 out_b=attn.to_out[0].bias, ln2=Norm.of(f[0]), fc1_w=f[1].weight, fc1_b=f[1].bias, fc2_w=f[4].weight,
                 fc2_b=f[4].bias, heads=attn.heads, dim_head=attn.dim_head, scale=attn.scale, ff_act="silu",
-                patch_groups=True))
+                attention=PatchGroups()))
         return layers, None
 
     def fused_reason(self, x: torch.Tensor) -> Optional[str]:
@@ -142,9 +142,7 @@ class Transformer(FusedEncoder, nn.Module):
             return r
         if x.shape[-1] % 8:
             return f"dim={x.shape[-1]} (the GEMMs need multiples of 8)"
-        if not 1 <= x.shape[2] <= GROUPS_MAX_TOKENS:
-            return f"{x.shape[2]} tokens per group (the patch-group attention kernel takes 1 to {GROUPS_MAX_TOKENS})"
-        return self.engine().unsupported_reason(x.shape[2])
+        return self.engine().unsupported_reason(x.shape[2], grid=(x.shape[2], 1), groups=(1, 1))
 
     def forward(self, x):
         if self.fused_reason(x) is None:
@@ -402,11 +400,7 @@ class MobileViT(FusedWeightsMixin, nn.Module):
                 return f"trunk {i}: channel={C}, dim={D} (the GEMMs need multiples of 8)"
             if h % ph or w % pw:
                 return f"trunk {i}: the {h} x {w} map is not divisible into {ph} x {pw} patches (the reference raises)"
-            n = (h // ph) * (w // pw)
-            if n > GROUPS_MAX_TOKENS:
-                return f"trunk {i}: {n} tokens per group (the patch-group attention kernel takes at most " \
-                       f"{GROUPS_MAX_TOKENS})"
-            r = blk.transformer.engine().unsupported_reason(h * w)
+            r = blk.transformer.engine().unsupported_reason(h * w, grid=(h, w), groups=(ph, pw))
             if r is not None:
                 return r
         return None

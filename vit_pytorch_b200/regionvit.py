@@ -35,7 +35,7 @@ from torch import nn
 from . import _lib
 from .engine import (HEAD_WIDTHS, PEG_KERNEL_SIZES, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm,
                      RegionLocalBlock, _bf16_rows, _f32, cached, common_reason, head_engine, head_ln_pool, on_device,
-                     region_local_reason, why_not_fused)
+                     why_not_fused)
 from .sep_vit import conv_weights, peg_weights
 
 __all__ = ["Attention", "ChanLayerNorm", "Downsample", "FeedForward", "PEG", "R2LTransformer", "RegionViT",
@@ -202,15 +202,12 @@ class R2LTransformer(FusedEncoder, nn.Module):
                 ln1=Norm.of(attn.norm), qkv_w=attn.to_qkv.weight, out_w=attn.to_out[0].weight,
                 out_b=attn.to_out[0].bias, ln2=Norm.of(ff[0]), fc1_w=ff[1].weight, fc1_b=ff[1].bias,
                 fc2_w=ff[4].weight, fc2_b=ff[4].bias, heads=attn.heads, dim_head=attn.dim_head, scale=attn.scale,
-                region_local=block))
+                attention=block))
         return layers, None
 
     def map_reason(self, lh: int, lw: int, rh: int, rw: int) -> Optional[str]:
         """Why an lh x lw local map with an rh x rw region map cannot run fused, or None."""
-        r = region_local_reason(lh, lw, rh, rw, self.window_size)
-        if r is not None:
-            return r
-        return self.engine().unsupported_reason(lh * lw)
+        return self.engine().unsupported_reason(lh * lw, grid=(lh, lw), regions=(rh, rw))
 
     def fused_reason(self, local_tokens: torch.Tensor, region_tokens: torch.Tensor) -> Optional[str]:
         if local_tokens.dim() != 4 or region_tokens.dim() != 4:

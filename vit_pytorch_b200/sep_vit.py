@@ -27,9 +27,8 @@ import torch
 from torch import nn
 
 from . import _lib
-from .engine import (PEG_KERNEL_SIZES, WINDOW_MIX_MAX_WINDOWS, WINDOW_TOKEN_MAX_WINDOW, EncoderLayer, FusedEncoder,
-                     FusedWeightsMixin, Norm, WindowTokenBlock, _bf16_rows, _f32, cached, common_reason, head_engine,
-                     head_ln_pool, on_device)
+from .engine import (PEG_KERNEL_SIZES, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, WindowTokenBlock,
+                     _bf16_rows, _f32, cached, common_reason, head_engine, head_ln_pool, on_device)
 
 __all__ = ["ChanLayerNorm", "DSSA", "FeedForward", "OverlappingPatchEmbed", "PEG", "SepViT", "Transformer",
            "cast_tuple"]
@@ -257,24 +256,19 @@ class Transformer(FusedEncoder, nn.Module):
                 out_w=attn.to_out[0].weight.reshape(D, I), out_b=attn.to_out[0].bias, ln2=_norm(f[0]),
                 fc1_w=f[1].weight.reshape(-1, D), fc1_b=f[1].bias, fc2_w=f[4].weight.reshape(D, -1), fc2_b=f[4].bias,
                 heads=attn.heads, dim_head=attn.dim_head, scale=attn.scale,
-                window_token=WindowTokenBlock(token=attn.window_tokens, ln=Norm.of(ln),
-                                              wqk_w=conv.weight.reshape(2 * I, I), wqk_b=conv.bias,
-                                              window=attn.window_size)))
+                attention=WindowTokenBlock(token=attn.window_tokens, ln=Norm.of(ln),
+                                           wqk_w=conv.weight.reshape(2 * I, I), wqk_b=conv.bias,
+                                           window=attn.window_size)))
         return layers, None if isinstance(self.norm, nn.Identity) else _norm(self.norm)
 
     def map_reason(self, h: int, w: int) -> Optional[str]:
-        """Why an h x w map cannot run fused (the reference raises on the first two), or None."""
+        """Why an h x w map cannot run fused, or None: a map the windows do not divide (the reference raises), then
+        the engine's rules."""
         for attn, _ in self.layers:
             p = attn.window_size
             if h % p or w % p:
                 return f"the {h} x {w} map is not divisible by window_size={p} (the reference raises)"
-            if p > WINDOW_TOKEN_MAX_WINDOW:
-                return (f"window_size={p} (the window-token attention kernel takes windows up to "
-                        f"{WINDOW_TOKEN_MAX_WINDOW} x {WINDOW_TOKEN_MAX_WINDOW})")
-            if (h // p) * (w // p) > WINDOW_MIX_MAX_WINDOWS:
-                return (f"{(h // p) * (w // p)} windows in a {h} x {w} map (the window-mixing kernel takes at most "
-                        f"{WINDOW_MIX_MAX_WINDOWS})")
-        return self.engine().unsupported_reason(h * w)
+        return self.engine().unsupported_reason(h * w, grid=(h, w))
 
     def fused_reason(self, x: torch.Tensor) -> Optional[str]:
         if x.dim() != 4:

@@ -30,7 +30,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from .engine import (PEG_KERNEL_SIZES, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm,
+from .engine import (PEG_KERNEL_SIZES, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, StridedKV, Windows,
                      _bf16_rows, _f32, cached, common_reason, head_engine, on_device)
 
 __all__ = ["FeedForward", "GlobalAttention", "LayerNorm", "LocalAttention", "PEG", "PatchEmbedding", "Residual",
@@ -222,8 +222,8 @@ class Transformer(FusedEncoder, nn.Module):
         return x
 
     def encoder_layers(self) -> Tuple[List[EncoderLayer], Optional[Norm]]:
-        """Two EncoderLayers per Twins layer: (local attention, FF) with `window`, then (global attention, FF) with
-        `kv_stride` / `kv_w`; only the second where the layer has no local attention."""
+        """Two EncoderLayers per Twins layer: (local attention, FF) with Windows, then (global attention, FF) with
+        StridedKV; only the second where the layer has no local attention."""
         layers = []
         for local_attn, ff1, global_attn, ff2 in self.layers:
             for attn, ff in ((local_attn, ff1), (global_attn, ff2)):
@@ -238,8 +238,8 @@ class Transformer(FusedEncoder, nn.Module):
                     ln1=_norm(a.norm), qkv_w=qkv_w, out_w=a.to_out[0].weight.reshape(D, I), out_b=a.to_out[0].bias,
                     ln2=_norm(f[0]), fc1_w=f[1].weight.reshape(-1, D), fc1_b=f[1].bias,
                     fc2_w=f[4].weight.reshape(D, -1), fc2_b=f[4].bias, heads=a.heads, dim_head=I // a.heads,
-                    scale=a.scale, window=a.patch_size if local else None,
-                    kv_stride=None if local else a.to_kv.kernel_size[0], kv_w=None if local else a.to_kv.weight))
+                    scale=a.scale,
+                    attention=Windows(a.patch_size) if local else StridedKV(a.to_kv.kernel_size[0], a.to_kv.weight)))
         return layers, None
 
 
@@ -369,7 +369,7 @@ class TwinsSVT(FusedWeightsMixin, nn.Module):
         # b200vit_attention_kv's limit
         for (_, t1, _, t2), (h, w) in zip(self.stages(), grids):
             for t in (t1, t2):
-                r = t.engine().unsupported_reason(h * w)
+                r = t.engine().unsupported_reason(h * w, grid=(h, w))
                 if r is not None:
                     return r
         return None

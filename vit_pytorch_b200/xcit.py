@@ -36,9 +36,9 @@ import torch.nn.functional as F
 from torch import nn
 
 from .cait import dropout_layers
-from .engine import (CrossAttentionEngine, CrossLayer, EncoderLayer, FeedForwardBlock, FusedWeightsMixin, LPIBlock,
-                     Norm, _f32, cached, cls_row_index, common_reason, head_engine, head_ln_pool, lpi_reason,
-                     on_device, patch_engine)
+from .engine import (CrossAttentionEngine, CrossCovariance, CrossLayer, EncoderLayer, FeedForwardBlock,
+                     FusedWeightsMixin, LPIBlock, Norm, _f32, cached, cls_row_index, common_reason, head_engine,
+                     head_ln_pool, lpi_reason, on_device, patch_engine)
 from . import _lib
 from .vit import FeedForward, FusedTransformer, Patchify
 
@@ -297,7 +297,7 @@ class XCATransformer(FusedTransformer):
                 ln1=Norm.of(attn.norm), qkv_w=attn.to_qkv.weight, out_w=out.weight, out_b=out.bias,
                 ln2=Norm.of(ff.net[0]), fc1_w=fc1.weight, fc1_b=fc1.bias, fc2_w=fc2.weight, fc2_b=fc2.bias,
                 heads=attn.heads, dim_head=attn.dim_head, scale=1.0, out_scale=ls_attn.scale, ff_scale=ls_ff.scale,
-                xca_tau=attn.temperature,
+                attention=CrossCovariance(attn.temperature),
                 lpi=LPIBlock(ln=Norm.of(net[0]), conv1_w=conv1.weight, conv1_b=conv1.bias, bn_w=bn.weight,
                              bn_b=bn.bias, bn_mean=bn.running_mean, bn_var=bn.running_var, bn_eps=bn.eps,
                              conv2_w=conv2.weight, conv2_b=conv2.bias, scale=ls_lpi.scale,
