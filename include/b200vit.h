@@ -720,6 +720,35 @@ int b200vit_relu_maxpool(const void* y, int64_t M, int B, int H, int W, int C, i
 int b200vit_seq_pool(const float* x, int B, int n, int D, const float* gamma, const float* beta, float eps,
                      const float* w, const float* bias, void* out_bf16, int64_t ldo, void* stream);
 
+/*
+ * NesT's level boundaries (nest.py).  A level's stream is block-major: with its H x W map cut into nb x nb blocks of
+ * sh x sw tokens (sh = H/nb, sw = W/nb), token (b, y, x) is at row
+ *   ((b*nb + y/sh)*nb + x/sw)*(sh*sw) + (y % sh)*sw + (x % sw),
+ * the reference's '(b b1 b2)' blocks with their tokens in '(h w)' order.  The last level (nb = 1) is in map order.
+ *
+ * b200vit_nest_level_entry: y[M, D] fp32 in map order (M = B*H*W, row (b*H + y)*W + x) ->
+ *   x[block-major row of (b, r, q)] = max_{i, j < pk} LN(y[(b, r*ps - pp + i, q*ps - pp + j)]) + pos[(r % sh)*sw + q % sw]
+ * over the oh x ow pooled map (oh = (H + 2pp - pk) / ps + 1, likewise ow) cut into nb x nb blocks of sh = oh/nb by
+ * sw = ow/nb tokens.  LN is the LayerNorm over the D channels of a pixel (gamma, beta, eps; biased variance, eps
+ * inside the sqrt); the pool counts padding as -inf and propagates NaN as F.max_pool2d does; pos[n_pos] fp32 is the
+ * level's scalar position embedding, n_pos >= sh*sw.  xb_bf16 and stats (both or neither): the bf16 copy of x and its
+ * row statistics [B*oh*ow][2], the bits b200vit_rowstats_cast writes for x.  1 <= pk <= B200VIT_NEST_POOL_MAX_KERNEL,
+ * ps >= 1, 0 <= pp <= pk / 2, H + 2pp and W + 2pp >= pk, oh and ow multiples of nb; y, x, xb_bf16, gamma, beta
+ * 16-byte aligned, stats 8-byte aligned; the outputs must not overlap y.  Exactly the B*oh*ow rows of x (xb_bf16,
+ * stats) are written, and an output pixel reads only its own image's pool window.
+ *
+ * b200vit_nest_im2col: the A operand of a Conv2d(D, *, 3, padding = 1) over the map of a block-major stream x[M, D]
+ * fp32 (M = B*H*W, nb x nb blocks) -> out[(b*H + y)*W + x, (i*3 + j)*D + c] bf16 = x[(b, y - 1 + i, x - 1 + j), c]
+ * rounded to nearest, zero outside the map and in the K padding [9D, ldo).  D a multiple of 8, H and W multiples of
+ * nb, ldo a multiple of 8 and >= 9D; x and out_bf16 16-byte aligned and not overlapping.
+ */
+#define B200VIT_NEST_POOL_MAX_KERNEL 3
+int b200vit_nest_level_entry(const float* y, int64_t M, const float* gamma, const float* beta, float eps,
+                             const float* pos, int n_pos, float* x, void* xb_bf16, float* stats, int B, int H, int W,
+                             int D, int pk, int ps, int pp, int nb, void* stream);
+int b200vit_nest_im2col(const float* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W, int D, int nb,
+                        void* stream);
+
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */
 int b200vit_mean_pool(const float* x, float* out, int B, int N, int D, int n_pool, void* stream);

@@ -50,6 +50,7 @@ SYMBOLS = [
     "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw", "b200vit_mbconv_dwconv_ex",
     "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex", "b200vit_attention_window_token",
     "b200vit_window_mix", "b200vit_head_layernorm_gelu", "b200vit_attention_region_local",
+    "b200vit_nest_level_entry", "b200vit_nest_im2col",
 ]
 
 
@@ -182,6 +183,11 @@ def lib() -> C.CDLL:
     L.b200vit_head_layernorm_gelu.argtypes = [vp, i64, vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_attention_region_local.restype = i32
     L.b200vit_attention_region_local.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_nest_level_entry.restype = i32
+    L.b200vit_nest_level_entry.argtypes = [vp, i64, vp, vp, f32, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32,
+                                           i32, vp]
+    L.b200vit_nest_im2col.restype = i32
+    L.b200vit_nest_im2col.argtypes = [vp, i64, vp, i64, i32, i32, i32, i32, i32, vp]
     L.b200vit_se_pool.restype = i32
     L.b200vit_se_pool.argtypes = [vp, vp, i32, i32, i32, f32, vp]
     L.b200vit_se_scale.restype = i32
@@ -1268,6 +1274,48 @@ def relu_maxpool(y: torch.Tensor, B: int, H: int, W: int, pk: int, ps: int, pp: 
         rc = lib().b200vit_relu_maxpool(_ptr(y), M, B, H, W, Cc, int(pk), int(ps), int(pp), _ptr(out_bf16),
                                         _ptr(out_f32), out.stride(0), _stream())
     _check(rc, "b200vit_relu_maxpool")
+
+
+NEST_POOL_MAX_KERNEL = 3      # B200VIT_NEST_POOL_MAX_KERNEL
+
+
+def nest_level_entry(y: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, pos: torch.Tensor, x: torch.Tensor,
+                     B: int, H: int, W: int, pk: int, ps: int, pp: int, nb: int, *, eps: float = 1e-5,
+                     xb: Optional[torch.Tensor] = None, stats: Optional[torch.Tensor] = None) -> None:
+    """NesT's level entry: y fp32 [B*H*W, D] in map order -> x fp32 [B*oh*ow, D] = max_pool2d(LN(y), pk, ps, pp) +
+    pos[r], in the block-major order of nb x nb blocks (r the token's place in its block); with xb / stats (both or
+    neither) also the bf16 copy of x and its row statistics, as rowstats_cast writes them."""
+    for nm, t in (("y", y), ("gamma", gamma), ("beta", beta), ("pos", pos), ("x", x), ("stats", stats)):
+        _chk(t, torch.float32, nm)
+    _chk(xb, torch.bfloat16, "xb")
+    M, D = y.shape
+    for t in (y, x, gamma, beta, pos, xb, stats):
+        assert t is None or t.is_contiguous()
+    rows = B * conv_out_size(H, pk, ps, pp) * conv_out_size(W, pk, ps, pp)
+    assert gamma.numel() == D and beta.numel() == D and x.shape == (rows, D), \
+        f"x must be [{rows}, {D}], got {tuple(x.shape)}"
+    assert xb is None or xb.shape == (rows, D)
+    assert stats is None or stats.numel() == 2 * rows
+    with _Timed("nest_level_entry", B=B, H=H, W=W, D=D, pk=pk, ps=ps, pp=pp, nb=nb,
+                bytes=M * D * 4 + rows * D * (4 + (2 if xb is not None else 0)) + (rows * 8 if stats is not None else 0)):
+        rc = lib().b200vit_nest_level_entry(_ptr(y), M, _ptr(gamma), _ptr(beta), float(eps), _ptr(pos), pos.numel(),
+                                            _ptr(x), _ptr(xb), _ptr(stats), B, int(H), int(W), D, int(pk), int(ps),
+                                            int(pp), int(nb), _stream())
+    _check(rc, "b200vit_nest_level_entry")
+
+
+def nest_im2col(x: torch.Tensor, out_bf16: torch.Tensor, B: int, H: int, W: int, nb: int) -> None:
+    """x fp32 [B*H*W, D] block-major (nb x nb blocks) -> out bf16 [B*H*W, ldo] in map order, column (i*3 + j)*D + c the
+    channel c of pixel (y - 1 + i, x - 1 + j) (zero outside the map), zero K padding up to ldo = out.stride(0)."""
+    _chk(x, torch.float32, "x"); _chk(out_bf16, torch.bfloat16, "out")
+    assert x.dim() == 2 and x.is_contiguous() and out_bf16.dim() == 2 and out_bf16.stride(1) == 1
+    M, D = x.shape
+    assert out_bf16.shape[0] == M and out_bf16.shape[1] >= 9 * D, \
+        f"out must be [{M}, >= {9 * D}], got {tuple(out_bf16.shape)}"
+    with _Timed("nest_im2col", B=B, H=H, W=W, D=D, nb=nb, bytes=M * D * 4 + M * out_bf16.stride(0) * 2):
+        rc = lib().b200vit_nest_im2col(_ptr(x), M, _ptr(out_bf16), out_bf16.stride(0), B, int(H), int(W), D, int(nb),
+                                       _stream())
+    _check(rc, "b200vit_nest_im2col")
 
 
 def seq_pool(x: torch.Tensor, B: int, n: int, gamma: torch.Tensor, beta: torch.Tensor, w: torch.Tensor,

@@ -100,9 +100,6 @@ im2col_nhwc_kernel(const uint4* __restrict__ x, long long lx8, uint4* __restrict
   }
 }
 
-// max that keeps a NaN once it has seen one, as F.max_pool2d does (fmaxf would drop it)
-__device__ __forceinline__ float nan_max(float m, float v) { return (v > m || v != v) ? v : m; }
-
 // y [B*H*W, C] bf16 channels-last; out pixel (b, r, q) = relu(max of y over the pixels (r*ps - pp + i, q*ps - pp + j),
 // i, j < pk, inside the image), channels-last, row stride ldo elements.  One thread per (output pixel, 8 channels).
 template <bool F32>

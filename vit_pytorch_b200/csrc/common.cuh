@@ -443,6 +443,9 @@ __device__ __forceinline__ void gelu_erf2(float& a, float& b) {
   f2_get(f2_mul(x, f2_make(fast_rcp(d0), fast_rcp(d1))), a, b);
 }
 
+// max that keeps a NaN once it has seen one, as F.max_pool2d does (fmaxf would drop it)
+__device__ __forceinline__ float nan_max(float m, float v) { return (v > m || v != v) ? v : m; }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
