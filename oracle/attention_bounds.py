@@ -46,7 +46,7 @@ What the kernel can do differently from that replay, and the bound of each:
 from __future__ import annotations
 
 import math
-from typing import Sequence, Tuple
+from typing import Optional, Sequence, Tuple
 
 import torch
 
@@ -77,11 +77,15 @@ def _bf16(x: Tensor) -> Tensor:
 
 
 def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: int = 64, emul: bool = False,
-                        mask_self: bool = False, elems: int = 1 << 23) -> Tuple[Tensor, Tensor]:
+                        mask_self: bool = False, key_mask: Optional[Tensor] = None, zero_masked_rows: bool = False,
+                        elems: int = 1 << 23) -> Tuple[Tensor, Tensor]:
     """(ref, bound) [G, n, dh] of the attention of G independent sequences of n tokens, q, k, v: [G, n, dh] bf16.
 
     kb: the instance's key block; emul: exponentials of the odd 8-key groups on the FMA path; mask_self: each query's
-    own key is excluded (n > 1).  Query rows go in chunks of at most `elems` scores, so 16384-key sequences fit."""
+    own key is excluded (n > 1); key_mask: None or bool [G, n] (True = keep), the masked keys -inf.  A sequence with no
+    kept key gets exactly 0 under zero_masked_rows, else every key at weight 1: the kernel's P = 1 and l = n are exact,
+    so its reference is the mean of the values with the P V and O fl(1 / l) terms alone.  Query rows go in chunks of at
+    most `elems` scores, so 16384-key sequences fit."""
     G, n, dh = q.shape
     dev = q.device
     k64, v64 = k.double(), v.double()
@@ -96,6 +100,11 @@ def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: in
     if emul:
         emul_key = ((key % kb) // 8) % 2 == 1
         rel = torch.where(emul_key, torch.full_like(rel, EMUL_REL), rel)
+    empty = None
+    if key_mask is not None:
+        km = key_mask.to(device=dev, dtype=torch.bool)
+        empty = ~km.any(-1)[:, None, None]                              # [G, 1, 1]: no kept key
+        rel = torch.where(empty, torch.zeros_like(rel), rel)             # [G, 1, n]: P = 1 exactly there
     ref = torch.empty(G, n, dh, dtype=torch.float64, device=dev)
     bound = torch.empty_like(ref)
     rows = max(1, min(n, elems // max(1, G * n)))
@@ -109,6 +118,10 @@ def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: in
             qi = torch.arange(r0, r1, device=dev)
             valid = qi[:, None] != key[None, :]
         valid = valid.expand(G, -1, -1)
+        if key_mask is not None:
+            valid = (valid & km[:, None, :]) | empty
+            x = torch.where(empty, torch.zeros_like(x), x)
+            dx = torch.where(empty, torch.zeros_like(dx), dx)
         x = torch.where(valid, x, torch.full_like(x, -math.inf))
         dx = torch.where(valid, dx, torch.zeros_like(dx))
         pad = nb * kb - n
@@ -137,6 +150,9 @@ def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: in
         eta = dl / l
         e32 = (e_num / l + out.abs() * eta) / (1 - eta)
         e32 = e32 + 3 * U * (out.abs() + e32)
+        if key_mask is not None and zero_masked_rows:
+            out = torch.where(empty, torch.zeros_like(out), out)
+            e32 = torch.where(empty, torch.zeros_like(e32), e32)
         ref[:, r0:r1] = out
         bound[:, r0:r1] = e32 + 0.5 * bf16_ulp(out.abs() + e32)
     return ref, bound

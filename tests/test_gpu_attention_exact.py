@@ -6,8 +6,8 @@ nor a dropped key at long lengths (one key of 4096 moves an output by ~2e-4).  S
      leave every other sequence's output bit-identical to the clean run -- each image of a batch is computed on its own;
   B. inputs whose answers are known exactly: q = 0 with indicator values (every included key gives 1/len, every
      excluded key exactly 0), values that are the one-hot sequence id, and dominant keys (out_i = v_i to the bit);
-  C. head routing of the head-mixing kernels: permutation mixes against plain attention, every head count, and random
-     mixes against an fp64 reference computed on the GPU in chunks of query rows;
+  C. head routing of the head-mixing kernels: permutation mixes and random mixes at every head count, each output
+     element within the bound of the fp64 references of oracle/headmix_bounds.py and oracle/attention_fp32_bounds.py;
   D. the GEMM's operand margins: NaN beyond K, past M and past N must not reach the output.
 plus model-level batches with one NaN image.
 """
@@ -17,6 +17,9 @@ import math
 import pytest
 import torch
 
+from oracle import attention_fp32_bounds as FB
+from oracle import bounds as Bd
+from oracle import headmix_bounds as HB
 from vit_pytorch_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -555,59 +558,33 @@ def test_attention_cls_uniform_exact_key_sets(kind, first):
 
 
 # ================================================================================================ C. head routing
-def headmix_fp64(qkv, B, N, H, dh, scale, pre, post, ln, chunk=256):
-    """fp64 reference on the GPU, query rows in chunks (N = 16384 fits)."""
-    q, k, v = qkv.double().view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
-    out = torch.empty(B, H, N, dh, device=DEV, dtype=torch.float64)
-    pre = None if pre is None else pre.double()
-    for i0 in range(0, N, chunk):
-        s = q[:, :, i0:i0 + chunk] @ k.transpose(-1, -2) * scale
-        if pre is not None:
-            s = torch.einsum('b h i j, h g -> b g i j', s, pre)
-        p = torch.einsum('b h i j, h g -> b g i j', s.softmax(-1), post.double())
-        if ln is not None:
-            p = torch.nn.functional.layer_norm(p.permute(0, 2, 3, 1), (H,), ln[0].double(), ln[1].double(),
-                                               ln[2]).permute(0, 3, 1, 2)
-        out[:, :, i0:i0 + chunk] = p @ v
-    return out.permute(0, 2, 1, 3).reshape(B * N, H * dh)
-
-
-def close_to(out, ref, what):
-    tol = 1e-2 * ref.abs().max().item() + 1e-3
-    err = (out.double() - ref).abs()
-    assert err.max().item() <= 2 * tol, (what, err.max().item(), ref.abs().max().item())
-    assert (err <= tol + 1e-2 * ref.abs()).double().mean().item() > 0.999, what
-
-
 HEAD_COUNTS = [(H, dh) for dh in (32, 48, 64, 80, 128) for H in range(1, 17) if H * dh <= 1024]
+
+
+def perm_mixes(H, seed):
+    """pre = sigma and post = pi permutation matrices ([input head, output head]): s'_f = s_sigma(f), p'_f = p_pi(f)."""
+    pi = torch.randperm(H, generator=torch.Generator().manual_seed(H)).tolist()
+    sg = torch.randperm(H, generator=torch.Generator().manual_seed(H + seed)).tolist()
+    post, pre = torch.zeros(H, H, device=DEV), torch.zeros(H, H, device=DEV)
+    for f in range(H):
+        post[pi[f], f] = 1.0
+        pre[sg[f], f] = 1.0
+    return pi, sg, pre, post
 
 
 @pytest.mark.parametrize("H,dh", HEAD_COUNTS)
 def test_attention_headmix_permutation_routes_heads(H, dh):
     """pre = sigma and post = pi permutation matrices, no LayerNorm: output head f is plain attention with the scores
-    of head sigma(pi(f)) and the values of head f -- checked against b200vit_attention on the rearranged heads."""
+    of head sigma(pi(f)) and the values of head f -- within the bound of oracle/headmix_bounds.py, whose fp64
+    reference routes the heads by the matrices alone."""
     B, N = 2, 77
     g = torch.Generator(device=DEV).manual_seed(H * 1000 + dh)
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV, generator=g).bfloat16()
-    pi = torch.randperm(H, generator=torch.Generator().manual_seed(H)).tolist()
-    sg = torch.randperm(H, generator=torch.Generator().manual_seed(H + 99)).tolist()
-    post = torch.zeros(H, H, device=DEV)
-    pre = torch.zeros(H, H, device=DEV)
-    for f in range(H):
-        post[pi[f], f] = 1.0           # p'_f = p_{pi(f)}
-        pre[sg[f], f] = 1.0            # s'_f = s_{sigma(f)}
+    _, _, pre, post = perm_mixes(H, 99)
     for use_pre in (False, True):
-        src = [sg[pi[f]] if use_pre else pi[f] for f in range(H)]
-        out = run_headmix(qkv, B, N, H, dh, pre if use_pre else None, post, None)
-        t = qkv.view(B * N, 3, H, dh)
-        re = torch.cat([t[:, 0, src], t[:, 1, src], t[:, 2]], 1).reshape(B * N, 3 * H * dh).contiguous()
-        if dh == 48:                   # b200vit_attention has no 48-wide instance: the fp64 reference instead
-            want = headmix_fp64(re, B, N, H, dh, dh ** -0.5, None, torch.eye(H, device=DEV), None)
-        else:
-            want = torch.empty(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
-            _lib.attention(re, want, B, N, H, dh, dh ** -0.5)
-            want = want.double()
-        close_to(out, want, (use_pre, src))
+        p_ = pre if use_pre else None
+        out = run_headmix(qkv, B, N, H, dh, p_, post, None)
+        Bd.check(out, *HB.headmix_reference(qkv, B, N, H, dh, dh ** -0.5, p_, post), f"permutation pre={use_pre}")
 
 
 @pytest.mark.parametrize("H,dh", HEAD_COUNTS)
@@ -619,7 +596,8 @@ def test_attention_headmix_random_mix_every_head_count(H, dh):
     ln = (1 + 0.2 * torch.randn(H, device=DEV, generator=g), 0.1 * torch.randn(H, device=DEV, generator=g), 1e-5)
     for p_, l_ in ((None, None), (pre, None), (None, ln), (pre, ln)):
         out = run_headmix(qkv, B, N, H, dh, p_, post, l_)
-        close_to(out, headmix_fp64(qkv, B, N, H, dh, dh ** -0.5, p_, post, l_), (p_ is not None, l_ is not None))
+        Bd.check(out, *HB.headmix_reference(qkv, B, N, H, dh, dh ** -0.5, p_, post, l_),
+                 f"random mix pre={p_ is not None} ln={l_ is not None}")
 
 
 @pytest.mark.parametrize("H,dh", [(6, 48), (16, 64), (5, 80)])
@@ -629,19 +607,7 @@ def test_attention_headmix_random_mix_16384(H, dh):
     qkv = torch.randn(N, 3 * H * dh, device=DEV, generator=g).bfloat16()
     pre, post = torch.randn(H, H, device=DEV, generator=g), torch.randn(H, H, device=DEV, generator=g)
     out = run_headmix(qkv, 1, N, H, dh, pre, post, None)
-    close_to(out, headmix_fp64(qkv, 1, N, H, dh, dh ** -0.5, pre, post, None, chunk=64), "16384")
-
-
-def cls_headmix_fp64(qkv_self, ctx, rows, first, n, H, dh, scale, pre, post):
-    B, I = qkv_self.shape[0], H * dh
-    q, ks, vs = qkv_self.double().view(B, 3, H, dh).unbind(1)
-    c = ctx.double().view(B, rows, -1)[:, first:first + n, :2 * I]
-    k = torch.cat([ks[:, None], c[..., :I].reshape(B, n, H, dh)], 1)
-    v = torch.cat([vs[:, None], c[..., I:].reshape(B, n, H, dh)], 1)
-    s = torch.einsum('b h d, b j h d -> b h j', q, k) * scale
-    p = torch.einsum('b h j, h g -> b g j', torch.einsum('b h j, h g -> b g j', s, pre.double()).softmax(-1),
-                     post.double())
-    return torch.einsum('b h j, b j h d -> b h d', p, v).reshape(B, I)
+    Bd.check(out, *HB.headmix_reference(qkv, 1, N, H, dh, dh ** -0.5, pre, post), "16384")
 
 
 @pytest.mark.parametrize("H,dh", HEAD_COUNTS)
@@ -651,22 +617,11 @@ def test_attention_cls_headmix_every_head_count(H, dh):
     qkv_self, ctx, rows = cls_inputs(B, n, first, H, dh, g)
     pre, post = torch.randn(H, H, device=DEV, generator=g), torch.randn(H, H, device=DEV, generator=g)
     out = run_cls("cls_headmix", qkv_self, ctx, rows, first, n, H, dh, pre, post)
-    close_to(out, cls_headmix_fp64(qkv_self, ctx, rows, first, n, H, dh, dh ** -0.5, pre, post), "random")
+    Bd.check(out, *FB.cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, dh ** -0.5, pre, post), "random")
     # permutations: output head f = plain class attention of scores sigma(pi(f)), values f
-    pi = torch.randperm(H, generator=torch.Generator().manual_seed(H)).tolist()
-    sg = torch.randperm(H, generator=torch.Generator().manual_seed(H + 5)).tolist()
-    P, S = torch.zeros(H, H, device=DEV), torch.zeros(H, H, device=DEV)
-    for f in range(H):
-        P[pi[f], f] = 1.0
-        S[sg[f], f] = 1.0
+    _, _, S, P = perm_mixes(H, 5)
     out = run_cls("cls_headmix", qkv_self, ctx, rows, first, n, H, dh, S, P)
-    src = [sg[pi[f]] for f in range(H)]
-    qs = qkv_self.view(B, 3, H, dh)
-    re_self = torch.cat([qs[:, 0, src], qs[:, 1, src], qs[:, 2]], 1).reshape(B, 3 * H * dh).contiguous()
-    c = ctx.view(B * rows, -1)
-    re_ctx = torch.cat([c[:, :H * dh].reshape(-1, H, dh)[:, src].reshape(-1, H * dh), c[:, H * dh:]], 1).contiguous()
-    eye = torch.eye(H, device=DEV)
-    close_to(out, cls_headmix_fp64(re_self, re_ctx, rows, first, n, H, dh, dh ** -0.5, eye, eye), "permutation")
+    Bd.check(out, *FB.cls_headmix_reference(qkv_self, ctx, rows, first, n, H, dh, dh ** -0.5, S, P), "permutation")
 
 
 # ================================================================================================ D. GEMM margins

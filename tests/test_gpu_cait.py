@@ -1,16 +1,16 @@
 """-m gpu: the talking-heads attention kernels (b200vit_attention_headmix_ex with a pre-softmax mix,
-b200vit_attention_cls_headmix) and the fused CaiT on the H100.  The kernels are checked against fp32 torch expressions
-on the same bf16 data; the model's CUDA-graph replay and fallback rules (its reference parity is in
-test_gpu_family_parity.py)."""
+b200vit_attention_cls_headmix) and the fused CaiT on the H100.  Every element of the kernels' outputs is checked against
+the fp64 references and bounds of oracle/headmix_bounds.py and oracle/attention_fp32_bounds.py; the model's CUDA-graph
+replay and fallback rules (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR
 from oracle import attention_fp32_bounds as FB
 from oracle import bounds as Bd
+from oracle import headmix_bounds as HB
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.cait import CaiT, Transformer
 
@@ -26,25 +26,7 @@ def stats(got, ref, rtol=1e-2, atol=1e-3):
     return d.max().item(), (d <= atol + rtol * ref.float().cpu().abs()).float().mean().item()
 
 
-def close_to(out, ref):
-    tol = 1e-2 * ref.abs().max().item() + 1e-3
-    err = (out.float() - ref).abs()
-    assert err.max().item() <= tol + 1e-2 * ref.abs().max().item(), (err.max().item(), ref.abs().max().item())
-    assert (err <= tol + 1e-2 * ref.abs()).float().mean().item() > 0.999
-
-
 # ------------------------------------------------------------------------------------------------ attention_headmix_ex
-def headmix_reference(qkv, B, N, H, dh, scale, pre, post, ln):
-    """fp32 (q k^T scale) mixed by pre, softmax, mixed by post (both 'b h i j, h g -> b g i j'), LayerNorm over the
-    heads of every (i, j) if ln = (gamma, beta, eps), then times v (cait.py:92-101)."""
-    q, k, v = qkv.float().view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
-    s = torch.einsum('b h i j, h g -> b g i j', q @ k.transpose(-1, -2) * scale, pre)
-    p = torch.einsum('b h i j, h g -> b g i j', s.softmax(-1), post)
-    if ln is not None:
-        p = F.layer_norm(p.permute(0, 2, 3, 1), (H,), ln[0], ln[1], ln[2]).permute(0, 3, 1, 2)
-    return (p @ v).permute(0, 2, 1, 3).reshape(B * N, H * dh)
-
-
 def headmix_inputs(B, N, H, dh, seed):
     g = torch.Generator(device=DEV).manual_seed(seed)
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV, generator=g).bfloat16()
@@ -67,7 +49,7 @@ def test_attention_headmix_pre_against_fp32(H, dh, N, mode):
     scale = dh ** -0.5
     out = torch.empty(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
     _lib.attention_headmix(qkv, out, B, N, H, dh, scale, post, ln, pre=pre)
-    close_to(out, headmix_reference(qkv, B, N, H, dh, scale, pre, post, ln))
+    Bd.check(out, *HB.headmix_reference(qkv, B, N, H, dh, scale, pre, post, ln), f"headmix H{H} dh{dh} N{N} {mode}")
 
 
 def test_one_head_negative_pre_turns_the_softmax_around():
@@ -77,9 +59,9 @@ def test_one_head_negative_pre_turns_the_softmax_around():
     pre, post = torch.full((1, 1), -1.0, device=DEV), torch.ones(1, 1, device=DEV)
     out = torch.empty(B * N, dh, device=DEV, dtype=torch.bfloat16)
     _lib.attention_headmix(qkv, out, B, N, H, dh, 0.125, post, None, pre=pre)
-    close_to(out, headmix_reference(qkv, B, N, H, dh, 0.125, pre, post, None))
-    plain = headmix_reference(qkv, B, N, H, dh, 0.125, -pre, post, None)
-    assert (out.float() - plain).abs().max().item() > 0.1
+    Bd.check(out, *HB.headmix_reference(qkv, B, N, H, dh, 0.125, pre, post), "pre = -1")
+    plain, _ = HB.headmix_reference(qkv, B, N, H, dh, 0.125, -pre, post)
+    assert (out.double() - plain).abs().max().item() > 0.1
 
 
 # ------------------------------------------------------------------------------------------------ attention_cls_headmix

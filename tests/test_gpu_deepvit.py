@@ -1,13 +1,14 @@
-"""-m gpu: the head-mixing attention kernel (b200vit_attention_headmix) and the fused DeepViT on the H100.  The kernel
-is checked against an fp32 torch expression on the same bf16 data; the model at batch one, its CUDA-graph replay
+"""-m gpu: the head-mixing attention kernel (b200vit_attention_headmix) and the fused DeepViT on the H100.  Every
+element of the kernel's output is checked against the fp64 reference and bound of oracle/headmix_bounds.py; the model at batch one, its CUDA-graph replay
 and fallback rules (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR
+from oracle import bounds as Bd
+from oracle import headmix_bounds as HB
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.deepvit import DeepViT, Transformer
 
@@ -24,17 +25,6 @@ def stats(got, ref, rtol=1e-2, atol=1e-3):
 
 
 # ------------------------------------------------------------------------------------------------ attention_headmix
-def headmix_reference(qkv, B, N, H, dh, scale, post, ln):
-    """fp32 softmax(q k^T scale), mixed across heads by post ('b h i j, h g -> b g i j'), LayerNorm over the heads of
-    every (i, j) if ln = (gamma, beta, eps), then times v (deepvit.py:56-67)."""
-    q, k, v = qkv.float().view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
-    p = (q @ k.transpose(-1, -2) * scale).softmax(-1)
-    p = torch.einsum('b h i j, h g -> b g i j', p, post)
-    if ln is not None:
-        p = F.layer_norm(p.permute(0, 2, 3, 1), (H,), ln[0], ln[1], ln[2]).permute(0, 3, 1, 2)
-    return (p @ v).permute(0, 2, 1, 3).reshape(B * N, H * dh)
-
-
 def headmix_inputs(B, N, H, dh, seed):
     g = torch.Generator(device=DEV).manual_seed(seed)
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV, generator=g).bfloat16()
@@ -56,11 +46,7 @@ def test_attention_headmix_against_fp32(H, dh, N, mode):
     scale = dh ** -0.5
     out = torch.empty(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
     _lib.attention_headmix(qkv, out, B, N, H, dh, scale, post, ln)
-    ref = headmix_reference(qkv, B, N, H, dh, scale, post, ln)
-    tol = 1e-2 * ref.abs().max().item() + 1e-3
-    err = (out.float() - ref).abs()
-    assert err.max().item() <= tol + 1e-2 * ref.abs().max().item(), (err.max().item(), ref.abs().max().item())
-    assert (err <= tol + 1e-2 * ref.abs()).float().mean().item() > 0.999
+    Bd.check(out, *HB.headmix_reference(qkv, B, N, H, dh, scale, None, post, ln), f"headmix H{H} dh{dh} N{N} {mode}")
 
 
 @pytest.mark.parametrize("H,dh,N", [(16, 64, 197), (3, 48, 65), (8, 128, 577)])
@@ -84,9 +70,11 @@ def test_one_head_layernorm_gives_beta():
     ln = (torch.tensor([1.3], device=DEV), torch.tensor([0.25], device=DEV), 1e-5)
     out = torch.empty(B * N, dh, device=DEV, dtype=torch.bfloat16)
     _lib.attention_headmix(qkv, out, B, N, H, dh, 0.125, post, ln)
-    v = qkv.float().view(B, N, 3, dh)[:, :, 2]
+    v = qkv.double().view(B, N, 3, dh)[:, :, 2]
     want = (0.25 * v.sum(1, keepdim=True)).expand(B, N, dh).reshape(B * N, dh)
-    assert stats(out, want, rtol=1e-2, atol=2e-2)[1] == 1.0
+    ref, bound = HB.headmix_reference(qkv, B, N, H, dh, 0.125, None, post, ln)
+    assert torch.allclose(ref, want, rtol=1e-12, atol=1e-12)
+    Bd.check(out, ref, bound, "one head")
 
 
 # ------------------------------------------------------------------------------------------------ model

@@ -1,5 +1,6 @@
 """-m gpu: the strided short-sequence attention kernel, the grouped token assembly and the fused ViViT on the H100.
-The kernels are checked against torch expressions on the same bf16 data; the model's fallback rules, direct
+Every element of the attention kernel's output is checked against the fp64 reference and bound of
+oracle/attention_bounds.py, the token assembly against a torch expression; the model's fallback rules, direct
 transformer calls and LayerNorm modes (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
@@ -7,6 +8,8 @@ import pytest
 import torch
 
 from conftest import GOLDEN_DIR
+from oracle import bounds as Bd
+from oracle.attention_bounds import attention_reference
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.vivit import FactorizedTransformer, Transformer, ViViT
 
@@ -25,18 +28,14 @@ def stats(got, ref):
 
 # ------------------------------------------------------------------------------------------------------ attention_axial
 def axial_reference(qkv, key_mask, B, L, G, H, dh, scale, zero_masked_rows):
-    """fp32 attention of the B*G sequences (token j of b*G + p at row b*L*G + j*G + p); masked keys filled with
-    -finfo.max, so a row without a kept key averages all values, then zeroed in the SDPA mode."""
-    t = qkv.float().view(B, L, G, 3, H, dh).permute(3, 0, 2, 4, 1, 5)          # (3, B, G, H, L, dh)
-    q, k, v = t[0], t[1], t[2]
-    dots = q @ k.transpose(-1, -2) * scale
-    if key_mask is not None:
-        keep = key_mask.bool()[:, None, None, None, :]
-        dots = dots.masked_fill(~keep, -torch.finfo(dots.dtype).max)
-    out = dots.softmax(dim=-1) @ v
-    if key_mask is not None and zero_masked_rows:
-        out = out.masked_fill(~key_mask.bool().any(dim=1)[:, None, None, None, None], 0.0)
-    return out.permute(0, 3, 1, 2, 4).reshape(B * L * G, H * dh)               # (B, L, G, H, dh)
+    """(ref, bound) [B L G, H dh] of the B*G*H sequences (token j of b*G + p at row b*L*G + j*G + p) from
+    attention_bounds.attention_reference with the key mask of each sequence's batch element: one 64-key block, a row
+    without a kept key 0 (zero_masked_rows) or the mean of its sequence's values."""
+    t = qkv.view(B, L, G, 3, H, dh).permute(3, 0, 2, 4, 1, 5).reshape(3, B * G * H, L, dh)
+    km = None if key_mask is None else key_mask.bool()[:, None, None, :].expand(B, G, H, L).reshape(B * G * H, L)
+    ref, bound = attention_reference(t[0], t[1], t[2], scale, kb=64, key_mask=km, zero_masked_rows=zero_masked_rows)
+    back = lambda x: x.view(B, G, H, L, dh).permute(0, 3, 1, 2, 4).reshape(B * L * G, H * dh)   # noqa: E731
+    return back(ref), back(bound)
 
 
 @pytest.mark.parametrize("dh", [32, 64, 80, 128])
@@ -60,9 +59,8 @@ def test_attention_axial_against_fp32(dh, L, G):
             # out has rows beyond the addressed set: they must keep their NaN fill
             buf = torch.full((T + 5, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
             _lib.attention_axial(qkv, buf[:T], km8, B, L, G, H, dh, scale, zero)
-            want = axial_reference(qkv, km, B, L, G, H, dh, scale, zero)
-            mx = (buf[:T].float() - want).abs().max().item()
-            assert mx < 2e-2, (name, zero, mx)
+            ref, bound = axial_reference(qkv, km, B, L, G, H, dh, scale, zero)
+            Bd.check(buf[:T], ref, bound, f"axial {name} zero={zero}")
             assert torch.isnan(buf[T:].float()).all()
             again = torch.empty(T, H * dh, device=DEV, dtype=torch.bfloat16)
             _lib.attention_axial(qkv, again, km8, B, L, G, H, dh, scale, zero)
