@@ -263,6 +263,19 @@ int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldk
                          int H, int dh, float scale, void* stream);
 
 /*
+ * b200vit_attention_kv with key heads of another width than the value heads (ScalableViT's SSA,
+ * scalable_vit.py:71-124, where dim_key and dim_value are separate hyperparameters):
+ *   q[B*Nq, H*dk] bf16 (row stride ldq), kv[B*Nk, H*dk + H*dv] bf16 packed k | v (row stride ldkv), head-major;
+ *   out[B*Nq, H*dv] bf16 (contiguous) = softmax(scale * q k^T) v per image and head.
+ * dk = 16, 32, 48 or 64; dv = 32 or 64.  A dim_key that is a multiple of 8 runs at the next multiple of 16: the caller
+ * inserts zero columns per head in q and k (zero rows of their projection weights), which add exactly 0 to every score,
+ * and passes the scale of the unpadded width.  out must overlap neither q nor kv.  Everything else (tiling, limits,
+ * checks, isolation) as b200vit_attention_kv, which is this call with dk = dv = dh (dh = 32, 64, 80 or 128).
+ */
+int b200vit_attention_kv_ex(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq, int Nk,
+                            int H, int dk, int dv, float scale, void* stream);
+
+/*
  * Attention with a learned relative-position bias over an F x F token map (LeViT, levit.py:40-108):
  *   qkv[B*F*F, ld] bf16, token (b, y, x) at row (b*F + y)*F + x; columns q (H*dk) | k (H*dk) | v (H*dv), head-major.
  *   Queries are the tokens (s*i, s*j), i, j < Fq = ceil(F / s), s = 1 or 2 (the downsampling attention's stride-2
@@ -748,6 +761,25 @@ int b200vit_nest_level_entry(const float* y, int64_t M, const float* gamma, cons
                              int D, int pk, int ps, int pp, int nb, void* stream);
 int b200vit_nest_im2col(const float* x, int64_t M, void* out_bf16, int64_t ldo, int B, int H, int W, int D, int nb,
                         void* stream);
+
+/*
+ * ScalableViT's interactive windowed self-attention (scalable_vit.py:155-194) over B channels-last token maps:
+ *   qkv[B*gh*gw, ld] bf16, token (b, y, x) at row (b*gh + y)*gw + x; columns q (H*dk) | k (H*dk) | v (H*dv),
+ *   head-major.  The map is cut into wh x ww windows (wh = gh, ww = gw: the whole map); per window and head
+ *     out = softmax(scale * q k^T) v + lim,
+ *   lim[B*gh*gw, H*dv] bf16 the local interactive module's output in map order, out[B*gh*gw, H*dv] bf16 in map order
+ *   (both contiguous).  The sum is formed in fp32, fma(O, 1 / l, lim) with O the unnormalised P V accumulator and l the
+ *   softmax denominator, and rounded to bf16 once.
+ * One CTA per 128 queries of a (window, head); keys and values stream in blocks of 64 with an fp32 online softmax,
+ * both products on wgmma; rows are gathered from their map-order addresses by cp.async, rows past the window are
+ * zero-filled and its keys masked.  One kernel for every window size from 1 to B200VIT_ATTN_KV_MAX_KEYS tokens.
+ * gh and gw multiples of wh and ww; dk = 16, 32, 48 or 64 (a padded dim_key as for b200vit_attention_kv_ex); dv = 32
+ * or 64; ld >= H*(2 dk + dv) and a multiple of 8; qkv, lim and out 16-byte aligned; out overlaps neither qkv nor lim;
+ * H <= 65535.  Isolation: a window's output is computed from its own rows and its lim rows only, so a NaN or Inf stays
+ * in its window, and nothing outside the B*gh*gw rows is read or written.
+ */
+int b200vit_attention_iwsa(const void* qkv, int64_t ld, const void* lim, void* out, int B, int gh, int gw, int wh,
+                           int ww, int H, int dk, int dv, float scale, void* stream);
 
 /* Mean over the first n_pool tokens of every image: x[B, N, D] fp32 -> out[B, D] fp32 (vit.py:135 pool == 'mean',
  * simple_vit.py:117: n_pool = N; simple_vit_with_register_tokens.py:130-132: the patch tokens only). */

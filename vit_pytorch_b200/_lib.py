@@ -50,7 +50,7 @@ SYMBOLS = [
     "b200vit_se_scale", "b200vit_conv_proj_dw", "b200vit_cross_embed_nchw", "b200vit_mbconv_dwconv_ex",
     "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex", "b200vit_attention_window_token",
     "b200vit_window_mix", "b200vit_head_layernorm_gelu", "b200vit_attention_region_local",
-    "b200vit_nest_level_entry", "b200vit_nest_im2col",
+    "b200vit_nest_level_entry", "b200vit_nest_im2col", "b200vit_attention_kv_ex", "b200vit_attention_iwsa",
 ]
 
 
@@ -161,6 +161,10 @@ def lib() -> C.CDLL:
     L.b200vit_attention_window.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_attention_kv.restype = i32
     L.b200vit_attention_kv.argtypes = [vp, i64, vp, i64, vp, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_attention_kv_ex.restype = i32
+    L.b200vit_attention_kv_ex.argtypes = [vp, i64, vp, i64, vp, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_attention_iwsa.restype = i32
+    L.b200vit_attention_iwsa.argtypes = [vp, i64, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_merge_patches_ln.restype = i32
     L.b200vit_merge_patches_ln.argtypes = [vp, i64, vp, vp, vp, i64, i32, i32, i32, i32, i32, f32, vp]
     L.b200vit_peg.restype = i32
@@ -660,6 +664,36 @@ def attention_kv(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, B: int, N
         rc = lib().b200vit_attention_kv(_ptr(q), q.stride(0), _ptr(kv), kv.stride(0), _ptr(out), B, int(Nq), int(Nk),
                                         H, dh, float(scale), _stream())
     _check(rc, "b200vit_attention_kv")
+
+
+def attention_kv_ex(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, B: int, Nq: int, Nk: int, H: int, dk: int,
+                    dv: int, scale: float) -> None:
+    """attention_kv with key heads dk wide and value heads dv wide: q[B*Nq, H*dk] (any row stride), kv[B*Nk, H*dk + H*dv]
+    packed k | v (any row stride), out[B*Nq, H*dv]."""
+    _chk(q, torch.bfloat16, "q"); _chk(kv, torch.bfloat16, "kv"); _chk(out, torch.bfloat16, "out")
+    assert q.dim() == 2 and q.stride(1) == 1 and kv.dim() == 2 and kv.stride(1) == 1 and out.is_contiguous()
+    assert q.shape == (B * Nq, H * dk) and kv.shape == (B * Nk, H * (dk + dv)) and out.shape == (B * Nq, H * dv)
+    with _Timed("attention_kv_ex", B=B, Nq=Nq, Nk=Nk, H=H, dk=dk, dv=dv,
+                bytes=(q.numel() + kv.numel() + out.numel()) * 2, flops=2.0 * B * H * Nq * Nk * (dk + dv)):
+        rc = lib().b200vit_attention_kv_ex(_ptr(q), q.stride(0), _ptr(kv), kv.stride(0), _ptr(out), B, int(Nq), int(Nk),
+                                           H, dk, dv, float(scale), _stream())
+    _check(rc, "b200vit_attention_kv_ex")
+
+
+def attention_iwsa(qkv: torch.Tensor, lim: torch.Tensor, out: torch.Tensor, B: int, gh: int, gw: int, wh: int, ww: int,
+                   H: int, dk: int, dv: int, scale: float) -> None:
+    """ScalableViT's windowed attention plus the local interactive module over B gh x gw maps in map order:
+    qkv[B*gh*gw, >= H*(2dk + dv)] q | k | v (any row stride), lim and out [B*gh*gw, H*dv]; per wh x ww window and head
+    out = softmax(scale q k^T) v + lim, summed in fp32 and rounded once."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(lim, torch.bfloat16, "lim"); _chk(out, torch.bfloat16, "out")
+    M = B * gh * gw
+    assert qkv.dim() == 2 and qkv.stride(1) == 1 and qkv.shape[0] == M and qkv.shape[1] >= H * (2 * dk + dv)
+    assert lim.is_contiguous() and out.is_contiguous() and lim.shape == out.shape == (M, H * dv)
+    with _Timed("attention_iwsa", B=B, h=gh, w=gw, wh=wh, ww=ww, H=H, dk=dk, dv=dv,
+                bytes=(M * H * (2 * dk + dv) + 2 * M * H * dv) * 2, flops=2.0 * M * H * wh * ww * (dk + dv)):
+        rc = lib().b200vit_attention_iwsa(_ptr(qkv), qkv.stride(0), _ptr(lim), _ptr(out), B, int(gh), int(gw), int(wh),
+                                          int(ww), H, dk, dv, float(scale), _stream())
+    _check(rc, "b200vit_attention_iwsa")
 
 
 def attention_posbias(qkv: torch.Tensor, out: torch.Tensor, table: torch.Tensor, B: int, F: int, s: int, H: int,

@@ -2,7 +2,9 @@
 // of a stage is kept token-major: x[B*gh*gw, C], token (b, y, x) at row (b*gh + y)*gw + x.  The window attention,
 // b200vit_attention_window, is in attention_tile64.cu.
 //   b200vit_attention_kv       every query of an image against that image's keys / values, which come from another
-//                              buffer and have another length (twins_svt.py:122-157: the sub-sampled keys)
+//                              buffer and have another length (twins_svt.py:122-157: the sub-sampled keys);
+//                              b200vit_attention_kv_ex takes key heads of another width than the value heads
+//                              (ScalableViT's SSA, scalable_vit.py:71-124)
 //   b200vit_merge_patches_ln   p x p patch merging + LayerNorm over the merged features (twins_svt.py:59-75)
 //   b200vit_peg                depthwise k x k convolution plus identity (twins_svt.py:77-83)
 //
@@ -27,31 +29,35 @@ constexpr int KV_RING = 4;             // block slots of the streaming mode
 constexpr int KV_SMEM = 200 * 1024;    // what a CTA may hold: the query tile and the resident key / value blocks
 constexpr int KV_MAX_SLOTS = 16;
 
-template <int DH>
+template <int DK, int DV>
 constexpr int kv_resident_slots() {
-  const int n = (KV_SMEM - 2 * Slabs<DH>::OP) / (2 * Slabs<DH>::OP);
+  const int n = (KV_SMEM - 2 * Slabs<DK>::OP) / (Slabs<DK>::OP + Slabs<DV>::OP);
   return n < KV_MAX_SLOTS ? n : KV_MAX_SLOTS;
 }
 
 struct KvParams {
   __nv_bfloat16* out;
-  int B, Nq, Nk, I;
+  int B, Nq, Nk;
+  int Ik, Iv;              // H * dk (q and k columns), H * dv (v and out columns)
   int slots;               // block slots in shared memory; all blocks resident iff ceil(Nk / 64) <= slots
   float scale_log2e;
 };
 
-template <int DH>
+// DK: width of the q and k heads, DV: of the v and output heads
+template <int DK, int DV>
 __global__ void __launch_bounds__(KV_THREADS)
 attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_constant__ CUtensorMap q16,
                     const __grid_constant__ CUtensorMap kv64, const __grid_constant__ CUtensorMap kv16,
                     const KvParams p) {
-  using S = Slabs<DH>;
-  constexpr int N64 = S::N64, N16 = S::N16;
+  using S = Slabs<DK>;
+  using SV = Slabs<DV>;
+  constexpr int N64 = SV::N64, N16 = SV::N16;
+  constexpr int SLOT = S::OP + SV::OP;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // Q: two operand blocks (one per warpgroup); then per slot K | V; then the barriers: Q, one per slot
   uint8_t* slot0 = smem + 2 * S::OP;
-  uint64_t* bar_q = reinterpret_cast<uint64_t*>(slot0 + (size_t)p.slots * 2 * S::OP);
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(slot0 + (size_t)p.slots * SLOT);
   uint64_t* bar_kv = bar_q + 1;
 
   const int h = blockIdx.y, b = blockIdx.z;
@@ -60,8 +66,8 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
   const bool resident = nkb <= p.slots;
 
   if (tid == 0) {
-    tma_prefetch_desc(N64 ? &q64 : &q16);
-    tma_prefetch_desc(N64 ? &kv64 : &kv16);
+    tma_prefetch_desc(S::N64 ? &q64 : &q16);
+    tma_prefetch_desc(S::N64 ? &kv64 : &kv16);
     mbar_init(bar_q, 1);
     for (int i = 0; i < p.slots; ++i) mbar_init(bar_kv + i, 1);
     fence_mbar_init();
@@ -69,17 +75,20 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
 
   auto load_block = [&](int j) {  // thread 0: keys [64 j, 64 j + 64) of image b into slot j % slots
     const int sl = j % p.slots;
-    uint8_t* dst = slot0 + (size_t)sl * 2 * S::OP;
-    mbar_arrive_expect_tx(bar_kv + sl, 2 * ROWS * DH * 2);
+    uint8_t* dst = slot0 + (size_t)sl * SLOT;
+    mbar_arrive_expect_tx(bar_kv + sl, ROWS * (DK + DV) * 2);
+    const int ck = h * DK;
 #pragma unroll
-    for (int o = 0; o < 2; ++o) {
-      const int col = o * p.I + h * DH;
+    for (int c = 0; c < S::N64; ++c) tma_load_3d(dst + c * S::S64, &kv64, bar_kv + sl, ck + 64 * c, 64 * j, b);
 #pragma unroll
-      for (int c = 0; c < N64; ++c) tma_load_3d(dst + o * S::OP + c * S::S64, &kv64, bar_kv + sl, col + 64 * c, 64 * j, b);
+    for (int c = 0; c < S::N16; ++c)
+      tma_load_3d(dst + S::N64 * S::S64 + c * S::S16, &kv16, bar_kv + sl, ck + 64 * S::N64 + 16 * c, 64 * j, b);
+    const int cv = p.Ik + h * DV;
 #pragma unroll
-      for (int c = 0; c < N16; ++c)
-        tma_load_3d(dst + o * S::OP + N64 * S::S64 + c * S::S16, &kv16, bar_kv + sl, col + 64 * N64 + 16 * c, 64 * j, b);
-    }
+    for (int c = 0; c < N64; ++c) tma_load_3d(dst + S::OP + c * SV::S64, &kv64, bar_kv + sl, cv + 64 * c, 64 * j, b);
+#pragma unroll
+    for (int c = 0; c < N16; ++c)
+      tma_load_3d(dst + S::OP + N64 * SV::S64 + c * SV::S16, &kv16, bar_kv + sl, cv + 64 * N64 + 16 * c, 64 * j, b);
   };
 
   uint32_t q_phase = 0, kv_phase = 0;  // kv_phase: one bit per slot
@@ -88,14 +97,15 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
     const int q0 = qt * 128;
     __syncthreads();  // the barriers are initialised; every thread is done with the previous tile's Q (and slots)
     if (tid == 0) {
-      mbar_arrive_expect_tx(bar_q, 2 * ROWS * DH * 2);
+      mbar_arrive_expect_tx(bar_q, 2 * ROWS * DK * 2);
 #pragma unroll
       for (int w = 0; w < 2; ++w) {
 #pragma unroll
-        for (int c = 0; c < N64; ++c) tma_load_3d(smem + w * S::OP + c * S::S64, &q64, bar_q, h * DH + 64 * c, q0 + 64 * w, b);
+        for (int c = 0; c < S::N64; ++c)
+          tma_load_3d(smem + w * S::OP + c * S::S64, &q64, bar_q, h * DK + 64 * c, q0 + 64 * w, b);
 #pragma unroll
-        for (int c = 0; c < N16; ++c)
-          tma_load_3d(smem + w * S::OP + N64 * S::S64 + c * S::S16, &q16, bar_q, h * DH + 64 * N64 + 16 * c,
+        for (int c = 0; c < S::N16; ++c)
+          tma_load_3d(smem + w * S::OP + S::N64 * S::S64 + c * S::S16, &q16, bar_q, h * DK + 64 * S::N64 + 16 * c,
                       q0 + 64 * w, b);
       }
       if (resident) {
@@ -131,11 +141,11 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
         mbar_wait(bar_kv + sl, (kv_phase >> sl) & 1u);
         kv_phase ^= 1u << sl;
       }
-      const uint32_t sk = smem_u32(slot0) + sl * 2 * S::OP, sv = sk + S::OP;
+      const uint32_t sk = smem_u32(slot0) + sl * SLOT, sv = sk + S::OP;
 
       float s[32];
       wgmma_fence();
-      qk_mma<DH>(s, sq, sk);
+      qk_mma<DK>(s, sq, sk);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(s);
@@ -183,7 +193,7 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
 #pragma unroll
       for (int c = 0; c < N16; ++c) fence_regs(o16[c]);
       wgmma_fence();
-      pv_mma<DH>(o, o16, s, sv);
+      pv_mma<DV>(o, o16, s, sv);
       wgmma_commit();
       wgmma_wait<0>();
 #pragma unroll
@@ -198,42 +208,43 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
       l[rh] += __shfl_xor_sync(0xffffffffu, l[rh], 2);
       const int q = q0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * rh;
       if (q >= p.Nq) continue;
-      store_rows<DH>(o, o16, p.out + ((long long)b * p.Nq + q) * p.I + h * DH + 2 * (lane & 3), rh, 1.0f / l[rh]);
+      store_rows<DV>(o, o16, p.out + ((long long)b * p.Nq + q) * p.Iv + h * DV + 2 * (lane & 3), rh, 1.0f / l[rh]);
     }
   }
 }
 
-template <int DH>
+template <int DK, int DV>
 static int launch_kv_t(const void* q, int64_t ldq, const void* kv, int64_t ldkv, KvParams p, int H,
                        cudaStream_t stream) {
-  using S = Slabs<DH>;
+  using S = Slabs<DK>;
+  using SV = Slabs<DV>;
   CUtensorMap tm[4];
-  const uint64_t qdims[3] = {(uint64_t)p.I, (uint64_t)p.Nq, (uint64_t)p.B};
+  const uint64_t qdims[3] = {(uint64_t)p.Ik, (uint64_t)p.Nq, (uint64_t)p.B};
   const uint64_t qstr[2] = {(uint64_t)ldq * 2, (uint64_t)ldq * 2 * p.Nq};
-  const uint64_t kdims[3] = {(uint64_t)2 * p.I, (uint64_t)p.Nk, (uint64_t)p.B};
+  const uint64_t kdims[3] = {(uint64_t)(p.Ik + p.Iv), (uint64_t)p.Nk, (uint64_t)p.B};
   const uint64_t kstr[2] = {(uint64_t)ldkv * 2, (uint64_t)ldkv * 2 * p.Nk};
   const uint32_t box64[3] = {64, ROWS, 1}, box16[3] = {16, ROWS, 1};
+  // q64 / q16 serve the q blocks; kv64 / kv16 the k and v blocks, whichever slab widths the two have
+  constexpr bool q64 = S::N64 > 0, q16 = S::N16 > 0, kv64 = S::N64 + SV::N64 > 0, kv16 = S::N16 + SV::N16 > 0;
   int rc = 0;
-  if (S::N64) {
-    rc = encode_tmap_bf16(&tm[0], q, 3, qdims, qstr, box64);
-    if (!rc) rc = encode_tmap_bf16(&tm[2], kv, 3, kdims, kstr, box64);
-  }
-  if (!rc && S::N16) {
-    rc = encode_tmap_bf16_sw(&tm[1], q, 3, qdims, qstr, box16, 32);
-    if (!rc) rc = encode_tmap_bf16_sw(&tm[3], kv, 3, kdims, kstr, box16, 32);
-  }
+  if (q64) rc = encode_tmap_bf16(&tm[0], q, 3, qdims, qstr, box64);
+  if (!rc && kv64) rc = encode_tmap_bf16(&tm[2], kv, 3, kdims, kstr, box64);
+  if (!rc && q16) rc = encode_tmap_bf16_sw(&tm[1], q, 3, qdims, qstr, box16, 32);
+  if (!rc && kv16) rc = encode_tmap_bf16_sw(&tm[3], kv, 3, kdims, kstr, box16, 32);
   if (rc) return rc;
-  if (!S::N16) tm[1] = tm[0], tm[3] = tm[2];
-  if (!S::N64) tm[0] = tm[1], tm[2] = tm[3];
+  if (!q16) tm[1] = tm[0];
+  if (!q64) tm[0] = tm[1];
+  if (!kv16) tm[3] = tm[2];
+  if (!kv64) tm[2] = tm[3];
   const int nkb = (p.Nk + 63) / 64, nqt = (p.Nq + 127) / 128;
-  p.slots = nkb <= kv_resident_slots<DH>() ? nkb : KV_RING;
-  const int bytes = (2 + 2 * p.slots) * S::OP + 8 * (1 + KV_MAX_SLOTS) + 1024;
+  p.slots = nkb <= kv_resident_slots<DK, DV>() ? nkb : KV_RING;
+  const int bytes = 2 * S::OP + p.slots * (S::OP + SV::OP) + 8 * (1 + KV_MAX_SLOTS) + 1024;
   // enough CTAs to fill the device about twice; an (image, head) with resident keys is not split further than that
   const long long pairs = (long long)p.B * H;
   long long per = (2LL * num_sms() + pairs - 1) / pairs;
   if (per > nqt) per = nqt;
   if (per < 1) per = 1;
-  auto kern = attention_kv_kernel<DH>;
+  auto kern = attention_kv_kernel<DK, DV>;
   B200_ENSURE_SMEM(kern, bytes);
   kern<<<dim3((unsigned)per, H, p.B), KV_THREADS, bytes, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -321,32 +332,66 @@ using namespace b200;
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq,
-                                    int Nk, int H, int dh, float scale, void* stream) {
-  B200_CHECK_ARG(q && kv && out, "attention_kv: null pointer");
-  B200_CHECK_ARG(B > 0 && Nq > 0 && Nk > 0 && H > 0, "attention_kv: bad shape B=%d Nq=%d Nk=%d H=%d", B, Nq, Nk, H);
-  B200_CHECK_ARG(head_width_ok(dh), "attention_kv: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
-  B200_CHECK_ARG(Nk <= B200VIT_ATTN_KV_MAX_KEYS, "attention_kv: Nk=%d > %d", Nk, B200VIT_ATTN_KV_MAX_KEYS);
-  B200_CHECK_ARG(ldq >= (int64_t)H * dh && ldq % 8 == 0, "attention_kv: ldq=%lld must be a multiple of 8 and >= %d",
-                 (long long)ldq, H * dh);
-  B200_CHECK_ARG(ldkv >= (int64_t)2 * H * dh && ldkv % 8 == 0,
-                 "attention_kv: ldkv=%lld must be a multiple of 8 and >= %d", (long long)ldkv, 2 * H * dh);
-  B200_CHECK_ARG(aligned16(q) && aligned16(kv) && aligned16(out), "attention_kv: pointers must be 16-byte aligned");
-  B200_CHECK_ARG(H <= 65535 && B <= 65535, "attention_kv: B=%d, H=%d exceed the grid", B, H);
+static bool overlap(const void* a, long long a_bytes, const void* b, long long b_bytes) {
+  const uintptr_t p = reinterpret_cast<uintptr_t>(a), q = reinterpret_cast<uintptr_t>(b);
+  return p < q + (uintptr_t)b_bytes && q < p + (uintptr_t)a_bytes;
+}
+
+// the checks and launch shared by b200vit_attention_kv (dk == dv) and b200vit_attention_kv_ex; `what` names the caller
+// (check_overlap: out must overlap neither q nor kv, which b200vit_attention_kv has never checked)
+static int attention_kv_impl(const char* what, const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out,
+                             int B, int Nq, int Nk, int H, int dk, int dv, float scale, void* stream,
+                             bool check_overlap = false) {
+  B200_CHECK_ARG(q && kv && out, "%s: null pointer", what);
+  B200_CHECK_ARG(B > 0 && Nq > 0 && Nk > 0 && H > 0, "%s: bad shape B=%d Nq=%d Nk=%d H=%d", what, B, Nq, Nk, H);
+  B200_CHECK_ARG(Nk <= B200VIT_ATTN_KV_MAX_KEYS, "%s: Nk=%d > %d", what, Nk, B200VIT_ATTN_KV_MAX_KEYS);
+  B200_CHECK_ARG(ldq >= (int64_t)H * dk && ldq % 8 == 0, "%s: ldq=%lld must be a multiple of 8 and >= %d", what,
+                 (long long)ldq, H * dk);
+  B200_CHECK_ARG(ldkv >= (int64_t)H * (dk + dv) && ldkv % 8 == 0, "%s: ldkv=%lld must be a multiple of 8 and >= %d",
+                 what, (long long)ldkv, H * (dk + dv));
+  B200_CHECK_ARG(aligned16(q) && aligned16(kv) && aligned16(out), "%s: pointers must be 16-byte aligned", what);
+  B200_CHECK_ARG(H <= 65535 && B <= 65535, "%s: B=%d, H=%d exceed the grid", what, B, H);
+  if (check_overlap) {
+    const long long out_b = (long long)B * Nq * H * dv * 2, q_b = (((long long)B * Nq - 1) * ldq + (long long)H * dk) * 2,
+                    kv_b = (((long long)B * Nk - 1) * ldkv + (long long)H * (dk + dv)) * 2;
+    B200_CHECK_ARG(!overlap(out, out_b, q, q_b) && !overlap(out, out_b, kv, kv_b), "%s: out overlaps q or kv", what);
+  }
   KvParams p{};
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.B = B;
   p.Nq = Nq;
   p.Nk = Nk;
-  p.I = H * dh;
+  p.Ik = H * dk;
+  p.Iv = H * dv;
   p.scale_log2e = scale * 1.4426950408889634f;
   const auto st = reinterpret_cast<cudaStream_t>(stream);
-  switch (dh) {
-    case 32: return launch_kv_t<32>(q, ldq, kv, ldkv, p, H, st);
-    case 80: return launch_kv_t<80>(q, ldq, kv, ldkv, p, H, st);
-    case 128: return launch_kv_t<128>(q, ldq, kv, ldkv, p, H, st);
-    default: return launch_kv_t<64>(q, ldq, kv, ldkv, p, H, st);
+  switch (dk * 1000 + dv) {
+    case 32032: return launch_kv_t<32, 32>(q, ldq, kv, ldkv, p, H, st);
+    case 64064: return launch_kv_t<64, 64>(q, ldq, kv, ldkv, p, H, st);
+    case 80080: return launch_kv_t<80, 80>(q, ldq, kv, ldkv, p, H, st);
+    case 128128: return launch_kv_t<128, 128>(q, ldq, kv, ldkv, p, H, st);
+    case 16032: return launch_kv_t<16, 32>(q, ldq, kv, ldkv, p, H, st);
+    case 16064: return launch_kv_t<16, 64>(q, ldq, kv, ldkv, p, H, st);
+    case 32064: return launch_kv_t<32, 64>(q, ldq, kv, ldkv, p, H, st);
+    case 48032: return launch_kv_t<48, 32>(q, ldq, kv, ldkv, p, H, st);
+    case 48064: return launch_kv_t<48, 64>(q, ldq, kv, ldkv, p, H, st);
+    case 64032: return launch_kv_t<64, 32>(q, ldq, kv, ldkv, p, H, st);
+    default: B200_CHECK_ARG(false, "%s: dk=%d, dv=%d not built", what, dk, dv);
   }
+}
+
+extern "C" int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq,
+                                    int Nk, int H, int dh, float scale, void* stream) {
+  B200_CHECK_ARG(head_width_ok(dh), "attention_kv: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
+  return attention_kv_impl("attention_kv", q, ldq, kv, ldkv, out, B, Nq, Nk, H, dh, dh, scale, stream);
+}
+
+extern "C" int b200vit_attention_kv_ex(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B,
+                                       int Nq, int Nk, int H, int dk, int dv, float scale, void* stream) {
+  B200_CHECK_ARG(dk == 16 || dk == 32 || dk == 48 || dk == 64,
+                 "attention_kv_ex: dk=%d not supported by this build (16, 32, 48 or 64)", dk);
+  B200_CHECK_ARG(dv == 32 || dv == 64, "attention_kv_ex: dv=%d not supported by this build (32 or 64)", dv);
+  return attention_kv_impl("attention_kv_ex", q, ldq, kv, ldkv, out, B, Nq, Nk, H, dk, dv, scale, stream, true);
 }
 
 extern "C" int b200vit_merge_patches_ln(const float* x, int64_t M, const float* gamma, const float* beta,

@@ -142,6 +142,9 @@ WINDOW_MIX_MAX_WINDOWS = 64                # b200vit_window_mix: windows of one 
 REGION_LOCAL_WIDTHS = (32,)                # b200vit_attention_region_local
 REGION_LOCAL_MAX_TOKENS = 256              # b200vit_attention_region_local: a window's local tokens + its region token
 REGION_MAX_TOKENS = 512                    # b200vit_attention over one image's region tokens
+KV_EX_KEY_WIDTHS = (16, 32, 48, 64)        # b200vit_attention_kv_ex and b200vit_attention_iwsa: q / k head widths
+KV_EX_VALUE_WIDTHS = (32, 64)              # ... and v head widths
+ATTN_KV_MAX_KEYS = 16384                   # B200VIT_ATTN_KV_MAX_KEYS: keys per image or window
 
 
 def head_width_reason(dh: int) -> Optional[str]:
@@ -179,6 +182,28 @@ def lpi_reason(kernel_size: int, grid_w: int) -> Optional[str]:
     if (3 * kernel_size - 1) * (grid_w + 2 * (kernel_size // 2)) * 4 * 4 > 100 * 1024:
         return f"a grid row of {grid_w} tokens is too wide for the local patch interaction kernel"
     return None
+
+
+def kv_ex_reason(dk: int, dv: int, what: str) -> Optional[str]:
+    """None if b200vit_attention_kv_ex / b200vit_attention_iwsa are built for key heads `dk` wide (after padding) and
+    value heads `dv` wide, else the reason the eager PyTorch graph is used; `what` names the attention."""
+    if dk not in KV_EX_KEY_WIDTHS or dv not in KV_EX_VALUE_WIDTHS:
+        return (f"dim_key={dk}, dim_value={dv} (the {what} attention kernel is built for key heads 16, 32, 48 or 64 "
+                f"and value heads 32 or 64 wide)")
+    return None
+
+
+def value_width(L: "EncoderLayer") -> int:
+    """The width of layer L's value heads: L.dim_head, unless its attention record says otherwise."""
+    A = L.attention
+    return A.value_width(L) if hasattr(A, "value_width") else L.dim_head
+
+
+def _rows_of(buf: torch.Tensor, cols: int) -> torch.Tensor:
+    """A contiguous [rows, cols] view at the start of the workspace buffer `buf` (at least as many elements)."""
+    if buf.shape[1] == cols:
+        return buf
+    return buf.view(-1)[: buf.shape[0] * cols].view(buf.shape[0], cols)
 
 
 class Norm(NamedTuple):
@@ -351,14 +376,23 @@ class StridedKV(NamedTuple):
     GlobalAttention, twins_svt.py:122-157; b200vit_attention_kv); EncoderLayer.qkv_w holds the query rows only.
     run_blocks needs `grid`.  The LayerNorm cannot be folded into the key / value projection (one convolution window
     spans tokens with different statistics): in both LayerNorm modes the layer runs layernorm(x -> xb), the query GEMM
-    on xb, conv_im2col_nhwc of xb and the key / value GEMM (stride 1: the GEMM on xb itself), then attention_kv."""
+    on xb, conv_im2col_nhwc of xb and the key / value GEMM (stride 1: the GEMM on xb itself), then attention_kv.
+    `dim_value`: value heads of another width than L.dim_head, the key heads (ScalableViT's SSA, scalable_vit.py:71-124;
+    b200vit_attention_kv_ex); kv_w then has heads * (dim_head + dim_value) rows and the output heads * dim_value
+    columns.  None: dim_value == dim_head."""
     stride: int
-    kv_w: torch.Tensor                            # the Conv2d weight [2 * heads * dim_head, D, k, k], rows k | v
+    kv_w: torch.Tensor                            # the Conv2d weight [heads * (dk + dv), D, k, k], rows k | v
+    dim_value: Optional[int] = None
     kernel = "kv"
     rejects = Windows.rejects
 
     def reason(self, L: EncoderLayer) -> Optional[str]:
-        return head_width_reason(L.dim_head)
+        if self.dim_value is None:
+            return head_width_reason(L.dim_head)
+        return kv_ex_reason(L.dim_head, self.dim_value, "sub-sampled-key")
+
+    def value_width(self, L: EncoderLayer) -> int:
+        return L.dim_head if self.dim_value is None else self.dim_value
 
     def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
         if grid is None or grid[0] * grid[1] != N:
@@ -383,10 +417,75 @@ class StridedKV(NamedTuple):
         else:
             col = torch.empty(c.B * kh * kw, k * k * x.shape[1], device=x.device, dtype=torch.bfloat16)
             _lib.conv_im2col_nhwc(xb, col, c.B, gh, gw, k, k, 0)
-        kv = torch.empty(c.B * kh * kw, 2 * I, device=x.device, dtype=torch.bfloat16)
+        kv = torch.empty(c.B * kh * kw, self.kv_w.shape[0], device=x.device, dtype=torch.bfloat16)
         _lib.gemm(col, t[f"{i}.kv.w"], out_bf16=kv)
-        _lib.attention_kv(q, kv, c.o, c.B, c.N, kh * kw, L.heads, L.dim_head, L.scale)
-        return c.o
+        if self.dim_value is None:
+            _lib.attention_kv(q, kv, c.o, c.B, c.N, kh * kw, L.heads, L.dim_head, L.scale)
+            return c.o
+        o = _rows_of(c.o, L.heads * self.dim_value)
+        _lib.attention_kv_ex(q, kv, o, c.B, c.N, kh * kw, L.heads, L.dim_head, self.dim_value, L.scale)
+        return o
+
+
+class InteractiveWindows(NamedTuple):
+    """ScalableViT's interactive windowed self-attention (scalable_vit.py:126-194; b200vit_attention_iwsa): attention
+    inside size x size windows of the token grid (None: the whole grid) plus the local interactive module, a dense
+    3 x 3 convolution with bias and zero padding 1 of the value map, added to the attention output before the
+    out-projection.  EncoderLayer.qkv_w holds the rows q | k | v, the q and k heads L.dim_head wide, the v heads
+    lim_w.shape[0] / heads.  The layer runs the QKV projection (c.project), conv_im2col_nhwc over the v columns of
+    qkv, the convolution's GEMM with its bias into a bf16 `lim` buffer, then attention_iwsa.  run_blocks needs `grid`."""
+    size: Optional[int]
+    lim_w: torch.Tensor                           # local_interactive_module.weight [heads * dv, heads * dv, 3, 3]
+    lim_b: torch.Tensor
+    kernel = "iwsa"
+    rejects = "interactive windowed attention runs over B token grids only"
+
+    def value_width(self, L: EncoderLayer) -> int:
+        return self.lim_w.shape[0] // L.heads
+
+    def window(self, grid: Tuple[int, int]) -> Tuple[int, int]:
+        return (grid[0], grid[1]) if self.size is None else (self.size, self.size)
+
+    def reason(self, L: EncoderLayer) -> Optional[str]:
+        r = kv_ex_reason(L.dim_head, self.value_width(L), "interactive windowed")
+        if r is None and self.size is not None and self.size ** 2 > ATTN_KV_MAX_KEYS:
+            r = (f"window_size={self.size}: a window of {self.size ** 2} tokens (the interactive windowed attention "
+                 f"kernel takes at most {ATTN_KV_MAX_KEYS})")
+        return r
+
+    def geometry_reason(self, L: EncoderLayer, N: int, grid, groups, regions, rows=None) -> Optional[str]:
+        if grid is None or grid[0] * grid[1] != N:
+            return "interactive windowed attention needs `grid` = (h, w) with h * w == N"
+        wh, ww = self.window(grid)
+        if grid[0] % wh or grid[1] % ww:
+            # the reference's assertion (scalable_vit.py:161)
+            return (f"height ({grid[0]}) or width ({grid[1]}) of feature map is not divisible by the window size "
+                    f"({wh}, {ww})")
+        if wh * ww > ATTN_KV_MAX_KEYS:
+            return (f"a {wh} x {ww} window of {wh * ww} tokens (the interactive windowed attention kernel takes at "
+                    f"most {ATTN_KV_MAX_KEYS})")
+        return None
+
+    def prepare(self, t: Dict[str, torch.Tensor], i: int, L: EncoderLayer) -> None:
+        # the Conv2d weight in the column order of b200vit_conv_im2col_nhwc: (tap row, tap column, channel)
+        w = self.lim_w.detach()
+        t[f"{i}.lim.w"] = _bf16_rows(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1))
+        t[f"{i}.lim.b"] = _f32(self.lim_b)
+
+    def launch(self, c: BlocksCall, L: EncoderLayer, i: int) -> torch.Tensor:
+        t, (gh, gw), M = c.t, c.grid, c.x.shape[0]
+        Ik, dv = L.heads * L.dim_head, self.value_width(L)
+        Iv = L.heads * dv
+        qkv = _rows_of(c.qkv, L.qkv_w.shape[0])
+        c.project(L, i, out=qkv)
+        col = torch.empty(M, 9 * Iv, device=c.x.device, dtype=torch.bfloat16)
+        _lib.conv_im2col_nhwc(qkv[:, 2 * Ik:], col, c.B, gh, gw, 3, 1, 1)
+        lim = torch.empty(M, Iv, device=c.x.device, dtype=torch.bfloat16)
+        _lib.gemm(col, t[f"{i}.lim.w"], out_bf16=lim, bias=t[f"{i}.lim.b"])
+        o = _rows_of(c.o, Iv)
+        wh, ww = self.window(c.grid)
+        _lib.attention_iwsa(qkv, lim, o, c.B, gh, gw, wh, ww, L.heads, L.dim_head, dv, L.scale)
+        return o
 
 
 class PatchGroups(NamedTuple):
@@ -634,8 +733,8 @@ class RegionLocalBlock(NamedTuple):
         return o
 
 
-AttentionVariant = Union[HeadMix, CrossCovariance, Windows, StridedKV, ConvProj, PatchGroups, WindowTokenBlock,
-                         RegionLocalBlock]
+AttentionVariant = Union[HeadMix, CrossCovariance, Windows, StridedKV, InteractiveWindows, ConvProj, PatchGroups,
+                         WindowTokenBlock, RegionLocalBlock]
 
 
 @dataclass
@@ -675,13 +774,16 @@ class EncoderLayer:
     post_norm: bool = False
     # the feed-forward block's activation: "gelu" (vit.py:21) or "silu" (MobileViT's FeedForward, mobile_vit.py:28-34)
     ff_act: str = "gelu"
+    # the feed-forward block runs before the attention: x += fc2(GELU(fc1(LN2(x)))); x += out(attention(...)) (the
+    # second half of a ScalableViT layer, scalable_vit.py:228-236); not with lpi, post_norm or temporal
+    ff_first: bool = False
 
 
 def attention_kernel(L: EncoderLayer, axial: bool = False, packed: bool = False, key_blocks: bool = False) -> str:
     """Which kernel runs layer L's attention: its record's `kernel` ('headmix', 'xca', 'window', 'window_relpos', 'kv',
-    'groups', 'window_token' or 'region_local'), or for softmax attention 'axial' (a run_blocks call with `axial`,
-    unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed batch, or more than 512 keys)
-    or 'plain'.  ValueError for an attention variant with `axial` or over a `packed` batch."""
+    'iwsa', 'groups', 'window_token' or 'region_local'), or for softmax attention 'axial' (a run_blocks call with
+    `axial`, unless the layer's temporal sub-block runs there), 'varlen' (`key_blocks`: a packed batch, or more than 512
+    keys) or 'plain'.  ValueError for an attention variant with `axial` or over a `packed` batch."""
     A = L.attention
     if A is not None:
         if axial or packed:
@@ -789,6 +891,14 @@ def _fold(t: Dict[str, torch.Tensor], prefix: str, w: torch.Tensor, b: Optional[
         t[prefix + ".t"] = (tb + b.detach().float() if b is not None else tb).contiguous()
 
 
+def depthwise_peg_weights(conv: nn.Conv2d) -> dict:
+    """'w' fp32 [k*k, C] (the depthwise k x k weights tap major) and 'b' fp32 [C] of b200vit_peg, from the PEG's
+    Conv2d(C, C, k, padding=k // 2, groups=C) (Twins-SVT, twins_svt.py:77-83; ScalableViT, scalable_vit.py:44-50)."""
+    C, kk = conv.weight.shape[0], conv.kernel_size[0] ** 2
+    bias = _f32(conv.bias) if conv.bias is not None else torch.zeros(C, device=conv.weight.device)
+    return {"w": conv.weight.detach().float().reshape(C, kk).t().contiguous(), "b": bias}
+
+
 class Workspace:
     """Scratch buffers of a TransformerEngine: `t` by name, `c` the _lib.EncoderWs over them, `key` what they were
     allocated for (rows, device, stream)."""
@@ -854,11 +964,12 @@ class BlocksCall:
         _lib.gemm(a, self.t[w + ".w"], out_f32=self.x, out_bf16=copy, bias=self.t[w + ".b"], resid=resid,
                   stats_out=stats)
 
-    def project(self, L: EncoderLayer, i: int) -> None:
-        """qkv = LN1(x) Wqkv^T with layer L's q / k head norm, then the call's rotary positions."""
+    def project(self, L: EncoderLayer, i: int, out: Optional[torch.Tensor] = None) -> None:
+        """qkv = LN1(x) Wqkv^T with layer L's q / k head norm, then the call's rotary positions; into `out` in place of
+        the workspace's qkv when given."""
         head = {} if L.qk_norm is None else dict(head_gamma=self.t[f"{i}.gqk"], norm_heads=2 * L.heads, dh=L.dim_head,
                                                  head_layernorm_eps=L.qk_eps if L.qk_norm == "ln" else None)
-        self.normed(self.x, f"{i}.ln1", L.ln1, f"{i}.qkv", self.qkv, **head)
+        self.normed(self.x, f"{i}.ln1", L.ln1, f"{i}.qkv", self.qkv if out is None else out, **head)
         if self.rope is not None:
             _lib.rope_qk(self.qkv, self.rope[0], self.rope[1], L.heads, L.dim_head)
 
@@ -970,7 +1081,8 @@ class TransformerEngine:
         long as `t` (which holds the tensors)."""
         sig = lambda L: (L.heads, L.dim_head, L.fc1_w.shape[0], L.mask_self)      # noqa: E731
         if any(L.qk_norm == "ln" or L.temporal is not None or L.attention is not None or L.lpi is not None
-               or L.post_norm or L.ff_act != "gelu" or sig(L) != sig(self.layers[0]) for L in self.layers):
+               or L.post_norm or L.ff_first or L.ff_act != "gelu" or sig(L) != sig(self.layers[0])
+               for L in self.layers):
             return None
         arr = (_lib.Layer * len(self.layers))()
         p = lambda v: None if v is None else v.data_ptr()      # noqa: E731
@@ -1003,11 +1115,14 @@ class TransformerEngine:
             self.prepared()
             L = self.layers[0]
             D, I, Hd = L.qkv_w.shape[1], L.heads * L.dim_head, L.fc1_w.shape[0]
+            # layers whose q / k and v heads differ in width (ScalableViT) take views of other widths of these two
+            Iqkv = max([3 * I] + [K.qkv_w.shape[0] for K in self.layers])
+            Io = max([I] + [K.heads * value_width(K) for K in self.layers])
             bf = dict(device=device, dtype=torch.bfloat16)
             slot.t = {
                 "xn": torch.empty(M, D, **bf),          # exact: LayerNorm output; fold: bf16 copy of x
-                "qkv": torch.empty(M, 3 * I, **bf),
-                "o": torch.empty(M, I, **bf),
+                "qkv": torch.empty(M, Iqkv, **bf),
+                "o": torch.empty(M, Io, **bf),
                 "h": torch.empty(M, Hd, **bf),
                 # LN-fold row statistics: [M, 1, 2] written by embed_tokens / rowstats_cast, [M, parts(D), 2] by GEMMs
                 "stats_in": torch.empty(M, 1, 2, device=device, dtype=torch.float32),
@@ -1093,11 +1208,16 @@ class TransformerEngine:
                 r = L.attention.geometry_reason(L, N, grid, groups, regions, rows=(B, x.shape[0]))
                 if r is not None:
                     raise ValueError(r)
+            if L.ff_first and (L.lpi is not None or L.post_norm or L.temporal is not None):
+                raise ValueError("a layer whose feed-forward block runs first has no lpi, post_norm or temporal block")
         c = BlocksCall(t, ws, x, B, N, grid, groups, regions, rope, axial, vl, fold, primed)
         xb, h = c.xb, c.h
         for i, kernel in zip(run, kernels):
             L = self.layers[i]
             act = dict(act="silu") if L.ff_act == "silu" else dict(gelu=True)
+            if L.ff_first:
+                c.normed(x, f"{i}.ln2", L.ln2, f"{i}.fc1", h, **act)
+                c.residual(h, f"{i}.fc2", x, "stats_a")
             if L.attention is None:
                 c.project(L, i)
                 c.attend(kernel, L, i)
@@ -1116,6 +1236,8 @@ class TransformerEngine:
                 _lib.local_patch_interaction(x, ff_in, ws["lnst"], ln, t[f"{i}.lpi.w1"], t[f"{i}.lpi.b1"],
                                              t[f"{i}.lpi.w2"], t[f"{i}.lpi.b2"], B, grid[0], grid[1],
                                              L.lpi.kernel_size, y_bf16=yb, y_stats=ys)
+            if L.ff_first:
+                continue
             if L.post_norm:
                 # the normalised stream and its bf16 copy; fc1 reads that copy as it is, with no LayerNorm of its own
                 _lib.layernorm(x, t[f"{i}.ln2.w"], t[f"{i}.ln2.b"], out_f32=ff_in, out_bf16=xb, eps=L.ln2.eps)

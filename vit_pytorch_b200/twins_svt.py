@@ -31,7 +31,7 @@ from torch import nn
 
 from . import _lib
 from .engine import (PEG_KERNEL_SIZES, EncoderLayer, FusedEncoder, FusedWeightsMixin, Norm, StridedKV, Windows,
-                     _bf16_rows, _f32, cached, common_reason, head_engine, on_device)
+                     _bf16_rows, _f32, cached, common_reason, depthwise_peg_weights, head_engine, on_device)
 
 __all__ = ["FeedForward", "GlobalAttention", "LayerNorm", "LocalAttention", "PEG", "PatchEmbedding", "Residual",
            "Transformer", "TwinsSVT", "group_by_key_prefix_and_remove_prefix", "group_dict_by_key", "merge_weights",
@@ -265,10 +265,7 @@ def merge_weights(pe: PatchEmbedding) -> dict:
 
 def peg_weights(peg: PEG) -> dict:
     """'w' fp32 [k*k, C] (the depthwise weights tap major) and 'b' fp32 [C] of b200vit_peg."""
-    conv = peg.proj.fn
-    C, kk = conv.weight.shape[0], conv.kernel_size[0] ** 2
-    bias = _f32(conv.bias) if conv.bias is not None else torch.zeros(C, device=conv.weight.device)
-    return {"w": conv.weight.detach().float().reshape(C, kk).t().contiguous(), "b": bias}
+    return depthwise_peg_weights(peg.proj.fn)
 
 
 class _Squeeze(nn.Module):
