@@ -180,6 +180,18 @@ def qkv_attention_reference(qkv: Tensor, lengths: Sequence[int], H: int, dh: int
     return ref, bound
 
 
+def axial_reference(qkv: Tensor, key_mask: Optional[Tensor], B: int, L: int, G: int, H: int, dh: int, scale: float,
+                    zero_masked_rows: bool) -> Tuple[Tensor, Tensor]:
+    """(ref, bound) [B L G, H dh] of the B*G*H sequences (token j of b*G + p at row b*L*G + j*G + p) from
+    attention_reference with the key mask of each sequence's batch element: one 64-key block, a row
+    without a kept key 0 (zero_masked_rows) or the mean of its sequence's values."""
+    t = qkv.view(B, L, G, 3, H, dh).permute(3, 0, 2, 4, 1, 5).reshape(3, B * G * H, L, dh)
+    km = None if key_mask is None else key_mask.bool()[:, None, None, :].expand(B, G, H, L).reshape(B * G * H, L)
+    ref, bound = attention_reference(t[0], t[1], t[2], scale, kb=64, key_mask=km, zero_masked_rows=zero_masked_rows)
+    back = lambda x: x.view(B, G, H, L, dh).permute(0, 3, 1, 2, 4).reshape(B * L * G, H * dh)   # noqa: E731
+    return back(ref), back(bound)
+
+
 def qkv_inputs(kind: str, lengths: Sequence[int], H: int, dh: int, *, seed: int = 0, device="cpu") -> Tensor:
     """Seeded packed q | k | v [sum(lengths), 3 H dh] bf16 in one of four distributions:
       normal    N(0, 1);

@@ -1,0 +1,832 @@
+"""Every launch of TransformerEngine.run_blocks traced back to the reference layer  --  TEST INFRASTRUCTURE.
+
+Whether the fused encoder computes what the reference module's forward defines splits into two questions that need no
+error propagation through softmax, LayerNorm or GELU:
+
+  provenance   every operand of every launch of a layer equals, bit for bit, the value the reference forward defines
+               at that point: derived here from the module's own parameters (read through the attribute paths of
+               the reference, `module_layers`) and from the snapshotted outputs of the launches before it -- the
+               stream entering the layer, bf16(x), bf16(gamma W), ...  Row statistics are the one exception: they
+               must be within the bound of the kernel that wrote them.  Scalars too: eps, softmax scale, heads,
+               dim_head, mask_self, the key mask, the rotary table.  (`check_provenance`)
+  accuracy     every output is within the fp64 bound its kernel already has, computed on the operands the kernel
+               actually received.  (`expected`, `check_accuracy`)
+
+Together they chain each layer back to the reference arithmetic: error enters only where the project chose it (the
+bf16 operands, the folded LayerNorm's definition) and each kernel is held to its own bound.
+
+The tracer (`trace`) wraps every _lib entry point run_blocks can reach, with the argument binding and the entry-point
+list of tests/golden/make_engine_schedule.py; a launch is kept with its arguments, a clone of every tensor argument
+taken before the call and a clone of every tensor it writes taken after it (the workspace buffers are overwritten
+within a layer).  The clones go on the current stream.  `impl` runs a launch: the real kernels on the GPU, or
+`emulate`, which writes the fp64 reference of `expected` rounded to the output's dtype, on a machine without one.  The
+trace runs the per-kernel Python loop; the one-call C loop must be bit-identical to it."""
+from __future__ import annotations
+
+import inspect
+import math
+import os
+import sys
+from dataclasses import dataclass, field
+from typing import Callable, Dict, List, Optional, Tuple
+
+import torch
+from torch import nn
+
+from oracle import attention_bounds as AB
+from oracle import attention_fp32_bounds as FB
+from oracle import bounds as Bd
+from oracle import headmix_bounds as HB
+from oracle import row_bounds as RB
+from oracle.lpi_bounds import lpi_reference
+
+Tensor = torch.Tensor
+U = Bd.U
+GOLDEN = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+
+# the tensors each entry point writes
+OUTPUTS = {
+    "gemm": ("out_f32", "out_bf16", "stats_out"),
+    "gemm_headnorm": ("out_bf16",),
+    "layernorm": ("out_f32", "out_bf16"),
+    "rowstats_cast": ("xb", "stats"),
+    "rope_qk": ("qkv",),
+    "attention": ("out",),
+    "attention_varlen": ("out",),
+    "attention_axial": ("out",),
+    "attention_headmix": ("out",),
+    "attention_xca": ("out",),
+    "local_patch_interaction": ("y", "y_bf16", "y_stats"),
+}
+
+
+def schedule():
+    """tests/golden/make_engine_schedule.py: ENTRY_POINTS, Recorder, recording, CASES."""
+    if GOLDEN not in sys.path:
+        sys.path.insert(0, GOLDEN)
+    import make_engine_schedule
+    return make_engine_schedule
+
+
+def f32(eps: float) -> float:
+    """A Python float as the C ABI's float receives it."""
+    return torch.tensor(eps, dtype=torch.float32).item()
+
+
+# ------------------------------------------------------------------------------------------------------ tracing
+@dataclass
+class Launch:
+    name: str
+    args: dict                                    # bound arguments, the live objects
+    pre: dict                                     # argument name -> clone before the call (tensors, tuples of them)
+    post: dict = field(default_factory=dict)      # written argument name -> clone after the call
+
+
+def _clone(v):
+    if isinstance(v, torch.Tensor):
+        return v.detach().clone()
+    if isinstance(v, tuple):
+        return tuple(_clone(e) for e in v)
+    return v
+
+
+def tracer(impl: Callable[[str, Callable], Callable]):
+    """A make_engine_schedule.Recorder whose entry points run `impl(name, real)` and keep Launch records in
+    `launches`."""
+    S = schedule()
+
+    class Tracer(S.Recorder):
+        def __init__(self, eng, owners) -> None:
+            super().__init__(eng, owners)
+            self.launches: List[Launch] = []
+
+        def recorder(self, name: str, real: Callable) -> Callable:
+            sig, run = inspect.signature(real), impl(name, real)
+
+            def call(*args, **kwargs):
+                a = self.bind(sig, args, kwargs)
+                rec = Launch(name, a, {k: _clone(v) for k, v in a.items()})
+                run(**a)
+                rec.post = {k: _clone(a[k]) for k in OUTPUTS.get(name, ()) if a.get(k) is not None}
+                self.launches.append(rec)
+            return call
+    return Tracer
+
+
+def real_impl(name: str, real: Callable) -> Callable:
+    return real
+
+
+def emulate_impl(name: str, real: Callable) -> Callable:
+    """The launch emulated: its outputs get the fp64 reference of `expected`, rounded to their dtype."""
+    def run(**a):
+        if name not in OUTPUTS:
+            raise NotImplementedError(f"no emulation of _lib.{name}")
+        pre = {k: _clone(v) for k, v in a.items()}
+        got: Dict[str, Tensor] = {}
+
+        def written(k, v):                        # expected() reads earlier outputs through `got`
+            a[k].copy_(v.reshape(a[k].shape).to(a[k].dtype))
+            got[k] = a[k].detach().clone()
+        expected(name, pre, got, on_output=written)
+    return run
+
+
+def trace(eng, x: Tensor, kw: dict, ln_mode: str, impl=real_impl, prime: Optional[Callable] = None) -> List[Launch]:
+    """Run eng.run_blocks(x, **kw) on the per-kernel loop in `ln_mode` with every launch traced.  In fold mode with
+    kw['primed'], prime(x, xb, stats) first writes the workspace's bf16 copy of x and its row statistics (not traced),
+    as an embedding kernel would; every other workspace buffer starts as NaN."""
+    S = schedule()
+    with S.recording(eng, S.caller_buffers(eng, x, kw), ln_mode, "python", recorder=tracer(impl)) as rec:
+        for buf in eng.workspace(x.shape[0], x.device).values():      # a launch reading a stale buffer reads NaN
+            buf.fill_(math.nan)
+        if kw.get("primed"):
+            xb, st = eng.entry_buffers(x.shape[0], x.device)
+            if xb is not None:
+                prime(x, xb, st)
+        eng.run_blocks(x, **kw)
+    return rec.launches
+
+
+def prime_exact(x: Tensor, xb: Tensor, stats: Tensor) -> None:
+    """The embedding's bf16 copy of x and its row statistics, from their fp64 reference."""
+    xb.copy_(x.bfloat16())
+    stats.copy_(RB.row_stats_reference(xb)[0].view(stats.shape).float())
+
+
+# ------------------------------------------------------------------------------------------------------ references
+def rope_reference(qkv: Tensor, cs: Tensor, rows: int, H: int, dh: int) -> Tensor:
+    """b200vit_rope_qk's arithmetic (GoldenGateRoPENd, vit_nd_rotary.py:79-96) on the packed buffer qkv[T, 3 H dh], in
+    fp32: q and k of token t rotated by table row t % rows, v as it was."""
+    T = qkv.shape[0]
+    t = qkv.view(T, 3, H, dh).float()
+    r = torch.arange(T, device=qkv.device) % rows
+    c, s = cs[r][..., 0][:, None], cs[r][..., 1][:, None]
+    a, b = t[:, :2, :, : dh // 2], t[:, :2, :, dh // 2:]
+    out = qkv.view(T, 3, H, dh).clone()
+    out[:, :2] = torch.cat((a * c - b * s, a * s + b * c), dim=-1).bfloat16()
+    return out.view(T, -1)
+
+
+def _exact(v: Tensor) -> Tuple[Tensor, Tensor]:
+    return v.double(), torch.zeros(v.shape, dtype=torch.float64, device=v.device)
+
+
+def _stats(xb: Tensor, like: Tensor) -> Tuple[Tensor, Tensor]:
+    """(ref, bound) of row statistics `like` ([M, 2], [M, 1, 2] or [M, parts, 2]) of the bf16 rows xb: one part, the
+    emit_row_stats writers (rowstats_cast, the embedding, the local patch interaction); several, a GEMM's EPI_STATS."""
+    parts = like.numel() // (2 * xb.shape[0])
+    if parts == 1:
+        r, b = RB.row_stats_reference(xb)
+    else:
+        r, b = Bd.stats_reference(xb, parts)
+    return r.view(like.shape), b.view(like.shape)
+
+
+def expected(name: str, a: dict, got: dict, on_output: Optional[Callable] = None, plain: Optional[Tensor] = None
+             ) -> Dict[str, Tuple[Tensor, Tensor]]:
+    """(ref, bound) of every output of launch `name` on its operands `a` (the clones taken before it), from the
+    existing fp64 oracle of its kernel.  Outputs that derive from another output (a bf16 copy, row statistics) are
+    referred to the kernel's own value of it in `got`.  on_output(name, ref) runs as each is made (the emulation
+    writes it and adds it to `got`).  gemm_headnorm: `plain`, the same launch's bf16 output without the head norm
+    (its norm is bounded on those values); the emulation rounds the GEMM's reference."""
+    out: Dict[str, Tuple[Tensor, Tensor]] = {}
+
+    def put(k, rb):
+        out[k] = rb
+        if on_output is not None:
+            on_output(k, rb[0])
+
+    if name in ("gemm", "gemm_headnorm"):
+        w = a["w"]
+        K = a.get("k") or w.shape[1]
+        kw = dict(bias=a["bias"], ln_sums=a["ln_sums"], col_s=a["col_s"], ln_eps=f32(a["ln_eps"]))
+        if name == "gemm":
+            kw.update(resid=a["resid"], gelu=a["gelu"])
+            if a["out_f32"] is not None:
+                put("out_f32", Bd.gemm_reference(a["a"][:, :K], w[:, :K], **kw))
+                if a["out_bf16"] is not None:       # the bf16 copy of the kernel's own fp32 result
+                    put("out_bf16", _exact(got["out_f32"].bfloat16()))
+            elif a["out_bf16"] is not None:
+                put("out_bf16", Bd.gemm_reference(a["a"][:, :K], w[:, :K], bf16_out=True, **kw))
+            if a["stats_out"] is not None:
+                put("stats_out", _stats(got["out_bf16"], a["stats_out"]))
+            return out
+        ref, bnd = Bd.gemm_reference(a["a"][:, :K], w[:, :K], bf16_out=True, **kw)
+        out["plain"] = (ref, bnd)
+        p = ref.float().bfloat16() if plain is None else plain
+        M, nh, dh = p.shape[0], a["norm_heads"], a["dh"]
+        heads = p[:, :nh * dh].reshape(M, nh, dh)
+        g = a["head_gamma"].view(nh, dh)
+        eps = a["head_layernorm_eps"]
+        r, b = RB.rmsnorm_heads_reference(heads, g) if eps is None else RB.layernorm_heads_reference(heads, g, f32(eps))
+        ref, bnd = _exact(p)
+        ref[:, :nh * dh], bnd[:, :nh * dh] = r.reshape(M, -1), b.reshape(M, -1)
+        put("out_bf16", (ref, bnd))
+        return out
+    if name == "layernorm":
+        kw = dict(row_index=a["row_index"], eps=f32(a["eps"]))
+        if a["out_f32"] is not None:
+            put("out_f32", RB.layernorm_reference(a["x"], a["gamma"], a["beta"], **kw))
+        if a["out_bf16"] is not None:
+            put("out_bf16", RB.layernorm_reference(a["x"], a["gamma"], a["beta"], bf16_out=True, **kw))
+        return out
+    if name == "rowstats_cast":
+        put("xb", _exact(a["x"].bfloat16()))
+        put("stats", _stats(got["xb"], a["stats"]))
+        return out
+    if name == "rope_qk":
+        put("qkv", _exact(rope_reference(a["qkv"], a["cs"], a["rows"], a["H"], a["dh"])))
+        return out
+    if name == "attention":
+        put("out", AB.qkv_attention_reference(a["qkv"], [a["N"]] * a["B"], a["H"], a["dh"], a["scale"],
+                                              mask_self=a["mask_self"]))
+        return out
+    if name == "attention_varlen":
+        lengths = a["cu_seqlens"].diff().tolist()
+        put("out", AB.qkv_attention_reference(a["qkv"], lengths, a["H"], a["dh"], a["scale"],
+                                              mask_self=a["mask_self"]))
+        return out
+    if name == "attention_axial":
+        put("out", AB.axial_reference(a["qkv"], a["key_mask"], a["B"], a["L"], a["G"], a["H"], a["dh"], a["scale"],
+                                      a["zero_masked_rows"]))
+        return out
+    if name == "attention_headmix":
+        ref, bnd = HB.headmix_reference(a["qkv"], a["B"], a["N"], a["H"], a["dh"], a["scale"], a["pre"], a["post"],
+                                        a["head_ln"])
+        put("out", (ref.reshape(a["B"] * a["N"], -1), bnd.reshape(a["B"] * a["N"], -1)))
+        return out
+    if name == "attention_xca":
+        put("out", FB.xca_reference(a["qkv"], a["tau"], a["B"], a["N"], a["H"], a["dh"]))
+        return out
+    if name == "local_patch_interaction":
+        put("y", lpi_reference(a["x"], a["ln"], a["w1"], a["b1"], a["w2"], a["b2"], a["B"], a["gh"], a["gw"], a["k"]))
+        if a["y_bf16"] is not None:
+            put("y_bf16", _exact(got["y"].bfloat16()))
+            put("y_stats", _stats(got["y_bf16"], a["y_stats"]))
+        return out
+    raise NotImplementedError(f"no reference of _lib.{name}")
+
+
+def launch_kind(c: Launch) -> str:
+    """A short name of what the launch does, for the accuracy report."""
+    if c.name == "gemm":
+        a = c.args
+        what = "ln-fold" if a["ln_sums"] is not None else "residual" if a["resid"] is not None else "plain"
+        return f"gemm {what}{' gelu' if a['gelu'] else ''}"
+    if c.name == "gemm_headnorm":
+        return "gemm_headnorm " + ("ln" if c.args["head_layernorm_eps"] is not None else "rms")
+    return c.name
+
+
+def check_accuracy(launches: List[Launch], what: str, rerun_plain: Optional[Callable] = None
+                   ) -> Dict[str, float]:
+    """Every traced output within its kernel's bound on the operands it received; worst |got - ref| / bound per
+    launch kind.  rerun_plain(pre): the bf16 output of a gemm_headnorm launch's GEMM without the head norm."""
+    worst: Dict[str, float] = {}
+    for n, c in enumerate(launches):
+        plain = rerun_plain(c.pre) if c.name == "gemm_headnorm" and rerun_plain is not None else None
+        exp = expected(c.name, c.pre, c.post, plain=plain)
+        kind = launch_kind(c)
+        for k, (ref, bnd) in exp.items():
+            got = plain if k == "plain" else c.post.get(k)
+            if got is None:
+                continue
+            r = Bd.check(got.reshape(ref.shape), ref, bnd, f"{what}: launch {n} {kind}: {k}")
+            worst[kind] = max(worst.get(kind, 0.0), r)
+    return worst
+
+
+# ------------------------------------------------------------------------------------------------------ module layers
+@dataclass
+class Ln:
+    gamma: Tensor
+    beta: Optional[Tensor]
+    eps: float
+
+
+def _ln(m: nn.Module) -> Ln:
+    if isinstance(m, nn.LayerNorm):
+        return Ln(m.weight, m.bias, m.eps)
+    return Ln(m.gamma, None, 1e-5)              # NaViT's LayerNorm: F.layer_norm with gamma and a zero beta buffer
+
+
+def _linears(seq: nn.Module) -> List[nn.Linear]:
+    return [m for m in seq if isinstance(m, nn.Linear)]
+
+
+def _out(attn: nn.Module) -> Optional[nn.Linear]:
+    """to_out's Linear, None for the identity (heads == 1 and dim_head == dim, reference vit.py:46-49)."""
+    o = attn.to_out
+    if isinstance(o, nn.Identity):
+        return None
+    return o[0] if isinstance(o, nn.Sequential) else o
+
+
+@dataclass
+class RefLayer:
+    """One layer of the reference module, read through the reference's own attribute paths.  The tensors are the
+    module's parameters (concatenations where the reference projects q, k and v separately); the walk of
+    check_provenance reads nothing else."""
+    ln1: Ln
+    qkv_w: Tensor
+    out: Optional[Tuple[Tensor, Optional[Tensor]]]          # None: to_out is the identity
+    ln2: Ln
+    fc1: Tuple[Tensor, Tensor]
+    fc2: Tuple[Tensor, Tensor]
+    heads: int
+    dim_head: int
+    scale: float
+    mask_self: bool = False
+    qk: Optional[Tuple[str, Tensor, Tensor, float]] = None   # (kind 'rms' | 'ln', q gamma [H, dh], k gamma, eps)
+    headmix: Optional[Tuple[Tensor, Optional[Tensor], Optional[Ln]]] = None   # (post, pre, LayerNorm over heads)
+    tau: Optional[Tensor] = None                             # XCiT's temperature
+    temporal: Optional[Tuple[Ln, Tensor, Optional[Tuple[Tensor, Optional[Tensor]]]]] = None  # (ln, qkv_w, out)
+    out_scale: Optional[Tensor] = None
+    ff_scale: Optional[Tensor] = None
+    lpi: Optional[dict] = None                               # ln, conv1, bn, conv2, scale
+    post_norm: bool = False
+    cat: Tuple[str, ...] = ()                                # fields the engine gets as a concatenation, not `is`
+
+
+def _plain(attn, ff, qkv_w: Optional[Tensor] = None, scale: Optional[float] = None, **kw) -> RefLayer:
+    """A pre-LN layer of `attn` (norm, to_qkv, to_out, heads, dim_head, scale) and `ff` (net: LayerNorm, Linear,
+    ..., Linear); qkv_w / scale in place of the attention's own to_qkv / scale."""
+    o = _out(attn)
+    fc1, fc2 = _linears(ff.net)
+    return RefLayer(ln1=_ln(attn.norm), qkv_w=attn.to_qkv.weight if qkv_w is None else qkv_w,
+                    out=None if o is None else (o.weight, o.bias), ln2=_ln(ff.net[0]), fc1=(fc1.weight, fc1.bias),
+                    fc2=(fc2.weight, fc2.bias), heads=attn.heads, dim_head=attn.dim_head,
+                    scale=float(attn.scale) if scale is None else scale, **kw)
+
+
+def module_layers(mod: nn.Module) -> List[RefLayer]:
+    """The layers of a reference Transformer, by family (the module's class)."""
+    from vit_pytorch_b200 import (cait, cct, deepvit, na_vit, na_vit_nested_tensor, simple_vit_with_qk_norm, vit,
+                                  vit_for_small_dataset, vit_nd_rotary, vivit, xcit)
+    t = type(mod)
+    if t is vit.Transformer:                                                # vit.py:66-83
+        return [_plain(attn, ff) for attn, ff in mod.layers]
+    if t is vit_nd_rotary.Transformer:                                      # vit_nd_rotary.py:115-156: to_qk | to_v
+        return [_plain(attn, ff, qkv_w=torch.cat([attn.to_qk.weight, attn.to_v.weight]), cat=("qkv_w",))
+                for attn, ff in mod.layers]
+    if t is simple_vit_with_qk_norm.Transformer:                            # simple_vit_with_qk_norm.py:66-77
+        return [_plain(attn, ff, qk=("rms", attn.q_norm.gamma, attn.k_norm.gamma, 0.0)) for attn, ff in mod.layers]
+    if t is vit_for_small_dataset.Transformer:                              # LSA, vit_for_small_dataset.py:53-63
+        return [_plain(attn, ff, scale=float(attn.temperature.detach().exp()), mask_self=True)
+                for attn, ff in mod.layers]
+    if t is na_vit.Transformer:                                             # na_vit.py:115-169: softmax scale 1
+        out = []
+        for attn, ff in mod.layers:
+            fc1, fc2 = _linears(ff)
+            H = attn.heads
+            out.append(RefLayer(
+                ln1=_ln(attn.norm), qkv_w=torch.cat([attn.to_q.weight, attn.to_kv.weight]),
+                out=(attn.to_out[0].weight, attn.to_out[0].bias), ln2=_ln(ff[0]), fc1=(fc1.weight, fc1.bias),
+                fc2=(fc2.weight, fc2.bias), heads=H, dim_head=attn.to_q.weight.shape[0] // H, scale=1.0,
+                qk=("rms", attn.q_norm.gamma, attn.k_norm.gamma, 0.0), cat=("qkv_w",)))
+        return out
+    if t is na_vit_nested_tensor.Transformer:                               # na_vit_nested_tensor.py: q / k LayerNorm
+        out = []
+        for attn, ff in mod.layers:
+            fc1, fc2 = _linears(ff)
+            H, dh = attn.heads, attn.dim_head
+            qn = attn.query_norm
+            qk = None if isinstance(qn, nn.Identity) else \
+                ("ln", qn.weight.expand(H, dh), attn.key_norm.weight.expand(H, dh), qn.eps)
+            out.append(RefLayer(
+                ln1=_ln(attn.norm), qkv_w=torch.cat([attn.to_queries.weight, attn.to_keys.weight,
+                                                     attn.to_values.weight]),
+                out=(attn.to_out.weight, attn.to_out.bias), ln2=_ln(ff[0]), fc1=(fc1.weight, fc1.bias),
+                fc2=(fc2.weight, fc2.bias), heads=H, dim_head=dh, scale=dh ** -0.5, qk=qk, cat=("qkv_w", "qk")))
+        return out
+    if t is vivit.Transformer:                                              # vivit.py:75-89
+        return [_plain(attn, ff) for attn, ff in mod.layers]
+    if t is vivit.FactorizedTransformer:                                    # vivit.py:144-150
+        out = []
+        for sa, ta, ff in mod.layers:
+            o = _out(ta)
+            out.append(_plain(sa, ff, temporal=(_ln(ta.norm), ta.to_qkv.weight,
+                                                None if o is None else (o.weight, o.bias))))
+        return out
+    if t is deepvit.Transformer:                                            # deepvit.py:40-75
+        return [_plain(attn, ff, headmix=(attn.reattn_weights, None, _ln(attn.reattn_norm[1])))
+                for attn, ff in mod.layers]
+    if t is cait.Transformer:                                               # cait.py:31-45, 83-122
+        out = []
+        for ls_attn, ls_ff in mod.layers:
+            attn, ff = ls_attn.fn, ls_ff.fn
+            out.append(_plain(attn, ff, qkv_w=torch.cat([attn.to_q.weight, attn.to_kv.weight]),
+                              headmix=(attn.mix_heads_post_attn, attn.mix_heads_pre_attn, None),
+                              out_scale=ls_attn.scale, ff_scale=ls_ff.scale, cat=("qkv_w",)))
+        return out
+    if t is xcit.XCATransformer:                                            # xcit.py:109-167, 196-212
+        out = []
+        for ls_attn, ls_lpi, ls_ff in mod.layers:
+            attn, net = ls_attn.fn, ls_lpi.fn.net
+            lpi = dict(ln=_ln(net[0]), conv1=net[2], bn=net[3], conv2=net[5], scale=ls_lpi.scale)
+            out.append(_plain(attn, ls_ff.fn, scale=1.0, tau=attn.temperature, out_scale=ls_attn.scale,
+                              ff_scale=ls_ff.scale, lpi=lpi))
+        return out
+    if t is cct.TransformerClassifier:                                      # cct.py:84-111, 137-142
+        out = []
+        for blk in mod.blocks:
+            a = blk.self_attn
+            D = a.qkv.in_features
+            out.append(RefLayer(
+                ln1=_ln(blk.pre_norm), qkv_w=a.qkv.weight, out=(a.proj.weight, a.proj.bias), ln2=_ln(blk.norm1),
+                fc1=(blk.linear1.weight, blk.linear1.bias), fc2=(blk.linear2.weight, blk.linear2.bias),
+                heads=a.heads, dim_head=D // a.heads, scale=float(a.scale), post_norm=True))
+        return out
+    raise NotImplementedError(f"no reference layer table for {t.__module__}.{t.__name__}")
+
+
+def check_identity(mod: nn.Module, case: str = "") -> None:
+    """Each EncoderLayer field the module describes to the engine IS the reference module's parameter (`is`; equal
+    values for the concatenations), so a swapped LayerNorm or a wrong layer index cannot hide behind a
+    self-consistent description."""
+    layers, _ = mod.encoder_layers()
+    refs = module_layers(mod)
+    if len(layers) != len(refs):
+        raise AssertionError(f"{case}: encoder_layers() describes {len(layers)} layers, the module has {len(refs)}")
+
+    def same(i, what, got, want, cat=False):
+        if got is None and want is None:
+            return
+        ok = got is want or (cat and got is not None and want is not None and got.shape == want.shape
+                             and torch.equal(got, want))
+        if not ok:
+            raise AssertionError(f"{case}: layer {i}: EncoderLayer.{what} is not the module's parameter")
+
+    for i, (L, R) in enumerate(zip(layers, refs)):
+        for nm, got, want in (("ln1", L.ln1, R.ln1), ("ln2", L.ln2, R.ln2)):
+            same(i, f"{nm}.gamma", got.gamma, want.gamma)
+            same(i, f"{nm}.beta", got.beta, want.beta)
+        same(i, "qkv_w", L.qkv_w, R.qkv_w, "qkv_w" in R.cat)
+        same(i, "out_w", L.out_w, None if R.out is None else R.out[0])
+        same(i, "out_b", L.out_b, None if R.out is None else R.out[1])
+        same(i, "fc1_w", L.fc1_w, R.fc1[0])
+        same(i, "fc1_b", L.fc1_b, R.fc1[1])
+        same(i, "fc2_w", L.fc2_w, R.fc2[0])
+        same(i, "fc2_b", L.fc2_b, R.fc2[1])
+        same(i, "out_scale", L.out_scale, R.out_scale)
+        same(i, "ff_scale", L.ff_scale, R.ff_scale)
+        if R.qk is not None:
+            same(i, "qk_gamma[0]", L.qk_gamma[0], R.qk[1], "qk" in R.cat)
+            same(i, "qk_gamma[1]", L.qk_gamma[1], R.qk[2], "qk" in R.cat)
+        if R.headmix is not None:
+            same(i, "attention.post", L.attention.post, R.headmix[0])
+            same(i, "attention.pre", L.attention.pre, R.headmix[1])
+            if R.headmix[2] is not None:
+                same(i, "attention.ln.gamma", L.attention.ln.gamma, R.headmix[2].gamma)
+                same(i, "attention.ln.beta", L.attention.ln.beta, R.headmix[2].beta)
+        if R.tau is not None:
+            same(i, "attention.tau", L.attention.tau, R.tau)
+        if R.temporal is not None:
+            T = L.temporal
+            same(i, "temporal.ln.gamma", T.ln.gamma, R.temporal[0].gamma)
+            same(i, "temporal.ln.beta", T.ln.beta, R.temporal[0].beta)
+            same(i, "temporal.qkv_w", T.qkv_w, R.temporal[1])
+            same(i, "temporal.out_w", T.out_w, None if R.temporal[2] is None else R.temporal[2][0])
+            same(i, "temporal.out_b", T.out_b, None if R.temporal[2] is None else R.temporal[2][1])
+        if R.lpi is not None:
+            P, r = L.lpi, R.lpi
+            for what, got, want in (("ln.gamma", P.ln.gamma, r["ln"].gamma), ("ln.beta", P.ln.beta, r["ln"].beta),
+                                    ("conv1_w", P.conv1_w, r["conv1"].weight), ("conv1_b", P.conv1_b, r["conv1"].bias),
+                                    ("bn_w", P.bn_w, r["bn"].weight), ("bn_b", P.bn_b, r["bn"].bias),
+                                    ("bn_mean", P.bn_mean, r["bn"].running_mean),
+                                    ("bn_var", P.bn_var, r["bn"].running_var),
+                                    ("conv2_w", P.conv2_w, r["conv2"].weight), ("conv2_b", P.conv2_b, r["conv2"].bias),
+                                    ("scale", P.scale, r["scale"])):
+                same(i, f"lpi.{what}", got, want)
+
+
+# ------------------------------------------------------------------------------------------------------ provenance
+def _bits(t: Tensor) -> Tensor:
+    return t.view({torch.float32: torch.int32, torch.bfloat16: torch.int16, torch.float64: torch.int64}.get(
+        t.dtype, t.dtype)) if t.dtype in (torch.float32, torch.bfloat16, torch.float64) else t
+
+
+def _lpi_folded(P: dict, k: int):
+    """(w1, b1, w2, b2) fp64 [k k, D] / [D] of the local patch interaction recomputed from the module's conv and
+    BatchNorm parameters (xcit.py:150-167): BatchNorm (eval) into conv1, LayerScale into conv2; and (bound) the fp32
+    rounding the host's fold may add: 5 u for w' = w g / sqrt(var + eps), 6 u |(b - mean) inv| + u |b1| for b1,
+    u for each product with the scale."""
+    d = lambda t: t.detach().double()                                                   # noqa: E731
+    c1, bn, c2 = P["conv1"], P["bn"], P["conv2"]
+    D = c1.weight.shape[0]
+    zeros = torch.zeros(D, dtype=torch.float64, device=c1.weight.device)
+    inv = d(bn.weight) / torch.sqrt(d(bn.running_var) + f32(bn.eps))
+    w1 = (d(c1.weight).reshape(D, k * k) * inv[:, None]).t()
+    cb = (d(c1.bias) if c1.bias is not None else zeros) - d(bn.running_mean)
+    b1 = cb * inv + d(bn.bias)
+    s = d(P["scale"]).reshape(D) if P["scale"] is not None else torch.ones_like(zeros)
+    w2 = (d(c2.weight).reshape(D, k * k) * s[:, None]).t()
+    b2 = (d(c2.bias) if c2.bias is not None else zeros) * s
+    return [(w1, 5 * U * w1.abs()), (b1, 6 * U * (cb * inv).abs() + U * (b1.abs() + d(bn.bias).abs())),
+            (w2, U * w2.abs()), (b2, U * b2.abs())]
+
+
+class ProvenanceError(AssertionError):
+    pass
+
+
+class Walk:
+    """The provenance walk of one trace (check_provenance)."""
+
+    def __init__(self, case: str, launches: List[Launch], fold: bool, kw: dict) -> None:
+        self.case, self.calls, self.fold, self.kw = case, launches, fold, kw
+        self.pos, self.where, self.cur = 0, "", None
+        self.have_stats = fold and bool(kw.get("primed"))
+
+    # ---------------------------------------------------------------- failures and comparisons
+    def fail(self, op: str, msg: str):
+        c = self.cur
+        launch = f"launch {self.pos - 1} {c.name}" if c is not None else "no launch"
+        raise ProvenanceError(f"{self.case}: {self.where}: {launch}: operand {op}: {msg}")
+
+    def take(self, *names: str) -> Launch:
+        if self.pos >= len(self.calls):
+            self.cur = None
+            self.fail("-", f"the trace ended, {' or '.join(names)} expected")
+        c = self.calls[self.pos]
+        self.pos, self.cur = self.pos + 1, c
+        if c.name not in names:
+            self.fail("-", f"{' or '.join(names)} expected")
+        return c
+
+    def same(self, op: str, got, want) -> None:
+        """Bit for bit (None only as None)."""
+        if want is None or got is None:
+            if got is not want:
+                self.fail(op, f"got {'None' if got is None else 'a tensor'}, want "
+                              f"{'None' if want is None else 'a tensor'}")
+            return
+        if got.dtype != want.dtype or tuple(got.shape) != tuple(want.shape):
+            self.fail(op, f"got {got.dtype} {tuple(got.shape)}, want {want.dtype} {tuple(want.shape)}")
+        want = want.to(got.device)
+        bad = _bits(got.contiguous()) != _bits(want.contiguous())
+        if bool(bad.any()):
+            i = tuple(bad.nonzero()[0].tolist())
+            self.fail(op, f"{int(bad.sum())} of {bad.numel()} elements differ, first at {i}: got {got[i].item()!r}, "
+                          f"want {want[i].item()!r}")
+
+    def within(self, op: str, got: Tensor, ref: Tensor, bound: Tensor) -> None:
+        ref, bound = ref.to(got.device), bound.to(got.device)
+        d = (got.double().reshape(ref.shape) - ref).abs()
+        bad = ~(d <= bound)
+        if bool(bad.any()):
+            i = tuple(bad.nonzero()[0].tolist())
+            self.fail(op, f"{int(bad.sum())} of {bad.numel()} elements outside the bound, first at {i}: got "
+                          f"{got.reshape(ref.shape)[i].item()!r}, want {ref[i].item()!r} +- {bound[i].item():.3e}")
+
+    def value(self, op: str, got, want) -> None:
+        if isinstance(want, float) and isinstance(got, (int, float)) and not isinstance(got, bool):
+            ok = f32(got) == f32(want)
+        else:
+            ok = got == want and type(got) is type(want)
+        if not ok:
+            self.fail(op, f"got {got!r}, want {want!r}")
+
+    def stats(self, op: str, got: Tensor, xb: Tensor) -> None:
+        self.within(op, got, *_stats(xb, got))
+
+    # ---------------------------------------------------------------- steps
+    def normed(self, S: Tensor, ln: Ln, W: Tensor, b: Optional[Tensor], gelu: bool = False,
+               head: Optional[tuple] = None, heads: int = 0, dh: int = 0) -> Tensor:
+        """out = LN(S) W^T + b (reference vit.py:19-21 / :52-54): the bf16 output of its GEMM."""
+        gemm = "gemm_headnorm" if head is not None else "gemm"
+        d = lambda t: t.detach().double()                                               # noqa: E731
+        if self.fold:
+            if not self.have_stats:
+                c = self.take("rowstats_cast")
+                self.same("x", c.pre["x"], S)
+                self.have_stats = True
+            c = self.take(gemm)
+            a = c.pre
+            self.same("a", a["a"], S.bfloat16())
+            self.stats("ln_sums", a["ln_sums"], a["a"])
+            self.value("ln_eps", a["ln_eps"], float(ln.eps))
+            wg = (d(W) * d(ln.gamma)[None]).float().bfloat16()
+            self.same("w (gamma W)", a["w"], wg)
+            K = W.shape[1]
+            wd = wg.double()
+            self.within("col_s", a["col_s"], wd.sum(1), K * U * wd.abs().sum(1))
+            t = torch.zeros(W.shape[0], dtype=torch.float64, device=W.device)
+            tb = torch.zeros_like(t)
+            if ln.beta is not None:
+                t, tb = d(W) @ d(ln.beta), d(W).abs() @ d(ln.beta).abs()
+            if b is not None:
+                t, tb = t + d(b), tb + d(b).abs()
+            self.within("bias (W beta + b)", a["bias"], t, (K + 1) * U * tb)
+        else:
+            c = self.take("layernorm")
+            a = c.pre
+            self.same("x", a["x"], S)
+            self.same("gamma", a["gamma"], ln.gamma.detach().float())
+            self.same("beta", a["beta"], None if ln.beta is None else ln.beta.detach().float())
+            self.value("eps", a["eps"], float(ln.eps))
+            self.same("row_index", a["row_index"], None)
+            self.same("out_f32", a["out_f32"], None)
+            xn = c.post["out_bf16"]
+            c = self.take(gemm)
+            a = c.pre
+            self.same("a", a["a"], xn)
+            self.same("w", a["w"], W.detach().bfloat16())
+            self.same("bias", a["bias"], None if b is None else b.detach().float())
+            self.same("ln_sums", a["ln_sums"], None)
+        if head is None:
+            self.value("gelu", a["gelu"], gelu)
+            self.same("resid", a["resid"], None)
+            self.same("out_f32", a["out_f32"], None)
+        else:
+            kind, gq, gk, eps = head
+            self.same("head_gamma", a["head_gamma"], torch.cat([gq.detach().float().reshape(-1),
+                                                                gk.detach().float().reshape(-1)]))
+            self.value("norm_heads", a["norm_heads"], 2 * heads)
+            self.value("dh", a["dh"], dh)
+            self.value("head_layernorm_eps", a["head_layernorm_eps"], float(eps) if kind == "ln" else None)
+        return c.post["out_bf16"]
+
+    def residual(self, A: Tensor, out: Optional[Tuple[Tensor, Optional[Tensor]]], s: Optional[Tensor],
+                 resid: Tensor, copy: bool, D: int) -> Tensor:
+        """resid + (A W^T + b) s (reference vit.py:64,80-81; LayerScale cait.py:31-45): the new fp32 stream."""
+        c = self.take("gemm")
+        a = c.pre
+        d = lambda t: t.detach().double()                                               # noqa: E731
+        W, b = (None, None) if out is None else out
+        Wd = torch.eye(D, dtype=torch.float64, device=resid.device) if W is None else d(W)
+        bd = None if b is None else d(b)
+        if s is not None:
+            Wd, bd = Wd * d(s).reshape(-1, 1), None if bd is None else bd * d(s).reshape(-1)
+        self.same("a", a["a"], A)
+        self.same("w", a["w"], Wd.float().bfloat16())
+        self.same("bias", a["bias"], None if bd is None else bd.float())
+        self.same("resid", a["resid"], resid)
+        self.same("ln_sums", a["ln_sums"], None)
+        self.value("gelu", a["gelu"], False)
+        if a["out_f32"] is None:
+            self.fail("out_f32", "the residual GEMM writes no fp32 stream")
+        new = c.post["out_f32"]
+        if copy and self.fold:
+            if a["out_bf16"] is None or a["stats_out"] is None:
+                self.fail("out_bf16", "the stream's bf16 copy and row statistics are not written")
+            self.same("out_bf16", c.post["out_bf16"], new.bfloat16())
+            self.stats("stats_out", c.post["stats_out"], c.post["out_bf16"])
+            self.have_stats = True
+        else:
+            self.same("out_bf16", a["out_bf16"], None)
+            self.same("stats_out", a["stats_out"], None)
+        return new
+
+    def attention(self, R: RefLayer, qkv: Tensor, M: int, temporal: bool = False) -> Tensor:
+        kw = self.kw
+        axial = kw.get("axial")
+        if R.headmix is not None:
+            c = self.take("attention_headmix")
+        elif R.tau is not None:
+            c = self.take("attention_xca")
+        elif temporal or (axial is not None and R.temporal is None):
+            c = self.take("attention_axial")
+        else:
+            c = self.take("attention", "attention_varlen")
+        a = c.pre
+        self.same("qkv", a["qkv"], qkv)
+        self.value("H", a["H"], R.heads)
+        self.value("dh", a["dh"], R.dim_head)
+        if c.name != "attention_xca":
+            self.value("scale", a["scale"], float(R.scale))
+        if c.name in ("attention", "attention_headmix", "attention_xca"):
+            self.value("B", a["B"], kw["B"])
+            self.value("N", a["N"], kw["N"])
+        if c.name in ("attention", "attention_varlen"):
+            self.value("mask_self", a["mask_self"], R.mask_self)
+        if c.name == "attention_varlen":
+            vl = kw.get("varlen")
+            want = vl.cu if vl is not None else torch.arange(0, kw["B"] * kw["N"] + 1, kw["N"], dtype=torch.int32)
+            self.same("cu_seqlens", a["cu_seqlens"], want.to(a["cu_seqlens"].device))
+        if c.name == "attention_axial":
+            G, T, km, zero = axial
+            self.value("L", a["L"], T)
+            self.value("G", a["G"], G)
+            self.value("B", a["B"], M // (T * G))
+            self.value("zero_masked_rows", a["zero_masked_rows"], zero)
+            self.same("key_mask", a["key_mask"], km)
+        if c.name == "attention_headmix":
+            post, pre, hln = R.headmix
+            self.same("post", a["post"], post.detach().float())
+            self.same("pre", a["pre"], None if pre is None else pre.detach().float())
+            if hln is None:
+                self.value("head_ln", a["head_ln"], None)
+            else:
+                self.same("head_ln gamma", a["head_ln"][0], hln.gamma.detach().float())
+                self.same("head_ln beta", a["head_ln"][1], hln.beta.detach().float())
+                self.value("head_ln eps", a["head_ln"][2], float(hln.eps))
+        if c.name == "attention_xca":
+            tau = R.tau.detach().double().exp().reshape(-1)
+            self.within("tau (exp temperature)", a["tau"], tau, 4 * U * tau)
+        return c.post["out"]
+
+    def lpi(self, R: RefLayer, S: Tensor) -> Tensor:
+        """y = S + LPI(S) (xcit.py:150-167, 208-211)."""
+        c = self.take("local_patch_interaction")
+        a, P = c.pre, R.lpi
+        k = P["conv1"].kernel_size[0]
+        self.same("x", a["x"], S)
+        self.same("ln gamma", a["ln"][0], P["ln"].gamma.detach().float())
+        self.same("ln beta", a["ln"][1], P["ln"].beta.detach().float())
+        self.value("ln eps", a["ln"][2], float(P["ln"].eps))
+        for op, (ref, bnd) in zip(("w1", "b1", "w2", "b2"), _lpi_folded(P, k)):
+            self.within(op, a[op], ref, bnd)
+        grid = self.kw["grid"]
+        self.value("B", a["B"], self.kw["B"])
+        self.value("gh", a["gh"], grid[0])
+        self.value("gw", a["gw"], grid[1])
+        self.value("k", a["k"], k)
+        y = c.post["y"]
+        if self.fold:
+            self.same("y_bf16", c.post.get("y_bf16"), y.bfloat16())
+            self.stats("y_stats", c.post["y_stats"], c.post["y_bf16"])
+            self.have_stats = True
+        else:
+            self.same("y_bf16", a["y_bf16"], None)
+        return y
+
+    def post_norm(self, R: RefLayer, S: Tensor) -> Tuple[Tensor, Tensor]:
+        """x = LN2(x); h = GELU(fc1(x)) (cct.py:137-142): (the new stream, h)."""
+        c = self.take("layernorm")
+        a = c.pre
+        self.same("x", a["x"], S)
+        self.same("gamma", a["gamma"], R.ln2.gamma.detach().float())
+        self.same("beta", a["beta"], R.ln2.beta.detach().float())
+        self.value("eps", a["eps"], float(R.ln2.eps))
+        if a["out_f32"] is None or a["out_bf16"] is None:
+            self.fail("out_f32", "the post-norm writes the stream and its bf16 copy")
+        y, yb = c.post["out_f32"], c.post["out_bf16"]
+        c = self.take("gemm")
+        a = c.pre
+        self.same("a", a["a"], yb)
+        self.same("w", a["w"], R.fc1[0].detach().bfloat16())
+        self.same("bias", a["bias"], R.fc1[1].detach().float())
+        self.value("gelu", a["gelu"], True)
+        self.same("ln_sums", a["ln_sums"], None)
+        self.have_stats = False
+        return y, c.post["out_bf16"]
+
+
+def check_provenance(mod: nn.Module, x0: Tensor, kw: dict, launches: List[Launch], ln_mode: str,
+                     case: str = "") -> int:
+    """Walk the trace of run_blocks(x0, **kw) through the layers of the reference module `mod` in its forward's
+    order (reference vit.py:78-81 and the family lines cited in module_layers) and assert every launch received what
+    that forward defines.  Returns the number of launches checked; raises ProvenanceError naming the case, the layer,
+    the launch, the operand and the first differing element."""
+    check_identity(mod, case)
+    refs = module_layers(mod)
+    w = Walk(case, launches, ln_mode == "fold", kw)
+    S = x0
+    M, D = x0.shape
+    rope = kw.get("rope")
+    run = kw.get("layers")
+    for i in (range(len(refs)) if run is None else run):
+        R = refs[i]
+        w.where = f"layer {i} qkv"
+        head = None if R.qk is None else R.qk
+        qkv = w.normed(S, R.ln1, R.qkv_w, None, head=head, heads=R.heads, dh=R.dim_head)
+        if rope is not None:                                   # vit_nd_rotary.py:143-147
+            w.where = f"layer {i} rope"
+            c = w.take("rope_qk")
+            w.same("qkv", c.pre["qkv"], qkv)
+            w.same("cs", c.pre["cs"], rope[0])
+            w.value("rows", c.pre["rows"], rope[1])
+            w.value("H", c.pre["H"], R.heads)
+            w.value("dh", c.pre["dh"], R.dim_head)
+            qkv = c.post["qkv"]
+        w.where = f"layer {i} attention"
+        o = w.attention(R, qkv, M)
+        w.where = f"layer {i} out"
+        S = w.residual(o, R.out, R.out_scale, S, copy=R.lpi is None and not R.post_norm, D=D)
+        if R.temporal is not None:                             # vivit.py:144-150
+            ln, tw, tout = R.temporal
+            w.where = f"layer {i} temporal qkv"
+            tq = w.normed(S, ln, tw, None)
+            w.where = f"layer {i} temporal attention"
+            to = w.attention(R, tq, M, temporal=True)
+            w.where = f"layer {i} temporal out"
+            S = w.residual(to, tout, None, S, copy=True, D=D)
+        Y = S
+        if R.lpi is not None:
+            w.where = f"layer {i} local patch interaction"
+            Y = w.lpi(R, S)
+        if R.post_norm:
+            w.where = f"layer {i} post-norm fc1"
+            Y, h = w.post_norm(R, S)
+        else:
+            w.where = f"layer {i} fc1"
+            h = w.normed(Y, R.ln2, R.fc1[0], R.fc1[1], gelu=True)
+        w.where = f"layer {i} fc2"
+        S = w.residual(h, R.fc2, R.ff_scale, Y, copy=True, D=D)
+    if w.pos != len(launches):
+        w.where, w.cur = "after the last layer", launches[w.pos]
+        w.pos += 1
+        w.fail("-", "a launch the reference forward does not define")
+    return w.pos

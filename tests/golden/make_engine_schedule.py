@@ -228,13 +228,18 @@ class Recorder:
                     for f, ty in v._fields_}
         raise TypeError(f"cannot record {type(v)}")
 
+    @staticmethod
+    def bind(sig: inspect.Signature, args: tuple, kwargs: dict) -> dict:
+        """A call's arguments by parameter name, bound against the real function's signature, defaults applied."""
+        bound = sig.bind(*args, **kwargs)
+        bound.apply_defaults()
+        return dict(bound.arguments)
+
     def recorder(self, name: str, real: Callable) -> Callable:
         sig = inspect.signature(real)
 
         def record(*args, **kwargs):
-            bound = sig.bind(*args, **kwargs)
-            bound.apply_defaults()
-            self.calls.append({"call": name, **{k: self.value(v) for k, v in bound.arguments.items()}})
+            self.calls.append({"call": name, **{k: self.value(v) for k, v in self.bind(sig, args, kwargs).items()}})
         return record
 
 

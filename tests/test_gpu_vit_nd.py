@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from conftest import GOLDEN_DIR, load_golden
+from oracle.layer_trace import rope_reference
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.vit_nd import PatchifyND, ViTND, ensure_tuple
 from vit_pytorch_b200.vit_nd_rotary import ViTND as RotaryViTND
@@ -65,18 +66,6 @@ def test_patchify_nd_large_rows_vector_path():
 
 
 # ------------------------------------------------------------------------------------------------------ rope_qk
-def rope_reference(qkv, cs, R, H, dh):
-    """GoldenGateRoPENd's arithmetic (vit_nd_rotary.py:79-96) on the packed buffer, in torch fp32."""
-    T = qkv.shape[0]
-    t = qkv.view(T, 3, H, dh).float()
-    rows = torch.arange(T, device=qkv.device) % R
-    c, s = cs[rows][..., 0][:, None], cs[rows][..., 1][:, None]     # (T, 1, H, f)
-    x, y = t[:, :2, :, : dh // 2], t[:, :2, :, dh // 2:]
-    out = qkv.view(T, 3, H, dh).clone()
-    out[:, :2] = torch.cat((x * c - y * s, x * s + y * c), dim=-1).bfloat16()
-    return out.view(T, -1)
-
-
 @pytest.mark.parametrize("dh", [32, 64, 80, 128])
 @pytest.mark.parametrize("per_token", [False, True])
 def test_rope_qk_bitwise(dh, per_token):

@@ -9,7 +9,7 @@ import torch
 
 from conftest import GOLDEN_DIR
 from oracle import bounds as Bd
-from oracle.attention_bounds import attention_reference
+from oracle.attention_bounds import axial_reference
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.vivit import FactorizedTransformer, Transformer, ViViT
 
@@ -27,17 +27,6 @@ def stats(got, ref):
 
 
 # ------------------------------------------------------------------------------------------------------ attention_axial
-def axial_reference(qkv, key_mask, B, L, G, H, dh, scale, zero_masked_rows):
-    """(ref, bound) [B L G, H dh] of the B*G*H sequences (token j of b*G + p at row b*L*G + j*G + p) from
-    attention_bounds.attention_reference with the key mask of each sequence's batch element: one 64-key block, a row
-    without a kept key 0 (zero_masked_rows) or the mean of its sequence's values."""
-    t = qkv.view(B, L, G, 3, H, dh).permute(3, 0, 2, 4, 1, 5).reshape(3, B * G * H, L, dh)
-    km = None if key_mask is None else key_mask.bool()[:, None, None, :].expand(B, G, H, L).reshape(B * G * H, L)
-    ref, bound = attention_reference(t[0], t[1], t[2], scale, kb=64, key_mask=km, zero_masked_rows=zero_masked_rows)
-    back = lambda x: x.view(B, G, H, L, dh).permute(0, 3, 1, 2, 4).reshape(B * L * G, H * dh)   # noqa: E731
-    return back(ref), back(bound)
-
-
 @pytest.mark.parametrize("dh", [32, 64, 80, 128])
 @pytest.mark.parametrize("L", [1, 2, 5, 8, 17, 33, 64])
 @pytest.mark.parametrize("G", [1, 3, 50, 197])

@@ -1,17 +1,17 @@
 """-m gpu: the cross-covariance attention kernel (b200vit_attention_xca), the local patch interaction kernel
 (b200vit_local_patch_interaction), class attention at dim_head 48 and the fused XCiT on the H100.  The attention kernels
 are checked against the fp64 references and per-element bounds of oracle/attention_fp32_bounds.py, the patch
-interaction against an fp32 torch expression on the same data; the model's CUDA-graph replay and fallback rules
+interaction against those of oracle/lpi_bounds.py; the model's CUDA-graph replay and fallback rules
 (its reference parity is in test_gpu_family_parity.py)."""
 import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from conftest import GOLDEN_DIR
 from oracle import attention_fp32_bounds as FB
 from oracle import bounds as Bd
+from oracle.lpi_bounds import lpi_reference
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.xcit import XCATransformer, XCiT
 
@@ -87,15 +87,6 @@ def test_attention_xca_keeps_each_image_to_itself():
 
 
 # ------------------------------------------------------------------------------------------------ local patch interaction
-def lpi_reference(x, B, gh, gw, ln, w1, b1, w2, b2, k):
-    """F.layer_norm -> depthwise conv (folded weights) -> GELU -> depthwise conv, plus x, in fp32."""
-    D = x.shape[1]
-    z = F.layer_norm(x.view(B, gh, gw, D), (D,), ln[0], ln[1], ln[2]).permute(0, 3, 1, 2)
-    u = F.gelu(F.conv2d(z, w1.t().reshape(D, 1, k, k), b1, padding=k // 2, groups=D))
-    y = F.conv2d(u, w2.t().reshape(D, 1, k, k), b2, padding=k // 2, groups=D).permute(0, 2, 3, 1)
-    return x + y.reshape(-1, D)
-
-
 @pytest.mark.parametrize("D", [64, 384, 1024])
 @pytest.mark.parametrize("k", [1, 3, 5, 7])
 @pytest.mark.parametrize("grid", [(1, 1), (1, 7), (2, 2), (6, 8), (14, 14), (56, 56)])
@@ -114,10 +105,8 @@ def test_local_patch_interaction_against_fp32(grid, k, D):
     ys = torch.empty(M, 2, device=DEV)
     scratch = torch.empty(M, 2, device=DEV)
     _lib.local_patch_interaction(x, y, scratch, ln, w1, b1, w2, b2, B, gh, gw, k, y_bf16=yb, y_stats=ys)
-    want = lpi_reference(x, B, gh, gw, ln, w1, b1, w2, b2, k)
     assert torch.equal(x, x0)                              # the input stream is left as it was
-    mx = (y - want).abs().max().item()
-    assert mx < 1e-4 * max(1.0, want.abs().max().item()), mx
+    Bd.check(y, *lpi_reference(x, ln, w1, b1, w2, b2, B, gh, gw, k), f"lpi {gh}x{gw} k{k} D{D}")
     # the bf16 copy and the statistics are exactly what rowstats_cast writes for y
     rb, rs = torch.empty_like(yb), torch.empty_like(ys)
     _lib.rowstats_cast(y, rb, rs)
