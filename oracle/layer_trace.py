@@ -23,6 +23,7 @@ within a layer).  The clones go on the current stream.  `impl` runs a launch: th
 trace runs the per-kernel Python loop; the one-call C loop must be bit-identical to it."""
 from __future__ import annotations
 
+import dataclasses
 import inspect
 import math
 import os
@@ -36,6 +37,7 @@ from torch import nn
 from oracle import attention_bounds as AB
 from oracle import attention_fp32_bounds as FB
 from oracle import bounds as Bd
+from oracle import grid_attention_bounds as GB
 from oracle import headmix_bounds as HB
 from oracle import row_bounds as RB
 from oracle.lpi_bounds import lpi_reference
@@ -57,7 +59,18 @@ OUTPUTS = {
     "attention_headmix": ("out",),
     "attention_xca": ("out",),
     "local_patch_interaction": ("y", "y_bf16", "y_stats"),
+    "gemm_act": ("out_f32", "out_bf16", "stats_out"),
+    "conv_im2col_nhwc": ("out_bf16",),
+    "attention_window": ("out",),
+    "attention_window_relpos": ("out",),
+    "attention_kv": ("out",),
+    "attention_groups": ("out",),
+    "conv_proj_dw": ("q_out", "kv_out"),
 }
+# the entry points of the attention records on token grids (engine.Windows, StridedKV, ConvProj, PatchGroups) and of
+# the SiLU feed-forward block, which make_engine_schedule.ENTRY_POINTS does not list
+GRID_ENTRY_POINTS = ("gemm_act", "conv_im2col_nhwc", "attention_window", "attention_window_relpos", "attention_kv",
+                     "attention_groups", "conv_proj_dw")
 
 
 def schedule():
@@ -137,7 +150,8 @@ def trace(eng, x: Tensor, kw: dict, ln_mode: str, impl=real_impl, prime: Optiona
     kw['primed'], prime(x, xb, stats) first writes the workspace's bf16 copy of x and its row statistics (not traced),
     as an embedding kernel would; every other workspace buffer starts as NaN."""
     S = schedule()
-    with S.recording(eng, S.caller_buffers(eng, x, kw), ln_mode, "python", recorder=tracer(impl)) as rec:
+    with S.recording(eng, S.caller_buffers(eng, x, kw), ln_mode, "python", extra_entry_points=GRID_ENTRY_POINTS,
+                     recorder=tracer(impl)) as rec:
         for buf in eng.workspace(x.shape[0], x.device).values():      # a launch reading a stale buffer reads NaN
             buf.fill_(math.nan)
         if kw.get("primed"):
@@ -224,6 +238,44 @@ def expected(name: str, a: dict, got: dict, on_output: Optional[Callable] = None
         ref[:, :nh * dh], bnd[:, :nh * dh] = r.reshape(M, -1), b.reshape(M, -1)
         put("out_bf16", (ref, bnd))
         return out
+    if name == "gemm_act":
+        kw = dict(bias=a["bias"], ln_sums=a["ln_sums"], col_s=a["col_s"], ln_eps=f32(a["ln_eps"]))
+        if a["act"] == "gelu":
+            y, e = Bd.gemm_reference(a["a"], a["w"], gelu=True, **kw)
+        else:
+            y, e = GB.silu_bound(*Bd.gemm_reference(a["a"], a["w"], **kw))
+        if a["out_f32"] is not None:
+            put("out_f32", (y, e))
+            if a["out_bf16"] is not None:
+                put("out_bf16", _exact(got["out_f32"].bfloat16()))
+        elif a["out_bf16"] is not None:
+            put("out_bf16", (y, Bd.bf16_bound(y, e)))
+        if a["stats_out"] is not None:
+            put("stats_out", _stats(got["out_bf16"], a["stats_out"]))
+        return out
+    if name == "conv_im2col_nhwc":
+        col = GB.im2col_reference(a["x"], a["B"], a["H"], a["W"], a["k"], a["s"], a["p"])
+        put("out_bf16", _exact(torch.nn.functional.pad(col, (0, a["out_bf16"].shape[1] - col.shape[1]))))
+        return out
+    if name == "attention_window":
+        put("out", GB.window_reference(a["qkv"], a["B"], a["gh"], a["gw"], a["p"], a["H"], a["dh"], f32(a["scale"])))
+        return out
+    if name == "attention_window_relpos":
+        put("out", GB.relpos_reference(a["qkv"], a["table"], a["B"], a["gh"], a["gw"], a["w"], a["grid"], a["H"],
+                                       a["dh"], a["scale"]))
+        return out
+    if name == "attention_kv":
+        put("out", GB.kv_reference(a["q"], a["kv"], a["B"], a["Nq"], a["Nk"], a["H"], a["dh"], f32(a["scale"])))
+        return out
+    if name == "attention_groups":
+        put("out", GB.groups_reference(a["qkv"], a["B"], a["gh"], a["gw"], a["ph"], a["pw"], a["H"], a["dh"],
+                                       f32(a["scale"])))
+        return out
+    if name == "conv_proj_dw":
+        geo = (a["B"], a["h"], a["w"], a["k"])
+        put("q_out", GB.conv_reference(a["x"], a["wq"], a["bq"], *geo, 1))
+        put("kv_out", GB.conv_reference(a["x"], a["wkv"], a["bkv"], *geo, a["s"]))
+        return out
     if name == "layernorm":
         kw = dict(row_index=a["row_index"], eps=f32(a["eps"]))
         if a["out_f32"] is not None:
@@ -276,6 +328,10 @@ def launch_kind(c: Launch) -> str:
         return f"gemm {what}{' gelu' if a['gelu'] else ''}"
     if c.name == "gemm_headnorm":
         return "gemm_headnorm " + ("ln" if c.args["head_layernorm_eps"] is not None else "rms")
+    if c.name == "gemm_act":
+        return f"gemm_act {'ln-fold ' if c.args['ln_sums'] is not None else ''}{c.args['act']}"
+    if c.name == "attention_window_relpos":
+        return f"attention_window_relpos {'dilated' if c.args['grid'] else 'block'}"
     return c.name
 
 
@@ -347,6 +403,8 @@ class RefLayer:
     lpi: Optional[dict] = None                               # ln, conv1, bn, conv2, scale
     post_norm: bool = False
     cat: Tuple[str, ...] = ()                                # fields the engine gets as a concatenation, not `is`
+    grid: Optional[dict] = None                              # the attention on the token grid, by `kind` (_grid_*)
+    ff_act: str = "gelu"                                     # the feed-forward block's activation
 
 
 def _plain(attn, ff, qkv_w: Optional[Tensor] = None, scale: Optional[float] = None, **kw) -> RefLayer:
@@ -360,11 +418,69 @@ def _plain(attn, ff, qkv_w: Optional[Tensor] = None, scale: Optional[float] = No
                     scale=float(attn.scale) if scale is None else scale, **kw)
 
 
+def _chan_ln(m: nn.Module) -> Ln:
+    """The channel LayerNorm of an NCHW map (twins_svt.py:33-43, cvt.py:25-35): g and b of shape (1, dim, 1, 1)."""
+    return Ln(m.g.reshape(-1), m.b.reshape(-1), m.eps)
+
+
+def _conv_layer(attn: nn.Module, ff: nn.Sequential, qkv_w: Tensor, grid: dict, cat=()) -> RefLayer:
+    """A layer of 1 x 1 convolutions over an NCHW map: `attn` (norm, to_out[0], heads, scale) and `ff` (channel
+    LayerNorm, Conv2d, GELU, Dropout, Conv2d) (twins_svt.py:45-57, cvt.py:37-49)."""
+    o, c1, c2 = attn.to_out[0], ff[1], ff[4]
+    I, D = o.weight.shape[1], o.weight.shape[0]
+    return RefLayer(ln1=_chan_ln(attn.norm), qkv_w=qkv_w, out=(o.weight.reshape(D, I), o.bias), ln2=_chan_ln(ff[0]),
+                    fc1=(c1.weight.reshape(-1, D), c1.bias), fc2=(c2.weight.reshape(D, -1), c2.bias),
+                    heads=attn.heads, dim_head=I // attn.heads, scale=float(attn.scale), grid=grid, cat=cat)
+
+
 def module_layers(mod: nn.Module) -> List[RefLayer]:
     """The layers of a reference Transformer, by family (the module's class)."""
-    from vit_pytorch_b200 import (cait, cct, deepvit, na_vit, na_vit_nested_tensor, simple_vit_with_qk_norm, vit,
-                                  vit_for_small_dataset, vit_nd_rotary, vivit, xcit)
+    from vit_pytorch_b200 import (cait, cct, crossformer, cvt, deepvit, max_vit, mobile_vit, na_vit,
+                                  na_vit_nested_tensor, simple_vit_with_qk_norm, twins_svt, vit, vit_for_small_dataset,
+                                  vit_nd_rotary, vivit, xcit)
     t = type(mod)
+    if t is twins_svt.Transformer:                                          # twins_svt.py:159-176
+        out = []
+        for local_attn, ff1, global_attn, ff2 in mod.layers:
+            if not isinstance(local_attn, nn.Identity):                     # LocalAttention, twins_svt.py:85-120
+                a = local_attn.fn
+                I, D = a.to_q.weight.shape[:2]
+                out.append(_conv_layer(a, ff1.fn.net, torch.cat([a.to_q.weight, a.to_kv.weight]).reshape(3 * I, D),
+                                       dict(kind="window", size=a.patch_size), cat=("qkv_w",)))
+            a = global_attn.fn                                              # GlobalAttention, twins_svt.py:122-157
+            I, D = a.to_q.weight.shape[:2]
+            out.append(_conv_layer(a, ff2.fn.net, a.to_q.weight.reshape(I, D), dict(kind="strided", conv=a.to_kv)))
+        return out
+    if issubclass(t, max_vit._BlockAttention):                              # max_vit.py:262-273: block[2:4], [6:8]
+        out = []
+        for ai, fi, dilated in ((2, 3, False), (6, 7, True)):
+            a, ff = mod.block[ai].fn, mod.block[fi].fn
+            out.append(_plain(a, ff, grid=dict(kind="relpos", module=a, size=a.window_size, dilated=dilated,
+                                               windows=mod.block[ai - 1])))
+        return out
+    if t is crossformer.Transformer:                                        # crossformer.py:167-199
+        out = []
+        for step in mod.layers:
+            for a, ff in ((step[0], step[1]), (step[2], step[3])):         # Attention crossformer.py:101-165
+                I, D = a.to_qkv.out_channels // 3, a.to_qkv.in_channels
+                o, c1, c2 = a.to_out, ff[1], ff[4]
+                out.append(RefLayer(
+                    ln1=_chan_ln(a.norm), qkv_w=a.to_qkv.weight.reshape(3 * I, D),
+                    out=(o.weight.reshape(D, I), o.bias), ln2=_chan_ln(ff[0]), fc1=(c1.weight.reshape(-1, D), c1.bias),
+                    fc2=(c2.weight.reshape(D, -1), c2.bias), heads=a.heads, dim_head=I // a.heads, scale=float(a.scale),
+                    grid=dict(kind="relpos", module=a, size=a.window_size, dilated=a.attn_type == "long", dpb=True)))
+        return out
+    if t is cvt.Transformer:                                                # cvt.py:99-112, Attention cvt.py:62-97
+        out = []
+        for a, ff in mod.layers:
+            pq, pkv = a.to_q.net[2], a.to_kv.net[2]
+            I, D = pq.weight.shape[:2]
+            out.append(_conv_layer(a, ff.net, pq.weight.reshape(I, D),
+                                   dict(kind="convproj", q=a.to_q.net, kv=a.to_kv.net,
+                                        kv_w=pkv.weight.reshape(2 * I, D))))
+        return out
+    if t is mobile_vit.Transformer:                                         # mobile_vit.py:79-96, FeedForward :28-34
+        return [dataclasses.replace(_plain(a, ff, grid=dict(kind="groups")), ff_act="silu") for a, ff in mod.layers]
     if t is vit.Transformer:                                                # vit.py:66-83
         return [_plain(attn, ff) for attn, ff in mod.layers]
     if t is vit_nd_rotary.Transformer:                                      # vit_nd_rotary.py:115-156: to_qk | to_v
@@ -441,10 +557,17 @@ def module_layers(mod: nn.Module) -> List[RefLayer]:
     raise NotImplementedError(f"no reference layer table for {t.__module__}.{t.__name__}")
 
 
+def _aliases(got: Tensor, want: Tensor) -> bool:
+    """got views the same elements of the same storage as want (a reshape of the parameter, not a copy of it)."""
+    return (got.untyped_storage().data_ptr() == want.untyped_storage().data_ptr()
+            and got.storage_offset() == want.storage_offset() and got.stride() == want.stride())
+
+
 def check_identity(mod: nn.Module, case: str = "") -> None:
-    """Each EncoderLayer field the module describes to the engine IS the reference module's parameter (`is`; equal
-    values for the concatenations), so a swapped LayerNorm or a wrong layer index cannot hide behind a
-    self-consistent description."""
+    """Each EncoderLayer field the module describes to the engine IS the reference module's parameter (`is`, or a view
+    of the same elements of its storage: the reshaped 1 x 1 convolutions and channel LayerNorms; equal values for the
+    concatenations), so a swapped LayerNorm or a wrong layer index cannot hide behind a self-consistent
+    description."""
     layers, _ = mod.encoder_layers()
     refs = module_layers(mod)
     if len(layers) != len(refs):
@@ -453,8 +576,8 @@ def check_identity(mod: nn.Module, case: str = "") -> None:
     def same(i, what, got, want, cat=False):
         if got is None and want is None:
             return
-        ok = got is want or (cat and got is not None and want is not None and got.shape == want.shape
-                             and torch.equal(got, want))
+        ok = got is want or (got is not None and want is not None and got.shape == want.shape
+                             and (cat or _aliases(got, want)) and torch.equal(got, want))
         if not ok:
             raise AssertionError(f"{case}: layer {i}: EncoderLayer.{what} is not the module's parameter")
 
@@ -527,6 +650,57 @@ def _lpi_folded(P: dict, k: int):
             (w2, U * w2.abs()), (b2, U * b2.abs())]
 
 
+def dpb_table_reference(attn: nn.Module) -> Tuple[Tensor, Tensor]:
+    """(table, bound) fp64 [(2w-1)^2, heads] of CrossFormer's relative-position table (crossformer.py:195-215): the
+    module's DynamicPositionBias evaluated in fp64 at the (2w+1)^2 offsets of _rel_offsets, the outputs that its
+    rel_pos_indices (stride 2w-1) address -- the first (2w-1)^2 -- shared by the heads.  The bound is the error of the
+    host's fp32 evaluation, carried layer by layer as a per-element bound e on the fp64 values v:
+      Linear (K inputs)   e' = |W| e + (K + 2) u (|W| |v| + |b|)   (any order of the K fp32 products and sums);
+      LayerNorm (D)       xhat = (v - mean) / sigma moves under a perturbation d of v by
+                          (d_j - mean(d) - xhat_j mean(xhat d)) / sigma to first order (sigma = sqrt(var + eps) of the
+                          fp64 input), so e' = |g| 1.01 (e + mean(e) + |xhat| mean(|xhat| e)) / sigma, the 1.01 for the
+                          higher orders (e / sigma stays below 1e-4 here), plus (D + 8) u |g| (1 + |xhat|) + 2 u |v'|
+                          for the mean, the variance's D-term sums, rsqrt and the products;
+      ReLU                e' = e (1-Lipschitz, exact), 0 where v + e < 0 (both evaluations give exactly 0)."""
+    from vit_pytorch_b200.crossformer import _rel_offsets
+    w = attn.window_size
+    d = lambda t: t.detach().double()                                                   # noqa: E731
+    v = _rel_offsets(w, attn.rel_pos_indices.device).double()
+    e = torch.zeros_like(v)
+    for m in attn.dpb:
+        if isinstance(m, nn.Linear):
+            W, b = d(m.weight), d(m.bias)
+            v, e = v @ W.t() + b, e @ W.abs().t() + (W.shape[1] + 2) * U * (v.abs() @ W.abs().t() + b.abs())
+        elif isinstance(m, nn.LayerNorm):
+            mu, var = v.mean(-1, keepdim=True), v.var(-1, unbiased=False, keepdim=True)
+            sig = torch.sqrt(var + m.eps)
+            xh = (v - mu) / sig
+            v = xh * d(m.weight) + d(m.bias)
+            g = d(m.weight).abs()
+            dx = (e + e.mean(-1, keepdim=True) + xh.abs() * (xh.abs() * e).mean(-1, keepdim=True)) / sig
+            e = g * 1.01 * dx + (v.shape[-1] + 8) * U * g * (1 + xh.abs()) + 2 * U * v.abs()
+        elif isinstance(m, nn.ReLU):
+            v, e = v.clamp_min(0), torch.where(v + e < 0, torch.zeros_like(e), e)
+        else:
+            v, e = m(v), m(e)
+    n = (2 * w - 1) ** 2
+    return v[:n, None].expand(-1, attn.heads), e[:n, None].expand(-1, attn.heads)
+
+
+def _bn_folded(conv: nn.Conv2d, bn: nn.BatchNorm2d):
+    """((w, bound), (b, bound)) fp64 of a bias-free depthwise convolution with the BatchNorm (eval) after it folded in,
+    tap-major [k k, C] (cvt.py:51-60): w' = w g / sqrt(var + eps), b' = beta - mean g / sqrt(var + eps), recomputed
+    from the module's parameters and its eps; the bound is the fp32 rounding the host's fold may add: 5 u for w'
+    (the sum, sqrt, quotient and product), 5 u |mean inv| + u (|b'| + |beta|) for b'."""
+    d = lambda t: t.detach().double()                                                   # noqa: E731
+    C = conv.weight.shape[0]
+    inv = d(bn.weight) / torch.sqrt(d(bn.running_var) + f32(bn.eps))
+    w = (d(conv.weight).reshape(C, -1) * inv[:, None]).t()
+    mi = d(bn.running_mean) * inv
+    b = d(bn.bias) - mi
+    return (w, 5 * U * w.abs()), (b, 5 * U * mi.abs() + U * (b.abs() + d(bn.bias).abs()))
+
+
 class ProvenanceError(AssertionError):
     pass
 
@@ -593,9 +767,10 @@ class Walk:
 
     # ---------------------------------------------------------------- steps
     def normed(self, S: Tensor, ln: Ln, W: Tensor, b: Optional[Tensor], gelu: bool = False,
-               head: Optional[tuple] = None, heads: int = 0, dh: int = 0) -> Tensor:
-        """out = LN(S) W^T + b (reference vit.py:19-21 / :52-54): the bf16 output of its GEMM."""
-        gemm = "gemm_headnorm" if head is not None else "gemm"
+               head: Optional[tuple] = None, heads: int = 0, dh: int = 0, act: Optional[str] = None) -> Tensor:
+        """out = LN(S) W^T + b (reference vit.py:19-21 / :52-54): the bf16 output of its GEMM; `act` "silu": the
+        activation of gemm_act (MobileViT's FeedForward, mobile_vit.py:28-34)."""
+        gemm = "gemm_headnorm" if head is not None else "gemm_act" if act is not None else "gemm"
         d = lambda t: t.detach().double()                                               # noqa: E731
         if self.fold:
             if not self.have_stats:
@@ -635,7 +810,11 @@ class Walk:
             self.same("w", a["w"], W.detach().bfloat16())
             self.same("bias", a["bias"], None if b is None else b.detach().float())
             self.same("ln_sums", a["ln_sums"], None)
-        if head is None:
+        if act is not None:
+            self.value("act", a["act"], act)
+            self.same("out_f32", a["out_f32"], None)
+            self.same("stats_out", a["stats_out"], None)
+        elif head is None:
             self.value("gelu", a["gelu"], gelu)
             self.same("resid", a["resid"], None)
             self.same("out_f32", a["out_f32"], None)
@@ -727,6 +906,132 @@ class Walk:
             self.within("tau (exp temperature)", a["tau"], tau, 4 * U * tau)
         return c.post["out"]
 
+    # ---------------------------------------------------------------- attention on the token grid
+    def exact_ln(self, S: Tensor, ln: Ln) -> Tensor:
+        """bf16(LN(S)) by the exact layernorm, in both modes: the normalised map a convolution reads."""
+        c = self.take("layernorm")
+        a = c.pre
+        self.same("x", a["x"], S)
+        self.same("gamma", a["gamma"], ln.gamma.detach().float())
+        self.same("beta", a["beta"], None if ln.beta is None else ln.beta.detach().float())
+        self.value("eps", a["eps"], float(ln.eps))
+        self.same("row_index", a["row_index"], None)
+        self.same("out_f32", a["out_f32"], None)
+        return c.post["out_bf16"]
+
+    def plain_gemm(self, A: Tensor, W: Tensor) -> Tensor:
+        """A W^T, no bias and no LayerNorm: a bias-free 1 x 1 convolution on a bf16 map."""
+        c = self.take("gemm")
+        a = c.pre
+        self.same("a", a["a"], A)
+        self.same("w", a["w"], W.detach().bfloat16())
+        for op in ("bias", "resid", "ln_sums", "out_f32", "stats_out"):
+            self.same(op, a[op], None)
+        self.value("gelu", a["gelu"], False)
+        return c.post["out_bf16"]
+
+    def grid_geometry(self, a: dict, B: bool = True) -> None:
+        gh, gw = self.kw["grid"]
+        if B:
+            self.value("B", a["B"], self.kw["B"])
+        self.value("gh", a["gh"], gh)
+        self.value("gw", a["gw"], gw)
+
+    def heads(self, a: dict, R: RefLayer) -> None:
+        self.value("H", a["H"], R.heads)
+        self.value("dh", a["dh"], R.dim_head)
+        self.value("scale", a["scale"], float(R.scale))
+
+    def grid_attention(self, R: RefLayer, S: Tensor, i: int) -> Tensor:
+        """The attention output of layer R on the stream S, by the kind of its attention on the grid."""
+        g, kind = R.grid, R.grid["kind"]
+        if kind in ("window", "relpos", "groups"):
+            qkv = self.normed(S, R.ln1, R.qkv_w, None)
+            self.where = f"layer {i} attention"
+            if kind == "window":                            # twins_svt.py:104-116: p x p blocks of the map
+                c = self.take("attention_window")
+                self.value("p", c.pre["p"], g["size"])
+            elif kind == "relpos":                          # max_vit.py:247-272, block or dilated windows
+                c = self.take("attention_window_relpos")
+                self.value("w", c.pre["w"], g["size"])
+                self.value("dilated", c.pre["grid"], g["dilated"])
+                if g.get("dpb"):                            # crossformer.py:195-215: dpb at the offsets, host fp32
+                    ref, bnd = dpb_table_reference(g["module"])
+                    self.within("table (dpb)", c.pre["table"], ref.t(), bnd.t())
+                else:
+                    self.same("table", c.pre["table"], g["module"].rel_pos_bias.weight.detach().float().t())
+            else:                                           # mobile_vit.py:150: strided patch groups
+                c = self.take("attention_groups")
+                ph, pw = self.kw["groups"]
+                self.value("ph", c.pre["ph"], ph)
+                self.value("pw", c.pre["pw"], pw)
+            self.same("qkv", c.pre["qkv"], qkv)
+            self.grid_geometry(c.pre)
+            self.heads(c.pre, R)
+            return c.post["out"]
+        gh, gw = self.kw["grid"]
+        B = self.kw["B"]
+        xn = self.exact_ln(S, R.ln1)
+        if kind == "strided":                               # twins_svt.py:140-157: keys from a k x k, stride-k conv
+            conv = g["conv"]
+            k, s = conv.kernel_size[0], conv.stride[0]
+            self.where = f"layer {i} queries"
+            q = self.plain_gemm(xn, R.qkv_w)
+            col = xn
+            if k > 1:
+                self.where = f"layer {i} key patches"
+                c = self.take("conv_im2col_nhwc")
+                a = c.pre
+                self.same("x", a["x"], xn)
+                self.value("B", a["B"], B)
+                self.value("H", a["H"], gh)
+                self.value("W", a["W"], gw)
+                self.value("k", a["k"], k)
+                self.value("s", a["s"], s)
+                self.value("p", a["p"], conv.padding[0])
+                col = c.post["out_bf16"]
+            self.where = f"layer {i} keys and values"
+            # the Conv2d weight in the im2col column order (tap row, tap column, channel)
+            kv = self.plain_gemm(col, conv.weight.permute(0, 2, 3, 1).reshape(conv.weight.shape[0], -1))
+            kh, kw = (gh + 2 * conv.padding[0] - k) // s + 1, (gw + 2 * conv.padding[1] - k) // s + 1
+        else:                                               # cvt.py:51-60, 74-75: depthwise convs + BatchNorm, 1 x 1
+            dq, bq, _ = g["q"]
+            dkv, bkv, _ = g["kv"]
+            k, s = dq.kernel_size[0], dkv.stride[0]
+            self.where = f"layer {i} convolutional projection"
+            if any(m.bias is not None for m in (dq, dkv, g["q"][2], g["kv"][2])):
+                self.fail("-", "a convolution of the module's projections has a bias, which the fold drops")
+            c = self.take("conv_proj_dw")
+            a = c.pre
+            self.same("x", a["x"], xn)
+            for op, conv, bn in (("q", dq, bq), ("kv", dkv, bkv)):
+                (w, wb), (b, bb) = _bn_folded(conv, bn)
+                self.within(f"w{op} (BatchNorm folded)", a[f"w{op}"], w, wb)
+                self.within(f"b{op} (BatchNorm folded)", a[f"b{op}"], b, bb)
+            self.value("B", a["B"], B)
+            self.value("h", a["h"], gh)
+            self.value("w", a["w"], gw)
+            self.value("k", a["k"], k)
+            self.value("s", a["s"], s)
+            if dq.stride[0] != 1 or dq.padding[0] != k // 2 or dkv.padding[0] != k // 2:
+                self.fail("-", "the module's query convolution is not stride 1, or a padding is not k // 2")
+            aq, akv = c.post["q_out"], c.post["kv_out"]
+            self.where = f"layer {i} queries"
+            q = self.plain_gemm(aq, R.qkv_w)
+            self.where = f"layer {i} keys and values"
+            kv = self.plain_gemm(akv, g["kv_w"])
+            kh, kw = (gh + 2 * dkv.padding[0] - k) // s + 1, (gw + 2 * dkv.padding[1] - k) // s + 1
+        self.where = f"layer {i} attention"
+        c = self.take("attention_kv")
+        a = c.pre
+        self.same("q", a["q"], q)
+        self.same("kv", a["kv"], kv)
+        self.value("B", a["B"], B)
+        self.value("Nq", a["Nq"], gh * gw)
+        self.value("Nk", a["Nk"], kh * kw)
+        self.heads(a, R)
+        return c.post["out"]
+
     def lpi(self, R: RefLayer, S: Tensor) -> Tensor:
         """y = S + LPI(S) (xcit.py:150-167, 208-211)."""
         c = self.take("local_patch_interaction")
@@ -790,6 +1095,16 @@ def check_provenance(mod: nn.Module, x0: Tensor, kw: dict, launches: List[Launch
     for i in (range(len(refs)) if run is None else run):
         R = refs[i]
         w.where = f"layer {i} qkv"
+        if R.grid is not None:
+            o = w.grid_attention(R, S, i)
+            w.where = f"layer {i} out"
+            S = w.residual(o, R.out, R.out_scale, S, copy=True, D=D)
+            w.where = f"layer {i} fc1"
+            act = None if R.ff_act == "gelu" else R.ff_act
+            h = w.normed(S, R.ln2, R.fc1[0], R.fc1[1], gelu=act is None, act=act)
+            w.where = f"layer {i} fc2"
+            S = w.residual(h, R.fc2, R.ff_scale, S, copy=True, D=D)
+            continue
         head = None if R.qk is None else R.qk
         qkv = w.normed(S, R.ln1, R.qkv_w, None, head=head, heads=R.heads, dh=R.dim_head)
         if rope is not None:                                   # vit_nd_rotary.py:143-147

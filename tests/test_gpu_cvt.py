@@ -9,7 +9,8 @@ import torch
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
-from oracle.bounds import bf16_ulp, check
+from oracle.bounds import check
+from oracle.grid_attention_bounds import conv_reference
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -19,7 +20,6 @@ from cvt_spec import CVT_CASES, FAMILY  # noqa: E402
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 NAN = float("nan")
-F = torch.nn.functional
 
 
 # ================================================================================================ conv_proj_dw
@@ -41,19 +41,6 @@ def run_conv_proj(x, wq, bq, wkv, bkv, B, h, w, k, s, pad_rows=3):
     _lib.conv_proj_dw(x, wq, bq, wkv, bkv, q, kv, B, h, w, k, s)
     torch.cuda.synchronize()
     return q, kv, bq_buf, bkv_buf
-
-
-def conv_reference(x, wt, b, B, h, w, k, s):
-    """fp64 (ref, bound): the depthwise convolution on the kernel's own bf16 input, bounded by half a bf16 ulp of the
-    fp64 value plus the fp32 accumulation of k*k products and the bias, about k^2 2^-23 sum |w x| + |b|."""
-    C = x.shape[1]
-    xi = x.double().reshape(B, h, w, C).permute(0, 3, 1, 2)
-    wd = wt.double().t().reshape(C, 1, k, k)
-    ref = F.conv2d(xi, wd, b.double(), stride=s, padding=k // 2, groups=C)
-    mag = F.conv2d(xi.abs(), wd.abs(), b.double().abs(), stride=s, padding=k // 2, groups=C)
-    ref, mag = (t.permute(0, 2, 3, 1).reshape(-1, C) for t in (ref, mag))
-    e = (k * k + 1) * 2.0 ** -23 * mag
-    return ref, e + bf16_ulp(ref.abs() + e) / 2
 
 
 @pytest.mark.parametrize("B,h,w,C,k,s", [(2, 56, 56, 64, 3, 2), (3, 25, 19, 64, 3, 2), (2, 7, 5, 384, 3, 2),

@@ -93,8 +93,13 @@ def make(name, seed=0):
     """The case's module on the GPU (fp32 parameters): default init moved by noise so that LayerNorm gains and shifts,
     LayerScales and temperatures are not their constants, LayerNorm eps as test_layer_trace.set_eps sets them, BatchNorm
     running statistics away from (0, 1)."""
+    return perturbed(CASES[name][0], seed)
+
+
+def perturbed(module, seed=0):
+    """module() as make() initialises it."""
     torch.manual_seed(seed)
-    mod = CASES[name][0]().eval()
+    mod = module().eval()
     with torch.no_grad():
         for p in mod.parameters():
             p.add_(0.05 * torch.randn_like(p))

@@ -11,6 +11,7 @@ import torch
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
 from oracle.bounds import C_ACC, U, bf16_ulp, check
+from oracle.grid_attention_bounds import relpos_reference, window_rows
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -24,42 +25,6 @@ WIDTHS = (32, 64, 80, 128)
 
 
 # ================================================================================================ window attention
-def window_rows(B, gh, gw, w, grid):
-    """[windows, w*w] map rows of every window, local token r = u*w + v (the kernel's address map)."""
-    X, Y = gh // w, gw // w
-    b, i, j, u, v = torch.meshgrid(*(torch.arange(n, device=DEV) for n in (B, X, Y, w, w)), indexing="ij")
-    y = u * X + i if grid else i * w + u
-    x = v * Y + j if grid else j * w + v
-    return ((b * gh + y) * gw + x).reshape(B * X * Y, w * w)
-
-
-def relpos_reference(qkv, table, B, gh, gw, w, grid, H, dh, scale):
-    """fp64 (ref, bound) of b200vit_attention_window_relpos on the kernel's own bf16 inputs, bounded as the
-    position-bias attention of test_gpu_levit.py: the bf16 probabilities before P V, the fp32 scores and the rounding
-    of the scale and the bias, fp32 accumulation, the output's bf16 rounding."""
-    rows = window_rows(B, gh, gw, w, grid)
-    x = qkv.double()[rows]                                                   # windows, n, 3 H dh
-    n = w * w
-    q, k, v = (x[..., s * H * dh:(s + 1) * H * dh].reshape(-1, n, H, dh).transpose(1, 2) for s in range(3))
-    r = torch.arange(n, device=DEV)
-    u, vv = r // w, r % w
-    idx = (u[:, None] - u[None, :] + w - 1) * (2 * w - 1) + (vv[:, None] - vv[None, :] + w - 1)
-    bias = table.double()[:, idx]                                            # H, n, n
-    sc = float(torch.tensor(scale, dtype=torch.float32))
-    logits = sc * q @ k.transpose(-1, -2) + bias
-    p = logits.softmax(-1)
-    out = p @ v
-    mag = p @ v.abs()
-    dx = (C_ACC * dh + 4) * U * sc * (q.abs() @ k.abs().transpose(-1, -2)) + 4 * U * (bias.abs() + logits.abs())
-    e = (2.0 ** -8 + 4 * dx.amax(-1, keepdim=True) + (C_ACC * n + n / 4 + 16) * U) * mag + 3 * U * out.abs()
-    bound = e + bf16_ulp(out.abs() + e) / 2
-    ref = torch.zeros(B * gh * gw, H * dh, device=DEV, dtype=torch.float64)
-    bnd = torch.zeros_like(ref)
-    ref[rows.reshape(-1)] = out.transpose(1, 2).reshape(-1, H * dh)
-    bnd[rows.reshape(-1)] = bound.transpose(1, 2).reshape(-1, H * dh)
-    return ref, bnd
-
-
 def make_inputs(B, gh, gw, w, H, dh, seed, pad_rows=3):
     """qkv bf16 [B*gh*gw, 3 H dh] as the head of a buffer whose rows past it are NaN (never to be read), and a bias
     table [H, (2w-1)^2]."""
@@ -98,7 +63,7 @@ def test_relpos_keeps_a_nan_inside_its_window(grid):
     B, gh, gw, w, H, dh = 2, 14, 21, 7, 2, 32
     qkv, table = make_inputs(B, gh, gw, w, H, dh, seed=11)
     _, clean = run_relpos(qkv, table, B, gh, gw, w, grid, H, dh)
-    rows = window_rows(B, gh, gw, w, grid)
+    rows = window_rows(B, gh, gw, w, w, DEV, dilated=grid)
     tok = int(rows[5, 10])
     inside = torch.zeros(B * gh * gw, dtype=torch.bool, device=DEV)
     inside[rows[5]] = True

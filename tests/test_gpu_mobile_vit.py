@@ -12,8 +12,8 @@ import torch
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
-from oracle.attention_bounds import attention_reference
 from oracle.bounds import U, bf16_bound, bf16_ulp, check, gemm_inputs, gemm_reference, stats_reference
+from oracle.grid_attention_bounds import group_rows, groups_reference, silu_bound
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -29,25 +29,6 @@ SCALE = DH ** -0.5
 
 
 # ================================================================================================ group attention
-def group_rows(B, gh, gw, ph, pw):
-    """[B*ph*pw, n] map rows of every group, group (b, i, j) in that order, token t = y'*(gw/pw) + x'."""
-    hh, ww = gh // ph, gw // pw
-    b, i, j, y, x = torch.meshgrid(*(torch.arange(n, device=DEV) for n in (B, ph, pw, hh, ww)), indexing="ij")
-    return ((b * gh + y * ph + i) * gw + x * pw + j).reshape(B * ph * pw, hh * ww)
-
-
-def groups_reference(qkv, B, gh, gw, ph, pw, H):
-    rows = group_rows(B, gh, gw, ph, pw)
-    G, n = rows.shape
-    x = qkv[rows.reshape(-1)].view(G, n, 3, H, DH).permute(2, 0, 3, 1, 4).reshape(3, G * H, n, DH)
-    r, b = attention_reference(x[0], x[1], x[2], SCALE, kb=64)
-    ref = torch.empty(B * gh * gw, H * DH, dtype=torch.float64, device=DEV)
-    bnd = torch.empty_like(ref)
-    ref[rows.reshape(-1)] = r.view(G, H, n, DH).permute(0, 2, 1, 3).reshape(-1, H * DH)
-    bnd[rows.reshape(-1)] = b.view(G, H, n, DH).permute(0, 2, 1, 3).reshape(-1, H * DH)
-    return ref, bnd
-
-
 PAD = 5          # poisoned rows before and after the addressed ones
 
 
@@ -82,7 +63,7 @@ def test_attention_groups_within_bounds_and_repeatable(B, gh, gw, ph, pw, H):
     qkv = (torch.randn(B * gh * gw, 3 * H * DH, device=DEV, generator=g) * 1.5).bfloat16()
     out = run_groups(qkv, B, gh, gw, ph, pw, H)
     assert torch.isfinite(out).all()
-    ref, bnd = groups_reference(qkv, B, gh, gw, ph, pw, H)
+    ref, bnd = groups_reference(qkv, B, gh, gw, ph, pw, H, DH, SCALE)
     check(out, ref, bnd, f"groups {B}x{gh}x{gw} patch {ph}x{pw} H={H}")
     assert torch.equal(run_groups(qkv, B, gh, gw, ph, pw, H), out)
 
@@ -101,7 +82,7 @@ def test_attention_groups_keeps_nan_and_inf_inside_the_group(bad):
     else:
         dirty[row, H * DH + 2 * DH + 1] = float("inf")    # head 2's key
     out = run_groups(dirty, B, gh, gw, ph, pw, H)
-    rows = group_rows(B, gh, gw, ph, pw)
+    rows = group_rows(B, gh, gw, ph, pw, DEV)
     inside = torch.zeros(B * gh * gw, dtype=torch.bool, device=DEV)
     inside[rows[(1 * ph + 1) * pw + 1]] = True
     same = (out == clean) | (torch.isnan(out) & torch.isnan(clean))
@@ -156,11 +137,6 @@ def test_dwconv_ex_gelu_gives_the_bits_of_mbconv_dwconv(stride):
 
 
 # ================================================================================================ SiLU GEMM epilogue
-def silu_bound(y, e_y):
-    ref = y * torch.sigmoid(y)
-    return ref, 1.1 * e_y + 8 * U * ref.abs() + 4 * U * y.abs() + 1e-30
-
-
 @pytest.mark.parametrize("M,N,K", [(4096, 192, 96), (3000, 480, 120), (8192, 576, 144)])
 def test_silu_with_ln_fold_against_bounds(M, N, K):
     d = gemm_inputs(M, N, K, parts=2, seed=M + N, device=DEV)

@@ -11,7 +11,8 @@ import torch
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
-from oracle.bounds import C_ACC, U, bf16_ulp, check
+from oracle.bounds import check
+from oracle.grid_attention_bounds import region_local_reference, region_window_rows
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -27,43 +28,6 @@ DH = 32
 
 
 # ======================================================================================= region-to-local attention
-def window_rows(B, lh, lw, rh, rw):
-    """[B*rh*rw, 1 + wh*ww] stream rows of every window in (b, i, j) order: the region row, then local (u, v)."""
-    wh, ww = lh // rh, lw // rw
-    b, i, j, u, v = torch.meshgrid(*(torch.arange(n, device=DEV) for n in (B, rh, rw, wh, ww)), indexing="ij")
-    local = ((b * lh + i * wh + u) * lw + j * ww + v).reshape(B * rh * rw, wh * ww)
-    region = B * lh * lw + torch.arange(B * rh * rw, device=DEV)
-    return torch.cat((region[:, None], local), 1)
-
-
-def region_local_reference(qkv, table, B, lh, lw, rh, rw, W, H, scale):
-    """fp64 (ref, bound) of b200vit_attention_region_local on the kernel's own bf16 inputs, bounded as the
-    relative-position window attention of test_gpu_max_vit.py."""
-    rows = window_rows(B, lh, lw, rh, rw)
-    wh, ww = lh // rh, lw // rw
-    n = rows.shape[1]
-    x = qkv.double()[rows]                                                   # windows, n, 3 H dh
-    q, k, v = (x[..., s * H * DH:(s + 1) * H * DH].reshape(-1, n, H, DH).transpose(1, 2) for s in range(3))
-    t = torch.arange(n - 1, device=DEV)
-    u, vv = t // ww, t % ww
-    idx = (u[:, None] - u[None, :] + W - 1) + (vv[:, None] - vv[None, :] + W - 1) * (2 * W - 1)
-    bias = torch.zeros(H, n, n, dtype=torch.float64, device=DEV)
-    bias[:, 1:, 1:] = table.double()[:, idx]
-    sc = float(torch.tensor(scale, dtype=torch.float32))
-    logits = sc * q @ k.transpose(-1, -2) + bias
-    p = logits.softmax(-1)
-    out = p @ v
-    mag = p @ v.abs()
-    dx = (C_ACC * DH + 4) * U * sc * (q.abs() @ k.abs().transpose(-1, -2)) + 4 * U * (bias.abs() + logits.abs())
-    e = (2.0 ** -8 + 4 * dx.amax(-1, keepdim=True) + (C_ACC * n + n / 4 + 16) * U) * mag + 3 * U * out.abs()
-    bound = e + bf16_ulp(out.abs() + e) / 2
-    ref = torch.zeros(qkv.shape[0], H * DH, device=DEV, dtype=torch.float64)
-    bnd = torch.zeros_like(ref)
-    ref[rows.reshape(-1)] = out.transpose(1, 2).reshape(-1, H * DH)
-    bnd[rows.reshape(-1)] = bound.transpose(1, 2).reshape(-1, H * DH)
-    return ref, bnd
-
-
 def run_region_local(qkv, table, B, lh, lw, rh, rw, W, H):
     """The kernel between NaN rows of qkv, writing between NaN rows of out; asserts the padding kept."""
     M = qkv.shape[0]
@@ -112,7 +76,7 @@ def test_attention_region_local_keeps_nan_and_inf_inside_the_window(bad):
     B, lh, lw, rh, rw, W, H = 2, 28, 28, 2, 2, 14, 2
     qkv, table = make_inputs(B, lh, lw, rh, rw, W, H, seed=3)
     clean = run_region_local(qkv, table, B, lh, lw, rh, rw, W, H)
-    rows = window_rows(B, lh, lw, rh, rw)
+    rows = region_window_rows(B, lh, lw, rh, rw, DEV)
     win = 1 * 4 + 1 * 2 + 0                               # window (b=1, i=1, j=0)
     dirty = qkv.clone()
     I = H * DH

@@ -13,8 +13,8 @@ import torch
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR, load_golden
-from oracle.attention_bounds import attention_reference
-from oracle.bounds import U, bf16_ulp, check
+from oracle.bounds import check
+from oracle.grid_attention_bounds import iwsa_reference, kv_ex_reference, window_rows
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -33,50 +33,6 @@ FALLBACK = {"fallback_value48"}
 def seeded(shape, seed, scale=1.0):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(shape, generator=g) * scale).to(**BF)
-
-
-def attention_ex_reference(q, k, v, scale):
-    """(ref, bound) [G, n, dv] of attention_reference for key heads dk and value heads dv wide: both padded with zero
-    columns to max(dk, dv) (zero q / k columns add exactly 0 to every score, the bound's score term grows with the
-    width), the zero value columns dropped again."""
-    dk, dv = q.shape[-1], v.shape[-1]
-    W = max(dk, dv)
-    pad = lambda t: torch.nn.functional.pad(t, (0, W - t.shape[-1]))     # noqa: E731
-    ref, bound = attention_reference(pad(q), pad(k), pad(v), scale, kb=64)
-    return ref[..., :dv], bound[..., :dv]
-
-
-def with_added(ref, bound, lim):
-    """(ref, bound) of bf16(fma(O, 1 / l, lim)) from attention_reference's (ref, bound) of bf16(O / l): its fp32 error
-    is at most bound - ulp(|ref|) / 2 (the rounding term it adds is at least that), plus the fma's rounding."""
-    e32 = (bound - 0.5 * bf16_ulp(ref.abs())).clamp_min(0)
-    tot = ref + lim.double()
-    e = e32 + U * (tot.abs() + e32)
-    return tot, e + 0.5 * bf16_ulp(tot.abs() + e)
-
-
-def window_rows(B, gh, gw, wh, ww):
-    """[B*nw, wh*ww] map rows of every window, windows in (b, wy, wx) order, tokens (u, v) inside."""
-    b, wy, wx, u, v = torch.meshgrid(torch.arange(B, device=DEV), torch.arange(gh // wh, device=DEV),
-                                     torch.arange(gw // ww, device=DEV), torch.arange(wh, device=DEV),
-                                     torch.arange(ww, device=DEV), indexing="ij")
-    return ((b * gh + wy * wh + u) * gw + wx * ww + v).reshape(-1, wh * ww)
-
-
-def iwsa_reference(qkv, lim, B, gh, gw, wh, ww, H, dk, dv, scale):
-    rows = window_rows(B, gh, gw, wh, ww)
-    G, n = rows.shape
-    x = qkv[rows.reshape(-1)].view(G, n, -1)
-    q = x[..., :H * dk].reshape(G, n, H, dk).transpose(1, 2).reshape(G * H, n, dk)
-    k = x[..., H * dk:2 * H * dk].reshape(G, n, H, dk).transpose(1, 2).reshape(G * H, n, dk)
-    v = x[..., 2 * H * dk:2 * H * dk + H * dv].reshape(G, n, H, dv).transpose(1, 2).reshape(G * H, n, dv)
-    r, b = attention_ex_reference(q, k, v, scale)
-    r = r.view(G, H, n, dv).transpose(1, 2).reshape(G * n, H * dv)
-    b = b.view(G, H, n, dv).transpose(1, 2).reshape(G * n, H * dv)
-    ref = torch.empty(B * gh * gw, H * dv, dtype=torch.float64, device=DEV)
-    bnd = torch.empty_like(ref)
-    ref[rows.reshape(-1)], bnd[rows.reshape(-1)] = r, b
-    return with_added(ref, bnd, lim)
 
 
 def iwsa_inputs(B, gh, gw, H, dk, dv, seed):
@@ -120,28 +76,6 @@ def test_iwsa_every_width_pair(dk, dv):
     check(out, ref, bound, f"attention_iwsa dk{dk} dv{dv}")
 
 
-def kv_rows_reference(q, k, v, scale):
-    """(ref, bound) [Nq, dv] of Nq queries against one set of Nk keys: attention_reference takes sequences with as many
-    queries as keys and bounds every query row on its own, so the queries go in as ceil(Nq / Nk) sequences of Nk rows
-    (the last one filled with repeats of the last query) over the same keys."""
-    Nq, Nk = q.shape[0], k.shape[0]
-    c = -(-Nq // Nk)
-    qq = q[torch.arange(c * Nk, device=q.device).clamp_max(Nq - 1)].view(c, Nk, -1)
-    r, b = attention_ex_reference(qq, k[None].expand(c, -1, -1).contiguous(), v[None].expand(c, -1, -1).contiguous(),
-                                  scale)
-    return r.reshape(c * Nk, -1)[:Nq], b.reshape(c * Nk, -1)[:Nq]
-
-
-def kv_reference(q, kv, B, Nq, Nk, H, dk, dv, scale):
-    qh = q.view(B, Nq, H, dk).transpose(1, 2).reshape(B * H, Nq, dk)
-    kh = kv[:, :H * dk].reshape(B, Nk, H, dk).transpose(1, 2).reshape(B * H, Nk, dk)
-    vh = kv[:, H * dk:].reshape(B, Nk, H, dv).transpose(1, 2).reshape(B * H, Nk, dv)
-    outs, bounds = zip(*(kv_rows_reference(qh[g], kh[g], vh[g], scale) for g in range(B * H)))
-    ref = torch.stack(outs).view(B, H, Nq, dv).transpose(1, 2).reshape(B * Nq, H * dv)
-    bnd = torch.stack(bounds).view(B, H, Nq, dv).transpose(1, 2).reshape(B * Nq, H * dv)
-    return ref, bnd
-
-
 # (B, Nq, Nk, H): key counts 1, 63, 64, 65, and 2000 keys (more than any resident set: the ring path)
 KV_SHAPES = [(2, 100, 1, 2), (2, 130, 63, 2), (1, 200, 64, 3), (2, 70, 65, 2), (1, 129, 2000, 1)]
 
@@ -154,7 +88,7 @@ def test_kv_ex_against_fp64(B, Nq, Nk, H, dk, dv):
     out = torch.empty(B * Nq, H * dv, **BF)
     scale = 40 ** -0.5
     _lib.attention_kv_ex(q, kv, out, B, Nq, Nk, H, dk, dv, scale)
-    ref, bound = kv_reference(q, kv, B, Nq, Nk, H, dk, dv, scale)
+    ref, bound = kv_ex_reference(q, kv, B, Nq, Nk, H, dk, dv, scale)
     check(out, ref, bound, f"attention_kv_ex B{B} Nq{Nq} Nk{Nk} dk{dk} dv{dv}")
 
 
@@ -165,7 +99,7 @@ def test_kv_ex_every_width_pair(dk, dv):
     kv = seeded((B * Nk, H * (dk + dv)), dv)
     out = torch.empty(B * Nq, H * dv, **BF)
     _lib.attention_kv_ex(q, kv, out, B, Nq, Nk, H, dk, dv, 0.15)
-    ref, bound = kv_reference(q, kv, B, Nq, Nk, H, dk, dv, 0.15)
+    ref, bound = kv_ex_reference(q, kv, B, Nq, Nk, H, dk, dv, 0.15)
     check(out, ref, bound, f"attention_kv_ex dk{dk} dv{dv}")
 
 
@@ -210,7 +144,7 @@ def test_iwsa_keeps_nan_and_inf_in_their_window(bad, win):
     M = qkv.shape[0]
     want = torch.empty(M, H * dv, **BF)
     _lib.attention_iwsa(qkv, lim, want, B, gh, gw, win, win, H, dk, dv, 0.2)
-    rows = window_rows(B, gh, gw, win, win)
+    rows = window_rows(B, gh, gw, win, win, DEV)
     hit = rows[1, 3].item()                   # a key / value row of the second window
     qkv2 = qkv.clone()
     qkv2[hit, H * dk:] = bad

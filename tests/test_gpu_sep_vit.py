@@ -5,7 +5,6 @@ outside the addressed rows) and repeatability; b200vit_head_layernorm_gelu again
 oracle/row_bounds.py; then the model: every case of tests/golden/sep_vit_spec.py through the comparison of
 test_gpu_family_parity.py in both LayerNorm modes, CUDA-graph replay, weight refresh, the direct transformer call at
 other window sizes and the eager fall-backs."""
-import math
 import sys
 
 import pytest
@@ -13,9 +12,9 @@ import torch
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
-from oracle.attention_bounds import attention_reference
-from oracle.bounds import U, U_BF16, bf16_ulp, check
-from oracle.row_bounds import layernorm_heads_reference
+from oracle.bounds import check
+from oracle.grid_attention_bounds import (head_layernorm_gelu_reference, mix_reference, window_rows,
+                                          window_token_reference)
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -29,14 +28,6 @@ NAN = float("nan")
 PAD = 5          # poisoned rows before and after the addressed ones
 
 
-def window_rows(B, gh, gw, p):
-    """[B*nw, p*p] map rows of every window, windows in (b, wy, wx) order, tokens (u, v) inside."""
-    b, wy, wx, u, v = torch.meshgrid(torch.arange(B, device=DEV), torch.arange(gh // p, device=DEV),
-                                     torch.arange(gw // p, device=DEV), torch.arange(p, device=DEV),
-                                     torch.arange(p, device=DEV), indexing="ij")
-    return ((b * gh + wy * p + u) * gw + wx * p + v).reshape(-1, p * p)
-
-
 def poisoned(t, rows=PAD):
     big = torch.full((t.shape[0] + 2 * rows, t.shape[1]), NAN, device=DEV, dtype=t.dtype)
     big[rows:rows + t.shape[0]] = t
@@ -44,23 +35,6 @@ def poisoned(t, rows=PAD):
 
 
 # ========================================================================================= window-token attention
-def window_token_reference(qkv, tok, B, gh, gw, p, H, dh):
-    """(ref, bound) of out [M, I] and tok_out [B*nw, I]: attention_reference over every (window, head) with the window
-    token's q | k | v prepended as token 0."""
-    I, rows = H * dh, window_rows(B, gh, gw, p)
-    G, n = rows.shape
-    x = qkv[rows.reshape(-1)].view(G, n, 3, H, dh)
-    x = torch.cat((tok.view(1, 1, 3, H, dh).expand(G, 1, -1, -1, -1), x), 1)
-    x = x.permute(2, 0, 3, 1, 4).reshape(3, G * H, n + 1, dh)
-    r, b = attention_reference(x[0], x[1], x[2], dh ** -0.5, kb=64)
-    r, b = r.view(G, H, n + 1, dh).transpose(1, 2), b.view(G, H, n + 1, dh).transpose(1, 2)
-    ref = torch.empty(B * gh * gw, I, dtype=torch.float64, device=DEV)
-    bnd = torch.empty_like(ref)
-    ref[rows.reshape(-1)] = r[:, 1:].reshape(-1, I)
-    bnd[rows.reshape(-1)] = b[:, 1:].reshape(-1, I)
-    return ref, bnd, r[:, 0].reshape(G, I), b[:, 0].reshape(G, I)
-
-
 def run_window_token(qkv, tok, B, gh, gw, p, H, dh, with_tok=True):
     """The kernel between NaN rows of qkv, writing between NaN rows of out and tok_out; asserts the padding kept."""
     M, I, nw = B * gh * gw, H * dh, (gh // p) * (gw // p)
@@ -111,7 +85,7 @@ def test_attention_window_token_keeps_nan_and_inf_inside_the_window(bad):
     qkv = torch.randn(B * gh * gw, 3 * H * dh, device=DEV, generator=g).bfloat16()
     tok = torch.randn(3 * H * dh, device=DEV, generator=g).bfloat16()
     clean, tclean = run_window_token(qkv, tok, B, gh, gw, p, H, dh)
-    rows = window_rows(B, gh, gw, p)
+    rows = window_rows(B, gh, gw, p, p, DEV)
     win = 1 * 6 + 1 * 3 + 2                               # window (b=1, wy=1, wx=2)
     dirty = qkv.clone()
     r = rows[win, 10]
@@ -131,24 +105,6 @@ def test_attention_window_token_keeps_nan_and_inf_inside_the_window(bad):
 
 
 # ================================================================================================ window mix
-def mix_reference(wqk, o, B, gh, gw, p, H, dh):
-    """(ref, bound) [M, I] of window_mix: attention_reference with q = wq, k = wk and v = each window's p*p*dh
-    outputs of the head, taken dh columns (one window position) at a time."""
-    I, rows = H * dh, window_rows(B, gh, gw, p)
-    nw, pp = rows.shape[0] // B, p * p
-    w = wqk.view(B, nw, H, 2, dh).permute(0, 2, 1, 3, 4)                 # b h n (q|k) d
-    q, k = (w[..., c, :].reshape(B * H, 1, nw, dh).expand(-1, pp, -1, -1).reshape(-1, nw, dh) for c in (0, 1))
-    v = o[rows.reshape(-1)].view(B, nw, pp, H, dh).permute(0, 3, 2, 1, 4).reshape(B * H * pp, nw, dh)
-    r, b = attention_reference(q, k, v, dh ** -0.5, kb=64)                # [(b h w), i, d]
-
-    def back(t):
-        t = t.view(B, H, pp, nw, dh).permute(0, 3, 2, 1, 4).reshape(-1, I)
-        out = torch.empty(B * gh * gw, I, dtype=torch.float64, device=DEV)
-        out[rows.reshape(-1)] = t
-        return out
-    return back(r), back(b)
-
-
 def run_mix(wqk, o, B, gh, gw, p, H, dh):
     M, I = B * gh * gw, H * dh
     nw = (gh // p) * (gw // p)
@@ -222,14 +178,8 @@ def test_head_layernorm_gelu_against_fp64(T, H, dh):
     _lib.head_layernorm_gelu(buf[:T], gamma, beta, H, dh)
     torch.cuda.synchronize()
     assert torch.isnan(buf[T:]).all() and torch.isnan(buf[:T, H * dh:]).all()
-    ln, bnd = layernorm_heads_reference(x.view(T, H, dh), gamma.expand(H, dh))
-    e_ln = (bnd - bf16_ulp(ln)) / (1 + U_BF16)           # the fp32 bound of the normalised value, before rounding
-    pre = ln + beta.double()
-    e_pre = e_ln + U * (pre.abs() + e_ln)
-    ref = 0.5 * pre * (1 + torch.erf(pre / math.sqrt(2)))
-    # GELU's slope is below 1.13; gelu_erf is within 1.2e-5 of it (common.cuh), plus its products' roundings
-    e = 1.13 * e_pre + 1.2e-5 + 8 * U * ref.abs()
-    check(buf[:T, :H * dh].view(T, H, dh), ref, bf16_ulp(ref.abs() + e) / 2 + e, f"head_layernorm_gelu {T}x{H}x{dh}")
+    ref, bound = head_layernorm_gelu_reference(x, gamma, beta, H, dh)
+    check(buf[:T, :H * dh].view(T, H, dh), ref, bound, f"head_layernorm_gelu {T}x{H}x{dh}")
 
 
 # ============================================================================================================ model

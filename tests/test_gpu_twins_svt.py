@@ -12,8 +12,8 @@ import torch.nn.functional as F
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
-from oracle.attention_bounds import attention_reference
 from oracle.bounds import U, check, layernorm_reference
+from oracle.grid_attention_bounds import kv_reference, window_reference, window_rows
 from vit_pytorch_b200 import _lib
 
 sys.path.insert(0, GOLDEN_DIR)
@@ -30,13 +30,6 @@ def rows_equal(a, b):
 
 
 # ================================================================================================ attention_window
-def window_rows(B, gh, gw, p):
-    """int64 [B * windows, p*p]: the rows of every window, in (p1 p2) order."""
-    b, wy, wx, i, j = torch.meshgrid(torch.arange(B), torch.arange(gh // p), torch.arange(gw // p), torch.arange(p),
-                                     torch.arange(p), indexing="ij")
-    return ((b * gh + wy * p + i) * gw + wx * p + j).reshape(-1, p * p).to(DEV)
-
-
 def run_window(qkv, B, gh, gw, p, H, dh, pad_rows=3):
     """attention_window into a view of a NaN-poisoned buffer longer than the output: (whole buffer, output view)."""
     big = torch.full((B * gh * gw + pad_rows, H * dh), NAN, device=DEV, dtype=torch.bfloat16)
@@ -44,18 +37,6 @@ def run_window(qkv, B, gh, gw, p, H, dh, pad_rows=3):
     _lib.attention_window(qkv, out, B, gh, gw, p, H, dh, dh ** -0.5)
     torch.cuda.synchronize()
     return big, out
-
-
-def window_reference(qkv, B, gh, gw, p, H, dh):
-    I, rows = H * dh, window_rows(B, gh, gw, p)
-    g = qkv[rows.reshape(-1)].view(rows.shape[0], p * p, 3, H, dh).permute(2, 0, 3, 1, 4)      # 3, W, H, n, dh
-    q, k, v = (t.reshape(-1, p * p, dh) for t in g)
-    ref, bound = attention_reference(q, k, v, dh ** -0.5)
-    back = lambda t: t.view(rows.shape[0], H, p * p, dh).permute(0, 2, 1, 3).reshape(-1, I)   # noqa: E731
-    full_ref = torch.empty(B * gh * gw, I, dtype=torch.float64, device=DEV)
-    full_bound = torch.empty_like(full_ref)
-    full_ref[rows.reshape(-1)], full_bound[rows.reshape(-1)] = back(ref), back(bound)
-    return full_ref, full_bound
 
 
 @pytest.mark.parametrize("p,gh,gw", [(1, 3, 5), (2, 4, 4), (2, 6, 10), (3, 9, 6), (4, 8, 8), (4, 4, 12), (5, 10, 5),
@@ -87,7 +68,7 @@ def test_attention_window_isolation(dh, p, gh, gw):
         bad = qkv.clone()
         bad[b * n:(b + 1) * n] = NAN
         assert rows_equal(run_window(bad, B, gh, gw, p, H, dh)[1], clean)[image != b].all(), f"NaN image {b}"
-    rows = window_rows(B, gh, gw, p)
+    rows = window_rows(B, gh, gw, p, p, DEV)
     for wi in (0, rows.shape[0] // 2, rows.shape[0] - 1):
         bad = qkv.clone()
         bad[rows[wi]] = NAN if p * p > 32 else 3.0e38
@@ -106,18 +87,6 @@ def run_kv(q, kv, B, Nq, Nk, H, dh, pad_rows=3):
     _lib.attention_kv(q, kv, out, B, Nq, Nk, H, dh, dh ** -0.5)
     torch.cuda.synchronize()
     return big, out
-
-
-def kv_reference(q, kv, B, Nq, Nk, H, dh):
-    """attention_reference takes as many queries as keys: the queries go in chunks of Nk (zero padded), each chunk a
-    sequence of its own over the image's keys."""
-    I, chunks = H * dh, -(-Nq // Nk)
-    q4 = F.pad(q.reshape(B, Nq, H, dh), (0, 0, 0, 0, 0, chunks * Nk - Nq)).view(B, chunks, Nk, H, dh)
-    qs = q4.permute(0, 3, 1, 2, 4).reshape(B * H * chunks, Nk, dh)
-    k, v = (kv[:, o * I:(o + 1) * I].reshape(B, Nk, H, dh).permute(0, 2, 1, 3).reshape(B * H, Nk, dh) for o in (0, 1))
-    ref, bound = attention_reference(qs, k.repeat_interleave(chunks, 0), v.repeat_interleave(chunks, 0), dh ** -0.5)
-    back = lambda t: t.view(B, H, chunks * Nk, dh)[:, :, :Nq].permute(0, 2, 1, 3).reshape(B * Nq, I)   # noqa: E731
-    return back(ref), back(bound)
 
 
 def kv_inputs(B, Nq, Nk, H, dh, seed, strided=True):

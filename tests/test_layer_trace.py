@@ -42,14 +42,24 @@ def _case(name):
     return next(c for c in CASES if c.name == name)
 
 
+def _ln_width(m):
+    """The width of a LayerNorm: nn.LayerNorm's, or the channels of a channel LayerNorm over an NCHW map (Twins-SVT,
+    CvT: `g` of shape (1, dim, 1, 1) and `eps`); None for any other module."""
+    if isinstance(m, nn.LayerNorm):
+        return m.normalized_shape[0]
+    if isinstance(getattr(m, "g", None), nn.Parameter) and isinstance(getattr(m, "eps", None), float):
+        return m.g.numel()
+    return None
+
+
 def set_eps(mod):
     """The LayerNorms over the model width take eps 1e-5, 1e-6, 1e-3 in module order, the narrower ones (q / k head
     norms, DeepViT's norm over heads) 1e-6."""
-    norms = [m for m in mod.modules() if isinstance(m, nn.LayerNorm)]
-    width = max(m.normalized_shape[0] for m in norms) if norms else 0
+    norms = [m for m in mod.modules() if _ln_width(m) is not None]
+    width = max(_ln_width(m) for m in norms) if norms else 0
     j = 0
     for m in norms:
-        if m.normalized_shape[0] == width:
+        if _ln_width(m) == width:
             m.eps, j = EPS[j % len(EPS)], j + 1
         else:
             m.eps = EPS[1]
