@@ -1,8 +1,8 @@
 """fp64 references with a per-element error bound for the attention kernels over token grids and the kernels around
 them: windows (Twins-SVT, MaxViT, CrossFormer), sub-sampled keys (Twins-SVT, CvT, ScalableViT), interactive windows
 (ScalableViT), patch groups (MobileViT), the depthwise convolutional projection (CvT), window tokens and window mixing
-(SepViT), region-to-local windows (RegionViT), and the SiLU GEMM epilogue and the head LayerNorm + GELU  --  TEST
-INFRASTRUCTURE.
+(SepViT), region-to-local windows (RegionViT), the positional encoding generator (Twins-SVT, ScalableViT), and the
+SiLU GEMM epilogue and the head LayerNorm + GELU  --  TEST INFRASTRUCTURE.
 
 Every reference returns `(ref, bound)`: fp64 tensors on the device of its inputs, to be checked with
 oracle.bounds.check.  The attention references gather each window's rows and hand them to
@@ -307,6 +307,18 @@ def conv_reference(x: Tensor, wt: Tensor, b: Tensor, B: int, h: int, w: int, k: 
     ref, mag = (t.permute(0, 2, 3, 1).reshape(-1, C) for t in (ref, mag))
     e = (k * k + 1) * 2.0 ** -23 * mag
     return ref, e + bf16_ulp(ref.abs() + e) / 2
+
+
+def peg_reference(x: Tensor, w: Tensor, b: Tensor, B: int, gh: int, gw: int, k: int) -> Tuple[Tensor, Tensor]:
+    """fp64 (ref, bound) of b200vit_peg (Twins-SVT, ScalableViT): conv2d plus the identity, and per element the fp32
+    error of k*k accumulated taps, the bias and the residual add."""
+    C = x.shape[1]
+    grid = x.double().view(B, gh, gw, C).permute(0, 3, 1, 2)
+    wt = w.double().t().reshape(C, 1, k, k)
+    ref = F.conv2d(grid, wt, b.double(), padding=k // 2, groups=C) + grid
+    mag = F.conv2d(grid.abs(), wt.abs(), b.double().abs(), padding=k // 2, groups=C) + grid.abs()
+    ref, mag = (t.permute(0, 2, 3, 1).reshape(-1, C) for t in (ref, mag))
+    return ref, (k * k + 4) * U * mag + 1e-30
 
 
 def im2col_reference(x: Tensor, B: int, H: int, W: int, k: int, s: int, pad: int) -> Tensor:

@@ -66,11 +66,20 @@ OUTPUTS = {
     "attention_kv": ("out",),
     "attention_groups": ("out",),
     "conv_proj_dw": ("q_out", "kv_out"),
+    "attention_kv_ex": ("out",),
+    "attention_iwsa": ("out",),
+    "attention_window_token": ("out", "tok_out"),
+    "head_layernorm_gelu": ("buf",),
+    "window_mix": ("out",),
+    "attention_region_local": ("out",),
+    "peg": ("y",),
 }
-# the entry points of the attention records on token grids (engine.Windows, StridedKV, ConvProj, PatchGroups) and of
-# the SiLU feed-forward block, which make_engine_schedule.ENTRY_POINTS does not list
+# the entry points of the attention records on token grids (engine.Windows, StridedKV, InteractiveWindows, ConvProj,
+# PatchGroups, WindowTokenBlock, RegionLocalBlock), of the SiLU feed-forward block and of ScalableViT's positional
+# encoding between two run_blocks calls, which make_engine_schedule.ENTRY_POINTS does not list
 GRID_ENTRY_POINTS = ("gemm_act", "conv_im2col_nhwc", "attention_window", "attention_window_relpos", "attention_kv",
-                     "attention_groups", "conv_proj_dw")
+                     "attention_groups", "conv_proj_dw", "attention_kv_ex", "attention_iwsa", "attention_window_token",
+                     "head_layernorm_gelu", "window_mix", "attention_region_local", "peg")
 
 
 def schedule():
@@ -145,10 +154,12 @@ def emulate_impl(name: str, real: Callable) -> Callable:
     return run
 
 
-def trace(eng, x: Tensor, kw: dict, ln_mode: str, impl=real_impl, prime: Optional[Callable] = None) -> List[Launch]:
-    """Run eng.run_blocks(x, **kw) on the per-kernel loop in `ln_mode` with every launch traced.  In fold mode with
-    kw['primed'], prime(x, xb, stats) first writes the workspace's bf16 copy of x and its row statistics (not traced),
-    as an embedding kernel would; every other workspace buffer starts as NaN."""
+def trace(eng, x: Tensor, kw: dict, ln_mode: str, impl=real_impl, prime: Optional[Callable] = None,
+          call: Optional[Callable[[], object]] = None) -> List[Launch]:
+    """Run call() -- by default eng.run_blocks(x, **kw); a module's own driver of several run_blocks calls and the
+    launches between them (ScalableViT's Transformer.run_fused) -- on the per-kernel loop in `ln_mode` with every
+    launch traced.  In fold mode with kw['primed'], prime(x, xb, stats) first writes the workspace's bf16 copy of x and
+    its row statistics (not traced), as an embedding kernel would; every other workspace buffer starts as NaN."""
     S = schedule()
     with S.recording(eng, S.caller_buffers(eng, x, kw), ln_mode, "python", extra_entry_points=GRID_ENTRY_POINTS,
                      recorder=tracer(impl)) as rec:
@@ -158,7 +169,10 @@ def trace(eng, x: Tensor, kw: dict, ln_mode: str, impl=real_impl, prime: Optiona
             xb, st = eng.entry_buffers(x.shape[0], x.device)
             if xb is not None:
                 prime(x, xb, st)
-        eng.run_blocks(x, **kw)
+        if call is None:
+            eng.run_blocks(x, **kw)
+        else:
+            call()
     return rec.launches
 
 
@@ -275,6 +289,39 @@ def expected(name: str, a: dict, got: dict, on_output: Optional[Callable] = None
         geo = (a["B"], a["h"], a["w"], a["k"])
         put("q_out", GB.conv_reference(a["x"], a["wq"], a["bq"], *geo, 1))
         put("kv_out", GB.conv_reference(a["x"], a["wkv"], a["bkv"], *geo, a["s"]))
+        return out
+    if name == "attention_kv_ex":
+        put("out", GB.kv_ex_reference(a["q"], a["kv"], a["B"], a["Nq"], a["Nk"], a["H"], a["dk"], a["dv"],
+                                      f32(a["scale"])))
+        return out
+    if name == "attention_iwsa":
+        put("out", GB.iwsa_reference(a["qkv"], a["lim"], a["B"], a["gh"], a["gw"], a["wh"], a["ww"], a["H"], a["dk"],
+                                     a["dv"], f32(a["scale"])))
+        return out
+    if name == "attention_window_token":
+        r, b, tr, tb = GB.window_token_reference(a["qkv"], a["tok_qkv"], a["B"], a["gh"], a["gw"], a["p"], a["H"],
+                                                 a["dh"], f32(a["scale"]))
+        put("out", (r, b))
+        if a["tok_out"] is not None:
+            put("tok_out", (tr, tb))
+        return out
+    if name == "head_layernorm_gelu":                 # in place on the first nheads * dh columns of buf
+        buf, n = a["buf"], a["nheads"] * a["dh"]
+        r, b = GB.head_layernorm_gelu_reference(buf[:, :n], a["gamma"], a["beta"], a["nheads"], a["dh"], f32(a["eps"]))
+        ref, bnd = _exact(buf)
+        ref[:, :n], bnd[:, :n] = r.reshape(-1, n), b.reshape(-1, n)
+        put("buf", (ref, bnd))
+        return out
+    if name == "window_mix":
+        put("out", GB.mix_reference(a["wqk"], a["o"], a["B"], a["gh"], a["gw"], a["p"], a["H"], a["dh"],
+                                    f32(a["scale"])))
+        return out
+    if name == "attention_region_local":
+        put("out", GB.region_local_reference(a["qkv"], a["table"], a["B"], a["lh"], a["lw"], a["rh"], a["rw"], a["W"],
+                                             a["H"], f32(a["scale"]), a["dh"]))
+        return out
+    if name == "peg":
+        put("y", GB.peg_reference(a["x"], a["w"], a["bias"], a["B"], a["gh"], a["gw"], a["k"]))
         return out
     if name == "layernorm":
         kw = dict(row_index=a["row_index"], eps=f32(a["eps"]))
@@ -405,6 +452,8 @@ class RefLayer:
     cat: Tuple[str, ...] = ()                                # fields the engine gets as a concatenation, not `is`
     grid: Optional[dict] = None                              # the attention on the token grid, by `kind` (_grid_*)
     ff_act: str = "gelu"                                     # the feed-forward block's activation
+    ff_first: bool = False                                   # the feed-forward block runs before the attention
+    peg: Optional[nn.Conv2d] = None                          # the depthwise PEG convolution that runs after the layer
 
 
 def _plain(attn, ff, qkv_w: Optional[Tensor] = None, scale: Optional[float] = None, **kw) -> RefLayer:
@@ -433,12 +482,75 @@ def _conv_layer(attn: nn.Module, ff: nn.Sequential, qkv_w: Tensor, grid: dict, c
                     heads=attn.heads, dim_head=I // attn.heads, scale=float(attn.scale), grid=grid, cat=cat)
 
 
+def padded_key_width(dk: int) -> int:
+    """The width the key-head kernels (attention_kv_ex, attention_iwsa) are built for that runs a dim_key: dk rounded
+    up to a multiple of 16."""
+    return -(-dk // 16) * 16
+
+
+def _padded_heads(w: Tensor, H: int, dp: int) -> Tensor:
+    """w [H d, ...] with dp - d zero rows after each head's d rows: [H dp, ...].  A zero q or k column adds exactly 0
+    to every score, so the padded heads' attention is the module's."""
+    d, rest = w.shape[0] // H, tuple(w.shape[1:])
+    out = torch.zeros((H, dp) + rest, dtype=w.dtype, device=w.device)
+    out[:, :d] = w.detach().reshape((H, d) + rest)
+    return out.reshape((H * dp,) + rest)
+
+
+def _scalable_layers(mod: nn.Module) -> List[RefLayer]:
+    """ScalableViT's Transformer (scalable_vit.py:214-236): each reference layer's modules [SSA, FeedForward, PEG,
+    FeedForward, IWSA] run in that order (its loop binds the 4th, a FeedForward, to `iwsa` and the 5th to `ff2`): two
+    layers, (SSA, FeedForward) and, feed-forward first, (FeedForward, IWSA); the first reference layer's PEG after the
+    first.  The q and k heads run dim_key wide padded to padded_key_width; the softmax scale stays dim_key ** -0.5."""
+    out = []
+    for ssa, ff1, peg, ff2, iwsa in mod.layers:
+        for a, ff, first in ((ssa, ff1, False), (iwsa, ff2, True)):
+            H, D = a.heads, a.to_q.in_channels
+            dk, dv = a.to_q.out_channels // H, a.to_v.out_channels // H
+            dp = padded_key_width(dk)
+            q = _padded_heads(a.to_q.weight.reshape(H * dk, D), H, dp)
+            if a is ssa:                                    # scalable_vit.py:117-146: keys / values r x r, stride r
+                qkv_w = q
+                grid = dict(kind="strided", conv=a.to_k, kv=torch.cat((_padded_heads(a.to_k.weight, H, dp),
+                                                                        a.to_v.weight.detach())), dv=dv)
+            else:                                           # scalable_vit.py:149-196
+                qkv_w = torch.cat((q, _padded_heads(a.to_k.weight.reshape(H * dk, D), H, dp),
+                                   a.to_v.weight.detach().reshape(H * dv, D)))
+                grid = dict(kind="iwsa", module=a, dv=dv)
+            o, c1, c2 = a.to_out[0], ff.net[1], ff.net[4]
+            out.append(RefLayer(
+                ln1=_chan_ln(a.norm), qkv_w=qkv_w, out=(o.weight.reshape(D, H * dv), o.bias), ln2=_chan_ln(ff.net[0]),
+                fc1=(c1.weight.reshape(-1, D), c1.bias), fc2=(c2.weight.reshape(D, -1), c2.bias), heads=H,
+                dim_head=dp, scale=dk ** -0.5, grid=grid, cat=("qkv_w",), ff_first=first,
+                peg=peg.proj if peg is not None and a is ssa else None))
+    return out
+
+
 def module_layers(mod: nn.Module) -> List[RefLayer]:
     """The layers of a reference Transformer, by family (the module's class)."""
     from vit_pytorch_b200 import (cait, cct, crossformer, cvt, deepvit, max_vit, mobile_vit, na_vit,
-                                  na_vit_nested_tensor, simple_vit_with_qk_norm, twins_svt, vit, vit_for_small_dataset,
-                                  vit_nd_rotary, vivit, xcit)
+                                  na_vit_nested_tensor, regionvit, scalable_vit, sep_vit, simple_vit_with_qk_norm,
+                                  twins_svt, vit, vit_for_small_dataset, vit_nd_rotary, vivit, xcit)
     t = type(mod)
+    if t is scalable_vit.Transformer:
+        return _scalable_layers(mod)
+    if t is sep_vit.Transformer:                                            # sep_vit.py:208-235, DSSA :91-205
+        out = []
+        for a, ff in mod.layers:
+            I, D = a.to_qkv.out_channels // 3, a.to_qkv.in_channels
+            out.append(_conv_layer(a, ff.net, a.to_qkv.weight.reshape(3 * I, D), dict(kind="window_token", module=a)))
+        return out
+    if t is regionvit.R2LTransformer:                                       # regionvit.py:114-190
+        out = []
+        for a, ff in mod.layers:
+            fc1, fc2 = _linears(ff)
+            o = a.to_out[0]
+            out.append(RefLayer(
+                ln1=_ln(a.norm), qkv_w=a.to_qkv.weight, out=(o.weight, o.bias), ln2=_ln(ff[0]),
+                fc1=(fc1.weight, fc1.bias), fc2=(fc2.weight, fc2.bias), heads=a.heads, dim_head=a.dim_head,
+                scale=float(a.scale), grid=dict(kind="region_local", table=mod.local_rel_pos_bias.weight,
+                                                window=mod.window_size)))
+        return out
     if t is twins_svt.Transformer:                                          # twins_svt.py:159-176
         out = []
         for local_attn, ff1, global_attn, ff2 in mod.layers:
@@ -622,6 +734,26 @@ def check_identity(mod: nn.Module, case: str = "") -> None:
                                     ("conv2_w", P.conv2_w, r["conv2"].weight), ("conv2_b", P.conv2_b, r["conv2"].bias),
                                     ("scale", P.scale, r["scale"])):
                 same(i, f"lpi.{what}", got, want)
+        if L.ff_first != R.ff_first:
+            raise AssertionError(f"{case}: layer {i}: EncoderLayer.ff_first is {L.ff_first}, the module's feed-forward "
+                                 f"block runs {'first' if R.ff_first else 'after the attention'}")
+        g, A = R.grid or {}, L.attention
+        kind = g.get("kind")
+        if kind == "strided":                  # Twins-SVT's to_kv as it is, ScalableViT's padded to_k | to_v
+            same(i, "attention.kv_w", A.kv_w, g.get("kv", g["conv"].weight), "kv" in g)
+        elif kind == "iwsa":
+            lim = g["module"].local_interactive_module
+            same(i, "attention.lim_w", A.lim_w, lim.weight)
+            same(i, "attention.lim_b", A.lim_b, lim.bias)
+        elif kind == "window_token":
+            m = g["module"]
+            ln, conv = m.window_tokens_to_qk[0], m.window_tokens_to_qk[3]
+            for what, got, want in (("token", A.token, m.window_tokens), ("ln.gamma", A.ln.gamma, ln.weight),
+                                    ("ln.beta", A.ln.beta, ln.bias), ("wqk_w", A.wqk_w, conv.weight.reshape(
+                                        conv.out_channels, conv.in_channels)), ("wqk_b", A.wqk_b, conv.bias)):
+                same(i, f"attention.{what}", got, want)
+        elif kind == "region_local":
+            same(i, "attention.bias", A.bias, g["table"])
 
 
 # ------------------------------------------------------------------------------------------------------ provenance
@@ -712,6 +844,9 @@ class Walk:
         self.case, self.calls, self.fold, self.kw = case, launches, fold, kw
         self.pos, self.where, self.cur = 0, "", None
         self.have_stats = fold and bool(kw.get("primed"))
+        # the statistics the next folded GEMM reads are the entry ones, one part per row (the prime or a rowstats_cast),
+        # not a residual GEMM's
+        self.entry_stats = self.have_stats
 
     # ---------------------------------------------------------------- failures and comparisons
     def fail(self, op: str, msg: str):
@@ -728,6 +863,9 @@ class Walk:
         if c.name not in names:
             self.fail("-", f"{' or '.join(names)} expected")
         return c
+
+    def peek(self) -> Optional[str]:
+        return self.calls[self.pos].name if self.pos < len(self.calls) else None
 
     def same(self, op: str, got, want) -> None:
         """Bit for bit (None only as None)."""
@@ -766,34 +904,45 @@ class Walk:
         self.within(op, got, *_stats(xb, got))
 
     # ---------------------------------------------------------------- steps
+    def entry_cast(self, S: Tensor) -> None:
+        """rowstats_cast(S): the bf16 copy and the one-part row statistics the next folded GEMM reads."""
+        c = self.take("rowstats_cast")
+        self.same("x", c.pre["x"], S)
+        self.have_stats = self.entry_stats = True
+
+    def folded(self, a: dict, S: Tensor, ln: Ln, W: Tensor, b: Optional[Tensor]) -> None:
+        """The operands of a LayerNorm-folded GEMM computing LN(S) W^T + b: bf16(S), its row statistics, gamma W,
+        its column sums and W beta + b."""
+        d = lambda t: t.detach().double()                                               # noqa: E731
+        self.same("a", a["a"], S.bfloat16())
+        self.stats("ln_sums", a["ln_sums"], a["a"])
+        self.value("ln_eps", a["ln_eps"], float(ln.eps))
+        wg = (d(W) * d(ln.gamma)[None]).float().bfloat16()
+        self.same("w (gamma W)", a["w"], wg)
+        K = W.shape[1]
+        wd = wg.double()
+        self.within("col_s", a["col_s"], wd.sum(1), K * U * wd.abs().sum(1))
+        t = torch.zeros(W.shape[0], dtype=torch.float64, device=W.device)
+        tb = torch.zeros_like(t)
+        if ln.beta is not None:
+            t, tb = d(W) @ d(ln.beta), d(W).abs() @ d(ln.beta).abs()
+        if b is not None:
+            t, tb = t + d(b), tb + d(b).abs()
+        self.within("bias (W beta + b)", a["bias"], t, (K + 1) * U * tb)
+
     def normed(self, S: Tensor, ln: Ln, W: Tensor, b: Optional[Tensor], gelu: bool = False,
                head: Optional[tuple] = None, heads: int = 0, dh: int = 0, act: Optional[str] = None) -> Tensor:
         """out = LN(S) W^T + b (reference vit.py:19-21 / :52-54): the bf16 output of its GEMM; `act` "silu": the
         activation of gemm_act (MobileViT's FeedForward, mobile_vit.py:28-34)."""
         gemm = "gemm_headnorm" if head is not None else "gemm_act" if act is not None else "gemm"
-        d = lambda t: t.detach().double()                                               # noqa: E731
         if self.fold:
-            if not self.have_stats:
-                c = self.take("rowstats_cast")
-                self.same("x", c.pre["x"], S)
-                self.have_stats = True
+            # a stream no launch has copied since it changed takes one rowstats_cast; without it the GEMM's operands
+            # below show what it read instead
+            if not self.have_stats and self.peek() == "rowstats_cast":
+                self.entry_cast(S)
             c = self.take(gemm)
             a = c.pre
-            self.same("a", a["a"], S.bfloat16())
-            self.stats("ln_sums", a["ln_sums"], a["a"])
-            self.value("ln_eps", a["ln_eps"], float(ln.eps))
-            wg = (d(W) * d(ln.gamma)[None]).float().bfloat16()
-            self.same("w (gamma W)", a["w"], wg)
-            K = W.shape[1]
-            wd = wg.double()
-            self.within("col_s", a["col_s"], wd.sum(1), K * U * wd.abs().sum(1))
-            t = torch.zeros(W.shape[0], dtype=torch.float64, device=W.device)
-            tb = torch.zeros_like(t)
-            if ln.beta is not None:
-                t, tb = d(W) @ d(ln.beta), d(W).abs() @ d(ln.beta).abs()
-            if b is not None:
-                t, tb = t + d(b), tb + d(b).abs()
-            self.within("bias (W beta + b)", a["bias"], t, (K + 1) * U * tb)
+            self.folded(a, S, ln, W, b)
         else:
             c = self.take("layernorm")
             a = c.pre
@@ -848,11 +997,12 @@ class Walk:
             self.fail("out_f32", "the residual GEMM writes no fp32 stream")
         new = c.post["out_f32"]
         if copy and self.fold:
-            if a["out_bf16"] is None or a["stats_out"] is None:
-                self.fail("out_bf16", "the stream's bf16 copy and row statistics are not written")
+            for op, what in (("out_bf16", "bf16 copy"), ("stats_out", "row statistics")):
+                if a[op] is None:
+                    self.fail(op, f"the stream's {what} the next folded GEMM reads is not written")
             self.same("out_bf16", c.post["out_bf16"], new.bfloat16())
             self.stats("stats_out", c.post["stats_out"], c.post["out_bf16"])
-            self.have_stats = True
+            self.have_stats, self.entry_stats = True, False
         else:
             self.same("out_bf16", a["out_bf16"], None)
             self.same("stats_out", a["stats_out"], None)
@@ -919,13 +1069,14 @@ class Walk:
         self.same("out_f32", a["out_f32"], None)
         return c.post["out_bf16"]
 
-    def plain_gemm(self, A: Tensor, W: Tensor) -> Tensor:
-        """A W^T, no bias and no LayerNorm: a bias-free 1 x 1 convolution on a bf16 map."""
+    def plain_gemm(self, A: Tensor, W: Tensor, b: Optional[Tensor] = None) -> Tensor:
+        """A W^T + b and no LayerNorm: a 1 x 1 convolution on a bf16 map, or a convolution on its im2col."""
         c = self.take("gemm")
         a = c.pre
         self.same("a", a["a"], A)
         self.same("w", a["w"], W.detach().bfloat16())
-        for op in ("bias", "resid", "ln_sums", "out_f32", "stats_out"):
+        self.same("bias", a["bias"], None if b is None else b.detach().float())
+        for op in ("resid", "ln_sums", "out_f32", "stats_out"):
             self.same(op, a[op], None)
         self.value("gelu", a["gelu"], False)
         return c.post["out_bf16"]
@@ -942,8 +1093,9 @@ class Walk:
         self.value("dh", a["dh"], R.dim_head)
         self.value("scale", a["scale"], float(R.scale))
 
-    def grid_attention(self, R: RefLayer, S: Tensor, i: int) -> Tensor:
-        """The attention output of layer R on the stream S, by the kind of its attention on the grid."""
+    def grid_attention(self, R: RefLayer, S: Tensor, i: int) -> Tuple[Tensor, Tensor]:
+        """(the attention output of layer R on the stream S, by the kind of its attention on the grid; the stream,
+        which RegionViT's region pass updates first)."""
         g, kind = R.grid, R.grid["kind"]
         if kind in ("window", "relpos", "groups"):
             qkv = self.normed(S, R.ln1, R.qkv_w, None)
@@ -968,11 +1120,30 @@ class Walk:
             self.same("qkv", c.pre["qkv"], qkv)
             self.grid_geometry(c.pre)
             self.heads(c.pre, R)
-            return c.post["out"]
+            return c.post["out"], S
+        if kind == "iwsa":
+            return self.interactive_windows(R, S, i), S
+        if kind == "window_token":
+            return self.window_tokens(R, S, i), S
+        if kind == "region_local":
+            S = self.region_pass(R, S, i)
+            qkv = self.normed(S, R.ln1, R.qkv_w, None)
+            self.where = f"layer {i} attention"
+            c = self.take("attention_region_local")
+            a = c.pre
+            self.same("qkv", a["qkv"], qkv)
+            # regionvit.py:260-270: local_rel_pos_bias(bias_indices), whose table the kernel reads transposed
+            self.same("table", a["table"], g["table"].detach().float().t())
+            (lh, lw), (rh, rw) = self.kw["grid"], self.kw["regions"]
+            self.value("B", a["B"], self.kw["B"])
+            for op, v in (("lh", lh), ("lw", lw), ("rh", rh), ("rw", rw), ("W", g["window"])):
+                self.value(op, a[op], v)
+            self.heads(a, R)
+            return c.post["out"], S
         gh, gw = self.kw["grid"]
         B = self.kw["B"]
         xn = self.exact_ln(S, R.ln1)
-        if kind == "strided":                               # twins_svt.py:140-157: keys from a k x k, stride-k conv
+        if kind == "strided":       # twins_svt.py:140-157, scalable_vit.py:126-146: keys from a k x k, stride-k conv
             conv = g["conv"]
             k, s = conv.kernel_size[0], conv.stride[0]
             self.where = f"layer {i} queries"
@@ -991,8 +1162,10 @@ class Walk:
                 self.value("p", a["p"], conv.padding[0])
                 col = c.post["out_bf16"]
             self.where = f"layer {i} keys and values"
-            # the Conv2d weight in the im2col column order (tap row, tap column, channel)
-            kv = self.plain_gemm(col, conv.weight.permute(0, 2, 3, 1).reshape(conv.weight.shape[0], -1))
+            # the Conv2d weight (ScalableViT: to_k's, heads padded, then to_v's) in the im2col column order (tap row,
+            # tap column, channel)
+            kvw = g.get("kv", conv.weight)
+            kv = self.plain_gemm(col, kvw.permute(0, 2, 3, 1).reshape(kvw.shape[0], -1))
             kh, kw = (gh + 2 * conv.padding[0] - k) // s + 1, (gw + 2 * conv.padding[1] - k) // s + 1
         else:                                               # cvt.py:51-60, 74-75: depthwise convs + BatchNorm, 1 x 1
             dq, bq, _ = g["q"]
@@ -1022,15 +1195,180 @@ class Walk:
             kv = self.plain_gemm(akv, g["kv_w"])
             kh, kw = (gh + 2 * dkv.padding[0] - k) // s + 1, (gw + 2 * dkv.padding[1] - k) // s + 1
         self.where = f"layer {i} attention"
-        c = self.take("attention_kv")
+        c = self.take("attention_kv_ex" if "dv" in g else "attention_kv")
         a = c.pre
         self.same("q", a["q"], q)
         self.same("kv", a["kv"], kv)
         self.value("B", a["B"], B)
         self.value("Nq", a["Nq"], gh * gw)
         self.value("Nk", a["Nk"], kh * kw)
+        if "dv" in g:                                       # ScalableViT: value heads of their own width
+            self.value("H", a["H"], R.heads)
+            self.value("dk", a["dk"], R.dim_head)
+            self.value("dv", a["dv"], g["dv"])
+            self.value("scale", a["scale"], float(R.scale))
+        else:
+            self.heads(a, R)
+        return c.post["out"], S
+
+    def interactive_windows(self, R: RefLayer, S: Tensor, i: int) -> Tensor:
+        """ScalableViT's IWSA (scalable_vit.py:170-196): q | k | v of LN(S), the local interactive module (a 3 x 3
+        convolution with bias) of the v map as im2col + GEMM, attention inside each window plus that term."""
+        g = R.grid
+        m, dv = g["module"], g["dv"]
+        lim = m.local_interactive_module
+        H, dp = R.heads, R.dim_head
+        Ik, Iv = H * dp, H * dv
+        (gh, gw), B = self.kw["grid"], self.kw["B"]
+        qkv = self.normed(S, R.ln1, R.qkv_w, None)
+        self.where = f"layer {i} local interactive module"
+        c = self.take("conv_im2col_nhwc")
+        a = c.pre
+        self.same("x (the v columns of qkv)", a["x"], qkv[:, 2 * Ik:2 * Ik + Iv])
+        self.value("B", a["B"], B)
+        self.value("H", a["H"], gh)
+        self.value("W", a["W"], gw)
+        self.value("k", a["k"], lim.kernel_size[0])
+        self.value("s", a["s"], lim.stride[0])
+        self.value("p", a["p"], lim.padding[0])
+        w = lim.weight
+        lo = self.plain_gemm(c.post["out_bf16"], w.permute(0, 2, 3, 1).reshape(w.shape[0], -1), lim.bias)
+        self.where = f"layer {i} attention"
+        c = self.take("attention_iwsa")
+        a = c.pre
+        self.same("qkv", a["qkv"], qkv)
+        self.same("lim", a["lim"], lo)
+        self.grid_geometry(a)
+        ws = m.window_size                                  # default(wsz, height), default(wsz, width)
+        self.value("wh", a["wh"], gh if ws is None else ws)
+        self.value("ww", a["ww"], gw if ws is None else ws)
+        self.value("H", a["H"], H)
+        self.value("dk", a["dk"], dp)
+        self.value("dv", a["dv"], dv)
+        self.value("scale", a["scale"], float(R.scale))
+        return c.post["out"]
+
+    def window_tokens(self, R: RefLayer, S: Tensor, i: int) -> Tensor:
+        """SepViT's DSSA (sep_vit.py:168-219): the windows' attention with the window token, then, with more than one
+        window, the window tokens' LayerNorm + GELU, their q | k projection and the attention across windows."""
+        m = R.grid["module"]
+        H, dh = R.heads, R.dim_head
+        I, p = H * dh, m.window_size
+        gh, gw = self.kw["grid"]
+        qkv = self.normed(S, R.ln1, R.qkv_w, None)
+        self.where = f"layer {i} attention"
+        c = self.take("attention_window_token")
+        a = c.pre
+        self.same("qkv", a["qkv"], qkv)
+        # the window token joins each window after the LayerNorm (sep_vit.py:175-184): to_qkv of the raw token, an
+        # fp32 dot product of D terms rounded to bf16
+        W, t = R.qkv_w.detach().double(), m.window_tokens.detach().double()
+        ref = W @ t
+        self.within("tok_qkv", a["tok_qkv"], ref, Bd.bf16_bound(ref, W.shape[1] * U * (W.abs() @ t.abs())))
+        self.value("p", a["p"], p)
+        self.grid_geometry(a)
+        self.heads(a, R)
+        o = c.post["out"]
+        if (gh // p) * (gw // p) == 1:                      # sep_vit.py:202-203: no attention across windows
+            self.same("tok_out", a["tok_out"], None)
+            return o
+        if a["tok_out"] is None:
+            self.fail("tok_out", "the window tokens' outputs are not written")
+        tok = c.post["tok_out"]
+        self.where = f"layer {i} window tokens"
+        c = self.take("head_layernorm_gelu")
+        a = c.pre
+        ln, act, conv = m.window_tokens_to_qk[0], m.window_tokens_to_qk[1], m.window_tokens_to_qk[3]
+        if not isinstance(act, nn.GELU) or act.approximate != "none":
+            self.fail("-", "the window tokens' activation is not the erf GELU the kernel computes")
+        self.same("buf", a["buf"], tok)
+        self.same("gamma", a["gamma"], ln.weight.detach().float())
+        self.same("beta", a["beta"], ln.bias.detach().float())
+        self.value("eps", a["eps"], float(ln.eps))
+        self.value("nheads", a["nheads"], H)
+        self.value("dh", a["dh"], dh)
+        # the rows of the window tokens' q | k in the order window_mix reads (head h's q, then its k): the
+        # convolution's output channels through the module's own _ChannelsToHeads and chunk(2, dim=-1)
+        chan = torch.arange(2 * I, dtype=torch.float64).view(1, 2 * I, 1)
+        wq, wk = m.window_tokens_to_qk[4](chan).chunk(2, dim=-1)          # [1, H, 1, dh] each
+        order = torch.cat((wq, wk), -1).reshape(-1).long()
+        wqk = self.plain_gemm(c.post["buf"], conv.weight.reshape(2 * I, I)[order.to(conv.weight.device)], conv.bias)
+        self.where = f"layer {i} window mixing"
+        c = self.take("window_mix")
+        a = c.pre
+        self.same("wqk", a["wqk"], wqk)
+        self.same("o", a["o"], o)
+        self.value("p", a["p"], p)
+        self.grid_geometry(a)
         self.heads(a, R)
         return c.post["out"]
+
+    def region_pass(self, R: RefLayer, S: Tensor, i: int) -> Tensor:
+        """RegionViT's regional attention (regionvit.py:275): the layer's attention over each image's region tokens
+        alone, with its residual, on the rows after the local ones; returns the stream with them updated.  In fold
+        mode the region rows take the exact LayerNorm while the statistics are the entry ones (their one part per
+        row is not read at a row offset), then a rowstats_cast of the new rows; after a residual GEMM wrote them, the
+        folded QKV reads them and the region residual writes the new ones."""
+        Ml = self.kw["B"] * self.kw["N"]
+        rh, rw = self.kw["regions"]
+        Sr = S[Ml:]
+        self.where = f"layer {i} region qkv"
+        if self.fold and not self.have_stats and self.peek() == "rowstats_cast":
+            self.entry_cast(S)
+        gemm_stats = self.fold and not self.entry_stats
+        if gemm_stats:
+            c = self.take("gemm")
+            a = c.pre
+            self.folded(a, Sr, R.ln1, R.qkv_w, None)
+            for op in ("resid", "out_f32", "stats_out"):
+                self.same(op, a[op], None)
+            self.value("gelu", a["gelu"], False)
+            qkv = c.post["out_bf16"]
+        else:
+            qkv = self.plain_gemm(self.exact_ln(Sr, R.ln1), R.qkv_w)
+        self.where = f"layer {i} region attention"
+        c = self.take("attention")
+        a = c.pre
+        self.same("qkv", a["qkv"], qkv)
+        self.value("B", a["B"], self.kw["B"])
+        self.value("N", a["N"], rh * rw)
+        self.value("mask_self", a["mask_self"], False)
+        self.heads(a, R)
+        self.where = f"layer {i} region out"
+        new = self.residual(c.post["out"], R.out, R.out_scale, Sr, copy=gemm_stats, D=S.shape[1])
+        if self.fold and not gemm_stats:
+            self.where = f"layer {i} region statistics"
+            self.entry_cast(new)
+        return torch.cat((S[:Ml], new))
+
+    def feed_forward(self, R: RefLayer, S: Tensor, i: int) -> Tensor:
+        """S + fc2(act(fc1(LN2(S)))): the new stream."""
+        self.where = f"layer {i} fc1"
+        act = None if R.ff_act == "gelu" else R.ff_act
+        h = self.normed(S, R.ln2, R.fc1[0], R.fc1[1], gelu=act is None, act=act)
+        self.where = f"layer {i} fc2"
+        return self.residual(h, R.fc2, R.ff_scale, S, copy=True, D=S.shape[1])
+
+    def peg(self, conv: nn.Conv2d, S: Tensor, i: int) -> Tensor:
+        """y = S + conv(S), the depthwise PEG (scalable_vit.py:85-91, 313-314) between two layers, into a new stream;
+        in fold mode a rowstats_cast of y then primes the next run_blocks call."""
+        self.where = f"layer {i} positional encoding"
+        c = self.take("peg")
+        a = c.pre
+        k, C = conv.kernel_size[0], conv.out_channels
+        if conv.groups != C or conv.stride[0] != 1 or conv.padding[0] != k // 2:
+            self.fail("-", "the PEG is not a depthwise k x k convolution at stride 1 with padding k // 2")
+        self.same("x", a["x"], S)
+        self.same("w (tap major)", a["w"], conv.weight.detach().float().reshape(C, k * k).t())
+        self.same("bias", a["bias"], conv.bias.detach().float() if conv.bias is not None else
+                  torch.zeros(C, dtype=torch.float32, device=S.device))
+        self.grid_geometry(a)
+        self.value("k", a["k"], k)
+        y = c.post["y"]
+        self.have_stats = False                 # the bf16 copy and statistics are S's
+        if self.fold and self.peek() == "rowstats_cast":
+            self.entry_cast(y)
+        return y
 
     def lpi(self, R: RefLayer, S: Tensor) -> Tensor:
         """y = S + LPI(S) (xcit.py:150-167, 208-211)."""
@@ -1052,7 +1390,7 @@ class Walk:
         if self.fold:
             self.same("y_bf16", c.post.get("y_bf16"), y.bfloat16())
             self.stats("y_stats", c.post["y_stats"], c.post["y_bf16"])
-            self.have_stats = True
+            self.have_stats, self.entry_stats = True, False
         else:
             self.same("y_bf16", a["y_bf16"], None)
         return y
@@ -1096,14 +1434,16 @@ def check_provenance(mod: nn.Module, x0: Tensor, kw: dict, launches: List[Launch
         R = refs[i]
         w.where = f"layer {i} qkv"
         if R.grid is not None:
-            o = w.grid_attention(R, S, i)
+            if R.ff_first:                                     # scalable_vit.py:316-317
+                S = w.feed_forward(R, S, i)
+                w.where = f"layer {i} qkv"
+            o, S = w.grid_attention(R, S, i)
             w.where = f"layer {i} out"
             S = w.residual(o, R.out, R.out_scale, S, copy=True, D=D)
-            w.where = f"layer {i} fc1"
-            act = None if R.ff_act == "gelu" else R.ff_act
-            h = w.normed(S, R.ln2, R.fc1[0], R.fc1[1], gelu=act is None, act=act)
-            w.where = f"layer {i} fc2"
-            S = w.residual(h, R.fc2, R.ff_scale, S, copy=True, D=D)
+            if not R.ff_first:
+                S = w.feed_forward(R, S, i)
+            if R.peg is not None:
+                S = w.peg(R.peg, S, i)
             continue
         head = None if R.qk is None else R.qk
         qkv = w.normed(S, R.ln1, R.qkv_w, None, head=head, heads=R.heads, dh=R.dim_head)

@@ -8,12 +8,11 @@ import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR
-from oracle.bounds import U, check, layernorm_reference
-from oracle.grid_attention_bounds import kv_reference, window_reference, window_rows
+from oracle.bounds import check, layernorm_reference
+from oracle.grid_attention_bounds import kv_reference, peg_reference, window_reference, window_rows
 from vit_pytorch_b200 import _lib
 
 sys.path.insert(0, GOLDEN_DIR)
@@ -158,18 +157,6 @@ def test_merge_patches_ln_within_bounds(p, gh, gw, C):
     check(out[:, :K], ref, bound, f"merge_patches_ln p={p} {gh}x{gw} C={C}")
     assert (out[:, K:] == 0).all(), "the K padding is not zero"
     assert torch.isnan(big[rows:].float()).all(), "rows past the output were written"
-
-
-def peg_reference(x, w, b, B, gh, gw, k):
-    """fp64 (ref, bound): conv2d plus the identity, and per element the fp32 error of k*k accumulated taps, the bias
-    and the residual add."""
-    C = x.shape[1]
-    grid = x.double().view(B, gh, gw, C).permute(0, 3, 1, 2)
-    wt = w.double().t().reshape(C, 1, k, k)
-    ref = F.conv2d(grid, wt, b.double(), padding=k // 2, groups=C) + grid
-    mag = F.conv2d(grid.abs(), wt.abs(), b.double().abs(), padding=k // 2, groups=C) + grid.abs()
-    ref, mag = (t.permute(0, 2, 3, 1).reshape(-1, C) for t in (ref, mag))
-    return ref, (k * k + 4) * U * mag + 1e-30
 
 
 @pytest.mark.parametrize("gh,gw", [(1, 1), (2, 5), (7, 7), (14, 9)])

@@ -1,15 +1,19 @@
 """The encoder layers that attend over a token grid traced back to their reference layers without a GPU
 (oracle/layer_trace.py, as tests/test_layer_trace.py does for the sequence families): Twins-SVT's local windows and
-strided keys, MaxViT's block and dilated windows under a relative-position bias, CvT's convolutional projections and
-MobileViT's patch groups with its SiLU feed-forward block.
+strided keys, MaxViT's block and dilated windows under a relative-position bias, CvT's convolutional projections,
+MobileViT's patch groups with its SiLU feed-forward block, ScalableViT's sub-sampled keys and interactive windows (its
+padded key heads, its feed-forward-first layers, and the PEG and entry prime between the run_blocks calls of
+Transformer.run_fused), SepViT's window tokens and window mixing, and RegionViT's region pass and region-to-local
+windows.
 
 Every case runs in both LayerNorm modes with per-LayerNorm eps (set_eps, the channel LayerNorms included) and
 BatchNorm eps 1e-3; the provenance walk must accept every launch and the emulated outputs must sit within their
 bounds.  Planted wiring and weight-preparation defects must be named by layer, launch and operand.
 
-The kernels' oracles (oracle/grid_attention_bounds.py) rebuild window membership and the bias look-up from the
-kernels' address formulas; the geometry tests here hold those formulas to the modules' own eager rearranges and bias
-look-ups, which the family parity tests hold to the reference's logits, on integer index maps."""
+The kernels' oracles (oracle/grid_attention_bounds.py) rebuild window membership, key patches and the bias look-up
+from the kernels' address formulas; the geometry tests here hold those formulas to the modules' own eager rearranges,
+convolutions and bias look-ups, which the family parity tests hold to the reference's logits, on integer index
+maps."""
 import copy
 import dataclasses
 
@@ -19,8 +23,10 @@ from torch import nn
 
 from oracle import grid_attention_bounds as GB
 from oracle import layer_trace as LT
-from test_layer_trace import lib, make, run  # noqa: F401  (lib: the module fixture that builds the library)
-from vit_pytorch_b200 import crossformer, cvt, engine, max_vit, mobile_vit, regionvit, twins_svt
+from test_layer_trace import lib, make  # noqa: F401  (lib: the module fixture that builds the library)
+from test_layer_trace import run as run_blocks_traced
+from vit_pytorch_b200 import (_lib, crossformer, cvt, engine, max_vit, mobile_vit, regionvit, scalable_vit, sep_vit,
+                              twins_svt)
 
 S = LT.schedule()
 D, B = S.D, 2
@@ -61,9 +67,30 @@ def _mobile():
     return mobile_vit.Transformer(D, 2, heads=2, dim_head=8, mlp_dim=2 * D)
 
 
+def _scalable(dk, r, window, dv=32, depth=1):
+    return lambda: scalable_vit.Transformer(D, depth, heads=2, ff_expansion_factor=2, ssa_dim_key=dk, ssa_dim_value=dv,
+                                            ssa_reduction_factor=r, iwsa_dim_key=dk, iwsa_dim_value=dv,
+                                            iwsa_window_size=window)
+
+
+def _sep(depth=1):
+    return lambda: sep_vit.Transformer(D, depth, dim_head=32, heads=2, ff_mult=2)
+
+
+def _region(W, depth=2):
+    return lambda: regionvit.R2LTransformer(D, window_size=W, depth=depth, heads=2)
+
+
 def _case(name, module, grid, primed=False, **kw):
     gh, gw = grid
     return S.Case(name, module, B * gh * gw, lambda: dict(B=B, N=gh * gw, grid=grid, primed=primed, **kw), False)
+
+
+def _region_case(name, module, grid, regions, b=B, primed=False):
+    """B local maps (the `grid`) followed by B region maps, in one stream."""
+    (lh, lw), (rh, rw) = grid, regions
+    return S.Case(name, module, b * (lh * lw + rh * rw),
+                  lambda: dict(B=b, N=lh * lw, grid=grid, regions=regions, primed=primed), False)
 
 
 CASES = [
@@ -82,7 +109,29 @@ CASES = [
     _case("cvt 2 heads k5 stride 3 on 4x6", _cvt(2, k=5, s=3), (4, 6)),
     _case("mobile_vit groups 2x2 on 4x6", _mobile, (4, 6), groups=(2, 2)),
     _case("mobile_vit groups 1x2 on 3x4 primed", _mobile, (3, 4), primed=True, groups=(1, 2)),
+    # dim_key 40 (run at 48) with value heads 64; 2 x 2 key patches of a 6 x 9 map (the last column dropped, as
+    # Conv2d); 3 x 3 windows; depth 2: the PEG and the entry prime between the first two layers
+    _case("scalable_vit dk40 dv64 reduction 2 window 3 on 6x9 depth 2", _scalable(40, 2, 3, dv=64, depth=2), (6, 9)),
+    _case("scalable_vit reduction 1 whole-map window on 4x6", _scalable(32, 1, None), (4, 6)),
+    # SepViT's windows are 7 x 7 (DSSA's default window_size)
+    _case("sep_vit 4 windows 2 heads on 14x14 depth 2", _sep(depth=2), (14, 14)),
+    _case("sep_vit single window on 7x7 primed", _sep(), (7, 7), primed=True),
+    _region_case("regionvit 4x4 windows on 8x8 / 2x2 depth 2", _region(4), (8, 8), (2, 2)),
+    _region_case("regionvit odd rows 3x5 / 1x1 primed", _region(5), (3, 5), (1, 1), b=3, primed=True),
+    _region_case("regionvit 2x3 windows on 4x6 / 2x2 primed", _region(3), (4, 6), (2, 2), primed=True),
 ]
+
+
+def _run_fused(mod, x, kw):
+    gh, gw = kw["grid"]
+    mod.run_fused(x, kw["B"], gh, gw)
+
+
+def run(case, ln_mode, plant=None):
+    """test_layer_trace.run; ScalableViT through its Transformer.run_fused: the first layer, the PEG and (fold) the
+    entry prime, the other layers."""
+    call = _run_fused if case.name.startswith("scalable_vit") else None
+    return run_blocks_traced(case, ln_mode, plant, call=call)
 
 
 def _named(name):
@@ -167,6 +216,105 @@ def _gelu_feed_forward(mp):
     mp.setattr(mobile_vit.Transformer, "encoder_layers", bad)
 
 
+def _iwsa_scale_padded(mp):
+    """The IWSA softmax scale from the padded key width (48) instead of dim_key (40)."""
+    orig = scalable_vit.Transformer.encoder_layers
+
+    def bad(self):
+        layers, norm = orig(self)
+        return [dataclasses.replace(L, scale=L.dim_head ** -0.5) if L.ff_first else L for L in layers], norm
+    mp.setattr(scalable_vit.Transformer, "encoder_layers", bad)
+
+
+def _lim_reads_k(mp):
+    """InteractiveWindows.launch with the LIM convolution's im2col over the k columns of qkv instead of the v."""
+    def bad(self, c, L, i):
+        t, (gh, gw), M = c.t, c.grid, c.x.shape[0]
+        Ik, dv = L.heads * L.dim_head, self.value_width(L)
+        Iv = L.heads * dv
+        qkv = engine._rows_of(c.qkv, L.qkv_w.shape[0])
+        c.project(L, i, out=qkv)
+        col = torch.empty(M, 9 * Iv, device=c.x.device, dtype=torch.bfloat16)
+        _lib.conv_im2col_nhwc(qkv[:, Ik:Ik + Iv], col, c.B, gh, gw, 3, 1, 1)
+        lim = torch.empty(M, Iv, device=c.x.device, dtype=torch.bfloat16)
+        _lib.gemm(col, t[f"{i}.lim.w"], out_bf16=lim, bias=t[f"{i}.lim.b"])
+        o = engine._rows_of(c.o, Iv)
+        wh, ww = self.window(c.grid)
+        _lib.attention_iwsa(qkv, lim, o, c.B, gh, gw, wh, ww, L.heads, L.dim_head, dv, L.scale)
+        return o
+    mp.setattr(engine.InteractiveWindows, "launch", bad)
+
+
+class _Without:
+    """The _lib module as a model file sees it, with one entry point replaced."""
+
+    def __init__(self, name, fn):
+        self.name, self.fn = name, fn
+
+    def __getattr__(self, name):
+        return self.fn if name == self.name else getattr(_lib, name)
+
+
+def _peg_prime_dropped(mp):
+    """run_fused without the rowstats_cast after the PEG: the second run_blocks call, primed, reads the bf16 copy and
+    statistics of the stream before the PEG."""
+    mp.setattr(scalable_vit, "_lib", _Without("rowstats_cast", lambda *a, **k: None))
+
+
+def _head_ln_default_eps(mp):
+    orig = sep_vit.Transformer.encoder_layers
+
+    def bad(self):
+        layers, norm = orig(self)
+        return [dataclasses.replace(L, attention=L.attention._replace(ln=L.attention.ln._replace(eps=1e-5)))
+                for L in layers], norm
+    mp.setattr(sep_vit.Transformer, "encoder_layers", bad)
+
+
+def _window_token_normalised(mp):
+    """The window token's q | k | v projected from the token after the layer's LayerNorm."""
+    orig = engine.WindowTokenBlock.prepare
+
+    def bad(self, t, i, L):
+        orig(self, t, i, L)
+        f = lambda p: p.detach().float()                                                # noqa: E731
+        tok = torch.nn.functional.layer_norm(f(self.token), self.token.shape, f(L.ln1.gamma), f(L.ln1.beta), L.ln1.eps)
+        t[f"{i}.tok_qkv"] = (L.qkv_w.detach().float() @ tok).to(torch.bfloat16)
+    mp.setattr(engine.WindowTokenBlock, "prepare", bad)
+
+
+def _wqk_blocked(mp):
+    """The window tokens' q | k rows as all heads' q, then all heads' k."""
+    orig = engine.WindowTokenBlock.prepare
+
+    def bad(self, t, i, L):
+        orig(self, t, i, L)
+        H, dh = L.heads, L.dim_head
+        w, b = t[f"{i}.wqk.w"], t[f"{i}.wqk.b"]
+        t[f"{i}.wqk.w"] = w.view(H, 2, dh, -1).transpose(0, 1).reshape(w.shape).contiguous()
+        t[f"{i}.wqk.b"] = b.view(H, 2, dh).transpose(0, 1).reshape(-1).contiguous()
+    mp.setattr(engine.WindowTokenBlock, "prepare", bad)
+
+
+def _region_residual_without_stats(mp):
+    """The region rows' out-projection residual (its fp32 stream a view at a row offset of x) writes no statistics."""
+    def gemm(*args, stats_out=None, resid=None, **kw):
+        if resid is not None and resid.storage_offset() > 0:
+            stats_out = None
+        return _lib.gemm(*args, stats_out=stats_out, resid=resid, **kw)
+    mp.setattr(engine, "_lib", _Without("gemm", gemm))
+
+
+def _r2l_table_reshaped(mp):
+    def bad(self, t, i, L):
+        t[f"{i}.r2l"] = self.bias.detach().float().reshape(self.bias.shape[1], -1).contiguous()
+    mp.setattr(engine.RegionLocalBlock, "prepare", bad)
+
+
+SCALABLE_A, SCALABLE_B = ("scalable_vit dk40 dv64 reduction 2 window 3 on 6x9 depth 2",
+                          "scalable_vit reduction 1 whole-map window on 4x6")
+SEP, REGION = "sep_vit 4 windows 2 heads on 14x14 depth 2", "regionvit 4x4 windows on 8x8 / 2x2 depth 2"
+
 # name: (case, LayerNorm mode, plant(monkeypatch), what the failure must name)
 DEFECTS = {
     "CvT BatchNorm folded with eps 1e-5 instead of the module's":
@@ -183,6 +331,22 @@ DEFECTS = {
          ("layer 0 attention", "attention_window_relpos", "operand table (dpb)")),
     "MobileViT feed-forward with GELU instead of SiLU":
         ("mobile_vit groups 2x2 on 4x6", "exact", _gelu_feed_forward, ("layer 0 fc1", "gemm_act expected")),
+    "IWSA scale from the padded key width":
+        (SCALABLE_A, "exact", _iwsa_scale_padded, ("layer 1 attention", "attention_iwsa", "operand scale")),
+    "LIM im2col over the k columns":
+        (SCALABLE_B, "fold", _lim_reads_k, ("layer 1 local interactive module", "conv_im2col_nhwc", "operand x")),
+    "no rowstats_cast after the PEG":
+        (SCALABLE_A, "fold", _peg_prime_dropped, ("layer 1 fc1", "gemm", "operand a")),
+    "SepViT head LayerNorm at the default eps":
+        (SEP, "fold", _head_ln_default_eps, ("layer 0 window tokens", "head_layernorm_gelu", "operand eps")),
+    "window token projected after the LayerNorm":
+        (SEP, "exact", _window_token_normalised, ("layer 0 attention", "attention_window_token", "operand tok_qkv")),
+    "window tokens' q | k rows blocked, not interleaved per head":
+        (SEP, "fold", _wqk_blocked, ("layer 0 window tokens", "gemm", "operand w")),
+    "region residual writes no statistics":
+        (REGION, "fold", _region_residual_without_stats, ("layer 1 region out", "gemm", "operand stats_out")),
+    "r2l table reshaped, not transposed":
+        (REGION, "exact", _r2l_table_reshaped, ("layer 0 attention", "attention_region_local", "operand table")),
 }
 
 
@@ -341,3 +505,96 @@ def test_region_local_bias_and_windows_are_the_modules(lh, lw, rh, rw, W):
     bias = GB.region_bias(t["0.r2l"], lh // rh, lw // rw, W)
     assert torch.equal(bias[None], cap.bias.double()), "the oracle's bias is not the module's"
     assert torch.equal(GB.region_window_rows(B, lh, lw, rh, rw, "cpu"), cap.tokens[..., 0].long())
+
+
+class _Ones(nn.Module):
+    def forward(self, t):
+        return torch.ones_like(t)
+
+
+@pytest.mark.parametrize("name", [SCALABLE_A, SCALABLE_B])
+def test_iwsa_windows_are_the_modules(name):
+    """GB.window_rows of each traced attention_iwsa launch (its wh x ww) is the window cut of
+    InteractiveWindowedSelfAttention.forward's windows() (scalable_vit.py:180-187) on the index map, seen in its
+    scores with q the map, k ones and scale 1: score (i, j) of window w is the map row of its token i."""
+    mod, _, kw, launches = run(_named(name), "exact")
+    gh, gw = kw["grid"]
+    iwsa = [c for c in launches if c.name == "attention_iwsa"]
+    assert len(iwsa) == len(mod.layers) > 0
+    for c, layer in zip(iwsa, mod.layers):
+        a = copy.deepcopy(layer[4])
+        a.norm, a.to_q, a.to_k, a.to_v, a.local_interactive_module = (nn.Identity(), nn.Identity(), _Ones(),
+                                                                       nn.Identity(), nn.Identity())
+        a.scale, a.attend = 1.0, _Capture()
+        with torch.no_grad(), pytest.raises(_Captured):
+            a(_index_map(gh, gw).expand(-1, a.heads, -1, -1))
+        got = a.attend.seen[:, 0, :, 0].long()                            # (b x y), heads, w1 w2, w1 w2
+        assert torch.equal(GB.window_rows(B, gh, gw, c.pre["wh"], c.pre["ww"], "cpu"), got), \
+            f"{name}: the oracle's windows are not the module's"
+
+
+def check_ssa_key_patches(mod, kw, launches):
+    """The key / value operands the walk derives for each SSA -- GB.im2col_reference of the traced key-patch
+    conv_im2col_nhwc launch (the oracle of that kernel's addresses) times the module's to_k (heads padded) | to_v
+    weights in tap order -- are to_k's and to_v's own Conv2d of the map (scalable_vit.py:127-128, 138), exactly, on an
+    integer map (the weights are multiples of 1/64: every sum is exact in fp64)."""
+    gh, gw = kw["grid"]
+    patches = [c for c in launches if c.name == "conv_im2col_nhwc" and c.pre["p"] == 0]
+    refs = [R for R in LT.module_layers(mod) if R.grid["kind"] == "strided"]
+    assert len(patches) == len(refs) == len(mod.layers) > 0
+    x = torch.randint(-8, 9, (B * gh * gw, D), generator=torch.Generator().manual_seed(1)).double()
+    xm = x.view(B, gh, gw, D).permute(0, 3, 1, 2)
+    for c, R, (ssa, *_rest) in zip(patches, refs, mod.layers):
+        a = c.pre
+        col = GB.im2col_reference(x, a["B"], a["H"], a["W"], a["k"], a["s"], a["p"])
+        kvw = R.grid["kv"].double()
+        got = col @ kvw.permute(0, 2, 3, 1).reshape(kvw.shape[0], -1).t()
+        H, dk, dp = ssa.heads, ssa.to_q.out_channels // ssa.heads, R.dim_head
+        with torch.no_grad():
+            k, v = (copy.deepcopy(m).double()(xm).permute(0, 2, 3, 1).reshape(got.shape[0], -1)
+                    for m in (ssa.to_k, ssa.to_v))
+        heads = got[:, :H * dp].reshape(-1, H, dp)
+        assert torch.equal(heads[..., :dk].reshape(-1, H * dk), k), "the oracle's key patches are not to_k's"
+        assert (heads[..., dk:] == 0).all(), "a padded key column is not zero"
+        assert torch.equal(got[:, H * dp:], v), "the oracle's key patches are not to_v's"
+
+
+def test_ssa_key_patches_are_the_modules_convolutions():
+    mod, _, kw, launches = run(_named(SCALABLE_A), "exact")
+    check_ssa_key_patches(mod, kw, launches)
+
+
+def _im2col_channel_major(x, B, H, W, k, s, pad):
+    """im2col with its columns in (channel, tap row, tap column) order, the Conv2d weight's own."""
+    C = x.shape[1]
+    cols = torch.nn.functional.unfold(x.reshape(B, H, W, C).permute(0, 3, 1, 2).double(), k, padding=pad, stride=s)
+    return cols.permute(0, 2, 1).reshape(-1, C * k * k)
+
+
+def test_oracle_side_key_patch_defect_is_flagged(monkeypatch):
+    mod, _, kw, launches = run(_named(SCALABLE_A), "exact")
+    monkeypatch.setattr(GB, "im2col_reference", _im2col_channel_major)
+    with pytest.raises(AssertionError, match="the oracle's key patches are not to_k's"):
+        check_ssa_key_patches(mod, kw, launches)
+
+
+@pytest.mark.parametrize("name", [SEP, "sep_vit single window on 7x7 primed"])
+def test_sep_vit_windows_are_the_modules(name):
+    """GB.window_rows of each traced attention_window_token launch -- the windows, and their order, that its oracle
+    (window_token_reference) and window_mix's (mix_reference) read -- is DSSA.forward's window cut and window order
+    with the window token first (sep_vit.py:178-184), seen at the input of its to_qkv on the index map."""
+    mod, _, kw, launches = run(_named(name), "exact")
+    gh, gw = kw["grid"]
+    wt = [c for c in launches if c.name == "attention_window_token"]
+    assert len(wt) == len(mod.layers) > 0
+    for c, (attn, _ff) in zip(wt, mod.layers):
+        a = copy.deepcopy(attn)
+        a.norm, a.to_qkv = nn.Identity(), _Capture()
+        a.window_tokens = nn.Parameter(torch.full((1,), -1.0, dtype=torch.float64))
+        with torch.no_grad(), pytest.raises(_Captured):
+            a(_index_map(gh, gw))
+        seen = a.to_qkv.seen                                                   # (b x y), 1, 1 + w1 w2
+        p = c.pre["p"]
+        assert (seen[:, 0, 0] == -1).all(), f"{name}: the window token is not each window's first token"
+        assert torch.equal(GB.window_rows(B, gh, gw, p, p, "cpu"), seen[:, 0, 1:].long()), \
+            f"{name}: the oracle's windows are not the module's"

@@ -75,9 +75,9 @@ def make(case):
     return mod
 
 
-def run(case, ln_mode, plant=None):
+def run(case, ln_mode, plant=None, call=None):
     """(module, x before run_blocks, run_blocks' arguments, traced launches) of one emulated run; plant(mod, eng) runs
-    before it."""
+    before it; call(mod, x, kw) in place of eng.run_blocks(x, **kw) (LT.trace)."""
     mod = make(case)
     eng = mod.engine()
     if plant is not None:
@@ -85,7 +85,8 @@ def run(case, ln_mode, plant=None):
     x = torch.randn(case.rows, S.D, generator=torch.Generator().manual_seed(len(case.name)))
     kw = case.kwargs()
     x0 = x.clone()
-    launches = LT.trace(eng, x, kw, ln_mode, LT.emulate_impl, prime=LT.prime_exact)
+    launches = LT.trace(eng, x, kw, ln_mode, LT.emulate_impl, prime=LT.prime_exact,
+                        call=None if call is None else lambda: call(mod, x, kw))
     return mod, x0, kw, launches
 
 
