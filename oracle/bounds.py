@@ -55,15 +55,17 @@ U_BF16 = 2.0 ** -8      # largest relative rounding error of a bf16 result (half
 C_ACC = 0.25
 GELU_SLOPE = 1.13
 GELU_ABS = 1.2e-5
+HARDSWISH_SLOPE = 1.5
 
 
 def gemm_reference(a: Tensor, w: Tensor, *, bias: Optional[Tensor] = None, resid: Optional[Tensor] = None,
                    ln_sums: Optional[Tensor] = None, col_s: Optional[Tensor] = None, ln_eps: float = 1e-5,
-                   gelu: bool = False, bf16_out: bool = False) -> Tuple[Tensor, Tensor]:
+                   gelu: bool = False, hardswish: bool = False, bf16_out: bool = False) -> Tuple[Tensor, Tensor]:
     """(ref, bound) of epilogue(a[m, K] @ w[N, K]^T) as b200vit_gemm_bf16 computes it.
 
     a, w: the bf16 operands (K = a.shape[1] exactly: slice off any row padding first).  ln_sums: [m, parts, 2] or
-    [m, 2] fp32 partial row sums; resid: [m, N] fp32.  bf16_out: bound the bf16 output instead of the fp32 one."""
+    [m, 2] fp32 partial row sums; resid: [m, N] fp32.  hardswish: EPI_HARDSWISH, y clamp(y + 3, 0, 6) / 6 (slope at
+    most 1.5, then its add, clamp, product and division).  bf16_out: bound the bf16 output instead of the fp32 one."""
     a64, w64 = a.double(), w.double()
     K = a.shape[1]
     acc = a64 @ w64.t()
@@ -99,6 +101,9 @@ def gemm_reference(a: Tensor, w: Tensor, *, bias: Optional[Tensor] = None, resid
     if gelu:
         ref = 0.5 * ref * (1.0 + torch.erf(ref / math.sqrt(2.0)))
         e = GELU_SLOPE * e + GELU_ABS + 4 * U * ref.abs()
+    if hardswish:
+        ref = ref * (ref + 3).clamp(0, 6) / 6
+        e = HARDSWISH_SLOPE * e + 4 * U * ref.abs() + 1e-30
     if resid is not None:
         ref = ref + resid.double()
         e = e + U * (ref.abs() + e)

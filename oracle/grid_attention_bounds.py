@@ -1,8 +1,9 @@
 """fp64 references with a per-element error bound for the attention kernels over token grids and the kernels around
 them: windows (Twins-SVT, MaxViT, CrossFormer), sub-sampled keys (Twins-SVT, CvT, ScalableViT), interactive windows
 (ScalableViT), patch groups (MobileViT), the depthwise convolutional projection (CvT), window tokens and window mixing
-(SepViT), region-to-local windows (RegionViT), the positional encoding generator (Twins-SVT, ScalableViT), and the
-SiLU GEMM epilogue and the head LayerNorm + GELU  --  TEST INFRASTRUCTURE.
+(SepViT), region-to-local windows (RegionViT), the position-bias attention of LeViT, the positional encoding generator
+(Twins-SVT, ScalableViT), the im2col gathers, and the SiLU GEMM epilogue and the head LayerNorm + GELU  --  TEST
+INFRASTRUCTURE.
 
 Every reference returns `(ref, bound)`: fp64 tensors on the device of its inputs, to be checked with
 oracle.bounds.check.  The attention references gather each window's rows and hand them to
@@ -10,8 +11,8 @@ oracle.attention_bounds.attention_reference, whose bound models the bf16 probabi
 the relative-position ones add the bias inside the score and bound it as the position-bias attention of LeViT.
 
 The row maps (`window_rows`, `group_rows`, `region_window_rows`) and the bias index maps (`relpos_index`,
-`region_bias_index`) are the kernels' address formulas; tests/test_grid_layer_trace.py ties each of them to the
-reference module's own rearranges and bias look-ups."""
+`region_bias_index`, `posbias_index`) are the kernels' address formulas; tests/test_grid_layer_trace.py and
+tests/test_class_layer_trace.py tie each of them to the reference module's own rearranges and bias look-ups."""
 from __future__ import annotations
 
 import math
@@ -329,6 +330,54 @@ def im2col_reference(x: Tensor, B: int, H: int, W: int, k: int, s: int, pad: int
     cols = F.unfold(xi, k, padding=pad, stride=s)                          # B, C k k, L: columns (c, ky, kx)
     L = cols.shape[-1]
     return cols.view(B, C, k * k, L).permute(0, 3, 2, 1).reshape(B * L, k * k * C)
+
+
+def im2col_nchw_reference(img: Tensor, k: int, s: int, pad: int) -> Tensor:
+    """b200vit_conv_im2col_nchw, exactly: F.unfold(img, k, padding=pad, stride=s) of the NCHW image [B, C, H, W], one
+    row per output position, columns (channel, tap row, tap column)."""
+    cols = F.unfold(img.double(), k, padding=pad, stride=s)               # B, C k k, L
+    return cols.transpose(1, 2).reshape(-1, cols.shape[1])
+
+
+def posbias_index(F_: int, s: int, device=None) -> Tensor:
+    """int64 [ceil(F / s)^2, F^2]: the bias-table column b200vit_attention_posbias adds to query (i, j) and key
+    (y, x) of an F x F map, the query at map position (s i, s j): |s i - y| F + |s j - x|."""
+    qy, qx = torch.meshgrid(torch.arange(0, F_, s, device=device), torch.arange(0, F_, s, device=device), indexing="ij")
+    ky, kx = torch.meshgrid(torch.arange(F_, device=device), torch.arange(F_, device=device), indexing="ij")
+    return (qy.reshape(-1, 1) - ky.reshape(1, -1)).abs() * F_ + (qx.reshape(-1, 1) - kx.reshape(1, -1)).abs()
+
+
+def posbias_reference(qkv: Tensor, table: Tensor, B: int, F_: int, s: int, H: int, dk: int, dv: int, scale: float,
+                      gelu: bool = True) -> Tuple[Tensor, Tensor]:
+    """fp64 (ref, bound) of b200vit_attention_posbias (LeViT, levit.py:133-158) on the kernel's own bf16 inputs.  The
+    bound counts: the bf16 rounding of the probabilities before P V (2^-8 relative per key, against sum_j p_j |v_j|),
+    the score error (the fp32 dot products, C_ACC dk u sum |q||k| scaled, and the rounding of the scale, the bias and
+    their sum: a relative change of the probabilities by e^(2 dx)), fp32 accumulation of P V and of l, then GELU
+    (slope at most 1.13) and the output's bf16 rounding."""
+    Fq = -(-F_ // s)
+    x = qkv.double()[:B * F_ * F_].view(B, F_, F_, -1)
+    q = x[:, ::s, ::s, :H * dk].reshape(B, Fq * Fq, H, dk).transpose(1, 2)
+    k = x[..., H * dk:2 * H * dk].reshape(B, F_ * F_, H, dk).transpose(1, 2)
+    v = x[..., 2 * H * dk:2 * H * dk + H * dv].reshape(B, F_ * F_, H, dv).transpose(1, 2)
+    bias = table.double()[:, posbias_index(F_, s, qkv.device)]                       # H, Nq, Nk
+    sc = float(torch.tensor(scale, dtype=torch.float32))
+    logits = sc * q @ k.transpose(-1, -2) + bias
+    p = logits.softmax(-1)
+    out = p @ v
+    mag = p @ v.abs()                                                                  # sum_j p_j |v_j|
+    dx = (C_ACC * dk + 4) * U * sc * (q.abs() @ k.abs().transpose(-1, -2)) + 4 * U * (bias.abs() + logits.abs())
+    dxm = dx.amax(-1, keepdim=True)
+    nk = F_ * F_
+    e_attn = (2.0 ** -8 + 4 * dxm + (C_ACC * nk + nk / 4 + 16) * U) * mag
+    e_attn = e_attn + 3 * U * out.abs()
+    if gelu:
+        ref = torch.nn.functional.gelu(out)
+        e = 1.13 * e_attn + 1e-6 * (ref.abs() + e_attn) + 1e-30
+    else:
+        ref, e = out, e_attn
+    bound = e + bf16_ulp(ref.abs() + e) / 2
+    back = lambda t: t.transpose(1, 2).reshape(B * Fq * Fq, H * dv)                   # noqa: E731
+    return back(ref), back(bound)
 
 
 # ------------------------------------------------------------------------------------------------------ epilogues

@@ -20,7 +20,13 @@ list of tests/golden/make_engine_schedule.py; a launch is kept with its argument
 taken before the call and a clone of every tensor it writes taken after it (the workspace buffers are overwritten
 within a layer).  The clones go on the current stream.  `impl` runs a launch: the real kernels on the GPU, or
 `emulate`, which writes the fp64 reference of `expected` rounded to the output's dtype, on a machine without one.  The
-trace runs the per-kernel Python loop; the one-call C loop must be bit-identical to it."""
+trace runs the per-kernel Python loop; the one-call C loop must be bit-identical to it.
+
+The encoders that run outside a single run_blocks call are traced through their drivers (`trace_call`) and walked by
+their own checks: CrossViT's two streams (`check_cross_vit_provenance`: each branch's layers, its final LayerNorm,
+both class-attention directions), CaiT's and XCiT's forward_fused after the patch embedding
+(`check_class_stage_provenance`: the patch encoder, the context, one CrossAttentionEngine.run against
+`cross_module_layers`, the head), and LeViT's whole forward_fused (`check_levit_provenance`)."""
 from __future__ import annotations
 
 import dataclasses
@@ -73,6 +79,13 @@ OUTPUTS = {
     "window_mix": ("out",),
     "attention_region_local": ("out",),
     "peg": ("y",),
+    "attention_cls": ("out",),
+    "attention_cls_headmix": ("out",),
+    "attention_posbias": ("out",),
+    "gemm_hardswish": ("out_bf16",),
+    "mean_pool": ("out",),
+    "cast_f32_bf16": ("out",),
+    "conv_im2col_nchw": ("out_bf16",),
 }
 # the entry points of the attention records on token grids (engine.Windows, StridedKV, InteractiveWindows, ConvProj,
 # PatchGroups, WindowTokenBlock, RegionLocalBlock), of the SiLU feed-forward block and of ScalableViT's positional
@@ -80,6 +93,9 @@ OUTPUTS = {
 GRID_ENTRY_POINTS = ("gemm_act", "conv_im2col_nhwc", "attention_window", "attention_window_relpos", "attention_kv",
                      "attention_groups", "conv_proj_dw", "attention_kv_ex", "attention_iwsa", "attention_window_token",
                      "head_layernorm_gelu", "window_mix", "attention_region_local", "peg")
+# the entry points of the class-token cross attention (engine.CrossAttentionEngine) and of LeViT's forward_fused
+CLASS_ENTRY_POINTS = ("attention_cls", "attention_cls_headmix", "attention_posbias", "gemm_hardswish", "mean_pool",
+                      "conv_im2col_nchw")
 
 
 def schedule():
@@ -140,7 +156,9 @@ def real_impl(name: str, real: Callable) -> Callable:
 
 
 def emulate_impl(name: str, real: Callable) -> Callable:
-    """The launch emulated: its outputs get the fp64 reference of `expected`, rounded to their dtype."""
+    """The launch emulated: its outputs get the fp64 reference of `expected`, rounded to their dtype.  An output that
+    the reference on these operands does not fit (a wrong map size or stride passed with the right buffers) is
+    written as NaN, so that the provenance walk, not the emulation, names the operand."""
     def run(**a):
         if name not in OUTPUTS:
             raise NotImplementedError(f"no emulation of _lib.{name}")
@@ -148,7 +166,10 @@ def emulate_impl(name: str, real: Callable) -> Callable:
         got: Dict[str, Tensor] = {}
 
         def written(k, v):                        # expected() reads earlier outputs through `got`
-            a[k].copy_(v.reshape(a[k].shape).to(a[k].dtype))
+            if v.numel() != a[k].numel():
+                a[k].fill_(math.nan)
+            else:
+                a[k].copy_(v.reshape(a[k].shape).to(a[k].dtype))
             got[k] = a[k].detach().clone()
         expected(name, pre, got, on_output=written)
     return run
@@ -266,6 +287,33 @@ def expected(name: str, a: dict, got: dict, on_output: Optional[Callable] = None
             put("out_bf16", (y, Bd.bf16_bound(y, e)))
         if a["stats_out"] is not None:
             put("stats_out", _stats(got["out_bf16"], a["stats_out"]))
+        return out
+    if name == "gemm_hardswish":
+        put("out_bf16", Bd.gemm_reference(a["a"], a["w"], bias=a["bias"], hardswish=True, bf16_out=True))
+        return out
+    if name == "conv_im2col_nchw":
+        col = GB.im2col_nchw_reference(a["img"], a["k"], a["s"], a["p"])
+        put("out_bf16", _exact(torch.nn.functional.pad(col, (0, a["out_bf16"].shape[1] - col.shape[1]))))
+        return out
+    if name == "attention_cls":
+        put("out", FB.cls_reference(a["qkv_self"], a["ctx"], a["rows_per_image"], a["first"], a["n"], a["H"], a["dh"],
+                                    a["scale"]))
+        return out
+    if name == "attention_cls_headmix":
+        put("out", FB.cls_headmix_reference(a["qkv_self"], a["ctx"], a["rows_per_image"], a["first"], a["n"], a["H"],
+                                            a["dh"], a["scale"], a["pre"], a["post"]))
+        return out
+    if name == "attention_posbias":
+        put("out", GB.posbias_reference(a["qkv"], a["table"], a["B"], a["F"], a["s"], a["H"], a["dk"], a["dv"],
+                                        a["scale"], gelu=a["gelu_out"]))
+        return out
+    if name == "mean_pool":
+        B, N, D = a["B"], a["N"], a["D"]
+        put("out", RB.mean_pool_reference(a["x"].reshape(-1)[:B * N * D].view(B, N, D),
+                                          N if a["n_pool"] is None else a["n_pool"]))
+        return out
+    if name == "cast_f32_bf16":
+        put("out", _exact(a["x"].bfloat16()))
         return out
     if name == "conv_im2col_nhwc":
         col = GB.im2col_reference(a["x"], a["B"], a["H"], a["W"], a["k"], a["s"], a["p"])
@@ -528,9 +576,10 @@ def _scalable_layers(mod: nn.Module) -> List[RefLayer]:
 
 def module_layers(mod: nn.Module) -> List[RefLayer]:
     """The layers of a reference Transformer, by family (the module's class)."""
-    from vit_pytorch_b200 import (cait, cct, crossformer, cvt, deepvit, max_vit, mobile_vit, na_vit,
-                                  na_vit_nested_tensor, regionvit, scalable_vit, sep_vit, simple_vit_with_qk_norm,
-                                  twins_svt, vit, vit_for_small_dataset, vit_nd_rotary, vivit, xcit)
+    from vit_pytorch_b200 import (cait, cct, cross_vit, crossformer, cvt, deepvit, max_vit, mobile_vit, na_vit,
+                                  na_vit_nested_tensor, nest, pit, regionvit, scalable_vit, sep_vit,
+                                  simple_flash_attn_vit, simple_vit, simple_vit_with_qk_norm, twins_svt, vit,
+                                  vit_for_small_dataset, vit_nd_rotary, vivit, xcit)
     t = type(mod)
     if t is scalable_vit.Transformer:
         return _scalable_layers(mod)
@@ -593,8 +642,20 @@ def module_layers(mod: nn.Module) -> List[RefLayer]:
         return out
     if t is mobile_vit.Transformer:                                         # mobile_vit.py:79-96, FeedForward :28-34
         return [dataclasses.replace(_plain(a, ff, grid=dict(kind="groups")), ff_act="silu") for a, ff in mod.layers]
-    if t is vit.Transformer:                                                # vit.py:66-83
+    if t is vit.Transformer or t is pit.Transformer:                        # vit.py:66-83, pit.py:69-82
         return [_plain(attn, ff) for attn, ff in mod.layers]
+    if t is simple_vit.Transformer or t is simple_flash_attn_vit.Transformer:
+        # simple_vit.py:32-77, simple_flash_attn_vit.py:36-66: to_out a Linear without bias
+        return [_plain(attn, ff) for attn, ff in mod.layers]
+    if t is cross_vit.Transformer:                                          # cross_vit.py:34-90: to_q | to_kv
+        return [_plain(attn, ff, qkv_w=torch.cat([attn.to_q.weight, attn.to_kv.weight]), cat=("qkv_w",))
+                for attn, ff in mod.layers]
+    if t is nest.Transformer:                                               # nest.py:84-104: 1 x 1 convs on NCHW
+        out = []
+        for attn, ff in mod.layers:
+            I, D = attn.to_qkv.out_channels // 3, attn.to_qkv.in_channels
+            out.append(_conv_layer(attn, ff.net, attn.to_qkv.weight.reshape(3 * I, D), None))
+        return out
     if t is vit_nd_rotary.Transformer:                                      # vit_nd_rotary.py:115-156: to_qk | to_v
         return [_plain(attn, ff, qkv_w=torch.cat([attn.to_qk.weight, attn.to_v.weight]), cat=("qkv_w",))
                 for attn, ff in mod.layers]
@@ -819,18 +880,24 @@ def dpb_table_reference(attn: nn.Module) -> Tuple[Tensor, Tensor]:
     return v[:n, None].expand(-1, attn.heads), e[:n, None].expand(-1, attn.heads)
 
 
-def _bn_folded(conv: nn.Conv2d, bn: nn.BatchNorm2d):
-    """((w, bound), (b, bound)) fp64 of a bias-free depthwise convolution with the BatchNorm (eval) after it folded in,
-    tap-major [k k, C] (cvt.py:51-60): w' = w g / sqrt(var + eps), b' = beta - mean g / sqrt(var + eps), recomputed
-    from the module's parameters and its eps; the bound is the fp32 rounding the host's fold may add: 5 u for w'
-    (the sum, sqrt, quotient and product), 5 u |mean inv| + u (|b'| + |beta|) for b'."""
+def _bn_folded(conv: nn.Conv2d, bn: nn.BatchNorm2d, tap_major: bool = True, bf16: bool = False):
+    """((w, bound), (b, bound)) fp64 of a convolution with the BatchNorm (eval) after it folded in, recomputed from the
+    module's parameters and its eps: w' = w g / sqrt(var + eps), b' = (b - mean) g / sqrt(var + eps) + beta, b the
+    convolution's bias (0 without one).  w' [out, in k k], or tap_major [k k, out] (CvT's bias-free depthwise
+    convolutions, cvt.py:51-60); LeViT's 1 x 1 convolutions take [out, in] (levit.py:92-108).  The bound is the fp32
+    rounding the host's fold may add: 5 u for w' (the sum, sqrt, quotient and product), 5 u |(b - mean) inv| (6 u with
+    the bias's subtraction) + u (|b'| + |beta|) for b'; bf16: w' then rounded to bf16."""
     d = lambda t: t.detach().double()                                                   # noqa: E731
     C = conv.weight.shape[0]
     inv = d(bn.weight) / torch.sqrt(d(bn.running_var) + f32(bn.eps))
-    w = (d(conv.weight).reshape(C, -1) * inv[:, None]).t()
-    mi = d(bn.running_mean) * inv
-    b = d(bn.bias) - mi
-    return (w, 5 * U * w.abs()), (b, 5 * U * mi.abs() + U * (b.abs() + d(bn.bias).abs()))
+    w = d(conv.weight).reshape(C, -1) * inv[:, None]
+    if tap_major:
+        w = w.t()
+    cb = (d(conv.bias) if conv.bias is not None else torch.zeros_like(inv)) - d(bn.running_mean)
+    b = cb * inv + d(bn.bias)
+    wb = 5 * U * w.abs()
+    return ((w, Bd.bf16_bound(w, wb) if bf16 else wb),
+            (b, (6 if conv.bias is not None else 5) * U * (cb * inv).abs() + U * (b.abs() + d(bn.bias).abs())))
 
 
 class ProvenanceError(AssertionError):
@@ -1069,17 +1136,47 @@ class Walk:
         self.same("out_f32", a["out_f32"], None)
         return c.post["out_bf16"]
 
-    def plain_gemm(self, A: Tensor, W: Tensor, b: Optional[Tensor] = None) -> Tensor:
-        """A W^T + b and no LayerNorm: a 1 x 1 convolution on a bf16 map, or a convolution on its im2col."""
+    def plain_gemm(self, A: Tensor, W: Tensor, b: Optional[Tensor] = None, gelu: bool = False) -> Tensor:
+        """[GELU](A W^T + b) and no LayerNorm: a 1 x 1 convolution on a bf16 map, or a convolution on its im2col."""
+        return self.prepared_gemm(A, W.detach().bfloat16(), None if b is None else b.detach().float(), gelu)
+
+    def prepared_gemm(self, A: Tensor, W: Tensor, b: Optional[Tensor], gelu: bool = False, what: str = "w",
+                      stats: bool = False) -> Tensor:
+        """[GELU](A W^T + b) into a bf16 output alone, W and b as prepared (bf16, fp32), no LayerNorm and no residual;
+        stats: with the row statistics of that output (a LayerNorm-folded GEMM reads them next)."""
         c = self.take("gemm")
         a = c.pre
         self.same("a", a["a"], A)
-        self.same("w", a["w"], W.detach().bfloat16())
-        self.same("bias", a["bias"], None if b is None else b.detach().float())
-        for op in ("resid", "ln_sums", "out_f32", "stats_out"):
+        self.same(what, a["w"], W)
+        self.same("bias", a["bias"], b)
+        for op in ("resid", "ln_sums", "out_f32"):
+            self.same(op, a[op], None)
+        self.value("gelu", a["gelu"], gelu)
+        if not stats:
+            self.same("stats_out", a["stats_out"], None)
+        elif a["stats_out"] is None:
+            self.fail("stats_out", "the row statistics the folded GEMM reads are not written")
+        else:
+            self.stats("stats_out", c.post["stats_out"], c.post["out_bf16"])
+        return c.post["out_bf16"]
+
+    def written_residual(self, A: Tensor, W: Tensor, b: Optional[Tensor], resid: Tensor) -> Tensor:
+        """resid + A W^T + b with the prepared W (bf16) and b (fp32), written in fp32 and as its bf16 copy, with no row
+        statistics (the cls rows of CrossAttentionEngine's stream A, LeViT's stream): the new fp32 rows."""
+        c = self.take("gemm")
+        a = c.pre
+        self.same("a", a["a"], A)
+        self.same("w", a["w"], W)
+        self.same("bias", a["bias"], b)
+        self.same("resid", a["resid"], resid)
+        for op in ("ln_sums", "stats_out"):
             self.same(op, a[op], None)
         self.value("gelu", a["gelu"], False)
-        return c.post["out_bf16"]
+        if a["out_f32"] is None or a["out_bf16"] is None:
+            self.fail("out_f32", "the cls rows and their bf16 copy are not both written")
+        new = c.post["out_f32"]
+        self.same("out_bf16", c.post["out_bf16"], new.bfloat16())
+        return new
 
     def grid_geometry(self, a: dict, B: bool = True) -> None:
         gh, gw = self.kw["grid"]
@@ -1417,15 +1514,12 @@ class Walk:
         return y, c.post["out_bf16"]
 
 
-def check_provenance(mod: nn.Module, x0: Tensor, kw: dict, launches: List[Launch], ln_mode: str,
-                     case: str = "") -> int:
-    """Walk the trace of run_blocks(x0, **kw) through the layers of the reference module `mod` in its forward's
-    order (reference vit.py:78-81 and the family lines cited in module_layers) and assert every launch received what
-    that forward defines.  Returns the number of launches checked; raises ProvenanceError naming the case, the layer,
-    the launch, the operand and the first differing element."""
-    check_identity(mod, case)
+def walk_blocks(w: Walk, mod: nn.Module, x0: Tensor) -> Tensor:
+    """The launches of one run_blocks(x0, **w.kw) call on the layers of `mod`, from w.pos on, walked in the reference
+    forward's order (reference vit.py:78-81 and the family lines cited in module_layers); returns the fp32 stream the
+    last launch wrote (x0 when no layer runs)."""
+    kw = w.kw
     refs = module_layers(mod)
-    w = Walk(case, launches, ln_mode == "fold", kw)
     S = x0
     M, D = x0.shape
     rope = kw.get("rope")
@@ -1480,8 +1574,436 @@ def check_provenance(mod: nn.Module, x0: Tensor, kw: dict, launches: List[Launch
             h = w.normed(Y, R.ln2, R.fc1[0], R.fc1[1], gelu=True)
         w.where = f"layer {i} fc2"
         S = w.residual(h, R.fc2, R.ff_scale, Y, copy=True, D=D)
-    if w.pos != len(launches):
-        w.where, w.cur = "after the last layer", launches[w.pos]
+    return S
+
+
+def _end(w: Walk) -> int:
+    """Every launch walked: the number of launches; else a failure naming the first one left."""
+    if w.pos != len(w.calls):
+        w.where, w.cur = "after the last layer", w.calls[w.pos]
         w.pos += 1
         w.fail("-", "a launch the reference forward does not define")
     return w.pos
+
+
+def check_provenance(mod: nn.Module, x0: Tensor, kw: dict, launches: List[Launch], ln_mode: str,
+                     case: str = "") -> int:
+    """Walk the trace of run_blocks(x0, **kw) through the layers of the reference module `mod` in its forward's
+    order (walk_blocks) and assert every launch received what that forward defines.  Returns the number of launches
+    checked; raises ProvenanceError naming the case, the layer, the launch, the operand and the first differing
+    element."""
+    check_identity(mod, case)
+    w = Walk(case, launches, ln_mode == "fold", kw)
+    walk_blocks(w, mod, x0)
+    return _end(w)
+
+
+# ------------------------------------------------------------------------------------------------------ class attention
+def trace_call(call: Callable[[], object], ln_mode: str, impl=real_impl, setup: Optional[Callable[[], None]] = None
+               ) -> List[Launch]:
+    """Run call() -- a driver of several engines' launches: CrossViT's fused_two_streams, a CrossAttentionEngine.run,
+    LeViT.forward_fused -- in `ln_mode` with every launch traced; setup() first, inside the tracing (it fills the
+    workspaces the call will use with NaN)."""
+    S = schedule()
+    with S.recording(None, lambda: [], ln_mode, "python", extra_entry_points=GRID_ENTRY_POINTS + CLASS_ENTRY_POINTS,
+                     recorder=tracer(impl)) as rec:
+        if setup is not None:
+            setup()
+        call()
+    return rec.launches
+
+
+@dataclass
+class RefCross:
+    """One class-attention layer of a reference module (CrossLayer's reference), read through its own attribute
+    paths: the cls rows of stream A attend to [LN(project_in(cls)); context rows of stream B]."""
+    proj_in: Optional[nn.Linear]
+    ln: Ln
+    q_w: Tensor
+    kv_w: Tensor
+    out: Tuple[Tensor, Optional[Tensor]]
+    proj_out: Optional[nn.Linear]
+    heads: int
+    dim_head: int
+    scale: float
+    skip: int                                     # leading rows of each image of B that are not context
+    talking: Optional[Tuple[Tensor, Tensor]] = None          # (pre, post), [input head, output head]
+    out_scale: Optional[Tensor] = None
+    ff: Optional[Tuple[Ln, nn.Linear, nn.Linear]] = None
+    ff_scale: Optional[Tensor] = None
+
+
+def cross_module_layers(mod: nn.Module, direction: int = 0) -> List[RefCross]:
+    """The class-attention layers of a reference module, by family: CrossViT's CrossTransformer (direction 0: sm cls
+    attends to lg, 1: lg cls attends to sm), CaiT's and XCiT's class-attention Transformer."""
+    from vit_pytorch_b200 import cait, cross_vit, xcit
+    t = type(mod)
+    out = []
+    if t is cross_vit.CrossTransformer:                     # cross_vit.py:94-130: context = the patch rows t[:, 1:]
+        for layer in mod.layers:
+            pio = layer[direction]
+            a = pio.fn
+            pin = None if isinstance(pio.project_in, nn.Identity) else pio.project_in
+            pout = None if isinstance(pio.project_out, nn.Identity) else pio.project_out
+            out.append(RefCross(pin, _ln(a.norm), a.to_q.weight, a.to_kv.weight, (a.to_out[0].weight, a.to_out[0].bias),
+                                pout, a.heads, a.dim_head, float(a.scale), skip=1))
+        return out
+    if t is cait.Transformer or t is xcit.Transformer:      # cait.py:61-122, xcit.py:72-107, 169-189: every row
+        for ls_attn, ls_ff in mod.layers:
+            a, ff = ls_attn.fn, ls_ff.fn
+            talking = (a.mix_heads_pre_attn, a.mix_heads_post_attn) if t is cait.Transformer else None
+            fc1, fc2 = _linears(ff.net)
+            out.append(RefCross(None, _ln(a.norm), a.to_q.weight, a.to_kv.weight,
+                                (a.to_out[0].weight, a.to_out[0].bias), None, a.heads, a.dim_head, float(a.scale),
+                                skip=0, talking=talking, out_scale=ls_attn.scale, ff=(_ln(ff.net[0]), fc1, fc2),
+                                ff_scale=ls_ff.scale))
+        return out
+    raise NotImplementedError(f"no reference class-attention table for {t.__module__}.{t.__name__}")
+
+
+def _scaled(W: Tensor, b: Optional[Tensor], s: Optional[Tensor]) -> Tuple[Tensor, Optional[Tensor]]:
+    """bf16(W s) and fp32 b s of a Linear whose output is scaled by LayerScale s (cait.py:31-45), from fp64."""
+    d = lambda t: t.detach().double()                                                   # noqa: E731
+    Wd, bd = d(W), None if b is None else d(b)
+    if s is not None:
+        Wd, bd = Wd * d(s).reshape(-1, 1), None if bd is None else bd * d(s).reshape(-1)
+    return Wd.float().bfloat16(), None if bd is None else bd.float()
+
+
+def _cls_rows(S: Tensor, B: int, N: int) -> Tensor:
+    return S.view(B, N, -1)[:, 0]
+
+
+def _with_cls(S: Tensor, B: int, N: int, cls: Tensor) -> Tensor:
+    out = S.clone()
+    out.view(B, N, -1)[:, 0] = cls
+    return out
+
+
+def walk_cross(w: Walk, mod: nn.Module, direction: int, xa: Tensor, xba: Tensor, Na: int, xbb: Tensor, Nb: int,
+               B: int, layers: Optional[List[int]] = None, tag: str = "") -> Tuple[Tensor, Tensor]:
+    """The launches of one CrossAttentionEngine.run from w.pos on, against the class-attention layers of the reference
+    module `mod`: stream A fp32 xa [B Na, D_A] and its bf16 copy xba, stream B's bf16 copy xbb [B Nb, D_B] (the keys and
+    values); `layers` the indices run.  Returns A's stream and its bf16 copy with the new cls rows."""
+    refs = cross_module_layers(mod, direction)
+    d = lambda t: t.detach().double()                                                   # noqa: E731
+    w.where = f"{tag}context"
+    # cross_vit.py:65 / cait.py:91: to_kv of the raw context rows, every layer's in one GEMM over all of B's rows
+    ctx = w.prepared_gemm(xbb, torch.cat([R.kv_w.detach() for R in refs]).bfloat16(), None,
+                          what="w (every layer's to_kv)")
+    rows = torch.arange(0, B * Na, Na, dtype=torch.int32)
+    for i in (range(len(refs)) if layers is None else layers):
+        R = refs[i]
+        I = R.heads * R.dim_head
+        Wqkv = torch.cat([R.q_w, R.kv_w])
+        cls, clsb = _cls_rows(xa, B, Na), _cls_rows(xba, B, Na)
+        w.where = f"{tag}layer {i} qkv"
+        if R.proj_in is not None:                           # cross_vit.py:104-107: project_in, then the LayerNorm
+            w.where = f"{tag}layer {i} project_in"
+            qin = w.prepared_gemm(clsb, R.proj_in.weight.detach().bfloat16(), R.proj_in.bias.detach().float(),
+                                  stats=True)
+            w.where = f"{tag}layer {i} qkv"
+            c = w.take("gemm")
+            a = c.pre
+            w.folded(a, qin, R.ln, Wqkv, None)
+            for op in ("resid", "out_f32", "stats_out"):
+                w.same(op, a[op], None)
+            w.value("gelu", a["gelu"], False)
+            qkv = c.post["out_bf16"]
+        else:                                               # the LayerNorm of A's fp32 cls rows
+            c = w.take("layernorm")
+            a = c.pre
+            w.same("x", a["x"], xa)
+            w.same("gamma", a["gamma"], R.ln.gamma.detach().float())
+            w.same("beta", a["beta"], R.ln.beta.detach().float())
+            w.value("eps", a["eps"], float(R.ln.eps))
+            w.same("row_index (the cls rows)", a["row_index"], rows.to(xa.device))
+            w.same("out_f32", a["out_f32"], None)
+            qkv = w.plain_gemm(c.post["out_bf16"], Wqkv)
+        w.where = f"{tag}layer {i} attention"
+        c = w.take("attention_cls_headmix" if R.talking is not None else "attention_cls")
+        a = c.pre
+        w.same("qkv_self", a["qkv_self"], qkv)
+        w.same("ctx (the layer's to_kv columns)", a["ctx"], ctx[:, 2 * I * i:2 * I * (i + 1)])
+        w.value("rows_per_image", a["rows_per_image"], Nb)
+        w.value("first", a["first"], R.skip)
+        w.value("n", a["n"], Nb - R.skip)
+        w.value("H", a["H"], R.heads)
+        w.value("dh", a["dh"], R.dim_head)
+        w.value("scale", a["scale"], float(R.scale))
+        if R.talking is not None:                           # cait.py:95-97: pre before the softmax, post after it
+            w.same("pre", a["pre"], R.talking[0].detach().float())
+            w.same("post", a["post"], R.talking[1].detach().float())
+        o = c.post["out"]
+        Wo, bo = _scaled(R.out[0], R.out[1], R.out_scale)
+        if R.proj_out is not None:
+            w.where = f"{tag}layer {i} out"
+            y = w.prepared_gemm(o, Wo, bo)
+            w.where = f"{tag}layer {i} project_out"
+            new = w.written_residual(y, R.proj_out.weight.detach().bfloat16(), R.proj_out.bias.detach().float(), cls)
+        else:
+            w.where = f"{tag}layer {i} out"
+            new = w.written_residual(o, Wo, bo, cls)
+        xa, xba = _with_cls(xa, B, Na, new), _with_cls(xba, B, Na, new.bfloat16())
+        if R.ff is not None:                                # cait.py:120-121: x = ff(x) + x on the cls rows
+            ln, fc1, fc2 = R.ff
+            w.where = f"{tag}layer {i} ff LayerNorm"
+            c = w.take("layernorm")
+            a = c.pre
+            w.same("x", a["x"], xa)
+            w.same("gamma", a["gamma"], ln.gamma.detach().float())
+            w.same("beta", a["beta"], ln.beta.detach().float())
+            w.value("eps", a["eps"], float(ln.eps))
+            w.same("row_index (the cls rows)", a["row_index"], rows.to(xa.device))
+            w.same("out_f32", a["out_f32"], None)
+            w.where = f"{tag}layer {i} fc1"
+            h = w.plain_gemm(c.post["out_bf16"], fc1.weight, fc1.bias, gelu=True)
+            w.where = f"{tag}layer {i} fc2"
+            W2, b2 = _scaled(fc2.weight, fc2.bias, R.ff_scale)
+            new = w.written_residual(h, W2, b2, _cls_rows(xa, B, Na))
+            xa, xba = _with_cls(xa, B, Na, new), _with_cls(xba, B, Na, new.bfloat16())
+    return xa, xba
+
+
+def check_class_stage_provenance(model: nn.Module, x0: Tensor, B: int, grid: Tuple[int, int], launches: List[Launch],
+                                 ln_mode: str, case: str = "") -> int:
+    """Walk the trace of CaiT's or XCiT's forward_fused after its patch embedding (cait.py:246-255, xcit.py:380-393):
+    the patch encoder's layers on the embedded stream x0 [B N, D] of the (h, w) patch `grid` (walk_blocks, the layers its kept_layers() names),
+    the context the class attention reads -- CaiT: bf16 of the encoder's output (the cast of it in exact mode), XCiT:
+    its final_norm -- then the class-attention layers (walk_cross: the cls token of every image attends to
+    [LN(cls); context], cls_transformer.kept_layers()), and the head's LayerNorm and Linear on the cls rows.  The number
+    of launches checked."""
+    from vit_pytorch_b200 import xcit
+    is_xcit = isinstance(model, xcit.XCiT)
+    enc = model.xcit_transformer if is_xcit else model.patch_transformer
+    fold = ln_mode == "fold"
+    check_identity(enc, case)
+    N = grid[0] * grid[1]
+    kw = dict(B=B, N=N, primed=fold, layers=enc.kept_layers())
+    if is_xcit:
+        kw["grid"] = grid
+    w = Walk(case, launches, fold, kw)
+    S = walk_blocks(w, enc, x0)
+    w.where = "context"
+    if is_xcit:                                             # xcit.py:388: final_norm of the patch rows
+        fn = model.final_norm
+        w.where = "context (final_norm)"
+        c = w.take("layernorm")
+        a = c.pre
+        w.same("x", a["x"], S)
+        w.same("gamma", a["gamma"], fn.weight.detach().float())
+        w.same("beta", a["beta"], fn.bias.detach().float())
+        w.value("eps", a["eps"], float(fn.eps))
+        for op in ("row_index", "out_f32"):
+            w.same(op, a[op], None)
+        ctx = c.post["out_bf16"]
+    else:                                                   # cait.py:252: the patch rows as they leave the encoder
+        if not fold:
+            c = w.take("cast_f32_bf16")
+            w.same("x", c.pre["x"].reshape(S.shape), S)
+        ctx = S.bfloat16()
+    D = S.shape[1]
+    cls = model.cls_token.detach().reshape(1, D).float().expand(B, D).contiguous()
+    clsb = torch.full((B, D), math.nan, dtype=torch.bfloat16, device=S.device)
+    w2 = Walk(case, launches, fold, {})
+    w2.pos = w.pos
+    cls, _ = walk_cross(w2, model.cls_transformer, 0, cls, clsb, 1, ctx, N, B,
+                        layers=model.cls_transformer.kept_layers())
+    w2.where = "head"                                       # cait.py:255 / xcit.py:393: mlp_head(x[:, 0])
+    ln, lin = model.mlp_head[0], model.mlp_head[1]
+    c = w2.take("layernorm")
+    a = c.pre
+    w2.same("x (the cls rows)", a["x"], cls)
+    w2.same("gamma", a["gamma"], ln.weight.detach().float())
+    w2.same("beta", a["beta"], ln.bias.detach().float())
+    w2.value("eps", a["eps"], float(ln.eps))
+    for op in ("row_index", "out_f32"):
+        w2.same(op, a[op], None)
+    w2.prepared_gemm(c.post["out_bf16"], lin.weight.detach().bfloat16(), lin.bias.detach().float())
+    return _end(w2)
+
+
+def check_cross_vit_provenance(mse: nn.Module, xs: Tensor, xl: Tensor, B: int, Ns: int, Nl: int, primed: bool,
+                               launches: List[Launch], ln_mode: str, case: str = "") -> int:
+    """Walk the trace of CrossViT's MultiScaleEncoder (engine.fused_two_streams; reference cross_vit.py:134-162): per
+    block, each branch's encoder layers (walk_blocks), its final LayerNorm, which replaces the stream, then the
+    sm-attends-lg and lg-attends-sm class attention (walk_cross) on the updated streams."""
+    fold = ln_mode == "fold"
+    x, xb, N = [xs, xl], [None, None], (Ns, Nl)
+    pos = 0
+    for k, (sm_enc, lg_enc, cross) in enumerate(mse.layers):
+        for b, enc in enumerate((sm_enc, lg_enc)):
+            branch = f"block {k} {'sm' if b == 0 else 'lg'} "
+            check_identity(enc, case + " | " + branch)
+            w = Walk(case, launches, fold, dict(B=B, N=N[b], primed=primed and k == 0))
+            w.pos = pos
+            S = walk_blocks(w, enc, x[b])
+            w.where = branch + "final LayerNorm"                    # cross_vit.py:90: replaces the stream
+            c = w.take("layernorm")
+            a = c.pre
+            w.same("x", a["x"], S)
+            w.same("gamma", a["gamma"], enc.norm.weight.detach().float())
+            w.same("beta", a["beta"], enc.norm.bias.detach().float())
+            w.value("eps", a["eps"], float(enc.norm.eps))
+            w.same("row_index", a["row_index"], None)
+            if a["out_f32"] is None or a["out_bf16"] is None:
+                w.fail("out_f32", "the final LayerNorm writes the new stream and its bf16 copy")
+            x[b], xb[b] = c.post["out_f32"], c.post["out_bf16"]
+            w.same("out_bf16", xb[b], x[b].bfloat16())
+            pos = w.pos
+        for direction, (A, Bs) in enumerate(((0, 1), (1, 0))):
+            w = Walk(case, launches, fold, {})
+            w.pos = pos
+            x[A], xb[A] = walk_cross(w, cross, direction, x[A], xb[A], N[A], xb[Bs], N[Bs], B,
+                                     tag=f"block {k} {('sm attends lg', 'lg attends sm')[direction]} ")
+            pos = w.pos
+    w = Walk(case, launches, fold, {})
+    w.pos = pos
+    return _end(w)
+
+
+# ------------------------------------------------------------------------------------------------------ LeViT
+def check_levit_provenance(mod: nn.Module, img: Tensor, launches: List[Launch], case: str = "") -> int:
+    """Walk the trace of LeViT.forward_fused(img) through the reference LeViT (levit.py:27-195): the four stride-2
+    convolutions of conv_embedding as im2col + GEMM; per Transformer layer the QKV GEMM of [to_q; to_k; to_v] with
+    their BatchNorms folded (the module's eps), the position-bias attention (the bias table pos_bias.weight^T / scale,
+    the module's pos_indices against the kernel's |s i - y| F + |s j - x| on the key grid, the stride of to_q), the
+    to_out GEMM with its BatchNorm folded onto the residual or into a fresh stream, the Hardswish fc1 and the fc2
+    residual; then the mean over the map, its bf16 cast and the [mlp_head; distill_head] GEMM.  The number of launches
+    checked."""
+    from vit_pytorch_b200 import levit
+    w = Walk(case, launches, False, {})
+    d = lambda t: t.detach().double()                                                   # noqa: E731
+    B = img.shape[0]
+    src = img.contiguous()
+    H, W = img.shape[2:]
+    S = Sb = None
+    for i, conv in enumerate(mod.conv_embedding):                  # levit.py:153-158
+        w.where = f"conv_embedding {i}"
+        k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+        c = w.take("conv_im2col_nchw" if i == 0 else "conv_im2col_nhwc")
+        a = c.pre
+        if i == 0:
+            w.same("img", a["img"], src)
+        else:
+            w.same("x", a["x"], src)
+            w.value("B", a["B"], B)
+            w.value("H", a["H"], H)
+            w.value("W", a["W"], W)
+        w.value("k", a["k"], k)
+        w.value("s", a["s"], s)
+        w.value("p", a["p"], p)
+        col = c.post["out_bf16"]
+        # the weight in the gather's column order, (channel, tap) of the image, (tap, channel) of a channels-last map
+        cw = conv.weight.detach() if i == 0 else conv.weight.detach().permute(0, 2, 3, 1)
+        cw = cw.reshape(conv.out_channels, -1)
+        cw = torch.nn.functional.pad(cw, (0, col.shape[1] - cw.shape[1])).bfloat16()
+        c = w.take("gemm")
+        a = c.pre
+        w.same("a", a["a"], col)
+        w.same("w", a["w"], cw)
+        w.same("bias", a["bias"], conv.bias.detach().float())
+        for op in ("resid", "ln_sums", "stats_out"):
+            w.same(op, a[op], None)
+        w.value("gelu", a["gelu"], False)
+        H, W = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1
+        if i + 1 < len(mod.conv_embedding):
+            w.same("out_f32", a["out_f32"], None)
+            src = c.post["out_bf16"]
+        else:
+            if a["out_f32"] is None:
+                w.fail("out_f32", "the last convolution writes no fp32 stream")
+            S, Sb = c.post["out_f32"], c.post["out_bf16"]
+            w.same("out_bf16", Sb, S.bfloat16())
+    F_ = H
+    for ti, tr in enumerate(mod.backbone):
+        for li, (attn, ff) in enumerate(tr.layers):
+            tag = f"transformer {ti} layer {li}"
+            w.where = f"{tag} qkv"
+            Hh = attn.heads
+            dk, dv = attn.to_q[0].out_channels // Hh, attn.to_v[0].out_channels // Hh
+            s = attn.to_q[0].stride[0]
+            c = w.take("gemm")
+            a = c.pre
+            w.same("a", a["a"], Sb)
+            parts = [_bn_folded(seq[0], seq[1], tap_major=False, bf16=True)
+                     for seq in (attn.to_q, attn.to_k, attn.to_v)]
+            w.within("w ([to_q; to_k; to_v], BatchNorm folded)", a["w"], torch.cat([p_[0][0] for p_ in parts]),
+                     torch.cat([p_[0][1] for p_ in parts]))
+            w.within("bias (BatchNorm folded)", a["bias"], torch.cat([p_[1][0] for p_ in parts]),
+                     torch.cat([p_[1][1] for p_ in parts]))
+            for op in ("resid", "ln_sums", "out_f32", "stats_out"):
+                w.same(op, a[op], None)
+            w.value("gelu", a["gelu"], False)
+            qkv = c.post["out_bf16"]
+            w.where = f"{tag} attention"
+            c = w.take("attention_posbias")
+            a = c.pre
+            w.same("qkv", a["qkv"], qkv)
+            # levit.py:110-136: pos_bias(pos_indices) / scale added to the scores; the kernel reads table[h][index]
+            tbl = d(attn.pos_bias.weight).t() / f32(attn.scale)
+            w.within("table (pos_bias^T / scale)", a["table"], tbl, 2 * U * tbl.abs())
+            want = GB.posbias_index(F_, s, attn.pos_indices.device)
+            if tuple(attn.pos_indices.shape) != tuple(want.shape) or not torch.equal(attn.pos_indices, want):
+                w.fail("table (pos_indices)", f"the module's pos_indices {tuple(attn.pos_indices.shape)} are not the "
+                                              f"kernel's |s i - y| F + |s j - x| (F {F_}, s {s}) of shape "
+                                              f"{tuple(want.shape)}")
+            w.value("B", a["B"], B)
+            w.value("F", a["F"], F_)
+            w.value("s (to_q's stride)", a["s"], s)
+            w.value("H", a["H"], Hh)
+            w.value("dk", a["dk"], dk)
+            w.value("dv", a["dv"], dv)
+            w.value("scale", a["scale"], float(attn.scale))
+            w.value("gelu_out", a["gelu_out"], isinstance(attn.to_out[0], nn.GELU))
+            o = c.post["out"]
+            Fq = -(-F_ // s)
+            w.where = f"{tag} out"
+            c = w.take("gemm")
+            a = c.pre
+            w.same("a", a["a"], o)
+            (ow, owb), (ob, obb) = _bn_folded(attn.to_out[1], attn.to_out[2], tap_major=False, bf16=True)
+            w.within("w (to_out, BatchNorm folded)", a["w"], ow, owb)
+            w.within("bias (BatchNorm folded)", a["bias"], ob, obb)
+            w.same("resid", a["resid"], S if tr.attn_residual else None)     # levit.py:178-179
+            for op in ("ln_sums", "stats_out"):
+                w.same(op, a[op], None)
+            w.value("gelu", a["gelu"], False)               # the GELU runs before to_out (attention_posbias)
+            if a["out_f32"] is None or a["out_bf16"] is None:
+                w.fail("out_f32", "the stream and its bf16 copy are not both written")
+            S, Sb = c.post["out_f32"], c.post["out_bf16"]
+            w.same("out_bf16", Sb, S.bfloat16())
+            F_ = Fq
+            w.where = f"{tag} fc1"
+            fc1, act, fc2 = ff.net[0], ff.net[1], ff.net[3]
+            if not isinstance(act, nn.Hardswish):
+                w.fail("-", "the feed-forward activation is not the Hardswish the GEMM epilogue computes")
+            c = w.take("gemm_hardswish")
+            a = c.pre
+            w.same("a", a["a"], Sb)
+            w.same("w", a["w"], fc1.weight.detach().reshape(fc1.out_channels, -1).bfloat16())
+            w.same("bias", a["bias"], fc1.bias.detach().float())
+            h = c.post["out_bf16"]
+            w.where = f"{tag} fc2"
+            # levit.py:180: x = ff(x) + x, the bf16 copy written beside it
+            S = w.written_residual(h, fc2.weight.detach().reshape(fc2.out_channels, -1).bfloat16(),
+                                   fc2.bias.detach().float(), S)
+            Sb = S.bfloat16()
+    w.where = "head"                                                # levit.py:174-195
+    D = S.shape[1]
+    c = w.take("mean_pool")
+    a = c.pre
+    w.same("x", a["x"], S)
+    w.value("B", a["B"], B)
+    w.value("N", a["N"], F_ * F_)
+    w.value("D", a["D"], D)
+    w.value("n_pool", a["n_pool"], None)
+    pm = c.post["out"]
+    c = w.take("cast_f32_bf16")
+    w.same("x", c.pre["x"], pm)
+    pooled = c.post["out"]
+    heads = [mod.mlp_head] + ([mod.distill_head] if isinstance(mod.distill_head, nn.Linear) else [])
+    w.prepared_gemm(pooled, torch.cat([h_.weight.detach() for h_ in heads]).bfloat16(),
+                    torch.cat([h_.bias.detach().float() for h_ in heads]), what="w ([mlp_head; distill_head])")
+    return _end(w)
+

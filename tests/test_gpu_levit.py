@@ -1,5 +1,6 @@
-"""-m gpu: LeViT on the H100.  b200vit_attention_posbias against an fp64 reference with per-element bounds (bias and
-GELU included), what it writes and which rows it reads; the Hardswish GEMM epilogue against fp64; then the model:
+"""-m gpu: LeViT on the H100.  b200vit_attention_posbias against its fp64 reference with per-element bounds
+(oracle/grid_attention_bounds.py: bias and GELU included), what it writes and which rows it reads; the Hardswish GEMM
+epilogue against fp64 (oracle/bounds.py gemm_reference); then the model:
 every case of tests/golden/levit_spec.py through the comparison of test_gpu_family_parity.py, the distill-head case,
 CUDA-graph replay, weight refresh and the eager fall-backs."""
 import sys
@@ -9,7 +10,8 @@ import torch
 
 import test_gpu_family_parity as P
 from conftest import GOLDEN_DIR, load_golden
-from oracle.bounds import C_ACC, U, bf16_ulp, check
+from oracle.bounds import bf16_ulp, check, gemm_reference
+from oracle.grid_attention_bounds import posbias_reference
 from vit_pytorch_b200 import _lib
 from vit_pytorch_b200.graph import GraphedForward
 
@@ -24,41 +26,6 @@ PAIRS = [(dk, dv) for dk in (16, 32, 64) for dv in (32, 64, 128)]
 
 
 # ================================================================================================ attention_posbias
-def posbias_reference(qkv, table, B, F, s, H, dk, dv, scale, gelu=True):
-    """fp64 (ref, bound) of b200vit_attention_posbias on the kernel's own bf16 inputs.  The bound counts: the bf16
-    rounding of the probabilities before P V (2^-8 relative per key, against sum_j p_j |v_j|), the score error (the
-    fp32 dot products, C_ACC dk u sum |q||k| scaled, and the rounding of the scale, the bias and their sum: a relative
-    change of the probabilities by e^(2 dx)), fp32 accumulation of P V and of l, then GELU (slope at most 1.13) and
-    the output's bf16 rounding."""
-    Fq = -(-F // s)
-    x = qkv.double()[:B * F * F].view(B, F, F, -1)
-    q = x[:, ::s, ::s, :H * dk].reshape(B, Fq * Fq, H, dk).transpose(1, 2)
-    k = x[..., H * dk:2 * H * dk].reshape(B, F * F, H, dk).transpose(1, 2)
-    v = x[..., 2 * H * dk:2 * H * dk + H * dv].reshape(B, F * F, H, dv).transpose(1, 2)
-    qy, qx = torch.meshgrid(torch.arange(0, F, s, device=DEV), torch.arange(0, F, s, device=DEV), indexing="ij")
-    ky, kx = torch.meshgrid(torch.arange(F, device=DEV), torch.arange(F, device=DEV), indexing="ij")
-    idx = (qy.reshape(-1, 1) - ky.reshape(1, -1)).abs() * F + (qx.reshape(-1, 1) - kx.reshape(1, -1)).abs()
-    bias = table.double()[:, idx]                                                     # H, Nq, Nk
-    sc = float(torch.tensor(scale, dtype=torch.float32))
-    logits = sc * q @ k.transpose(-1, -2) + bias
-    p = logits.softmax(-1)
-    out = p @ v
-    mag = p @ v.abs()                                                                  # sum_j p_j |v_j|
-    dx = (C_ACC * dk + 4) * U * sc * (q.abs() @ k.abs().transpose(-1, -2)) + 4 * U * (bias.abs() + logits.abs())
-    dxm = dx.amax(-1, keepdim=True)
-    nk = F * F
-    e_attn = (2.0 ** -8 + 4 * dxm + (C_ACC * nk + nk / 4 + 16) * U) * mag
-    e_attn = e_attn + 3 * U * out.abs()
-    if gelu:
-        ref = torch.nn.functional.gelu(out)
-        e = 1.13 * e_attn + 1e-6 * (ref.abs() + e_attn) + 1e-30
-    else:
-        ref, e = out, e_attn
-    bound = e + bf16_ulp(ref.abs() + e) / 2
-    back = lambda t: t.transpose(1, 2).reshape(B * Fq * Fq, H * dv)                   # noqa: E731
-    return back(ref), back(bound)
-
-
 def make_qkv(B, F, H, dk, dv, seed, pad_cols=8, pad_rows=3):
     """A bf16 [B*F*F, H*(2 dk + dv)] view with row stride H*(2 dk + dv) + pad_cols of a buffer whose rows past B*F*F
     are NaN (never to be read), and an fp32 bias table [H, F*F]."""
@@ -131,10 +98,7 @@ def test_hardswish_epilogue_against_fp64(M, N, K):
     _lib.gemm_hardswish(a, w, out_bf16=big[:M], bias=b)
     torch.cuda.synchronize()
     assert torch.isnan(big[M:]).all()
-    y = a.double() @ w.double().t() + b.double()
-    ref = y * (y + 3).clamp(0, 6) / 6
-    e = 1.5 * ((C_ACC * K + 2) * U * (a.double().abs() @ w.double().abs().t()) + 2 * U * b.double().abs()) \
-        + 4 * U * ref.abs() + 1e-30
+    ref, e = gemm_reference(a, w, bias=b, hardswish=True)
     check(big[:M], ref, e + bf16_ulp(ref.abs() + e) / 2, f"hardswish gemm {M}x{N}x{K}")
 
 
