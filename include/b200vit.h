@@ -841,21 +841,13 @@ int b200vit_encoder_blocks_ex(const b200vit_layer* layers, int depth, float* x, 
 /*
  * TEST HOOKS -- process-global switches for A/B tests and bring-up; NOT part of the re-entrant API above (a value set
  * here changes every later call of every thread).  Production code never calls them.
- *   key 1: b200vit_attention key block: 0 / 1 = 64 keys (default), 2 = 128 keys
- *   key 11: b200vit_attention_varlen: 0 = 64-key blocks (default), 1 = 128-key blocks, 2 = 64-key blocks with half of
- *           the softmax exponentials on the FMA pipe
  *   key 12: BLOCK_N of b200vit_gemm_bf16: 0 = auto (256 when N > 128, else 128; residual launches on the TMA-store
  *           epilogue: 128), 1 = 128, 2 = 256
- *   key 13: b200vit_attention: 0 = all softmax exponentials on MUFU (default), 1 = half of them on the FMA pipe
  *   key 14: b200vit_gemm_bf16 epilogue: 0 = bf16 outputs and residual launches with ldo and N multiples of 8 are staged
  *           in shared memory and written by TMA stores (default; 256-wide residual tiles excepted), 1 = every launch
  *           stores straight from the accumulator registers.  Both give the same bits.
  *   key 15: b200vit_attention: 0 = launches with 128 < N <= 256 and dh = 32 or 64 run the persistent kernel (default),
- *           1 = every launch runs the tiled kernel.  Both give the same bits.  Keys 1 and 13 select instances of the
- *           tiled kernel: while either is non-zero every launch runs it, as with key 15.
- * Keys 1, 11 and 13 select real attention instances for every head width (32, 64, 80, 128): all (key block, FMA
- * exponential) combinations are built without register spills, so no setting falls back to a width's default.
- * They do not apply to calls with B200VIT_ATTN_MASK_SELF: those always run 64-key blocks with every exponential on MUFU.
+ *           1 = every launch runs the tiled kernel.  Both give the same bits.
  */
 int b200vit_debug_set(int key, int value);
 

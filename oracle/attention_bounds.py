@@ -8,9 +8,9 @@ rounding the kernel does.  Notation as in oracle/bounds.py: u = 2^-24, C_ACC the
 The kernel rounds the probabilities to bf16 before P V on purpose, and that rounding (up to 2^-8 relative per key) is
 far larger than all of its fp32 noise.  A bound that treated it as an independent error per key would be loose enough
 to let a 1 % error through, so the reference replays it: per query row i,
-  - the keys go in blocks of KB (64; 128 under test hook 1 = 2 or hook 11 = 1; 64 for MASK_SELF) counted from the
-    sequence start; x_j = s_j c with c = scale log2(e) (log2 units), masked keys (past the sequence, and the row's own
-    key under MASK_SELF unless the sequence has one token) x_j = -inf;
+  - the keys go in blocks of KB = 64 counted from the sequence start; x_j = s_j c with c = scale log2(e) (log2
+    units), masked keys (past the sequence, and the row's own key under MASK_SELF unless the sequence has one token)
+    x_j = -inf;
   - m_b = the max of x over blocks 0..b (the running max after block b), e_j = 2^(x_j - m_b(j)), P_j = bf16(e_j);
   - O and l are rescaled by corr = 2^(m_old - m_new) when the max rises.  corr multiplies O and l alike, so its ex2
     error cancels in O / l; relative to the final max M every key weighs W_j = P_j 2^(m_b(j) - M), and
@@ -22,11 +22,9 @@ What the kernel can do differently from that replay, and the bound of each:
   - Max.  The kernel's m_b is the max of its own x, within dm_b = max dx over the keys of blocks 0..b of m_b.  Scaling
     e's block by f = 2^(m_b - m~_b) changes nothing after corr except where the bf16 grid falls: the kernel weighs key j
     with P'_j / f, P'_j = bf16(e_j f g_j).
-  - exp2.  x~_j - m~_b is rounded in fp32 (u |x_j - m_b|), and ex2.approx.ftz.f32 has a relative error EX2_REL;
-    exp2_emul2 (the FMA path, odd 8-key groups of a block under test hook 13 / hook 11 = 2) has EMUL_REL and clamps
-    its argument at -125.  So e_j f g_j lies in [lo_j, hi_j] = e_j [2^-d_j (1 - r_j), 2^d_j (1 + r_j)] with
-    d_j = dx_j + dm_b + u |x_j - m_b|, r_j the ex2 constant of the key; lo_j = 0 where it falls below 2^-126 (ftz), and
-    hi_j >= 2^-124 on emulated keys (the clamp).
+  - exp2.  x~_j - m~_b is rounded in fp32 (u |x_j - m_b|), and ex2.approx.ftz.f32 has a relative error EX2_REL.  So
+    e_j f g_j lies in [lo_j, hi_j] = e_j [2^-d_j (1 - EX2_REL), 2^d_j (1 + EX2_REL)]
+    with d_j = dx_j + dm_b + u |x_j - m_b|; lo_j = 0 where it falls below 2^-126 (ftz).
   - Ambiguous roundings.  bf16 rounding is monotone, so P'_j lies in [bf16(lo_j), bf16(hi_j)], and
     |P'_j / f - P_j| <= A_j = max(bf16(hi_j) - P_j, P_j - bf16(lo_j)) 2^dm_b + P_j (2^dm_b - 1).  A_j is 0 up to the
     fp32 noise for every key whose interval lies within one bf16 rounding interval, and an ulp of P_j for the few
@@ -59,11 +57,8 @@ LOG2E = 1.4426950408889634
 # Programming Guide, exp2f); EX2_REL = 2^-21 is 4 ulp of fp32.  Against the 2^-8 rounding of P the constant is
 # irrelevant, so it is generous rather than exact.
 EX2_REL = 2.0 ** -21
-# exp2_emul2 (common.cuh): the relative error its comment claims, checked in tests/test_attention_bounds.py on a dense
-# grid over [-125, 0] with the kernel's fp32 arithmetic.
-EMUL_REL = 7.5e-5
 FTZ = 2.0 ** -126           # smallest normal fp32: ex2.approx.ftz flushes results below it to 0
-EMUL_FLOOR = 2.0 ** -124    # exp2_emul2 clamps its argument at -125: its result is at least 2^-125 (1 - EMUL_REL)
+KB = 64                     # keys per block of attention.cu
 
 
 def scale_log2e(scale: float) -> float:
@@ -76,30 +71,25 @@ def _bf16(x: Tensor) -> Tensor:
     return x.float().bfloat16().double()
 
 
-def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: int = 64, emul: bool = False,
-                        mask_self: bool = False, key_mask: Optional[Tensor] = None, zero_masked_rows: bool = False,
+def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, mask_self: bool = False,
+                        key_mask: Optional[Tensor] = None, zero_masked_rows: bool = False,
                         elems: int = 1 << 23) -> Tuple[Tensor, Tensor]:
     """(ref, bound) [G, n, dh] of the attention of G independent sequences of n tokens, q, k, v: [G, n, dh] bf16.
 
-    kb: the instance's key block; emul: exponentials of the odd 8-key groups on the FMA path; mask_self: each query's
-    own key is excluded (n > 1); key_mask: None or bool [G, n] (True = keep), the masked keys -inf.  A sequence with no
-    kept key gets exactly 0 under zero_masked_rows, else every key at weight 1: the kernel's P = 1 and l = n are exact,
-    so its reference is the mean of the values with the P V and O fl(1 / l) terms alone.  Query rows go in chunks of at
-    most `elems` scores, so 16384-key sequences fit."""
+    mask_self: each query's own key is excluded (n > 1); key_mask: None or bool [G, n] (True = keep), the masked keys
+    -inf.  A sequence with no kept key gets exactly 0 under zero_masked_rows, else every key at weight 1: the kernel's
+    P = 1 and l = n are exact, so its reference is the mean of the values with the P V and O fl(1 / l) terms alone.
+    Query rows go in chunks of at most `elems` scores, so 16384-key sequences fit."""
     G, n, dh = q.shape
     dev = q.device
     k64, v64 = k.double(), v.double()
     kabs, vabs = k64.abs(), v64.abs()
     vmax = vabs.amax(dim=(1, 2))[:, None, None]
-    nb = -(-n // kb)
+    nb = -(-n // KB)
     c = float(torch.tensor(scale, dtype=torch.float32).item()) * LOG2E
     key = torch.arange(n, device=dev)
-    blk = key // kb
+    blk = key // KB
     rel = torch.full((n,), EX2_REL, dtype=torch.float64, device=dev)
-    emul_key = torch.zeros(n, dtype=torch.bool, device=dev)
-    if emul:
-        emul_key = ((key % kb) // 8) % 2 == 1
-        rel = torch.where(emul_key, torch.full_like(rel, EMUL_REL), rel)
     empty = None
     if key_mask is not None:
         km = key_mask.to(device=dev, dtype=torch.bool)
@@ -124,9 +114,9 @@ def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: in
             dx = torch.where(empty, torch.zeros_like(dx), dx)
         x = torch.where(valid, x, torch.full_like(x, -math.inf))
         dx = torch.where(valid, dx, torch.zeros_like(dx))
-        pad = nb * kb - n
-        xp = torch.nn.functional.pad(x, (0, pad), value=-math.inf).view(G, r1 - r0, nb, kb)
-        dxp = torch.nn.functional.pad(dx, (0, pad)).view(G, r1 - r0, nb, kb)
+        pad = nb * KB - n
+        xp = torch.nn.functional.pad(x, (0, pad), value=-math.inf).view(G, r1 - r0, nb, KB)
+        dxp = torch.nn.functional.pad(dx, (0, pad)).view(G, r1 - r0, nb, KB)
         mb = xp.amax(-1).cummax(-1).values           # running max after each block
         dmb = dxp.amax(-1).cummax(-1).values
         m, dm = mb[..., blk], dmb[..., blk]
@@ -136,8 +126,6 @@ def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: in
         hi = e * torch.exp2(d) * (1 + rel)
         lo = e * torch.exp2(-d) * (1 - rel)
         lo = torch.where(lo < FTZ, torch.zeros_like(lo), lo)
-        if emul:
-            hi = torch.where(valid & emul_key, hi.clamp_min(EMUL_FLOOR), hi)
         p = _bf16(e)
         fm = torch.exp2(dm)
         amb = torch.maximum(_bf16(hi) - p, p - _bf16(lo)) * fm + p * (fm - 1)
@@ -158,8 +146,8 @@ def attention_reference(q: Tensor, k: Tensor, v: Tensor, scale: float, *, kb: in
     return ref, bound
 
 
-def qkv_attention_reference(qkv: Tensor, lengths: Sequence[int], H: int, dh: int, scale: float, *, kb: int = 64,
-                            emul: bool = False, mask_self: bool = False) -> Tuple[Tensor, Tensor]:
+def qkv_attention_reference(qkv: Tensor, lengths: Sequence[int], H: int, dh: int, scale: float, *,
+                            mask_self: bool = False) -> Tuple[Tensor, Tensor]:
     """(ref, bound) [T, H dh] of the attention of the packed q | k | v buffer qkv[T, 3 H dh] (bf16) over consecutive
     sequences of `lengths` tokens (T = sum(lengths)), as b200vit_attention (equal lengths) or _varlen lays it out."""
     T, I = qkv.shape[0], H * dh
@@ -174,7 +162,7 @@ def qkv_attention_reference(qkv: Tensor, lengths: Sequence[int], H: int, dh: int
     for n, st in by_len.items():
         idx = (torch.tensor(st, device=dev)[:, None] + torch.arange(n, device=dev)[None]).reshape(-1)
         x = qkv[idx].view(len(st), n, 3, H, dh).permute(2, 0, 3, 1, 4).reshape(3, len(st) * H, n, dh)
-        r, b = attention_reference(x[0], x[1], x[2], scale, kb=kb, emul=emul, mask_self=mask_self)
+        r, b = attention_reference(x[0], x[1], x[2], scale, mask_self=mask_self)
         ref[idx] = r.view(len(st), H, n, dh).permute(0, 2, 1, 3).reshape(-1, I)
         bound[idx] = b.view(len(st), H, n, dh).permute(0, 2, 1, 3).reshape(-1, I)
     return ref, bound
@@ -187,7 +175,7 @@ def axial_reference(qkv: Tensor, key_mask: Optional[Tensor], B: int, L: int, G: 
     without a kept key 0 (zero_masked_rows) or the mean of its sequence's values."""
     t = qkv.view(B, L, G, 3, H, dh).permute(3, 0, 2, 4, 1, 5).reshape(3, B * G * H, L, dh)
     km = None if key_mask is None else key_mask.bool()[:, None, None, :].expand(B, G, H, L).reshape(B * G * H, L)
-    ref, bound = attention_reference(t[0], t[1], t[2], scale, kb=64, key_mask=km, zero_masked_rows=zero_masked_rows)
+    ref, bound = attention_reference(t[0], t[1], t[2], scale, key_mask=km, zero_masked_rows=zero_masked_rows)
     back = lambda x: x.view(B, G, H, L, dh).permute(0, 3, 1, 2, 4).reshape(B * L * G, H * dh)   # noqa: E731
     return back(ref), back(bound)
 

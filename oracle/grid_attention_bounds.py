@@ -177,7 +177,7 @@ def attention_ex_reference(q: Tensor, k: Tensor, v: Tensor, scale: float) -> Tup
     dk, dv = q.shape[-1], v.shape[-1]
     W = max(dk, dv)
     pad = lambda t: F.pad(t, (0, W - t.shape[-1]))     # noqa: E731
-    ref, bound = attention_reference(pad(q), pad(k), pad(v), scale, kb=64)
+    ref, bound = attention_reference(pad(q), pad(k), pad(v), scale)
     return ref[..., :dv], bound[..., :dv]
 
 
@@ -240,7 +240,7 @@ def groups_reference(qkv: Tensor, B: int, gh: int, gw: int, ph: int, pw: int, H:
     rows = group_rows(B, gh, gw, ph, pw, qkv.device)
     G, n = rows.shape
     x = qkv[rows.reshape(-1)].view(G, n, 3, H, dh).permute(2, 0, 3, 1, 4).reshape(3, G * H, n, dh)
-    r, b = attention_reference(x[0], x[1], x[2], scale, kb=64)
+    r, b = attention_reference(x[0], x[1], x[2], scale)
     M = B * gh * gw
     back = lambda t: t.view(G, H, n, dh).permute(0, 2, 1, 3).reshape(-1, H * dh)      # noqa: E731
     return _scatter(rows, back(r), M), _scatter(rows, back(b), M)
@@ -257,7 +257,7 @@ def window_token_reference(qkv: Tensor, tok: Tensor, B: int, gh: int, gw: int, p
     x = qkv[rows.reshape(-1)].view(G, n, 3, H, dh)
     x = torch.cat((tok.view(1, 1, 3, H, dh).expand(G, 1, -1, -1, -1), x), 1)
     x = x.permute(2, 0, 3, 1, 4).reshape(3, G * H, n + 1, dh)
-    r, b = attention_reference(x[0], x[1], x[2], scale, kb=64)
+    r, b = attention_reference(x[0], x[1], x[2], scale)
     r, b = r.view(G, H, n + 1, dh).transpose(1, 2), b.view(G, H, n + 1, dh).transpose(1, 2)
     M = B * gh * gw
     return (_scatter(rows, r[:, 1:].reshape(-1, I), M), _scatter(rows, b[:, 1:].reshape(-1, I), M),
@@ -274,7 +274,7 @@ def mix_reference(wqk: Tensor, o: Tensor, B: int, gh: int, gw: int, p: int, H: i
     w = wqk.view(B, nw, H, 2, dh).permute(0, 2, 1, 3, 4)                 # b h n (q|k) d
     q, k = (w[..., c, :].reshape(B * H, 1, nw, dh).expand(-1, pp, -1, -1).reshape(-1, nw, dh) for c in (0, 1))
     v = o[rows.reshape(-1)].view(B, nw, pp, H, dh).permute(0, 3, 2, 1, 4).reshape(B * H * pp, nw, dh)
-    r, b = attention_reference(q, k, v, scale, kb=64)                     # [(b h w), i, d]
+    r, b = attention_reference(q, k, v, scale)                            # [(b h w), i, d]
     back = lambda t: t.view(B, H, pp, nw, dh).permute(0, 3, 2, 1, 4).reshape(-1, I)    # noqa: E731
     return _scatter(rows, back(r), B * gh * gw), _scatter(rows, back(b), B * gh * gw)
 

@@ -1,9 +1,8 @@
 """The error bounds of oracle/attention_bounds.py are neither loose nor tight (CPU only).
 
-Tight: an fp32 emulation of attention.cu's arithmetic -- fp32 scores, the online softmax over key blocks of the
-instance's KB with a running max, bf16 P, fp32 l and O rescaled by corr, the FMA-path exponential exp2_emul2 on the
-odd 8-key groups, the self mask, O * (1 / l) rounded to bf16 -- passes the checker on every distribution the GPU sweep
-uses, and exp2_emul2 itself keeps the relative error its comment claims.
+Tight: an fp32 emulation of attention.cu's arithmetic -- fp32 scores, the online softmax over 64-key blocks with a
+running max, bf16 P, fp32 l and O rescaled by corr, the self mask, O * (1 / l) rounded to bf16 -- passes the checker on
+every distribution the GPU sweep uses.
 Loose: each defect an attention kernel could plausibly have, planted into the emulation, is flagged, at a size the
 former criterion (at least 99.5 % of the elements within 1e-2 relative + 1e-3, and none off by 2e-2, against an fp32
 softmax) lets through where it does."""
@@ -16,48 +15,11 @@ from oracle import attention_bounds as AB
 from oracle import bounds as Bd
 from oracle import vit_oracle as O
 
-# instance: (KB, FMA exponentials, MASK_SELF), as attention.cu's launch_attention_dh instantiates them
-CONFIGS = {"kb64": (64, False, False), "kb128": (128, False, False), "kb64_fma": (64, True, False),
-           "kb128_fma": (128, True, False), "mask_self": (64, False, True)}
-C0, C1, C2, C3 = 0.05517210811376572, 0.24261118471622467, 0.693260908126831, 0.9999280571937561   # common.cuh
+# instance: MASK_SELF, as attention.cu's launch_attention_dh instantiates them
+CONFIGS = {"kb64": False, "mask_self": True}
 
 
-def fma32(a, b, c):
-    """fp32 fma, nearly: the product of two fp32 values is exact in fp64, but the sum is rounded twice (to fp64, then
-    to fp32), which in rare double-rounding cases differs by one fp32 ulp from the single rounding of a hardware fma."""
-    return (a.double() * b.double() + c.double()).float()
-
-
-def exp2_emul2(x):
-    """common.cuh exp2_emul2 in fp32: round-to-nearest split by the 1.5 * 2^23 trick, the degree-3 polynomial in
-    fp32 fmas, the exponent added to the bit pattern as an integer."""
-    x = x.float().clamp_min(-125.0)
-    t = x + torch.tensor(12582912.0)
-    n = t - torch.tensor(12582912.0)
-    f = fma32(n, torch.tensor(-1.0), x)
-    one = torch.ones_like(f)
-    p = fma32(torch.tensor(C0) * one, f, torch.tensor(C1) * one)
-    p = fma32(p, f, torch.tensor(C2) * one)
-    p = fma32(p, f, torch.tensor(C3) * one)
-    bits = (p.view(torch.int32).long() + (t.view(torch.int32).long() << 23)) & 0xFFFFFFFF
-    bits = torch.where(bits >= 2 ** 31, bits - 2 ** 32, bits)
-    return bits.int().view(torch.float32)
-
-
-def test_exp2_emul2_relative_error():
-    """The 7.5e-5 of exp2_emul2's comment (EMUL_REL) on a sample of [-125, 0]: a grid of step 2^-14 (2 million
-    points, every fraction f = x - round(x) on that grid) and the edges.  A sample, not every fp32 value: the measured
-    worst is 7.48e-5.  EMUL_REL only widens the ambiguity bands of the FMA-path keys."""
-    x = torch.cat([torch.arange(-125 * 2 ** 14, 1, dtype=torch.float64) / 2 ** 14,
-                   torch.tensor([-124.5, -0.5, 0.5 - 2 ** -24, -1e-30, 0.0])]).float()
-    x = x[x <= 0]
-    got = exp2_emul2(x).double()
-    rel = ((got - torch.exp2(x.double())) / torch.exp2(x.double())).abs()
-    print(f"exp2_emul2 worst relative error {rel.max().item():.3e} (EMUL_REL {AB.EMUL_REL:.1e})")
-    assert rel.max().item() <= AB.EMUL_REL
-
-
-def emulate(q, k, v, scale, kb=64, emul=False, mask_self=False, defect=None):
+def emulate(q, k, v, scale, mask_self=False, defect=None):
     """attention.cu's arithmetic in fp32 on G sequences q, k, v [G, n, dh] (bf16); returns the fp32 output before its
     bf16 rounding.  defect: None or one of DEFECTS (planted into this arithmetic)."""
     G, n, dh = q.shape
@@ -74,6 +36,7 @@ def emulate(q, k, v, scale, kb=64, emul=False, mask_self=False, defect=None):
     o = torch.zeros(G, n, dh)
     l = torch.zeros(G, n, 1)
     m = torch.full((G, n, 1), -math.inf)
+    kb = AB.KB
     nb = -(-n // kb)
     for b in range(nb):
         xb = x[..., b * kb:(b + 1) * kb]
@@ -86,9 +49,6 @@ def emulate(q, k, v, scale, kb=64, emul=False, mask_self=False, defect=None):
         m_old, m = m, mx
         t = xb - (m_old if defect == "prev_max" and last else m)
         e = torch.exp2(t)
-        if emul:
-            grp = (torch.arange(xb.shape[-1]) // 8) % 2 == 1
-            e = torch.where(grp, torch.where(xb == -math.inf, torch.zeros_like(t), exp2_emul2(t)), e)
         l = l + e.sum(-1, keepdim=True)
         o = o + e.bfloat16().float() @ v[:, b * kb:(b + 1) * kb].float()
     y = o * (1.0 / l)
@@ -118,22 +78,21 @@ def old_criterion(out, q, k, v, scale, mask_self=False):
 @pytest.mark.parametrize("dh", [32, 64, 80, 128])
 @pytest.mark.parametrize("kind", AB.KINDS)
 def test_fp32_emulation_passes(kind, dh, cfg):
-    kb, emul, ms = CONFIGS[cfg]
+    ms = CONFIGS[cfg]
     B, H = 2, 2
     worst, fp32_part = 0.0, []
     for N in (1, 2, 63, 65, 129, 197):
         scale = dh ** -0.5
         q, k, v = split(AB.qkv_inputs(kind, [N] * B, H, dh, seed=N + dh), B, N, H, dh)
-        got = emulate(q, k, v, scale, kb, emul, ms).bfloat16()
-        ref, bound = AB.attention_reference(q, k, v, scale, kb=kb, emul=emul, mask_self=ms)
+        got = emulate(q, k, v, scale, ms).bfloat16()
+        ref, bound = AB.attention_reference(q, k, v, scale, mask_self=ms)
         worst = max(worst, Bd.check(got, ref, bound, f"{cfg} {kind} dh{dh} N{N}"))
         half_ulp = 0.5 * Bd.bf16_ulp(ref.abs())
         fp32_part.append(((bound - half_ulp) / half_ulp)[ref != 0])
     # The worst ratio says nothing about looseness: the half-ulp output term alone brings it near 1 wherever ref sits
     # near a bf16 midpoint.  What could be loose are the fp32 terms (ambiguity bands, C_ACC, eta); on the typical
-    # element they must stay a fraction of the output rounding (measured medians 0.006 to 0.39, the larger ones on the
-    # FMA path, whose 7.5e-5 exponential makes more keys ambiguous; a 2^-8-per-key treatment of P would be several
-    # times the half ulp).  The planted defects below show the rest.
+    # element they must stay a fraction of the output rounding (measured medians 0.006 to 0.19; a 2^-8-per-key
+    # treatment of P would be several times the half ulp).  The planted defects below show the rest.
     med = torch.cat(fp32_part).median().item()
     print(f"fp32 emulation {cfg} {kind} dh{dh}: worst |got - ref| / bound {worst:.3f}, "
           f"median fp32 part of the bound {med:.3f} half ulps")
@@ -154,14 +113,14 @@ DEFECTS = {
 @pytest.mark.parametrize("defect", sorted(DEFECTS))
 def test_planted_defect_is_flagged(defect):
     cfg, kind, dh, N, old_accepts = DEFECTS[defect]
-    kb, emul, ms = CONFIGS[cfg]
+    ms = CONFIGS[cfg]
     B, H = 2, 2
     scale = dh ** -0.5
     q, k, v = split(AB.qkv_inputs(kind, [N] * B, H, dh, seed=3), B, N, H, dh)
-    ref, bound = AB.attention_reference(q, k, v, scale, kb=kb, emul=emul, mask_self=ms)
-    clean = emulate(q, k, v, scale, kb, emul, ms).bfloat16()
+    ref, bound = AB.attention_reference(q, k, v, scale, mask_self=ms)
+    clean = emulate(q, k, v, scale, ms).bfloat16()
     Bd.check(clean, ref, bound, "clean")
-    got = emulate(q, k, v, scale, kb, emul, ms, defect=defect).bfloat16()
+    got = emulate(q, k, v, scale, ms, defect=defect).bfloat16()
     ratio = Bd.excess(got, ref, bound)
     old = old_criterion(got, q, k, v, scale, ms)
     print(f"{defect}: worst |got - ref| / bound {ratio:.2f}, former criterion accepts: {old}")

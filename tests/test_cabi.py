@@ -61,6 +61,15 @@ def test_bad_arguments_return_error_codes(lib):
     assert ctypes.sizeof(_lib.Layer) == 11 * 8 + 8 and ctypes.sizeof(_lib.EncoderWs) == 7 * 8   # as the C structs
 
 
+def test_debug_set_accepts_only_the_documented_hooks(lib):
+    """Keys 12, 14 and 15 are the test hooks include/b200vit.h lists (set to their defaults here); any other key is
+    B200VIT_ERR_INVALID."""
+    for key in (12, 14, 15):
+        assert lib.b200vit_debug_set(key, 0) == 0, key
+    for key in (1, 11, 13, 0, 16):
+        assert lib.b200vit_debug_set(key, 0) == -1, key
+
+
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
     monkeypatch.setattr(_lib, "_lib", None)
     monkeypatch.setattr(_lib, "LIB_PATH", tmp_path / "nope.so")

@@ -2,10 +2,11 @@
 b200vit_attention_varlen / _ex) within its bound of the fp64 reference of oracle/attention_bounds.py, which replays the
 kernel's deliberate bf16 rounding of the probabilities and bounds only its fp32 noise and the output rounding.
 
-Every instance (64- and 128-key blocks, FMA exponentials, MASK_SELF) on four input distributions (attention_bounds.KINDS),
-at the key counts around the block edges, the production launches with more CTAs than two waves, a NaViT pack and
-single sequences of 4097 and 16384 keys.  Outputs start as NaN, so an element the kernel does not write fails too.  The
-worst |got - ref| / bound of each kernel and instance is printed at the end of the module."""
+Every instance (the default kernel of each length, the tiled kernel at every length, MASK_SELF) on four input
+distributions (attention_bounds.KINDS), at the key counts around the block edges, the production launches with more
+CTAs than two waves, a NaViT pack and single sequences of 4097 and 16384 keys.  Outputs start as NaN, so an element the
+kernel does not write fails too.  The worst |got - ref| / bound of each kernel and instance is printed at the end of the
+module."""
 import contextlib
 import random
 
@@ -18,11 +19,10 @@ from vit_pytorch_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-# instance: (test hook 1, test hook 13, MASK_SELF) of b200vit_attention; key block and FMA exponentials it selects
-PLAIN_CONFIGS = {"kb64": (0, 0, False), "kb128": (2, 0, False), "kb64_fma": (0, 1, False), "kb128_fma": (2, 1, False),
-                 "mask_self": (0, 0, True)}
-# instance: (test hook 11, MASK_SELF) of b200vit_attention_varlen
-VARLEN_CONFIGS = {"kb64": (0, False), "kb128": (1, False), "kb64_fma": (2, False), "mask_self": (0, True)}
+# instance: (test hook 15, MASK_SELF) of b200vit_attention; hook 15 = 1 runs the tiled kernel at 128 < N <= 256 too
+PLAIN_CONFIGS = {"default": (0, False), "tiled": (1, False), "mask_self": (0, True)}
+# instance: MASK_SELF of b200vit_attention_varlen
+VARLEN_CONFIGS = {"kb64": False, "mask_self": True}
 LENGTHS = (1, 2, 16, 63, 64, 65, 127, 128, 129, 197, 256, 257, 511, 512)
 WORST = {}
 
@@ -54,27 +54,24 @@ def hooks(**kv):
 
 def plain_bound(qkv, B, N, H, dh, cfg):
     """b200vit_attention under instance `cfg` against its bound: returns the worst ratio."""
-    k1, k13, ms = PLAIN_CONFIGS[cfg]
+    k15, ms = PLAIN_CONFIGS[cfg]
     out = torch.full((B * N, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
-    with hooks(k1=k1, k13=k13):
+    with hooks(k15=k15):
         _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5, mask_self=ms)
         torch.cuda.synchronize()
-    ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5, kb=128 if k1 == 2 else 64,
-                                            emul=k13 == 1, mask_self=ms)
+    ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5, mask_self=ms)
     ratio = Bd.check(out, ref, bound, f"attention {cfg} B{B} N{N} H{H} dh{dh}")
     record(("attention", cfg), ratio)
     return ratio
 
 
 def varlen_bound(qkv, lengths, H, dh, cfg):
-    k11, ms = VARLEN_CONFIGS[cfg]
+    ms = VARLEN_CONFIGS[cfg]
     cu, tp, tiles = _lib.varlen_index(lengths, DEV)
     out = torch.full((sum(lengths), H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
-    with hooks(k11=k11):
-        _lib.attention_varlen(qkv, out, cu, tp, tiles, H, dh, dh ** -0.5, mask_self=ms)
-        torch.cuda.synchronize()
-    ref, bound = AB.qkv_attention_reference(qkv, lengths, H, dh, dh ** -0.5, kb=128 if k11 == 1 else 64,
-                                            emul=k11 == 2, mask_self=ms)
+    _lib.attention_varlen(qkv, out, cu, tp, tiles, H, dh, dh ** -0.5, mask_self=ms)
+    torch.cuda.synchronize()
+    ref, bound = AB.qkv_attention_reference(qkv, lengths, H, dh, dh ** -0.5, mask_self=ms)
     ratio = Bd.check(out, ref, bound, f"attention_varlen {cfg} {len(lengths)} sequences H{H} dh{dh}")
     record(("attention_varlen", cfg), ratio)
     return ratio
@@ -104,7 +101,7 @@ def test_attention_production_launch_within_bound(name, H, dh, N, ms, kind):
     B = 2 * sms // (tiles * H) + 1
     assert B * tiles * H > 2 * sms
     qkv = AB.qkv_inputs(kind, [N] * B, H, dh, seed=B + N, device=DEV)
-    plain_bound(qkv, B, N, H, dh, "mask_self" if ms else "kb64")
+    plain_bound(qkv, B, N, H, dh, "mask_self" if ms else "default")
 
 
 def navit_lengths(count, seed):

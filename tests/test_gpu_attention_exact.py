@@ -30,8 +30,7 @@ BF16_REL = 2.0 ** -7          # one bf16 ulp, relative
 
 @contextlib.contextmanager
 def hooks(**kv):
-    """Test hooks of include/b200vit.h (key -> value), reset to 0 afterwards: k1 = key block, k11 = varlen mode,
-    k13 = FMA exponentials."""
+    """Test hooks of include/b200vit.h (key -> value), reset to 0 afterwards: k15 = the tiled kernel at every length."""
     L = _lib.lib()
     try:
         for k, v in kv.items():
@@ -59,21 +58,21 @@ def assert_rows_equal(got, want, keep, what):
 
 
 # ====================================================================================================== A. isolation
-# (test hook 1, test hook 13, MASK_SELF): the key block, FMA exponentials, and the self-masked instance
-PLAIN_CONFIGS = {"kb64": (0, 0, False), "kb128": (2, 0, False), "kb64_fma": (0, 1, False), "kb128_fma": (2, 1, False),
-                 "mask_self": (0, 0, True)}
+# (test hook 15, MASK_SELF): the kernel each length runs by default, the tiled kernel at 128 < N <= 256 as well, and
+# the self-masked instance
+PLAIN_CONFIGS = {"default": (0, False), "tiled": (1, False), "mask_self": (0, True)}
 
 
 def run_plain(qkv, B, N, H, dh, cfg):
-    k1, k13, ms = PLAIN_CONFIGS[cfg]
+    k15, ms = PLAIN_CONFIGS[cfg]
     out = torch.full((B * N, H * dh), 5.0, device=DEV, dtype=torch.bfloat16)
-    with hooks(k1=k1, k13=k13):
+    with hooks(k15=k15):
         _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5, mask_self=ms)
         torch.cuda.synchronize()
     return out
 
 
-@pytest.mark.parametrize("N", [64, 65, 127, 128, 129, 197, 255])      # len % KB in {0, 1, KB - 1} for KB = 64, 128
+@pytest.mark.parametrize("N", [64, 65, 127, 128, 129, 197, 255])      # len % 64 in {0, 1, 63}
 @pytest.mark.parametrize("cfg", sorted(PLAIN_CONFIGS))
 @pytest.mark.parametrize("dh", [32, 64, 80, 128])
 def test_attention_isolation_under_poisoning(dh, cfg, N):
@@ -95,18 +94,16 @@ def test_attention_isolation_under_poisoning(dh, cfg, N):
     assert torch.equal(run_plain(buf[:B * N], B, N, H, dh, cfg), clean)
 
 
-VARLEN_CONFIGS = {"kb64": (0, False), "kb128": (1, False), "fma": (2, False), "mask_self": (0, True)}   # test hook 11
+VARLEN_CONFIGS = {"kb64": False, "mask_self": True}                      # MASK_SELF
 # length-1 sequences, lengths on and around 64 / 128 boundaries, sequences crossing 128-row tiles of the pack
 VARLEN_PACK = [1, 130, 64, 1, 63, 257, 128, 65, 1, 200, 127, 129, 2]
 
 
 def run_varlen(qkv, lengths, H, dh, cfg):
-    k11, ms = VARLEN_CONFIGS[cfg]
     cu, tp, tiles = _lib.varlen_index(lengths, DEV)
     out = torch.full((qkv.shape[0], H * dh), 5.0, device=DEV, dtype=torch.bfloat16)
-    with hooks(k11=k11):
-        _lib.attention_varlen(qkv, out, cu, tp, tiles, H, dh, dh ** -0.5, mask_self=ms)
-        torch.cuda.synchronize()
+    _lib.attention_varlen(qkv, out, cu, tp, tiles, H, dh, dh ** -0.5, mask_self=VARLEN_CONFIGS[cfg])
+    torch.cuda.synchronize()
     return out
 
 
@@ -391,7 +388,7 @@ def test_attention_uniform_exact_key_sets(dh, cfg):
             v, j = indicator_v(B * N, local, H, dh, wins)
             qkv[:, 2 * H * dh:] = v
             out = run_plain(qkv, B, N, H, dh, cfg)
-            assert_exact_keys(out, uniform_expect(local, length, j, PLAIN_CONFIGS[cfg][2]), f"N={N} windows {wins}")
+            assert_exact_keys(out, uniform_expect(local, length, j, PLAIN_CONFIGS[cfg][1]), f"N={N} windows {wins}")
 
 
 def pack_index(lengths):
@@ -415,7 +412,7 @@ def test_attention_varlen_uniform_exact_key_sets(dh, cfg):
         v, j = indicator_v(T, local, H, dh, wins)
         qkv[:, 2 * H * dh:] = v
         out = run_varlen(qkv, lengths, H, dh, cfg)
-        assert_exact_keys(out, uniform_expect(local, length, j, VARLEN_CONFIGS[cfg][1]), f"windows {wins}")
+        assert_exact_keys(out, uniform_expect(local, length, j, VARLEN_CONFIGS[cfg]), f"windows {wins}")
 
 
 def test_attention_varlen_sequence_id_values():
@@ -464,15 +461,14 @@ def dominant_qkv(T, H, dh, alpha, g):
 def test_attention_dominant_key_lands_in_its_own_row(dh):
     H, alpha = 2, 16.0 if dh == 64 else 24.0
     g = torch.Generator(device=DEV).manual_seed(dh)
-    for cfg in ("kb64", "kb128", "kb64_fma"):
+    for cfg in ("default", "tiled"):
         for N in (1, 2, 17, 65, 128, 129, 197, 257, 512):
             B = 3
             qkv, v = dominant_qkv(B * N, H, dh, alpha, g)
             assert torch.equal(run_plain(qkv, B, N, H, dh, cfg), v), (cfg, N)
-    for cfg in ("kb64", "kb128", "fma"):
-        lengths = [1, 2, 65, 129, 511, 4097, 16384, 3]
-        qkv, v = dominant_qkv(sum(lengths), H, dh, alpha, g)
-        assert torch.equal(run_varlen(qkv, lengths, H, dh, cfg), v), cfg
+    lengths = [1, 2, 65, 129, 511, 4097, 16384, 3]
+    qkv, v = dominant_qkv(sum(lengths), H, dh, alpha, g)
+    assert torch.equal(run_varlen(qkv, lengths, H, dh, "kb64"), v)
 
 
 @pytest.mark.parametrize("dh", [32, 48, 64, 80, 128])

@@ -114,10 +114,3 @@ def test_dispatch_by_length_width_and_hooks():
             assert not is_short(names(197, dh))
     for dh in (80, 128):                           # two resident items do not fit in shared memory
         assert not is_short(names(197, dh))
-    L = _lib.lib()
-    for key, value in ((1, 2), (13, 1)):           # hooks that select instances of the tiled kernel
-        assert L.b200vit_debug_set(key, value) == 0
-        try:
-            assert not is_short(names(197, 64))
-        finally:
-            L.b200vit_debug_set(key, 0)

@@ -1,6 +1,6 @@
 """-m gpu: head widths 32, 80 and 128 through every layer that knows the head width -- the attention kernels (single
-pass and key-block, every test-hook instance), the per-head norms, the NaViT attention pooling and whole models --
-against the fp32 oracle or the module's own fp32 graph."""
+pass and key-block, and the tiled kernel test hook 15 forces), the per-head norms, the NaViT attention pooling and whole
+models -- against the fp32 oracle or the module's own fp32 graph."""
 import pytest
 import torch
 
@@ -16,13 +16,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
 
-def attention_bound(qkv, lengths, H, dh, hooks):
-    """(ref, bound) of the attention.cu instance the test hooks {key: value} select (oracle/attention_bounds.py)."""
-    kb = 128 if hooks.get(1) == 2 or hooks.get(11) == 1 else 64
-    emul = hooks.get(13) == 1 or hooks.get(11) == 2
-    return AB.qkv_attention_reference(qkv, lengths, H, dh, dh ** -0.5, kb=kb, emul=emul)
-
-
 def run_attention(qkv, B, N, H, dh, hooks):
     """b200vit_attention with test hooks {key: value} set for this call only."""
     L = _lib.lib()
@@ -33,13 +26,12 @@ def run_attention(qkv, B, N, H, dh, hooks):
         _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5)
         torch.cuda.synchronize()
     finally:
-        L.b200vit_debug_set(1, 0)
-        L.b200vit_debug_set(13, 0)
+        L.b200vit_debug_set(15, 0)
     return out
 
 
-# every instance of the single-pass kernel: 64- / 128-key blocks (hook 1) x exponentials on MUFU / half on FMA (hook 13)
-HOOKS = [{}, {1: 2}, {13: 1}, {1: 2, 13: 1}]
+# the kernel each length runs by default, and the tiled kernel at 128 < N <= 256 as well (hook 15)
+HOOKS = [{}, {15: 1}]
 GRID = [(4, 197, 12), (3, 64, 3), (2, 257, 16), (5, 50, 4), (2, 16, 2), (2, 129, 2), (1, 512, 1), (2, 1, 2),
         # more CTAs than SMs, key counts on and just past a key-block boundary
         (40, 197, 12), (70, 196, 16), (200, 128, 3), (37, 224, 5), (3, 225, 2), (9, 33, 7)]
@@ -52,53 +44,46 @@ def test_attention_new_widths(B, N, H, dh):
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV).bfloat16()
     for hooks in HOOKS:
         out = run_attention(qkv, B, N, H, dh, hooks)
-        Bd.check(out, *attention_bound(qkv, [N] * B, H, dh, hooks), f"hooks {hooks}")
+        Bd.check(out, *AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5), f"hooks {hooks}")
 
 
 @pytest.mark.parametrize("dh", [32, 128])
 @pytest.mark.parametrize("B,N,H", [(3, 257, 4), (2, 258, 2), (2, 260, 3), (40, 257, 16), (1, 261, 2), (300, 257, 2)])
 def test_attention_key_tail_new_widths(B, N, H, dh):
-    """N = 256 + (1..5) with the tail keys made the dominant ones, 64- and 128-key blocks."""
+    """N = 256 + (1..5) with the tail keys made the dominant ones."""
     torch.manual_seed(N + dh)
     I = H * dh
     qkv = torch.randn(B * N, 3 * I, device=DEV)
     qkv.view(B, N, 3, I)[:, N - 2:, 1] *= 2.5            # the last keys attract most of the attention
     qkv = qkv.bfloat16()
-    for tails in (1, 2):
-        out = run_attention(qkv, B, N, H, dh, {1: tails})
-        Bd.check(out, *attention_bound(qkv, [N] * B, H, dh, {1: tails}), f"hook 1 = {tails}")
+    out = run_attention(qkv, B, N, H, dh, {})
+    Bd.check(out, *AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5), f"key tail N{N} dh{dh}")
 
 
 @pytest.mark.parametrize("dh", [32, 80, 128])
 def test_varlen_attention_new_widths(dh):
-    """Packed sequences of mixed lengths (1 token to 1024) with every key-block instance (test hook 11 = 0 / 1 / 2)."""
+    """Packed sequences of mixed lengths (1 token to 1024)."""
     lengths = [197, 1, 130, 577, 64, 1024, 129, 65, 63, 128, 300, 1]
     H = 3
     T = sum(lengths)
     torch.manual_seed(dh)
     qkv = torch.randn(T, 3 * H * dh, device=DEV).bfloat16()
     cu, tp, tiles = _lib.varlen_index(lengths, DEV)
-    for mode in (0, 1, 2):
-        out = torch.full((T, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
-        _lib.lib().b200vit_debug_set(11, mode)
-        try:
-            _lib.attention_varlen(qkv, out, cu, tp, tiles, H, dh, dh ** -0.5)
-            torch.cuda.synchronize()
-        finally:
-            _lib.lib().b200vit_debug_set(11, 0)
-        Bd.check(out, *attention_bound(qkv, lengths, H, dh, {11: mode}), f"hook 11 = {mode}")
+    out = torch.full((T, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
+    _lib.attention_varlen(qkv, out, cu, tp, tiles, H, dh, dh ** -0.5)
+    torch.cuda.synchronize()
+    Bd.check(out, *AB.qkv_attention_reference(qkv, lengths, H, dh, dh ** -0.5), f"varlen dh{dh}")
 
 
 def test_attention_dh128_is_deterministic_and_batch_invariant():
     torch.manual_seed(11)
     B, N, H, dh = 64, 197, 8, 128
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV).bfloat16()
-    for hooks in ({}, {1: 2}):
-        out = run_attention(qkv, B, N, H, dh, hooks)
-        out2 = run_attention(qkv, B, N, H, dh, hooks)
-        assert torch.equal(out, out2), hooks
-        out3 = run_attention(qkv[5 * N: 9 * N].contiguous(), 4, N, H, dh, hooks)
-        assert torch.equal(out3, out[5 * N: 9 * N]), hooks
+    out = run_attention(qkv, B, N, H, dh, {})
+    out2 = run_attention(qkv, B, N, H, dh, {})
+    assert torch.equal(out, out2)
+    out3 = run_attention(qkv[5 * N: 9 * N].contiguous(), 4, N, H, dh, {})
+    assert torch.equal(out3, out[5 * N: 9 * N])
 
 
 def _layernorm_heads(buf, gamma, nheads, dh, eps):

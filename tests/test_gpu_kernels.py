@@ -198,48 +198,22 @@ def test_gelu_epilogue_accuracy():
                                    (1, 512, 1), (2, 1, 2),
                                    # more CTAs than SMs, key counts on and just past a key-block boundary
                                    (40, 197, 12), (70, 196, 16), (200, 128, 3), (37, 224, 5), (3, 225, 2), (9, 33, 7)])
-@pytest.mark.parametrize("kernel", [0, 2])      # test hook 1: 0 = 64-key blocks (default), 2 = 128-key blocks
-def test_attention(B, N, H, kernel):
+@pytest.mark.parametrize("tiled", [False, True])  # test hook 15: the tiled kernel at 128 < N <= 256 as well
+def test_attention(B, N, H, tiled):
     torch.manual_seed(N)
     dh = 64
     I = H * dh
     qkv = torch.randn(B * N, 3 * I, device=DEV).bfloat16()
     out = torch.full((B * N, I), float("nan"), device=DEV, dtype=torch.bfloat16)   # unwritten elements fail
-    _lib.lib().b200vit_debug_set(1, kernel)
+    _lib.lib().b200vit_debug_set(15, int(tiled))
     try:
         _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5)
         torch.cuda.synchronize()
     finally:
-        _lib.lib().b200vit_debug_set(1, 0)
+        _lib.lib().b200vit_debug_set(15, 0)
     # every element within its bound of the fp64 attention that replays the kernel's bf16 P (oracle/attention_bounds.py)
-    ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5, kb=128 if kernel == 2 else 64)
-    Bd.check(out, ref, bound, f"attention B{B} N{N} H{H} hook 1 = {kernel}")
-
-
-@pytest.mark.parametrize("knob,value,B,N", [(1, 2, 3, 197), (1, 2, 40, 128), (1, 2, 2, 50), (13, 1, 3, 197)])
-def test_attention_kernel_variants_agree(knob, value, B, N):
-    """b200vit_debug_set(1, 2) streams the keys in 128-key blocks, (13, 1) puts half of the softmax exponentials on
-    the FMA pipe: every implementation must produce the same attention, each within the bound of its own arithmetic."""
-    L = _lib.lib()
-    torch.manual_seed(7)
-    H, dh = 4, 64
-    qkv = torch.randn(B * N, 3 * H * dh, device=DEV).bfloat16()
-    ref_out = torch.full((B * N, H * dh), float("nan"), device=DEV, dtype=torch.bfloat16)
-    _lib.attention(qkv, ref_out, B, N, H, dh, dh ** -0.5)
-    out = torch.full_like(ref_out, float("nan"))
-    L.b200vit_debug_set(knob, value)
-    if knob == 13:
-        L.b200vit_debug_set(1, 2)
-    try:
-        _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5)
-        torch.cuda.synchronize()
-    finally:
-        L.b200vit_debug_set(knob, 0)
-        L.b200vit_debug_set(1, 0)
-    Bd.check(ref_out, *AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5), "64-key blocks")
-    # (13, 1) runs with 128-key blocks as well
-    ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5, kb=128, emul=knob == 13)
-    Bd.check(out, ref, bound, f"hook {knob} = {value}")
+    ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5)
+    Bd.check(out, ref, bound, f"attention B{B} N{N} H{H} hook 15 = {tiled}")
 
 
 @pytest.mark.parametrize("B,N,H", [(2, 257, 16), (3, 197, 4), (5, 64, 2), (2, 400, 3), (1, 512, 2), (40, 129, 5)])
@@ -261,34 +235,24 @@ def test_attention_dim_head_80(B, N, H):
 @pytest.mark.parametrize("dh", [64, 80])
 @pytest.mark.parametrize("B,N,H", [(3, 257, 4), (2, 258, 2), (2, 260, 3), (40, 257, 16), (1, 261, 2), (300, 257, 2)])
 def test_attention_key_tail(B, N, H, dh):
-    """N = 256 + (1..5): the last keys sit alone in the final key block.  Checked against the fp32 oracle with the tail
-    keys made the dominant ones, with 64-key and 128-key blocks (test hook 1 = 1 / 2), each within its bound."""
+    """N = 256 + (1..5): the last keys sit alone in the final key block.  Checked against the fp64 oracle with the tail
+    keys made the dominant ones."""
     torch.manual_seed(N + dh)
     I = H * dh
     qkv = torch.randn(B * N, 3 * I, device=DEV)
     qkv.view(B, N, 3, I)[:, N - 2:, 1] *= 2.5            # the last keys attract most of the attention
     qkv = qkv.bfloat16()
-    L = _lib.lib()
-    outs = {}
-    for tails in (1, 2):
-        out = torch.full((B * N, I), float("nan"), device=DEV, dtype=torch.bfloat16)
-        L.b200vit_debug_set(1, tails)
-        try:
-            _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5)
-            torch.cuda.synchronize()
-        finally:
-            L.b200vit_debug_set(1, 0)
-        outs[tails] = out
-    for tails in (1, 2):
-        ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5, kb=128 if tails == 2 else 64)
-        Bd.check(outs[tails], ref, bound, f"key tail N{N} dh{dh} hook 1 = {tails}")
+    out = torch.full((B * N, I), float("nan"), device=DEV, dtype=torch.bfloat16)
+    _lib.attention(qkv, out, B, N, H, dh, dh ** -0.5)
+    ref, bound = AB.qkv_attention_reference(qkv, [N] * B, H, dh, dh ** -0.5)
+    Bd.check(out, ref, bound, f"key tail N{N} dh{dh}")
 
 
 def test_attention_is_deterministic_and_batch_invariant():
     """The same (image, head) must give the same bits wherever it lands in the batch and on repeated launches."""
     torch.manual_seed(11)
     B, N, H, dh = 64, 197, 12, 64
-    _lib.lib().b200vit_debug_set(1, 2)          # 128-key blocks (test hook), restored below
+    _lib.lib().b200vit_debug_set(15, 1)         # the tiled kernel at N 197 (test hook), restored below
     qkv = torch.randn(B * N, 3 * H * dh, device=DEV).bfloat16()
     out = torch.zeros(B * N, H * dh, device=DEV, dtype=torch.bfloat16)
     out2 = torch.zeros_like(out)
@@ -299,7 +263,7 @@ def test_attention_is_deterministic_and_batch_invariant():
     out3 = torch.zeros(4 * N, H * dh, device=DEV, dtype=torch.bfloat16)
     _lib.attention(sub, out3, 4, N, H, dh, dh ** -0.5)
     torch.cuda.synchronize()
-    _lib.lib().b200vit_debug_set(1, 0)
+    _lib.lib().b200vit_debug_set(15, 0)
     assert torch.equal(out3, out[5 * N: 9 * N])
 
 

@@ -38,7 +38,8 @@ struct AttnParams {
 // A head of DH columns is DH / 64 slabs 64 columns wide (128B swizzle) followed by (DH % 64) / 16 slabs 16 columns
 // wide (32B swizzle): dh 32 = 2 x 16, 64 = 64, 80 = 64 + 16, 128 = 2 x 64.  Shared memory: Q64[N64] | Q16[N16], then
 // per stage K64[N64] | V64[N64] | K16[N16] | V16[N16].
-template <int DH, int KB>
+constexpr int KB = 64;  // keys per block
+template <int DH>
 struct AttnSmem {
   static constexpr int N64 = DH / 64;
   static constexpr int N16 = (DH % 64) / 16;
@@ -56,14 +57,14 @@ struct AttnSmem {
 };
 
 // CTAs per SM the register budget is planned for (ptxas -v: no spills at these bounds)
-constexpr int att_min_blocks(int dh, int kb) { return (dh == 64 && kb == 64) || dh == 32 ? 2 : 1; }
+constexpr int att_min_blocks(int dh) { return dh == 64 || dh == 32 ? 2 : 1; }
 
-template <int DH, int KB, bool VARLEN, bool EMUL, bool MASK_SELF>
-__global__ void __launch_bounds__(ATT_THREADS, att_min_blocks(DH, KB))
+template <int DH, bool VARLEN, bool MASK_SELF>
+__global__ void __launch_bounds__(ATT_THREADS, att_min_blocks(DH))
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                  const __grid_constant__ CUtensorMap tmQ16, const __grid_constant__ CUtensorMap tmKV16,
                  const AttnParams p) {
-  using L = AttnSmem<DH, KB>;
+  using L = AttnSmem<DH>;
   constexpr int N64 = L::N64, N16 = L::N16;
   constexpr int NS = KB / 2;  // score accumulators per thread
   extern __shared__ uint8_t smem_raw[];
@@ -192,15 +193,13 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       for (int k = 0; k < 4; ++k) {
         const uint64_t ad = make_wgmma_desc(qa + c * L::Q64, 1024, WGMMA_SW128) + 2 * k;
         const uint64_t bd = make_wgmma_desc(sb + c * L::KV64, 1024, WGMMA_SW128) + 2 * k;
-        if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, c != 0 || k != 0);
-        else wgmma_m64n64k16(s, ad, bd, c != 0 || k != 0);
+        wgmma_m64n64k16(s, ad, bd, c != 0 || k != 0);
       }
 #pragma unroll
     for (int c = 0; c < N16; ++c) {
       const uint64_t ad = make_wgmma_desc(qa16 + c * L::Q16, 256, WGMMA_SW32);
       const uint64_t bd = make_wgmma_desc(sb + L::K16_OFF + c * L::KV16, 256, WGMMA_SW32);
-      if constexpr (KB == 128) wgmma_m64n128k16(s, ad, bd, N64 != 0 || c != 0);
-      else wgmma_m64n64k16(s, ad, bd, N64 != 0 || c != 0);
+      wgmma_m64n64k16(s, ad, bd, N64 != 0 || c != 0);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -246,17 +245,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     for (int j = 0; j < KB / 8; ++j) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        float e0, e1;
-        const float x0 = s[4 * j + 2 * r] - m[r], x1 = s[4 * j + 2 * r + 1] - m[r];
-        if (EMUL && (j & 1)) {
-          // half of the exponentials on the FMA pipe (masked keys are -inf: forced to 0)
-          exp2_emul2(f2_make(x0, x1), e0, e1);
-          e0 = s[4 * j + 2 * r] == -INFINITY ? 0.f : e0;
-          e1 = s[4 * j + 2 * r + 1] == -INFINITY ? 0.f : e1;
-        } else {
-          e0 = fast_ex2(x0);
-          e1 = fast_ex2(x1);
-        }
+        const float e0 = fast_ex2(s[4 * j + 2 * r] - m[r]), e1 = fast_ex2(s[4 * j + 2 * r + 1] - m[r]);
         s[4 * j + 2 * r] = e0;
         s[4 * j + 2 * r + 1] = e1;
         l[r] += e0 + e1;
@@ -321,9 +310,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 // Tensor maps over qkv[T, 3 I] (varlen) or its [B][N][3 I] view (fixed length, T = B N): 64-column boxes (128B swizzle)
 // of 128 query rows / KB key rows for the 64-wide slabs, and the same with 16 columns (32B swizzle) for the 16-wide
 // ones.  A kind the head does not use gets a copy of the other (never read).
-template <int DH, int KB, bool VARLEN, bool EMUL, bool MASK_SELF>
+template <int DH, bool VARLEN, bool MASK_SELF>
 static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 grid, cudaStream_t stream) {
-  using L = AttnSmem<DH, KB>;
+  using L = AttnSmem<DH>;
   CUtensorMap tm[4];
   const int rank = VARLEN ? 2 : 3;
   const uint64_t ld = (uint64_t)3 * p.I;
@@ -339,7 +328,7 @@ static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 
   if (rc) return rc;
   if (!L::N16) tm[2] = tm[0], tm[3] = tm[1];
   if (!L::N64) tm[0] = tm[2], tm[1] = tm[3];
-  auto kern = attention_kernel<DH, KB, VARLEN, EMUL, MASK_SELF>;
+  auto kern = attention_kernel<DH, VARLEN, MASK_SELF>;
   B200_ENSURE_SMEM(kern, L::BYTES);
   kern<<<grid, ATT_THREADS, L::BYTES, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -347,35 +336,27 @@ static int launch_attention_t(const void* qkv, int T, const AttnParams& p, dim3 
   return 0;
 }
 
-// the self-masked instances exist for the default key block and exponential mode only (test hooks 1, 11, 13 do not
-// apply to them)
 template <int DH, bool VARLEN>
-static int launch_attention_dh(const void* qkv, int T, const AttnParams& p, int kb, bool emul, bool mask_self,
-                               dim3 grid, cudaStream_t st) {
-  if (mask_self) return launch_attention_t<DH, 64, VARLEN, false, true>(qkv, T, p, grid, st);
-  if (kb == 128) return emul ? launch_attention_t<DH, 128, VARLEN, true, false>(qkv, T, p, grid, st)
-                             : launch_attention_t<DH, 128, VARLEN, false, false>(qkv, T, p, grid, st);
-  return emul ? launch_attention_t<DH, 64, VARLEN, true, false>(qkv, T, p, grid, st)
-              : launch_attention_t<DH, 64, VARLEN, false, false>(qkv, T, p, grid, st);
+static int launch_attention_dh(const void* qkv, int T, const AttnParams& p, bool mask_self, dim3 grid,
+                               cudaStream_t st) {
+  return mask_self ? launch_attention_t<DH, VARLEN, true>(qkv, T, p, grid, st)
+                   : launch_attention_t<DH, VARLEN, false>(qkv, T, p, grid, st);
 }
 
 // one instance per width of head_width_ok() (dh 96 = 64 + 2 x 16 would fall out of the same slab scheme)
 template <bool VARLEN>
-static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, int kb, bool emul, bool mask_self,
-                            dim3 grid, cudaStream_t st) {
+static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, bool mask_self, dim3 grid,
+                            cudaStream_t st) {
   switch (dh) {
-    case 32: return launch_attention_dh<32, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
-    case 80: return launch_attention_dh<80, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
-    case 128: return launch_attention_dh<128, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
-    default: return launch_attention_dh<64, VARLEN>(qkv, T, p, kb, emul, mask_self, grid, st);
+    case 32: return launch_attention_dh<32, VARLEN>(qkv, T, p, mask_self, grid, st);
+    case 80: return launch_attention_dh<80, VARLEN>(qkv, T, p, mask_self, grid, st);
+    case 128: return launch_attention_dh<128, VARLEN>(qkv, T, p, mask_self, grid, st);
+    default: return launch_attention_dh<64, VARLEN>(qkv, T, p, mask_self, grid, st);
   }
 }
 
-// test hooks (include/b200vit.h)
-static std::atomic<int> g_attn_mode{0};    // key 1
-static std::atomic<int> g_attn_emul{0};    // key 13
-static std::atomic<int> g_varlen_mode{0};  // key 11
-static std::atomic<int> g_attn_tiled{0};   // key 15
+// test hook (include/b200vit.h)
+static std::atomic<int> g_attn_tiled{0};  // key 15
 
 }  // namespace b200
 
@@ -383,10 +364,7 @@ using namespace b200;
 
 extern "C" int b200vit_debug_set(int key, int value) {
   switch (key) {
-    case 1: g_attn_mode = value; return 0;
-    case 11: g_varlen_mode = value; return 0;
     case 12: gemm_set_block_n(value); return 0;
-    case 13: g_attn_emul = value; return 0;
     case 14: gemm_set_direct_store(value); return 0;
     case 15: g_attn_tiled = value; return 0;
     default: return B200VIT_ERR_INVALID;
@@ -408,9 +386,8 @@ extern "C" int b200vit_attention_ex(const void* qkv, void* out, int B, int N, in
   B200_CHECK_ARG(B <= 65535, "attention: B=%d exceeds the grid", B);
   B200_CHECK_ARG((flags & ~B200VIT_ATTN_MASK_SELF) == 0, "attention: unknown flags 0x%x", flags);
   // 129 to 256 tokens: the persistent kernel of attention_short.cu, which gives the same bits.  The self-masked
-  // instances and the ones test hooks 1 and 13 select exist in this file only, and hook 15 asks for this file's kernel.
-  const bool tiled_only = (flags & B200VIT_ATTN_MASK_SELF) || g_attn_mode.load() != 0 || g_attn_emul.load() != 0 ||
-                          g_attn_tiled.load() != 0;
+  // instances exist in this file only, and test hook 15 asks for this file's kernel.
+  const bool tiled_only = (flags & B200VIT_ATTN_MASK_SELF) || g_attn_tiled.load() != 0;
   if (!tiled_only && attention_short_ok(N, dh))
     return attention_short(qkv, out, B, N, H, dh, scale * 1.4426950408889634f, reinterpret_cast<cudaStream_t>(stream));
   AttnParams p{};
@@ -420,8 +397,8 @@ extern "C" int b200vit_attention_ex(const void* qkv, void* out, int B, int N, in
   p.I = H * dh;
   p.scale_log2e = scale * 1.4426950408889634f;
   const dim3 grid((N + ATT_QROWS - 1) / ATT_QROWS, H, B);
-  return launch_attention<false>(qkv, B * N, p, dh, g_attn_mode.load() == 2 ? 128 : 64, g_attn_emul.load() != 0,
-                                 (flags & B200VIT_ATTN_MASK_SELF) != 0, grid, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention<false>(qkv, B * N, p, dh, (flags & B200VIT_ATTN_MASK_SELF) != 0, grid,
+                                 reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev,
@@ -450,8 +427,7 @@ extern "C" int b200vit_attention_varlen_ex(const void* qkv, void* out, const int
   p.H = H;
   p.I = H * dh;
   p.scale_log2e = scale * 1.4426950408889634f;
-  const int mode = g_varlen_mode.load();
   const dim3 grid(total_tiles, H, 1);
-  return launch_attention<true>(qkv, total_tokens, p, dh, mode == 1 ? 128 : 64, mode == 2,
-                                (flags & B200VIT_ATTN_MASK_SELF) != 0, grid, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention<true>(qkv, total_tokens, p, dh, (flags & B200VIT_ATTN_MASK_SELF) != 0, grid,
+                                reinterpret_cast<cudaStream_t>(stream));
 }

@@ -387,28 +387,6 @@ __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
 __device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
-// 2^x for x <= 0 on the FMA / ALU pipes instead of MUFU (two elements per call): round-to-nearest split x = n + f with the
-// 1.5*2^23 trick, degree-3 minimax polynomial for 2^f on [-0.5, 0.5] (max rel. error 7.5e-5, far below the bf16
-// resolution of the probabilities it feeds), exponent patched in with an integer add.  Used for a fraction of the
-// softmax exponentials so that the MUFU pipe is no longer the only exp engine.
-__device__ __forceinline__ void exp2_emul2(f32x2 x, float& e0, float& e1) {
-  float x0, x1;
-  f2_get(x, x0, x1);
-  x = f2_make(fmaxf(x0, -125.0f), fmaxf(x1, -125.0f));
-  const f32x2 t = f2_add(x, f2_make(12582912.0f, 12582912.0f));
-  const f32x2 n = f2_add(t, f2_make(-12582912.0f, -12582912.0f));
-  const f32x2 f = f2_fma(n, f2_make(-1.0f, -1.0f), x);
-  f32x2 pl = f2_fma(f2_make(0.05517210811376572f, 0.05517210811376572f), f,
-                    f2_make(0.24261118471622467f, 0.24261118471622467f));
-  pl = f2_fma(pl, f, f2_make(0.693260908126831f, 0.693260908126831f));
-  pl = f2_fma(pl, f, f2_make(0.9999280571937561f, 0.9999280571937561f));
-  float p0, p1, t0, t1;
-  f2_get(pl, p0, p1);
-  f2_get(t, t0, t1);
-  e0 = __uint_as_float(__float_as_uint(p0) + (__float_as_uint(t0) << 23));
-  e1 = __uint_as_float(__float_as_uint(p1) + (__float_as_uint(t1) << 23));
-}
-
 // GELU in its exact-erf definition (nn.GELU() default, reference vit.py:21), evaluated as x * Phi(x) with
 //   Phi(x) = 1 / (1 + exp(-x * (c0 + c1 x^2 + c2 x^4 + c3 x^6))),   x^2 clamped to 36 inside the polynomial,
 // the odd polynomial being a minimax fit of logit(Phi) (max |gelu_fit - gelu_erf| = 1.2e-5 over all x, checked in
