@@ -65,6 +65,10 @@ extern "C" {
 #define B200VIT_CROSS_EMBED_MAX_STRIDE 8     /* the shared stride s */
 #define B200VIT_CROSS_EMBED_MAX_WIDTH 64     /* output channels n of a scale (a multiple of 8) */
 
+/* what b200vit_attention_wide (the soft-split attention of T2T-ViT, one head as wide as the token) is built for */
+#define B200VIT_ATTN_WIDE_MAX_TOKENS 1024  /* tokens n per image */
+#define B200VIT_ATTN_WIDE_MAX_WIDTH 4096   /* padded head width dp */
+
 const char* b200vit_last_error(void);
 int b200vit_version(void);
 /* number of kernels this library has launched in the calling process (all threads) since load / last reset */
@@ -83,7 +87,9 @@ int b200vit_device_ok(int dev);
  * EPI_LNFOLD: ln_sums[M][ln_parts][2] = per-row PARTIAL (sum, sum of squares) of A (added up in index order, so the
  *             result is deterministic), ln_dim = K, col_s[N] = sum_k W[n,k] (fp32).
  * EPI_STATS:  stats_out[M][P][2], P = b200vit_stats_parts(N): every slot is written exactly once (no atomics).
- * Requirements: A, W 16-byte aligned, lda, ldw multiples of 8, K multiple of 8.
+ * Requirements: A, W 16-byte aligned, lda, ldw multiples of 8 and >= K.  Any K >= 1: the operands are read through
+ * TMA, which zero-fills columns K .. of a k block, so columns past K of A and W are never read (T2T-ViT's soft splits
+ * run at K = the true width w, e.g. 147 or 1323).
  */
 int b200vit_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void* out_bf16, float* out_f32,
                       int64_t ldo, const float* bias, const float* resid, const float* ln_sums, int ln_parts,
@@ -208,7 +214,8 @@ int b200vit_attention_ex(const void* qkv, void* out, int B, int N, int H, int dh
  * Variable-length attention over PACKED sequences (any length): tokens [cu_seqlens[s], cu_seqlens[s+1]) of
  * qkv[total_tokens, 3*H*dh] attend only among themselves; out[total_tokens, H*dh].  This is the block-diagonal
  * "same image" attention of NaViT (na_vit.py:335-337 mask + 161-166 SDPA) without padding or an O(L^2) mask, and the
- * long-sequence (N > 512) path of ViT.  dh = 32, 64, 80 or 128.  cu_seqlens_dev[num_seqs+1] and tile_prefix_dev[num_seqs+1] (number of 128-row
+ * long-sequence (N > 512) path of ViT.  dh = 32, 64, 80 or 128, and 160 without B200VIT_ATTN_MASK_SELF (the one head of a
+ * T2T-ViT soft-split layer up to 160 wide, t2t.py:40 / vit.py Attention, 2 x 64 + 2 x 16 column slabs).  cu_seqlens_dev[num_seqs+1] and tile_prefix_dev[num_seqs+1] (number of 128-row
  * query tiles before sequence s; tile_prefix[num_seqs] == total_tiles) are DEVICE int32 arrays built by the caller.
  */
 int b200vit_attention_varlen(const void* qkv, void* out, const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev,
@@ -837,6 +844,44 @@ int b200vit_encoder_blocks_ex(const b200vit_layer* layers, int depth, float* x, 
                               const int32_t* cu_seqlens_dev, const int32_t* tile_prefix_dev, int total_tiles,
                               const float* rope_cs, int rope_rows, const float* layer_scales, int attn_flags,
                               void* stream);
+
+/*
+ * T2T-ViT soft split (nn.Unfold(k, stride=s, padding=p) + Rearrange('b c n -> b n c'), t2t.py:37-38) as bit copies:
+ *   out[b*oh*ow + r*ow + q, c*k*k + i*k + j] = src(b, c, r*s - p + i, q*s - p + j), 0 outside the map,
+ * oh = (H + 2p - k) / s + 1 (likewise ow), channel-major columns (nn.Unfold's order), columns [C*k*k, ldo) zero filled.
+ * Exactly one of out_bf16 (the A operand of a GEMM) and out_f32 (the fp32 residual stream of the soft-split Transformer
+ * that follows) is given; ldo a multiple of 8 and >= C*k*k; out 16-byte aligned.  1 <= k, 1 <= s, 0 <= p < k, and the
+ * padded map at least one window wide.  Every output row reads its own image's pixels / tokens only.
+ * _image: src = img[B, C, H, W] bf16 (the first stage).
+ * _tokens: src = x[B*n, ldx] bf16 (ldx >= C), the token rows of the previous soft-split Transformer's final LayerNorm,
+ *   read as RearrangeImage does (t2t.py:20-22): a map of h = int(sqrt(n)) rows of w = n / h tokens, token r*w + c of
+ *   image b at row b*n + r*w + c, channel c at column c.  An n that h does not divide is rejected (einops raises).
+ */
+int b200vit_t2t_unfold_image(const void* img, void* out_bf16, float* out_f32, int64_t ldo, int B, int C, int H, int W,
+                             int k, int s, int p, void* stream);
+int b200vit_t2t_unfold_tokens(const void* x, int64_t ldx, int B, int n, int C, void* out_bf16, float* out_f32,
+                              int64_t ldo, int k, int s, int p, void* stream);
+
+/*
+ * Softmax attention of ONE head as wide as the token: the attention of a T2T-ViT soft-split Transformer (heads == 1,
+ * dim_head == dim, t2t.py:40 / vit.py Attention), for widths past the 160 of b200vit_attention_varlen.
+ *   qkv[B*n, 3*dp] bf16, columns [q | k | v], each padded from the true width w to dp with zero columns (zero rows of
+ *   the projection), image b at rows b*n ..;  O = softmax(q k^T * scale) v, scale = w^-0.5 of the TRUE width.
+ * The scores are materialised per image, in the caller's workspace (the library allocates nothing):
+ *   S = scale * Q K^T in fp32 (wgmma: bf16 products, fp32 accumulation), P = softmax(S) rounded to bf16 once,
+ *   O = P V accumulated in fp32 (wgmma) and rounded to bf16.
+ * Outputs: out[B*n, dp] bf16 (may be NULL) and/or, x given, x[(b*n + i)*ldx + c] += bf16(O[b*n + i, c]) for
+ * c < n_resid -- the residual add of the identity to_out (vit.py: heads == 1 and dim_head == dim) on the true columns.
+ * Limits: n <= B200VIT_ATTN_WIDE_MAX_TOKENS, dp a multiple of 64 and <= B200VIT_ATTN_WIDE_MAX_WIDTH; qkv, out and ws
+ * 16-byte aligned.  ws_bytes >= b200vit_attention_wide_workspace(n, dp, 1); the batch runs in chunks of as many images
+ * as the workspace holds (b200vit_attention_wide_workspace(n, dp, images) bytes hold `images`), three launches each.
+ * Isolation: q, k, v and P reach the tensor cores through 3-D tensor maps (column, token, image) that zero-fill past
+ * each image's n tokens, so a NaN or Inf in one image leaves every other image's output bit-identical, and no row past
+ * B*n is read.
+ */
+int64_t b200vit_attention_wide_workspace(int n, int dp, int images);
+int b200vit_attention_wide(const void* qkv, void* out, float* x, int64_t ldx, int n_resid, int B, int n, int dp,
+                           float scale, void* ws, int64_t ws_bytes, void* stream);
 
 /*
  * TEST HOOKS -- process-global switches for A/B tests and bring-up; NOT part of the re-entrant API above (a value set

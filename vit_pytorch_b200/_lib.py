@@ -30,6 +30,8 @@ ATTN_GELU_OUT = 4
 ATTN_POSBIAS_MAX_KEYS = 4096    # B200VIT_ATTN_POSBIAS_MAX_KEYS
 MBCONV_PART_ROWS = 64           # B200VIT_MBCONV_PART_ROWS
 ATTN_GROUPS_MAX_TOKENS = 4096   # B200VIT_ATTN_GROUPS_MAX_TOKENS
+ATTN_WIDE_MAX_TOKENS = 1024     # B200VIT_ATTN_WIDE_MAX_TOKENS
+ATTN_WIDE_MAX_WIDTH = 4096      # B200VIT_ATTN_WIDE_MAX_WIDTH
 
 # every symbol include/b200vit.h declares (tests check that the library exports each of them)
 SYMBOLS = [
@@ -51,6 +53,8 @@ SYMBOLS = [
     "b200vit_attention_groups", "b200vit_conv_im2col_nhwc_ex", "b200vit_attention_window_token",
     "b200vit_window_mix", "b200vit_head_layernorm_gelu", "b200vit_attention_region_local",
     "b200vit_nest_level_entry", "b200vit_nest_im2col", "b200vit_attention_kv_ex", "b200vit_attention_iwsa",
+    "b200vit_t2t_unfold_image", "b200vit_t2t_unfold_tokens", "b200vit_attention_wide",
+    "b200vit_attention_wide_workspace",
 ]
 
 
@@ -229,6 +233,14 @@ def lib() -> C.CDLL:
     L.b200vit_encoder_blocks_ex.restype = i32
     L.b200vit_encoder_blocks_ex.argtypes = [C.POINTER(Layer), i32, vp, C.POINTER(EncoderWs), i32, i32, i32, i32, i32,
                                             i32, f32, i32, vp, vp, i32, vp, i32, C.POINTER(C.c_float), i32, vp]
+    L.b200vit_t2t_unfold_image.restype = i32
+    L.b200vit_t2t_unfold_image.argtypes = [vp, vp, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]
+    L.b200vit_t2t_unfold_tokens.restype = i32
+    L.b200vit_t2t_unfold_tokens.argtypes = [vp, i64, i32, i32, i32, vp, vp, i64, i32, i32, i32, vp]
+    L.b200vit_attention_wide_workspace.restype = i64
+    L.b200vit_attention_wide_workspace.argtypes = [i32, i32, i32]
+    L.b200vit_attention_wide.restype = i32
+    L.b200vit_attention_wide.argtypes = [vp, vp, vp, i64, i32, i32, i32, i32, f32, vp, i64, vp]
     _lib = L
     return L
 
@@ -1386,3 +1398,68 @@ def cast_f32_bf16(x: torch.Tensor, out: torch.Tensor) -> None:
     with _Timed("cast", bytes=x.numel() * 6):
         rc = lib().b200vit_cast_f32_bf16(_ptr(x), _ptr(out), x.numel(), _stream())
     _check(rc, "b200vit_cast_f32_bf16")
+
+
+def _unfold_out(out: torch.Tensor, rows: int, K: int, what: str):
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[0] == rows and out.shape[1] >= K, \
+        f"{what}: out must be [{rows}, >= {K}], got {tuple(out.shape)}"
+    if out.dtype == torch.float32:
+        _chk(out, torch.float32, "out")
+        return None, out
+    _chk(out, torch.bfloat16, "out")
+    return out, None
+
+
+def t2t_unfold_image(img: torch.Tensor, out: torch.Tensor, k: int, s: int, p: int) -> None:
+    """img [B, C, H, W] bf16 -> out [B*oh*ow, ldo] (bf16 or fp32) rows of F.unfold(img, k, padding=p, stride=s)
+    .transpose(1, 2) (columns (c, i, j), channel slowest), zero K padding up to ldo = out.stride(0)."""
+    _chk(img, torch.bfloat16, "img")
+    assert img.is_contiguous() and img.dim() == 4
+    B, Cc, H, W = img.shape
+    rows = B * conv_out_size(H, k, s, p) * conv_out_size(W, k, s, p)
+    ob, of = _unfold_out(out, rows, Cc * k * k, "t2t_unfold_image")
+    with _Timed("t2t_unfold", bytes=img.numel() * 2 + rows * out.stride(0) * out.element_size()):
+        rc = lib().b200vit_t2t_unfold_image(_ptr(img), _ptr(ob), _ptr(of), out.stride(0), B, Cc, H, W, int(k), int(s),
+                                            int(p), _stream())
+    _check(rc, "b200vit_t2t_unfold_image")
+
+
+def t2t_unfold_tokens(x: torch.Tensor, grid, out: torch.Tensor, k: int, s: int, p: int) -> None:
+    """x [B*n, C] bf16 (rows x.stride(0) apart), the token rows of B images read as the map grid = (h, w) that
+    RearrangeImage makes of n = h*w tokens (pit.pool_grid; the library checks h == int(sqrt(n))) -> out [B*oh*ow, ldo]
+    (bf16 or fp32) rows of the zero-padded unfold, as t2t_unfold_image."""
+    _chk(x, torch.bfloat16, "x")
+    h, w = grid
+    n = h * w
+    assert x.dim() == 2 and x.stride(1) == 1 and x.shape[0] % n == 0
+    B, Cc = x.shape[0] // n, x.shape[1]
+    rows = B * conv_out_size(h, k, s, p) * conv_out_size(w, k, s, p)
+    ob, of = _unfold_out(out, rows, Cc * k * k, "t2t_unfold_tokens")
+    with _Timed("t2t_unfold", bytes=x.shape[0] * Cc * 2 + rows * out.stride(0) * out.element_size()):
+        rc = lib().b200vit_t2t_unfold_tokens(_ptr(x), x.stride(0), B, int(n), Cc, _ptr(ob), _ptr(of), out.stride(0),
+                                             int(k), int(s), int(p), _stream())
+    _check(rc, "b200vit_t2t_unfold_tokens")
+
+
+def attention_wide_workspace(n: int, dp: int, images: int) -> int:
+    """Bytes of the workspace b200vit_attention_wide needs to run `images` images per chunk."""
+    return int(lib().b200vit_attention_wide_workspace(int(n), int(dp), int(images)))
+
+
+def attention_wide(qkv: torch.Tensor, B: int, n: int, dp: int, scale: float, ws: torch.Tensor, *,
+                   out: Optional[torch.Tensor] = None, x: Optional[torch.Tensor] = None,
+                   n_resid: int = 0) -> None:
+    """One head as wide as the token over B images of n tokens: qkv [B*n, 3*dp] bf16 -> out [B*n, dp] bf16 and/or, x
+    fp32 given (rows x.stride(0) apart), x[:, :n_resid] += bf16(O[:, :n_resid]).  ws: uint8 scratch (any size holding
+    one image, see attention_wide_workspace)."""
+    _chk(qkv, torch.bfloat16, "qkv"); _chk(out, torch.bfloat16, "out"); _chk(x, torch.float32, "x")
+    _chk(ws, torch.uint8, "ws")
+    assert qkv.is_contiguous() and qkv.shape == (B * n, 3 * dp) and ws.is_contiguous()
+    assert out is None or (out.is_contiguous() and out.shape == (B * n, dp))
+    assert x is None or (x.dim() == 2 and x.stride(1) == 1 and x.shape[0] == B * n)
+    with _Timed("attention_wide", B=B, N=n, H=1, bytes=(qkv.numel() + B * n * dp) * 2,
+                flops=4.0 * B * n * n * dp):
+        rc = lib().b200vit_attention_wide(_ptr(qkv), _ptr(out), _ptr(x), 0 if x is None else x.stride(0),
+                                          int(n_resid), B, int(n), int(dp), float(scale), _ptr(ws), ws.numel(),
+                                          _stream())
+    _check(rc, "b200vit_attention_wide")

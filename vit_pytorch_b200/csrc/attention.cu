@@ -56,7 +56,8 @@ struct AttnSmem {
   static constexpr int BYTES = BAR_OFF + 5 * 8 + 1024;  // full[2], empty[2], q; slack for 1024B alignment
 };
 
-// CTAs per SM the register budget is planned for (ptxas -v: no spills at these bounds)
+// CTAs per SM the register budget is planned for (ptxas -v: no spills at these bounds).  dh 160 = 2 x 64 + 2 x 16
+// (varlen only, the one head of a T2T-ViT soft split up to 160 wide): 40 KB of Q and two 40 KB K / V stages.
 constexpr int att_min_blocks(int dh) { return dh == 64 || dh == 32 ? 2 : 1; }
 
 template <int DH, bool VARLEN, bool MASK_SELF>
@@ -343,10 +344,13 @@ static int launch_attention_dh(const void* qkv, int T, const AttnParams& p, bool
                    : launch_attention_t<DH, VARLEN, false>(qkv, T, p, grid, st);
 }
 
-// one instance per width of head_width_ok() (dh 96 = 64 + 2 x 16 would fall out of the same slab scheme)
+// one instance per width of head_width_ok() (dh 96 = 64 + 2 x 16 would fall out of the same slab scheme), and the
+// varlen kernel at dh 160 without self-masking (varlen_head_width_ok)
 template <bool VARLEN>
 static int launch_attention(const void* qkv, int T, const AttnParams& p, int dh, bool mask_self, dim3 grid,
                             cudaStream_t st) {
+  if constexpr (VARLEN)
+    if (dh == 160) return launch_attention_t<160, true, false>(qkv, T, p, grid, st);
   switch (dh) {
     case 32: return launch_attention_dh<32, VARLEN>(qkv, T, p, mask_self, grid, st);
     case 80: return launch_attention_dh<80, VARLEN>(qkv, T, p, mask_self, grid, st);
@@ -413,8 +417,9 @@ extern "C" int b200vit_attention_varlen_ex(const void* qkv, void* out, const int
                                            int total_tiles, int H, int dh, float scale, int flags, void* stream) {
   B200_CHECK_ARG(qkv && out && cu_seqlens_dev && tile_prefix_dev, "attention_varlen: null pointer");
   B200_CHECK_ARG(num_seqs > 0 && total_tokens > 0 && total_tiles > 0 && H > 0, "attention_varlen: bad shape");
-  B200_CHECK_ARG(head_width_ok(dh), "attention_varlen: dim_head=%d not supported by this build (32, 64, 80 or 128)",
-                 dh);
+  B200_CHECK_ARG(head_width_ok(dh) || (dh == 160 && !(flags & B200VIT_ATTN_MASK_SELF)),
+                 "attention_varlen: dim_head=%d not supported by this build (32, 64, 80 or 128), nor 160 with "
+                 "B200VIT_ATTN_MASK_SELF", dh);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                  "attention_varlen: pointers must be 16-byte aligned");
   B200_CHECK_ARG(H <= 65535, "attention_varlen: H=%d exceeds the grid", H);
