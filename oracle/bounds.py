@@ -157,6 +157,16 @@ def stats_reference(out_bf16: Tensor, parts: int) -> Tuple[Tensor, Tensor]:
     return ref, bound
 
 
+def patch_stats_reference(a: Tensor) -> Tuple[Tensor, Tensor]:
+    """(ref, bound) [m, 2] of b200vit_patch_stats, the (sum, sum of squares) of each bf16 patch row a[m, pd] the TMA
+    patch embedding folds its LayerNorm with.  The squares of bf16 values are exact in fp32 and no fp32 sum of the
+    kernel is deeper than the row, so the bound is pd u sum|x| and pd u sum x^2."""
+    x = a.double()
+    pd = x.shape[1]
+    return (torch.stack([x.sum(1), (x * x).sum(1)], 1),
+            pd * U * torch.stack([x.abs().sum(1), (x * x).sum(1)], 1))
+
+
 def bf16_ulp(x: Tensor) -> Tensor:
     """The spacing of bf16 numbers at |x| (8-bit significand): 2^(floor(log2 |x|) - 7); 0 at x = 0."""
     _, ex = torch.frexp(x.abs())

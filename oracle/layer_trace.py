@@ -26,7 +26,11 @@ The encoders that run outside a single run_blocks call are traced through their 
 their own checks: CrossViT's two streams (`check_cross_vit_provenance`: each branch's layers, its final LayerNorm,
 both class-attention directions), CaiT's and XCiT's forward_fused after the patch embedding
 (`check_class_stage_provenance`: the patch encoder, the context, one CrossAttentionEngine.run against
-`cross_module_layers`, the head), and LeViT's whole forward_fused (`check_levit_provenance`)."""
+`cross_module_layers`, the head), and LeViT's whole forward_fused (`check_levit_provenance`).
+
+The ViT, SimpleViT-family, small-dataset ViT, DeepViT and NaViT forwards are walked from the pixels to the logits
+(`check_forward_provenance`): the patch embedding in either patch mode, the token assembly, the layers, the final
+LayerNorm, the pooling and the head, every operand read from the module's own attributes."""
 from __future__ import annotations
 
 import dataclasses
@@ -46,6 +50,7 @@ from oracle import bounds as Bd
 from oracle import grid_attention_bounds as GB
 from oracle import headmix_bounds as HB
 from oracle import row_bounds as RB
+from oracle import vit_oracle as O
 from oracle.lpi_bounds import lpi_reference
 
 Tensor = torch.Tensor
@@ -86,6 +91,15 @@ OUTPUTS = {
     "mean_pool": ("out",),
     "cast_f32_bf16": ("out",),
     "conv_im2col_nchw": ("out_bf16",),
+    "patch_embed_tma": ("stats", "out_f32"),
+    "patchify_ln": ("out_bf16",),
+    "patchify_spt_ln": ("out_bf16",),
+    "patchify_nd": ("out_bf16",),
+    "patchify_varlen_ln": ("out_bf16",),
+    "embed_tokens": ("x", "xb", "stats"),
+    "embed_tokens_grouped": ("x", "xb", "stats"),
+    "embed_varlen": ("x", "xb", "stats"),
+    "attn_pool": ("out",),
 }
 # the entry points of the attention records on token grids (engine.Windows, StridedKV, InteractiveWindows, ConvProj,
 # PatchGroups, WindowTokenBlock, RegionLocalBlock), of the SiLU feed-forward block and of ScalableViT's positional
@@ -96,6 +110,9 @@ GRID_ENTRY_POINTS = ("gemm_act", "conv_im2col_nhwc", "attention_window", "attent
 # the entry points of the class-token cross attention (engine.CrossAttentionEngine) and of LeViT's forward_fused
 CLASS_ENTRY_POINTS = ("attention_cls", "attention_cls_headmix", "attention_posbias", "gemm_hardswish", "mean_pool",
                       "conv_im2col_nchw")
+# the entry points of the patch embeddings, token assembly and NaViT's attention pooling (a whole forward_fused)
+FRONT_ENTRY_POINTS = ("patch_embed_tma", "patchify_ln", "patchify_spt_ln", "patchify_nd", "patchify_varlen_ln",
+                      "embed_tokens", "embed_tokens_grouped", "embed_varlen", "attn_pool")
 
 
 def schedule():
@@ -217,6 +234,45 @@ def rope_reference(qkv: Tensor, cs: Tensor, rows: int, H: int, dh: int) -> Tenso
     return out.view(T, -1)
 
 
+def tma_patches(img: Tensor) -> Tensor:
+    """The 16 x 16 patch rows [B n, C 256] of img [B, C, H, W] in the (c p1 p2) column order b200vit_patch_embed_tma
+    reads the image in (the reference's Rearrange writes (p1 p2 c), vit.py:100)."""
+    B, C, H, W = img.shape
+    return img.reshape(B, C, H // 16, 16, W // 16, 16).permute(0, 2, 4, 1, 3, 5).reshape(-1, C * 256)
+
+
+def spt_patches(img: Tensor, p: int) -> Tensor:
+    """The (p1 p2 c) patch rows of cat(img, its four one-pixel shifts) over 5 C channels (vit_for_small_dataset.py:
+    96-112), zero-filled shifts as F.pad makes them."""
+    from vit_pytorch_b200.vit_for_small_dataset import SPT_SHIFTS
+    xs = torch.cat([img] + [torch.nn.functional.pad(img, s) for s in SPT_SHIFTS], dim=1)
+    return O.patchify(xs, p, p).reshape(-1, 5 * img.shape[1] * p * p)
+
+
+def nd_patches(img: Tensor, patch) -> Tensor:
+    """The (p0 .. p_{r-1} c) patch rows of img [B, C, S_0 .. S_{r-1}] (vit_nd.py's Rearrange), grid row-major."""
+    B, C, *shape = img.shape
+    r = len(shape)
+    v = img.reshape(B, C, *[e for s, p in zip(shape, patch) for e in (s // p, p)])
+    perm = [0] + [2 + 2 * i for i in range(r)] + [3 + 2 * i for i in range(r)] + [1]
+    return v.permute(*perm).reshape(-1, C * math.prod(patch))
+
+
+def varlen_patches(images, p: int) -> Tensor:
+    """The (c p1 p2) patch rows of every image of a packed batch, in order (na_vit.py: _tokenise_row)."""
+    rows = []
+    for im in images:
+        C, h, w = im.shape
+        rows.append(im.reshape(C, h // p, p, w // p, p).permute(1, 3, 0, 2, 4).reshape(-1, C * p * p))
+    return torch.cat(rows)
+
+
+def _padded(rb: Tuple[Tensor, Tensor], width: int) -> Tuple[Tensor, Tensor]:
+    """(ref, bound) of rows written with zero K padding up to `width` columns: the padding exactly 0."""
+    pad = lambda t: torch.nn.functional.pad(t, (0, width - t.shape[1]))                 # noqa: E731
+    return pad(rb[0]), pad(rb[1])
+
+
 def _exact(v: Tensor) -> Tuple[Tensor, Tensor]:
     return v.double(), torch.zeros(v.shape, dtype=torch.float64, device=v.device)
 
@@ -309,8 +365,9 @@ def expected(name: str, a: dict, got: dict, on_output: Optional[Callable] = None
         return out
     if name == "mean_pool":
         B, N, D = a["B"], a["N"], a["D"]
-        put("out", RB.mean_pool_reference(a["x"].reshape(-1)[:B * N * D].view(B, N, D),
-                                          N if a["n_pool"] is None else a["n_pool"]))
+        flat = a["x"].reshape(-1)[:B * N * D]           # read at a row offset: the last rows past the view are not read
+        flat = torch.nn.functional.pad(flat, (0, B * N * D - flat.numel()), value=math.nan)
+        put("out", RB.mean_pool_reference(flat.view(B, N, D), N if a["n_pool"] is None else a["n_pool"]))
         return out
     if name == "cast_f32_bf16":
         put("out", _exact(a["x"].bfloat16()))
@@ -411,6 +468,47 @@ def expected(name: str, a: dict, got: dict, on_output: Optional[Callable] = None
         if a["y_bf16"] is not None:
             put("y_bf16", _exact(got["y"].bfloat16()))
             put("y_stats", _stats(got["y_bf16"], a["y_stats"]))
+        return out
+    if name == "patch_embed_tma":                     # the patch statistics, then the LN-folded GEMM reading them
+        rows = tma_patches(a["img"])
+        put("stats", Bd.patch_stats_reference(rows))
+        put("out_f32", Bd.gemm_reference(rows, a["w_perm"], bias=a["bias"], ln_sums=got["stats"], col_s=a["col_s"],
+                                         ln_eps=f32(a["eps"])))
+        return out
+    if name in ("patchify_ln", "patchify_spt_ln", "patchify_varlen_ln"):
+        if name == "patchify_ln":
+            rows = O.patchify(a["img"], a["ph"], a["pw"])
+            rows = rows.reshape(-1, rows.shape[-1])
+        elif name == "patchify_spt_ln":
+            rows = spt_patches(a["img"], a["p"])
+        else:
+            rows = varlen_patches(a["images"], a["p"])
+        rb = Bd.layernorm_reference(rows, a["gamma"], a.get("beta"), f32(a["eps"]))
+        put("out_bf16", _padded(rb, a["out_bf16"].shape[1]))
+        return out
+    if name == "patchify_nd":                         # a pure gather: exact
+        put("out_bf16", _padded(_exact(nd_patches(a["img"], list(a["patch"]))), a["out_bf16"].shape[1]))
+        return out
+    if name in ("embed_tokens", "embed_tokens_grouped", "embed_varlen"):
+        if name == "embed_varlen":
+            ix = a["index"]
+            dims = [tuple(d) for d in ix.dims.view(-1, 2).tolist()]
+            put("x", RB.embed_varlen_reference(a["y"], a["gamma"], a["pos_h"], a["pos_w"], ix.lengths, dims, a["p"],
+                                               f32(a["eps"])))
+        elif name == "embed_tokens":                  # cls and pos: rows of D values, whatever their view's shape
+            rows = lambda t: None if t is None else t.reshape(-1, a["y"].shape[1])              # noqa: E731
+            put("x", RB.embed_tokens_reference(a["y"], a["gamma"], a["beta"], rows(a["cls"]), rows(a["pos"]), a["B"],
+                                               a["n"], a["ncls"], tail=a["tail"], eps=f32(a["eps"])))
+        else:
+            put("x", RB.embed_tokens_reference(a["y"], a["gamma"], a["beta"], a["cls"], a["pos"], a["groups"], a["n"],
+                                               a["ncls"], eps=f32(a["eps"]), pos_period=a["pos_period"],
+                                               pos_stride=a["pos_stride"], cls_pos=a["cls_pos"]))
+        if a["xb"] is not None:                       # the first layer's bf16 copy and row statistics
+            put("xb", _exact(got["x"].bfloat16()))
+            put("stats", _stats(got["xb"], a["stats"]))
+        return out
+    if name == "attn_pool":
+        put("out", FB.navit_pool_reference(a["kv"], a["qn"], a["cu_seqlens"].diff().tolist(), a["H"], a["dh"]))
         return out
     raise NotImplementedError(f"no reference of _lib.{name}")
 
@@ -910,6 +1008,7 @@ class Walk:
     def __init__(self, case: str, launches: List[Launch], fold: bool, kw: dict) -> None:
         self.case, self.calls, self.fold, self.kw = case, launches, fold, kw
         self.pos, self.where, self.cur = 0, "", None
+        self.ratios: Dict[str, float] = {}            # operand -> worst |got - ref| / bound of its `within` checks
         self.have_stats = fold and bool(kw.get("primed"))
         # the statistics the next folded GEMM reads are the entry ones, one part per row (the prime or a rowstats_cast),
         # not a residual GEMM's
@@ -954,6 +1053,7 @@ class Walk:
         ref, bound = ref.to(got.device), bound.to(got.device)
         d = (got.double().reshape(ref.shape) - ref).abs()
         bad = ~(d <= bound)
+        self.ratios[op] = max(self.ratios.get(op, 0.0), Bd.excess(got.reshape(ref.shape), ref, bound))
         if bool(bad.any()):
             i = tuple(bad.nonzero()[0].tolist())
             self.fail(op, f"{int(bad.sum())} of {bad.numel()} elements outside the bound, first at {i}: got "
@@ -1605,7 +1705,8 @@ def trace_call(call: Callable[[], object], ln_mode: str, impl=real_impl, setup: 
     LeViT.forward_fused -- in `ln_mode` with every launch traced; setup() first, inside the tracing (it fills the
     workspaces the call will use with NaN)."""
     S = schedule()
-    with S.recording(None, lambda: [], ln_mode, "python", extra_entry_points=GRID_ENTRY_POINTS + CLASS_ENTRY_POINTS,
+    with S.recording(None, lambda: [], ln_mode, "python",
+                     extra_entry_points=GRID_ENTRY_POINTS + CLASS_ENTRY_POINTS + FRONT_ENTRY_POINTS,
                      recorder=tracer(impl)) as rec:
         if setup is not None:
             setup()
@@ -2007,3 +2108,503 @@ def check_levit_provenance(mod: nn.Module, img: Tensor, launches: List[Launch], 
                     torch.cat([h_.bias.detach().float() for h_ in heads]), what="w ([mlp_head; distill_head])")
     return _end(w)
 
+
+
+# ------------------------------------------------------------------------------------------------------ whole forwards
+def _d(t: Tensor) -> Tensor:
+    return t.detach().double()
+
+
+def _f(t: Optional[Tensor]) -> Optional[Tensor]:
+    return None if t is None else t.detach().float()
+
+
+def _layernorm_launch(w: Walk, x: Tensor, ln: Ln, *, f32_out: bool = False, row_index: Optional[Tensor] = None
+                      ) -> Tensor:
+    """One b200vit_layernorm of the rows x (row_index: of those rows) with the LayerNorm ln: its bf16 output, or with
+    f32_out its fp32 one (and no bf16 output)."""
+    c = w.take("layernorm")
+    a = c.pre
+    w.same("x", a["x"], x)
+    w.same("gamma", a["gamma"], _f(ln.gamma))
+    w.same("beta", a["beta"], _f(ln.beta))
+    w.value("eps", a["eps"], float(ln.eps))
+    w.same("row_index", a["row_index"], None if row_index is None else row_index.to(x.device))
+    if f32_out:
+        w.same("out_bf16", a["out_bf16"], None)
+        if a["out_f32"] is None:
+            w.fail("out_f32", "the LayerNorm's fp32 output is not written")
+        return c.post["out_f32"]
+    w.same("out_f32", a["out_f32"], None)
+    return c.post["out_bf16"]
+
+
+def _head_gemm(w: Walk, A: Tensor, lin: nn.Linear, what: str) -> Tensor:
+    """logits = A W^T + b of the classifier Linear `lin` into a bf16 output (engine.HeadEngine)."""
+    return w.prepared_gemm(A, lin.weight.detach().bfloat16(), _f(lin.bias), what=f"w ({what})")
+
+
+def _mean_pool(w: Walk, x: Tensor, B: int, N: int, n_pool: Optional[int], D: Optional[int] = None) -> Tensor:
+    """mean_pool of the rows x (a flat view: read from a row offset, D its width)."""
+    c = w.take("mean_pool")
+    a = c.pre
+    w.same("x", a["x"], x)
+    w.value("B", a["B"], B)
+    w.value("N", a["N"], N)
+    w.value("D", a["D"], x.shape[1] if D is None else D)
+    w.value("n_pool", a["n_pool"], n_pool)
+    return c.post["out"]
+
+
+def _cast(w: Walk, x: Tensor) -> Tensor:
+    c = w.take("cast_f32_bf16")
+    w.same("x", c.pre["x"].reshape(x.shape), x)
+    return c.post["out"]
+
+
+def walk_patch_projection(w: Walk, model: nn.Module, img: Tensor, box: Optional[Tuple[int, int]] = None) -> Tensor:
+    """y = LayerNorm(patch) W^T + b of every patch of img (vit.py:99-102; the SPT's shifted patches,
+    vit_for_small_dataset.py:96-112): the 16 x 16 TMA launch with LayerNorm(patch) folded into the projection -- gamma W
+    with its columns permuted from the Rearrange's (p1 p2 c) to the image's (c p1 p2), their column sums, W beta + b
+    -- or the patchify kernel and a GEMM at K padded to a multiple of 64.  `box`: the patch of img when it is not the
+    module's patch_size (the 1-D and 3-D front ends' [B, C, H', W'] views).  Returns y fp32 [B n, D]."""
+    pe = model.to_patch_embedding
+    spt = getattr(pe, "to_patch_tokens", None)
+    ln1, lin = (spt[1], spt[2]) if spt is not None else (pe[1], pe[2])
+    ph, pw = box if box is not None else model.patch_size
+    src = img.contiguous()
+    D, K = lin.weight.shape
+    w.where = "patch embedding"
+    if w.peek() == "patch_embed_tma":
+        c = w.take("patch_embed_tma")
+        a = c.pre
+        if spt is not None or (ph, pw) != (16, 16):
+            w.fail("-", f"the 16 x 16 TMA patch embedding runs for {ph} x {pw}{' shifted' if spt else ''} patches")
+        w.same("img", a["img"], src)
+        C = K // 256
+        wg = (_d(lin.weight) * _d(ln1.weight)[None]).float().bfloat16()
+        w.same("w_perm (gamma W, columns (c p1 p2))", a["w_perm"], wg.view(D, 256, C).permute(0, 2, 1).reshape(D, K))
+        wd = a["w_perm"].double()
+        w.within("col_s (column sums of the bf16 w_perm)", a["col_s"], wd.sum(1), K * U * wd.abs().sum(1))
+        t = _d(lin.weight) @ _d(ln1.bias) + _d(lin.bias)
+        tb = _d(lin.weight).abs() @ _d(ln1.bias).abs() + _d(lin.bias).abs()
+        w.within("bias (W beta + b)", a["bias"], t, (K + 1) * U * tb)
+        w.value("eps", a["eps"], float(ln1.eps))
+        return c.post["out_f32"]
+    if spt is not None:
+        c = w.take("patchify_spt_ln")
+        w.value("p", c.pre["p"], ph)
+    else:
+        c = w.take("patchify_ln")
+        w.value("ph", c.pre["ph"], ph)
+        w.value("pw", c.pre["pw"], pw)
+    a = c.pre
+    w.same("img", a["img"], src)
+    w.same("gamma", a["gamma"], _f(ln1.weight))
+    w.same("beta", a["beta"], _f(ln1.bias))
+    w.value("eps", a["eps"], float(ln1.eps))
+    a0 = c.post["out_bf16"]
+    kp = a0.shape[1]
+    c = w.take("gemm")
+    a = c.pre
+    w.same("a", a["a"], a0)
+    w.same("w (Linear, K padded)", a["w"], torch.nn.functional.pad(lin.weight.detach(), (0, kp - K)).bfloat16())
+    w.same("bias", a["bias"], _f(lin.bias))
+    for op in ("resid", "ln_sums", "out_bf16", "stats_out"):
+        w.same(op, a[op], None)
+    w.value("gelu", a["gelu"], False)
+    if a["out_f32"] is None:
+        w.fail("out_f32", "the patch projection writes no fp32 output")
+    return c.post["out_f32"]
+
+
+def walk_tokens(w: Walk, model: nn.Module, y: Tensor, B: int, grid: Tuple[int, int], pos: Optional[Tensor] = None,
+                ln2: Optional[nn.Module] = None) -> Tuple[Tensor, int]:
+    """embed_tokens: [cls; LayerNorm(dim)(y) + pos; register tokens] per image (vit.py:103,122-124,
+    simple_vit_with_register_tokens.py:116-126; no LayerNorm(dim) after an SPT), with the first layer's bf16 copy and
+    row statistics in fold mode.  `pos`: the positional table when the module builds it in its forward (the 1-D and
+    3-D sin-cos tables); `ln2`: LayerNorm(dim) when it is not to_patch_embedding[3].  Returns (x fp32 [B N, D], N)."""
+    pe = model.to_patch_embedding
+    if ln2 is None:
+        ln2 = None if hasattr(pe, "to_patch_tokens") else pe[3]
+    ln2 = None if ln2 is None else _ln(ln2)
+    D = y.shape[1]
+    cls = getattr(model, "cls_token", None) if getattr(model, "cls_in_sequence", True) else None
+    cls = None if cls is None or cls.numel() == 0 else cls.detach().float().reshape(-1, D)
+    reg = getattr(model, "register_tokens", None)
+    reg = None if reg is None or reg.numel() == 0 else reg.detach().float()
+    if pos is None:
+        pos = getattr(model, "pos_embedding", None)
+    if pos is None and hasattr(model, "fused_pos_table"):    # the sin-cos table of the input's own patch grid
+        pos = O.posemb_sincos_2d(*grid, D)                  # (simple_flash_attn_vit.py:110-114)
+    ncls, ntail = 0 if cls is None else cls.shape[0], 0 if reg is None else reg.shape[0]
+    w.where = "token assembly"
+    c = w.take("embed_tokens")
+    a = c.pre
+    w.same("y", a["y"], y)
+    w.same("gamma (LayerNorm(dim))", a["gamma"], None if ln2 is None else _f(ln2.gamma))
+    if ln2 is not None:
+        w.same("beta (LayerNorm(dim))", a["beta"], _f(ln2.beta))
+        w.value("eps (LayerNorm(dim))", a["eps"], float(ln2.eps))
+    rows = lambda t: None if t is None else t.reshape(-1, D)                            # noqa: E731
+    w.same("cls", rows(a["cls"]), cls)
+    w.same("pos", rows(a["pos"]), None if pos is None else pos.detach().float().reshape(-1, D))
+    w.same("tail (register tokens)", a["tail"], reg)
+    w.value("B", a["B"], B)
+    n = math.prod(grid)
+    w.value("n", a["n"], n)
+    w.value("ncls", a["ncls"], ncls)
+    x = c.post["x"]
+    _entry_copy(w, c, x)
+    return x, n + ncls + ntail
+
+
+def _entry_copy(w: Walk, c: Launch, x: Tensor) -> None:
+    """The bf16 copy of x and its row statistics the first folded GEMM reads, written by the embedding in fold mode."""
+    a = c.pre
+    if not w.fold:
+        w.same("xb", a["xb"], None)
+        w.same("stats", a["stats"], None)
+        return
+    if a["xb"] is None or a["stats"] is None:
+        w.fail("xb", "the first layer's bf16 copy and row statistics are not written")
+    w.same("xb", c.post["xb"], x.bfloat16())
+    w.stats("stats", c.post["stats"], c.post["xb"])
+
+
+def walk_head(w: Walk, model: nn.Module, S: Tensor, B: int, N: int, n: int) -> None:
+    """After the last layer on the fp32 stream S: the final LayerNorm, the pooling and the head, by family --
+    ViT (vit.py:129-138): LayerNorm of the cls rows (row_index) or of every row then the mean; the SimpleViT family
+    (simple_vit.py:116-120 and its variants): LayerNorm, the mean over the patch tokens (not the register tokens), its
+    bf16 cast, the head GEMM or the head LayerNorm; a LayerNorm + Linear mlp_head without a final LayerNorm
+    (vit_for_small_dataset.py:173-178, deepvit.py:162-167): the cls rows or the mean, then mlp_head[0] and
+    mlp_head[1]."""
+    from vit_pytorch_b200 import deepvit, simple_vit_with_qk_norm, simple_vit_with_register_tokens, vit
+    from vit_pytorch_b200 import vit_for_small_dataset, vit_nd, vit_nd_rotary
+    enc = model.transformer
+    norm = getattr(enc, "norm", None)
+    rows = torch.arange(0, B * N, N, dtype=torch.int32)
+    w.where = "head"
+    if isinstance(model, (vit_for_small_dataset.ViT, deepvit.DeepViT)):
+        ln, lin = _ln(model.mlp_head[0]), model.mlp_head[1]
+        if model.pool == "mean":
+            pooled = _layernorm_launch(w, _mean_pool(w, S, B, N, None), ln)
+        else:
+            pooled = _layernorm_launch(w, S, ln, row_index=rows)
+        _head_gemm(w, pooled, lin, "mlp_head[1]")
+        return
+    if isinstance(model, (vit_nd.ViTND, vit_nd_rotary.ViTND)):
+        # vit_nd.py:213-216: the mean over the patch tokens x[:, 1:] or the cls row; vit_nd_rotary.py:277: the mean
+        if isinstance(model, vit_nd_rotary.ViTND) or model.pool == "mean":
+            skip = 0 if isinstance(model, vit_nd_rotary.ViTND) else N - n
+            xf = _layernorm_launch(w, S, _ln(norm), f32_out=True)
+            flat = xf.reshape(-1)[skip * S.shape[1]:] if skip else xf
+            pooled = _cast(w, _mean_pool(w, flat, B, N, None if skip == 0 else n, D=S.shape[1]))
+        else:
+            pooled = _layernorm_launch(w, S, _ln(norm), row_index=rows)
+        _head_gemm(w, pooled, model.mlp_head, "mlp_head")
+        return
+    if isinstance(model, vit.ViT):
+        if model.pool == "mean":
+            pooled = _cast(w, _mean_pool(w, _layernorm_launch(w, S, _ln(norm), f32_out=True), B, N, None))
+        else:
+            pooled = _layernorm_launch(w, S, _ln(norm), row_index=rows)
+        _head_gemm(w, pooled, model.mlp_head, "mlp_head")
+        return
+    xf = S if norm is None else _layernorm_launch(w, S, _ln(norm), f32_out=True)
+    registers = isinstance(model, simple_vit_with_register_tokens.SimpleViT)
+    pm = _mean_pool(w, xf, B, N, n if registers else None)
+    pooled = _cast(w, pm)
+    if isinstance(model, simple_vit_with_qk_norm.SimpleViT):       # linear_head is a LayerNorm (sic, reference :128)
+        _layernorm_launch(w, pm, _ln(model.linear_head))
+        return
+    if isinstance(model.linear_head, nn.Sequential):     # simple_flash_attn_vit.py:116-117: LayerNorm, Linear
+        _head_gemm(w, _layernorm_launch(w, pm, _ln(model.linear_head[0])), model.linear_head[1], "linear_head[1]")
+        return
+    _head_gemm(w, pooled, model.linear_head, "linear_head")
+
+
+def _navit_query_reference(model: nn.Module) -> Tuple[Tensor, Tensor]:
+    """(ref, bound) [H dh] of NaViT's pooling query after its LayerNorm, to_q and per-head RMSNorm (na_vit.py:105-112,
+    the same for every image), which the host computes in fp32 once per weight version.  The fp32 LayerNorm of D values
+    is within layernorm_e32 at depth D, to_q adds D u |W| |ln| (any order of its sums), and the normalised head
+    qh / ||qh|| moves by e / ||qh|| + |qh| ||e|| / ||qh||^2 under an error e of qh (first order, 1.01 for the rest);
+    then (dh + 6) u |ref| for the norm, the quotient and the products with scale and gamma."""
+    pool = model.attn_pool
+    H = pool.heads
+    q = _d(model.attn_pool_queries)[None]
+    ln, e_ln = Bd.layernorm_e32(q, _d(pool.norm.gamma), None, 1e-5, q.shape[1])
+    W = _d(pool.to_q.weight)
+    qh = (W @ ln[0]).view(H, -1)
+    e = (W.abs() @ e_ln[0] + W.shape[1] * U * (W.abs() @ ln[0].abs())).view(H, -1)
+    nrm = torch.linalg.vector_norm(qh, dim=-1, keepdim=True)
+    g = _d(pool.q_norm.gamma).view(H, -1) * pool.q_norm.scale
+    ref = qh / nrm * g
+    dh = qh.shape[1]
+    bound = 1.01 * g.abs() * (e / nrm + qh.abs() * torch.linalg.vector_norm(e, dim=-1, keepdim=True) / nrm ** 2)
+    return ref.reshape(-1), (bound + (dh + 6) * U * ref.abs()).reshape(-1)
+
+
+def check_navit_provenance(model: nn.Module, images: List[Tensor], launches: List[Launch], ln_mode: str,
+                           case: str = "", ratios: Optional[dict] = None) -> int:
+    """Walk the trace of na_vit.NaViT.forward_fused(images) (na_vit.py:254-308) through the reference NaViT
+    (reference na_vit.py:270-328): the packed (c p1 p2) patch rows of every image and their bias-free LayerNorm, the
+    projection, LayerNorm(dim) + pos_embed_height[row] + pos_embed_width[col] of each token's place in its own image's
+    grid, the encoder layers over the packed sequences, the final LayerNorm, the attention pooling -- to_kv of the
+    normalised tokens with k_norm on the k half, one query per image, + the queries -- and the bias-free head LayerNorm
+    and Linear.  The number of launches checked."""
+    fold = ln_mode == "fold"
+    p = model.patch_size
+    pe = model.to_patch_embedding
+    lengths = [(im.shape[-2] // p) * (im.shape[-1] // p) for im in images]
+    cu = torch.tensor([0] + lengths, dtype=torch.int32).cumsum(0).to(torch.int32)
+    dims = [(im.shape[-2], im.shape[-1]) for im in images]
+    T, S_ = sum(lengths), len(images)
+    w = Walk(case, launches, fold, dict(primed=fold, varlen=None))
+    w.ratios = w.ratios if ratios is None else ratios
+    w.where = "patch embedding"
+    c = w.take("patchify_varlen_ln")
+    a = c.pre
+    if len(a["images"]) != S_:
+        w.fail("images", f"{len(a['images'])} images, want {S_}")
+    for i, (got, im) in enumerate(zip(a["images"], images)):
+        w.same(f"images[{i}]", got, im.contiguous())
+    w.same("gamma", a["gamma"], _f(_ln(pe[0]).gamma))
+    w.same("cu_seqlens", a["cu_seqlens"], cu.to(a["cu_seqlens"].device))
+    w.value("p", a["p"], p)
+    w.value("eps", a["eps"], float(_ln(pe[0]).eps))
+    a0 = c.post["out_bf16"]
+    lin = pe[1]
+    c = w.take("gemm")
+    a = c.pre
+    w.same("a", a["a"], a0)
+    w.same("w", a["w"], lin.weight.detach().bfloat16())
+    w.same("bias", a["bias"], _f(lin.bias))
+    for op in ("resid", "ln_sums", "out_bf16", "stats_out"):
+        w.same(op, a[op], None)
+    if a["out_f32"] is None:
+        w.fail("out_f32", "the patch projection writes no fp32 output")
+    y = c.post["out_f32"]
+    w.where = "token assembly"
+    c = w.take("embed_varlen")
+    a = c.pre
+    ix = a["index"]
+    w.same("y", a["y"], y)
+    w.same("gamma (LayerNorm(dim))", a["gamma"], _f(_ln(pe[2]).gamma))
+    w.same("pos_h (pos_embed_height)", a["pos_h"], _f(model.pos_embed_height))
+    w.same("pos_w (pos_embed_width)", a["pos_w"], _f(model.pos_embed_width))
+    w.same("index.cu", ix.cu, cu.to(ix.cu.device))
+    w.same("index.dims", ix.dims, torch.tensor(dims, dtype=torch.int32).reshape(-1).to(ix.dims.device))
+    w.value("p", a["p"], p)
+    w.value("eps", a["eps"], float(_ln(pe[2]).eps))
+    x = c.post["x"]
+    _entry_copy(w, c, x)
+    enc = model.transformer
+    check_identity(enc, case)
+    w.kw["varlen"] = ix                        # its cu_seqlens checked above
+    S = walk_blocks(w, enc, x)
+    w.where = "final LayerNorm"
+    xn = _layernorm_launch(w, S, _ln(enc.norm))
+    pool = model.attn_pool
+    H = pool.heads
+    I = pool.to_q.weight.shape[0]
+    dh = I // H
+    w.where = "attention pooling keys and values"        # na_vit.py:111-112: to_kv of the context, k_norm on k
+    c = w.take("gemm_headnorm")
+    a = c.pre
+    w.same("a", a["a"], xn)
+    w.same("w (to_kv)", a["w"], pool.to_kv.weight.detach().bfloat16())
+    for op in ("bias", "ln_sums"):
+        w.same(op, a[op], None)
+    w.same("head_gamma (k_norm)", a["head_gamma"], _f(pool.k_norm.gamma).reshape(-1))
+    w.value("norm_heads", a["norm_heads"], H)
+    w.value("dh", a["dh"], dh)
+    w.value("head_layernorm_eps", a["head_layernorm_eps"], None)
+    kv = c.post["out_bf16"]
+    w.where = "attention pooling"
+    c = w.take("attn_pool")
+    a = c.pre
+    w.same("kv", a["kv"], kv)
+    w.within("qn (the normalised query)", a["qn"], *_navit_query_reference(model))
+    w.same("cu_seqlens", a["cu_seqlens"], cu.to(a["cu_seqlens"].device))
+    w.value("H", a["H"], H)
+    w.value("dh", a["dh"], dh)
+    pooled = c.post["out"]
+    w.where = "attention pooling out"                    # na_vit.py:384: attn_pool(...) + queries
+    queries = _f(model.attn_pool_queries)[None].expand(S_, -1).to(S.device)
+    out = pool.to_out[0]
+    c = w.take("gemm")
+    a = c.pre
+    w.same("a", a["a"], pooled)
+    w.same("w (to_out)", a["w"], out.weight.detach().bfloat16())
+    w.same("bias", a["bias"], _f(out.bias))
+    w.same("resid (the queries)", a["resid"], queries)
+    for op in ("ln_sums", "out_bf16", "stats_out"):
+        w.same(op, a[op], None)
+    if a["out_f32"] is None:
+        w.fail("out_f32", "the pooled rows are not written in fp32")
+    z = c.post["out_f32"]
+    w.where = "head"
+    zl = _layernorm_launch(w, z, _ln(model.mlp_head[0]))
+    _head_gemm(w, zl, model.mlp_head[1], "mlp_head[1]")
+    return _end(w)
+
+
+def walk_nd_projection(w: Walk, model: nn.Module, img: Tensor) -> Tensor:
+    """y = (p0 .. p_{r-1} c) patches of img W^T + b (vit_nd.py:160-167, vit_nd_rotary.py:197-202): the N-d gather and
+    a GEMM at K padded to a multiple of 64, no LayerNorm of the patches.  Returns y fp32 [B n, D]."""
+    pe = model.to_patch_embedding
+    lin = pe[1]
+    D, K = lin.weight.shape
+    w.where = "patch embedding"
+    c = w.take("patchify_nd")
+    a = c.pre
+    w.same("img", a["img"], img.contiguous())
+    w.value("patch", tuple(a["patch"]), tuple(pe[0].patch_size))
+    a0 = c.post["out_bf16"]
+    kp = a0.shape[1]
+    c = w.take("gemm")
+    a = c.pre
+    w.same("a", a["a"], a0)
+    w.same("w (Linear, K padded)", a["w"], torch.nn.functional.pad(lin.weight.detach(), (0, kp - K)).bfloat16())
+    w.same("bias", a["bias"], _f(lin.bias))
+    for op in ("resid", "ln_sums", "out_bf16", "stats_out"):
+        w.same(op, a[op], None)
+    if a["out_f32"] is None:
+        w.fail("out_f32", "the patch projection writes no fp32 output")
+    return c.post["out_f32"]
+
+
+def _video_view(model: nn.Module, video: Tensor) -> Tuple[Tensor, Tuple[int, int], Tuple[int, int, int]]:
+    """(the [b, c, (f pf h p1), w p2] view whose (pf p1) x p2 boxes hold the (pf p1 p2 c) patches of the reference's
+    Rearrange (simple_vit_3d.py:97, vivit.py:196), the box, the (f, h, w) grid)."""
+    pf = model.frame_patch_size if hasattr(model, "frame_patch_size") else model._pf
+    p1, p2 = model.patch_size
+    b, c, ft, ht, wt = video.shape
+    f, h = ft // pf, ht // p1
+    img = video.reshape(b, c, f, pf, h, p1, wt).permute(0, 1, 2, 4, 3, 5, 6).reshape(b, c, ft * ht, wt)
+    return img, (pf * p1, p2), (f, h, wt // p2)
+
+
+def check_vivit_provenance(model: nn.Module, video: Tensor, launches: List[Launch], ln_mode: str, case: str = "",
+                           ratios: Optional[dict] = None) -> int:
+    """Walk the trace of vivit.ViViT.forward_fused(video) (no mask) through the reference ViViT (vivit.py:214-262):
+    the (pf p1 p2 c) tubelet embedding, the token assembly of every frame -- the spatial cls token without a position,
+    the frame's block of pos_embedding (embed_tokens_grouped) -- then, factorized encoder: the spatial layers over
+    every frame, the frame's cls row or mean, the temporal cls token and the temporal layers over the frames, the
+    pooling and the head; factorized self-attention: the layers with their axial attention over the frames, then the
+    pooling and the head."""
+    from vit_pytorch_b200 import vivit
+    fold = ln_mode == "fold"
+    img, box, (f, h, wg) = _video_view(model, video)
+    b, n = video.shape[0], h * wg
+    w = Walk(case, launches, fold, dict(primed=fold))
+    w.ratios = w.ratios if ratios is None else ratios
+    y = walk_patch_projection(w, model, img, box)
+    D = y.shape[1]
+    cls = not model.global_average_pool
+    ncls = int(cls)
+    N = n + ncls
+    ln2 = _ln(model.to_patch_embedding[3])
+    w.where = "token assembly"
+    c = w.take("embed_tokens_grouped")
+    a = c.pre
+    w.same("y", a["y"], y)
+    w.same("gamma (LayerNorm(dim))", a["gamma"], _f(ln2.gamma))
+    w.same("beta (LayerNorm(dim))", a["beta"], _f(ln2.beta))
+    w.value("eps (LayerNorm(dim))", a["eps"], float(ln2.eps))
+    w.same("cls (spatial_cls_token)", None if a["cls"] is None else a["cls"].reshape(-1, D),
+           _f(model.spatial_cls_token.reshape(-1, D)) if cls else None)
+    w.same("pos (pos_embedding)", a["pos"].reshape(-1, D), _f(model.pos_embedding.reshape(-1, D)))
+    for op, v in (("groups", b * f), ("n", n), ("ncls", ncls), ("pos_period", f),
+                  ("pos_stride", model.pos_embedding.shape[2]), ("cls_pos", False)):
+        w.value(op, a[op], v)
+    x = c.post["x"]
+    _entry_copy(w, c, x)
+    rows = lambda B_, N_: torch.arange(0, B_ * N_, N_, dtype=torch.int32)               # noqa: E731
+    if model.variant == "factorized_encoder":
+        sp, tr = model.spatial_transformer, model.temporal_transformer
+        check_identity(sp, case)
+        w.kw.update(B=b * f, N=N)
+        S = walk_blocks(w, sp, x)
+        w.where = "spatial pooling"                        # vivit.py:245-247: x[:, 0] or the mean, per frame
+        if cls:
+            xs = _layernorm_launch(w, S, _ln(sp.norm), f32_out=True, row_index=rows(b * f, N))
+        else:
+            xs = _mean_pool(w, _layernorm_launch(w, S, _ln(sp.norm), f32_out=True), b * f, N, None)
+        if cls:                                            # vivit.py:251-254: the temporal cls token, then the frames
+            xt = torch.cat((_f(model.temporal_cls_token).reshape(1, 1, D).expand(b, 1, D).to(xs.device),
+                            xs.view(b, f, D)), 1).reshape(b * (f + 1), D)
+        else:
+            xt = xs
+        Lt = f + ncls
+        check_identity(tr, case)
+        w.kw, w.have_stats, w.entry_stats = dict(B=b, N=Lt), False, False
+        S = walk_blocks(w, tr, xt)
+        w.where = "head"
+        if cls:
+            pooled = _layernorm_launch(w, S, _ln(tr.norm), row_index=rows(b, Lt))
+        else:
+            pooled = _cast(w, _mean_pool(w, _layernorm_launch(w, S, _ln(tr.norm), f32_out=True), b, Lt, None))
+    else:
+        tr = model.factorized_transformer
+        check_identity(tr, case)
+        w.kw.update(B=b * f, N=N, axial=(N, f, None, bool(vivit._flash_mode(tr))))
+        S = walk_blocks(w, tr, x)
+        w.where = "head"                                   # vivit.py:258-260: the first frame's cls row, or the mean
+        if cls:
+            pooled = _layernorm_launch(w, S, _ln(tr.norm), row_index=rows(b, f * N))
+        else:
+            pooled = _cast(w, _mean_pool(w, _layernorm_launch(w, S, _ln(tr.norm), f32_out=True), b, f * N, None))
+    _head_gemm(w, pooled, model.mlp_head, "mlp_head")
+    return _end(w)
+
+
+def check_forward_provenance(model: nn.Module, inputs, launches: List[Launch], ln_mode: str, case: str = "",
+                             ratios: Optional[dict] = None) -> int:
+    """Walk the trace of model.forward_fused(inputs) from the pixels to the logits through the reference module's
+    forward: the patch embedding (walk_patch_projection; the N-d gather, walk_nd_projection), the token assembly
+    (walk_tokens), the encoder layers (walk_blocks, with the embedding's bf16 copy and row statistics in fold mode), the
+    final LayerNorm, pooling and head (walk_head); NaViT by check_navit_provenance, ViViT by check_vivit_provenance.
+    Every operand comes from the module's own attributes (to_patch_embedding, cls_token, pos_embedding,
+    register_tokens, the head) or the tables its forward builds from the input's grid, never from the engine's
+    prepared tensors.  Returns the number of launches checked; raises ProvenanceError naming the launch and the
+    operand.  ratios: filled with the worst |got - ref| / bound of each operand checked within a bound (the host's
+    fp32 weight preparation, the row statistics)."""
+    from vit_pytorch_b200 import na_vit, simple_vit_1d, simple_vit_3d, vit_nd, vit_nd_rotary, vivit
+    if isinstance(model, na_vit.NaViT):
+        return check_navit_provenance(model, inputs, launches, ln_mode, case, ratios)
+    if isinstance(model, vivit.ViViT):
+        return check_vivit_provenance(model, inputs, launches, ln_mode, case, ratios)
+    fold = ln_mode == "fold"
+    w = Walk(case, launches, fold, dict(primed=fold))
+    w.ratios = w.ratios if ratios is None else ratios
+    B, rope = inputs.shape[0], None
+    if isinstance(model, (vit_nd.ViTND, vit_nd_rotary.ViTND)):
+        grid = tuple(s // p for s, p in zip(inputs.shape[2:], model.to_patch_embedding[0].patch_size))
+        y = walk_nd_projection(w, model, inputs)
+        x, N = walk_tokens(w, model, y, B, grid, ln2=model.to_patch_embedding[2])
+        if isinstance(model, vit_nd_rotary.ViTND):        # vit_nd_rotary.py:143-147: the grid's rotary table
+            cs = model.grid_table(grid, inputs.device)
+            rope = (cs, cs.shape[0])
+    else:
+        if isinstance(model, simple_vit_1d.SimpleViT):    # simple_vit_1d.py:84-90: 'b c (n p) -> b n (p c)'
+            b, ch, L = inputs.shape
+            p = model.fused_patch_box[1]
+            img, box, grid = inputs.contiguous().view(b, ch, 1, L), (1, p), (1, L // p)
+            # posemb_sincos_1d / _3d build the table on the input's device (simple_vit_1d.py:21-25)
+            pos = simple_vit_1d.sincos_table_1d(L // p, model.linear_head.in_features, device=inputs.device)
+        elif isinstance(model, simple_vit_3d.SimpleViT):
+            img, box, grid = _video_view(model, inputs)
+            pos = simple_vit_3d.sincos_table_3d(*grid, model.linear_head.in_features, device=inputs.device)
+        else:
+            img, box = inputs, model.patch_size
+            grid, pos = (img.shape[2] // box[0], img.shape[3] // box[1]), None
+        y = walk_patch_projection(w, model, img, box)
+        x, N = walk_tokens(w, model, y, B, grid, pos=None if pos is None else pos.to(y.device))
+    enc = model.transformer
+    check_identity(enc, case)
+    w.kw.update(B=B, N=N, rope=rope)
+    S = walk_blocks(w, enc, x)
+    walk_head(w, model, S, B, N, math.prod(grid))
+    return _end(w)

@@ -2,7 +2,7 @@
 every library launch traced (oracle/layer_trace.tracer, the recording of make_engine_schedule) and emulated -- each
 output gets the fp64 reference of its kernel on the operands the launch actually received, rounded to the output's
 dtype (oracle/layer_trace.emulate_impl, and below for the T2T entry points: the unfold as F.unfold, the wide attention
-from oracle/wide_attention_bounds.py, the token assembly as cat(cls, y) + pos).
+from oracle/wide_attention_bounds.py).
 
 Then every launch of every soft split is attributed to its reference layer and its operands checked bit for bit
 (`check_soft_splits`): the unfold reads the image or the previous soft split's final LayerNorm output on the map
@@ -30,7 +30,7 @@ sys.path.insert(0, GOLDEN_DIR)
 import make_engine_schedule as S  # noqa: E402
 from t2t_spec import FAMILY, T2T_CASES  # noqa: E402
 
-T2T_ENTRY_POINTS = ("t2t_unfold_image", "t2t_unfold_tokens", "attention_wide", "embed_tokens")
+T2T_ENTRY_POINTS = ("t2t_unfold_image", "t2t_unfold_tokens", "attention_wide")
 
 
 def _unfold_ref(src: torch.Tensor, k: int, s: int, p: int) -> torch.Tensor:
@@ -44,7 +44,7 @@ def _write(dst: torch.Tensor, val: torch.Tensor) -> None:
 
 
 def t2t_impl(name, real):
-    """The T2T entry points emulated, every other one by oracle/layer_trace.emulate_impl."""
+    """The T2T entry points emulated, every other one (token assembly included) by oracle/layer_trace.emulate_impl."""
     if name == "t2t_unfold_image":
         def run(img, out, k, s, p):
             _write(out, _unfold_ref(img, k, s, p))
@@ -63,29 +63,20 @@ def t2t_impl(name, real):
             if x is not None:
                 x[:, :n_resid] += o[:, :n_resid].float()
         return run
-    if name == "embed_tokens":
-        def run(y, gamma, beta, cls, pos, x, B, n, ncls, eps=1e-5, xb=None, stats=None, tail=None):
-            assert gamma is None and tail is None and ncls == 1
-            D = y.shape[1]
-            t = torch.cat([cls.expand(B, 1, D), y.view(B, n, D)], 1) + pos[:n + 1]
-            x.copy_(t.reshape(B * (n + 1), D))
-            if xb is not None:
-                LT.prime_exact(x, xb, stats)
-        return run
     return LT.emulate_impl(name, real)
 
 
 # what the T2T entry points write, for the tracer's after-call clones
-T2T_OUTPUTS = {"t2t_unfold_image": ("out",), "t2t_unfold_tokens": ("out",), "attention_wide": ("out", "x"),
-               "embed_tokens": ("x", "xb", "stats")}
+T2T_OUTPUTS = {"t2t_unfold_image": ("out",), "t2t_unfold_tokens": ("out",), "attention_wide": ("out", "x")}
 
 
-def trace(model: T2TViT, img: torch.Tensor, ln_mode: str, monkeypatch):
+def trace(model: T2TViT, img: torch.Tensor, ln_mode: str, monkeypatch, impl=t2t_impl):
+    """(launches, logits) of model.forward_fused(img), every launch run by impl (LT.real_impl: the real kernels)."""
     outs = []
     for k, v in T2T_OUTPUTS.items():
         monkeypatch.setitem(LT.OUTPUTS, k, v)
     with S.recording(None, lambda: [], ln_mode, "python", LT.GRID_ENTRY_POINTS + LT.CLASS_ENTRY_POINTS +
-                     T2T_ENTRY_POINTS, recorder=LT.tracer(t2t_impl)) as rec:
+                     LT.FRONT_ENTRY_POINTS + T2T_ENTRY_POINTS, recorder=LT.tracer(impl)) as rec:
         with torch.inference_mode():
             outs.append(model.forward_fused(img))
     return rec.launches, outs[0]
@@ -103,7 +94,7 @@ class Walk:
 
     def same(self, what: str, got, want) -> None:
         if isinstance(want, torch.Tensor):
-            ok = got is not None and got.shape == want.shape and torch.equal(got.double(), want.double())
+            ok = got is not None and got.shape == want.shape and torch.equal(got.double(), want.to(got.device).double())
         else:
             ok = got == want
         assert ok, f"{self.case}: launch {self.i - 1} ({self.launches[self.i - 1].name}): {what} differs"
@@ -120,7 +111,7 @@ class Walk:
         self.same(f"{what} K", c.args["k"], K)
         self.same(f"{what} A", c.pre["a"][:, :K], a[:, :K])
         W = c.pre["w"]
-        want = torch.zeros(W.shape[0], K, dtype=torch.bfloat16)
+        want = torch.zeros(W.shape[0], K, dtype=torch.bfloat16, device=W.device)
         if rows is None:
             want[:lin_w.shape[0]] = lin_w[:, :K].bfloat16()
         else:
