@@ -69,6 +69,10 @@ extern "C" {
 #define B200VIT_ATTN_WIDE_MAX_TOKENS 1024  /* tokens n per image */
 #define B200VIT_ATTN_WIDE_MAX_WIDTH 4096   /* padded head width dp */
 
+/* what b200vit_ats_select (Adaptive Token Sampling's token selection) is built for */
+#define B200VIT_ATS_MAX_TOKENS 4096         /* row slot S_in per image */
+#define B200VIT_ATS_MAX_HEAD_TOKENS 16384   /* H * S_in: the per-head scores and value norms held in shared memory */
+
 const char* b200vit_last_error(void);
 int b200vit_version(void);
 /* number of kernels this library has launched in the calling process (all threads) since load / last reset */
@@ -268,6 +272,18 @@ int b200vit_attention_window(const void* qkv, void* out, int B, int gh, int gw, 
  */
 int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq, int Nk,
                          int H, int dh, float scale, void* stream);
+
+/*
+ * b200vit_attention_kv with a key count per image: image b attends over its first nk[b] keys (clamped to [1, Nk]) of
+ * its Nk-row slot, nk_dev a DEVICE int32 [B] array (Adaptive Token Sampling: the kept queries over the image's valid
+ * keys, ats_vit.py:142-150 and 160, whose padded keys get probability 0).  Rows of the slot past nk[b] inside its last
+ * 64-key block are loaded with probability exactly 0, so only a NaN or Inf there (which can come only from the same
+ * image) reaches the image's output; no row outside the image's slot is read.  out must overlap neither q nor kv.  Everything else (layout, limits,
+ * isolation, dh = 32, 64, 80 or 128) as b200vit_attention_kv, which stays a separate instance and gives the same bits
+ * as before.
+ */
+int b200vit_attention_kv_lens(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B, int Nq,
+                              int Nk, const int32_t* nk_dev, int H, int dh, float scale, void* stream);
 
 /*
  * b200vit_attention_kv with key heads of another width than the value heads (ScalableViT's SSA,
@@ -882,6 +898,44 @@ int b200vit_t2t_unfold_tokens(const void* x, int64_t ldx, int B, int n, int C, v
 int64_t b200vit_attention_wide_workspace(int n, int dp, int images);
 int b200vit_attention_wide(const void* qkv, void* out, float* x, int64_t ldx, int n_resid, int B, int n, int dp,
                            float scale, void* ws, int64_t ws_bytes, void* stream);
+
+/*
+ * Adaptive Token Sampling's token selection (ats_vit.py:48-109, 167-170) over images that each own a slot of S_in rows,
+ * the first len_in[b] of them valid (row 0 the cls token):
+ *   qkv[B*S_in, >= 3*H*dh] bf16 (row stride ld), packed [q | k | v] head-major as for b200vit_attention;
+ *   len_in[B], ids_in[B*S_in]: DEVICE int32 valid lengths and the original token index of every row.
+ * The layer samples iff max_b len_in[b] - 1 > K (the batch's padded length, so one image switches it for all).  Then,
+ * per image, in fp32 over its valid rows only:
+ *   p_h[j] = softmax_j(scale * q_h[0] . k_h[j]),  s_j = sum_h p_h[j] |v_h[j]| (j >= 1),
+ *   l_c = log(s_{c+1} / (sum_j s_j + 1e-6) + 1e-6),  draw k: argmax_c (l_c - log(-log(u[b,k,c] + 1e-6) + 1e-6)), ties
+ *   to the lowest c (torch.argmax), over c < len_in[b] - 1;
+ * and row 0 plus the drawn rows 1 + c, once each in increasing order, are kept: U of them besides the cls row.
+ *   u: [B, K, S_in - 1] uniforms in [0, 1], fp32 (u_bf16 = 0) or bf16 (u_bf16 = 1), contiguous; only c < len_in[b] - 1
+ *   is read.
+ * Outputs, S_out = min(S_in, K + 1) rows per image:
+ *   src[B*S_out]: row r of image b comes from row src[b*S_out + r] = b*S_in + pos_r, pos_0 = 0, pos_1 < .. < pos_U the
+ *     kept rows; rows r > U point at the cls row b*S_in (pad_sequence + F.pad, ats_vit.py:94-103);
+ *   len_out[b] = 1 + U;  ids_out[b*S_out + r] = ids_in[b*S_in + pos_r].
+ * Without sampling the map is the identity on the valid rows (pos_r = r for r < len_in[b], else 0) and
+ * len_out = len_in.  len_out and ids_out must not be len_in and ids_in (every CTA reads all of len_in).
+ * One CTA per image; S_in <= B200VIT_ATS_MAX_TOKENS, H * S_in <= B200VIT_ATS_MAX_HEAD_TOKENS, dh = 32, 64, 80 or 128,
+ * ld a multiple of 8, qkv 16-byte aligned, B <= 65535.
+ * Isolation: an image's selection reads only its own valid qkv rows and uniforms (and every image's len_in), so a NaN
+ * or Inf in one image leaves every other image's outputs bit-identical.
+ */
+int b200vit_ats_select(const void* qkv, int64_t ld, const int32_t* len_in, const int32_t* ids_in, const void* u,
+                       int u_bf16, int32_t* src, int32_t* len_out, int32_t* ids_out, int B, int S_in, int S_out, int K,
+                       int H, int dh, float scale, void* stream);
+
+/*
+ * Row gather as bit copies (the residual stream and the kept queries after b200vit_ats_select, ats_vit.py:161-163):
+ *   x_out[r, :D] = x[src[r], :D] (fp32, row strides ldx / ldx_out) when x is given;
+ *   a_out[r, :ncols] = a[src[r], :ncols] (bf16, row strides lda / lda_out) when a is given; r < rows.
+ * D, ldx, ldx_out multiples of 4; ncols, lda, lda_out multiples of 8; pointers 16-byte aligned; outputs distinct from
+ * their inputs (other rows may still be read).
+ */
+int b200vit_ats_gather(const int32_t* src, int rows, const float* x, int64_t ldx, float* x_out, int64_t ldx_out, int D,
+                       const void* a, int64_t lda, void* a_out, int64_t lda_out, int ncols, void* stream);
 
 /*
  * TEST HOOKS -- process-global switches for A/B tests and bring-up; NOT part of the re-entrant API above (a value set

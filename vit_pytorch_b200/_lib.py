@@ -32,6 +32,8 @@ MBCONV_PART_ROWS = 64           # B200VIT_MBCONV_PART_ROWS
 ATTN_GROUPS_MAX_TOKENS = 4096   # B200VIT_ATTN_GROUPS_MAX_TOKENS
 ATTN_WIDE_MAX_TOKENS = 1024     # B200VIT_ATTN_WIDE_MAX_TOKENS
 ATTN_WIDE_MAX_WIDTH = 4096      # B200VIT_ATTN_WIDE_MAX_WIDTH
+ATS_MAX_TOKENS = 4096           # B200VIT_ATS_MAX_TOKENS
+ATS_MAX_HEAD_TOKENS = 16384     # B200VIT_ATS_MAX_HEAD_TOKENS
 
 # every symbol include/b200vit.h declares (tests check that the library exports each of them)
 SYMBOLS = [
@@ -54,7 +56,7 @@ SYMBOLS = [
     "b200vit_window_mix", "b200vit_head_layernorm_gelu", "b200vit_attention_region_local",
     "b200vit_nest_level_entry", "b200vit_nest_im2col", "b200vit_attention_kv_ex", "b200vit_attention_iwsa",
     "b200vit_t2t_unfold_image", "b200vit_t2t_unfold_tokens", "b200vit_attention_wide",
-    "b200vit_attention_wide_workspace",
+    "b200vit_attention_wide_workspace", "b200vit_ats_select", "b200vit_ats_gather", "b200vit_attention_kv_lens",
 ]
 
 
@@ -241,6 +243,12 @@ def lib() -> C.CDLL:
     L.b200vit_attention_wide_workspace.argtypes = [i32, i32, i32]
     L.b200vit_attention_wide.restype = i32
     L.b200vit_attention_wide.argtypes = [vp, vp, vp, i64, i32, i32, i32, i32, f32, vp, i64, vp]
+    L.b200vit_ats_select.restype = i32
+    L.b200vit_ats_select.argtypes = [vp, i64, vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp]
+    L.b200vit_ats_gather.restype = i32
+    L.b200vit_ats_gather.argtypes = [vp, i32, vp, i64, vp, i64, i32, vp, i64, vp, i64, i32, vp]
+    L.b200vit_attention_kv_lens.restype = i32
+    L.b200vit_attention_kv_lens.argtypes = [vp, i64, vp, i64, vp, i32, i32, i32, vp, i32, i32, f32, vp]
     _lib = L
     return L
 
@@ -1463,3 +1471,96 @@ def attention_wide(qkv: torch.Tensor, B: int, n: int, dp: int, scale: float, ws:
                                           int(n_resid), B, int(n), int(dp), float(scale), _ptr(ws), ws.numel(),
                                           _stream())
     _check(rc, "b200vit_attention_wide")
+
+
+def _need(cond: bool, msg: str) -> None:
+    """An argument check of the Adaptive Token Sampling wrappers: raises B200VitError (not an assert, which -O drops)."""
+    if not cond:
+        raise B200VitError(msg)
+
+
+def _rows2d(t: Optional[torch.Tensor], name: str) -> None:
+    _need(t is None or (t.dim() == 2 and t.stride(1) == 1), f"{name} must be 2-D with unit column stride")
+
+
+def ats_select(qkv: torch.Tensor, lens: torch.Tensor, ids: torch.Tensor, u: torch.Tensor, src: torch.Tensor,
+               lens_out: torch.Tensor, ids_out: torch.Tensor, B: int, S_in: int, K: int, H: int, dh: int,
+               scale: float) -> None:
+    """Adaptive Token Sampling's selection over B images of S_in-row slots (b200vit_ats_select): qkv [B*S_in, >= 3*H*dh]
+    bf16 (any row stride), lens int32 [B] and ids int32 [B*S_in] in; u [B, K, S_in - 1] fp32 or bf16 uniforms; out
+    src int32 [B*S_out], lens_out int32 [B], ids_out int32 [B*S_out], S_out = min(S_in, K + 1)."""
+    S_out = min(S_in, K + 1)
+    _rows2d(qkv, "qkv")
+    _need(qkv.shape[0] == B * S_in and qkv.shape[1] >= 3 * H * dh,
+          f"ats_select: qkv must be [{B * S_in}, >= {3 * H * dh}], got {tuple(qkv.shape)}")
+    _need(u.dtype in (torch.float32, torch.bfloat16), f"ats_select: u must be fp32 or bf16 uniforms, got {u.dtype}")
+    _need(u.is_contiguous() and tuple(u.shape) == (B, K, S_in - 1),
+          f"ats_select: u must be contiguous [{B}, {K}, {S_in - 1}], got {tuple(u.shape)}")
+    for t, name, n in ((lens, "lens", B), (ids, "ids", B * S_in), (src, "src", B * S_out),
+                       (lens_out, "lens_out", B), (ids_out, "ids_out", B * S_out)):
+        _need(t.dtype == torch.int32 and t.is_contiguous() and tuple(t.shape) == (n,),
+              f"ats_select: {name} must be contiguous int32 [{n}], got {t.dtype} {tuple(t.shape)}")
+    _need(lens.data_ptr() != lens_out.data_ptr() and ids.data_ptr() != ids_out.data_ptr(),
+          "ats_select: lengths and ids cannot be updated in place")
+    _chk(qkv, torch.bfloat16, "qkv")
+    _chk(u, u.dtype, "u")
+    for t, name in ((lens, "lens"), (ids, "ids"), (src, "src"), (lens_out, "lens_out"), (ids_out, "ids_out")):
+        _chk(t, torch.int32, name)
+    with _Timed("ats_select", B=B, S=S_in, K=K, H=H, bytes=B * S_in * 3 * H * dh * 2 + u.numel() * u.element_size()):
+        rc = lib().b200vit_ats_select(_ptr(qkv), qkv.stride(0), _ptr(lens), _ptr(ids), _ptr(u),
+                                      1 if u.dtype == torch.bfloat16 else 0, _ptr(src), _ptr(lens_out), _ptr(ids_out),
+                                      B, int(S_in), int(S_out), int(K), H, dh, float(scale), _stream())
+    _check(rc, "b200vit_ats_select")
+
+
+def ats_gather(src: torch.Tensor, *, x: Optional[torch.Tensor] = None, x_out: Optional[torch.Tensor] = None,
+               a: Optional[torch.Tensor] = None, a_out: Optional[torch.Tensor] = None, ncols: int = 0) -> None:
+    """x_out[r] = x[src[r]] (fp32 rows) and / or a_out[r, :ncols] = a[src[r], :ncols] (bf16), r < src.numel(), as bit
+    copies (b200vit_ats_gather); rows of any stride."""
+    rows = src.numel()
+    _need(src.dtype == torch.int32 and src.is_contiguous() and src.dim() == 1,
+          f"ats_gather: src must be a contiguous int32 vector, got {src.dtype} {tuple(src.shape)}")
+    _need((x is None) == (x_out is None) and (a is None) == (a_out is None) and (x is not None or a is not None),
+          "ats_gather: give x with x_out and/or a with a_out")
+    for t, name in ((x, "x"), (x_out, "x_out"), (a, "a"), (a_out, "a_out")):
+        _rows2d(t, f"ats_gather: {name}")
+    if x is not None:
+        _need(x_out.shape == (rows, x.shape[1]), f"ats_gather: x_out must be [{rows}, {x.shape[1]}], "
+              f"got {tuple(x_out.shape)}")
+        _need(x.dtype == x_out.dtype == torch.float32, "ats_gather: x and x_out must be fp32")
+    if a is not None:
+        _need(a_out.shape[0] == rows and 0 < ncols <= min(a.shape[1], a_out.shape[1]),
+              f"ats_gather: a_out must have {rows} rows and a, a_out at least ncols={ncols} columns")
+        _need(a.dtype == a_out.dtype == torch.bfloat16, "ats_gather: a and a_out must be bf16")
+    _chk(src, torch.int32, "src")
+    _chk(x, torch.float32, "x"); _chk(x_out, torch.float32, "x_out")
+    _chk(a, torch.bfloat16, "a"); _chk(a_out, torch.bfloat16, "a_out")
+    D = 0 if x is None else x.shape[1]
+    with _Timed("ats_gather", rows=rows, bytes=rows * (8 * D + 4 * ncols)):
+        rc = lib().b200vit_ats_gather(_ptr(src), rows, _ptr(x), 0 if x is None else x.stride(0), _ptr(x_out),
+                                      0 if x_out is None else x_out.stride(0), D, _ptr(a),
+                                      0 if a is None else a.stride(0), _ptr(a_out),
+                                      0 if a_out is None else a_out.stride(0), int(ncols), _stream())
+    _check(rc, "b200vit_ats_gather")
+
+
+def attention_kv_lens(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, lens: torch.Tensor, B: int, Nq: int,
+                      Nk: int, H: int, dh: int, scale: float) -> None:
+    """attention_kv with image b attending over its first lens[b] keys (int32 [B] on the device, clamped to [1, Nk]):
+    q[B*Nq, H*dh] (any row stride), kv[B*Nk, 2*H*dh] packed k | v (any row stride), out[B*Nq, H*dh]."""
+    _rows2d(q, "attention_kv_lens: q")
+    _rows2d(kv, "attention_kv_lens: kv")
+    _need(tuple(q.shape) == (B * Nq, H * dh), f"attention_kv_lens: q must be [{B * Nq}, {H * dh}], got {tuple(q.shape)}")
+    _need(tuple(kv.shape) == (B * Nk, 2 * H * dh),
+          f"attention_kv_lens: kv must be [{B * Nk}, {2 * H * dh}], got {tuple(kv.shape)}")
+    _need(out.is_contiguous() and tuple(out.shape) == (B * Nq, H * dh),
+          f"attention_kv_lens: out must be contiguous [{B * Nq}, {H * dh}], got {tuple(out.shape)}")
+    _need(lens.dtype == torch.int32 and lens.is_contiguous() and tuple(lens.shape) == (B,),
+          f"attention_kv_lens: lens must be contiguous int32 [{B}], got {lens.dtype} {tuple(lens.shape)}")
+    _chk(q, torch.bfloat16, "q"); _chk(kv, torch.bfloat16, "kv"); _chk(out, torch.bfloat16, "out")
+    _chk(lens, torch.int32, "lens")
+    with _Timed("attention_kv_lens", B=B, Nq=Nq, Nk=Nk, H=H, bytes=(q.numel() + kv.numel() + out.numel()) * 2,
+                flops=4.0 * B * H * Nq * Nk * dh):
+        rc = lib().b200vit_attention_kv_lens(_ptr(q), q.stride(0), _ptr(kv), kv.stride(0), _ptr(out), B, int(Nq),
+                                             int(Nk), _ptr(lens), H, dh, float(scale), _stream())
+    _check(rc, "b200vit_attention_kv_lens")

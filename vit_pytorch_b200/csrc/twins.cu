@@ -4,7 +4,8 @@
 //   b200vit_attention_kv       every query of an image against that image's keys / values, which come from another
 //                              buffer and have another length (twins_svt.py:122-157: the sub-sampled keys);
 //                              b200vit_attention_kv_ex takes key heads of another width than the value heads
-//                              (ScalableViT's SSA, scalable_vit.py:71-124)
+//                              (ScalableViT's SSA, scalable_vit.py:71-124); b200vit_attention_kv_lens takes each
+//                              image's key count from a device array (Adaptive Token Sampling, ats_vit.py)
 //   b200vit_merge_patches_ln   p x p patch merging + LayerNorm over the merged features (twins_svt.py:59-75)
 //   b200vit_peg                depthwise k x k convolution plus identity (twins_svt.py:77-83)
 //
@@ -41,10 +42,11 @@ struct KvParams {
   int Ik, Iv;              // H * dk (q and k columns), H * dv (v and out columns)
   int slots;               // block slots in shared memory; all blocks resident iff ceil(Nk / 64) <= slots
   float scale_log2e;
+  const int* nk;           // LENS: keys of image b = nk[b], clamped to [1, Nk] (b200vit_attention_kv_lens)
 };
 
-// DK: width of the q and k heads, DV: of the v and output heads
-template <int DK, int DV>
+// DK: width of the q and k heads, DV: of the v and output heads; LENS: per-image key counts from p.nk
+template <int DK, int DV, bool LENS = false>
 __global__ void __launch_bounds__(KV_THREADS)
 attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_constant__ CUtensorMap q16,
                     const __grid_constant__ CUtensorMap kv64, const __grid_constant__ CUtensorMap kv16,
@@ -62,7 +64,8 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
 
   const int h = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
-  const int nqt = (p.Nq + 127) / 128, nkb = (p.Nk + 63) / 64;
+  const int Nk = LENS ? min(max(p.nk[b], 1), p.Nk) : p.Nk;
+  const int nqt = (p.Nq + 127) / 128, nkb = (Nk + 63) / 64;
   const bool resident = nkb <= p.slots;
 
   if (tid == 0) {
@@ -158,7 +161,7 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int rh = e >> 1;
-          s[4 * jj + e] = key0 + 8 * jj + (e & 1) < p.Nk ? s[4 * jj + e] * p.scale_log2e : -INFINITY;
+          s[4 * jj + e] = key0 + 8 * jj + (e & 1) < Nk ? s[4 * jj + e] * p.scale_log2e : -INFINITY;
           mn[rh] = fmaxf(mn[rh], s[4 * jj + e]);
         }
       float alpha[2];
@@ -213,7 +216,7 @@ attention_kv_kernel(const __grid_constant__ CUtensorMap q64, const __grid_consta
   }
 }
 
-template <int DK, int DV>
+template <int DK, int DV, bool LENS = false>
 static int launch_kv_t(const void* q, int64_t ldq, const void* kv, int64_t ldkv, KvParams p, int H,
                        cudaStream_t stream) {
   using S = Slabs<DK>;
@@ -244,7 +247,7 @@ static int launch_kv_t(const void* q, int64_t ldq, const void* kv, int64_t ldkv,
   long long per = (2LL * num_sms() + pairs - 1) / pairs;
   if (per > nqt) per = nqt;
   if (per < 1) per = 1;
-  auto kern = attention_kv_kernel<DK, DV>;
+  auto kern = attention_kv_kernel<DK, DV, LENS>;
   B200_ENSURE_SMEM(kern, bytes);
   kern<<<dim3((unsigned)per, H, p.B), KV_THREADS, bytes, stream>>>(tm[0], tm[1], tm[2], tm[3], p);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -384,6 +387,43 @@ extern "C" int b200vit_attention_kv(const void* q, int64_t ldq, const void* kv, 
                                     int Nk, int H, int dh, float scale, void* stream) {
   B200_CHECK_ARG(head_width_ok(dh), "attention_kv: dim_head=%d not supported by this build (32, 64, 80 or 128)", dh);
   return attention_kv_impl("attention_kv", q, ldq, kv, ldkv, out, B, Nq, Nk, H, dh, dh, scale, stream);
+}
+
+extern "C" int b200vit_attention_kv_lens(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B,
+                                         int Nq, int Nk, const int32_t* nk_dev, int H, int dh, float scale,
+                                         void* stream) {
+  B200_CHECK_ARG(nk_dev, "attention_kv_lens: null key counts");
+  B200_CHECK_ARG(head_width_ok(dh), "attention_kv_lens: dim_head=%d not supported by this build (32, 64, 80 or 128)",
+                 dh);
+  B200_CHECK_ARG(q && kv && out, "attention_kv_lens: null pointer");
+  B200_CHECK_ARG(B > 0 && Nq > 0 && Nk > 0 && H > 0, "attention_kv_lens: bad shape B=%d Nq=%d Nk=%d H=%d", B, Nq, Nk,
+                 H);
+  B200_CHECK_ARG(Nk <= B200VIT_ATTN_KV_MAX_KEYS, "attention_kv_lens: Nk=%d > %d", Nk, B200VIT_ATTN_KV_MAX_KEYS);
+  B200_CHECK_ARG(ldq >= (int64_t)H * dh && ldq % 8 == 0, "attention_kv_lens: ldq=%lld must be a multiple of 8 and >= %d",
+                 (long long)ldq, H * dh);
+  B200_CHECK_ARG(ldkv >= (int64_t)H * 2 * dh && ldkv % 8 == 0,
+                 "attention_kv_lens: ldkv=%lld must be a multiple of 8 and >= %d", (long long)ldkv, 2 * H * dh);
+  B200_CHECK_ARG(aligned16(q) && aligned16(kv) && aligned16(out), "attention_kv_lens: pointers must be 16-byte aligned");
+  B200_CHECK_ARG(H <= 65535 && B <= 65535, "attention_kv_lens: B=%d, H=%d exceed the grid", B, H);
+  const long long out_b = (long long)B * Nq * H * dh * 2, q_b = (((long long)B * Nq - 1) * ldq + (long long)H * dh) * 2,
+                  kv_b = (((long long)B * Nk - 1) * ldkv + 2LL * H * dh) * 2;
+  B200_CHECK_ARG(!overlap(out, out_b, q, q_b) && !overlap(out, out_b, kv, kv_b), "attention_kv_lens: out overlaps q or kv");
+  KvParams p{};
+  p.out = reinterpret_cast<__nv_bfloat16*>(out);
+  p.B = B;
+  p.Nq = Nq;
+  p.Nk = Nk;
+  p.Ik = H * dh;
+  p.Iv = H * dh;
+  p.scale_log2e = scale * 1.4426950408889634f;
+  p.nk = nk_dev;
+  const auto st = reinterpret_cast<cudaStream_t>(stream);
+  switch (dh) {
+    case 32: return launch_kv_t<32, 32, true>(q, ldq, kv, ldkv, p, H, st);
+    case 80: return launch_kv_t<80, 80, true>(q, ldq, kv, ldkv, p, H, st);
+    case 128: return launch_kv_t<128, 128, true>(q, ldq, kv, ldkv, p, H, st);
+    default: return launch_kv_t<64, 64, true>(q, ldq, kv, ldkv, p, H, st);
+  }
 }
 
 extern "C" int b200vit_attention_kv_ex(const void* q, int64_t ldq, const void* kv, int64_t ldkv, void* out, int B,
